@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """bench.py -- train-points/sec of the projected-process statistics hot path
-(`getMatrixKmnKnmAndVectorKmny`, PGPH:20-36) on N B200s, next to the reference's CPU path.
+(`getMatrixKmnKnmAndVectorKmny`, PGPH:20-36) on N H100s, next to the reference's CPU path.
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched under torch.distributed.run)
   python bench.py --impl reference --gpus N --steps K --warmup W
+  python bench.py ... --dump-outputs DIR                   (also writes DIR/G.npy, DIR/b.npy: see below)
 
 A "step" = one pass of the hot path over one batch of synthetic input: begin(active set) ->
 accumulate(shard) -> finish (one ncclAllReduce of [G;b;status] across ranks).
@@ -22,11 +23,14 @@ fixed = weak scaling in each series), so the 1 -> 8 efficiency of either series 
           memory, G and b copied back), host<->device copies inside the timed region.
   stats_plus_tail : value with the m x m tail (sgp_magic: K_mm, Cholesky PD check, magicVector, magicMatrix on rank 0's
           GPU) added to every step.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step -- the all-reduced statistics G (m x m)
+and b (m) of the primary workload, float64 -- as DIR/G.npy and DIR/b.npy.  Inputs are seeded, so two builds run with
+the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
 import argparse
-import glob
 import json
 import os
 import subprocess
@@ -44,7 +48,7 @@ UNIT = "points/s"
 N_E = 100
 SIGMA2 = 1e-4
 # the arithmetic the statistics kernel really computes in (the reference is fp64 throughout; north_star tolerance 1e-5)
-DTYPE = "i8x3 digits (23-bit fixed point) -> exact i32 accumulate -> f64 fold; distances f16x2 split -> f32 (TMEM)"
+DTYPE = "i8x3 digits (23-bit fixed point) -> exact i32 accumulate -> f64 fold; distances f16x2 split -> f32 (wgmma)"
 
 WORKLOADS = {
     "configs1": dict(n_per_gpu=1_000_000, d=16, m=1000,
@@ -67,7 +71,7 @@ def workload_config(name: str, n_gpus: int) -> dict:
             "d": w["d"], "m": w["m"], "n_total": w["n_per_gpu"] * n_gpus,
             "parallelism": "points sharded over %d GPU(s), one ncclAllReduce of [G;b]" % n_gpus,
             "l2": "flushed between timed steps (256 MiB memset)",
-            "precision_mode": "SGP_PREC_AUTO -> tcgen05 int8 exact-accumulation kernel"}
+            "precision_mode": "SGP_PREC_AUTO -> wgmma int8 exact-accumulation kernel"}
 
 
 def make_shard(name: str, rank: int):
@@ -98,33 +102,13 @@ def cpu_sample_points(name: str, cores: int) -> int:
     return int(min(w["n_per_gpu"], max(cores * per_worker * N_E, 20_000)))
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        j = json.load(open(p))
-        return float(j.get("bf16_tflops_sustained", j["bf16_tflops"])), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
-    return 1400.0, "fallback (B200_PROFILING.md sustained ~1.4 PFLOP/s)"
-
-
-def ncu_traffic(name: str):
-    """dram__bytes_read.sum + dram__bytes_write.sum of ONE Gram-kernel launch over this workload's per-GPU shard, from the
-    newest committed `ncu --set full` summary (profiles/*_traffic.json written by tools/ncu_summary.py); None if the
-    current kernel has no capture for this workload."""
-    best, src = None, None
-    for p in sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_traffic.json"))):
-        try:
-            j = json.load(open(p))
-        except Exception:
-            continue
-        if j.get("workload") == name:
-            best, src = j, os.path.basename(p)
-    if best is None:
-        return None, None
-    return int(best["dram_bytes_per_launch"]), src
+def tensor_peak():
+    """Dense BF16 tensor rate of the H100 SXM data sheet (at 700 W); the roofline fraction is taken against it."""
+    return 989.0, "H100 SXM data sheet, dense BF16 (700 W)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region, plus the card's name and power limit."""
 
     def __init__(self, gpu_index: int):
         self.rows, self.proc, self.gpu = [], None, gpu_index
@@ -151,6 +135,14 @@ class ClockSampler:
         if self.proc is None:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
+        card = {}
+        try:
+            r = subprocess.run(["nvidia-smi", "-i", str(self.gpu), "--query-gpu=name,power.limit",
+                                "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=10)
+            name, plimit = [c.strip() for c in r.stdout.strip().split(",")[:2]]
+            card = {"gpu": name, "power_limit_w": float(plimit)}
+        except Exception:
+            pass
         try:
             self.proc.wait(timeout=5)
         except Exception:
@@ -170,7 +162,7 @@ class ClockSampler:
                 if v.lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else (float(np.max(all_sm)) if all_sm else None), "sm_max_mhz": mx,
-                "samples": len(sm), "samples_total": len(all_sm), "reasons": sorted(reasons)}
+                "samples": len(sm), "samples_total": len(all_sm), "reasons": sorted(reasons), **card}
 
 
 def oracle_factory(d: int):
@@ -257,7 +249,7 @@ def run_ours(args):
         sampler.start()
     prim = primary_workload(world)
 
-    def measure(name: str, with_e2e: bool, steps: int, warmup: int, precision=None):
+    def measure(name: str, with_e2e: bool, steps: int, warmup: int, precision=None, dump: bool = False):
         eng.set_precision(sg._native.SGP_PREC_AUTO if precision is None else precision)
         w = WORKLOADS[name]
         n, d, m = w["n_per_gpu"], w["d"], w["m"]
@@ -294,8 +286,12 @@ def run_ours(args):
             barrier()
         t_wall1 = time.perf_counter()
         launches = eng.launch_count() - launches0
+        outputs = None
+        if dump:
+            G, b = eng.finish()                         # the last timed step's statistics (already finished: copy only)
+            outputs = {"G": G, "b": b}
         res = {"name": name, "n": n, "d": d, "m": m, "dev_ms": dev_ms, "kern_ms": kern_ms, "kern_n": kern_n,
-               "launches": launches, "t_wall": (t_wall0, t_wall1), "path": path, "e2e_ms": None}
+               "launches": launches, "t_wall": (t_wall0, t_wall1), "path": path, "e2e_ms": None, "outputs": outputs}
 
         # tail (m x m, fp64; rank 0 does it in a fit): statistics of the last step are still on the device
         eng.magic(copy_out=False)                       # first call pays cuSOLVER's lazy initialisation / workspace
@@ -377,7 +373,7 @@ def run_ours(args):
         return e
 
     other = "configs1" if prim == "configs3" else "configs3"
-    rp = measure(prim, True, args.steps, args.warmup)
+    rp = measure(prim, True, args.steps, args.warmup, dump=args.dump_outputs is not None)
     ro = measure(other, False, max(2, min(args.steps, 3)), 3)
     clocks = sampler.stop(*rp["t_wall"]) if rank == 0 else None
     rd = None
@@ -389,14 +385,13 @@ def run_ours(args):
         n_total = rp["n"] * world
         value = n_total * args.steps / (rp["dev_ms"] / 1e3)
         e2e_value = n_total * args.steps / (rp["e2e_ms"] / 1e3)
-        peak_tf, peak_src = measured_peaks()
+        peak_tf, peak_src = tensor_peak()
         launch_ms = rp["kern_ms"] / max(rp["kern_n"], 1)
         flops = algorithmic_flops_per_point(rp["m"], rp["d"]) * rp["n"] * args.steps / max(rp["kern_n"], 1)
         achieved_tf = flops / (launch_ms / 1e3) / 1e12
-        traffic, traffic_src = ncu_traffic(prim)
-        roof = {"bound": "tensor", "kernel": "kmn_gram_i8_ring_kernel", "achieved": achieved_tf, "peak": peak_tf,
+        roof = {"bound": "tensor", "kernel": "kmn_gram_i8_wgmma_kernel", "achieved": achieved_tf, "peak": peak_tf,
                 "unit": "TFLOP/s", "frac": achieved_tf / peak_tf, "peak_source": peak_src,
-                "traffic": traffic, "traffic_source": traffic_src, "launch_ms": launch_ms,
+                "launch_ms": launch_ms,
                 "launches_timed": rp["kern_n"], "algorithmic_flops_per_launch": flops,
                 "note": "algorithmic flops = N*(2md + m(m+1) + 2m); the kernel executes 6 int8 products per Gram "
                         "tile pair (exact 23-bit arithmetic), none of the extra products is credited"}
@@ -426,6 +421,10 @@ def run_ours(args):
             out["fit"] = fit_number(sg, args)
         if world == 1 and args.sweep:
             out["sweep"] = sweep_number(sg, eng, torch, dev)
+        if args.dump_outputs is not None:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for k, v in rp["outputs"].items():
+                np.save(os.path.join(args.dump_outputs, k + ".npy"), np.asarray(v, dtype=np.float64))
         print(json.dumps(out))
     eng.close()
     if world > 1:
@@ -435,7 +434,7 @@ def run_ours(args):
 def sweep_number(sg, eng, torch, dev):
     """BASELINE configs[4] shape per GPU (12.5M x 8, active=4000): the HBM-bound K_nm sweep -- materialise the fp32 cross
     kernel of a 262144-point chunk (the full shard's 200 GB of K_nm does not fit in HBM; the chunk buffer is rewritten),
-    CUDA events on the library's stream, vs the measured HBM copy bandwidth."""
+    CUDA events on the library's stream, vs the data-sheet HBM bandwidth."""
     n, d, m = 262_144, 8, 4000
     rng = np.random.default_rng(5)
     X = rng.random((n, d), dtype=np.float32)
@@ -454,15 +453,12 @@ def sweep_number(sg, eng, torch, dev):
     eng.event_record(3)
     ms = eng.event_elapsed_ms(2, 3) / reps
     bytes_alg = n * m * 4.0 + n * d * 4.0
-    peak = None
-    try:
-        peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
-    except Exception:
-        pass
+    peak = 3350.0                                      # H100 SXM data sheet, HBM3
     gbs = bytes_alg / (ms / 1e3) / 1e9
     return {"workload": "BASELINE configs[4] shard shape: K_nm sweep of %d x %d points against active=%d, fp32 out" % (n, d, m),
             "ms_per_chunk": ms, "points_per_sec": n / (ms / 1e3), "elements_per_sec": n * m / (ms / 1e3),
-            "roofline": {"bound": "hbm", "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": (gbs / peak) if peak else None,
+            "roofline": {"bound": "hbm", "achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak,
+                         "peak_source": "H100 SXM data sheet, HBM3 bandwidth",
                          "algorithmic_bytes": bytes_alg, "note": "bytes = n*m*4 written + n*d*4 read; prep of the fp16 images included"}}
 
 
@@ -505,6 +501,8 @@ def main():
     ap.add_argument("--no-sweep", dest="sweep", action="store_false", help="skip the K_nm sweep number (N=1 only)")
     ap.add_argument("--no-direct", dest="direct", action="store_false",
                     help="skip the direct-distance int8 series entry (N=1 only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's G and b (float64 .npy) into DIR")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

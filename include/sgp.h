@@ -1,4 +1,4 @@
-/* sgp.h -- C-ABI of the B200-native projected-process (sparse GP) hot path.
+/* sgp.h -- C-ABI of the H100-native projected-process (sparse GP) hot path.
  *
  * Drop-in boundary for ONE path of akopich/spark-gp (reference paths relative to
  * /root/reference/src/main/scala/org/apache/spark/ml/):
@@ -71,8 +71,8 @@ enum {
   SGP_PREC_F64 = 0,        /* default: fp32-accurate kernel elements (direct-form distances, full-precision expf),
                               fp64 DMMA Gram.  Parity-grade (<= 1e-6 on mean/variance, see DESIGN.md). */
   SGP_PREC_F64_STRICT = 1, /* elements in fp64 as well (verification mode, ~1e-13 on G,b)               */
-  SGP_PREC_I8 = 2,         /* tcgen05 path: distance contraction on fp16 hi/lo splits (fp32 in TMEM), kernel elements
-                              as 23-bit fixed point in three balanced int8 digits, Gram = six kind::i8 products with
+  SGP_PREC_I8 = 2,         /* wgmma path: distance contraction on fp16 hi/lo splits (fp32 accumulators), kernel elements
+                              as 23-bit fixed point in three balanced int8 digits, Gram = six int8 products with
                               EXACT int32 accumulation, folded into fp64.  Kernels with one non-Eye term, d <= 32; other
                               qualifying shapes are served by SGP_PREC_I8_DIRECT (sgp_last_path tells which ran).       */
   SGP_PREC_AUTO = 3,       /* default.  An accumulate call of >= 32768 points whose scaled squared norms are small (mean over
@@ -208,10 +208,9 @@ int sgp_last_bcm_path(const sgp_ctx* ctx);
  * the first CTA of the last launch, T = -q*log2(e) (128 active rows x 64 points, fp32) and the fixed-point words
  * (0x4B000000 | (u + 0x4040)), u = s2*2^15 + s1*2^7 + s0 in balanced digits. */
 int sgp_debug_i8_tile(sgp_ctx* ctx, float* T_out /* 128*64 */, uint32_t* w_out /* 128*64 */);
-/* Debug aid: clock64 timeline [2 CTAs: tile (0,0) = publisher, tile (1,0) = consumer][5 roles: distance issuer, Gram
- * issuer, epilogue group 0, group 1, sharing warp][32 units: 64..95][8 events] of the last SGP_PREC_I8 launch made while
- * armed (see sgp_debug_i8_tile). */
-int sgp_debug_i8_timeline(sgp_ctx* ctx, long long* out /* 2560 + 148*32: timeline, then per-CTA progress marks */);
+/* Debug aid kept for ABI compatibility: the int8 Gram kernel of this build records no timeline, so this returns
+ * SGP_E_STATE. */
+int sgp_debug_i8_timeline(sgp_ctx* ctx, long long* out);
 /* GreedilyOptimizingActiveSetProvider (commons/ActiveSetProvider.scala:58-139) with rank-1 updates: selects m_target points
  * of the shard X (n x d fp64, host) by the reference's forward selection and returns their row indices.  The reference
  * recomputes the statistics, two m x m inverses and three quadratic forms per candidate in every round (ASP:83-137); here

@@ -1,4 +1,4 @@
-"""spark_gp_b200 -- B200-native projected-process (sparse GP) hot path behind the reference's API.
+"""spark_gp_b200 -- H100-native projected-process (sparse GP) hot path behind the reference's API.
 
 Only what the path needs: `csrc/` (CUDA kernels + the C-ABI of include/sgp.h), the ctypes binding, and a
 host-side mirror of the reference's kernel DSL / Estimator surface.  No CPU fallback."""

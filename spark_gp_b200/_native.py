@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI in include/sgp.h (the same .so a JNI shim would load).
 
-There is NO CPU fallback: if libsgp.so is missing or no B200 is visible, calls raise."""
+There is NO CPU fallback: if libsgp.so is missing or no H100 is visible, calls raise."""
 from __future__ import annotations
 
 import ctypes as C

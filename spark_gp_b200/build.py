@@ -1,5 +1,5 @@
-"""Builds libsgp.so (CUDA kernels + C-ABI) in-tree for sm_100a with nvcc.  No JIT cache: the built .so
-travels to the GPU box with the snapshot."""
+"""Builds libsgp.so (CUDA kernels + C-ABI) in-tree for sm_90a (H100) with nvcc.  No JIT cache: the package loads the
+.so from its own directory."""
 from __future__ import annotations
 
 import os
@@ -9,8 +9,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsgp.so")
-SOURCES = ["api.cu", "bcm_nll.cu", "gram_f64.cu", "gram_i8.cu", "gram_i8_ring.cu", "greedy.cu", "kmn_sweep.cu", "laplace.cu", "misc_kernels.cu", "tail.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+SOURCES = ["api.cu", "bcm_nll.cu", "gram_f64.cu", "gram_i8.cu", "gram_i8_wgmma.cu", "greedy.cu", "kmn_sweep.cu", "laplace.cu", "misc_kernels.cu", "tail.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-Xptxas", "-v"]
 LINK = ["-lcusolver", "-lcublas", "-ldl", "-Xlinker", "-rpath=/usr/local/cuda/lib64"]
 

@@ -43,14 +43,6 @@ static NcclApi& nccl() {
 int fail(Ctx* c, int code, const std::string& msg) {
   if (c) {
     c->err = msg;
-    if (code == SGP_E_CUDA && c->i8_pm_host && c->i8_pm_host[0] != 0) {
-      const int* pm = c->i8_pm_host;            // int8 kernel post-mortem: first wait that made no progress for ~1 s
-      long long unit;
-      std::memcpy(&unit, pm + 4, sizeof(unit));
-      c->err += " [kmn_gram_i8 post-mortem: wait site " + std::to_string(pm[0]) + " block (" + std::to_string(pm[1]) + "," +
-                std::to_string(pm[2]) + ") warp " + std::to_string(pm[3]) + " unit " + std::to_string(unit) + " a=" +
-                std::to_string(static_cast<unsigned>(pm[6])) + " b=" + std::to_string(static_cast<unsigned>(pm[7])) + "]";
-    }
   } else {
     g_create_err = msg;
   }
@@ -119,14 +111,9 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   if (n_slices < 1) n_slices = 1;
   const long long blocks = (n + 15) / 16;
   if (n_slices > blocks) n_slices = static_cast<int>(blocks);
-  // int8 kernel: cooperative launches of whole tile columns (all CTAs of a launch are co-resident)
-  I8Launch plan[64];
-  int n_plan = 0, plan_slices = 1;
-  if ((c->i8_ok || c->i8_direct_ok) && c->i8_impl == 1) {
-    n_plan = i8_plan(c->m_pad, c->num_sms, (n + 63) / 64, plan, 64);
-    for (int i = 0; i < n_plan; ++i) plan_slices = plan[i].n_slices > plan_slices ? plan[i].n_slices : plan_slices;
-  }
-  int rc = ensure_partials(c, n_slices > plan_slices ? n_slices : plan_slices);
+  // int8 kernel: one launch over the upper block triangle x point slices
+  const int i8_n_slices = (c->i8_ok || c->i8_direct_ok) ? i8_slices(c->m_pad, c->num_sms, (n + 63) / 64) : 1;
+  int rc = ensure_partials(c, n_slices > i8_n_slices ? n_slices : i8_n_slices);
   if (rc != SGP_OK) return rc;
 
   GramParams p{};
@@ -138,14 +125,14 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   p.Gpart = c->dGpart; p.bpart = c->dBpart;
   p.n_slices = n_slices; p.n_tiles_1d = nt1;
 
-  // AUTO: the tcgen05 int8 kernel inside its measured parity envelope -- accumulate calls of >= 32768 points (posterior
-  // mean within 1.1e-6 .. 2.4e-6 of the all-fp64 kernel for N = 16k .. 4M: profiles/r01_i8_scaling.txt,
-  // profiles/r02n_i8_small_shards.txt; the limit is the two dropped low-order digit products, tools/i8_error_model.py,
+  // AUTO: the int8 kernel inside its measured parity envelope -- accumulate calls of >= 32768 points (posterior
+  // mean within a few 1e-6 of the all-fp64 kernel from N = 16k up; the limit is the two dropped low-order digit
+  // products, tools/i8_error_model.py,
   // and does not grow towards small N) and small scaled norms (gate below).  Smaller calls stay on the fp64 DMMA kernel
   // (2e-7), which needs < 2 ms at that size.
   // Path of this launch: 0 = fp64 DMMA kernel, 1 = int8 Gram with tensor-core distances (one term, d <= 32, benign norms),
   // 2 = int8 Gram with direct fp32 distances (up to 4 terms, d <= 72; AUTO: same magnitude budget as path 1).
-  const bool tensor_ok = c->i8_ok, direct_ok = c->i8_direct_ok && c->i8_impl == 1 && n_plan > 0;
+  const bool tensor_ok = c->i8_ok, direct_ok = c->i8_direct_ok;
   int path = 0;
   if (c->precision == SGP_PREC_I8) {
     if (tensor_ok) path = 1;
@@ -160,20 +147,12 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
     if (!first_of_call) path = c->call_path;
   }
   bool use_i8 = (path == 1);
-  if (use_i8 && c->i8_impl == 1 && n_plan <= 0) {
-    if (c->precision == SGP_PREC_I8) return fail(c, SGP_E_BADARG, "active set too large for the int8 kernel's launch plan");
-    use_i8 = false; path = 0;
-  }
   if (path != 0) {
     const size_t yb = static_cast<size_t>((n + 63) / 64) * 64 * sizeof(float);
     if (yb > c->i8_ys_bytes) {
       cudaFree(c->dI8Ys); c->dI8Ys = nullptr; c->i8_ys_bytes = 0;
       SGP_CUDA(c, cudaMalloc(&c->dI8Ys, yb));
       c->i8_ys_bytes = yb;
-    }
-    if (c->i8_impl == 1) {
-      rc = ctx_scratch(c, c->i8_share, i8_share_bytes(c->m_pad, plan_slices));
-      if (rc != SGP_OK) return rc;
     }
   }
   if (use_i8) {
@@ -203,7 +182,7 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
       if (xsum / static_cast<double>(n) + c->i8_z_norm_mean > c->i8_norm_budget) {
         // Large scaled norms mean tiny kernel values, and the fixed-point digits carry an ABSOLUTE error of 2^-24: on
         // such shards the int8 Gram -- with either distance form -- loses the posterior mean (airfoil-like data: 1.5e-4
-        // to 1.5e-2 against 7e-7 .. 7e-6 of the fp64 kernel, profiles/r02o_i8_conditioning.txt).  fp64 DMMA kernel.
+        // to 1.5e-2 against 7e-7 .. 7e-6 of the fp64 kernel).  fp64 DMMA kernel.
         use_i8 = false;
         path = 0;
       }
@@ -260,28 +239,15 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   c->gram_events_used += 1;
   SGP_CUDA(c, cudaEventRecord(e0, c->stream));
   const size_t mm = static_cast<size_t>(c->m) * c->m;
-  if (use_i8 && c->i8_impl == 0) {
-    SGP_CUDA(c, launch_gram_i8(c->dI8Xt, c->dI8Ys, c->dI8Zt, n, c->d, c->m_pad, n_slices, c->dGpart, c->dBpart,
-                               c->kf.scale[0], c->dbgT, c->dbgW, nullptr, c->stream));
-    SGP_CUDA(c, cudaEventRecord(e1, c->stream));
-    SGP_CUDA(c, launch_gram_reduce(c->dGb, c->dGb + mm, c->dGpart, c->dBpart, n_slices, c->m, c->m_pad, c->stream));
-    c->launches += 2;
-    return SGP_OK;
-  }
   if (use_i8 || path == 2) {
     const uint8_t* zop = (path == 2) ? reinterpret_cast<const uint8_t*>(c->dI8Zd) : c->dI8Zt;
-    for (int i = 0; i < n_plan; ++i) {
-      SGP_CUDA(c, launch_gram_i8_ring(c->dI8Xt, c->dI8Ys, zop, n, c->d, c->m_pad, plan[i], direct, c->dGpart, c->dBpart,
-                                 c->kf.scale[0], static_cast<uint8_t*>(c->i8_share.p), c->dbgT, c->dbgW, c->dbgClk,
-                                 c->i8_pm_dev, c->stream));
-      c->launches += 1;
-    }
+    SGP_CUDA(c, launch_gram_i8(c->dI8Xt, c->dI8Ys, zop, n, c->d, c->m_pad, i8_n_slices, direct, c->dGpart, c->dBpart,
+                               c->kf.scale[0], c->dbgT, c->dbgW, c->stream));
     SGP_CUDA(c, cudaEventRecord(e1, c->stream));
-    for (int i = 0; i < n_plan; ++i) {          // deterministic slice reduction, per launch (its columns, its slices)
-      SGP_CUDA(c, launch_gram_reduce_upper(c->dGb, c->dGb + mm, c->dGpart, c->dBpart, plan[i].n_slices, c->m, c->m_pad,
-                                           plan[i].col_lo * kTile, plan[i].col_hi * kTile, c->stream));
-      c->launches += 1;
-    }
+    // deterministic slice reduction (partial tiles at the mirror position: upper block triangle)
+    SGP_CUDA(c, launch_gram_reduce_upper(c->dGb, c->dGb + mm, c->dGpart, c->dBpart, i8_n_slices, c->m, c->m_pad, 0, c->m,
+                                         c->stream));
+    c->launches += 2;
     return SGP_OK;
   }
   SGP_CUDA(c, launch_gram_f64(p, c->precision == SGP_PREC_F64_STRICT, c->stream));
@@ -321,8 +287,8 @@ int sgp_ctx_create(sgp_ctx** out, int device) {
   if ((e = cudaSetDevice(device)) != cudaSuccess) return bail(SGP_E_CUDA, cudaGetErrorString(e));
   cudaDeviceProp prop;
   if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return bail(SGP_E_CUDA, cudaGetErrorString(e));
-  if (prop.major != 10)
-    return bail(SGP_E_CUDA, "this library is built for sm_100a (B200) only; device is sm_" +
+  if (prop.major != 9 || prop.minor != 0)
+    return bail(SGP_E_CUDA, "this library is built for sm_90a (H100) only; device is sm_" +
                                 std::to_string(prop.major) + std::to_string(prop.minor));
   c->num_sms = prop.multiProcessorCount;
   if ((e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking)) != cudaSuccess ||
@@ -336,12 +302,6 @@ int sgp_ctx_create(sgp_ctx** out, int device) {
       (e = cudaEventCreateWithFlags(&c->tail_fork, cudaEventDisableTiming)) != cudaSuccess ||
       (e = cudaEventCreateWithFlags(&c->tail_join, cudaEventDisableTiming)) != cudaSuccess)
     return bail(SGP_E_CUDA, cudaGetErrorString(e));
-  if (cudaHostAlloc(reinterpret_cast<void**>(&c->i8_pm_host), 64, cudaHostAllocMapped) == cudaSuccess) {
-    std::memset(c->i8_pm_host, 0, 64);
-    if (cudaHostGetDevicePointer(&c->i8_pm_dev, c->i8_pm_host, 0) != cudaSuccess) c->i8_pm_dev = nullptr;
-  }
-  c->i8_impl = 1;                 // shared-panel ring kernel; SGP_I8_IMPL=v1 selects round 1's self-contained kernel
-  if (const char* ev = getenv("SGP_I8_IMPL")) c->i8_impl = (std::string(ev) == "v1") ? 0 : 1;
   if (cusolverDnCreate(&c->solver) != CUSOLVER_STATUS_SUCCESS) return bail(SGP_E_CUDA, "cusolverDnCreate failed");
   if (cusolverDnCreate(&c->solver2) != CUSOLVER_STATUS_SUCCESS) return bail(SGP_E_CUDA, "cusolverDnCreate failed");
   if (cublasCreate(&c->blas) != CUBLAS_STATUS_SUCCESS) return bail(SGP_E_CUDA, "cublasCreate failed");
@@ -359,14 +319,13 @@ int sgp_ctx_destroy(sgp_ctx* h) {
   free_active_set(c);
   cudaFree(c->dGpart); cudaFree(c->dBpart);
   cudaFree(c->dEx); cudaFree(c->dEy); cudaFree(c->dEoff); cudaFree(c->dEf); cudaFree(c->dNllPer); cudaFree(c->dNllScratch);
-  cudaFree(c->dI8Xt); cudaFree(c->dI8Ys); cudaFree(c->dbgT); cudaFree(c->dbgW); cudaFree(c->dbgClk); cudaFree(c->i8_share.p);
+  cudaFree(c->dI8Xt); cudaFree(c->dI8Ys); cudaFree(c->dbgT); cudaFree(c->dbgW);
   for (int i = 0; i < 2; ++i) {
     cudaFree(c->stageX[i]); cudaFree(c->stageY[i]);
     if (c->stage_free[i]) cudaEventDestroy(c->stage_free[i]);
     if (c->stage_ready[i]) cudaEventDestroy(c->stage_ready[i]);
   }
   if (c->comm && nccl().ok) nccl().CommDestroy(c->comm);
-  if (c->i8_pm_host) cudaFreeHost(c->i8_pm_host);
   cudaFree(c->greedy_ws.p); cudaFree(c->sweep_ws.p); cudaFree(c->bcm_ws.p); cudaFree(c->tail_ws.p); cudaFree(c->tail_ws2.p); cudaFree(c->predict_ws.p); cudaFree(c->cross_ws.p);
   if (c->tail_fork) cudaEventDestroy(c->tail_fork);
   if (c->tail_join) cudaEventDestroy(c->tail_join);
@@ -447,7 +406,7 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
     kf.scale[kf.n_terms++] = term.scale;
   }
   // device buffers are kept across begin() calls with the same (m, d, term count): cudaMalloc/cudaFree are
-  // synchronising and cost milliseconds -- more than the whole statistics pass on a B200
+  // synchronising and cost milliseconds -- more than the whole statistics pass on the GPU
   const int nt = kf.n_terms > 0 ? kf.n_terms : 1;
   const bool same_shape = c->dZ && c->m == m && c->d == d && c->alloc_terms == nt;
   if (!same_shape) {
@@ -473,7 +432,7 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
                                   c->dBeta + static_cast<size_t>(t) * dpad, m, c->m_pad, d, dpad, c->stream));
     c->launches += 1;
   }
-  // ---- tcgen05 int8 path: qualifies for one non-Eye term and d <= 32 (two 64-column K chunks) -------------
+  // ---- int8 path with tensor-core distances: qualifies for one non-Eye term and d <= 32 (two 64-column K chunks) -------------
   c->i8_ok = (kf.n_terms == 1 && d <= 32);
   std::vector<double> sc16, ctr16;               // live until the synchronisation at the end of this function
   if (!c->dI8Flags) {
@@ -1032,8 +991,6 @@ int sgp_debug_i8_tile(sgp_ctx* h, float* T_out, uint32_t* w_out) {
     SGP_CUDA(c, cudaMalloc(&c->dbgW, 128 * 64 * 4));
     SGP_CUDA(c, cudaMemset(c->dbgT, 0, 128 * 64 * 4));
     SGP_CUDA(c, cudaMemset(c->dbgW, 0, 128 * 64 * 4));
-    SGP_CUDA(c, cudaMalloc(&c->dbgClk, (2560 + 148 * 32) * 8));
-    SGP_CUDA(c, cudaMemset(c->dbgClk, 0, (2560 + 148 * 32) * 8));
   }
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   if (T_out) SGP_CUDA(c, cudaMemcpy(T_out, c->dbgT, 128 * 64 * 4, cudaMemcpyDeviceToHost));
@@ -1044,11 +1001,7 @@ int sgp_debug_i8_tile(sgp_ctx* h, float* T_out, uint32_t* w_out) {
 int sgp_debug_i8_timeline(sgp_ctx* h, long long* out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c || !out) return SGP_E_BADARG;
-  if (!c->dbgClk) return fail(c, SGP_E_STATE, "arm with sgp_debug_i8_tile first");
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  SGP_CUDA(c, cudaMemcpy(out, c->dbgClk, (2560 + 148 * 32) * 8, cudaMemcpyDeviceToHost));
-  return SGP_OK;
+  return fail(c, SGP_E_STATE, "the int8 Gram kernel of this build records no timeline");
 }
 
 int sgp_event_record(sgp_ctx* h, int slot) {

@@ -20,8 +20,7 @@
 //
 // Tile shapes.  Strict mode keeps the 128x128 tile (128 accumulator registers per thread, one CTA per SM).  The default
 // mode uses 128x64 tiles (TN = 64): 64 accumulator registers per thread, so TWO CTAs fit on an SM and the panel phase
-// (FMA / XU pipes) of one overlaps the DMMA phase of the other -- with one CTA per SM the two phases alternate and
-// the DMMA pipe sat at 43.5 % (profiles/r01_t1_gram_f64_ncu_summary.txt).  Column tiles of 64 inside the 128-row
+// (FMA / XU pipes) of one overlaps the DMMA phase of the other -- with one CTA per SM the two phases alternate.  Column tiles of 64 inside the 128-row
 // diagonal block reuse the I panel (no second panel); the tile map is the staircase tj <= 2 ti + 1.
 //
 // Why fp64 accumulation: tools/precision_study.py -- the posterior mean needs the Gram accumulated to
@@ -33,6 +32,12 @@
 
 namespace sgp {
 namespace {
+
+// f32x2 helpers on two scalar lanes (Hopper has no packed fp32 FADD/FFMA); round-to-nearest like the scalar ops
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 
 constexpr int PB = 16;            // points per block (DMMA k extent per block = 4 steps of k=4)
 constexpr int PS = kTile + 4;     // panel row stride (doubles): 132 -> conflict-free 8-byte fragment loads
@@ -122,7 +127,7 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
   long long blk_hi = blk_lo + bps;
   if (blk_hi > total_blocks) blk_hi = total_blocks;
 
-  constexpr bool kPacked = sizeof(ET) == 4;                  // fp32 elements: packed f32x2 arithmetic, z staged negated
+  constexpr bool kPacked = sizeof(ET) == 4;                  // fp32 elements: f32x2 arithmetic, z staged negated
   constexpr double kZSign = kPacked ? -1.0 : 1.0;
   const bool z_resident = (p.n_terms == 1 && p.dpad <= DC);
 
@@ -163,7 +168,7 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
   // two co-resident CTAs do not fix that: they phase-lock (both share the pipe in the DMMA phase, finish together, then
   // both build panels): measured 45 % DMMA utilisation either way.  Here the DMMAs of block i and the panel build of
   // block i+1 sit in the same barrier-free region (double-buffered panels / x staging, ONE __syncthreads per block),
-  // so warps drift apart and FFMA2 / MUFU work of some warps fills the issue slots of warps blocked on the tensor pipe.
+  // so warps drift apart and FFMA / MUFU work of some warps fills the issue slots of warps blocked on the tensor pipe.
   if constexpr (kPacked) {
     if (z_resident) {
       const int nk4 = p.dpad >> 2;                               // <= 8
@@ -188,9 +193,9 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
 #pragma unroll
           for (int pp = 0; pp < PB; ++pp) {
             const float4 x = *reinterpret_cast<const float4*>(xb + pp * DC + k4 * 4);         // warp-wide broadcast
-            const float2 d01 = __fadd2_rn(make_float2(x.x, x.y), z01), d23 = __fadd2_rn(make_float2(x.z, x.w), z23);
-            q[pp] = __ffma2_rn(d01, d01, q[pp]);
-            q[pp] = __ffma2_rn(d23, d23, q[pp]);
+            const float2 d01 = fadd2(make_float2(x.x, x.y), z01), d23 = fadd2(make_float2(x.z, x.w), z23);
+            q[pp] = ffma2(d01, d01, q[pp]);
+            q[pp] = ffma2(d23, d23, q[pp]);
           }
         }
         (void)blk; (void)pbuf;
@@ -267,8 +272,8 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
   for (long long blk = blk_lo; blk < blk_hi; ++blk) {
     const long long pt0 = blk * PB;
     // ---------------- phase 1: panels -----------------------------------------------------------
-    // fp32 elements: q is accumulated as float2 (even / odd feature dims) with packed f32x2 FADD/FFMA -- half the
-    // instructions of the scalar form; per-term results go straight into the panel (the thread owns its column).
+    // fp32 elements: q is accumulated as float2 (even / odd feature dims, two independent chains); per-term results go
+    // straight into the panel (the thread owns its column).
     double* ys = ys2 + ((blk - blk_lo) & 1) * PB;   // stragglers of block k-1 may still read the other half
     if (tid < PB) ys[tid] = (pt0 + tid < p.n) ? p.y[pt0 + tid] : 0.0;
     double* dst = panel + pan * PB * PS + col;
@@ -292,9 +297,9 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
 #pragma unroll
               for (int pp = 0; pp < PB; ++pp) {
                 const float4 x = *reinterpret_cast<const float4*>(xs + pp * DC + k4 * 4);          // warp-wide broadcast
-                const float2 d01 = __fadd2_rn(make_float2(x.x, x.y), z01), d23 = __fadd2_rn(make_float2(x.z, x.w), z23);
-                q[pp] = __ffma2_rn(d01, d01, q[pp]);
-                q[pp] = __ffma2_rn(d23, d23, q[pp]);
+                const float2 d01 = fadd2(make_float2(x.x, x.y), z01), d23 = fadd2(make_float2(x.z, x.w), z23);
+                q[pp] = ffma2(d01, d01, q[pp]);
+                q[pp] = ffma2(d23, d23, q[pp]);
               }
             } else {
               ET z4[4];
@@ -385,7 +390,7 @@ __global__ void gram_reduce_kernel(double* __restrict__ G, double* __restrict__ 
   }
 }
 
-// Same for partial tiles stored at the MIRROR position (upper block triangle; the int8 ring kernel folds its TMEM tiles
+// Same for partial tiles stored at the MIRROR position (upper block triangle; the int8 kernel folds its accumulators
 // transposed so that its global writes coalesce): G[i][j] (+ mirror) += sum_s Gpart[s][i][j] for rows i in [row_lo, row_hi),
 // j >= i.
 __global__ void gram_reduce_upper_kernel(double* __restrict__ G, double* __restrict__ b,

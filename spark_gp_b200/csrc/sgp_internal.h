@@ -18,7 +18,7 @@ namespace sgp {
 constexpr long long kAutoI8MinPoints = 32768;
 constexpr int kMaxTerms = 4;      // non-Eye terms of a flattened kernel
 constexpr int kTile = 128;        // edge of one G tile (active-set indices per CTA tile)
-constexpr int kSMsB200 = 148;
+constexpr int kSMsH100 = 132;      // H100 SXM; the context reads the real count from the device
 
 // Flattened, device-ready kernel description (built by sgp_stats_begin).
 struct KernelFlat {
@@ -69,7 +69,7 @@ struct Ctx {
   bool tail_fast = false;              // last sgp_magic took the Cholesky path for both matrices
   ncclComm_t comm = nullptr;
   int rank = 0, nranks = 1;
-  int num_sms = kSMsB200;
+  int num_sms = kSMsH100;
 
   // active set / kernel (valid after begin)
   bool begun = false, finished = false, has_magic = false;
@@ -83,7 +83,7 @@ struct Ctx {
   double* dGpart = nullptr;  size_t gpart_bytes = 0;
   double* dBpart = nullptr;  size_t bpart_bytes = 0;
   int n_slices = 1;
-  // tcgen05 int8 path (gram_i8.cu)
+  // int8 exact-accumulation path (gram_i8.cu operand preparation, gram_i8_wgmma.cu Gram kernel)
   bool i8_ok = false;            // kernel/shape qualifies for tensor-core distances (one non-Eye term, d <= 32)
   bool i8_direct_ok = false;     // ... for the direct-distance mode (<= 4 non-Eye terms, n_terms * (dpad4 + 4) <= 72)
   int i8_dpad4 = 0;
@@ -106,7 +106,7 @@ struct Ctx {
   long long i8_points = 0;       // points that went through the int8 kernel since begin
   double i8_z_norm_mean = 0.0;   // mean over the active set of |z^|^2
   double i8_norm_budget = 6.0;   // AUTO: int8 path only if mean|x^|^2 + mean|z^|^2 <= budget (posterior mean vs the all-fp64
-                                 // mode at 4.3 / 5.8 / 7.2 / 7.9: 1.8e-6 / 2.4e-6 / 5.7e-6 / 1.0e-5, profiles/r02p_i8_budget_edge.txt)
+                                 // mode at 4.3 / 5.8 / 7.2 / 7.9: 1.8e-6 / 2.4e-6 / 5.7e-6 / 1.0e-5, tools/i8_budget_edge.py)
   uint8_t* dI8Zt = nullptr;      // active-set operand images
   uint8_t* dI8Xt = nullptr;  size_t i8_xt_bytes = 0;   // point operand images (scratch)
   float* dI8Ys = nullptr;    size_t i8_ys_bytes = 0;
@@ -135,11 +135,6 @@ struct Ctx {
   cudaEvent_t user_events[8] = {nullptr};
   float* dbgT = nullptr;       // sgp_debug_i8_tile
   uint32_t* dbgW = nullptr;
-  long long* dbgClk = nullptr; // [2 CTAs][5 roles][32 units][8 events] clock64 timeline
-  int* i8_pm_host = nullptr;   // host-mapped post-mortem record of the int8 kernel (8 ints), and its device alias
-  void* i8_pm_dev = nullptr;
-  int i8_impl = 0;             // 0: self-contained kernel (gram_i8.cu), 1: shared-panel ring kernel (gram_i8_ring.cu)
-  DevScratch i8_share;         // L2 ring + flags through which diagonal CTAs publish their digit planes
 };
 
 // error helpers ---------------------------------------------------------------------------------
@@ -180,7 +175,7 @@ cudaError_t launch_predict_finish(double* mean, double* var, const double* K /*n
                                   const double* W /*n x m = K*M*/, const double* mv, double self_k,
                                   long long n, int m, cudaStream_t s);
 
-// tcgen05 path
+// int8 exact-accumulation path
 size_t i8_points_scratch_bytes(long long n, int nchunks);
 size_t i8_active_scratch_bytes(int m_pad, int nchunks);
 int i8_nchunks(int d);
@@ -189,7 +184,7 @@ cudaError_t launch_i8_prep_active(uint8_t* Zt, const double* dZ, int m, int m_pa
 cudaError_t launch_i8_prep_points(uint8_t* Xt, float* ys, const void* dX, int x_is_f32, const double* dy, long long n,
                                   int d, const double* dScale, const double* dCentre, int* dFlags, double* dNormSum,
                                   double* dNormSumCall, cudaStream_t s);
-// direct-distance mode of the ring kernel: fp32 coordinate tiles instead of fp16 operand images
+// direct-distance mode of the int8 Gram: fp32 coordinate tiles instead of fp16 operand images
 cudaError_t launch_i8_prep_active_direct(float* Zd, const double* dZ, int m, int m_pad, int d, int dpad4, int n_terms,
                                          const double* dScale, const double* dCentre, int* flags, float r2max,
                                          cudaStream_t s);
@@ -203,21 +198,11 @@ struct I8Direct {
   double csum = 0.0;     // sum of the term scales = the fixed-point scale
 };
 
-// One cooperative launch of the int8 Gram kernel: whole tile columns [col_lo, col_hi) x n_slices point slices.
-struct I8Launch {
-  int col_lo, col_hi, tiles, n_slices;
-};
-int i8_plan(int m_pad, int num_sms, long long n_units, I8Launch* out, int max_out);
-size_t i8_share_bytes(int m_pad, int n_slices);
-size_t i8_share_flag_bytes(int m_pad, int n_slices);
-cudaError_t launch_gram_i8_ring(const uint8_t* Xt, const float* ys, const uint8_t* Zt, long long n, int d, int m_pad,
-                                const I8Launch& plan, const I8Direct& direct, double* Gpart, double* bpart, double C,
-                                uint8_t* share, float* dbg_T, uint32_t* dbg_w, long long* dbg_clk, void* post_mortem,
-                                cudaStream_t s);
-// round-1 kernel (every CTA builds both panels of its tile; SGP_I8_IMPL=v1): kept as the A/B reference of the ring kernel
+// int8 Gram kernel (gram_i8_wgmma.cu): point slices per launch, and one launch over every tile of the upper block triangle
+int i8_slices(int m_pad, int num_sms, long long n_units);
 cudaError_t launch_gram_i8(const uint8_t* Xt, const float* ys, const uint8_t* Zt, long long n, int d, int m_pad,
-                           int n_slices, double* Gpart, double* bpart, double C, float* dbg_T, uint32_t* dbg_w,
-                           long long* dbg_clk, cudaStream_t s);
+                           int n_slices, const I8Direct& direct, double* Gpart, double* bpart, double C, float* dbg_T,
+                           uint32_t* dbg_w, cudaStream_t s);
 
 // K_nm sweep (kmn_sweep.cu): fp32 cross kernel of a block of points, row-major n x m
 cudaError_t launch_kmn_sweep(const uint8_t* Xt, const uint8_t* Zt, long long n, int d, int m, int m_pad, int num_sms, double C,

@@ -32,7 +32,7 @@ class SgpError(RuntimeError):
 
 
 class OperandRangeError(SgpError):
-    """SGP_E_RANGE: the tcgen05 int8 path cannot represent these coordinates; rerun in SGP_PREC_F64."""
+    """SGP_E_RANGE: the int8 path cannot represent these coordinates; rerun in SGP_PREC_F64."""
 
 
 def _make_desc(kernel: Kernel, d: int):
@@ -171,7 +171,7 @@ class ProjectedProcessEngine:
 
     def statistics(self, kernel: Kernel, active_set, X, y, shard_points: int = 1 << 22):
         """`getMatrixKmnKnmAndVectorKmny` over host data in shards (PGPH:23 broadcast, PGPH:25-35 seqOp over shards).
-        When the tcgen05 int8 path reports SGP_E_RANGE (coordinates outside its operand range, or AUTO's magnitude
+        When the int8 path reports SGP_E_RANGE (coordinates outside its operand range, or AUTO's magnitude
         budget exceeded over the whole window) the pass is repeated on the fp64 DMMA kernel -- still on the GPU."""
         def run():
             self.begin(kernel, active_set)

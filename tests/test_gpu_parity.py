@@ -1,7 +1,7 @@
-"""GPU parity tests (run on a B200: `pytest -m gpu`).  Everything goes through the C-ABI (ctypes) and is
+"""GPU parity tests (run on an H100: `pytest -m gpu`).  Everything goes through the C-ABI (ctypes) and is
 compared with the fp64 oracle on identical seeded inputs, or with the committed golden fixtures.
 
-Arithmetic modes (include/sgp.h): AUTO (default) = the tcgen05 int8 exact-accumulation Gram on accumulate calls of
+Arithmetic modes (include/sgp.h): AUTO (default) = the wgmma int8 exact-accumulation Gram on accumulate calls of
 >= 32768 points whose scaled squared norms are inside the magnitude budget (tensor-core distances for one non-Eye term and
 d <= 32, direct fp32 distances for sums of up to 4 terms / d <= 72), else the fp64 DMMA kernel (F64); I8 / I8_DIRECT force
 the two int8 modes; F64_STRICT = all-fp64 verification mode.
@@ -176,8 +176,7 @@ def test_airfoil_golden(eng, mode):
 def test_auto_magnitude_gate(eng):
     """AUTO runs the int8 Gram only on shards whose scaled squared norms are small: large norms mean tiny kernel values,
     where the 2^-24 ABSOLUTE error of the fixed-point elements -- with either distance form -- loses the posterior mean on
-    ill-conditioned systems (profiles/r02o_i8_conditioning.txt: airfoil-like data 1.5e-4 .. 1.5e-2 against 7e-7 .. 7e-6 of
-    the fp64 kernel).  Airfoil (mean scaled squared norm ~6 for points and active set, maxima ~40) stays on the fp64
+    ill-conditioned systems (airfoil-like data: 1.5e-4 .. 1.5e-2 against 7e-7 .. 7e-6 of the fp64 kernel).  Airfoil (mean scaled squared norm ~6 for points and active set, maxima ~40) stays on the fp64
     kernel even when the shard is large -- and keeps the posterior mean / variance inside 1e-5 of the all-fp64 mode; the
     benchmark's unit cube (mean ~2.2) runs the int8 kernel; small shards stay on the fp64 kernel."""
     c = np.load(os.path.join(GOLD, "airfoil_case.npz"))
@@ -372,7 +371,7 @@ def test_full_size_config2_properties(eng):
     assert np.all(np.abs(G) <= np.sqrt(np.outer(np.diag(G), np.diag(G))) * (1 + 1e-12))   # Cauchy-Schwarz
     mv, _ = eng.magic(G, b, copy_out=True)
     assert np.all(np.isfinite(mv))
-    # (e) full-size prediction parity of the default (tcgen05 int8) path against the all-fp64 kernel, which the small
+    # (e) full-size prediction parity of the default (int8) path against the all-fp64 kernel, which the small
     # cases above pin on the oracle:  posterior mean and variance at 1000 held-out points within TOL_PRED
     Xt = rng.random((1000, d))
     mean8, var8 = eng.predict(Xt)
@@ -599,7 +598,7 @@ def _oracle_stats_chunked(ok, X, y, Z, chunk=2048):
 
 
 def test_i8_headline_path_vs_oracle(eng):
-    """BASELINE configs[1] shape on a shard AUTO routes to the tcgen05 int8 kernel (>= 32768 points): G, b <= 1e-6
+    """BASELINE configs[1] shape on a shard AUTO routes to the int8 kernel (>= 32768 points): G, b <= 1e-6
     (SURVEY 8(d) gate) and posterior mean / variance at 1000 held-out points <= 1e-5 against the ORACLE itself (all
     worker cores, ~3 s) -- not against another kernel of this library."""
     from oracle.cpu_baseline import stats_parallel
@@ -627,8 +626,7 @@ def test_i8_headline_path_vs_oracle(eng):
 def test_i8_config_shapes_vs_oracle(eng, n, d, m):
     """Sub-shards of BASELINE configs[3] (d=32, m=2000: two 64-column K chunks of the distance contraction, 136 G tiles)
     and configs[4] (d=8, m=4000: 528 G tiles = more CTAs than SMs), plus d = 17 / 31 / 1 and a ragged point count, on
-    the forced int8 kernel against the oracle, at the SURVEY 8(d) gate of 1e-6 (measured 1.3e-7 .. 7.7e-7,
-    profiles/r02a_gpu_tests_r1kernel.log)."""
+    the forced int8 kernel against the oracle, at the SURVEY 8(d) gate of 1e-6."""
     X, y, Z, k, ok = _bench_workload(n, d, m, seed=100 + d)
     G0, b0 = _oracle_stats_chunked(ok, X, y, Z)
     G, b = run_stats(eng, k, X, y, Z, N.SGP_PREC_I8)

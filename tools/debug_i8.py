@@ -1,4 +1,4 @@
-"""GPU-side bring-up diagnostics for the tcgen05 int8 path (run on the GPU box).
+"""GPU-side bring-up diagnostics for the int8 path (run on the GPU box).
 Stage 1: T tile of the distance contraction vs an exact CPU model of the fp16 split operands.
 Stage 2: fixed-point words vs round(2^T * C0).   Stage 3: G, b vs the fp64 oracle, several shapes."""
 import sys, time

@@ -1,4 +1,4 @@
-"""CPU emulation of the tcgen05 int8 path's arithmetic (design study, not product code): which error term moves the
+"""CPU emulation of the int8 path's arithmetic (design study, not product code): which error term moves the
 posterior mean?  (a) fixed-point quantisation + dropped low-digit products (exact integer model);
 (b) fp32 accumulation of T = -q log2 e in the tensor core, modelled as round-toward-zero at each k-step."""
 import sys, time
