@@ -208,9 +208,6 @@ int sgp_last_bcm_path(const sgp_ctx* ctx);
  * the first CTA of the last launch, T = -q*log2(e) (128 active rows x 64 points, fp32) and the fixed-point words
  * (0x4B000000 | (u + 0x4040)), u = s2*2^15 + s1*2^7 + s0 in balanced digits. */
 int sgp_debug_i8_tile(sgp_ctx* ctx, float* T_out /* 128*64 */, uint32_t* w_out /* 128*64 */);
-/* Debug aid kept for ABI compatibility: the int8 Gram kernel of this build records no timeline, so this returns
- * SGP_E_STATE. */
-int sgp_debug_i8_timeline(sgp_ctx* ctx, long long* out);
 /* GreedilyOptimizingActiveSetProvider (commons/ActiveSetProvider.scala:58-139) with rank-1 updates: selects m_target points
  * of the shard X (n x d fp64, host) by the reference's forward selection and returns their row indices.  The reference
  * recomputes the statistics, two m x m inverses and three quadratic forms per candidate in every round (ASP:83-137); here

@@ -52,47 +52,120 @@ int fail(Ctx* c, int code, const std::string& msg) {
 static void free_active_set(Ctx* c) {
   cudaFree(c->dZ); cudaFree(c->dZs); cudaFree(c->dBeta); cudaFree(c->dGb);
   cudaFree(c->dMagicVec); cudaFree(c->dMagicMat);
-  cudaFree(c->dI8Scale); cudaFree(c->dI8Centre); cudaFree(c->dI8Flags); cudaFree(c->dI8Zt); cudaFree(c->dI8NormSum);
-  cudaFree(c->dI8Zd); cudaFree(c->dI8DScale); c->dI8Zd = nullptr; c->dI8DScale = nullptr; c->i8_direct_ok = false;
-  c->i8d_zd_bytes = c->i8d_sc_bytes = 0; c->i8d_prepared = false;
-  c->dI8NormSum = nullptr;
+  cudaFree(c->dI8Scale); cudaFree(c->dI8Flags); cudaFree(c->dI8Zt); cudaFree(c->dI8NormSum);
   c->dZ = c->dZs = c->dBeta = c->dGb = c->dMagicVec = c->dMagicMat = nullptr;
-  c->dI8Scale = c->dI8Centre = nullptr; c->dI8Flags = nullptr; c->dI8Zt = nullptr; c->i8_ok = false;
+  c->dI8Scale = c->dI8NormSum = nullptr; c->dI8Flags = nullptr; c->dI8Zt = nullptr;
+  c->i8_ok = c->i8_direct_ok = c->i8d_prepared = false;
 }
 
-static int ensure_partials(Ctx* c, int n_slices) {
-  const size_t gb = static_cast<size_t>(n_slices) * c->m_pad * c->m_pad * sizeof(double);
-  const size_t bb = static_cast<size_t>(n_slices) * c->m_pad * sizeof(double);
-  if (gb > c->gpart_bytes) {
-    cudaFree(c->dGpart); c->dGpart = nullptr; c->gpart_bytes = 0;
-    SGP_CUDA(c, cudaMalloc(&c->dGpart, gb));
-    c->gpart_bytes = gb;
-  }
-  if (bb > c->bpart_bytes) {
-    cudaFree(c->dBpart); c->dBpart = nullptr; c->bpart_bytes = 0;
-    SGP_CUDA(c, cudaMalloc(&c->dBpart, bb));
-    c->bpart_bytes = bb;
+// Flattens a kernel description: Eye terms drop out of the cross kernel (kernel/Kernel.scala:157) and only sum their
+// coefficients into eye_sum; the other terms' feature scales go to beta = [kMaxTerms][beta_stride] (zero padded).
+// flat_of (optional) receives the flattened index of every term, -1 for Eye terms.
+static int flatten_kernel(Ctx* c, const sgp_kernel_desc* k, int d, int beta_stride, KernelFlat& kf,
+                          std::vector<double>& beta, std::vector<int>* flat_of) {
+  kf = KernelFlat{};
+  beta.assign(static_cast<size_t>(kMaxTerms) * beta_stride, 0.0);
+  if (flat_of) flat_of->assign(k->n_terms, -1);
+  for (int t = 0; t < k->n_terms; ++t) {
+    const sgp_kernel_term& term = k->terms[t];
+    if (!(term.scale >= 0.0)) return fail(c, SGP_E_BADARG, "requirement failed: C should be positive");
+    kf.self_kernel += term.scale;
+    if (term.type == SGP_TERM_EYE) { kf.eye_sum += term.scale; continue; }
+    if (kf.n_terms == kMaxTerms) return fail(c, SGP_E_BADARG, "too many non-Eye kernel terms (max 4)");
+    double* bt = beta.data() + static_cast<size_t>(kf.n_terms) * beta_stride;
+    if (term.type == SGP_TERM_ARD) {
+      if (!term.beta) return fail(c, SGP_E_BADARG, "ARD term without beta");
+      for (int j = 0; j < d; ++j) bt[j] = term.beta[j];
+    } else if (term.type == SGP_TERM_RBF) {
+      if (!(term.sigma > 0.0)) return fail(c, SGP_E_BADARG, "RBF sigma must be > 0");
+      // exp(-|x-z|^2 / (2 sigma^2)) = exp(-sum_k (x_k - z_k)^2 beta^2), beta = 1/(sqrt(2) sigma)
+      for (int j = 0; j < d; ++j) bt[j] = 1.0 / (std::sqrt(2.0) * term.sigma);
+    } else {
+      return fail(c, SGP_E_BADARG, "unknown kernel term type");
+    }
+    if (flat_of) (*flat_of)[t] = kf.n_terms;
+    kf.scale[kf.n_terms++] = term.scale;
   }
   return SGP_OK;
 }
 
-// Device side of the direct-distance mode for the current begin() window: per-term scales + centre, active-set tiles
-int direct_prepare(Ctx* c) {
-  if (c->i8d_prepared) return SGP_OK;
-  const int dpad4 = c->i8_dpad4;
-  const size_t zd_bytes = static_cast<size_t>(c->m_pad / kTile) * c->kf.n_terms * kTile * dpad4 * sizeof(float);
-  const size_t sc_bytes = c->i8d_sc.size() * 8;
-  if (zd_bytes > c->i8d_zd_bytes || sc_bytes > c->i8d_sc_bytes || !c->dI8Zd) {
-    cudaFree(c->dI8Zd); cudaFree(c->dI8DScale); c->dI8Zd = nullptr; c->dI8DScale = nullptr;
-    c->i8d_zd_bytes = c->i8d_sc_bytes = 0;
-    SGP_CUDA(c, cudaMalloc(&c->dI8Zd, zd_bytes));
-    SGP_CUDA(c, cudaMalloc(&c->dI8DScale, sc_bytes));
-    c->i8d_zd_bytes = zd_bytes; c->i8d_sc_bytes = sc_bytes;
+// Streams the host rows X (n rows of `row` bytes) and y through the two staging buffers, so that the copy of one chunk
+// (copy_stream) overlaps the kernels of the previous one (compute stream).  The first chunk has `first` points, the
+// others `chunk` (first <= chunk); launch(dX, dy, p0, cn) enqueues the consumer of points [p0, p0 + cn) on the compute
+// stream.  Returns when every copy is done: the caller may reuse X and y.
+template <class Launch>
+static int stage_rows(Ctx* c, const void* X, const double* y, long long n, size_t row, long long first, long long chunk,
+                      Launch&& launch) {
+  const size_t xb = row * chunk, yb = static_cast<size_t>(chunk) * 8;
+  if (xb > c->stage_x[0].cap || yb > c->stage_y[0].cap) {
+    SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+    SGP_CUDA(c, cudaStreamSynchronize(c->copy_stream));
+    for (int i = 0; i < 2; ++i) {
+      int rc = ctx_scratch(c, c->stage_x[i], xb);
+      if (rc == SGP_OK) rc = ctx_scratch(c, c->stage_y[i], yb);
+      if (rc != SGP_OK) return rc;
+      SGP_CUDA(c, cudaEventRecord(c->stage_free[i], c->stream));
+    }
   }
-  SGP_CUDA(c, cudaMemcpyAsync(c->dI8DScale, c->i8d_sc.data(), sc_bytes, cudaMemcpyHostToDevice, c->stream));
-  SGP_CUDA(c, launch_i8_prep_active_direct(c->dI8Zd, c->dZ, c->m, c->m_pad, c->d, dpad4, c->kf.n_terms, c->dI8DScale,
-                                           c->dI8DScale + static_cast<size_t>(kMaxTerms) * dpad4, c->dI8Flags,
-                                           c->i8_direct_r2max, c->stream));
+  const char* Xb = static_cast<const char*>(X);
+  int buf = 0;
+  for (long long p0 = 0, step = first; p0 < n; p0 += step, step = chunk, buf ^= 1) {
+    const long long cn = (n - p0 < step) ? (n - p0) : step;
+    void* sx = c->stage_x[buf].p;
+    double* sy = c->stage_y[buf].as<double>();
+    SGP_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->stage_free[buf], 0));
+    SGP_CUDA(c, cudaMemcpyAsync(sx, Xb + static_cast<size_t>(p0) * row, row * cn, cudaMemcpyHostToDevice, c->copy_stream));
+    SGP_CUDA(c, cudaMemcpyAsync(sy, y + p0, static_cast<size_t>(cn) * 8, cudaMemcpyHostToDevice, c->copy_stream));
+    SGP_CUDA(c, cudaEventRecord(c->stage_ready[buf], c->copy_stream));
+    SGP_CUDA(c, cudaStreamWaitEvent(c->stream, c->stage_ready[buf], 0));
+    const int rc = launch(sx, sy, p0, cn);
+    if (rc != SGP_OK) return rc;
+    SGP_CUDA(c, cudaEventRecord(c->stage_free[buf], c->stream));
+  }
+  SGP_CUDA(c, cudaStreamSynchronize(c->copy_stream));
+  return SGP_OK;
+}
+
+// Host state of both int8 modes for the active set Z (m x d) and the flattened beta ([kMaxTerms][dpad]):
+// sc = [kMaxTerms][dpad] sqrt(log2 e) * beta_tk, then the [dpad] centre (distances are translation invariant, the
+// active-set mean keeps the operands small).  Returns the mean scaled squared norm of the active set under the widest
+// term, which AUTO's magnitude budget adds to the points' mean.
+static double i8_scales(const double* Z, int m, int d, int dpad, int n_terms, const std::vector<double>& beta,
+                        std::vector<double>& sc) {
+  sc.assign(static_cast<size_t>(kMaxTerms + 1) * dpad, 0.0);
+  double* ctr = sc.data() + static_cast<size_t>(kMaxTerms) * dpad;
+  const double s2 = std::sqrt(1.4426950408889634074);          // sqrt(log2 e): exponent in base 2
+  for (int t = 0; t < n_terms; ++t)
+    for (int j = 0; j < d; ++j) sc[static_cast<size_t>(t) * dpad + j] = s2 * beta[static_cast<size_t>(t) * dpad + j];
+  for (int j = 0; j < d; ++j) {
+    double acc = 0.0;
+    for (int i = 0; i < m; ++i) acc += Z[static_cast<size_t>(i) * d + j];
+    ctr[j] = acc / m;
+  }
+  double best = 1e300;
+  for (int t = 0; t < n_terms; ++t) {
+    const double* st = sc.data() + static_cast<size_t>(t) * dpad;
+    double zsum = 0.0;
+    for (int i = 0; i < m; ++i)
+      for (int j = 0; j < d; ++j) {
+        const double v = (Z[static_cast<size_t>(i) * d + j] - ctr[j]) * st[j];
+        zsum += v * v;
+      }
+    best = std::min(best, zsum / m);
+  }
+  return best;
+}
+
+// Active-set tiles of the direct-distance mode, built on its first launch in a begin() window: a window that only runs
+// tensor-core or fp64 launches never pays for them.
+static int direct_prepare(Ctx* c) {
+  if (c->i8d_prepared) return SGP_OK;
+  const size_t zd_bytes = static_cast<size_t>(c->m_pad / kTile) * c->kf.n_terms * kTile * c->dpad * sizeof(float);
+  const int rc = ctx_scratch(c, c->i8_zd_ws, zd_bytes);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, launch_i8_prep_active_direct(c->i8_zd_ws.as<float>(), c->dZ, c->m, c->m_pad, c->d, c->dpad, c->kf.n_terms,
+                                           c->dI8Scale, c->dI8Scale + static_cast<size_t>(kMaxTerms) * c->dpad,
+                                           c->dI8Flags, kI8DirectR2Max, c->stream));
   c->launches += 1;
   c->i8d_prepared = true;
   return SGP_OK;
@@ -112,18 +185,11 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   const long long blocks = (n + 15) / 16;
   if (n_slices > blocks) n_slices = static_cast<int>(blocks);
   // int8 kernel: one launch over the upper block triangle x point slices
-  const int i8_n_slices = (c->i8_ok || c->i8_direct_ok) ? i8_slices(c->m_pad, c->num_sms, (n + 63) / 64) : 1;
-  int rc = ensure_partials(c, n_slices > i8_n_slices ? n_slices : i8_n_slices);
+  const int i8_n_slices = c->i8_direct_ok ? i8_slices(c->m_pad, c->num_sms, (n + 63) / 64) : 1;
+  const int max_slices = n_slices > i8_n_slices ? n_slices : i8_n_slices;
+  int rc = ctx_scratch(c, c->gpart_ws, static_cast<size_t>(max_slices) * c->m_pad * c->m_pad * sizeof(double));
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->bpart_ws, static_cast<size_t>(max_slices) * c->m_pad * sizeof(double));
   if (rc != SGP_OK) return rc;
-
-  GramParams p{};
-  p.X = dX; p.y = dy; p.n = n; p.x_is_f32 = x_is_f32;
-  p.d = c->d; p.dpad = c->dpad; p.m = c->m; p.m_pad = c->m_pad;
-  p.n_terms = c->kf.n_terms;
-  for (int t = 0; t < kMaxTerms; ++t) p.scale[t] = c->kf.scale[t];
-  p.Zs = c->dZs; p.beta = c->dBeta;
-  p.Gpart = c->dGpart; p.bpart = c->dBpart;
-  p.n_slices = n_slices; p.n_tiles_1d = nt1;
 
   // AUTO: the int8 kernel inside its measured parity envelope -- accumulate calls of >= 32768 points (posterior
   // mean within a few 1e-6 of the all-fp64 kernel from N = 16k up; the limit is the two dropped low-order digit
@@ -132,101 +198,62 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   // (2e-7), which needs < 2 ms at that size.
   // Path of this launch: 0 = fp64 DMMA kernel, 1 = int8 Gram with tensor-core distances (one term, d <= 32, benign norms),
   // 2 = int8 Gram with direct fp32 distances (up to 4 terms, d <= 72; AUTO: same magnitude budget as path 1).
-  const bool tensor_ok = c->i8_ok, direct_ok = c->i8_direct_ok;
   int path = 0;
   if (c->precision == SGP_PREC_I8) {
-    if (tensor_ok) path = 1;
-    else if (direct_ok) path = 2;
+    if (c->i8_ok) path = 1;
+    else if (c->i8_direct_ok) path = 2;
     else return fail(c, SGP_E_BADARG, "SGP_PREC_I8 needs a kernel with 1..4 non-Eye terms and n_terms * d <= 72 "
                                       "(tensor-core distances: exactly one term and d <= 32)");
   } else if (c->precision == SGP_PREC_I8_DIRECT) {
-    if (!direct_ok) return fail(c, SGP_E_BADARG, "SGP_PREC_I8_DIRECT needs a kernel with 1..4 non-Eye terms and n_terms * d <= 72");
+    if (!c->i8_direct_ok) return fail(c, SGP_E_BADARG, "SGP_PREC_I8_DIRECT needs a kernel with 1..4 non-Eye terms and n_terms * d <= 72");
     path = 2;
   } else if (c->precision == SGP_PREC_AUTO && n_call >= kAutoI8MinPoints) {
-    path = tensor_ok ? 1 : (direct_ok ? 2 : 0);
-    if (!first_of_call) path = c->call_path;
+    path = !first_of_call ? c->call_path : c->i8_ok ? 1 : c->i8_direct_ok ? 2 : 0;
   }
-  bool use_i8 = (path == 1);
   if (path != 0) {
-    const size_t yb = static_cast<size_t>((n + 63) / 64) * 64 * sizeof(float);
-    if (yb > c->i8_ys_bytes) {
-      cudaFree(c->dI8Ys); c->dI8Ys = nullptr; c->i8_ys_bytes = 0;
-      SGP_CUDA(c, cudaMalloc(&c->dI8Ys, yb));
-      c->i8_ys_bytes = yb;
-    }
-  }
-  if (use_i8) {
-    const int nch = i8_nchunks(c->d);
-    const size_t xb = i8_points_scratch_bytes(n, nch);
-    if (xb > c->i8_xt_bytes) {
-      cudaFree(c->dI8Xt); c->dI8Xt = nullptr; c->i8_xt_bytes = 0;
-      SGP_CUDA(c, cudaMalloc(&c->dI8Xt, xb));
-      c->i8_xt_bytes = xb;
-    }
-    const bool gate = (c->precision == SGP_PREC_AUTO) && first_of_call;
+    const bool autop = c->precision == SGP_PREC_AUTO;
+    const bool gate = autop && first_of_call;
+    const size_t xb = (path == 1) ? i8_points_scratch_bytes(n, i8_nchunks(c->d))
+                                  : static_cast<size_t>((n + 63) / 64) * c->kf.n_terms * 64 * c->dpad * sizeof(float);
+    rc = ctx_scratch(c, c->i8_ys_ws, static_cast<size_t>((n + 63) / 64) * 64 * sizeof(float));
+    if (rc == SGP_OK) rc = ctx_scratch(c, c->i8_xt_ws, xb);
+    if (rc == SGP_OK && path == 2) rc = direct_prepare(c);
+    if (rc != SGP_OK) return rc;
     // the scaled squared norms of EVERY chunk are summed on the device (dI8NormSum[0]: whole begin..finish window,
     // checked against the budget at finish so that an unrepresentative first chunk cannot silently degrade the
-    // statistics; dI8NormSum[1]: this call's first chunk, read back here for the kernel choice)
-    if (gate) SGP_CUDA(c, cudaMemsetAsync(c->dI8NormSum + 1, 0, sizeof(double), c->stream));
-    SGP_CUDA(c, launch_i8_prep_points(c->dI8Xt, c->dI8Ys, dX, x_is_f32, dy, n, c->d, c->dI8Scale, c->dI8Centre,
-                                      c->dI8Flags, c->dI8NormSum, gate ? c->dI8NormSum + 1 : nullptr, c->stream));
+    // statistics; dI8NormSum[1]: this call's first chunk, read back here for the kernel choice).  The direct mode sums
+    // the WIDEST term's scaled squared norms: they set the size of the kernel values.
+    double* call_sum = gate ? c->dI8NormSum + 1 : nullptr;
+    if (gate) SGP_CUDA(c, cudaMemsetAsync(call_sum, 0, sizeof(double), c->stream));
+    if (path == 1)
+      SGP_CUDA(c, launch_i8_prep_points(c->i8_xt_ws.as<uint8_t>(), c->i8_ys_ws.as<float>(), dX, x_is_f32, dy, n, c->d,
+                                        c->dI8Scale, c->dI8Scale + static_cast<size_t>(kMaxTerms) * c->dpad, c->dI8Flags,
+                                        c->dI8NormSum, call_sum, c->stream));
+    else
+      SGP_CUDA(c, launch_i8_prep_points_direct(c->i8_xt_ws.as<float>(), c->i8_ys_ws.as<float>(), dX, x_is_f32, dy, n, c->d,
+                                               c->dpad, c->kf.n_terms, c->dI8Scale,
+                                               c->dI8Scale + static_cast<size_t>(kMaxTerms) * c->dpad, c->dI8Flags,
+                                               kI8DirectR2Max, autop ? c->dI8NormSum : nullptr, call_sum, c->stream));
     c->launches += 1;
     if (gate) {
       // AUTO's magnitude gate.  The distance contraction accumulates 2 x^.z^ - |x^|^2 - |z^|^2 in fp32 in tensor
       // memory; its rounding (toward zero, measured) scales with those magnitudes: at mean|x^|^2 + mean|z^|^2 ~ 4.4
       // the elements are good to 2.7e-7 rms (parity holds, tests), at ~12 (airfoil: norms up to 40) they are not
-      // (posterior mean off by 5e-4).  Above the budget the shard goes to the fp64 DMMA kernel instead.
+      // (posterior mean off by 5e-4).  Large scaled norms also mean tiny kernel values, and the fixed-point digits carry
+      // an ABSOLUTE error of 2^-24: on such shards the int8 Gram -- with either distance form -- loses the posterior
+      // mean (airfoil-like data: 1.5e-4 to 1.5e-2 against 7e-7 .. 7e-6 of the fp64 kernel).  Above the budget the
+      // shard goes to the fp64 DMMA kernel instead.
       double xsum = 0.0;
-      SGP_CUDA(c, cudaMemcpyAsync(&xsum, c->dI8NormSum + 1, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+      SGP_CUDA(c, cudaMemcpyAsync(&xsum, call_sum, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
       SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-      if (xsum / static_cast<double>(n) + c->i8_z_norm_mean > c->i8_norm_budget) {
-        // Large scaled norms mean tiny kernel values, and the fixed-point digits carry an ABSOLUTE error of 2^-24: on
-        // such shards the int8 Gram -- with either distance form -- loses the posterior mean (airfoil-like data: 1.5e-4
-        // to 1.5e-2 against 7e-7 .. 7e-6 of the fp64 kernel).  fp64 DMMA kernel.
-        use_i8 = false;
-        path = 0;
-      }
+      if (xsum / static_cast<double>(n) + c->i8_z_norm_mean > kI8NormBudget) path = 0;
     }
-  }
-  I8Direct direct;
-  if (path == 2) {
-    const size_t xb = static_cast<size_t>((n + 63) / 64) * c->kf.n_terms * 64 * c->i8_dpad4 * sizeof(float);
-    if (xb > c->i8_xt_bytes) {
-      cudaFree(c->dI8Xt); c->dI8Xt = nullptr; c->i8_xt_bytes = 0;
-      SGP_CUDA(c, cudaMalloc(&c->dI8Xt, xb));
-      c->i8_xt_bytes = xb;
-    }
-    // AUTO applies the same magnitude budget as with tensor-core distances (on the WIDEST term's scaled squared norms: it
-    // sets the size of the kernel values): first chunk here, whole window at finish
-    rc = direct_prepare(c);
-    if (rc != SGP_OK) return rc;
-    const bool dgate = (c->precision == SGP_PREC_AUTO) && first_of_call;
-    const bool dbudget = (c->precision == SGP_PREC_AUTO);
-    if (dgate) SGP_CUDA(c, cudaMemsetAsync(c->dI8NormSum + 1, 0, sizeof(double), c->stream));
-    SGP_CUDA(c, launch_i8_prep_points_direct(reinterpret_cast<float*>(c->dI8Xt), c->dI8Ys, dX, x_is_f32, dy, n, c->d,
-                                             c->i8_dpad4, c->kf.n_terms, c->dI8DScale,
-                                             c->dI8DScale + static_cast<size_t>(kMaxTerms) * c->i8_dpad4, c->dI8Flags,
-                                             c->i8_direct_r2max, dbudget ? c->dI8NormSum : nullptr,
-                                             dgate ? c->dI8NormSum + 1 : nullptr, c->stream));
-    c->launches += 1;
-    if (dgate) {
-      double xsum = 0.0;
-      SGP_CUDA(c, cudaMemcpyAsync(&xsum, c->dI8NormSum + 1, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-      SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-      if (xsum / static_cast<double>(n) + c->i8d_z_norm_mean > c->i8_norm_budget) path = 0;
-    }
-  }
-  if (path == 2) {
-    direct.on = 1; direct.n_terms = c->kf.n_terms; direct.dpad4 = c->i8_dpad4;
-    double csum = 0.0;
-    for (int t = 0; t < c->kf.n_terms; ++t) csum += c->kf.scale[t];
-    for (int t = 0; t < c->kf.n_terms; ++t) direct.w[t] = static_cast<float>(c->kf.scale[t] / csum);
-    direct.csum = csum;
-    c->i8_direct_used = true;
   }
   if (first_of_call) c->call_path = path;
-  if (use_i8 || path == 2) c->i8_points += n;
-  if (use_i8) c->i8_used = true;
+  if (path != 0) {
+    c->i8_points += n;
+    c->i8_flag_mask |= (path == 1) ? 1 : 4;
+  }
   c->last_path = (path == 1) ? SGP_PREC_I8 : (path == 2) ? SGP_PREC_I8_DIRECT
                  : (c->precision == SGP_PREC_F64_STRICT ? SGP_PREC_F64_STRICT : SGP_PREC_F64);
   if (c->gram_events_used == c->gram_events.size()) {          // grow the event pool (steady state: no creation)
@@ -239,20 +266,38 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   c->gram_events_used += 1;
   SGP_CUDA(c, cudaEventRecord(e0, c->stream));
   const size_t mm = static_cast<size_t>(c->m) * c->m;
-  if (use_i8 || path == 2) {
-    const uint8_t* zop = (path == 2) ? reinterpret_cast<const uint8_t*>(c->dI8Zd) : c->dI8Zt;
-    SGP_CUDA(c, launch_gram_i8(c->dI8Xt, c->dI8Ys, zop, n, c->d, c->m_pad, i8_n_slices, direct, c->dGpart, c->dBpart,
-                               c->kf.scale[0], c->dbgT, c->dbgW, c->stream));
+  double* Gpart = c->gpart_ws.as<double>();
+  double* bpart = c->bpart_ws.as<double>();
+  if (path != 0) {
+    I8Direct direct;
+    if (path == 2) {
+      direct.on = 1; direct.n_terms = c->kf.n_terms; direct.dpad4 = c->dpad;
+      double csum = 0.0;
+      for (int t = 0; t < c->kf.n_terms; ++t) csum += c->kf.scale[t];
+      for (int t = 0; t < c->kf.n_terms; ++t) direct.w[t] = static_cast<float>(c->kf.scale[t] / csum);
+      direct.csum = csum;
+    }
+    const uint8_t* zop = (path == 2) ? c->i8_zd_ws.as<uint8_t>() : c->dI8Zt;
+    SGP_CUDA(c, launch_gram_i8(c->i8_xt_ws.as<uint8_t>(), c->i8_ys_ws.as<float>(), zop, n, c->d, c->m_pad, i8_n_slices,
+                               direct, Gpart, bpart, c->kf.scale[0], c->dbgT, c->dbgW, c->stream));
     SGP_CUDA(c, cudaEventRecord(e1, c->stream));
     // deterministic slice reduction (partial tiles at the mirror position: upper block triangle)
-    SGP_CUDA(c, launch_gram_reduce_upper(c->dGb, c->dGb + mm, c->dGpart, c->dBpart, i8_n_slices, c->m, c->m_pad, 0, c->m,
+    SGP_CUDA(c, launch_gram_reduce_upper(c->dGb, c->dGb + mm, Gpart, bpart, i8_n_slices, c->m, c->m_pad, 0, c->m,
                                          c->stream));
     c->launches += 2;
     return SGP_OK;
   }
+  GramParams p{};
+  p.X = dX; p.y = dy; p.n = n; p.x_is_f32 = x_is_f32;
+  p.d = c->d; p.dpad = c->dpad; p.m = c->m; p.m_pad = c->m_pad;
+  p.n_terms = c->kf.n_terms;
+  for (int t = 0; t < kMaxTerms; ++t) p.scale[t] = c->kf.scale[t];
+  p.Zs = c->dZs; p.beta = c->dBeta;
+  p.Gpart = Gpart; p.bpart = bpart;
+  p.n_slices = n_slices; p.n_tiles_1d = nt1;
   SGP_CUDA(c, launch_gram_f64(p, c->precision == SGP_PREC_F64_STRICT, c->stream));
   SGP_CUDA(c, cudaEventRecord(e1, c->stream));
-  SGP_CUDA(c, launch_gram_reduce(c->dGb, c->dGb + mm, c->dGpart, c->dBpart, n_slices, c->m, c->m_pad, c->stream));
+  SGP_CUDA(c, launch_gram_reduce(c->dGb, c->dGb + mm, Gpart, bpart, n_slices, c->m, c->m_pad, c->stream));
   c->launches += 2;
   return SGP_OK;
 }
@@ -317,16 +362,17 @@ int sgp_ctx_destroy(sgp_ctx* h) {
   drop_gram_events(c);
   for (auto& e : c->user_events) if (e) cudaEventDestroy(e);
   free_active_set(c);
-  cudaFree(c->dGpart); cudaFree(c->dBpart);
-  cudaFree(c->dEx); cudaFree(c->dEy); cudaFree(c->dEoff); cudaFree(c->dEf); cudaFree(c->dNllPer); cudaFree(c->dNllScratch);
-  cudaFree(c->dI8Xt); cudaFree(c->dI8Ys); cudaFree(c->dbgT); cudaFree(c->dbgW);
+  cudaFree(c->dEx); cudaFree(c->dEy); cudaFree(c->dEoff); cudaFree(c->dEf); cudaFree(c->dNllScratch);
+  cudaFree(c->dbgT); cudaFree(c->dbgW);
   for (int i = 0; i < 2; ++i) {
-    cudaFree(c->stageX[i]); cudaFree(c->stageY[i]);
+    cudaFree(c->stage_x[i].p); cudaFree(c->stage_y[i].p);
     if (c->stage_free[i]) cudaEventDestroy(c->stage_free[i]);
     if (c->stage_ready[i]) cudaEventDestroy(c->stage_ready[i]);
   }
   if (c->comm && nccl().ok) nccl().CommDestroy(c->comm);
-  cudaFree(c->greedy_ws.p); cudaFree(c->sweep_ws.p); cudaFree(c->bcm_ws.p); cudaFree(c->tail_ws.p); cudaFree(c->tail_ws2.p); cudaFree(c->predict_ws.p); cudaFree(c->cross_ws.p);
+  for (DevScratch* s : {&c->gpart_ws, &c->bpart_ws, &c->i8_zd_ws, &c->i8_xt_ws, &c->i8_ys_ws, &c->nll_per_ws, &c->greedy_ws,
+                        &c->sweep_ws, &c->bcm_ws, &c->tail_ws, &c->tail_ws2, &c->predict_ws, &c->cross_ws})
+    cudaFree(s->p);
   if (c->tail_fork) cudaEventDestroy(c->tail_fork);
   if (c->tail_join) cudaEventDestroy(c->tail_join);
   if (c->tail_stream) cudaStreamDestroy(c->tail_stream);
@@ -382,29 +428,11 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
   if (!k || !Z || m <= 0 || d <= 0 || k->n_terms <= 0 || !k->terms)
     return fail(c, SGP_E_BADARG, "sgp_stats_begin: null or empty argument");
   SGP_CUDA(c, cudaSetDevice(c->device));
-  // ---- flatten: drop Eye terms from the cross path (kernel/Kernel.scala:157), sum their coefficients ----
   KernelFlat kf;
+  std::vector<double> beta;
   const int dpad = (d + 3) & ~3;
-  std::vector<double> beta(static_cast<size_t>(kMaxTerms) * dpad, 0.0);
-  for (int t = 0; t < k->n_terms; ++t) {
-    const sgp_kernel_term& term = k->terms[t];
-    if (!(term.scale >= 0.0)) return fail(c, SGP_E_BADARG, "requirement failed: C should be positive");
-    kf.self_kernel += term.scale;
-    if (term.type == SGP_TERM_EYE) { kf.eye_sum += term.scale; continue; }
-    if (kf.n_terms == kMaxTerms) return fail(c, SGP_E_BADARG, "too many non-Eye kernel terms (max 4)");
-    double* bt = beta.data() + static_cast<size_t>(kf.n_terms) * dpad;
-    if (term.type == SGP_TERM_ARD) {
-      if (!term.beta) return fail(c, SGP_E_BADARG, "ARD term without beta");
-      for (int j = 0; j < d; ++j) bt[j] = term.beta[j];
-    } else if (term.type == SGP_TERM_RBF) {
-      if (!(term.sigma > 0.0)) return fail(c, SGP_E_BADARG, "RBF sigma must be > 0");
-      // exp(-|x-z|^2 / (2 sigma^2)) = exp(-sum_k (x_k - z_k)^2 beta^2), beta = 1/(sqrt(2) sigma)
-      for (int j = 0; j < d; ++j) bt[j] = 1.0 / (std::sqrt(2.0) * term.sigma);
-    } else {
-      return fail(c, SGP_E_BADARG, "unknown kernel term type");
-    }
-    kf.scale[kf.n_terms++] = term.scale;
-  }
+  int rc = flatten_kernel(c, k, d, dpad, kf, beta, nullptr);
+  if (rc != SGP_OK) return rc;
   // device buffers are kept across begin() calls with the same (m, d, term count): cudaMalloc/cudaFree are
   // synchronising and cost milliseconds -- more than the whole statistics pass on the GPU
   const int nt = kf.n_terms > 0 ? kf.n_terms : 1;
@@ -414,6 +442,10 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
     free_active_set(c);
   }
   c->m = m; c->d = d; c->dpad = dpad; c->m_pad = (m + kTile - 1) / kTile * kTile; c->kf = kf;
+  // int8 Gram: direct distances for 1..4 non-Eye terms with n_terms * dpad <= 72 (shared memory); tensor-core distances
+  // for one term and d <= 32 (two 64-column K chunks)
+  c->i8_direct_ok = kf.n_terms >= 1 && kf.n_terms * dpad <= 72;
+  c->i8_ok = kf.n_terms == 1 && d <= 32;
   const size_t mm = static_cast<size_t>(m) * m;
   if (!same_shape) {
     c->alloc_terms = nt;
@@ -423,7 +455,12 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
     SGP_CUDA(c, cudaMalloc(&c->dGb, (mm + m + 1) * 8));     // [G ; b ; status] -- one all-reduce
     SGP_CUDA(c, cudaMalloc(&c->dMagicVec, static_cast<size_t>(m) * 8));
     SGP_CUDA(c, cudaMalloc(&c->dMagicMat, mm * 8));
+    SGP_CUDA(c, cudaMalloc(&c->dI8Flags, sizeof(int)));
+    SGP_CUDA(c, cudaMalloc(&c->dI8NormSum, 2 * sizeof(double)));
+    SGP_CUDA(c, cudaMalloc(&c->dI8Scale, static_cast<size_t>(kMaxTerms + 1) * dpad * 8));
   }
+  if (c->i8_ok && !c->dI8Zt)          // same_shape does not tell 0 from 1 non-Eye term
+    SGP_CUDA(c, cudaMalloc(&c->dI8Zt, i8_active_scratch_bytes(c->m_pad, i8_nchunks(d))));
   SGP_CUDA(c, cudaMemcpyAsync(c->dZ, Z, static_cast<size_t>(m) * d * 8, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaMemcpyAsync(c->dBeta, beta.data(), beta.size() * 8, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaMemsetAsync(c->dGb, 0, (mm + m + 1) * 8, c->stream));
@@ -432,88 +469,25 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
                                   c->dBeta + static_cast<size_t>(t) * dpad, m, c->m_pad, d, dpad, c->stream));
     c->launches += 1;
   }
-  // ---- int8 path with tensor-core distances: qualifies for one non-Eye term and d <= 32 (two 64-column K chunks) -------------
-  c->i8_ok = (kf.n_terms == 1 && d <= 32);
-  std::vector<double> sc16, ctr16;               // live until the synchronisation at the end of this function
-  if (!c->dI8Flags) {
-    SGP_CUDA(c, cudaMalloc(&c->dI8Flags, sizeof(int)));
-    SGP_CUDA(c, cudaMalloc(&c->dI8NormSum, 2 * sizeof(double)));
-  }
   SGP_CUDA(c, cudaMemsetAsync(c->dI8Flags, 0, sizeof(int), c->stream));
   SGP_CUDA(c, cudaMemsetAsync(c->dI8NormSum, 0, 2 * sizeof(double), c->stream));
+  std::vector<double> i8_sc;                       // live until the synchronisation at the end of this function
+  if (c->i8_direct_ok) {
+    c->i8_z_norm_mean = i8_scales(Z, m, d, dpad, kf.n_terms, beta, i8_sc);
+    SGP_CUDA(c, cudaMemcpyAsync(c->dI8Scale, i8_sc.data(), i8_sc.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  }
   if (c->i8_ok) {
-    const int dp16 = (d + 15) / 16 * 16;
-    std::vector<double>& sc = sc16; std::vector<double>& ctr = ctr16;
-    sc.assign(dp16, 0.0); ctr.assign(dp16, 0.0);
-    const double s2 = std::sqrt(1.4426950408889634074);          // sqrt(log2 e): exponent in base 2
-    for (int j = 0; j < d; ++j) {
-      sc[j] = s2 * beta[j];
-      double acc = 0.0;
-      for (int i = 0; i < m; ++i) acc += Z[static_cast<size_t>(i) * d + j];
-      ctr[j] = acc / m;                                          // distances are translation invariant
-    }
-    if (!c->dI8Scale) {
-      SGP_CUDA(c, cudaMalloc(&c->dI8Scale, dp16 * 8));
-      SGP_CUDA(c, cudaMalloc(&c->dI8Centre, dp16 * 8));
-      SGP_CUDA(c, cudaMalloc(&c->dI8Zt, i8_active_scratch_bytes(c->m_pad, i8_nchunks(d))));
-    }
-    {
-      double zsum = 0.0;
-      for (int i = 0; i < m; ++i)
-        for (int j = 0; j < d; ++j) {
-          const double v = (Z[static_cast<size_t>(i) * d + j] - ctr[j]) * sc[j];
-          zsum += v * v;
-        }
-      c->i8_z_norm_mean = zsum / m;
-      if (const char* e = getenv("SGP_I8_NORM_BUDGET")) c->i8_norm_budget = atof(e);
-    }
-    SGP_CUDA(c, cudaMemcpyAsync(c->dI8Scale, sc.data(), dp16 * 8, cudaMemcpyHostToDevice, c->stream));
-    SGP_CUDA(c, cudaMemcpyAsync(c->dI8Centre, ctr.data(), dp16 * 8, cudaMemcpyHostToDevice, c->stream));
-    SGP_CUDA(c, launch_i8_prep_active(c->dI8Zt, c->dZ, m, c->m_pad, d, c->dI8Scale, c->dI8Centre, c->dI8Flags,
-                                      c->stream));
+    // the tensor-core operand images are built here, the direct mode's active-set tiles on its first launch
+    SGP_CUDA(c, launch_i8_prep_active(c->dI8Zt, c->dZ, m, c->m_pad, d, c->dI8Scale,
+                                      c->dI8Scale + static_cast<size_t>(kMaxTerms) * dpad, c->dI8Flags, c->stream));
     c->launches += 1;
   }
-  // ---- direct-distance mode of the int8 Gram: 1..4 non-Eye terms, n_terms * dpad4 <= 72 (smem) ------------
-  {
-    const int dpad4 = (d + 3) & ~3;
-    c->i8_direct_ok = kf.n_terms >= 1 && kf.n_terms * dpad4 <= 72;
-    if (c->i8_direct_ok) {
-      c->i8_dpad4 = dpad4;
-      if (const char* e = getenv("SGP_I8_DIRECT_R2MAX")) c->i8_direct_r2max = static_cast<float>(atof(e));
-      std::vector<double>& sc = c->i8d_sc;                                           // [term][k] scales, then the centre
-      sc.assign(static_cast<size_t>(kMaxTerms + 1) * dpad4, 0.0);
-      const double s2 = std::sqrt(1.4426950408889634074);
-      for (int t = 0; t < kf.n_terms; ++t)
-        for (int j = 0; j < d; ++j) sc[static_cast<size_t>(t) * dpad4 + j] = s2 * beta[static_cast<size_t>(t) * dpad + j];
-      for (int j = 0; j < d; ++j) {
-        double acc = 0.0;
-        for (int i = 0; i < m; ++i) acc += Z[static_cast<size_t>(i) * d + j];
-        sc[static_cast<size_t>(kMaxTerms) * dpad4 + j] = acc / m;
-      }
-      {                                                   // mean scaled squared norm of the active set, widest term
-        double best = 1e300;
-        for (int t = 0; t < kf.n_terms; ++t) {
-          double zsum = 0.0;
-          for (int i = 0; i < m; ++i)
-            for (int j = 0; j < d; ++j) {
-              const double v = (Z[static_cast<size_t>(i) * d + j] - sc[static_cast<size_t>(kMaxTerms) * dpad4 + j]) *
-                               sc[static_cast<size_t>(t) * dpad4 + j];
-              zsum += v * v;
-            }
-          best = std::min(best, zsum / m);
-        }
-        c->i8d_z_norm_mean = best;
-        if (const char* e = getenv("SGP_I8_NORM_BUDGET")) c->i8_norm_budget = atof(e);
-      }
-      // the device side (scales upload, active-set tiles) is prepared on first use of the mode: direct_prepare()
-    }
-  }
   c->i8d_prepared = false;
-  c->i8_direct_used = false;
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));   // Z / beta are host temporaries of the caller
   c->gram_events_used = 0;
   c->i8_points = 0;
-  c->begun = true; c->finished = false; c->has_magic = false; c->i8_used = false;
+  c->i8_flag_mask = 0;
+  c->begun = true; c->finished = false; c->has_magic = false;
   return SGP_OK;
 }
 
@@ -556,36 +530,10 @@ int sgp_stats_accumulate(sgp_ctx* h, const void* X, int32_t x_is_f32, const doub
     chunk = ((rest + nchunks - 1) / nchunks + 63) / 64 * 64;
     if (chunk < first) chunk = first;
   }
-  if (chunk > c->stage_points || row * chunk > c->stage_bytes) {
-    SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-    SGP_CUDA(c, cudaStreamSynchronize(c->copy_stream));
-    for (int i = 0; i < 2; ++i) {
-      cudaFree(c->stageX[i]); cudaFree(c->stageY[i]);
-      c->stageX[i] = nullptr; c->stageY[i] = nullptr;
-      SGP_CUDA(c, cudaMalloc(&c->stageX[i], row * chunk));
-      SGP_CUDA(c, cudaMalloc(&c->stageY[i], static_cast<size_t>(chunk) * 8));
-      SGP_CUDA(c, cudaEventRecord(c->stage_free[i], c->stream));
-    }
-    c->stage_bytes = row * chunk; c->stage_points = chunk;
-  }
-  const char* Xb = static_cast<const char*>(X);
-  int buf = 0;
-  for (long long p0 = 0, step = first; p0 < n; p0 += step, step = chunk, buf ^= 1) {
-    const long long cn = (n - p0 < step) ? (n - p0) : step;
-    SGP_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->stage_free[buf], 0));
-    SGP_CUDA(c, cudaMemcpyAsync(c->stageX[buf], Xb + static_cast<size_t>(p0) * row, row * cn, cudaMemcpyHostToDevice,
-                                c->copy_stream));
-    SGP_CUDA(c, cudaMemcpyAsync(c->stageY[buf], y + p0, static_cast<size_t>(cn) * 8, cudaMemcpyHostToDevice,
-                                c->copy_stream));
-    SGP_CUDA(c, cudaEventRecord(c->stage_ready[buf], c->copy_stream));
-    SGP_CUDA(c, cudaStreamWaitEvent(c->stream, c->stage_ready[buf], 0));
-    int rc = launch_stats(c, c->stageX[buf], x_is_f32, c->stageY[buf], cn, n, p0 == 0);
-    if (rc != SGP_OK) return rc;
-    SGP_CUDA(c, cudaEventRecord(c->stage_free[buf], c->stream));
-  }
   // the caller may reuse / free X, y as soon as we return
-  SGP_CUDA(c, cudaStreamSynchronize(c->copy_stream));
-  return SGP_OK;
+  return stage_rows(c, X, y, n, row, first, chunk, [&](const void* dX, const double* dy, long long p0, long long cn) {
+    return launch_stats(c, dX, x_is_f32, dy, cn, n, p0 == 0);
+  });
 }
 
 int sgp_stats_finish(sgp_ctx* h, double* G_out, double* b_out) {
@@ -600,12 +548,10 @@ int sgp_stats_finish(sgp_ctx* h, double* G_out, double* b_out) {
     // WHOLE window, not just the first chunk the kernel choice looked at) rides in the last slot of the all-reduced
     // buffer: every rank sees the same sum and takes the same return decision AFTER the collective -- a rank that
     // bailed out before it would leave its peers blocked in ncclAllReduce.
-    const bool i8 = c->i8_ok && c->i8_used && c->dI8Flags;
-    const bool i8d = c->i8_direct_used && c->dI8Flags;          // direct mode: bit 2 = scaled squared norm above its limit
-    const bool budget = (i8 || i8d) && c->precision == SGP_PREC_AUTO;
-    const double zmean = (i8 && i8d) ? std::min(c->i8_z_norm_mean, c->i8d_z_norm_mean) : (i8 ? c->i8_z_norm_mean : c->i8d_z_norm_mean);
-    const double limit = (c->i8_norm_budget - zmean) * static_cast<double>(c->i8_points) * 1.25;
-    SGP_CUDA(c, launch_status_to_double(c->dGb + mm + c->m, (i8 || i8d) ? c->dI8Flags : nullptr, (i8 ? 1 : 0) | (i8d ? 4 : 0),
+    const int mask = c->i8_flag_mask;
+    const bool budget = mask != 0 && c->precision == SGP_PREC_AUTO;
+    const double limit = (kI8NormBudget - c->i8_z_norm_mean) * static_cast<double>(c->i8_points) * 1.25;
+    SGP_CUDA(c, launch_status_to_double(c->dGb + mm + c->m, mask ? c->dI8Flags : nullptr, mask,
                                         budget ? c->dI8NormSum : nullptr, limit, c->stream));
     c->launches += 1;
     if (c->comm && c->nranks > 1) {
@@ -755,31 +701,12 @@ int sgp_experts_upload_grouped(sgp_ctx* h, const void* X, int32_t x_is_f32, cons
   long long chunk = static_cast<long long>((32u << 20) / row);
   if (chunk < 65536) chunk = 65536;
   if (chunk > n) chunk = n;
-  if (chunk > c->stage_points || row * chunk > c->stage_bytes) {
-    SGP_CUDA(c, cudaStreamSynchronize(c->copy_stream));
-    for (int i = 0; i < 2; ++i) {
-      cudaFree(c->stageX[i]); cudaFree(c->stageY[i]);
-      c->stageX[i] = nullptr; c->stageY[i] = nullptr;
-      SGP_CUDA(c, cudaMalloc(&c->stageX[i], row * chunk));
-      SGP_CUDA(c, cudaMalloc(&c->stageY[i], static_cast<size_t>(chunk) * 8));
-      SGP_CUDA(c, cudaEventRecord(c->stage_free[i], c->stream));
-    }
-    c->stage_bytes = row * chunk; c->stage_points = chunk;
-  }
-  const char* Xb = static_cast<const char*>(X);
-  int buf = 0;
-  for (long long p0 = 0; p0 < n; p0 += chunk, buf ^= 1) {
-    const long long cn = (n - p0 < chunk) ? (n - p0) : chunk;
-    SGP_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->stage_free[buf], 0));
-    SGP_CUDA(c, cudaMemcpyAsync(c->stageX[buf], Xb + static_cast<size_t>(p0) * row, row * cn, cudaMemcpyHostToDevice, c->copy_stream));
-    SGP_CUDA(c, cudaMemcpyAsync(c->stageY[buf], y + p0, static_cast<size_t>(cn) * 8, cudaMemcpyHostToDevice, c->copy_stream));
-    SGP_CUDA(c, cudaEventRecord(c->stage_ready[buf], c->copy_stream));
-    SGP_CUDA(c, cudaStreamWaitEvent(c->stream, c->stage_ready[buf], 0));
-    SGP_CUDA(c, launch_group_experts(c->dEx, c->dEy, c->stageX[buf], x_is_f32, c->stageY[buf], n, d, E, p0, cn, c->stream));
-    SGP_CUDA(c, cudaEventRecord(c->stage_free[buf], c->stream));
+  const int rc = stage_rows(c, X, y, n, row, chunk, chunk, [&](const void* dX, const double* dy, long long p0, long long cn) -> int {
+    SGP_CUDA(c, launch_group_experts(c->dEx, c->dEy, dX, x_is_f32, dy, n, d, E, p0, cn, c->stream));
     c->launches += 1;
-  }
-  SGP_CUDA(c, cudaStreamSynchronize(c->copy_stream));
+    return SGP_OK;
+  });
+  if (rc != SGP_OK) return rc;
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   const long long kq = n / E;
   c->n_experts = E; c->ex_d = d; c->ex_nmax = static_cast<int>(kq + ((n % E) ? 1 : 0)); c->ex_n = n;
@@ -795,7 +722,7 @@ struct ObjectiveArgs {          // device-side view of (kernel, hyper-parameter 
   int *dKind = nullptr, *dTerm = nullptr, *dDim = nullptr, *dFlags = nullptr;
 };
 
-// Flattens the kernel (same rules as sgp_stats_begin: Eye terms only add to the diagonal), maps the hyper-parameter
+// Flattens the kernel (flatten_kernel: Eye terms only add to the diagonal), maps the hyper-parameter
 // descriptors onto the flattened terms and uploads everything into one scratch allocation.
 int objective_setup(Ctx* c, const sgp_kernel_desc* k, const sgp_hyper* hypers, int nh, ObjectiveArgs& o) {
   if (!c->dEx) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
@@ -803,26 +730,10 @@ int objective_setup(Ctx* c, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   if (nh > bcm_nll_max_hypers()) return fail(c, SGP_E_BADARG, "too many hyper-parameters");
   const int d = c->ex_d;
   KernelFlat kf;
-  std::vector<int> flat_of(k->n_terms, -1);
-  std::vector<double> beta(static_cast<size_t>(kMaxTerms) * d, 0.0);
-  for (int t = 0; t < k->n_terms; ++t) {
-    const sgp_kernel_term& term = k->terms[t];
-    if (!(term.scale >= 0.0)) return fail(c, SGP_E_BADARG, "requirement failed: C should be positive");
-    if (term.type == SGP_TERM_EYE) { kf.eye_sum += term.scale; continue; }
-    if (kf.n_terms == kMaxTerms) return fail(c, SGP_E_BADARG, "too many non-Eye kernel terms (max 4)");
-    double* bt = beta.data() + static_cast<size_t>(kf.n_terms) * d;
-    if (term.type == SGP_TERM_ARD) {
-      if (!term.beta) return fail(c, SGP_E_BADARG, "ARD term without beta");
-      for (int j = 0; j < d; ++j) bt[j] = term.beta[j];
-    } else if (term.type == SGP_TERM_RBF) {
-      if (!(term.sigma > 0.0)) return fail(c, SGP_E_BADARG, "RBF sigma must be > 0");
-      for (int j = 0; j < d; ++j) bt[j] = 1.0 / (std::sqrt(2.0) * term.sigma);
-    } else {
-      return fail(c, SGP_E_BADARG, "unknown kernel term type");
-    }
-    flat_of[t] = kf.n_terms;
-    kf.scale[kf.n_terms++] = term.scale;
-  }
+  std::vector<int> flat_of;
+  std::vector<double> beta;
+  int rc = flatten_kernel(c, k, d, d, kf, beta, &flat_of);
+  if (rc != SGP_OK) return rc;
   const int W = 1 + nh;
   std::vector<int> kind(nh), hterm(nh, 0), hdim(nh, 0);
   std::vector<double> coef(static_cast<size_t>(nh) * (kMaxTerms + 1), 0.0), value(nh, 0.0);
@@ -865,12 +776,8 @@ int objective_setup(Ctx* c, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   SGP_CUDA(c, cudaMemcpyAsync(dD, hd.data(), n_dbl * 8, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaMemcpyAsync(dI, hi.data(), n_int * 4, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));          // hd / hi are locals
-  const size_t per_bytes = static_cast<size_t>(c->n_experts) * W * 8;
-  if (per_bytes > c->nll_per_cap) {
-    cudaFree(c->dNllPer); c->dNllPer = nullptr; c->nll_per_cap = 0;
-    SGP_CUDA(c, cudaMalloc(&c->dNllPer, per_bytes));
-    c->nll_per_cap = per_bytes;
-  }
+  rc = ctx_scratch(c, c->nll_per_ws, static_cast<size_t>(c->n_experts) * W * 8);
+  if (rc != SGP_OK) return rc;
   o.kf = kf; o.W = W;
   o.dBeta = dD; o.dCoef = dD + beta.size(); o.dValue = o.dCoef + coef.size(); o.dTotal = o.dValue + value.size();
   o.dKind = dI; o.dTerm = dI + nh; o.dDim = dI + 2 * nh; o.dFlags = dI + 3 * nh;
@@ -915,7 +822,8 @@ int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   bool general = bcm_nll_smem_bytes(c->ex_nmax) > 227 * 1024;
   if (!general) {
     SGP_CUDA(c, launch_bcm_nll(c->dEx, c->dEy, c->dEoff, c->n_experts, c->ex_d, c->ex_nmax, o.kf, o.dBeta, nh, o.dKind,
-                               o.dTerm, o.dDim, o.dCoef, o.dValue, o.any_ard, c->dNllPer, o.dTotal, o.dFlags, c->stream));
+                               o.dTerm, o.dDim, o.dCoef, o.dValue, o.any_ard, c->nll_per_ws.as<double>(), o.dTotal, o.dFlags,
+                               c->stream));
     c->launches += 2;
     int flags = 0;
     SGP_CUDA(c, cudaMemcpyAsync(&flags, o.dFlags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -930,7 +838,7 @@ int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
     int blas_status = 0;
     SGP_CUDA(c, launch_bcm_nll_general(c->blas, &blas_status, c->bcm_ws.p, c->dEx, c->dEy, c->dEoff, c->n_experts, c->ex_d,
                                        c->ex_nmax, o.kf, o.dBeta, nh, o.dKind, o.dTerm, o.dDim, o.dCoef, o.dValue,
-                                       o.any_ard, c->dNllPer, o.dTotal, o.dFlags, c->stream));
+                                       o.any_ard, c->nll_per_ws.as<double>(), o.dTotal, o.dFlags, c->stream));
     if (blas_status != 0) return fail(c, SGP_E_CUDA, "cuBLAS batched LU failed, status " + std::to_string(blas_status));
     c->launches += 5;
   }
@@ -950,7 +858,8 @@ int sgp_laplace_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hyper
   if (laplace_smem_bytes(c->ex_nmax) > 227 * 1024)
     return fail(c, SGP_E_BADARG, "datasetSizeForExpert too large for the on-chip Laplace kernel (max ~115 points per expert)");
   SGP_CUDA(c, launch_laplace(c->dEx, c->dEy, c->dEf, c->dEoff, c->n_experts, c->ex_d, c->ex_nmax, o.kf, o.dBeta, nh,
-                             o.dKind, o.dTerm, o.dDim, o.dCoef, o.dValue, o.any_ard, tol, c->dNllPer, o.dTotal, o.dFlags, c->stream));
+                             o.dKind, o.dTerm, o.dDim, o.dCoef, o.dValue, o.any_ard, tol, c->nll_per_ws.as<double>(), o.dTotal,
+                             o.dFlags, c->stream));
   c->launches += 2;
   return objective_finish(c, o, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD,
                           "an expert's B = I + sqrt(W) K sqrt(W) is not positive definite (increase sigma2)");
@@ -998,12 +907,6 @@ int sgp_debug_i8_tile(sgp_ctx* h, float* T_out, uint32_t* w_out) {
   return SGP_OK;
 }
 
-int sgp_debug_i8_timeline(sgp_ctx* h, long long* out) {
-  Ctx* c = reinterpret_cast<Ctx*>(h);
-  if (!c || !out) return SGP_E_BADARG;
-  return fail(c, SGP_E_STATE, "the int8 Gram kernel of this build records no timeline");
-}
-
 int sgp_event_record(sgp_ctx* h, int slot) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
@@ -1029,24 +932,14 @@ int sgp_event_elapsed_ms(sgp_ctx* h, int a, int b, double* ms) {
 
 // One sweep launch over n device-resident points (prep of the fp16 operand images + the sweep kernel).
 static int sweep_device(Ctx* c, const void* dX, int x_is_f32, long long n, float* dK) {
-  const int nch = i8_nchunks(c->d);
-  const size_t xb = i8_points_scratch_bytes(n, nch);
-  const size_t yb = static_cast<size_t>((n + 63) / 64) * 64 * sizeof(float);
-  if (xb > c->i8_xt_bytes) {
-    SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-    cudaFree(c->dI8Xt); c->dI8Xt = nullptr; c->i8_xt_bytes = 0;
-    SGP_CUDA(c, cudaMalloc(&c->dI8Xt, xb));
-    c->i8_xt_bytes = xb;
-  }
-  if (yb > c->i8_ys_bytes) {
-    SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-    cudaFree(c->dI8Ys); c->dI8Ys = nullptr; c->i8_ys_bytes = 0;
-    SGP_CUDA(c, cudaMalloc(&c->dI8Ys, yb));
-    c->i8_ys_bytes = yb;
-  }
-  SGP_CUDA(c, launch_i8_prep_points(c->dI8Xt, c->dI8Ys, dX, x_is_f32, nullptr, n, c->d, c->dI8Scale, c->dI8Centre, c->dI8Flags,
+  int rc = ctx_scratch(c, c->i8_xt_ws, i8_points_scratch_bytes(n, i8_nchunks(c->d)));
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->i8_ys_ws, static_cast<size_t>((n + 63) / 64) * 64 * sizeof(float));
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, launch_i8_prep_points(c->i8_xt_ws.as<uint8_t>(), c->i8_ys_ws.as<float>(), dX, x_is_f32, nullptr, n, c->d,
+                                    c->dI8Scale, c->dI8Scale + static_cast<size_t>(kMaxTerms) * c->dpad, c->dI8Flags,
                                     c->dI8NormSum, nullptr, c->stream));
-  SGP_CUDA(c, launch_kmn_sweep(c->dI8Xt, c->dI8Zt, n, c->d, c->m, c->m_pad, c->num_sms, c->kf.scale[0], dK, c->stream));
+  SGP_CUDA(c, launch_kmn_sweep(c->i8_xt_ws.as<uint8_t>(), c->dI8Zt, n, c->d, c->m, c->m_pad, c->num_sms, c->kf.scale[0], dK,
+                               c->stream));
   c->launches += 2;
   return SGP_OK;
 }
@@ -1104,25 +997,9 @@ int sgp_greedy_active_set(sgp_ctx* h, const sgp_kernel_desc* k, const double* X,
   if (n > 2147483647LL) return fail(c, SGP_E_BADARG, "sgp_greedy_active_set: n too large for one device");
   SGP_CUDA(c, cudaSetDevice(c->device));
   KernelFlat kf;
-  std::vector<double> beta(static_cast<size_t>(kMaxTerms) * d, 0.0);
-  for (int t = 0; t < k->n_terms; ++t) {
-    const sgp_kernel_term& term = k->terms[t];
-    if (!(term.scale >= 0.0)) return fail(c, SGP_E_BADARG, "requirement failed: C should be positive");
-    kf.self_kernel += term.scale;
-    if (term.type == SGP_TERM_EYE) { kf.eye_sum += term.scale; continue; }
-    if (kf.n_terms == kMaxTerms) return fail(c, SGP_E_BADARG, "too many non-Eye kernel terms (max 4)");
-    double* bt = beta.data() + static_cast<size_t>(kf.n_terms) * d;
-    if (term.type == SGP_TERM_ARD) {
-      if (!term.beta) return fail(c, SGP_E_BADARG, "ARD term without beta");
-      for (int j = 0; j < d; ++j) bt[j] = term.beta[j];
-    } else if (term.type == SGP_TERM_RBF) {
-      if (!(term.sigma > 0.0)) return fail(c, SGP_E_BADARG, "RBF sigma must be > 0");
-      for (int j = 0; j < d; ++j) bt[j] = 1.0 / (std::sqrt(2.0) * term.sigma);
-    } else {
-      return fail(c, SGP_E_BADARG, "unknown kernel term type");
-    }
-    kf.scale[kf.n_terms++] = term.scale;
-  }
+  std::vector<double> beta;
+  const int rc = flatten_kernel(c, k, d, d, kf, beta, nullptr);
+  if (rc != SGP_OK) return rc;
   static_assert(sizeof(long long) == sizeof(int64_t), "index type");
   return run_greedy(c, kf, beta, X, y, n, d, n_experts, first_index, m_target, reinterpret_cast<long long*>(indices_out));
 }

@@ -301,11 +301,9 @@ cudaError_t launch_i8_prep_active(uint8_t* Zt, const double* dZ, int m, int m_pa
 cudaError_t launch_i8_prep_points(uint8_t* Xt, float* ys, const void* dX, int x_is_f32, const double* dy, long long n,
                                   int d, const double* dScale, const double* dCentre, int* dFlags, double* dNormSum,
                                   double* dNormSumCall, cudaStream_t s) {
-  const int dp = (d + 15) / 16 * 16;
   const long long units = (n + UP - 1) / UP;
   const long long threads = units * UP;
   const unsigned grid = static_cast<unsigned>((threads + 127) / 128);
-  (void)dp;
   if (d <= 16)
     prep_points_kernel<16><<<grid, 128, 128 * (1 * 128 + 16), s>>>(Xt, ys, dX, x_is_f32, dy, n, units, d, dScale, dCentre, dFlags,
                                                                   dNormSum, dNormSumCall);

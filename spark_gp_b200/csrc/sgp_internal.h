@@ -16,6 +16,12 @@ namespace sgp {
 
 // SGP_PREC_AUTO runs the int8 Gram on accumulate calls of at least this many points (smaller ones: fp64 DMMA kernel)
 constexpr long long kAutoI8MinPoints = 32768;
+// ... and only if mean|x^|^2 + mean|z^|^2 <= this budget (posterior mean vs the all-fp64 mode at 4.3 / 5.8 / 7.2 / 7.9:
+// 1.8e-6 / 2.4e-6 / 5.7e-6 / 1.0e-5, tools/i8_budget_edge.py)
+constexpr double kI8NormBudget = 6.0;
+// direct-distance mode: largest scaled squared norm accepted; measured dG 6.6e-7 at ~1300 and 2.7e-6 at ~7700 on
+// clustered data (tests: error_growth)
+constexpr float kI8DirectR2Max = 2048.f;
 constexpr int kMaxTerms = 4;      // non-Eye terms of a flattened kernel
 constexpr int kTile = 128;        // edge of one G tile (active-set indices per CTA tile)
 constexpr int kSMsH100 = 132;      // H100 SXM; the context reads the real count from the device
@@ -50,6 +56,7 @@ struct GramParams {
 struct DevScratch {
   void* p = nullptr;
   size_t cap = 0;
+  template <class T> T* as() const { return static_cast<T*>(p); }
 };
 
 struct Ctx {
@@ -80,52 +87,36 @@ struct Ctx {
   double* dZs = nullptr;     // [n_terms][m_pad][dpad]
   double* dBeta = nullptr;   // [n_terms][dpad]
   double* dGb = nullptr;     // packed [G (m*m) ; b (m)] -- one all-reduce
-  double* dGpart = nullptr;  size_t gpart_bytes = 0;
-  double* dBpart = nullptr;  size_t bpart_bytes = 0;
-  int n_slices = 1;
-  // int8 exact-accumulation path (gram_i8.cu operand preparation, gram_i8_wgmma.cu Gram kernel)
-  bool i8_ok = false;            // kernel/shape qualifies for tensor-core distances (one non-Eye term, d <= 32)
-  bool i8_direct_ok = false;     // ... for the direct-distance mode (<= 4 non-Eye terms, n_terms * (dpad4 + 4) <= 72)
-  int i8_dpad4 = 0;
-  float* dI8Zd = nullptr;        // direct mode: active-set tiles [tile][term][128][dpad4 + 4] fp32
-  double* dI8DScale = nullptr;   // [n_terms][dpad4] sqrt(log2 e) * beta_tk ; then [dpad4] centre
-  bool i8_direct_used = false;
-  bool i8_used = false;          // an int8 launch contributed to the current statistics
-  std::vector<double> i8d_sc;      // direct mode: host copy of [term][k] scales + centre of the current begin() window
-  bool i8d_prepared = false;       // ... uploaded and the active-set tiles built (on first use of the mode in the window)
-  size_t i8d_zd_bytes = 0, i8d_sc_bytes = 0;
-  double i8d_z_norm_mean = 0.0;    // direct mode: mean scaled squared norm of the active set (widest term) for AUTO's budget
-  float i8_direct_r2max = 2048.f;  // direct mode: largest scaled squared norm accepted (env SGP_I8_DIRECT_R2MAX); measured
-                                   // dG 6.6e-7 at ~1300 and 2.7e-6 at ~7700 on clustered data (tests: error_growth)
+  DevScratch gpart_ws, bpart_ws;   // per-slice partial tiles of the statistics kernels
+  // int8 exact-accumulation path (gram_i8.cu operand preparation, gram_i8_wgmma.cu Gram kernel).  Two modes:
+  // tensor-core distances (one non-Eye term, d <= 32) and direct fp32 distances (1..4 non-Eye terms, n_terms * dpad <= 72);
+  // the first qualifies only where the second does, and both use the same scales, centre and active-set norm.
+  bool i8_ok = false;            // the kernel/shape qualifies for tensor-core distances
+  bool i8_direct_ok = false;     // ... for direct distances
+  double* dI8Scale = nullptr;    // [kMaxTerms][dpad] sqrt(log2 e) * beta_tk, then [dpad] centre (active-set mean)
+  double i8_z_norm_mean = 0.0;   // mean scaled squared norm of the active set (widest term), for AUTO's budget
+  uint8_t* dI8Zt = nullptr;      // tensor-core mode: active-set operand images
+  DevScratch i8_zd_ws;           // direct mode: active-set tiles [tile][term][dpad][128] fp32
+  bool i8d_prepared = false;     // ... built in this begin() window (on the first direct-mode launch)
+  DevScratch i8_xt_ws, i8_ys_ws; // point operand images / tiles and fp32 y (scratch)
+  int* dI8Flags = nullptr;       // bit 0: coordinates out of fp16 operand range; bit 2: above kI8DirectR2Max
+  double* dI8NormSum = nullptr;  // [0]: sum of |x^|^2 over every int8 chunk since begin; [1]: first chunk of this call
   int call_path = 0;             // AUTO's decision for the current accumulate call (taken on its first chunk): 0 fp64,
                                  // 1 int8 Gram with tensor-core distances, 2 int8 Gram with direct fp32 distances
-  double* dI8Scale = nullptr;    // [dp16] sqrt(log2 e) * beta_k
-  double* dI8Centre = nullptr;   // [dp16] per-feature centre (active-set mean)
-  int* dI8Flags = nullptr;       // bit 0: coordinates out of fp16 operand range
-  double* dI8NormSum = nullptr;  // [0]: sum of |x^|^2 over every int8 chunk since begin; [1]: first chunk of this call
+  int i8_flag_mask = 0;          // dI8Flags bits the int8 launches since begin can have set (0: no int8 launch)
   long long i8_points = 0;       // points that went through the int8 kernel since begin
-  double i8_z_norm_mean = 0.0;   // mean over the active set of |z^|^2
-  double i8_norm_budget = 6.0;   // AUTO: int8 path only if mean|x^|^2 + mean|z^|^2 <= budget (posterior mean vs the all-fp64
-                                 // mode at 4.3 / 5.8 / 7.2 / 7.9: 1.8e-6 / 2.4e-6 / 5.7e-6 / 1.0e-5, tools/i8_budget_edge.py)
-  uint8_t* dI8Zt = nullptr;      // active-set operand images
-  uint8_t* dI8Xt = nullptr;  size_t i8_xt_bytes = 0;   // point operand images (scratch)
-  float* dI8Ys = nullptr;    size_t i8_ys_bytes = 0;
   // BCM objective state (experts resident on the device)
   double* dEx = nullptr; double* dEy = nullptr; long long* dEoff = nullptr;
   double* dEf = nullptr;         // per-point latent mode of the Laplace approximation (warm start across evaluations)
   long long n_experts = 0, ex_n = 0; int ex_d = 0; int ex_nmax = 0;
-  double* dNllPer = nullptr; size_t nll_per_cap = 0;
+  DevScratch nll_per_ws;         // per-expert objective rows
   bool bcm_general = false;      // the last sgp_bcm_nll took the global-memory LU path
   void* dNllScratch = nullptr;   // hyper descriptors + totals + flags
   // tail / predict state
   double* dMagicVec = nullptr;   // m
   double* dMagicMat = nullptr;   // m x m
-  size_t magic_cap = 0;
   // host->device staging (double buffered)
-  void* stageX[2] = {nullptr, nullptr};
-  double* stageY[2] = {nullptr, nullptr};
-  size_t stage_bytes = 0;       // per X buffer
-  long long stage_points = 0;
+  DevScratch stage_x[2], stage_y[2];
   cudaEvent_t stage_free[2] = {nullptr, nullptr};   // recorded when the kernel consuming buffer i is done
   cudaEvent_t stage_ready[2] = {nullptr, nullptr};  // recorded when the H2D into buffer i is done
   // instrumentation

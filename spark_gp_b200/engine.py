@@ -244,26 +244,12 @@ class ProjectedProcessEngine:
     def bcm_nll(self, kernel: Kernel):
         """(sum over experts of 1/2 y'K^-1 y + 1/2 log|K|, gradient w.r.t. kernel.getHyperparameters())."""
         desc, keep = _make_desc(kernel, self._experts_d)
-        hd = kernel.hyper_descriptors()
-        nterms = desc.n_terms
-        arr = (N.Hyper * max(len(hd), 1))()
-        coefs = []
-        for i, h in enumerate(hd):
-            arr[i].kind = h["kind"]
-            arr[i].term = h.get("term", 0)
-            arr[i].dim = h.get("dim", 0)
-            arr[i].value = h.get("value", 0.0)
-            if h["kind"] == N.SGP_HYPER_SCALE:
-                cf = np.zeros(nterms)
-                for t, v in h["coef"].items():
-                    cf[t] = v
-                coefs.append(cf)
-                arr[i].coef = cf.ctypes.data_as(C.POINTER(C.c_double))
+        arr, nh, coefs = self._hyper_array(kernel, desc.n_terms)
         nll = C.c_double()
-        grad = np.zeros(max(len(hd), 1))
-        self._check(self._lib.sgp_bcm_nll(self._h, C.byref(desc), arr, len(hd), C.byref(nll), N.ptr(grad)))
+        grad = np.zeros(max(nh, 1))
+        self._check(self._lib.sgp_bcm_nll(self._h, C.byref(desc), arr, nh, C.byref(nll), N.ptr(grad)))
         del keep, coefs
-        return nll.value, grad[:len(hd)]
+        return nll.value, grad[:nh]
 
     # ---- getMagicVector -------------------------------------------------------------------------------
     def magic(self, G=None, b=None, copy_out: bool = True):
@@ -337,12 +323,6 @@ class ProjectedProcessEngine:
         w = np.zeros((128, 64), dtype=np.uint32)
         self._check(self._lib.sgp_debug_i8_tile(self._h, N.ptr(T), N.ptr(w)))
         return T, w
-
-    def debug_i8_timeline(self):
-        out = np.zeros(2560 + 148 * 32, dtype=np.int64)
-        self._check(self._lib.sgp_debug_i8_timeline(self._h, N.ptr(out)))
-        self.i8_progress = out[2560:].reshape(148, 32)        # [CTA][unit / 128] clock64 of the Gram issuer
-        return out[:2560].reshape(2, 5, 32, 8)
 
     # ---- introspection ---------------------------------------------------------------------------------
     def last_path(self) -> int:
