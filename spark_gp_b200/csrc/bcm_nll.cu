@@ -89,10 +89,10 @@ __global__ void __launch_bounds__(EX_THREADS, 2) bcm_nll_kernel(const NllParams 
 // rank-1 update to its RB x RB block from registers; the pivots are the Schur complements (> 0 iff K is positive
 // definite, their logs sum to log|det K|), and after n sweeps the registers hold -K^-1.
 // The gradient needs no second exp(): the unscaled kernel values k_ab are parked in shared memory by the build, and with
-// M = k o W (W = alpha alpha^T - K^-1) the per-dimension sums are quadratic forms,
-//   D_k = sum_ab (x_ak - x_bk)^2 M_ab = 2 (sum_a x_ak^2 m_a - x_k^T M x_k),  m = M 1,
-// evaluated from registers (the expert's rows are translated by its first row when staged, so the expansion does not
-// cancel).
+// M = k o W (W = alpha alpha^T - K^-1) the per-dimension sums D_k = sum_ab (x_ak - x_bk)^2 M_ab are evaluated from
+// registers, term by term from the pair differences like the shared-memory sweep does.  (The expanded form
+// 2 (sum_a x_ak^2 m_a - x_k^T M x_k) is cheaper but cancels: its rounding error grows with |x_k|^2 / (x_ak - x_bk)^2, and
+// on data spread over ~3 length scales it already exceeds the rounding bound of the pair sums.)
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int REG_GY = 32, REG_THREADS = REG_GY * 16, REG_WARPS = REG_THREADS / 32;   // 32 x 16 thread grid
 template <int RBR, int RBC>      // rows / columns per thread: thread (ty, tx) owns entries (ty + 32 r, tx + 16 c)
@@ -235,7 +235,7 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
   double* out = p.out + static_cast<size_t>(e) * (1 + p.hv.n_hypers);
   if (tid == 0) out[0] = 0.5 * yay + 0.5 * logdet;
   // ---- gradient: M = k o (alpha alpha^T - K^-1) in place of A --------------------------------------------------------------
-  double S[kMaxTerms], Q[kMaxTerms], D[DCH], trW = 0.0, m[RBR];
+  double S[kMaxTerms], Q[kMaxTerms], D[DCH], trW = 0.0;
 #pragma unroll
   for (int t = 0; t < kMaxTerms; ++t) { S[t] = 0.0; Q[t] = 0.0; }
   {
@@ -246,7 +246,6 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
     for (int c = 0; c < RBC; ++c) ab[c] = alpha[tx + 16 * c];
 #pragma unroll
     for (int r = 0; r < RBR; ++r) {
-      double ms = 0.0;
 #pragma unroll
       for (int c = 0; c < RBC; ++c) {
         const int a = ty + 32 * r, b = tx + 16 * c;
@@ -254,14 +253,11 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
         if (a == b && a < n) trW += W;
         const double Mv = Ks[a * NP + b] * W;                     // 0 on the padding
         A[r][c] = Mv;
-        ms += Mv;
+        S[0] += Mv;
       }
-      S[0] += ms;
-      for (int o = 8; o > 0; o >>= 1) ms += __shfl_xor_sync(0xffffffffu, ms, o);
-      m[r] = ms;                                                  // full row sum, on all 16 threads of the row group
     }
   }
-  // quadratic forms per dimension: this thread's share of sum_a x_ak^2 m_a - sum_ab x_ak M_ab x_bk
+  // this thread's share of D_k = sum_ab (x_ak - x_bk)^2 M_ab
   auto dim_sum = [&](int k) -> double {
     double xa[RBR], xb[RBC];
 #pragma unroll
@@ -270,14 +266,13 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
     for (int c = 0; c < RBC; ++c) xb[c] = Xs[(tx + 16 * c) * xld + k];
     double acc = 0.0;
 #pragma unroll
-    for (int r = 0; r < RBR; ++r) {
-      double t = 0.0;
+    for (int r = 0; r < RBR; ++r)
 #pragma unroll
-      for (int c = 0; c < RBC; ++c) t = fma(A[r][c], xb[c], t);
-      acc = fma(-xa[r], t, acc);
-      if (tx == 0) acc = fma(xa[r] * xa[r], m[r], acc);
-    }
-    return 2.0 * acc;
+      for (int c = 0; c < RBC; ++c) {
+        const double df = xa[r] - xb[c];
+        acc = fma(df * df, A[r][c], acc);
+      }
+    return acc;
   };
   const int chunks = (d + DCH - 1) / DCH;
   const int n_sweeps = p.hv.any_ard ? chunks : 1;

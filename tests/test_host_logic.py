@@ -283,11 +283,156 @@ def test_greedy_rank1_update_identities():
         assert np.allclose(mu, cross.T @ np.linalg.solve(A, cross @ y), rtol=1e-7, atol=1e-12)
 
 
+# ---- which device kernel evaluates a per-expert objective (tests/test_gpu_objectives.py is built on this rule) -------
+# The rule lives in three places: sgp_bcm_nll (csrc/api.cu) sends experts whose shared-memory Cholesky does not fit
+# (bcm_nll_smem_bytes > 227 KB) to the global-memory LU path; launch_bcm_nll (csrc/bcm_nll.cu) runs the register kernel
+# for one non-Eye term and n_max <= 128 (template shape by 16-row blocks) unless its shared memory exceeds 227 KB, and
+# otherwise the shared-memory kernel, which stages the expert's rows when two CTAs per SM still fit (113 KB each);
+# sgp_laplace_nll (csrc/api.cu) refuses laplace_smem_bytes > 227 KB and launch_laplace (csrc/laplace.cu) stages the rows
+# when they fit beside it.  A Cholesky pivot <= 0 also sends sgp_bcm_nll to the LU path (not modelled: SPD inputs only).
+K_MAX_TERMS, DCH = 4, 16
+EX_SUMS = 2 * K_MAX_TERMS + 1 + DCH
+SMEM_MAX, SMEM_STAGE_BCM = 227 * 1024, 113 * 1024
+BCM_REG_SHAPES = ((4, (2, 4)), (6, (3, 6)), (7, (4, 7)), (8, (4, 8)))     # (16-row blocks <=, (RBR, RBC))
+MAX_HYPERS = 72
+
+
+def bcm_nll_smem_bytes(n):
+    return 8 * (n * (n + 1) + 3 * n + 8 + EX_SUMS)
+
+
+def bcm_nll_reg_smem_bytes(rbr, rbc, d):
+    nr, npad = 32 * rbr, 16 * rbc
+    return 8 * (5 * nr + 16 + EX_SUMS + nr * (d | 1) + nr * npad)
+
+
+def laplace_smem_bytes(n):
+    return 8 * (2 * n * (n + 1) + 12 * n + 8 + EX_SUMS)
+
+
+def bcm_variant(n_max, n_terms, d, force_smem=False):
+    """'reg<RBR,RBC>', 'smem-staged', 'smem-global' or 'lu': the kernel sgp_bcm_nll runs for an SPD objective.
+    force_smem: SGP_BCM_IMPL=smem (read once per process)."""
+    if bcm_nll_smem_bytes(n_max) > SMEM_MAX:
+        return "lu"
+    if n_terms == 1 and n_max <= 128 and not force_smem:
+        rb = (n_max + 15) // 16
+        rbr, rbc = next(shape for lim, shape in BCM_REG_SHAPES if rb <= lim)
+        if bcm_nll_reg_smem_bytes(rbr, rbc, d) <= SMEM_MAX:
+            return "reg<%d,%d>" % (rbr, rbc)
+    staged = bcm_nll_smem_bytes(n_max) + 8 * n_max * (d | 1) <= SMEM_STAGE_BCM
+    return "smem-staged" if staged else "smem-global"
+
+
+def laplace_variant(n_max, d):
+    """None when sgp_laplace_nll refuses the expert size, else 'staged' / 'global'."""
+    if laplace_smem_bytes(n_max) > SMEM_MAX:
+        return None
+    return "staged" if laplace_smem_bytes(n_max) + 8 * n_max * (d | 1) <= SMEM_MAX else "global"
+
+
+def test_objective_dispatch_thresholds():
+    # register kernel: one term, shape by n_max; the largest shape falls back above d = 93 (RBF: 2 hyper-parameters)
+    assert [bcm_variant(n, 1, 4) for n in (1, 64, 65, 96, 97, 112, 113, 128)] == [
+        "reg<2,4>", "reg<2,4>", "reg<3,6>", "reg<3,6>", "reg<4,7>", "reg<4,7>", "reg<4,8>", "reg<4,8>"]
+    assert bcm_variant(128, 1, 93) == "reg<4,8>" and bcm_variant(128, 1, 94) == "smem-global"
+    assert bcm_variant(128, 1, 100) == "smem-global"
+    assert bcm_variant(128, 1, 64) == "reg<4,8>"             # 64 ARD betas + scale + noise = 66 hyper-parameters
+    # shared-memory kernel: 129..168 points or >= 2 terms; staging limit 113 KB (n_max 110 / 111 at d = 16; never
+    # above 117 points)
+    assert bcm_variant(129, 1, 4) == "smem-global" and bcm_variant(168, 1, 4) == "smem-global"
+    assert max(n for n in range(1, 200) if bcm_variant(n, 2, 1) == "smem-staged") == 117
+    assert bcm_variant(104, 2, 4) == "smem-staged" and bcm_variant(100, 1, 4, force_smem=True) == "smem-staged"
+    assert bcm_variant(110, 2, 16) == "smem-staged" and bcm_variant(111, 2, 16) == "smem-global"
+    assert bcm_variant(168, 2, 1) == "smem-global"
+    # LU path from 169 points on, whatever the kernel
+    assert bcm_variant(168, 4, 20) != "lu" and bcm_variant(169, 1, 1) == "lu" and bcm_variant(406, 2, 5) == "lu"
+    assert max(n for n in range(1, 400) if bcm_nll_smem_bytes(n) <= SMEM_MAX) == 168
+    # Laplace: largest expert 117, rows not staged there; the error message's "~115" is the staged size at small d
+    assert max(n for n in range(1, 400) if laplace_variant(n, 1) is not None) == 117
+    assert laplace_variant(118, 1) is None and laplace_variant(117, 1) == "global"
+    assert laplace_variant(100, 20) == "staged" and laplace_variant(115, 1) == "staged"
+    # hyper-parameter limit: 71 ARD betas + scale fit, 72 + scale do not; d = 71 fits every register shape
+    assert 1 + 71 == MAX_HYPERS and bcm_variant(64, 1, 71) == "reg<2,4>"
+
+
+# ---- per-component error bound of the objective gradient (test_gpu_objectives.py asserts it on the GPU) --------------
+# g_i = -1/2 sum_ab dK_i[a,b] W_ab,  W = alpha alpha' - K^-1.  Rounding of the pair sums (direct form, n terms per
+# partial sum) and of K^-1 (condition number kappa) give, per expert,
+#   |dg_i| <= C_BOUND eps (n + kappa) * 1/2 sum_ab |dK_i[a,b]| (|alpha_a alpha_b| + |K^-1_ab|)
+# summed over experts.  For an ARD beta_k, dK_i = -2 beta_k scale (x_ak - x_bk)^2 k_ab.  The expanded form
+# 2 (sum_a x_ak^2 m_a - x_k' M x_k) has a rounding error of ~n eps 2|beta_k| scale sum_ab |x_ak| |M_ab| |x_bk| instead,
+# which exceeds this bound as soon as |x_k| is large against the distances that carry the kernel values.
+EPS = float(np.finfo(np.float64).eps)
+C_BOUND = 4.0
+
+
+def gradient_atol(K, dK, y):
+    """Absolute error bound of every gradient component of one expert (see above)."""
+    Kinv = np.linalg.inv(K)
+    alpha = Kinv @ y
+    absW = np.abs(np.outer(alpha, alpha)) + np.abs(Kinv)
+    scale = C_BOUND * EPS * (len(y) + np.linalg.cond(K))
+    return np.array([scale * 0.5 * float((np.abs(d) * absW).sum()) for d in dK])
+
+
+def _layout(name, n, d, rng):
+    """'standardised': N(0,1) features, beta in [0.3, 3] / sqrt(d) (what L-BFGS visits); 'clustered': unit-scale
+    structure inside clusters 300 apart, beta = 1 -- coordinates large against the distances inside a cluster."""
+    if name == "standardised":
+        return rng.standard_normal((n, d)), rng.uniform(0.3, 3.0, d) / np.sqrt(d)
+    X = rng.random((n, d)) + 300.0 * rng.integers(0, 4, (n, 1))
+    return X, np.ones(d)
+
+
+@pytest.mark.parametrize("layout", ["standardised", "clustered"])
+def test_gradient_error_bound_vs_extended_precision(layout):
+    """The per-component bound holds for the direct pair-sum gradient in fp64 against an extended-precision reference
+    (long double kernel, inverse refined by one Newton step in long double); the expanded quadratic form breaks it on
+    the clustered layout."""
+    rng = np.random.default_rng(7)
+    n, d, scale, noise = 100, 4, 1.3, 1e-2
+    X, beta = _layout(layout, n, d, rng)
+    y = rng.standard_normal(n)
+    diff = X[:, None, :] - X[None, :, :]
+    k = np.exp(-((diff * beta) ** 2).sum(2))
+    K = scale * k + noise * np.eye(n)
+    dK = [k] + [scale * (-2.0 * beta[j]) * diff[:, :, j] ** 2 * k for j in range(d)]
+    atol = gradient_atol(K, dK, y)
+    Kinv = np.linalg.inv(K)
+    W = np.outer(Kinv @ y, Kinv @ y) - Kinv
+    g = np.array([-0.5 * float((dk * W).sum()) for dk in dK])
+    # reference: everything in long double
+    L = np.longdouble
+    Xl, bl = X.astype(L), beta.astype(L)
+    dl = Xl[:, None, :] - Xl[None, :, :]
+    kl = np.exp(-((dl * bl) ** 2).sum(2))
+    Kl = L(scale) * kl + L(noise) * np.eye(n, dtype=L)
+    Xi = Kinv.astype(L)
+    Xi = Xi + Xi @ (np.eye(n, dtype=L) - Kl @ Xi)
+    al = Xi @ y.astype(L)
+    Wl = np.outer(al, al) - Xi
+    dKl = [kl] + [L(scale) * (L(-2.0) * bl[j]) * dl[:, :, j] ** 2 * kl for j in range(d)]
+    g_ref = np.array([float(L(-0.5) * (dk * Wl).sum()) for dk in dKl])
+    err = np.abs(g - g_ref)
+    assert np.all(err <= atol), (err / atol).max()
+    # the expanded form of the ARD sums (rows translated by the first row, as the register kernel's build does)
+    M = k * W
+    Xt = X - X[0]
+    g_exp = np.array([-0.5 * scale * (-2.0 * beta[j]) * 2.0 * ((Xt[:, j] ** 2) @ M.sum(1) - Xt[:, j] @ M @ Xt[:, j])
+                      for j in range(d)])
+    ratio = np.abs(g_exp - g_ref[1:]) / atol[1:]
+    print("%s: direct form max err/bound %.1e, expanded form %.1e" % (layout, (err / atol).max(), ratio.max()))
+    if layout == "clustered":
+        assert ratio.max() > 10.0
+
+
 def test_bcm_register_kernel_identities():
-    """The two identities `bcm_nll_reg_kernel` (csrc/bcm_nll.cu) rests on, in NumPy: (1) n sweeps of Goodnight's sweep
-    operator turn an SPD matrix into minus its inverse, the pivots are the Schur complements (all positive) and their logs
-    sum to log|det|; (2) the per-dimension gradient sums are quadratic forms,
-    sum_ab (x_ak - x_bk)^2 M_ab = 2 (sum_a x_ak^2 m_a - x_k' M x_k) with m = M 1, for any symmetric M."""
+    """Two identities of `bcm_nll_reg_kernel` (csrc/bcm_nll.cu), in NumPy: (1) n sweeps of Goodnight's sweep operator
+    turn an SPD matrix into minus its inverse, the pivots are the Schur complements (all positive) and their logs sum to
+    log|det|; (2) the per-dimension gradient sums equal the quadratic forms
+    sum_ab (x_ak - x_bk)^2 M_ab = 2 (sum_a x_ak^2 m_a - x_k' M x_k) with m = M 1, for any symmetric M -- in exact
+    arithmetic; the kernel sums the pair differences, because the expanded form cancels (test_gradient_error_bound_...)."""
     rng = np.random.default_rng(4)
     n, d = 37, 5
     X = rng.standard_normal((n, d))
