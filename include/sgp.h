@@ -39,8 +39,8 @@ enum {
   SGP_E_STATE = 5,    /* call order violated (e.g. accumulate before begin) ~ TrainingVectorsNotInitializedException */
   SGP_E_SINGULAR = 6, /* MatrixSingularException (commons/util/logDetAndInv.scala:27-28), LU info > 0 */
   SGP_E_NOMEM = 7,
-  SGP_E_RANGE = 8     /* int8 modes only: scaled coordinates outside the fp16 operand range / above the magnitude budget
-                         (SGP_PREC_I8), or scaled squared norms above 2048 (SGP_PREC_I8_DIRECT); rerun in SGP_PREC_F64 */
+  SGP_E_RANGE = 8     /* int8 modes only: scaled squared norms above 4096 (the tensor-core operand range) / above the
+                         magnitude budget (SGP_PREC_I8), or scaled squared norms above 2048 (SGP_PREC_I8_DIRECT); rerun in SGP_PREC_F64 */
 };
 
 /* Flattened kernel DSL (the files under commons/kernel/).  A kernel is a sum of terms  sum_t scale_t * k_t:
@@ -226,11 +226,16 @@ int sgp_cross_kernel(sgp_ctx* ctx, const double* X, int64_t n, double* K_out);
 
 /* ---- K_nm sweep (BASELINE configs[4]: the HBM-bound member of the family) ---------------------------------------
  * Materialises crossKernel(X) against the active set of the last sgp_stats_begin: K[i][j] = k(x_i, z_j), n x m row-major,
- * in FP32 (elements good to ~3e-7 relative; sgp_cross_kernel is the fp64 form).  What commons/ActiveSetProvider.scala:90-92
+ * in FP32; sgp_cross_kernel is the fp64 form.  The relative error of an element grows with the scaled squared norms
+ * s = |x^|^2 + |z^|^2 of its pair (x^ = sqrt(log2 e) beta (x - active-set mean)): measured up to 5.2e-6 at s ~ 13 (H100),
+ * bounded in the tests by 3e-7 + 24 ln2 2^-24 s.  What commons/ActiveSetProvider.scala:90-92
  * materialises and caches per expert (transposed) and commons/GaussianProcessCommons.scala:121-125 evaluates row by row.
  * Tensor-core distance contraction + exp + coalesced stores; kernels with one non-Eye term, d <= 32.
- * _device: X (fp32 / fp64) and K_out are device pointers, asynchronous on the context's stream (bench leg).
- * SGP_E_RANGE (host form) if coordinates leave the fp16 operand range. */
+ * The host form returns SGP_E_RANGE if the active set or this call's points leave the operand range (scaled squared
+ * norm above 4096).
+ * _device: X (fp32 / fp64) and K_out are device pointers.  It is asynchronous on the context's stream (synchronise with
+ * sgp_sync before reading K_out) and reports no range errors: out-of-range rows come back as garbage.
+ * Neither form changes the statistics of an open begin..finish window. */
 int sgp_kmn_sweep(sgp_ctx* ctx, const void* X, int32_t x_is_f32, int64_t n, float* K_out);
 int sgp_kmn_sweep_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n, float* dK_out);
 

@@ -455,7 +455,7 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
     SGP_CUDA(c, cudaMalloc(&c->dGb, (mm + m + 1) * 8));     // [G ; b ; status] -- one all-reduce
     SGP_CUDA(c, cudaMalloc(&c->dMagicVec, static_cast<size_t>(m) * 8));
     SGP_CUDA(c, cudaMalloc(&c->dMagicMat, mm * 8));
-    SGP_CUDA(c, cudaMalloc(&c->dI8Flags, sizeof(int)));
+    SGP_CUDA(c, cudaMalloc(&c->dI8Flags, 3 * sizeof(int)));
     SGP_CUDA(c, cudaMalloc(&c->dI8NormSum, 2 * sizeof(double)));
     SGP_CUDA(c, cudaMalloc(&c->dI8Scale, static_cast<size_t>(kMaxTerms + 1) * dpad * 8));
   }
@@ -469,7 +469,7 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
                                   c->dBeta + static_cast<size_t>(t) * dpad, m, c->m_pad, d, dpad, c->stream));
     c->launches += 1;
   }
-  SGP_CUDA(c, cudaMemsetAsync(c->dI8Flags, 0, sizeof(int), c->stream));
+  SGP_CUDA(c, cudaMemsetAsync(c->dI8Flags, 0, 3 * sizeof(int), c->stream));
   SGP_CUDA(c, cudaMemsetAsync(c->dI8NormSum, 0, 2 * sizeof(double), c->stream));
   std::vector<double> i8_sc;                       // live until the synchronisation at the end of this function
   if (c->i8_direct_ok) {
@@ -478,8 +478,10 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
   }
   if (c->i8_ok) {
     // the tensor-core operand images are built here, the direct mode's active-set tiles on its first launch
+    // the active set's range status goes to its own word; the window's status starts from it
     SGP_CUDA(c, launch_i8_prep_active(c->dI8Zt, c->dZ, m, c->m_pad, d, c->dI8Scale,
-                                      c->dI8Scale + static_cast<size_t>(kMaxTerms) * dpad, c->dI8Flags, c->stream));
+                                      c->dI8Scale + static_cast<size_t>(kMaxTerms) * dpad, c->dI8Flags + 1, c->stream));
+    SGP_CUDA(c, cudaMemcpyAsync(c->dI8Flags, c->dI8Flags + 1, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
     c->launches += 1;
   }
   c->i8d_prepared = false;
@@ -544,7 +546,7 @@ int sgp_stats_finish(sgp_ctx* h, double* G_out, double* b_out) {
   const size_t mm = static_cast<size_t>(c->m) * c->m;
   double status = 0.0;
   if (!c->finished) {
-    // The rank-local status of the int8 path (fp16 operand range overflow; AUTO's magnitude budget exceeded over the
+    // The rank-local status of the int8 path (operand range exceeded; AUTO's magnitude budget exceeded over the
     // WHOLE window, not just the first chunk the kernel choice looked at) rides in the last slot of the all-reduced
     // buffer: every rank sees the same sum and takes the same return decision AFTER the collective -- a rank that
     // bailed out before it would leave its peers blocked in ncclAllReduce.
@@ -568,8 +570,8 @@ int sgp_stats_finish(sgp_ctx* h, double* G_out, double* b_out) {
     SGP_CUDA(c, cudaMemcpyAsync(b_out, c->dGb + mm, static_cast<size_t>(c->m) * 8, cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   if (status != 0.0)
-    return fail(c, SGP_E_RANGE, "the int8 path cannot represent this shard on some rank (scaled coordinates outside the "
-                                "fp16 operand range, scaled squared norms above AUTO's magnitude budget for tensor-core "
+    return fail(c, SGP_E_RANGE, "the int8 path cannot represent this shard on some rank (scaled squared norms outside the "
+                                "tensor-core operand range, scaled squared norms above AUTO's magnitude budget for tensor-core "
                                 "distances, or above the fp32 direct-distance limit); rerun the statistics with "
                                 "sgp_set_precision(SGP_PREC_I8_DIRECT) or sgp_set_precision(SGP_PREC_F64)");
   return SGP_OK;
@@ -930,14 +932,16 @@ int sgp_event_elapsed_ms(sgp_ctx* h, int a, int b, double* ms) {
   return SGP_OK;
 }
 
-// One sweep launch over n device-resident points (prep of the fp16 operand images + the sweep kernel).
+// One sweep launch over n device-resident points (prep of the fp16 operand images + the sweep kernel).  The sweep's
+// points are not statistics points: their range bits go to the sweep's own status word (dI8Flags[2]) and their norms
+// to no budget, so a sweep inside a begin..finish window leaves the window's status alone.
 static int sweep_device(Ctx* c, const void* dX, int x_is_f32, long long n, float* dK) {
   int rc = ctx_scratch(c, c->i8_xt_ws, i8_points_scratch_bytes(n, i8_nchunks(c->d)));
   if (rc == SGP_OK) rc = ctx_scratch(c, c->i8_ys_ws, static_cast<size_t>((n + 63) / 64) * 64 * sizeof(float));
   if (rc != SGP_OK) return rc;
   SGP_CUDA(c, launch_i8_prep_points(c->i8_xt_ws.as<uint8_t>(), c->i8_ys_ws.as<float>(), dX, x_is_f32, nullptr, n, c->d,
-                                    c->dI8Scale, c->dI8Scale + static_cast<size_t>(kMaxTerms) * c->dpad, c->dI8Flags,
-                                    c->dI8NormSum, nullptr, c->stream));
+                                    c->dI8Scale, c->dI8Scale + static_cast<size_t>(kMaxTerms) * c->dpad, c->dI8Flags + 2,
+                                    nullptr, nullptr, c->stream));
   SGP_CUDA(c, launch_kmn_sweep(c->i8_xt_ws.as<uint8_t>(), c->dI8Zt, n, c->d, c->m, c->m_pad, c->num_sms, c->kf.scale[0], dK,
                                c->stream));
   c->launches += 2;
@@ -968,6 +972,8 @@ int sgp_kmn_sweep(sgp_ctx* h, const void* X, int32_t x_is_f32, int64_t n, float*
   if (rc != SGP_OK) return rc;
   float* dK = static_cast<float*>(c->sweep_ws.p);
   void* dX = dK + static_cast<size_t>(cn0) * c->m;
+  // this call's status: the active set's range bit from begin, then the bits of this call's points
+  SGP_CUDA(c, cudaMemcpyAsync(c->dI8Flags + 2, c->dI8Flags + 1, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
   for (long long p0 = 0; p0 < n; p0 += chunk) {
     const long long cn = (n - p0 < chunk) ? (n - p0) : chunk;
     SGP_CUDA(c, cudaMemcpyAsync(dX, static_cast<const char*>(X) + static_cast<size_t>(p0) * c->d * esz,
@@ -979,9 +985,10 @@ int sgp_kmn_sweep(sgp_ctx* h, const void* X, int32_t x_is_f32, int64_t n, float*
     SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   }
   int flags = 0;
-  SGP_CUDA(c, cudaMemcpy(&flags, c->dI8Flags, sizeof(int), cudaMemcpyDeviceToHost));
+  SGP_CUDA(c, cudaMemcpyAsync(&flags, c->dI8Flags + 2, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   if (flags & 1)
-    return fail(c, SGP_E_RANGE, "scaled coordinates exceed the fp16 operand range of the tensor-core distance contraction; "
+    return fail(c, SGP_E_RANGE, "scaled squared norms exceed the operand range of the tensor-core distance contraction (4096); "
                                 "use sgp_cross_kernel");
   return SGP_OK;
 }

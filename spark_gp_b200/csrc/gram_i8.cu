@@ -119,7 +119,7 @@ __global__ void prep_points_kernel(uint8_t* __restrict__ Xt, float* __restrict__
     ll[k / 2] = __halves2half2(__hadd(l0, l0), __hadd(l1, l1));
   }
   const double norm2 = acc;
-  if (valid && !(norm2 <= 16384.0)) atomicOr(flags, 1);          // out of the fp16 operand range -> caller falls back
+  if (valid && !(norm2 <= kI8TensorR2Max)) atomicOr(flags, 1);    // out of the operand range -> caller falls back
   if (norm_sum) {                                                // sum of scaled squared norms (AUTO's magnitude gate)
     double v2 = valid ? norm2 : 0.0;
     for (int o = 16; o > 0; o >>= 1) v2 += __shfl_xor_sync(0xffffffffu, v2, o);
@@ -190,7 +190,7 @@ __global__ void prep_active_kernel(uint8_t* __restrict__ Zt, const double* __res
   SplitRow s;
   double norm2;
   split_row(v, dp, s, norm2);
-  if (valid && !(norm2 <= 16384.0)) atomicOr(flags, 1);
+  if (valid && !(norm2 <= kI8TensorR2Max)) atomicOr(flags, 1);
   const int tile = j / kTile, r = j % kTile;
   for (int c = 0; c < nchunks; ++c) {
     uint8_t* img = Zt + (static_cast<size_t>(tile) * nchunks + c) * PANEL_BYTES;

@@ -22,6 +22,11 @@ constexpr double kI8NormBudget = 6.0;
 // direct-distance mode: largest scaled squared norm accepted; measured dG 6.6e-7 at ~1300 and 2.7e-6 at ~7700 on
 // clustered data (tests: error_growth)
 constexpr float kI8DirectR2Max = 2048.f;
+// tensor-core distance mode: largest scaled squared norm |x^|^2 of a point or an active point.  fp16 operands would take
+// 16384, but the fp32 contraction returns T = 2 x^.z^ - |x^|^2 - |z^|^2 up to +2.9e-3 for coinciding points at 15500
+// (+2.0e-3 at 8800, +3.7e-4 at 2200; H100, tests/test_gpu_entry_points.py), and the int8 Gram's fixed-point encoding
+// breaks from kappa = 2^T = 1 + 2.05e-3 on (the element would read back as ~0).  4096 keeps kappa < 1 + 2e-3.
+constexpr double kI8TensorR2Max = 4096.0;
 constexpr int kMaxTerms = 4;      // non-Eye terms of a flattened kernel
 constexpr int kTile = 128;        // edge of one G tile (active-set indices per CTA tile)
 constexpr int kSMsH100 = 132;      // H100 SXM; the context reads the real count from the device
@@ -99,7 +104,9 @@ struct Ctx {
   DevScratch i8_zd_ws;           // direct mode: active-set tiles [tile][term][dpad][128] fp32
   bool i8d_prepared = false;     // ... built in this begin() window (on the first direct-mode launch)
   DevScratch i8_xt_ws, i8_ys_ws; // point operand images / tiles and fp32 y (scratch)
-  int* dI8Flags = nullptr;       // bit 0: coordinates out of fp16 operand range; bit 2: above kI8DirectR2Max
+  int* dI8Flags = nullptr;       // [0] the window's int8 status, [1] the active set's (begin), [2] the K_nm sweep's
+                                 // (reset to [1] by each host-form call); bit 0: scaled squared norm above
+                                 // kI8TensorR2Max; bit 2: above kI8DirectR2Max
   double* dI8NormSum = nullptr;  // [0]: sum of |x^|^2 over every int8 chunk since begin; [1]: first chunk of this call
   int call_path = 0;             // AUTO's decision for the current accumulate call (taken on its first chunk): 0 fp64,
                                  // 1 int8 Gram with tensor-core distances, 2 int8 Gram with direct fp32 distances

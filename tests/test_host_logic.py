@@ -454,3 +454,199 @@ def test_bcm_register_kernel_identities():
     for k in range(d):
         direct = (((X[:, None, k] - X[None, :, k]) ** 2) * M).sum()
         assert abs(direct - 2.0 * ((X[:, k] ** 2) @ m1 - X[:, k] @ M @ X[:, k])) < 1e-9 * max(1.0, abs(direct))
+
+
+# ---- launch geometry of the int8 Gram (tests/test_gpu_entry_points.py picks its shapes with these mirrors) -----------
+# i8_slices transcribes csrc/gram_i8_wgmma.cu: a launch over n_units 64-point units runs nt(nt+1) CTAs per point slice
+# (two half tiles per tile of the upper block triangle) and takes the slice count <= 16 that minimises waves x units per
+# slice.  host_chunks transcribes the chunk plan of sgp_stats_accumulate (csrc/api.cu): ~16 MB of X per chunk, at least
+# 65536 points, equal chunks in multiples of 64 points, and a first chunk of a quarter of the others.  The device entry
+# (sgp_stats_accumulate_device) makes one launch over the whole shard.  Inside a slice, the kernel folds its int32
+# accumulators into the fp64 partial tile every FLUSH_UNITS units: the first fold stores, later folds add.
+UNIT_POINTS, FLUSH_UNITS, SLICES_MAX, TILE = 64, 400, 16, 128
+H100_SXM_SMS = 132
+
+
+def i8_slices(m_pad, num_sms, n_units):
+    nt = m_pad // TILE
+    ctas = nt * (nt + 1)
+    best, best_cost = 1, None
+    for s in range(1, min(SLICES_MAX, n_units) + 1):
+        cost = -(-ctas * s // num_sms) * -(-n_units // s)
+        if best_cost is None or cost < best_cost:
+            best, best_cost = s, cost
+    return best
+
+
+def host_chunks(n, d, x_is_f32):
+    """Point counts of the launches sgp_stats_accumulate makes for one call of n points."""
+    row = d * (4 if x_is_f32 else 8)
+    chunk = max((16 << 20) // row, 65536)
+    nchunks = -(-n // chunk)
+    chunk = min((-(-n // nchunks) + 63) // 64 * 64, n)
+    first = chunk
+    if n > chunk:
+        first = min(max((chunk // 4 + 63) // 64 * 64, 65536), chunk)
+        rest = n - first
+        nchunks = -(-rest // chunk)
+        chunk = max((-(-rest // nchunks) + 63) // 64 * 64, first)
+    sizes, p0, step = [], 0, first
+    while p0 < n:
+        sizes.append(min(step, n - p0))
+        p0 += step
+        step = chunk
+    return sizes
+
+
+def units_per_slice(n, m, d, x_is_f32=True, device=False, num_sms=H100_SXM_SMS):
+    """Units the first (fullest) point slice of every int8 launch of one accumulate call runs through."""
+    m_pad = -(-m // TILE) * TILE
+    out = []
+    for cn in ([n] if device else host_chunks(n, d, x_is_f32)):
+        nu = -(-cn // UNIT_POINTS)
+        out.append(-(-nu // i8_slices(m_pad, num_sms, nu)))
+    return out
+
+
+def points_for_units(m, target, num_sms, jag=0):
+    """A device-entry point count n whose fullest slice runs exactly `target` units (n = units * 64 - jag)."""
+    m_pad = -(-m // TILE) * TILE
+    for nu in range(target, SLICES_MAX * target + 1):
+        s = i8_slices(m_pad, num_sms, nu)
+        if -(-nu // s) == target:
+            return nu * UNIT_POINTS - jag
+    raise ValueError("no point count gives %d units per slice" % target)
+
+
+# (n, m, d, fp32, device entry) -> units per slice of the fullest launch, on 132 SMs
+UNITS_TABLE = [
+    ((1_000_000, 1000, 16, True, False), 332),   # test_full_size_config2_properties (AUTO, host entry)
+    ((1_600_000, 128, 8, True, False), 367),     # test_auto_budget_checked_over_whole_window
+    ((300_000, 1000, 16, True, False), 167),     # test_i8_headline_path_vs_oracle
+    ((300_000, 512, 16, True, False), 141),      # __graft_entry__.smoke
+    ((20480, 2000, 32, True, False), 20),        # test_i8_config_shapes_vs_oracle
+    ((8192, 4000, 8, True, False), 128),
+    ((120_000, 500, 8, True, False), 145),       # test_auto_routes_multi_term_kernels_to_direct_mode
+    ((1_000_000, 1000, 16, True, True), 1421),   # bench.py configs1, device entry: three folds that add
+    ((1_250_000, 2000, 32, True, True), 1221),   # bench.py configs3, device entry
+    ((399 * 64, 1300, 16, True, True), 399),     # fold boundaries: m_pad = 1408 is one slice on 132 SMs
+    ((400 * 64 - 17, 1300, 16, True, True), 400),
+    ((401 * 64, 1300, 16, True, True), 401),
+    ((800 * 64, 1300, 16, True, True), 800),
+    ((801 * 64 - 5, 1300, 16, True, True), 801),
+    ((1201 * 64, 1300, 16, True, True), 1201),
+    ((1_300_000, 1300, 2, True, False), 20313),  # d <= 2: one 1.3M-point chunk through the host entry
+    ((6400 * 64, 4, 4, True, True), 400),        # one tile, 16 slices
+    ((16 * 1201 * 64, 4, 4, True, True), 1201),
+]
+
+
+@pytest.mark.parametrize("args,want", UNITS_TABLE)
+def test_int8_units_per_slice_table(args, want):
+    assert max(units_per_slice(*args)) == want
+
+
+def test_int8_launch_geometry_rules():
+    # every int8 test that compares values before tests/test_gpu_entry_points.py stayed below the first fold that adds
+    assert max(want for (n, m, d, f32, dev), want in UNITS_TABLE[:7]) < FLUSH_UNITS
+    # m_pad in (1280, 1408]: 11 tiles, 132 CTAs per slice -- one slice on an H100 SXM, so units per slice = ceil(n / 64)
+    for m in (1281, 1300, 1408):
+        assert all(i8_slices(-(-m // TILE) * TILE, H100_SXM_SMS, nu) == 1 for nu in (1, 399, 400, 401, 5000))
+    # ... but not on a 114-SM part: the shape picker reads the SM count instead of assuming it
+    assert i8_slices(1408, 114, 4000) != 1
+    for sms in (114, 132):
+        for target in (399, 400, 401, 800, 801, 1201):
+            n = points_for_units(1300, target, sms)
+            assert units_per_slice(n, 1300, 16, device=True, num_sms=sms) == [target]
+    # host chunk plan: covers the call, multiples of 64 except the last, first chunk the smallest
+    for n, d, f32 in ((1_000_000, 16, True), (1_250_000, 32, True), (70001, 3, False), (65536, 8, True), (65537, 8, True),
+                      (10_000_000, 4, False), (1_300_000, 2, True)):
+        sizes = host_chunks(n, d, f32)
+        assert sum(sizes) == n and all(s % 64 == 0 for s in sizes[:-1]) and sizes[0] == min(sizes[:-1] or sizes)
+
+
+def test_int8_mirror_constants_match_source():
+    """The constants the mirrors and the fixed-point emulation below transcribe, read from the kernel source."""
+    import os
+    import re
+    src = open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "spark_gp_b200", "csrc",
+                            "gram_i8_wgmma.cu")).read()
+    assert re.search(r"constexpr int FLUSH_UNITS = (\d+);", src).group(1) == str(FLUSH_UNITS)
+    assert re.search(r"constexpr int UP = (\d+);", src).group(1) == str(UNIT_POINTS)
+    assert re.search(r"for \(int s = 1; s <= (\d+) && s <= n_units; \+\+s\)", src).group(1) == str(SLICES_MAX)
+    assert float(re.search(r"constexpr float C0 = ([0-9.]+)f;", src).group(1)) == float(FIXED_C0)
+    m = re.search(r"constexpr float MAGIC = ([0-9.]+)f \+ ([0-9.]+)f;", src)
+    assert float(m.group(1)) + float(m.group(2)) == float(FIXED_MAGIC)
+
+
+# ---- the fixed-point encoding of the int8 Gram (fixed_word in csrc/gram_i8_wgmma.cu), emulated exactly ----------------
+# fixed_word(kappa) = bits(fmaf(kappa, C0, MAGIC)) << 1.  kappa * C0 is exact in fp64 (24 + 23 bits); below 2^24 the fp32
+# result has ulp 1, so fmaf = MAGIC + rint(kappa * C0) (round half to even, like the FMA's single rounding); from 2^24 on
+# the ulp is 2.  The bytes of the word are (2 s0 + 128, s1 + 128, s2); the planes are P0 = 2 s0, P1 = s1 (both signed)
+# and P2 = s2 (unsigned), the base-256 digits of 2u with u = s2 2^15 + s1 2^7 + s0.
+FIXED_C0 = np.float32(8355000.0)
+FIXED_MAGIC = np.float32(8388608.0 + 16448.0)
+
+
+def fixed_word(kappa):
+    p = np.asarray(kappa, dtype=np.float32).astype(np.float64) * np.float64(FIXED_C0)
+    below = np.float64(FIXED_MAGIC) + np.rint(p)
+    above = 2.0 * np.rint((np.float64(FIXED_MAGIC) + p) / 2.0)
+    f = np.where(below < 2.0 ** 24, below, above).astype(np.float32)
+    return (f.view(np.uint32).astype(np.uint64) << np.uint64(1)) & np.uint64(0xFFFFFFFF)
+
+
+def digit_planes(word):
+    b = [((word >> np.uint64(8 * i)) & np.uint64(0xFF)).astype(np.int64) for i in range(3)]
+    return b[0] - 128, b[1] - 128, b[2]                       # P0 (x ^ 0x80 as int8), P1, P2
+
+
+def test_fixed_point_digits_exact_in_range():
+    kappa = np.unique(np.concatenate([np.linspace(0.0, 1.0 + 2e-3, 2_000_001, dtype=np.float32),
+                                      np.float32(1.0) + np.arange(-4096, 4097, dtype=np.float32) * np.float32(2 ** -23),
+                                      np.float32(2.0) ** -np.arange(0, 150, dtype=np.float32)]))
+    kappa = kappa[kappa <= np.float32(1.0 + 2e-3)]
+    P0, P1, P2 = digit_planes(fixed_word(kappa))
+    u = np.rint(kappa.astype(np.float64) * np.float64(FIXED_C0)).astype(np.int64)
+    assert np.array_equal(P2 * 2 ** 16 + P1 * 2 ** 8 + P0, 2 * u)           # u comes back exactly from the planes
+    assert np.all(P0 % 2 == 0)
+    assert P0.min() >= -128 and P0.max() <= 126                             # s0 in [-64, 63]
+    assert P1.min() >= -128 and P1.max() <= 127                             # s1 in [-128, 127]
+    assert P2.min() >= 0 and P2.max() <= 255                                # s2 in [0, 255]: the unsigned operand
+    assert P2.max() == 255 and P1.min() == -128 and P0.max() == 126          # the ranges are used to their ends
+
+
+def test_fixed_point_accumulator_bounds():
+    """Per-point products of the three int32 accumulators, and the fold interval that keeps them exact."""
+    per_fold = FLUSH_UNITS * UNIT_POINTS                                    # 25600 points between folds
+    # box bounds over the digit ranges: P2'P2, P2'P1 + P1'P2, P2'P0 + P0'P2 + P1'P1
+    b4, b3, b2 = 255 * 255, 2 * 255 * 128, 2 * 255 * 128 + 128 * 128
+    assert (b4, b3, b2) == (65025, 65280, 81664)
+    assert max(b4, b3, b2) * per_fold < 2 ** 31 - 1                         # 2.09e9: a 2.6 % margin
+    assert b2 * (per_fold + UNIT_POINTS) < 2 ** 31 - 1 < b2 * 2 * per_fold    # one more unit fits, a doubled interval not
+    # the digit patterns that reach the bounds on a diagonal element (the same kappa on both sides)
+    u_worst = 255 * 2 ** 15 - 128 * 2 ** 7 + 63                             # s2 = 255, s1 = -128, s0 = 63
+    for u, want in ((u_worst, (65025, -65280, 80644)), (int(FIXED_C0), None)):
+        kappa = np.float32(u / float(FIXED_C0))
+        P0, P1, P2 = (int(v) for v in digit_planes(fixed_word(kappa)))
+        assert P2 * 2 ** 16 + P1 * 2 ** 8 + P0 == 2 * u
+        acc = (P2 * P2, 2 * P2 * P1, 2 * P2 * P0 + P1 * P1)
+        assert all(abs(a) * per_fold < 2 ** 31 for a in acc)
+        if want:
+            assert acc == want
+
+
+def test_fixed_point_breaks_just_above_margin():
+    """u + 0x4040 must stay below 2^23: the encoding holds up to kappa = 8372160 / C0 = 1 + 2.05e-3 and breaks above --
+    an element there reads back as a different, much smaller value.  The GPU tests check that the kernel's kappa stays
+    below 1 + 2e-3 at every norm the operand gate admits (test_gpu_entry_points.py::test_kappa_margin_...)."""
+    kappa = np.float32(1.0) + np.arange(0, 40000, dtype=np.float32) * np.float32(2 ** -23)
+    P0, P1, P2 = digit_planes(fixed_word(kappa))
+    u = np.rint(kappa.astype(np.float64) * np.float64(FIXED_C0)).astype(np.int64)
+    ok = P2 * 2 ** 16 + P1 * 2 ** 8 + P0 == 2 * u
+    first_bad = kappa[np.argmin(ok)]
+    assert np.all(ok[kappa < first_bad]) and not np.any(ok[kappa >= first_bad])
+    assert 1.0 + 2e-3 < first_bad <= 1.0 + 2.06e-3
+    assert abs(float(first_bad) - 8372160.0 / float(FIXED_C0)) < 2 ** -22
+    back = (P2 * 2 ** 16 + P1 * 2 ** 8 + P0) / 2.0 / float(FIXED_C0)
+    assert np.all(back[~ok] < 0.5)                                          # silently O(1) wrong
