@@ -68,9 +68,12 @@ typedef struct {
 
 /* Arithmetic modes of the statistics kernel.  All modes accumulate G and b in fp64. */
 enum {
-  SGP_PREC_F64 = 0,        /* default: fp32-accurate kernel elements (direct-form distances, full-precision expf),
-                              fp64 DMMA Gram.  Parity-grade (<= 1e-6 on mean/variance, see DESIGN.md). */
-  SGP_PREC_F64_STRICT = 1, /* elements in fp64 as well (verification mode, ~1e-13 on G,b)               */
+  SGP_PREC_F64 = 0,        /* fp32-accurate kernel elements (direct-form distances, full-precision expf), fp64 DMMA Gram.
+                              Points and active set are centred in fp64 before the fp32 rounding (on the active-set
+                              mean, rounded to a whole multiple of its standard deviation), so the error does not grow
+                              with the data's distance from the origin: G, b <= 1e-6 and mean / variance <= 1e-5 also
+                              for data 1e3 length scales out (see DESIGN.md). */
+  SGP_PREC_F64_STRICT = 1, /* elements in fp64 as well, same centring (verification mode, ~1e-13 on G,b)   */
   SGP_PREC_I8 = 2,         /* wgmma path: distance contraction on fp16 hi/lo splits (fp32 accumulators), kernel elements
                               as 23-bit fixed point in three balanced int8 digits, Gram = six int8 products with
                               EXACT int32 accumulation, folded into fp64.  Kernels with one non-Eye term, d <= 32; other

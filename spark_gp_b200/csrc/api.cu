@@ -50,10 +50,10 @@ int fail(Ctx* c, int code, const std::string& msg) {
 }
 
 static void free_active_set(Ctx* c) {
-  cudaFree(c->dZ); cudaFree(c->dZs); cudaFree(c->dBeta); cudaFree(c->dGb);
+  cudaFree(c->dZ); cudaFree(c->dZs); cudaFree(c->dZc); cudaFree(c->dBeta); cudaFree(c->dGb);
   cudaFree(c->dMagicVec); cudaFree(c->dMagicMat);
   cudaFree(c->dI8Scale); cudaFree(c->dI8Flags); cudaFree(c->dI8Zt); cudaFree(c->dI8NormSum);
-  c->dZ = c->dZs = c->dBeta = c->dGb = c->dMagicVec = c->dMagicMat = nullptr;
+  c->dZ = c->dZs = c->dZc = c->dBeta = c->dGb = c->dMagicVec = c->dMagicMat = nullptr;
   c->dI8Scale = c->dI8NormSum = nullptr; c->dI8Flags = nullptr; c->dI8Zt = nullptr;
   c->i8_ok = c->i8_direct_ok = c->i8d_prepared = false;
 }
@@ -126,22 +126,39 @@ static int stage_rows(Ctx* c, const void* X, const double* y, long long n, size_
   return SGP_OK;
 }
 
-// Host state of both int8 modes for the active set Z (m x d) and the flattened beta ([kMaxTerms][dpad]):
-// sc = [kMaxTerms][dpad] sqrt(log2 e) * beta_tk, then the [dpad] centre (distances are translation invariant, the
-// active-set mean keeps the operands small).  Returns the mean scaled squared norm of the active set under the widest
-// term, which AUTO's magnitude budget adds to the points' mean.
-static double i8_scales(const double* Z, int m, int d, int dpad, int n_terms, const std::vector<double>& beta,
-                        std::vector<double>& sc) {
+// Host state of the statistics kernels for the active set Z (m x d) and the flattened beta ([kMaxTerms][dpad]):
+// sc = [kMaxTerms][dpad] sqrt(log2 e) * beta_tk (int8 modes only, with_scales), then the [dpad] centre of the int8 modes,
+// the active-set mean; ctr64 = [dpad] the centre of the fp64 kernel.  Distances are translation invariant, and centred
+// operands keep the rounding of the staged coordinates proportional to the spread of the data instead of to their
+// distance from the origin.  The fp64 kernel's centre is the mean rounded to a whole multiple of the active set's
+// standard deviation in that dimension (the mean itself where the deviation is 0).  It lies within half a deviation of
+// the mean, which removes any offset just as well, and it is exactly 0 for data that are centred already (standardised
+// features): those keep the arithmetic they had without a centre.  The fp32 rounding of the active set is common to all
+// the kernel values of an active point and does not average out over points; moving centred data by a fraction of a
+// deviation re-draws it for no gain in expectation (airfoil, cond(A) ~ 6e7: posterior mean 6.7e-6 -> 1.2e-5 off the
+// all-fp64 mode).
+// Returns the mean scaled squared norm of the active set under the widest term, which AUTO's magnitude budget adds to the
+// points' mean.
+static double stats_scales(const double* Z, int m, int d, int dpad, int n_terms, const std::vector<double>& beta,
+                           bool with_scales, std::vector<double>& sc, double* ctr64) {
   sc.assign(static_cast<size_t>(kMaxTerms + 1) * dpad, 0.0);
   double* ctr = sc.data() + static_cast<size_t>(kMaxTerms) * dpad;
-  const double s2 = std::sqrt(1.4426950408889634074);          // sqrt(log2 e): exponent in base 2
-  for (int t = 0; t < n_terms; ++t)
-    for (int j = 0; j < d; ++j) sc[static_cast<size_t>(t) * dpad + j] = s2 * beta[static_cast<size_t>(t) * dpad + j];
   for (int j = 0; j < d; ++j) {
     double acc = 0.0;
     for (int i = 0; i < m; ++i) acc += Z[static_cast<size_t>(i) * d + j];
     ctr[j] = acc / m;
+    double var = 0.0;
+    for (int i = 0; i < m; ++i) {
+      const double v = Z[static_cast<size_t>(i) * d + j] - ctr[j];
+      var += v * v;
+    }
+    const double sd = std::sqrt(var / m);
+    ctr64[j] = sd > 0.0 ? std::nearbyint(ctr[j] / sd) * sd : ctr[j];
   }
+  if (!with_scales) return 0.0;
+  const double s2 = std::sqrt(1.4426950408889634074);          // sqrt(log2 e): exponent in base 2
+  for (int t = 0; t < n_terms; ++t)
+    for (int j = 0; j < d; ++j) sc[static_cast<size_t>(t) * dpad + j] = s2 * beta[static_cast<size_t>(t) * dpad + j];
   double best = 1e300;
   for (int t = 0; t < n_terms; ++t) {
     const double* st = sc.data() + static_cast<size_t>(t) * dpad;
@@ -292,7 +309,7 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   p.d = c->d; p.dpad = c->dpad; p.m = c->m; p.m_pad = c->m_pad;
   p.n_terms = c->kf.n_terms;
   for (int t = 0; t < kMaxTerms; ++t) p.scale[t] = c->kf.scale[t];
-  p.Zs = c->dZs; p.beta = c->dBeta;
+  p.Zs = c->dZc; p.beta = c->dBeta;
   p.Gpart = Gpart; p.bpart = bpart;
   p.n_slices = n_slices; p.n_tiles_1d = nt1;
   SGP_CUDA(c, launch_gram_f64(p, c->precision == SGP_PREC_F64_STRICT, c->stream));
@@ -451,7 +468,8 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
     c->alloc_terms = nt;
     SGP_CUDA(c, cudaMalloc(&c->dZ, static_cast<size_t>(m) * d * 8));
     SGP_CUDA(c, cudaMalloc(&c->dZs, static_cast<size_t>(nt) * c->m_pad * dpad * 8));
-    SGP_CUDA(c, cudaMalloc(&c->dBeta, static_cast<size_t>(kMaxTerms) * dpad * 8));
+    SGP_CUDA(c, cudaMalloc(&c->dZc, static_cast<size_t>(nt) * c->m_pad * dpad * 8));
+    SGP_CUDA(c, cudaMalloc(&c->dBeta, static_cast<size_t>(kMaxTerms + 1) * dpad * 8));
     SGP_CUDA(c, cudaMalloc(&c->dGb, (mm + m + 1) * 8));     // [G ; b ; status] -- one all-reduce
     SGP_CUDA(c, cudaMalloc(&c->dMagicVec, static_cast<size_t>(m) * 8));
     SGP_CUDA(c, cudaMalloc(&c->dMagicMat, mm * 8));
@@ -462,20 +480,22 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
   if (c->i8_ok && !c->dI8Zt)          // same_shape does not tell 0 from 1 non-Eye term
     SGP_CUDA(c, cudaMalloc(&c->dI8Zt, i8_active_scratch_bytes(c->m_pad, i8_nchunks(d))));
   SGP_CUDA(c, cudaMemcpyAsync(c->dZ, Z, static_cast<size_t>(m) * d * 8, cudaMemcpyHostToDevice, c->stream));
+  std::vector<double> sc;                          // live until the synchronisation at the end of this function
+  beta.resize(static_cast<size_t>(kMaxTerms + 1) * dpad, 0.0);
+  c->i8_z_norm_mean = stats_scales(Z, m, d, dpad, kf.n_terms, beta, c->i8_direct_ok, sc,
+                                   beta.data() + static_cast<size_t>(kMaxTerms) * dpad);
   SGP_CUDA(c, cudaMemcpyAsync(c->dBeta, beta.data(), beta.size() * 8, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaMemsetAsync(c->dGb, 0, (mm + m + 1) * 8, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(c->dI8Scale, sc.data(), sc.size() * 8, cudaMemcpyHostToDevice, c->stream));
   for (int t = 0; t < kf.n_terms; ++t) {
-    SGP_CUDA(c, launch_scale_rows(c->dZs + static_cast<size_t>(t) * c->m_pad * dpad, c->dZ,
-                                  c->dBeta + static_cast<size_t>(t) * dpad, m, c->m_pad, d, dpad, c->stream));
+    const size_t off = static_cast<size_t>(t) * c->m_pad * dpad;
+    SGP_CUDA(c, launch_scale_rows(c->dZs + off, c->dZc + off, c->dZ, c->dBeta + static_cast<size_t>(t) * dpad,
+                                  c->dBeta + static_cast<size_t>(kMaxTerms) * dpad, m, c->m_pad, d, dpad,
+                                  c->stream));
     c->launches += 1;
   }
   SGP_CUDA(c, cudaMemsetAsync(c->dI8Flags, 0, 3 * sizeof(int), c->stream));
   SGP_CUDA(c, cudaMemsetAsync(c->dI8NormSum, 0, 2 * sizeof(double), c->stream));
-  std::vector<double> i8_sc;                       // live until the synchronisation at the end of this function
-  if (c->i8_direct_ok) {
-    c->i8_z_norm_mean = i8_scales(Z, m, d, dpad, kf.n_terms, beta, i8_sc);
-    SGP_CUDA(c, cudaMemcpyAsync(c->dI8Scale, i8_sc.data(), i8_sc.size() * 8, cudaMemcpyHostToDevice, c->stream));
-  }
   if (c->i8_ok) {
     // the tensor-core operand images are built here, the direct mode's active-set tiles on its first launch
     // the active set's range status goes to its own word; the window's status starts from it

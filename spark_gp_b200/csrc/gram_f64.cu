@@ -10,7 +10,8 @@
 // boundaries are irrelevant to it), so a CTA owns one 128x128 tile (I,J), I>=J, of the lower block
 // triangle of G and one contiguous slice of the shard's points.  Per block of 16 points it
 //   (1) evaluates the two panels P_I[16][128], P_J[16][128] of the cross kernel into shared memory
-//       (direct-form sum_k (x~_k - z~_k)^2 on pre-scaled coordinates x~ = x*beta, full-precision exp,
+//       (direct-form sum_k (x~_k - z~_k)^2 on centred, pre-scaled coordinates x~ = (x - c)*beta with c within half
+//       a standard deviation of the active-set mean, full-precision exp,
 //       fp32 by default / fp64 in strict mode; Eye terms contribute nothing),
 //   (2) accumulates  acc += P_I^T P_J  with fp64 tensor-core MMAs (mma.sync m8n8k4 f64), accumulators in
 //       registers for the CTA's whole lifetime, and (diagonal tiles only) b_I += P_I^T y.
@@ -131,6 +132,13 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
   constexpr double kZSign = kPacked ? -1.0 : 1.0;
   const bool z_resident = (p.n_terms == 1 && p.dpad <= DC);
 
+  // Both operands are centred on c (the row after the kMaxTerms beta rows of p.beta; within half a standard deviation of
+  // the active-set mean) in fp64 before they are rounded to ET: x~ = (x - c) beta here, z~ = (Z - c) beta once per
+  // begin() (p.Zs).  Uncentred, the rounding error of every staged coordinate would grow with |x| beta -- the distance
+  // from the origin in length scales -- instead of with the spread of the data.
+  static_assert(NT % DC == 0, "a thread stages the same feature dim of every point it stages");
+  const double* centre = p.beta + kMaxTerms * p.dpad;
+  const int kx = tid % DC;
   auto load_z_chunk = [&](int term, int c0, int clen) {
     // (threads 192..255 of a 128x64 tile have no column: their zrow may point past the padded active set)
     const bool in_range = zrow < p.m_pad;
@@ -138,16 +146,19 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
     for (int k = 0; k < clen; ++k) zs[((k >> 2) * 256 + tid) * 4 + (k & 3)] = in_range ? static_cast<ET>(kZSign * ElemOps<ET>::kPrescale * src[k]) : ET(0);
   };
   auto load_x_chunk = [&](long long pt0, int term, int c0, int clen) {
-    const double* bt = p.beta + term * p.dpad + c0;
+    const int k = kx;
+    const bool k_in = k < clen && c0 + k < p.d;
+    const double ck = k_in ? centre[c0 + k] : 0.0;
+    const double sk = k_in ? p.beta[term * p.dpad + c0 + k] * ElemOps<ET>::kPrescale : 0.0;
     for (int e = tid; e < PB * DC; e += NT) {
-      const int pp = e / DC, k = e % DC;
+      const int pp = e / DC;
       const long long pt = pt0 + pp;
       double v = 0.0;
-      if (k < clen && pt < p.n && c0 + k < p.d) {
+      if (k_in && pt < p.n) {
         const size_t off = static_cast<size_t>(pt) * p.d + c0 + k;
         v = p.x_is_f32 ? static_cast<double>(reinterpret_cast<const float*>(p.X)[off])
                        : reinterpret_cast<const double*>(p.X)[off];
-        v *= bt[k] * ElemOps<ET>::kPrescale;
+        v = (v - ck) * sk;
       }
       xs[pp * DC + k] = static_cast<ET>(v);
     }
@@ -172,17 +183,17 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
   if constexpr (kPacked) {
     if (z_resident) {
       const int nk4 = p.dpad >> 2;                               // <= 8
-      const double* bt = p.beta;
-      // this thread's two elements of a 16-point x 32-dim staging tile
+      // this thread's two elements of a 16-point x 32-dim staging tile (both in feature dim kx)
       const int e0 = tid, e1 = tid + NT;
+      const double ck = kx < p.d ? centre[kx] : 0.0, bk = kx < p.d ? p.beta[kx] : 0.0;
       auto fetch_x = [&](long long blk, int e) -> float {
-        const int pp = e / DC, k = e % DC;
+        const int pp = e / DC, k = kx;
         const long long pt = blk * PB + pp;
         if (blk < blk_hi && k < p.d && pt < p.n) {
           const size_t off = static_cast<size_t>(pt) * p.d + k;
           const double v = p.x_is_f32 ? static_cast<double>(reinterpret_cast<const float*>(p.X)[off])
                                       : reinterpret_cast<const double*>(p.X)[off];
-          return static_cast<float>(v * bt[k] * ElemOps<ET>::kPrescale);
+          return static_cast<float>((v - ck) * bk * ElemOps<ET>::kPrescale);
         }
         return 0.f;
       };

@@ -7,12 +7,17 @@ namespace sgp {
 namespace {
 
 // out[r][k] = (r < rows_in && k < d) ? in[r][k] * beta[k] : 0      (out is rows_out x dpad)
-__global__ void scale_rows_kernel(double* __restrict__ out, const double* __restrict__ in,
-                                  const double* __restrict__ beta, int rows_in, int rows_out, int d, int dpad) {
+// out_centred[r][k] (optional): the same with (in[r][k] - centre[k]) * beta[k]
+__global__ void scale_rows_kernel(double* __restrict__ out, double* __restrict__ out_centred,
+                                  const double* __restrict__ in, const double* __restrict__ beta,
+                                  const double* __restrict__ centre, int rows_in, int rows_out, int d, int dpad) {
   const size_t idx = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (idx >= static_cast<size_t>(rows_out) * dpad) return;
   const int r = static_cast<int>(idx / dpad), k = static_cast<int>(idx % dpad);
-  out[idx] = (r < rows_in && k < d) ? in[static_cast<size_t>(r) * d + k] * beta[k] : 0.0;
+  const bool in_range = r < rows_in && k < d;
+  const double v = in_range ? in[static_cast<size_t>(r) * d + k] : 0.0;
+  out[idx] = in_range ? v * beta[k] : 0.0;
+  if (out_centred) out_centred[idx] = in_range ? (v - centre[k]) * beta[k] : 0.0;
 }
 
 struct Scales { double s[kMaxTerms]; };
@@ -159,10 +164,11 @@ Scales to_scales(const KernelFlat& kf) {
 
 }  // namespace
 
-cudaError_t launch_scale_rows(double* out, const double* in, const double* beta, int rows_in, int rows_out, int d,
-                              int dpad, cudaStream_t s) {
+cudaError_t launch_scale_rows(double* out, double* out_centred, const double* in, const double* beta, const double* centre,
+                              int rows_in, int rows_out, int d, int dpad, cudaStream_t s) {
   const size_t n = static_cast<size_t>(rows_out) * dpad;
-  scale_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(out, in, beta, rows_in, rows_out, d, dpad);
+  scale_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(out, out_centred, in, beta, centre, rows_in,
+                                                                            rows_out, d, dpad);
   return cudaGetLastError();
 }
 

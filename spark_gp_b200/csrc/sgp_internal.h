@@ -49,8 +49,9 @@ struct GramParams {
   int m, m_pad;         // m_pad = m rounded up to a multiple of kTile
   int n_terms;
   double scale[kMaxTerms];
-  const double* Zs;     // [n_terms][m_pad][dpad]  beta-scaled active set (zero padded)
-  const double* beta;   // [n_terms][dpad]         per-term feature scales (zero padded)
+  const double* Zs;     // [n_terms][m_pad][dpad]  centred, beta-scaled active set (Z - centre) * beta (zero padded)
+  const double* beta;   // [kMaxTerms + 1][dpad]   per-term feature scales (zero padded), then the centre c of the
+                        //                         staged coordinates (v - c) * beta (stats_scales in api.cu)
   double* Gpart;        // [n_slices][m_pad*m_pad] per-slice partial tiles (lower block triangle)
   double* bpart;        // [n_slices][m_pad]
   int n_slices;
@@ -89,8 +90,9 @@ struct Ctx {
   int alloc_terms = 0;   // term count the active-set buffers were sized for
   KernelFlat kf;
   double* dZ = nullptr;      // m x d raw active set (fp64)
-  double* dZs = nullptr;     // [n_terms][m_pad][dpad]
-  double* dBeta = nullptr;   // [n_terms][dpad]
+  double* dZs = nullptr;     // [n_terms][m_pad][dpad]  Z * beta (K_mm, cross kernel, prediction)
+  double* dZc = nullptr;     // [n_terms][m_pad][dpad]  (Z - centre) * beta (fp64 statistics kernel)
+  double* dBeta = nullptr;   // [kMaxTerms][dpad], then [dpad] the centre of the fp64 statistics kernel
   double* dGb = nullptr;     // packed [G (m*m) ; b (m)] -- one all-reduce
   DevScratch gpart_ws, bpart_ws;   // per-slice partial tiles of the statistics kernels
   // int8 exact-accumulation path (gram_i8.cu operand preparation, gram_i8_wgmma.cu Gram kernel).  Two modes:
@@ -153,8 +155,10 @@ cudaError_t launch_gram_reduce_upper(double* G, double* b, const double* Gpart, 
 // same, restricted to the G columns / b entries [col_lo, col_hi) (one int8 launch covers whole tile columns)
 cudaError_t launch_gram_reduce_cols(double* G, double* b, const double* Gpart, const double* bpart, int n_slices, int m,
                                     int m_pad, int col_lo, int col_hi, cudaStream_t s);
-cudaError_t launch_scale_rows(double* out /*[rows][dpad]*/, const double* in /*rows x d*/, const double* beta,
-                              int rows_in, int rows_out, int d, int dpad, cudaStream_t s);
+// out = in * beta; out_centred (optional) = (in - centre) * beta; both zero padded to [rows_out][dpad]
+cudaError_t launch_scale_rows(double* out /*[rows][dpad]*/, double* out_centred, const double* in /*rows x d*/,
+                              const double* beta, const double* centre, int rows_in, int rows_out, int d, int dpad,
+                              cudaStream_t s);
 cudaError_t launch_kmm_build(double* Kmm /*m x m*/, const double* Zs, const double* scale_dev_or_null,
                              const KernelFlat& kf, int m, int m_pad, int dpad, cudaStream_t s);
 cudaError_t launch_cross_kernel(double* K /*n x m*/, const double* X /*n x d*/, const double* Zs,

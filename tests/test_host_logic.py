@@ -650,3 +650,171 @@ def test_fixed_point_breaks_just_above_margin():
     assert abs(float(first_bad) - 8372160.0 / float(FIXED_C0)) < 2 ** -22
     back = (P2 * 2 ** 16 + P1 * 2 ** 8 + P0) / 2.0 / float(FIXED_C0)
     assert np.all(back[~ok] < 0.5)                                          # silently O(1) wrong
+
+
+# ---- the fp64 DMMA statistics kernel (kmn_gram_f64_kernel, csrc/gram_f64.cu) and the int8 direct-mode gate ----------
+# launch_stats (csrc/api.cu) runs one of four loop variants of the kernel and splits the points into slices:
+#   SGP_PREC_F64 (and AUTO's fp64 path): fp32 elements on a 128 x 64 staircase of tiles (two CTAs per SM), the
+#     pipelined loop for one non-Eye term with dpad <= DC, else the generic loop (z reloaded per term and per DC-dim
+#     chunk, the terms summed into the panel);
+#   SGP_PREC_F64_STRICT: fp64 elements on the 128 x 128 triangle, z resident for one term with dpad <= DC, else chunked.
+# Slices: num_sms // (tiles of the 128 x 128 triangle), at least 1 and at most one per 16-point block; every slice
+# takes ceil(blocks / slices) blocks, so the last slices can be empty.  tests/test_gpu_gram_variants.py builds its
+# cases from these mirrors.  sgp_stats_begin admits the int8 direct-distance mode for n_terms * dpad <= 72.
+F64_PB, F64_DC, DIRECT_WIDTH = 16, 32, 72
+
+
+def dpad4(d):
+    return (d + 3) // 4 * 4
+
+
+def f64_variant(precision, n_terms, d):
+    """'pipelined' / 'generic' (fp32 elements) or 'resident' / 'chunked' (SGP_PREC_F64_STRICT) for n_terms non-Eye terms."""
+    one = n_terms == 1 and dpad4(d) <= F64_DC
+    if precision == N.SGP_PREC_F64_STRICT:
+        return "resident" if one else "chunked"
+    return "pipelined" if one else "generic"
+
+
+def f64_slices(m, n, num_sms):
+    """16-point blocks of every point slice of one fp64-kernel launch over n points (len = the slice count)."""
+    nt1 = -(-m // TILE)
+    blocks = -(-n // F64_PB)
+    slices = min(max(num_sms // (nt1 * (nt1 + 1) // 2), 1), blocks)
+    bps = -(-blocks // slices)
+    return [max(0, min(bps * (s + 1), blocks) - bps * s) for s in range(slices)]
+
+
+def direct_ok(n_terms, d):
+    return 1 <= n_terms and n_terms * dpad4(d) <= DIRECT_WIDTH
+
+
+def test_f64_mirror_constants_match_source():
+    """The constants and rules the fp64-kernel mirrors transcribe, read from the sources."""
+    import os
+    import re
+    csrc = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "spark_gp_b200", "csrc")
+    read = lambda f: open(os.path.join(csrc, f)).read()
+    gram, api, internal = read("gram_f64.cu"), read("api.cu"), read("sgp_internal.h")
+    assert re.search(r"constexpr int PB = (\d+);", gram).group(1) == str(F64_PB)
+    assert re.search(r"constexpr int DC = (\d+);", gram).group(1) == str(F64_DC)
+    assert re.search(r"constexpr int kTile = (\d+);", internal).group(1) == str(TILE)
+    assert re.search(r"i8_direct_ok = kf\.n_terms >= 1 && kf\.n_terms \* dpad <= (\d+);", api).group(1) == str(DIRECT_WIDTH)
+    assert "const bool z_resident = (p.n_terms == 1 && p.dpad <= DC);" in gram
+    assert "int n_slices = c->num_sms / ntiles;" in api and "const int ntiles = nt1 * (nt1 + 1) / 2;" in api
+    assert "const long long bps = (total_blocks + p.n_slices - 1) / p.n_slices;" in gram
+    assert "const int dpad = (d + 3) & ~3;" in api
+
+
+def test_f64_dispatch_and_slices():
+    assert [f64_variant(N.SGP_PREC_F64, 1, d) for d in (1, 32, 33)] == ["pipelined", "pipelined", "generic"]
+    assert [f64_variant(N.SGP_PREC_F64, t, 4) for t in (1, 2, 4)] == ["pipelined", "generic", "generic"]
+    assert [f64_variant(N.SGP_PREC_F64_STRICT, t, d) for t, d in ((1, 29), (1, 31), (1, 33), (2, 1))] == [
+        "resident", "resident", "chunked", "chunked"]
+    assert [direct_ok(t, d) for t, d in ((1, 72), (1, 69), (1, 73), (2, 36), (2, 33), (2, 37), (3, 24), (3, 21),
+                                         (3, 25), (4, 16), (4, 13), (4, 17), (0, 4))] == [
+        True, True, False, True, True, False, True, True, False, True, True, False, False]
+    for sms in (114, 132):
+        # m <= 128: one tile, one slice per SM
+        assert f64_slices(128, 16 * sms - 1, sms) == [1] * sms
+        assert f64_slices(1, 16 * sms + 1, sms) == [2] * (sms // 2) + [1] + [0] * (sms - sms // 2 - 1)
+        s = f64_slices(64, 16 * (sms + 1), sms)
+        assert len(s) == sms and sum(s) == sms + 1 and s.count(0) == sms - (sms + 1 + 1) // 2   # trailing slices empty
+        assert f64_slices(65, 15, sms) == [1] and f64_slices(128, 33, sms) == [1, 1, 1]
+        # m >= 2049 (on these SM counts): more tiles than SMs, one slice
+        assert -(-2049 // TILE) * (-(-2049 // TILE) + 1) // 2 > sms and f64_slices(2049, 10 ** 6, sms) == [62500]
+    for m, n, sms in ((1000, 77777, 132), (129, 5, 132), (257, 16 * 44 + 3, 132), (4000, 1, 114)):
+        s = f64_slices(m, n, sms)
+        assert sum(s) == -(-n // F64_PB) and s == sorted(s, reverse=True)
+
+
+# The CTA's tile decode (kmn_gram_f64_kernel): blockIdx.x -> (ti, tj) from an fp32 sqrtf estimate corrected by two
+# while loops; TN = 128 covers the lower block triangle tj <= ti, TN = 64 the staircase tj <= 2 ti + 1 of 64-column tiles.
+def tile_decode(t, tn):
+    f = np.float32
+    if tn == 128:
+        ti = int((np.sqrt(f(8.0) * f(t) + f(1.0)) - f(1.0)) * f(0.5))
+        est = ti
+        while (ti + 1) * (ti + 2) // 2 <= t:
+            ti += 1
+        while ti * (ti + 1) // 2 > t:
+            ti -= 1
+        return ti, t - ti * (ti + 1) // 2, ti - est
+    ti = int((np.sqrt(f(4.0) * f(t) + f(1.0)) - f(1.0)) * f(0.5))
+    est = ti
+    while (ti + 1) * (ti + 2) <= t:
+        ti += 1
+    while ti * (ti + 1) > t:
+        ti -= 1
+    return ti, t - ti * (ti + 1), ti - est
+
+
+@pytest.mark.parametrize("tn", [128, 64])
+def test_f64_tile_decode_covers_every_tile_once(tn):
+    fixes = 0
+    for nt1 in range(1, 65):
+        count = nt1 * (nt1 + 1) // 2 if tn == 128 else nt1 * (nt1 + 1)
+        tiles = [tile_decode(t, tn) for t in range(count)]
+        want = {(i, j) for i in range(nt1) for j in range(i + 1 if tn == 128 else 2 * i + 2)}
+        got = [(i, j) for i, j, _ in tiles]
+        assert len(set(got)) == len(got) == count and set(got) == want
+        fixes = max(fixes, max(abs(c) for _, _, c in tiles))
+    assert fixes <= 1                       # the fp32 estimate is off by at most one row tile up to 64 row tiles
+    if tn == 64:
+        # diagonal block: tiles 2 ti (b_I, joff 0) and 2 ti + 1 (joff 64) read the J columns from the I panel; at
+        # m = 64 / 192 the second one lies wholly past m, at m = 65 / 193 partly
+        for m in (64, 65, 192, 193):
+            ti = (m - 1) // TILE
+            lo = (2 * ti + 1) * 64
+            assert (lo >= m) == (m % TILE == 64)
+
+
+# ---- why the fp64 kernel centres its operands ------------------------------------------------------------------------
+# The fp32-element variants stage x~ = (x - c) beta sqrt(log2 e) and z~ = (Z beta - c beta) sqrt(log2 e), each rounded
+# to fp32, then form d = x~ - z~ and q = sum d^2 in fp32 and K = 2^-q.  Without the centre c, the staged coordinates
+# carry a rounding of 2^-24 |x| beta -- the distance from the origin in length scales -- into every element; centred,
+# the rounding follows the spread of the data.  f64_centre transcribes the centre of stats_scales (csrc/api.cu): the
+# active-set mean rounded to a whole multiple of the active set's standard deviation, 0 for data centred already.
+def f64_centre(Z):
+    mean = Z.sum(0) / len(Z)
+    sd = np.sqrt(((Z - mean) ** 2).sum(0) / len(Z))
+    return np.where(sd > 0, np.rint(mean / np.where(sd > 0, sd, 1.0)) * sd, mean)
+
+
+def test_f64_centre_rule():
+    rng = np.random.default_rng(5)
+    Z = rng.standard_normal((300, 6)) * [1.0, 2.0, 0.1, 5.0, 1.0, 1.0] + [0.1, -0.5, 0.0, 2.0, 1e3, -1e3]
+    Z[:, 5] = -1e3                                              # constant column: the mean itself
+    c, mean = f64_centre(Z), Z.mean(0)
+    sd = Z.std(0)
+    assert np.all(np.abs(c - mean) <= 0.5 * sd + 1e-9 * np.abs(mean))
+    assert np.all(c[:3] == 0.0) and c[5] == -1e3                # standardised columns keep the uncentred arithmetic
+    assert abs(c[4] - 1e3) <= 0.5                               # an offset of 1e3 is removed to within half a deviation
+def f32_elements(X, Z, beta, centre):
+    P = np.sqrt(np.log2(np.e))
+    xs = ((X - centre) * beta * P).astype(np.float32)
+    zs = (-(P * (Z * beta - centre * beta))).astype(np.float32)
+    q = np.zeros((len(X), len(Z)), dtype=np.float32)
+    for k in range(X.shape[1]):
+        dk = xs[:, None, k] + zs[None, :, k]
+        q += dk * dk
+    return np.exp2(-q.astype(np.float64))
+
+
+def test_f64_kernel_centring_emulated():
+    rng = np.random.default_rng(3)
+    n, d, m = 6000, 5, 200
+    beta = np.ones(d)
+    errs = {}
+    for off in (0.0, 100.0, 1000.0):
+        X = rng.random((n, d)) * 3 + off
+        Z = X[:m]
+        diff = X[:, None, :] - Z[None, :, :]
+        K0 = np.exp(-((diff * beta) ** 2).sum(-1))
+        G0 = K0.T @ K0
+        for name, c in (("uncentred", np.zeros(d)), ("centred", f64_centre(Z))):
+            K = f32_elements(X, Z, beta, c)
+            errs[(off, name)] = float(np.abs(K.T @ K - G0).max() / np.abs(G0).max())
+    print(", ".join("%g %s: dG=%.1e" % (o, nm, e) for (o, nm), e in errs.items()))
+    assert all(errs[(off, "centred")] < 1e-7 for off in (0.0, 100.0, 1000.0))
+    assert errs[(1000.0, "uncentred")] > 1e-5 and errs[(100.0, "uncentred")] > 1e-6
