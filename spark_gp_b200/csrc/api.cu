@@ -379,7 +379,7 @@ int sgp_ctx_destroy(sgp_ctx* h) {
   drop_gram_events(c);
   for (auto& e : c->user_events) if (e) cudaEventDestroy(e);
   free_active_set(c);
-  cudaFree(c->dEx); cudaFree(c->dEy); cudaFree(c->dEoff); cudaFree(c->dEf); cudaFree(c->dNllScratch);
+  cudaFree(c->ex.X); cudaFree(c->ex.y); cudaFree(c->ex.off); cudaFree(c->ex.f);
   cudaFree(c->dbgT); cudaFree(c->dbgW);
   for (int i = 0; i < 2; ++i) {
     cudaFree(c->stage_x[i].p); cudaFree(c->stage_y[i].p);
@@ -387,8 +387,8 @@ int sgp_ctx_destroy(sgp_ctx* h) {
     if (c->stage_ready[i]) cudaEventDestroy(c->stage_ready[i]);
   }
   if (c->comm && nccl().ok) nccl().CommDestroy(c->comm);
-  for (DevScratch* s : {&c->gpart_ws, &c->bpart_ws, &c->i8_zd_ws, &c->i8_xt_ws, &c->i8_ys_ws, &c->nll_per_ws, &c->greedy_ws,
-                        &c->sweep_ws, &c->bcm_ws, &c->tail_ws, &c->tail_ws2, &c->predict_ws, &c->cross_ws})
+  for (DevScratch* s : {&c->gpart_ws, &c->bpart_ws, &c->i8_zd_ws, &c->i8_xt_ws, &c->i8_ys_ws, &c->nll_per_ws, &c->hyper_ws,
+                        &c->greedy_ws, &c->sweep_ws, &c->bcm_ws, &c->tail_ws, &c->tail_ws2, &c->predict_ws, &c->cross_ws})
     cudaFree(s->p);
   if (c->tail_fork) cudaEventDestroy(c->tail_fork);
   if (c->tail_join) cudaEventDestroy(c->tail_join);
@@ -668,6 +668,23 @@ int sgp_gram_kernel_time(sgp_ctx* h, double* total_ms, int64_t* launches) {
   return SGP_OK;
 }
 
+namespace {
+// Replaces the context's experts by buffers of exactly this size, with f = zeros (GPCls:54).
+int experts_alloc(Ctx* c, long long E, long long n, int d, int n_max) {
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  ExpertSet& ex = c->ex;
+  cudaFree(ex.X); cudaFree(ex.y); cudaFree(ex.off); cudaFree(ex.f);
+  ex = ExpertSet{};
+  SGP_CUDA(c, cudaMalloc(&ex.X, static_cast<size_t>(n) * d * 8));
+  SGP_CUDA(c, cudaMalloc(&ex.y, static_cast<size_t>(n) * 8));
+  SGP_CUDA(c, cudaMalloc(&ex.off, static_cast<size_t>(E + 1) * 8));
+  SGP_CUDA(c, cudaMalloc(&ex.f, static_cast<size_t>(n) * 8));
+  SGP_CUDA(c, cudaMemsetAsync(ex.f, 0, static_cast<size_t>(n) * 8, c->stream));
+  ex.E = E; ex.n = n; ex.d = d; ex.n_max = n_max;
+  return SGP_OK;
+}
+}  // namespace
+
 int sgp_experts_upload(sgp_ctx* h, const double* X, const double* y, const int64_t* offsets, int64_t E, int32_t d) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
@@ -682,19 +699,12 @@ int sgp_experts_upload(sgp_ctx* h, const double* X, const double* y, const int64
   }
   // (no upper bound on the expert size -- GaussianProcessParams.scala:36: experts above the on-chip kernel's ~165 points
   //  take the global-memory LU path of sgp_bcm_nll)
+  const int rc = experts_alloc(c, E, n, d, nmax);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaMemcpyAsync(c->ex.X, X, static_cast<size_t>(n) * d * 8, cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(c->ex.y, y, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(c->ex.off, offsets, static_cast<size_t>(E + 1) * 8, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  cudaFree(c->dEx); cudaFree(c->dEy); cudaFree(c->dEoff); cudaFree(c->dEf);
-  c->dEx = c->dEy = c->dEf = nullptr; c->dEoff = nullptr;
-  SGP_CUDA(c, cudaMalloc(&c->dEx, static_cast<size_t>(n) * d * 8));
-  SGP_CUDA(c, cudaMalloc(&c->dEy, static_cast<size_t>(n) * 8));
-  SGP_CUDA(c, cudaMalloc(&c->dEoff, static_cast<size_t>(E + 1) * 8));
-  SGP_CUDA(c, cudaMalloc(&c->dEf, static_cast<size_t>(n) * 8));
-  SGP_CUDA(c, cudaMemsetAsync(c->dEf, 0, static_cast<size_t>(n) * 8, c->stream));   // f = zeros (GPCls:54)
-  SGP_CUDA(c, cudaMemcpyAsync(c->dEx, X, static_cast<size_t>(n) * d * 8, cudaMemcpyHostToDevice, c->stream));
-  SGP_CUDA(c, cudaMemcpyAsync(c->dEy, y, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, c->stream));
-  SGP_CUDA(c, cudaMemcpyAsync(c->dEoff, offsets, static_cast<size_t>(E + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  c->n_experts = E; c->ex_d = d; c->ex_nmax = nmax; c->ex_n = n;
   return SGP_OK;
 }
 
@@ -708,55 +718,42 @@ int sgp_experts_upload_grouped(sgp_ctx* h, const void* X, int32_t x_is_f32, cons
   // GPC:27  numberOfExperts = Math.round(points.count() / datasetSizeForExpert)  (round half up on a positive double)
   const long long E = static_cast<long long>(std::floor(static_cast<double>(n) / dataset_size_for_expert + 0.5));
   if (E <= 0) return fail(c, SGP_E_BADARG, "numberOfExperts == 0 (N < datasetSizeForExpert / 2): the reference fails with / by zero");
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  cudaFree(c->dEx); cudaFree(c->dEy); cudaFree(c->dEoff); cudaFree(c->dEf);
-  c->dEx = c->dEy = c->dEf = nullptr; c->dEoff = nullptr;
-  SGP_CUDA(c, cudaMalloc(&c->dEx, static_cast<size_t>(n) * d * 8));
-  SGP_CUDA(c, cudaMalloc(&c->dEy, static_cast<size_t>(n) * 8));
-  SGP_CUDA(c, cudaMalloc(&c->dEoff, static_cast<size_t>(E + 1) * 8));
-  SGP_CUDA(c, cudaMalloc(&c->dEf, static_cast<size_t>(n) * 8));
-  SGP_CUDA(c, cudaMemsetAsync(c->dEf, 0, static_cast<size_t>(n) * 8, c->stream));   // f = zeros (GPCls:54)
-  SGP_CUDA(c, launch_expert_offsets(c->dEoff, n, E, c->stream));
+  int rc = experts_alloc(c, E, n, d, static_cast<int>(n / E + ((n % E) ? 1 : 0)));
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, launch_expert_offsets(c->ex.off, n, E, c->stream));
   // stream the row-major input through the double-buffered staging area of the statistics path, gather on the device
   const size_t esz = x_is_f32 ? 4 : 8;
   const size_t row = static_cast<size_t>(d) * esz;
   long long chunk = static_cast<long long>((32u << 20) / row);
   if (chunk < 65536) chunk = 65536;
   if (chunk > n) chunk = n;
-  const int rc = stage_rows(c, X, y, n, row, chunk, chunk, [&](const void* dX, const double* dy, long long p0, long long cn) -> int {
-    SGP_CUDA(c, launch_group_experts(c->dEx, c->dEy, dX, x_is_f32, dy, n, d, E, p0, cn, c->stream));
+  rc = stage_rows(c, X, y, n, row, chunk, chunk, [&](const void* dX, const double* dy, long long p0, long long cn) -> int {
+    SGP_CUDA(c, launch_group_experts(c->ex.X, c->ex.y, dX, x_is_f32, dy, n, d, E, p0, cn, c->stream));
     c->launches += 1;
     return SGP_OK;
   });
   if (rc != SGP_OK) return rc;
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  const long long kq = n / E;
-  c->n_experts = E; c->ex_d = d; c->ex_nmax = static_cast<int>(kq + ((n % E) ? 1 : 0)); c->ex_n = n;
   return SGP_OK;
 }
 
 namespace {
-struct ObjectiveArgs {          // device-side view of (kernel, hyper-parameter descriptors) for the per-expert objectives
-  KernelFlat kf;
-  int W = 0;                    // 1 + n_hypers
-  int any_ard = 0;              // some hyper-parameter is an ARD beta (per-dimension sums needed)
-  double *dBeta = nullptr, *dCoef = nullptr, *dValue = nullptr, *dTotal = nullptr;
-  int *dKind = nullptr, *dTerm = nullptr, *dDim = nullptr, *dFlags = nullptr;
-};
-
-// Flattens the kernel (flatten_kernel: Eye terms only add to the diagonal), maps the hyper-parameter
-// descriptors onto the flattened terms and uploads everything into one scratch allocation.
-int objective_setup(Ctx* c, const sgp_kernel_desc* k, const sgp_hyper* hypers, int nh, ObjectiveArgs& o) {
-  if (!c->dEx) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
+// Flattens the kernel (flatten_kernel: Eye terms only add to the diagonal), maps the hyper-parameter descriptors onto
+// the flattened terms and uploads them, with zeroed totals and flags, into the context's descriptor block.
+int objective_setup(Ctx* c, const sgp_kernel_desc* k, const sgp_hyper* hypers, int nh, HyperView& hv, double*& dTotal,
+                    int*& dFlags) {
+  if (!c->ex.X) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
   if (!k || !k->terms || k->n_terms <= 0 || nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, "null argument");
-  if (nh > bcm_nll_max_hypers()) return fail(c, SGP_E_BADARG, "too many hyper-parameters");
-  const int d = c->ex_d;
+  if (nh > kMaxHypers) return fail(c, SGP_E_BADARG, "too many hyper-parameters");
+  const int d = c->ex.d;
   KernelFlat kf;
   std::vector<int> flat_of;
   std::vector<double> beta;
   int rc = flatten_kernel(c, k, d, d, kf, beta, &flat_of);
   if (rc != SGP_OK) return rc;
-  const int W = 1 + nh;
+  hv = HyperView{};
+  hv.d = d; hv.n_terms = kf.n_terms; hv.eye_sum = kf.eye_sum; hv.n_hypers = nh;
+  std::copy(kf.scale, kf.scale + kMaxTerms, hv.scale);
   std::vector<int> kind(nh), hterm(nh, 0), hdim(nh, 0);
   std::vector<double> coef(static_cast<size_t>(nh) * (kMaxTerms + 1), 0.0), value(nh, 0.0);
   for (int i = 0; i < nh; ++i) {
@@ -773,14 +770,14 @@ int objective_setup(Ctx* c, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
         return fail(c, SGP_E_BADARG, "hyper-parameter refers to a bad term");
       hterm[i] = flat_of[hypers[i].term];
       hdim[i] = hypers[i].dim;
-      if (hypers[i].kind == SGP_HYPER_ARD_BETA) o.any_ard = 1;
+      if (hypers[i].kind == SGP_HYPER_ARD_BETA) hv.any_ard = 1;
       if (hypers[i].kind == SGP_HYPER_ARD_BETA && (hdim[i] < 0 || hdim[i] >= d)) return fail(c, SGP_E_BADARG, "bad ARD dim");
     } else {
       return fail(c, SGP_E_BADARG, "unknown hyper-parameter kind");
     }
   }
-  // one scratch allocation: [beta | coef | value | total] doubles, then [kind | term | dim | flags] ints
-  const size_t n_dbl = beta.size() + coef.size() + value.size() + W + 1;    // ... + totals [W] + status [1]
+  // [beta | coef | value | totals | status] doubles, then [kind | term | dim | flags] ints
+  const size_t n_dbl = beta.size() + coef.size() + value.size() + (1 + nh) + 1;
   const size_t n_int = 3 * static_cast<size_t>(nh) + 1;
   std::vector<double> hd(n_dbl, 0.0);
   std::vector<int> hi(n_int, 0);
@@ -790,39 +787,40 @@ int objective_setup(Ctx* c, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   std::copy(kind.begin(), kind.end(), hi.begin());
   std::copy(hterm.begin(), hterm.end(), hi.begin() + nh);
   std::copy(hdim.begin(), hdim.end(), hi.begin() + 2 * nh);
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  cudaFree(c->dNllScratch); c->dNllScratch = nullptr;
-  SGP_CUDA(c, cudaMalloc(&c->dNllScratch, n_dbl * 8 + n_int * 4));
-  double* dD = static_cast<double*>(c->dNllScratch);
+  rc = ctx_scratch(c, c->hyper_ws, n_dbl * 8 + n_int * 4);
+  if (rc != SGP_OK) return rc;
+  double* dD = c->hyper_ws.as<double>();
   int* dI = reinterpret_cast<int*>(dD + n_dbl);
   SGP_CUDA(c, cudaMemcpyAsync(dD, hd.data(), n_dbl * 8, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaMemcpyAsync(dI, hi.data(), n_int * 4, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));          // hd / hi are locals
-  rc = ctx_scratch(c, c->nll_per_ws, static_cast<size_t>(c->n_experts) * W * 8);
+  rc = ctx_scratch(c, c->nll_per_ws, static_cast<size_t>(c->ex.E) * (1 + nh) * 8);
   if (rc != SGP_OK) return rc;
-  o.kf = kf; o.W = W;
-  o.dBeta = dD; o.dCoef = dD + beta.size(); o.dValue = o.dCoef + coef.size(); o.dTotal = o.dValue + value.size();
-  o.dKind = dI; o.dTerm = dI + nh; o.dDim = dI + 2 * nh; o.dFlags = dI + 3 * nh;
+  hv.beta = dD; hv.h_coef = dD + beta.size(); hv.h_value = hv.h_coef + coef.size();
+  dTotal = dD + beta.size() + coef.size() + value.size();
+  hv.h_kind = dI; hv.h_term = dI + nh; hv.h_dim = dI + 2 * nh;
+  dFlags = dI + 3 * nh;
   return SGP_OK;
 }
 
 // all-reduce over ranks, copy the (objective, gradient) row back, map a bad pivot to SGP_E_NOT_PD
-int objective_finish(Ctx* c, const ObjectiveArgs& o, double* val_out, double* grad_out, int mask, int err_code,
-                     const char* err_msg) {
+int objective_finish(Ctx* c, int nh, double* dTotal, const int* dFlags, double* val_out, double* grad_out, int mask,
+                     int err_code, const char* err_msg) {
+  const int W = 1 + nh;
   // the rank-local status flag is all-reduced WITH the totals so that every rank raises (or none does)
-  SGP_CUDA(c, launch_status_to_double(o.dTotal + o.W, o.dFlags, mask, nullptr, 0.0, c->stream));
+  SGP_CUDA(c, launch_status_to_double(dTotal + W, dFlags, mask, nullptr, 0.0, c->stream));
   c->launches += 1;
   if (c->comm && c->nranks > 1) {
-    ncclResult_t r = nccl().AllReduce(o.dTotal, o.dTotal, o.W + 1, ncclDouble, ncclSum, c->comm, c->stream);
+    ncclResult_t r = nccl().AllReduce(dTotal, dTotal, W + 1, ncclDouble, ncclSum, c->comm, c->stream);
     if (r != ncclSuccess) return fail(c, SGP_E_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
     c->launches += 1;
   }
-  std::vector<double> tot(o.W + 1);
-  SGP_CUDA(c, cudaMemcpyAsync(tot.data(), o.dTotal, static_cast<size_t>(o.W + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+  std::vector<double> tot(W + 1);
+  SGP_CUDA(c, cudaMemcpyAsync(tot.data(), dTotal, static_cast<size_t>(W + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (tot[o.W] != 0.0) return fail(c, err_code, err_msg);
+  if (tot[W] != 0.0) return fail(c, err_code, err_msg);
   *val_out = tot[0];
-  for (int i = 1; i < o.W; ++i) grad_out[i - 1] = tot[i];
+  for (int i = 1; i < W; ++i) grad_out[i - 1] = tot[i];
   return SGP_OK;
 }
 }  // namespace
@@ -833,38 +831,38 @@ int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   if (!c) return SGP_E_BADARG;
   if (!nll_out || (nh > 0 && !grad_out)) return fail(c, SGP_E_BADARG, "sgp_bcm_nll: null output");
   SGP_CUDA(c, cudaSetDevice(c->device));
-  ObjectiveArgs o;
-  int rc = objective_setup(c, k, hypers, nh, o);
+  HyperView hv;
+  double* dTotal = nullptr;
+  int* dFlags = nullptr;
+  int rc = objective_setup(c, k, hypers, nh, hv, dTotal, dFlags);
   if (rc != SGP_OK) return rc;
+  double* rows = c->nll_per_ws.as<double>();
   // fast path: on-chip Cholesky per expert (SPD kernel matrices of <= ~165 points -- every default configuration).
   // general path: experts of any size, or a kernel matrix on which Cholesky broke down (not positive definite): the
   // reference's own arithmetic, LU with partial pivoting and log|det| with the sign dropped (logDetAndInv.scala:36-63,
   // GPR:59), on kernel matrices staged in global memory.  The choice is rank-local; the one all-reduce per evaluation
   // happens afterwards on every rank.
-  bool general = bcm_nll_smem_bytes(c->ex_nmax) > 227 * 1024;
-  if (!general) {
-    SGP_CUDA(c, launch_bcm_nll(c->dEx, c->dEy, c->dEoff, c->n_experts, c->ex_d, c->ex_nmax, o.kf, o.dBeta, nh, o.dKind,
-                               o.dTerm, o.dDim, o.dCoef, o.dValue, o.any_ard, c->nll_per_ws.as<double>(), o.dTotal, o.dFlags,
-                               c->stream));
+  ObjectivePlan plan = plan_objective(Objective::kBcm, c->ex, hv.n_terms);
+  if (plan.variant != ObjectiveVariant::kLu) {
+    SGP_CUDA(c, launch_bcm_nll(plan, c->ex, hv, rows, dTotal, dFlags, c->stream));
     c->launches += 2;
     int flags = 0;
-    SGP_CUDA(c, cudaMemcpyAsync(&flags, o.dFlags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    SGP_CUDA(c, cudaMemcpyAsync(&flags, dFlags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-    general = (flags & 1) != 0;
+    if (flags & 1) plan = plan_objective(Objective::kBcmLu, c->ex, hv.n_terms);
   }
-  c->bcm_general = general;
-  if (general) {
-    rc = ctx_scratch(c, c->bcm_ws, bcm_general_workspace_bytes(c->n_experts, c->ex_nmax));
+  c->bcm_general = plan.variant == ObjectiveVariant::kLu;
+  if (c->bcm_general) {
+    rc = ctx_scratch(c, c->bcm_ws, plan.lu_ws);
     if (rc != SGP_OK) return rc;
-    SGP_CUDA(c, cudaMemsetAsync(o.dFlags, 0, sizeof(int), c->stream));
+    SGP_CUDA(c, cudaMemsetAsync(dFlags, 0, sizeof(int), c->stream));
     int blas_status = 0;
-    SGP_CUDA(c, launch_bcm_nll_general(c->blas, &blas_status, c->bcm_ws.p, c->dEx, c->dEy, c->dEoff, c->n_experts, c->ex_d,
-                                       c->ex_nmax, o.kf, o.dBeta, nh, o.dKind, o.dTerm, o.dDim, o.dCoef, o.dValue,
-                                       o.any_ard, c->nll_per_ws.as<double>(), o.dTotal, o.dFlags, c->stream));
+    SGP_CUDA(c, launch_bcm_nll_general(plan, c->blas, &blas_status, c->bcm_ws.p, c->ex, hv, rows, dTotal, dFlags,
+                                       c->stream));
     if (blas_status != 0) return fail(c, SGP_E_CUDA, "cuBLAS batched LU failed, status " + std::to_string(blas_status));
     c->launches += 5;
   }
-  return objective_finish(c, o, nll_out, grad_out, 2, SGP_E_SINGULAR,
+  return objective_finish(c, nh, dTotal, dFlags, nll_out, grad_out, 2, SGP_E_SINGULAR,
                           "an expert's kernel matrix is singular (MatrixSingularException, logDetAndInv.scala:27-28)");
 }
 
@@ -874,25 +872,26 @@ int sgp_laplace_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hyper
   if (!c) return SGP_E_BADARG;
   if (!neg_log_z_out || (nh > 0 && !grad_out) || !(tol > 0.0)) return fail(c, SGP_E_BADARG, "sgp_laplace_nll: bad argument");
   SGP_CUDA(c, cudaSetDevice(c->device));
-  ObjectiveArgs o;
-  int rc = objective_setup(c, k, hypers, nh, o);
+  HyperView hv;
+  double* dTotal = nullptr;
+  int* dFlags = nullptr;
+  int rc = objective_setup(c, k, hypers, nh, hv, dTotal, dFlags);
   if (rc != SGP_OK) return rc;
-  if (laplace_smem_bytes(c->ex_nmax) > 227 * 1024)
+  const ObjectivePlan plan = plan_objective(Objective::kLaplace, c->ex, hv.n_terms);
+  if (plan.variant == ObjectiveVariant::kRefused)
     return fail(c, SGP_E_BADARG, "datasetSizeForExpert too large for the on-chip Laplace kernel (max ~115 points per expert)");
-  SGP_CUDA(c, launch_laplace(c->dEx, c->dEy, c->dEf, c->dEoff, c->n_experts, c->ex_d, c->ex_nmax, o.kf, o.dBeta, nh,
-                             o.dKind, o.dTerm, o.dDim, o.dCoef, o.dValue, o.any_ard, tol, c->nll_per_ws.as<double>(), o.dTotal,
-                             o.dFlags, c->stream));
+  SGP_CUDA(c, launch_laplace(plan, c->ex, hv, tol, c->nll_per_ws.as<double>(), dTotal, dFlags, c->stream));
   c->launches += 2;
-  return objective_finish(c, o, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD,
+  return objective_finish(c, nh, dTotal, dFlags, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD,
                           "an expert's B = I + sqrt(W) K sqrt(W) is not positive definite (increase sigma2)");
 }
 
 int sgp_experts_get_f(sgp_ctx* h, double* f_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
-  if (!c->dEf || !f_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
+  if (!c->ex.f || !f_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
   SGP_CUDA(c, cudaSetDevice(c->device));
-  SGP_CUDA(c, cudaMemcpyAsync(f_out, c->dEf, static_cast<size_t>(c->ex_n) * 8, cudaMemcpyDeviceToHost, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(f_out, c->ex.f, static_cast<size_t>(c->ex.n) * 8, cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   return SGP_OK;
 }

@@ -22,8 +22,6 @@
 namespace sgp {
 namespace {
 
-constexpr int MAX_HYPERS = 72;      // 1 scale + 64 ARD betas + a few more
-
 struct NllParams {
   const double* X;          // packed expert-major: expert e owns rows off[e] .. off[e+1]-1 (row-major, d columns)
   const double* y;
@@ -297,11 +295,6 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
   }
 }
 
-size_t bcm_nll_reg_smem_bytes(int rbr, int rbc, int d) {
-  const size_t nr = 32 * static_cast<size_t>(rbr), np = 16 * static_cast<size_t>(rbc);
-  return sizeof(double) * (5 * nr + 16 + EX_SUMS + nr * (d | 1) + nr * np);
-}
-
 // Sum the per-expert rows: one CTA per column, thread t adds experts t, t+256, ... and the 256 partials are combined by
 // a fixed tree -- the order never depends on timing, so the result is deterministic.
 __global__ void __launch_bounds__(EX_THREADS) rows_reduce_kernel(double* __restrict__ total,
@@ -396,21 +389,92 @@ __global__ void __launch_bounds__(EX_THREADS) gen_objective_kernel(const GenPara
                          -0.5, out + 1, sums, red);                                           // GPR:63-66
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Dispatch: the shared memory of the BCM kernels and the one rule that picks the kernel of either objective.
+// ---------------------------------------------------------------------------------------------------------------------
+// bcm_nll_reg_kernel shapes for one non-Eye term, by 16-row blocks of the largest expert (up to 128 points)
+struct RegShape { int blocks, rbr, rbc; void (*kernel)(NllParams); };
+const RegShape kRegShapes[] = {{4, 2, 4, bcm_nll_reg_kernel<2, 4>}, {6, 3, 6, bcm_nll_reg_kernel<3, 6>},
+                               {7, 4, 7, bcm_nll_reg_kernel<4, 7>}, {8, 4, 8, bcm_nll_reg_kernel<4, 8>}};
+constexpr size_t kStageTwoCtas = 113 * 1024;   // bcm_nll_kernel stages the expert's rows while two CTAs fit per SM
+constexpr size_t kStageGeneral = 200 * 1024;   // gen_objective_kernel (general path) stages them up to this size
+
+size_t bcm_nll_reg_smem_bytes(int rbr, int rbc, int d) {
+  const size_t nr = 32 * static_cast<size_t>(rbr), np = 16 * static_cast<size_t>(rbc);
+  return sizeof(double) * (5 * nr + 16 + EX_SUMS + nr * (d | 1) + nr * np);
+}
+size_t gen_objective_smem_bytes(int n_max) { return sizeof(double) * (2 * static_cast<size_t>(n_max) + 8 + EX_SUMS); }
+
 }  // namespace
 
 size_t bcm_general_workspace_bytes(long long E, int n_max) {
   const size_t mat = static_cast<size_t>(E) * n_max * n_max * sizeof(double);
   return 2 * mat + static_cast<size_t>(E) * (2 * sizeof(double*) + sizeof(int) * (1 + static_cast<size_t>(n_max))) + 256;
 }
+size_t bcm_nll_smem_bytes(int n_max) {
+  return sizeof(double) * (static_cast<size_t>(n_max) * (n_max + 1) + 3 * static_cast<size_t>(n_max) + 8 + EX_SUMS);
+}
 
-// ws: bcm_general_workspace_bytes(E, n_max) bytes of device memory.  Returns cudaSuccess / a CUDA error; cuBLAS failures
-// are reported through *blas_status.
-cudaError_t launch_bcm_nll_general(cublasHandle_t blas, int* blas_status, void* ws, const double* dX, const double* dy,
-                                   const long long* dOff, long long E, int d, int n_max, const KernelFlat& kf,
-                                   const double* dBeta, int n_hypers, const int* dKind, const int* dTerm, const int* dDim,
-                                   const double* dCoef, const double* dValue, int any_ard, double* dPerExpert,
-                                   double* dTotal, int* dFlags, cudaStream_t s) {
+ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms) {
+  ObjectivePlan plan;
+  auto stage_rows = [&](ObjectiveVariant v, size_t smem, size_t limit) {
+    const size_t with_x = smem + sizeof(double) * static_cast<size_t>(ex.n_max) * (ex.d | 1);
+    plan.variant = v;
+    plan.x_in_smem = (with_x <= limit) ? 1 : 0;
+    plan.smem = plan.x_in_smem ? with_x : smem;
+    return plan;
+  };
+  if (kind == Objective::kLaplace) {
+    if (laplace_smem_bytes(ex.n_max) > kSmemOptInMax) return plan;      // kRefused
+    return stage_rows(ObjectiveVariant::kLaplace, laplace_smem_bytes(ex.n_max), kSmemOptInMax);
+  }
+  // experts whose shared-memory Cholesky does not fit, or a kernel matrix on which it broke down: the LU path
+  if (kind == Objective::kBcmLu || bcm_nll_smem_bytes(ex.n_max) > kSmemOptInMax) {
+    plan.lu_ws = bcm_general_workspace_bytes(ex.E, ex.n_max);
+    return stage_rows(ObjectiveVariant::kLu, gen_objective_smem_bytes(ex.n_max), kStageGeneral);
+  }
+  // one non-Eye term, experts of <= 128 points: the register-resident kernel (SGP_BCM_IMPL=smem selects the other one)
+  static const bool force_smem = [] { const char* e = getenv("SGP_BCM_IMPL"); return e && std::string(e) == "smem"; }();
+  if (n_terms == 1 && !force_smem) {
+    const int rb = (ex.n_max + 15) / 16;
+    for (const RegShape& r : kRegShapes) {
+      if (rb > r.blocks) continue;
+      const size_t smem = bcm_nll_reg_smem_bytes(r.rbr, r.rbc, ex.d);
+      if (smem > kSmemOptInMax) break;                 // too wide: the shared-memory kernel
+      plan.variant = static_cast<ObjectiveVariant>(&r - kRegShapes);   // kReg24 .. kReg48 in kRegShapes' order
+      plan.smem = smem;
+      return plan;
+    }
+  }
+  return stage_rows(ObjectiveVariant::kSmem, bcm_nll_smem_bytes(ex.n_max), kStageTwoCtas);
+}
+
+cudaError_t launch_rows_reduce(double* dTotal, const double* dPerExpert, long long E, int width, cudaStream_t s) {
+  rows_reduce_kernel<<<width, EX_THREADS, 0, s>>>(dTotal, dPerExpert, E, width);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double* rows, double* total,
+                           int* flags, cudaStream_t s) {
+  NllParams p{};
+  p.X = ex.X; p.y = ex.y; p.off = ex.off; p.n_max = ex.n_max; p.x_in_smem = plan.x_in_smem;
+  p.hv = hv; p.out = rows; p.flags = flags;
+  const bool reg = plan.variant < ObjectiveVariant::kSmem;
+  void (*kernel)(NllParams) = reg ? kRegShapes[static_cast<int>(plan.variant)].kernel : bcm_nll_kernel;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(plan.smem));
+  if (e != cudaSuccess) return e;
+  kernel<<<static_cast<unsigned>(ex.E), reg ? REG_THREADS : EX_THREADS, plan.smem, s>>>(p);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  return launch_rows_reduce(total, rows, ex.E, 1 + hv.n_hypers, s);
+}
+
+cudaError_t launch_bcm_nll_general(const ObjectivePlan& plan, cublasHandle_t blas, int* blas_status, void* ws,
+                                   const ExpertSet& ex, const HyperView& hv, double* rows, double* total, int* flags,
+                                   cudaStream_t s) {
   *blas_status = 0;
+  const long long E = ex.E;
+  const int n_max = ex.n_max;
   const size_t mat = static_cast<size_t>(E) * n_max * n_max;
   double* A = static_cast<double*>(ws);
   double* Ainv = A + mat;
@@ -419,9 +483,8 @@ cudaError_t launch_bcm_nll_general(cublasHandle_t blas, int* blas_status, void* 
   int* info = reinterpret_cast<int*>(Cptr + E);
   int* piv = info + E;
   GenParams p{};
-  p.X = dX; p.y = dy; p.off = dOff; p.n_max = n_max;
-  p.hv = make_hyper_view(d, kf, dBeta, n_hypers, dKind, dTerm, dDim, dCoef, dValue, any_ard);
-  p.A = A; p.Ainv = Ainv; p.info = info; p.out = dPerExpert; p.flags = dFlags;
+  p.X = ex.X; p.y = ex.y; p.off = ex.off; p.n_max = n_max; p.x_in_smem = plan.x_in_smem;
+  p.hv = hv; p.A = A; p.Ainv = Ainv; p.info = info; p.out = rows; p.flags = flags;
   gen_build_kernel<<<static_cast<unsigned>(E), EX_THREADS, 0, s>>>(p, Aptr, Cptr, Ainv);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
@@ -431,82 +494,12 @@ cudaError_t launch_bcm_nll_general(cublasHandle_t blas, int* blas_status, void* 
   if (st == CUBLAS_STATUS_SUCCESS)
     st = cublasDgetriBatched(blas, n_max, Aptr, n_max, piv, Cptr, n_max, info + 0, static_cast<int>(E));
   if (st != CUBLAS_STATUS_SUCCESS) { *blas_status = static_cast<int>(st); return cudaSuccess; }
-  size_t smem = sizeof(double) * (2 * static_cast<size_t>(n_max) + 8 + EX_SUMS);
-  const size_t with_x = smem + sizeof(double) * static_cast<size_t>(n_max) * (d | 1);
-  p.x_in_smem = (with_x <= 200 * 1024) ? 1 : 0;
-  if (p.x_in_smem) smem = with_x;
-  e = cudaFuncSetAttribute(gen_objective_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  e = cudaFuncSetAttribute(gen_objective_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(plan.smem));
   if (e != cudaSuccess) return e;
-  gen_objective_kernel<<<static_cast<unsigned>(E), EX_THREADS, smem, s>>>(p);
+  gen_objective_kernel<<<static_cast<unsigned>(E), EX_THREADS, plan.smem, s>>>(p);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  return launch_rows_reduce(dTotal, dPerExpert, E, 1 + n_hypers, s);
-}
-
-size_t bcm_nll_smem_bytes(int n_max) {
-  return sizeof(double) * (static_cast<size_t>(n_max) * (n_max + 1) + 3 * static_cast<size_t>(n_max) + 8 + EX_SUMS);
-}
-int bcm_nll_max_hypers() { return MAX_HYPERS; }
-
-cudaError_t launch_rows_reduce(double* dTotal, const double* dPerExpert, long long E, int width, cudaStream_t s) {
-  rows_reduce_kernel<<<width, EX_THREADS, 0, s>>>(dTotal, dPerExpert, E, width);
-  return cudaGetLastError();
-}
-
-HyperView make_hyper_view(int d, const KernelFlat& kf, const double* dBeta, int n_hypers, const int* dKind, const int* dTerm,
-                          const int* dDim, const double* dCoef, const double* dValue, int any_ard) {
-  HyperView hv{};
-  hv.d = d; hv.n_terms = kf.n_terms;
-  for (int t = 0; t < kMaxTerms; ++t) hv.scale[t] = kf.scale[t];
-  hv.beta = dBeta; hv.eye_sum = kf.eye_sum;
-  hv.n_hypers = n_hypers; hv.any_ard = any_ard;
-  hv.h_kind = dKind; hv.h_term = dTerm; hv.h_dim = dDim; hv.h_coef = dCoef; hv.h_value = dValue;
-  return hv;
-}
-
-cudaError_t launch_bcm_nll(const double* dX, const double* dy, const long long* dOff, long long E, int d, int n_max,
-                           const KernelFlat& kf, const double* dBeta, int n_hypers, const int* dKind, const int* dTerm,
-                           const int* dDim, const double* dCoef, const double* dValue, int any_ard,
-                           double* dPerExpert, double* dTotal, int* dFlags, cudaStream_t s) {
-  NllParams p{};
-  p.X = dX; p.y = dy; p.off = dOff; p.n_max = n_max;
-  p.hv = make_hyper_view(d, kf, dBeta, n_hypers, dKind, dTerm, dDim, dCoef, dValue, any_ard);
-  p.out = dPerExpert; p.flags = dFlags;
-  // one non-Eye term, experts of <= 128 points: the register-resident kernel (SGP_BCM_IMPL=smem selects the other one)
-  static const bool force_smem = [] { const char* e = getenv("SGP_BCM_IMPL"); return e && std::string(e) == "smem"; }();
-  if (kf.n_terms == 1 && n_max <= 128 && !force_smem) {
-    const int rb = (n_max + 15) / 16;            // 16-column blocks
-    cudaError_t e = cudaSuccess;
-    auto go = [&](auto kern, int rbr, int rbc) {
-      const size_t smem = bcm_nll_reg_smem_bytes(rbr, rbc, d);
-      if (smem > 227 * 1024) return false;
-      e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-      if (e != cudaSuccess) return true;
-      kern<<<static_cast<unsigned>(E), REG_THREADS, smem, s>>>(p);
-      e = cudaGetLastError();
-      return true;
-    };
-    bool done = false;
-    if (rb <= 4) done = go(bcm_nll_reg_kernel<2, 4>, 2, 4);
-    else if (rb <= 6) done = go(bcm_nll_reg_kernel<3, 6>, 3, 6);
-    else if (rb <= 7) done = go(bcm_nll_reg_kernel<4, 7>, 4, 7);
-    else done = go(bcm_nll_reg_kernel<4, 8>, 4, 8);
-    if (done) {
-      if (e != cudaSuccess) return e;
-      return launch_rows_reduce(dTotal, dPerExpert, E, 1 + n_hypers, s);
-    }
-  }
-  // stage the expert's rows in shared memory when two CTAs per SM still fit (113 KB each)
-  size_t smem = bcm_nll_smem_bytes(n_max);
-  const size_t with_x = smem + sizeof(double) * static_cast<size_t>(n_max) * (d | 1);
-  p.x_in_smem = (with_x <= 113 * 1024) ? 1 : 0;
-  if (p.x_in_smem) smem = with_x;
-  cudaError_t e = cudaFuncSetAttribute(bcm_nll_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-  if (e != cudaSuccess) return e;
-  bcm_nll_kernel<<<static_cast<unsigned>(E), EX_THREADS, smem, s>>>(p);
-  e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
-  return launch_rows_reduce(dTotal, dPerExpert, E, 1 + n_hypers, s);
+  return launch_rows_reduce(total, rows, E, 1 + hv.n_hypers, s);
 }
 
 }  // namespace sgp

@@ -22,23 +22,7 @@ constexpr int EX_WARPS = EX_THREADS / 32;
 constexpr int DCH = 16;                                   // ARD dimensions per sweep
 constexpr int EX_SUMS = 2 * kMaxTerms + 1 + DCH;          // doubles of shared memory the sweep needs
 
-struct HyperView {
-  int d, n_terms;
-  double scale[kMaxTerms];
-  const double* beta;        // [n_terms][d]  per-term coordinate scales (ARD betas; RBF: 1/(sqrt2 sigma))
-  double eye_sum;
-  int n_hypers, any_ard;
-  const int* h_kind;         // [n_hypers] 0 = SCALE, 1 = ARD_BETA, 2 = RBF_SIGMA
-  const int* h_term;         // [n_hypers] flattened term index (ARD_BETA / RBF_SIGMA)
-  const int* h_dim;          // [n_hypers] feature index (ARD_BETA)
-  const double* h_coef;      // [n_hypers][kMaxTerms+1]  SCALE: d(scale_t)/d(theta_i) per term, last = d(eye_sum)/d(theta_i)
-  const double* h_value;     // [n_hypers] current value of the hyper-parameter (beta_k or sigma)
-};
-
-// host side (bcm_nll.cu)
-HyperView make_hyper_view(int d, const KernelFlat& kf, const double* dBeta, int n_hypers, const int* dKind, const int* dTerm,
-                          const int* dDim, const double* dCoef, const double* dValue, int any_ard);
-// total[c] = sum_e per_expert[e][c], deterministic
+// host side (bcm_nll.cu): total[c] = sum_e per_expert[e][c], deterministic
 cudaError_t launch_rows_reduce(double* dTotal, const double* dPerExpert, long long E, int width, cudaStream_t s);
 
 template <int NW = EX_WARPS>

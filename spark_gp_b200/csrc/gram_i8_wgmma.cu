@@ -371,9 +371,8 @@ cudaError_t launch_gram_i8(const uint8_t* Xt, const float* ys, const uint8_t* Zt
   }
   p.gscale = C * C / (4.0 * static_cast<double>(C0) * static_cast<double>(C0));      // the planes are the digits of 2 u
   p.bscale = C;
-  constexpr long kSmemMax = 227L * 1024;
   const long fixed = 1024 + 2L * p.zbytes + 2L * PLANES_BYTES + 8 * (XSTAGES_MAX + 1);
-  long xs = (kSmemMax - fixed) / static_cast<long>(p.xbytes + UP * 4);
+  long xs = (static_cast<long>(kSmemOptInMax) - fixed) / static_cast<long>(p.xbytes + UP * 4);
   if (xs > XSTAGES_MAX) xs = XSTAGES_MAX;
   if (xs < 2) return cudaErrorInvalidConfiguration;
   p.xstages = static_cast<int>(xs);

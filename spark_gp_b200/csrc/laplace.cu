@@ -174,24 +174,17 @@ size_t laplace_smem_bytes(int n_max) {
   return sizeof(double) * (2 * static_cast<size_t>(n_max) * (n_max + 1) + 12 * static_cast<size_t>(n_max) + 8 + EX_SUMS);
 }
 
-cudaError_t launch_laplace(const double* dX, const double* dy, double* df, const long long* dOff, long long E, int d,
-                           int n_max, const KernelFlat& kf, const double* dBeta, int n_hypers, const int* dKind,
-                           const int* dTerm, const int* dDim, const double* dCoef, const double* dValue, int any_ard,
-                           double tol, double* dPerExpert, double* dTotal, int* dFlags, cudaStream_t s) {
+cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol, double* rows,
+                           double* total, int* flags, cudaStream_t s) {
   LapParams p{};
-  p.X = dX; p.y = dy; p.f = df; p.off = dOff; p.n_max = n_max;
-  p.hv = make_hyper_view(d, kf, dBeta, n_hypers, dKind, dTerm, dDim, dCoef, dValue, any_ard);
-  p.tol = tol; p.out = dPerExpert; p.flags = dFlags;
-  size_t smem = laplace_smem_bytes(n_max);
-  const size_t with_x = smem + sizeof(double) * static_cast<size_t>(n_max) * (d | 1);
-  p.x_in_smem = (with_x <= 227 * 1024) ? 1 : 0;
-  if (p.x_in_smem) smem = with_x;
-  cudaError_t e = cudaFuncSetAttribute(laplace_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  p.X = ex.X; p.y = ex.y; p.f = ex.f; p.off = ex.off; p.n_max = ex.n_max; p.x_in_smem = plan.x_in_smem;
+  p.hv = hv; p.tol = tol; p.out = rows; p.flags = flags;
+  cudaError_t e = cudaFuncSetAttribute(laplace_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(plan.smem));
   if (e != cudaSuccess) return e;
-  laplace_kernel<<<static_cast<unsigned>(E), LT, smem, s>>>(p);
+  laplace_kernel<<<static_cast<unsigned>(ex.E), LT, plan.smem, s>>>(p);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  return launch_rows_reduce(dTotal, dPerExpert, E, 1 + n_hypers, s);
+  return launch_rows_reduce(total, rows, ex.E, 1 + hv.n_hypers, s);
 }
 
 }  // namespace sgp

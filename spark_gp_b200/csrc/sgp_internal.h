@@ -30,6 +30,8 @@ constexpr double kI8TensorR2Max = 4096.0;
 constexpr int kMaxTerms = 4;      // non-Eye terms of a flattened kernel
 constexpr int kTile = 128;        // edge of one G tile (active-set indices per CTA tile)
 constexpr int kSMsH100 = 132;      // H100 SXM; the context reads the real count from the device
+constexpr size_t kSmemOptInMax = 227 * 1024;   // largest dynamic shared memory a CTA can opt in to (H100)
+constexpr int kMaxHypers = 72;     // hyper-parameters of one objective evaluation: 1 scale + 64 ARD betas + a few more
 
 // Flattened, device-ready kernel description (built by sgp_stats_begin).
 struct KernelFlat {
@@ -63,6 +65,16 @@ struct DevScratch {
   void* p = nullptr;
   size_t cap = 0;
   template <class T> T* as() const { return static_cast<T*>(p); }
+};
+
+// Experts resident on the device for the per-expert objectives: expert e owns rows off[e] .. off[e+1]-1.
+struct ExpertSet {
+  double* X = nullptr;        // [n][d] expert-major
+  double* y = nullptr;        // [n]
+  long long* off = nullptr;   // [E+1]
+  double* f = nullptr;        // [n] latent mode of the Laplace approximation (warm start across evaluations)
+  long long E = 0, n = 0;
+  int d = 0, n_max = 0;       // n_max: largest expert
 };
 
 struct Ctx {
@@ -114,13 +126,11 @@ struct Ctx {
                                  // 1 int8 Gram with tensor-core distances, 2 int8 Gram with direct fp32 distances
   int i8_flag_mask = 0;          // dI8Flags bits the int8 launches since begin can have set (0: no int8 launch)
   long long i8_points = 0;       // points that went through the int8 kernel since begin
-  // BCM objective state (experts resident on the device)
-  double* dEx = nullptr; double* dEy = nullptr; long long* dEoff = nullptr;
-  double* dEf = nullptr;         // per-point latent mode of the Laplace approximation (warm start across evaluations)
-  long long n_experts = 0, ex_n = 0; int ex_d = 0; int ex_nmax = 0;
+  // per-expert objective state
+  ExpertSet ex;
   DevScratch nll_per_ws;         // per-expert objective rows
+  DevScratch hyper_ws;           // hyper-parameter descriptors + totals + flags of one evaluation
   bool bcm_general = false;      // the last sgp_bcm_nll took the global-memory LU path
-  void* dNllScratch = nullptr;   // hyper descriptors + totals + flags
   // tail / predict state
   double* dMagicVec = nullptr;   // m
   double* dMagicMat = nullptr;   // m x m
@@ -210,28 +220,48 @@ cudaError_t launch_gram_i8(const uint8_t* Xt, const float* ys, const uint8_t* Zt
 cudaError_t launch_kmn_sweep(const uint8_t* Xt, const uint8_t* Zt, long long n, int d, int m, int m_pad, int num_sms, double C,
                              float* K, cudaStream_t s);
 
-// BCM objective (bcm_nll.cu)
-size_t bcm_nll_smem_bytes(int n_max);
-int bcm_nll_max_hypers();
-cudaError_t launch_bcm_nll(const double* dX, const double* dy, const long long* dOff, long long E, int d, int n_max,
-                           const KernelFlat& kf, const double* dBeta, int n_hypers, const int* dKind, const int* dTerm,
-                           const int* dDim, const double* dCoef, const double* dValue, int any_ard,
-                           double* dPerExpert, double* dTotal, int* dFlags, cudaStream_t s);
+// Per-expert objectives (bcm_nll.cu, laplace.cu) ----------------------------------------------------------------------
+// Device-side view of the flattened kernel and the hyper-parameter descriptors of one evaluation.
+struct HyperView {
+  int d, n_terms;
+  double scale[kMaxTerms];
+  const double* beta;        // [n_terms][d]  per-term coordinate scales (ARD betas; RBF: 1/(sqrt2 sigma))
+  double eye_sum;
+  int n_hypers, any_ard;
+  const int* h_kind;         // [n_hypers] 0 = SCALE, 1 = ARD_BETA, 2 = RBF_SIGMA
+  const int* h_term;         // [n_hypers] flattened term index (ARD_BETA / RBF_SIGMA)
+  const int* h_dim;          // [n_hypers] feature index (ARD_BETA)
+  const double* h_coef;      // [n_hypers][kMaxTerms+1]  SCALE: d(scale_t)/d(theta_i) per term, last = d(eye_sum)/d(theta_i)
+  const double* h_value;     // [n_hypers] current value of the hyper-parameter (beta_k or sigma)
+};
 
-// general path (any expert size, LU like the reference): global-memory kernel matrices + cuBLAS batched LU / inverse
-size_t bcm_general_workspace_bytes(long long E, int n_max);
-cudaError_t launch_bcm_nll_general(cublasHandle_t blas, int* blas_status, void* ws, const double* dX, const double* dy,
-                                   const long long* dOff, long long E, int d, int n_max, const KernelFlat& kf,
-                                   const double* dBeta, int n_hypers, const int* dKind, const int* dTerm, const int* dDim,
-                                   const double* dCoef, const double* dValue, int any_ard, double* dPerExpert,
-                                   double* dTotal, int* dFlags, cudaStream_t s);
+enum class Objective { kBcm, kBcmLu, kLaplace };   // kBcmLu: the BCM objective after its Cholesky broke down
+enum class ObjectiveVariant {
+  kReg24, kReg36, kReg47, kReg48,   // BCM: bcm_nll_reg_kernel<RBR, RBC>
+  kSmem,                            // BCM: bcm_nll_kernel (shared-memory Cholesky)
+  kLu,                              // BCM: global-memory LU path (cuBLAS batched LU / inverse)
+  kLaplace,                         // laplace_kernel
+  kRefused                          // Laplace: the expert does not fit on chip
+};
+// Which kernel evaluates an objective on the uploaded experts, with which launch resources (plan_objective, bcm_nll.cu).
+struct ObjectivePlan {
+  ObjectiveVariant variant = ObjectiveVariant::kRefused;
+  int x_in_smem = 0;   // the kernel stages the expert's rows in shared memory
+  size_t smem = 0;     // dynamic shared memory per CTA
+  size_t lu_ws = 0;    // kLu: global-memory workspace
+};
+ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms);
+size_t laplace_smem_bytes(int n_max);   // laplace_kernel without the staged rows (laplace.cu)
 
-size_t laplace_smem_bytes(int n_max);
-cudaError_t launch_laplace(const double* dX, const double* dy, double* df, const long long* dOff, long long E, int d,
-                           int n_max, const KernelFlat& kf, const double* dBeta, int n_hypers, const int* dKind,
-                           const int* dTerm, const int* dDim, const double* dCoef, const double* dValue, int any_ard,
-                           double tol,
-                           double* dPerExpert, double* dTotal, int* dFlags, cudaStream_t s);
+// Each launcher runs the planned kernel and sums the per-expert rows [E][1 + n_hypers] into total.
+cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double* rows, double* total,
+                           int* flags, cudaStream_t s);
+// ws: plan.lu_ws bytes.  cuBLAS failures are reported through *blas_status.
+cudaError_t launch_bcm_nll_general(const ObjectivePlan& plan, cublasHandle_t blas, int* blas_status, void* ws,
+                                   const ExpertSet& ex, const HyperView& hv, double* rows, double* total, int* flags,
+                                   cudaStream_t s);
+cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol, double* rows,
+                           double* total, int* flags, cudaStream_t s);
 
 int ctx_scratch(Ctx* c, DevScratch& s, size_t bytes);
 // csrc/greedy.cu: forward selection with rank-1 updates (ActiveSetProvider.scala:58-139); beta_flat = [n_terms][d]

@@ -208,7 +208,10 @@ class ProjectedProcessEngine:
         self._experts_d = X.shape[1]
         return int(np.floor(len(X) / dataset_size_for_expert + 0.5))
 
-    def _hyper_array(self, kernel: Kernel, nterms: int):
+    def _objective(self, fn, kernel: Kernel, *args):
+        """Runs one per-expert objective of the library over the uploaded experts: (value, gradient w.r.t.
+        kernel.getHyperparameters())."""
+        desc, keep = _make_desc(kernel, self._experts_d)
         hd = kernel.hyper_descriptors()
         arr = (N.Hyper * max(len(hd), 1))()
         coefs = []
@@ -218,23 +221,21 @@ class ProjectedProcessEngine:
             arr[i].dim = h.get("dim", 0)
             arr[i].value = h.get("value", 0.0)
             if h["kind"] == N.SGP_HYPER_SCALE:
-                cf = np.zeros(nterms)
+                cf = np.zeros(desc.n_terms)
                 for t, v in h["coef"].items():
                     cf[t] = v
                 coefs.append(cf)
                 arr[i].coef = cf.ctypes.data_as(C.POINTER(C.c_double))
-        return arr, len(hd), coefs
+        val = C.c_double()
+        grad = np.zeros(max(len(hd), 1))
+        self._check(fn(self._h, C.byref(desc), arr, len(hd), *args, C.byref(val), N.ptr(grad)))
+        del keep, coefs
+        return val.value, grad[:len(hd)]
 
     def laplace_nll(self, kernel: Kernel, tol: float):
         """Binary classification: (-log Z summed over experts, its gradient).  Updates the device-resident latent
         modes f of the uploaded experts (warm start), as GaussianProcessClassifier.likelihoodAndGradient does."""
-        desc, keep = _make_desc(kernel, self._experts_d)
-        arr, nh, coefs = self._hyper_array(kernel, desc.n_terms)
-        val = C.c_double()
-        grad = np.zeros(max(nh, 1))
-        self._check(self._lib.sgp_laplace_nll(self._h, C.byref(desc), arr, nh, float(tol), C.byref(val), N.ptr(grad)))
-        del keep, coefs
-        return val.value, grad[:nh]
+        return self._objective(self._lib.sgp_laplace_nll, kernel, float(tol))
 
     def experts_f(self, n: int):
         f = np.empty(n)
@@ -243,13 +244,7 @@ class ProjectedProcessEngine:
 
     def bcm_nll(self, kernel: Kernel):
         """(sum over experts of 1/2 y'K^-1 y + 1/2 log|K|, gradient w.r.t. kernel.getHyperparameters())."""
-        desc, keep = _make_desc(kernel, self._experts_d)
-        arr, nh, coefs = self._hyper_array(kernel, desc.n_terms)
-        nll = C.c_double()
-        grad = np.zeros(max(nh, 1))
-        self._check(self._lib.sgp_bcm_nll(self._h, C.byref(desc), arr, nh, C.byref(nll), N.ptr(grad)))
-        del keep, coefs
-        return nll.value, grad[:nh]
+        return self._objective(self._lib.sgp_bcm_nll, kernel)
 
     # ---- getMagicVector -------------------------------------------------------------------------------
     def magic(self, G=None, b=None, copy_out: bool = True):

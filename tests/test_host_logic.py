@@ -284,15 +284,15 @@ def test_greedy_rank1_update_identities():
 
 
 # ---- which device kernel evaluates a per-expert objective (tests/test_gpu_objectives.py is built on this rule) -------
-# The rule lives in three places: sgp_bcm_nll (csrc/api.cu) sends experts whose shared-memory Cholesky does not fit
-# (bcm_nll_smem_bytes > 227 KB) to the global-memory LU path; launch_bcm_nll (csrc/bcm_nll.cu) runs the register kernel
-# for one non-Eye term and n_max <= 128 (template shape by 16-row blocks) unless its shared memory exceeds 227 KB, and
-# otherwise the shared-memory kernel, which stages the expert's rows when two CTAs per SM still fit (113 KB each);
-# sgp_laplace_nll (csrc/api.cu) refuses laplace_smem_bytes > 227 KB and launch_laplace (csrc/laplace.cu) stages the rows
-# when they fit beside it.  A Cholesky pivot <= 0 also sends sgp_bcm_nll to the LU path (not modelled: SPD inputs only).
+# The rule is plan_objective (csrc/bcm_nll.cu); sgp_bcm_nll and sgp_laplace_nll launch what it returns.  BCM: experts
+# whose shared-memory Cholesky does not fit (bcm_nll_smem_bytes > 227 KB) take the global-memory LU path; one non-Eye
+# term and n_max <= 128 run the register kernel (template shape by 16-row blocks) unless its shared memory exceeds
+# 227 KB; otherwise the shared-memory kernel runs, and stages the expert's rows when two CTAs per SM still fit (113 KB
+# each).  Laplace: refused when laplace_smem_bytes > 227 KB, rows staged when they fit beside it.  A Cholesky pivot <= 0
+# also sends sgp_bcm_nll to the LU path (not modelled: SPD inputs only), whose kernel stages the rows up to 200 KB.
 K_MAX_TERMS, DCH = 4, 16
 EX_SUMS = 2 * K_MAX_TERMS + 1 + DCH
-SMEM_MAX, SMEM_STAGE_BCM = 227 * 1024, 113 * 1024
+SMEM_MAX, SMEM_STAGE_BCM, SMEM_STAGE_LU = 227 * 1024, 113 * 1024, 200 * 1024
 BCM_REG_SHAPES = ((4, (2, 4)), (6, (3, 6)), (7, (4, 7)), (8, (4, 8)))     # (16-row blocks <=, (RBR, RBC))
 MAX_HYPERS = 72
 
@@ -354,6 +354,25 @@ def test_objective_dispatch_thresholds():
     assert laplace_variant(100, 20) == "staged" and laplace_variant(115, 1) == "staged"
     # hyper-parameter limit: 71 ARD betas + scale fit, 72 + scale do not; d = 71 fits every register shape
     assert 1 + 71 == MAX_HYPERS and bcm_variant(64, 1, 71) == "reg<2,4>"
+
+
+def test_objective_mirror_constants_match_source():
+    """The limits and shapes the objective-dispatch mirrors above transcribe, read from the sources."""
+    import os
+    import re
+    csrc = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "spark_gp_b200", "csrc")
+    read = lambda f: open(os.path.join(csrc, f)).read()
+    bcm, internal = read("bcm_nll.cu"), read("sgp_internal.h")
+    kib = lambda src, name: int(re.search(r"constexpr size_t %s = (\d+) \* 1024;" % name, src).group(1)) * 1024
+    assert kib(internal, "kSmemOptInMax") == SMEM_MAX
+    assert kib(bcm, "kStageTwoCtas") == SMEM_STAGE_BCM
+    assert kib(bcm, "kStageGeneral") == SMEM_STAGE_LU
+    assert int(re.search(r"constexpr int kMaxHypers = (\d+);", internal).group(1)) == MAX_HYPERS
+    table = re.search(r"const RegShape kRegShapes\[\] = \{(.*?)\};", bcm, re.S).group(1)
+    shapes = re.findall(r"\{(\d+), (\d+), (\d+), bcm_nll_reg_kernel<(\d+), (\d+)>\}", table)
+    assert [(int(b), (int(r), int(c))) for b, r, c, _, _ in shapes] == list(BCM_REG_SHAPES)
+    assert all((r, c) == (tr, tc) for _, r, c, tr, tc in shapes)       # each row names the template it launches
+    assert 16 * BCM_REG_SHAPES[-1][0] == 128                            # the register kernel's largest expert
 
 
 # ---- per-component error bound of the objective gradient (test_gpu_objectives.py asserts it on the GPU) --------------
