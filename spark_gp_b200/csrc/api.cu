@@ -188,7 +188,8 @@ static int direct_prepare(Ctx* c) {
   return SGP_OK;
 }
 
-// One fused-kernel launch over n device-resident points + the deterministic slice reduction.
+// The statistics of n device-resident points: the fp64 kernel, or the int8 digit-plane producer and Gram (per launch
+// window), then the deterministic slice reduction.
 static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, long long n, long long n_call,
                         bool first_of_call) {
   // n: points of this launch; n_call: points of the whole accumulate call.  AUTO decides per CALL -- the size gate
@@ -201,8 +202,13 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   if (n_slices < 1) n_slices = 1;
   const long long blocks = (n + 15) / 16;
   if (n_slices > blocks) n_slices = static_cast<int>(blocks);
-  // int8 kernel: one launch over the upper block triangle x point slices
-  const int i8_n_slices = c->i8_direct_ok ? i8_slices(c->m_pad, c->num_sms, (n + 63) / 64) : 1;
+  // int8 path: the digit planes of a launch window take kI8PlaneBytes per unit and active tile, so a launch covers at
+  // most kI8PlaneCapBytes of them; larger launches split into equal windows, all run with the first window's slices
+  const long long n_units = (n + 63) / 64;
+  const long long cap_units = std::max<long long>(1, kI8PlaneCapBytes / (kI8PlaneBytes * nt1));
+  const long long n_windows = (n_units + cap_units - 1) / cap_units;
+  const long long win_units = (n_units + n_windows - 1) / n_windows;
+  const int i8_n_slices = c->i8_direct_ok ? i8_slices(c->m_pad, c->num_sms, win_units) : 1;
   const int max_slices = n_slices > i8_n_slices ? n_slices : i8_n_slices;
   int rc = ctx_scratch(c, c->gpart_ws, static_cast<size_t>(max_slices) * c->m_pad * c->m_pad * sizeof(double));
   if (rc == SGP_OK) rc = ctx_scratch(c, c->bpart_ws, static_cast<size_t>(max_slices) * c->m_pad * sizeof(double));
@@ -227,13 +233,14 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   } else if (c->precision == SGP_PREC_AUTO && n_call >= kAutoI8MinPoints) {
     path = !first_of_call ? c->call_path : c->i8_ok ? 1 : c->i8_direct_ok ? 2 : 0;
   }
+  // bytes of one 64-point unit of the int8 point operands: fp16 images (path 1) or fp32 coordinate tiles (path 2)
+  const size_t x_unit = (path == 1) ? i8_points_scratch_bytes(64, i8_nchunks(c->d))
+                                    : static_cast<size_t>(c->kf.n_terms) * 64 * c->dpad * sizeof(float);
   if (path != 0) {
     const bool autop = c->precision == SGP_PREC_AUTO;
     const bool gate = autop && first_of_call;
-    const size_t xb = (path == 1) ? i8_points_scratch_bytes(n, i8_nchunks(c->d))
-                                  : static_cast<size_t>((n + 63) / 64) * c->kf.n_terms * 64 * c->dpad * sizeof(float);
-    rc = ctx_scratch(c, c->i8_ys_ws, static_cast<size_t>((n + 63) / 64) * 64 * sizeof(float));
-    if (rc == SGP_OK) rc = ctx_scratch(c, c->i8_xt_ws, xb);
+    rc = ctx_scratch(c, c->i8_ys_ws, static_cast<size_t>(n_units) * 64 * sizeof(float));
+    if (rc == SGP_OK) rc = ctx_scratch(c, c->i8_xt_ws, static_cast<size_t>(n_units) * x_unit);
     if (rc == SGP_OK && path == 2) rc = direct_prepare(c);
     if (rc != SGP_OK) return rc;
     // the scaled squared norms of EVERY chunk are summed on the device (dI8NormSum[0]: whole begin..finish window,
@@ -273,6 +280,10 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   }
   c->last_path = (path == 1) ? SGP_PREC_I8 : (path == 2) ? SGP_PREC_I8_DIRECT
                  : (c->precision == SGP_PREC_F64_STRICT ? SGP_PREC_F64_STRICT : SGP_PREC_F64);
+  if (path != 0) {
+    rc = ctx_scratch(c, c->i8_planes_ws, static_cast<size_t>(win_units) * nt1 * kI8PlaneBytes);
+    if (rc != SGP_OK) return rc;
+  }
   if (c->gram_events_used == c->gram_events.size()) {          // grow the event pool (steady state: no creation)
     cudaEvent_t a, b;
     SGP_CUDA(c, cudaEventCreate(&a));
@@ -294,14 +305,25 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
       for (int t = 0; t < c->kf.n_terms; ++t) direct.w[t] = static_cast<float>(c->kf.scale[t] / csum);
       direct.csum = csum;
     }
+    const double C = (path == 2) ? direct.csum : c->kf.scale[0];
     const uint8_t* zop = (path == 2) ? c->i8_zd_ws.as<uint8_t>() : c->dI8Zt;
-    SGP_CUDA(c, launch_gram_i8(c->i8_xt_ws.as<uint8_t>(), c->i8_ys_ws.as<float>(), zop, n, c->d, c->m_pad, i8_n_slices,
-                               direct, Gpart, bpart, c->kf.scale[0], c->dbgT, c->dbgW, c->stream));
+    // per window: digit planes + b partials, then the Gram over them; the first window stores the slice partials,
+    // later ones add to them, and one deterministic slice reduction follows
+    for (long long w = 0; w < n_windows; ++w) {
+      const long long u0 = w * win_units;
+      const long long nu = std::min(win_units, n_units - u0);
+      SGP_CUDA(c, launch_i8_planes(c->i8_xt_ws.as<uint8_t>() + static_cast<size_t>(u0) * x_unit,
+                                   c->i8_ys_ws.as<float>() + static_cast<size_t>(u0) * 64, zop, nu, c->d, c->m_pad,
+                                   i8_n_slices, direct, C, w > 0, c->i8_planes_ws.as<uint8_t>(), bpart,
+                                   w == 0 ? c->dbgT : nullptr, w == 0 ? c->dbgW : nullptr, c->stream));
+      SGP_CUDA(c, launch_gram_i8(c->i8_planes_ws.as<uint8_t>(), nu, c->m_pad, i8_n_slices, C, w > 0, Gpart, c->stream));
+      c->launches += 2;
+    }
     SGP_CUDA(c, cudaEventRecord(e1, c->stream));
     // deterministic slice reduction (partial tiles at the mirror position: upper block triangle)
     SGP_CUDA(c, launch_gram_reduce_upper(c->dGb, c->dGb + mm, Gpart, bpart, i8_n_slices, c->m, c->m_pad, 0, c->m,
                                          c->stream));
-    c->launches += 2;
+    c->launches += 1;
     return SGP_OK;
   }
   GramParams p{};
@@ -387,8 +409,9 @@ int sgp_ctx_destroy(sgp_ctx* h) {
     if (c->stage_ready[i]) cudaEventDestroy(c->stage_ready[i]);
   }
   if (c->comm && nccl().ok) nccl().CommDestroy(c->comm);
-  for (DevScratch* s : {&c->gpart_ws, &c->bpart_ws, &c->i8_zd_ws, &c->i8_xt_ws, &c->i8_ys_ws, &c->nll_per_ws, &c->hyper_ws,
-                        &c->greedy_ws, &c->sweep_ws, &c->bcm_ws, &c->tail_ws, &c->tail_ws2, &c->predict_ws, &c->cross_ws})
+  for (DevScratch* s : {&c->gpart_ws, &c->bpart_ws, &c->i8_zd_ws, &c->i8_xt_ws, &c->i8_ys_ws, &c->i8_planes_ws,
+                        &c->nll_per_ws, &c->hyper_ws, &c->greedy_ws, &c->sweep_ws, &c->bcm_ws, &c->tail_ws, &c->tail_ws2,
+                        &c->predict_ws, &c->cross_ws})
     cudaFree(s->p);
   if (c->tail_fork) cudaEventDestroy(c->tail_fork);
   if (c->tail_join) cudaEventDestroy(c->tail_join);

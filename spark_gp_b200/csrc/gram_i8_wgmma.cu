@@ -1,4 +1,4 @@
-// Fused K_mn + Gram kernel on the Hopper tensor cores (wgmma), exact-accumulation path.
+// K_mn + Gram on the Hopper tensor cores (wgmma), exact-accumulation path: a digit-plane producer and an int8 Gram.
 //
 // Same contract as gram_f64.cu (one shard of points -> per-slice partial tiles of G = sum_n k_n k_n^T and
 // b = sum_n k_n y_n; replaces commons/ProjectedGaussianProcessHelper.scala:27-29 and the crossKernel chain
@@ -13,20 +13,21 @@
 // is six int8 products into three int32 accumulators.  The dropped products (weights 2^8, 2^0) are zero-mean because the
 // low digits are balanced; they bound this path's accuracy (posterior mean within ~2e-6 of fp64, DESIGN.md section 3).
 //
-// One CTA (256 threads = two warpgroups) owns the half tile  rows I-tile (128 active points) x 64 columns (half h of
-// J-tile), I >= J, and a slice of the shard's 64-point units; its three 64 x 64 int32 accumulators per warpgroup live in
-// registers (96 per thread).  Per unit:
-//   distances  tensor mode: T = -q*log2(e) as ONE fp16 wgmma contraction over the hi/lo split of the scaled, centred
-//              coordinates with the norms folded in as extra K columns (images from launch_i8_prep_points); panel I
-//              (warpgroup w: rows 64w.., m64n64) and, off the diagonal, the 64 rows of panel J (warpgroup w: points 32w..,
-//              m64n32).  Direct mode: sum of up to 4 terms of 2^(-|x~ - z~|^2) from fp32 coordinates on the CUDA cores,
-//              at the same fragment positions.
-//   epilogue   ex2 -> fixed point via one FFMA against 2^23 -> byte planes (PRMT) -> K-major SWIZZLE_64B int8 planes in
-//              shared memory (double buffered), b += kappa*y on diagonal tiles.
-//   Gram       12 int8 wgmma m64n64k32 per warpgroup (6 products x 2 k-steps of 32 points), issued asynchronously: they
-//              run while the next unit's distances are contracted.  Every 400 units the accumulators are folded into
-//              the fp64 partial tile (no overflow possible).
-// Operands arrive by bulk copy (cp.async.bulk, completion on an mbarrier) into a ring of point stages.
+// Two kernels, so that every kernel element is computed once per unit (not once per CTA whose tile holds its row):
+//   kmn_i8_planes_kernel   one CTA (two warpgroups, 64 rows each) per (active tile of 128 rows, point slice).  Per
+//              64-point unit: distances (tensor mode: T = -q*log2(e) as ONE fp16 wgmma contraction over the hi/lo split
+//              of the scaled, centred coordinates with the norms folded in as extra K columns, images from
+//              launch_i8_prep_points / launch_i8_prep_active; direct mode: sum of up to 4 terms of 2^(-|x~ - z~|^2) from
+//              fp32 coordinates on the CUDA cores), then ex2 -> fixed point via one FFMA against 2^23 -> byte planes
+//              (PRMT) in shared memory, in exactly the K-major SWIZZLE_64B byte image the Gram reads, and one 24 KB bulk
+//              store of the tile's three planes to the plane workspace [unit][tile][3][128 x 64].  b += kappa*y for the
+//              tile's rows (fp32 per unit, fp64 across units).
+//   gram_i8_kernel   one CTA per (tile pair I >= J of the upper block triangle, point slice), warp specialised: one
+//              thread of the copy warpgroup streams the I and J plane images of each unit into a ring of stages
+//              (cp.async.bulk, mbarrier completion, released by the consumers through a second mbarrier); two consumer
+//              warpgroups (64 rows of I each, all 128 columns of J) issue twelve int8 wgmma m64n128k32 per unit into three
+//              int32 accumulators (192 registers, handed over from the copy warpgroup with setmaxnreg).  Every 400 units
+//              the accumulators are folded into the fp64 partial tile (no overflow possible).
 #include <cuda_fp16.h>
 
 #include "hopper.cuh"
@@ -38,13 +39,16 @@ namespace {
 using namespace hop;
 
 constexpr int UP = 64;                  // points per pipeline unit
-constexpr int NTHREADS = 256;           // two warpgroups
-constexpr int XSTAGES_MAX = 8;
+constexpr int NTHREADS = 256;           // producer: two warpgroups
+constexpr int XSTAGES = 4;              // producer: ring of point stages
 constexpr int ZPANEL_BYTES = 16384;     // fp16 active-set operand image: 128 rows x 128 bytes, SWIZZLE_128B K-major
 constexpr int XIMG_BYTES = 8192;        // fp16 point operand image: 64 rows x 128 bytes
-constexpr int PLANE_I = 8192;           // int8 digit plane of panel I: 128 rows x 64 points, K-major SWIZZLE_64B
-constexpr int PLANE_J = 4096;           // ... of the 64 rows of panel J this CTA multiplies with
-constexpr int PLANES_BYTES = 3 * PLANE_I + 3 * PLANE_J;
+constexpr int PLANE = 8192;             // int8 digit plane of one tile: 128 rows x 64 points, K-major SWIZZLE_64B
+constexpr int TILE_PLANES = 3 * PLANE;  // the three planes of one (unit, tile): one bulk copy
+static_assert(TILE_PLANES == kI8PlaneBytes, "plane workspace stride");
+constexpr int GTHREADS = 384;           // Gram: copy warpgroup + two consumer warpgroups
+constexpr int GSTAGES = 4;              // Gram: ring of [I planes | J planes] stages, 48 KB each
+constexpr int COPY_REGS = 24, MMA_REGS = 240;   // setmaxnreg split: 128 x 24 + 256 x 240 <= 65536
 constexpr int FLUSH_UNITS = 400;        // |ACC4| <= 255^2 n, |ACC3| <= 2*255*128 n, |ACC2| <= (2*255*128 + 128^2) n < 2^31
 // Fixed point: mantissa(kappa * C0 + MAGIC) = u + 0x4040, and the bytes of (that << 1) are (2 s0 + 128, s1 + 128, s2).
 constexpr float C0 = 8355000.0f;        // u <= C0*(1+2e-3) keeps u + 0x4040 < 2^23
@@ -68,7 +72,16 @@ __device__ __forceinline__ void store_digits(uint8_t* planes, int plane_bytes, i
   *reinterpret_cast<uint16_t*>(planes + 2 * plane_bytes + off) = static_cast<uint16_t>(prmt(w0, w1, 0x0062));         // P2
 }
 
-struct I8Params {
+// units [u_lo, u_lo + nu) of point slice `slice` (the producer and the Gram split a launch identically)
+__device__ __forceinline__ long long slice_units(long long n_units, int n_slices, int slice, long long* u_lo) {
+  const long long ups = (n_units + n_slices - 1) / n_slices;
+  *u_lo = ups * slice;
+  long long u_hi = *u_lo + ups;
+  if (u_hi > n_units) u_hi = n_units;
+  return u_hi > *u_lo ? u_hi - *u_lo : 0;
+}
+
+struct PlaneParams {
   const uint8_t* Xt;    // tensor mode: [n_units][nchunks][8192] fp16 images; direct: [n_units][n_terms][dpad4][64] fp32
   const float* ys;      // [n_units*64]
   const uint8_t* Zt;    // tensor mode: [nt][nchunks][16384]; direct: [nt][n_terms][dpad4][128 rows] fp32, negated
@@ -76,62 +89,39 @@ struct I8Params {
   uint32_t xbytes, zbytes;
   int n_terms, dpad4;   // direct mode
   float w[4];           // term weights C_t / sum_t C_t
-  int xstages;
   int m_pad, nt, n_slices;
-  double* Gpart;        // [n_slices][m_pad*m_pad]
+  uint8_t* planes;      // [n_units][nt][TILE_PLANES]
   double* bpart;        // [n_slices][m_pad]
-  double gscale;        // C^2 / (4 C0^2)
   double bscale;        // C
-  float* dbg_T;         // optional [128*64] : T of the first distance tile of CTA (0,0)
+  int accumulate;       // 0: store b, 1: add to it (later windows of one call)
+  float* dbg_T;         // optional [128*64] : T of tile 0, unit 0
   uint32_t* dbg_w;      // optional [128*64] : fixed-point words of the same tile
 };
 
 // KS: 16-column k-steps of the tensor-mode distance contraction (4 for d <= 16, 7 for d <= 32; unused in direct mode).
-// Every MMA of a unit is issued unconditionally (a branch around wgmma makes ptxas serialise them): on diagonal tiles the
-// panel-J contraction runs against panel I and its result is not used.
 template <bool DIRECT, int KS>
-__global__ void __launch_bounds__(NTHREADS, 1) kmn_gram_i8_wgmma_kernel(const I8Params p) {
+__global__ void __launch_bounds__(NTHREADS, 1) kmn_i8_planes_kernel(const PlaneParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* sm = smem_raw + (base - raw);
-  const uint32_t s_zi = base, s_zj = s_zi + p.zbytes;                 // active tiles I and J
-  const uint32_t s_pl = s_zj + p.zbytes;                              // [2 buffers][PI0 PI1 PI2 PJ0 PJ1 PJ2]
-  const uint32_t s_xs = s_pl + 2 * PLANES_BYTES;                      // [xstages][xbytes]
-  const uint32_t s_ys = s_xs + p.xstages * p.xbytes;                  // [xstages][64] float
-  const uint32_t s_bar = s_ys + p.xstages * UP * 4;                   // zfull, xfull[xstages]
+  const uint32_t s_pl = base;                                 // [2 buffers][P0 P1 P2]
+  const uint32_t s_zt = s_pl + 2 * TILE_PLANES;               // active tile
+  const uint32_t s_xs = s_zt + p.zbytes;                      // [XSTAGES][xbytes]
+  const uint32_t s_ys = s_xs + XSTAGES * p.xbytes;            // [XSTAGES][64] float
+  const uint32_t s_bar = s_ys + XSTAGES * UP * 4;             // zfull, xfull[XSTAGES]
   const uint32_t b_zfull = s_bar, b_xfull = s_bar + 8;
 
   const int tid = threadIdx.x, wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
-  const int h = blockIdx.x & 1;
-  int ti, tj;
-  {
-    int t = blockIdx.x >> 1;
-    tj = 0;
-    while (t >= p.nt - tj) { t -= p.nt - tj; ++tj; }
-    ti = tj + t;
-  }
-  const bool diag = ti == tj;
-
-  const long long ups = (p.n_units + p.n_slices - 1) / p.n_slices;
-  const long long u_lo = ups * blockIdx.y;
-  long long u_hi = u_lo + ups;
-  if (u_hi > p.n_units) u_hi = p.n_units;
-  const long long nu = u_hi > u_lo ? u_hi - u_lo : 0;
-
-  double* Gp = p.Gpart + static_cast<size_t>(blockIdx.y) * p.m_pad * p.m_pad;
-  double* bp = p.bpart + static_cast<size_t>(blockIdx.y) * p.m_pad;
-  // partial tile stored TRANSPOSED (mirror position, upper block triangle; gram_reduce_upper reads it):
-  // element (row R of tile I, column c of half h of tile J) at Gp[(tj*128 + 64h + c) * m_pad + ti*128 + R]
-  double* gtile = Gp + static_cast<size_t>(tj * kTile + 64 * h) * p.m_pad + ti * kTile;
-
-  if (nu == 0) {   // empty slice: the partial tile must still be defined
-    for (int e = tid; e < 64 * kTile; e += NTHREADS) gtile[static_cast<size_t>(e / kTile) * p.m_pad + (e % kTile)] = 0.0;
-    if (diag && h == 0 && tid < kTile) bp[ti * kTile + tid] = 0.0;
+  const int ti = blockIdx.x;
+  long long u_lo;
+  const long long nu = slice_units(p.n_units, p.n_slices, blockIdx.y, &u_lo);
+  double* bp = p.bpart + static_cast<size_t>(blockIdx.y) * p.m_pad + ti * kTile;
+  if (nu == 0) {   // empty slice: its b partial must still be defined
+    if (!p.accumulate && tid < kTile) bp[tid] = 0.0;
     return;
   }
 
-  const int xs_n = p.xstages;
   auto issue_unit = [&](long long i, int s) {
     mbar_expect_tx(b_xfull + 8 * s, p.xbytes + UP * 4);
     bulk_g2s(s_xs + s * p.xbytes, p.Xt + static_cast<size_t>(u_lo + i) * p.xbytes, p.xbytes, b_xfull + 8 * s);
@@ -139,203 +129,267 @@ __global__ void __launch_bounds__(NTHREADS, 1) kmn_gram_i8_wgmma_kernel(const I8
   };
   if (tid == 0) {
     mbar_init(b_zfull, 1);
-    for (int s = 0; s < xs_n; ++s) mbar_init(b_xfull + 8 * s, 1);
+    for (int s = 0; s < XSTAGES; ++s) mbar_init(b_xfull + 8 * s, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   if (tid == 0) {
-    mbar_expect_tx(b_zfull, diag ? p.zbytes : 2 * p.zbytes);
-    bulk_g2s(s_zi, p.Zt + static_cast<size_t>(ti) * p.zbytes, p.zbytes, b_zfull);
-    if (!diag) bulk_g2s(s_zj, p.Zt + static_cast<size_t>(tj) * p.zbytes, p.zbytes, b_zfull);
-    for (long long i = 0; i < xs_n && i < nu; ++i) issue_unit(i, static_cast<int>(i));
+    mbar_expect_tx(b_zfull, p.zbytes);
+    bulk_g2s(s_zt, p.Zt + static_cast<size_t>(ti) * p.zbytes, p.zbytes, b_zfull);
+    for (long long i = 0; i < XSTAGES && i < nu; ++i) issue_unit(i, static_cast<int>(i));
   }
 
-  // fragment coordinates of a wgmma m64nN accumulator: element 4j+e sits at row r0 (+8 if e >= 2), column 8j + c0 + (e & 1)
+  // fragment coordinates of a wgmma m64n64 accumulator: element 4j+e sits at row r0 (+8 if e >= 2), point 8j + c0 + (e & 1)
   const int r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
-  const int RI = 64 * wg + r0;            // panel-I row (of 128) of this thread's first fragment row
-
-  int acc4[32], acc3[32], acc2[32];
-#pragma unroll
-  for (int e = 0; e < 32; ++e) acc4[e] = acc3[e] = acc2[e] = 0;
+  const int R = 64 * wg + r0;             // tile row (of 128) of this thread's first fragment row
   double bsum0 = 0.0, bsum1 = 0.0;
-  int until_flush = FLUSH_UNITS;
-  bool first_flush = true;
-  const bool want_b = diag && h == 0;
 
   mbar_wait(b_zfull, 0);
   for (long long i = 0; i < nu; ++i) {
-    const int s = static_cast<int>(i % xs_n);
-    // stage (i-1) % xs_n was released by every thread at the barrier of unit i-1
-    if (tid == 0 && i >= 1 && i + xs_n - 1 < nu) issue_unit(i + xs_n - 1, static_cast<int>((i - 1) % xs_n));
-    mbar_wait(b_xfull + 8 * s, static_cast<uint32_t>((i / xs_n) & 1));
+    const int s = static_cast<int>(i % XSTAGES);
+    mbar_wait(b_xfull + 8 * s, static_cast<uint32_t>((i / XSTAGES) & 1));
     const uint32_t xst = s_xs + s * p.xbytes;
 
-    float TI[32], TJ[16];
+    float T[32];
     if constexpr (!DIRECT) {
-      const uint32_t za = s_zi + wg * 8192, zja = (diag ? s_zi : s_zj) + h * 8192;
       wg_fence();
 #pragma unroll
       for (int k = 0; k < KS; ++k) {
-        const uint32_t off = (k >> 2) * ZPANEL_BYTES + (k & 3) * 32, xoff = (k >> 2) * XIMG_BYTES + (k & 3) * 32;
-        wgmma_f16_n64(TI, desc_sw128(za + off), desc_sw128(xst + xoff), k > 0);
-        wgmma_f16_n32(TJ, desc_sw128(zja + off), desc_sw128(xst + wg * 4096 + xoff), k > 0);
+        const uint32_t za = s_zt + (k >> 2) * ZPANEL_BYTES + wg * 8192 + (k & 3) * 32;
+        const uint32_t xb = xst + (k >> 2) * XIMG_BYTES + (k & 3) * 32;
+        wgmma_f16_n64(T, desc_sw128(za), desc_sw128(xb), k > 0);
       }
       wg_commit();
-      wg_wait<0>();      // also drains this warpgroup's Gram MMAs of unit i-1
+      wg_wait<0>();
       if (p.dbg_T && i == 0 && blockIdx.x == 0 && blockIdx.y == 0) {
 #pragma unroll
-        for (int e = 0; e < 32; ++e) p.dbg_T[(RI + ((e & 2) ? 8 : 0)) * UP + 8 * (e >> 2) + c0 + (e & 1)] = TI[e];
+        for (int e = 0; e < 32; ++e) p.dbg_T[(R + ((e & 2) ? 8 : 0)) * UP + 8 * (e >> 2) + c0 + (e & 1)] = T[e];
       }
 #pragma unroll
-      for (int e = 0; e < 32; ++e) TI[e] = ex2f(TI[e]);
-#pragma unroll
-      for (int e = 0; e < 16; ++e) TJ[e] = ex2f(TJ[e]);
+      for (int e = 0; e < 32; ++e) T[e] = ex2f(T[e]);
     } else {
 #pragma unroll
-      for (int e = 0; e < 32; ++e) TI[e] = 0.f;
-#pragma unroll
-      for (int e = 0; e < 16; ++e) TJ[e] = 0.f;
-      wg_wait<0>();
+      for (int e = 0; e < 32; ++e) T[e] = 0.f;
       // kappa = sum_t w_t 2^(-|x~_t - z~_t|^2), direct form (no cancellation: any norms)
       const float* xs = reinterpret_cast<const float*>(sm + (xst - base));
-      const float* zi = reinterpret_cast<const float*>(sm + (s_zi - base));
-      const float* zj = reinterpret_cast<const float*>(sm + ((diag ? s_zi : s_zj) - base));
-      const int pi0 = RI, pi1 = RI + 8, pj0 = 64 * h + r0, pj1 = 64 * h + r0 + 8;
+      const float* zt = reinterpret_cast<const float*>(sm + (s_zt - base));
       for (int t = 0; t < p.n_terms; ++t) {
-        float qi[32], qj[16];
+        float q[32];
 #pragma unroll
-        for (int e = 0; e < 32; ++e) qi[e] = 0.f;
-#pragma unroll
-        for (int e = 0; e < 16; ++e) qj[e] = 0.f;
+        for (int e = 0; e < 32; ++e) q[e] = 0.f;
         const float* xt = xs + t * p.dpad4 * UP;
-        const float* zit = zi + t * p.dpad4 * kTile;
-        const float* zjt = zj + t * p.dpad4 * kTile;
+        const float* ztt = zt + t * p.dpad4 * kTile;
 #pragma unroll 2
         for (int k = 0; k < p.dpad4; ++k) {
-          const float a0 = zit[k * kTile + pi0], a1 = zit[k * kTile + pi1];      // stored negated
+          const float a0 = ztt[k * kTile + R], a1 = ztt[k * kTile + R + 8];      // stored negated
           const float* xk = xt + k * UP + c0;
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const float2 x = *reinterpret_cast<const float2*>(xk + 8 * j);
             float e0 = x.x + a0, e1 = x.y + a0, e2 = x.x + a1, e3 = x.y + a1;
-            qi[4 * j + 0] = fmaf(e0, e0, qi[4 * j + 0]); qi[4 * j + 1] = fmaf(e1, e1, qi[4 * j + 1]);
-            qi[4 * j + 2] = fmaf(e2, e2, qi[4 * j + 2]); qi[4 * j + 3] = fmaf(e3, e3, qi[4 * j + 3]);
-          }
-          if (!diag) {
-            const float b0 = zjt[k * kTile + pj0], b1 = zjt[k * kTile + pj1];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float2 x = *reinterpret_cast<const float2*>(xk + 32 * wg + 8 * j);
-              float e0 = x.x + b0, e1 = x.y + b0, e2 = x.x + b1, e3 = x.y + b1;
-              qj[4 * j + 0] = fmaf(e0, e0, qj[4 * j + 0]); qj[4 * j + 1] = fmaf(e1, e1, qj[4 * j + 1]);
-              qj[4 * j + 2] = fmaf(e2, e2, qj[4 * j + 2]); qj[4 * j + 3] = fmaf(e3, e3, qj[4 * j + 3]);
-            }
+            q[4 * j + 0] = fmaf(e0, e0, q[4 * j + 0]); q[4 * j + 1] = fmaf(e1, e1, q[4 * j + 1]);
+            q[4 * j + 2] = fmaf(e2, e2, q[4 * j + 2]); q[4 * j + 3] = fmaf(e3, e3, q[4 * j + 3]);
           }
         }
         const float wt = p.w[t];
 #pragma unroll
-        for (int e = 0; e < 32; ++e) TI[e] = fmaf(wt, ex2f(-qi[e]), TI[e]);
-#pragma unroll
-        for (int e = 0; e < 16; ++e) TJ[e] = fmaf(wt, ex2f(-qj[e]), TJ[e]);
+        for (int e = 0; e < 32; ++e) T[e] = fmaf(wt, ex2f(-q[e]), T[e]);
       }
     }
 
-    // ---- epilogue: b on diagonal tiles, digit planes of panel I (and of the 64 rows of panel J) ----------------
-    uint8_t* planes = sm + (s_pl - base) + static_cast<int>(i & 1) * PLANES_BYTES;
-    if (want_b) {
+    {   // b: fp32 over the unit's points, fp64 across units
       const float* yv = reinterpret_cast<const float*>(sm + (s_ys - base)) + s * UP + c0;
       float b0 = 0.f, b1 = 0.f;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float2 y2 = *reinterpret_cast<const float2*>(yv + 8 * j);
-        b0 = fmaf(TI[4 * j + 0], y2.x, fmaf(TI[4 * j + 1], y2.y, b0));
-        b1 = fmaf(TI[4 * j + 2], y2.x, fmaf(TI[4 * j + 3], y2.y, b1));
+        b0 = fmaf(T[4 * j + 0], y2.x, fmaf(T[4 * j + 1], y2.y, b0));
+        b1 = fmaf(T[4 * j + 2], y2.x, fmaf(T[4 * j + 3], y2.y, b1));
       }
       bsum0 += static_cast<double>(b0);
       bsum1 += static_cast<double>(b1);
     }
+
+    // point stage s is consumed; plane buffer i&1 is free once the bulk store of unit i-2 has read it
+    if (tid == 0) bulk_wait_read<1>();
+    __syncthreads();
+    if (tid == 0 && i + XSTAGES < nu) issue_unit(i + XSTAGES, s);
+
+    uint8_t* planes = sm + (s_pl - base) + static_cast<int>(i & 1) * TILE_PLANES;
     const bool dbg = p.dbg_w != nullptr && i == 0 && blockIdx.x == 0 && blockIdx.y == 0;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const uint32_t w0 = fixed_word(TI[4 * j + 0]), w1 = fixed_word(TI[4 * j + 1]);
-      const uint32_t w2 = fixed_word(TI[4 * j + 2]), w3 = fixed_word(TI[4 * j + 3]);
-      store_digits(planes, PLANE_I, RI, 8 * j + c0, w0, w1);
-      store_digits(planes, PLANE_I, RI + 8, 8 * j + c0, w2, w3);
+      const uint32_t w0 = fixed_word(T[4 * j + 0]), w1 = fixed_word(T[4 * j + 1]);
+      const uint32_t w2 = fixed_word(T[4 * j + 2]), w3 = fixed_word(T[4 * j + 3]);
+      store_digits(planes, PLANE, R, 8 * j + c0, w0, w1);
+      store_digits(planes, PLANE, R + 8, 8 * j + c0, w2, w3);
       if (dbg) {
         const int k = 8 * j + c0;
-        p.dbg_w[RI * UP + k] = w0 >> 1; p.dbg_w[RI * UP + k + 1] = w1 >> 1;
-        p.dbg_w[(RI + 8) * UP + k] = w2 >> 1; p.dbg_w[(RI + 8) * UP + k + 1] = w3 >> 1;
-      }
-    }
-    if (!diag) {
-      uint8_t* pj = planes + 3 * PLANE_I;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int k = 32 * wg + 8 * j + c0;
-        store_digits(pj, PLANE_J, r0, k, fixed_word(TJ[4 * j + 0]), fixed_word(TJ[4 * j + 1]));
-        store_digits(pj, PLANE_J, r0 + 8, k, fixed_word(TJ[4 * j + 2]), fixed_word(TJ[4 * j + 3]));
+        p.dbg_w[R * UP + k] = w0 >> 1; p.dbg_w[R * UP + k + 1] = w1 >> 1;
+        p.dbg_w[(R + 8) * UP + k] = w2 >> 1; p.dbg_w[(R + 8) * UP + k + 1] = w3 >> 1;
       }
     }
     fence_proxy_async();
-    __syncthreads();     // planes complete (both warpgroups); point stage s and its y released
-
-    // ---- Gram: 6 products x 2 k-steps of 32 points, asynchronous -------------------------------------------------
-    {
-      const uint32_t pl = s_pl + static_cast<uint32_t>(i & 1) * PLANES_BYTES;
-      const uint32_t a_base = pl + wg * 4096;
-      const uint32_t b_base = diag ? pl + h * 4096 : pl + 3 * PLANE_I;
-      const uint32_t b_stride = diag ? PLANE_I : PLANE_J;
-      wg_fence();
-#pragma unroll
-      for (int ks = 0; ks < 2; ++ks) {
-        const uint64_t A0 = desc_sw64(a_base + 32 * ks), A1 = desc_sw64(a_base + PLANE_I + 32 * ks),
-                       A2 = desc_sw64(a_base + 2 * PLANE_I + 32 * ks);
-        const uint64_t B0 = desc_sw64(b_base + 32 * ks), B1 = desc_sw64(b_base + b_stride + 32 * ks),
-                       B2 = desc_sw64(b_base + 2 * b_stride + 32 * ks);
-        wgmma_uu(acc4, A2, B2);                   // weight 2^32 : P2'P2
-        wgmma_us(acc3, A2, B1);                   // weight 2^24 : P2'P1 + P1'P2
-        wgmma_su(acc3, A1, B2);
-        wgmma_us(acc2, A2, B0);                   // weight 2^16 : P2'P0 + P0'P2 + P1'P1
-        wgmma_su(acc2, A0, B2);
-        wgmma_ss(acc2, A1, B1);
-      }
-      wg_commit();
-    }
-
-    if (--until_flush == 0 || i == nu - 1) {
-      // ---- fold the exact int32 accumulators into the fp64 partial tile ---------------------------------------
-      until_flush = FLUSH_UNITS;
-      wg_wait<0>();
-#pragma unroll
-      for (int e = 0; e < 32; ++e) {
-        const int R = RI + ((e & 2) ? 8 : 0), c = 8 * (e >> 2) + c0 + (e & 1);
-        const double v = p.gscale * (4294967296.0 * static_cast<double>(acc4[e]) + 16777216.0 * static_cast<double>(acc3[e]) +
-                                     65536.0 * static_cast<double>(acc2[e]));
-        double* dst = gtile + static_cast<size_t>(c) * p.m_pad + R;
-        if (first_flush) *dst = v;
-        else *dst += v;
-        acc4[e] = acc3[e] = acc2[e] = 0;
-      }
-      first_flush = false;
+    __syncthreads();     // planes of unit i complete
+    if (tid == 0) {
+      bulk_s2g(p.planes + (static_cast<size_t>(u_lo + i) * p.nt + ti) * TILE_PLANES,
+               s_pl + static_cast<uint32_t>(i & 1) * TILE_PLANES, TILE_PLANES);
+      bulk_commit();
     }
   }
-  if (want_b) {
-    // a row's 64 points are spread over the 4 lanes of a quad
-    bsum0 += __shfl_xor_sync(0xffffffffu, bsum0, 1);
-    bsum0 += __shfl_xor_sync(0xffffffffu, bsum0, 2);
-    bsum1 += __shfl_xor_sync(0xffffffffu, bsum1, 1);
-    bsum1 += __shfl_xor_sync(0xffffffffu, bsum1, 2);
-    if ((lane & 3) == 0) {
-      bp[ti * kTile + RI] = p.bscale * bsum0;
-      bp[ti * kTile + RI + 8] = p.bscale * bsum1;
+  if (tid == 0) bulk_wait<0>();
+
+  // a row's 64 points are spread over the 4 lanes of a quad
+  bsum0 += __shfl_xor_sync(0xffffffffu, bsum0, 1);
+  bsum0 += __shfl_xor_sync(0xffffffffu, bsum0, 2);
+  bsum1 += __shfl_xor_sync(0xffffffffu, bsum1, 1);
+  bsum1 += __shfl_xor_sync(0xffffffffu, bsum1, 2);
+  if ((lane & 3) == 0) {
+    if (p.accumulate) {
+      bp[R] += p.bscale * bsum0;
+      bp[R + 8] += p.bscale * bsum1;
+    } else {
+      bp[R] = p.bscale * bsum0;
+      bp[R + 8] = p.bscale * bsum1;
     }
   }
 }
 
+struct GramI8Params {
+  const uint8_t* planes;   // [n_units][nt][TILE_PLANES]
+  long long n_units;
+  int m_pad, nt, n_slices;
+  double* Gpart;           // [n_slices][m_pad*m_pad]
+  double gscale;           // C^2 / (4 C0^2)
+  int accumulate;          // 0: the first fold stores, 1: every fold adds (later windows of one call)
+};
+
+__global__ void __launch_bounds__(GTHREADS, 1) gram_i8_kernel(const GramI8Params p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;
+  const uint32_t s_st = base;                                  // [GSTAGES][I planes | J planes]
+  const uint32_t b_full = s_st + GSTAGES * 2 * TILE_PLANES;    // [GSTAGES]
+  const uint32_t b_empty = b_full + 8 * GSTAGES;               // [GSTAGES]
+
+  const int tid = threadIdx.x, wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
+  int ti, tj;
+  {
+    int t = blockIdx.x;
+    tj = 0;
+    while (t >= p.nt - tj) { t -= p.nt - tj; ++tj; }
+    ti = tj + t;
+  }
+  const bool diag = ti == tj;
+  long long u_lo;
+  const long long nu = slice_units(p.n_units, p.n_slices, blockIdx.y, &u_lo);
+
+  // partial tile stored TRANSPOSED (mirror position, upper block triangle; gram_reduce_upper reads it):
+  // element (row R of tile I, column c of tile J) at Gp[(tj*128 + c) * m_pad + ti*128 + R]
+  double* gtile = p.Gpart + static_cast<size_t>(blockIdx.y) * p.m_pad * p.m_pad +
+                  static_cast<size_t>(tj * kTile) * p.m_pad + ti * kTile;
+  if (nu == 0) {   // empty slice: the partial tile must still be defined
+    if (!p.accumulate)
+      for (int e = tid; e < kTile * kTile; e += GTHREADS) gtile[static_cast<size_t>(e / kTile) * p.m_pad + (e % kTile)] = 0.0;
+    return;
+  }
+
+  if (tid == 0) {
+    for (int s = 0; s < GSTAGES; ++s) {
+      mbar_init(b_full + 8 * s, 1);
+      mbar_init(b_empty + 8 * s, 2);      // one arrival per consumer warpgroup
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (wg == 0) {   // ---- copy warpgroup: one thread streams the plane images of tiles I and J -------------------------
+    setmaxnreg_dec<COPY_REGS>();
+    if (tid == 0) {
+      const uint32_t bytes = diag ? TILE_PLANES : 2 * TILE_PLANES;
+      for (long long i = 0; i < nu; ++i) {
+        const int s = static_cast<int>(i % GSTAGES);
+        if (i >= GSTAGES) mbar_wait(b_empty + 8 * s, static_cast<uint32_t>(((i / GSTAGES) & 1) ^ 1));
+        const uint8_t* src = p.planes + static_cast<size_t>(u_lo + i) * p.nt * TILE_PLANES;
+        const uint32_t dst = s_st + s * 2 * TILE_PLANES;
+        mbar_expect_tx(b_full + 8 * s, bytes);
+        bulk_g2s(dst, src + static_cast<size_t>(ti) * TILE_PLANES, TILE_PLANES, b_full + 8 * s);
+        if (!diag) bulk_g2s(dst + TILE_PLANES, src + static_cast<size_t>(tj) * TILE_PLANES, TILE_PLANES, b_full + 8 * s);
+      }
+      // the consumers spin on the full barriers without a bound: waiting here for their release of the last stages
+      // keeps a copy that never lands a trap, not a hang
+      for (long long i = nu > GSTAGES ? nu - GSTAGES : 0; i < nu; ++i)
+        mbar_wait(b_empty + 8 * static_cast<int>(i % GSTAGES), static_cast<uint32_t>((i / GSTAGES) & 1));
+    }
+    return;
+  }
+
+  // ---- consumer warpgroups: rows 64 cw .. 64 cw + 63 of tile I against the 128 rows of tile J --------------------------
+  setmaxnreg_inc<MMA_REGS>();
+  const int cw = wg - 1;
+  // fragment coordinates of a wgmma m64n128 accumulator: element 4j+e sits at row r0 (+8 if e >= 2), column 8j + c0 + (e & 1)
+  const int r0 = 16 * wq + (lane >> 2), c0 = 2 * (lane & 3);
+  const int R = 64 * cw + r0;
+  int acc4[64], acc3[64], acc2[64];    // restarted (not zeroed) by the first MMAs after each fold
+  int until_flush = FLUSH_UNITS;
+  bool first_flush = !p.accumulate, fresh = true;
+
+  for (long long i = 0; i < nu; ++i) {
+    const int s = static_cast<int>(i % GSTAGES);
+    mbar_wait_spin(b_full + 8 * s, static_cast<uint32_t>((i / GSTAGES) & 1));
+    const uint32_t st = s_st + s * 2 * TILE_PLANES;
+    const uint32_t a_base = st + cw * 4096;                    // 64 rows of the I planes
+    const uint32_t b_base = diag ? st : st + TILE_PLANES;      // all 128 rows of the J planes
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {   // 2 k-steps of 32 points
+      const uint64_t A0 = desc_sw64(a_base + 32 * ks), A1 = desc_sw64(a_base + PLANE + 32 * ks),
+                     A2 = desc_sw64(a_base + 2 * PLANE + 32 * ks);
+      const uint64_t B0 = desc_sw64(b_base + 32 * ks), B1 = desc_sw64(b_base + PLANE + 32 * ks),
+                     B2 = desc_sw64(b_base + 2 * PLANE + 32 * ks);
+      const int acc = (ks == 0 && fresh) ? 0 : 1;
+      wgmma_uu(acc4, A2, B2, acc);              // weight 2^32 : P2'P2
+      wgmma_us(acc3, A2, B1, acc);              // weight 2^24 : P2'P1 + P1'P2
+      wgmma_su(acc3, A1, B2, 1);
+      wgmma_us(acc2, A2, B0, acc);              // weight 2^16 : P2'P0 + P0'P2 + P1'P1
+      wgmma_su(acc2, A0, B2, 1);
+      wgmma_ss(acc2, A1, B1, 1);
+    }
+    wg_commit();
+    fresh = false;
+    wg_wait<1>();                               // the MMAs of unit i-1 are done: release its stage
+    if (i >= 1 && (tid & 127) == 0) mbar_arrive(b_empty + 8 * static_cast<int>((i - 1) % GSTAGES));
+
+    if (--until_flush == 0 || i == nu - 1) {
+      // ---- fold the exact int32 accumulators into the fp64 partial tile -----------------------------------------
+      until_flush = FLUSH_UNITS;
+      wg_wait<0>();
+      // the row stride, read through an opaque move: the 32 column addresses are formed here, not hoisted out of the
+      // unit loop into registers the accumulators need
+      uint32_t ld;
+      asm volatile("mov.b32 %0, %1;" : "=r"(ld) : "r"(static_cast<uint32_t>(p.m_pad)));
+      double* const trow = gtile + R;
+#pragma unroll
+      for (int e = 0; e < 64; ++e) {
+        const int c = 8 * (e >> 2) + c0 + (e & 1);
+        const double v = p.gscale * (4294967296.0 * static_cast<double>(acc4[e]) + 16777216.0 * static_cast<double>(acc3[e]) +
+                                     65536.0 * static_cast<double>(acc2[e]));
+        double* dst = trow + static_cast<size_t>(c) * ld + ((e & 2) ? 8 : 0);
+        if (first_flush) *dst = v;
+        else *dst += v;
+      }
+      first_flush = false;
+      fresh = true;
+    }
+  }
+  if ((tid & 127) == 0) mbar_arrive(b_empty + 8 * static_cast<int>((nu - 1) % GSTAGES));   // the last unit's stage
+}
+
 }  // namespace
 
-// Point slices of one launch: the grid has 2 * nt(nt+1)/2 CTAs per slice, one CTA per SM; pick the slice count (<= 16)
-// that minimises (waves x units per slice).
+// Point slices of one launch: pick the slice count (<= 16) that minimises (waves x units per slice), counting two CTA
+// slots per tile of the upper block triangle.  The Gram kernel runs one CTA per tile, so its grid is half that count:
+// configs[1] (m_pad = 1024) gets 11 slices x 36 tiles = 396 CTAs, three full waves on 132 SMs.
 int i8_slices(int m_pad, int num_sms, long long n_units) {
   const int nt = m_pad / kTile;
   const long long ctas = static_cast<long long>(nt) * (nt + 1);
@@ -349,16 +403,18 @@ int i8_slices(int m_pad, int num_sms, long long n_units) {
   return best;
 }
 
-cudaError_t launch_gram_i8(const uint8_t* Xt, const float* ys, const uint8_t* Zt, long long n, int d, int m_pad,
-                           int n_slices, const I8Direct& direct, double* Gpart, double* bpart, double C, float* dbg_T,
-                           uint32_t* dbg_w, cudaStream_t s) {
-  I8Params p{};
+cudaError_t launch_i8_planes(const uint8_t* Xt, const float* ys, const uint8_t* Zt, long long n_units, int d, int m_pad,
+                             int n_slices, const I8Direct& direct, double C, bool accumulate, uint8_t* planes,
+                             double* bpart, float* dbg_T, uint32_t* dbg_w, cudaStream_t s) {
+  PlaneParams p{};
   const int dp = (d + 15) / 16 * 16;
   p.Xt = Xt; p.ys = ys; p.Zt = Zt;
-  p.n_units = (n + UP - 1) / UP;
+  p.n_units = n_units;
   const int nchunks = i8_nchunks(d);    // 64-column K chunks of the distance contraction (1 or 2)
   p.m_pad = m_pad; p.nt = m_pad / kTile; p.n_slices = n_slices;
-  p.Gpart = Gpart; p.bpart = bpart;
+  p.planes = planes; p.bpart = bpart;
+  p.bscale = C;
+  p.accumulate = accumulate ? 1 : 0;
   p.dbg_T = dbg_T; p.dbg_w = dbg_w;
   p.xbytes = static_cast<uint32_t>(nchunks * XIMG_BYTES);
   p.zbytes = static_cast<uint32_t>(nchunks * ZPANEL_BYTES);
@@ -367,25 +423,36 @@ cudaError_t launch_gram_i8(const uint8_t* Xt, const float* ys, const uint8_t* Zt
     for (int t = 0; t < 4; ++t) p.w[t] = direct.w[t];
     p.xbytes = static_cast<uint32_t>(direct.n_terms * UP * direct.dpad4 * sizeof(float));
     p.zbytes = static_cast<uint32_t>(direct.n_terms * kTile * direct.dpad4 * sizeof(float));
-    C = direct.csum;
   }
-  p.gscale = C * C / (4.0 * static_cast<double>(C0) * static_cast<double>(C0));      // the planes are the digits of 2 u
-  p.bscale = C;
-  const long fixed = 1024 + 2L * p.zbytes + 2L * PLANES_BYTES + 8 * (XSTAGES_MAX + 1);
-  long xs = (static_cast<long>(kSmemOptInMax) - fixed) / static_cast<long>(p.xbytes + UP * 4);
-  if (xs > XSTAGES_MAX) xs = XSTAGES_MAX;
-  if (xs < 2) return cudaErrorInvalidConfiguration;
-  p.xstages = static_cast<int>(xs);
-  const size_t smem = fixed + xs * (p.xbytes + UP * 4);
-  const void* fn = direct.on ? reinterpret_cast<const void*>(kmn_gram_i8_wgmma_kernel<true, 0>)
-                   : (3 * dp + 16) / 16 == 4 ? reinterpret_cast<const void*>(kmn_gram_i8_wgmma_kernel<false, 4>)
-                                             : reinterpret_cast<const void*>(kmn_gram_i8_wgmma_kernel<false, 7>);
+  const size_t smem = 1024 + 2 * TILE_PLANES + p.zbytes + XSTAGES * (p.xbytes + UP * 4) + 8 * (XSTAGES + 1);
+  if (smem > kSmemOptInMax) return cudaErrorInvalidConfiguration;
+  const void* fn = direct.on ? reinterpret_cast<const void*>(kmn_i8_planes_kernel<true, 0>)
+                   : (3 * dp + 16) / 16 == 4 ? reinterpret_cast<const void*>(kmn_i8_planes_kernel<false, 4>)
+                                             : reinterpret_cast<const void*>(kmn_i8_planes_kernel<false, 7>);
   // per-device attribute: set on every launch (contexts on several GPUs may live in one process)
   cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
-  dim3 grid(p.nt * (p.nt + 1), n_slices);
+  dim3 grid(p.nt, n_slices);
   void* args[] = {&p};
   return cudaLaunchKernel(fn, grid, dim3(NTHREADS), args, smem, s);
+}
+
+cudaError_t launch_gram_i8(const uint8_t* planes, long long n_units, int m_pad, int n_slices, double C, bool accumulate,
+                           double* Gpart, cudaStream_t s) {
+  GramI8Params p{};
+  p.planes = planes;
+  p.n_units = n_units;
+  p.m_pad = m_pad; p.nt = m_pad / kTile; p.n_slices = n_slices;
+  p.Gpart = Gpart;
+  p.gscale = C * C / (4.0 * static_cast<double>(C0) * static_cast<double>(C0));      // the planes are the digits of 2 u
+  p.accumulate = accumulate ? 1 : 0;
+  const size_t smem = 1024 + GSTAGES * 2 * TILE_PLANES + 16 * GSTAGES;
+  const void* fn = reinterpret_cast<const void*>(gram_i8_kernel);
+  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  if (e != cudaSuccess) return e;
+  dim3 grid(p.nt * (p.nt + 1) / 2, n_slices);
+  void* args[] = {&p};
+  return cudaLaunchKernel(fn, grid, dim3(GTHREADS), args, smem, s);
 }
 
 }  // namespace sgp

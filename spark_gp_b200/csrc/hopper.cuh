@@ -37,11 +37,36 @@ __device__ __noinline__ inline void mbar_wait_slow(uint32_t bar, uint32_t parity
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (!mbar_try(bar, parity)) mbar_wait_slow(bar, parity);
 }
+// Unbounded spin, for loops that keep 192 accumulator registers live (the int8 Gram's consumer warpgroups): a call, a
+// clock read or a trap path there spills.  The thread that fills the barrier must then wait with mbar_wait for the
+// spinning threads' release, so that a copy that never lands still ends in its trap.
+__device__ __forceinline__ void mbar_wait_spin(uint32_t bar, uint32_t parity) {
+  while (!mbar_try(bar, parity)) {
+  }
+}
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads)
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// shared -> global bulk copy, tracked by the issuing thread's bulk groups
+__device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// warpgroup-wide register budget hand-over (every thread of the warpgroup executes it)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma operand reads, bulk stores)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_barrier(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
@@ -80,36 +105,32 @@ __device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t a, uint64
         "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(a), "l"(b), "r"(acc));
 }
-// D[64 x 32] (+)= A[64 x 16] B[32 x 16]^T
-__device__ __forceinline__ void wgmma_f16_n32(float (&d)[16], uint64_t a, uint64_t b, int acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b), "r"(acc));
-}
-
-// D[64 x 64] += A[64 x 32] B[64 x 32]^T, 8-bit integers (AT, BT = s8 or u8), exact int32 accumulation
-#define SGP_WGMMA_I8_N64(NAME, AT, BT)                                                                              \
-  __device__ __forceinline__ void NAME(int (&d)[32], uint64_t a, uint64_t b) {                                      \
+// D[64 x 128] (+)= A[64 x 32] B[128 x 32]^T, 8-bit integers (AT, BT = s8 or u8), exact int32 accumulation; acc = 0
+// overwrites D (no register moves needed to restart an accumulator)
+#define SGP_WGMMA_I8_N128(NAME, AT, BT)                                                                             \
+  __device__ __forceinline__ void NAME(int (&d)[64], uint64_t a, uint64_t b, int acc) {                             \
     asm volatile(                                                                                                   \
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"                                                           \
-        "wgmma.mma_async.sync.aligned.m64n64k32.s32." AT "." BT " "                                                 \
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                                         \
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32." AT "." BT " "                                                \
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                   \
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}"      \
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                          \
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                          \
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n\t}"      \
         : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),           \
           "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),     \
           "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),   \
-          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])    \
-        : "l"(a), "l"(b));                                                                                          \
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),   \
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),   \
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),   \
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),   \
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])    \
+        : "l"(a), "l"(b), "r"(acc));                                                                                \
   }
-SGP_WGMMA_I8_N64(wgmma_uu, "u8", "u8")
-SGP_WGMMA_I8_N64(wgmma_us, "u8", "s8")
-SGP_WGMMA_I8_N64(wgmma_su, "s8", "u8")
-SGP_WGMMA_I8_N64(wgmma_ss, "s8", "s8")
-#undef SGP_WGMMA_I8_N64
+SGP_WGMMA_I8_N128(wgmma_uu, "u8", "u8")
+SGP_WGMMA_I8_N128(wgmma_us, "u8", "s8")
+SGP_WGMMA_I8_N128(wgmma_su, "s8", "u8")
+SGP_WGMMA_I8_N128(wgmma_ss, "s8", "s8")
+#undef SGP_WGMMA_I8_N128
 
 }  // namespace hop
 }  // namespace sgp

@@ -32,6 +32,10 @@ constexpr int kTile = 128;        // edge of one G tile (active-set indices per 
 constexpr int kSMsH100 = 132;      // H100 SXM; the context reads the real count from the device
 constexpr size_t kSmemOptInMax = 227 * 1024;   // largest dynamic shared memory a CTA can opt in to (H100)
 constexpr int kMaxHypers = 72;     // hyper-parameters of one objective evaluation: 1 scale + 64 ARD betas + a few more
+// int8 Gram: three int8 digit planes of one active tile for one 64-point unit, and the largest plane workspace of one
+// launch window (3 bytes per point and padded active row: configs[1] 3.1 GB in one window, configs[3] 7.7 GB in two)
+constexpr size_t kI8PlaneBytes = 3 * kTile * 64;
+constexpr size_t kI8PlaneCapBytes = size_t(4) << 30;
 
 // Flattened, device-ready kernel description (built by sgp_stats_begin).
 struct KernelFlat {
@@ -118,6 +122,7 @@ struct Ctx {
   DevScratch i8_zd_ws;           // direct mode: active-set tiles [tile][term][dpad][128] fp32
   bool i8d_prepared = false;     // ... built in this begin() window (on the first direct-mode launch)
   DevScratch i8_xt_ws, i8_ys_ws; // point operand images / tiles and fp32 y (scratch)
+  DevScratch i8_planes_ws;       // digit planes of one launch window (at most kI8PlaneCapBytes)
   int* dI8Flags = nullptr;       // [0] the window's int8 status, [1] the active set's (begin), [2] the K_nm sweep's
                                  // (reset to [1] by each host-form call); bit 0: scaled squared norm above
                                  // kI8TensorR2Max; bit 2: above kI8DirectR2Max
@@ -210,11 +215,17 @@ struct I8Direct {
   double csum = 0.0;     // sum of the term scales = the fixed-point scale
 };
 
-// int8 Gram kernel (gram_i8_wgmma.cu): point slices per launch, and one launch over every tile of the upper block triangle
+// int8 Gram (gram_i8_wgmma.cu).  A launch window over n_units 64-point units is two kernels: the digit-plane producer
+// (kernel elements, their fixed-point digit planes in the workspace [n_units][m_pad / kTile][kI8PlaneBytes], and the
+// b partials) and the int8 Gram over the workspace (partial tiles of the upper block triangle).  accumulate = false:
+// the window stores its partials (first window of a call); true: it adds to them.  C: the fixed-point scale (the term
+// scale, or the sum of the term scales in direct mode).
 int i8_slices(int m_pad, int num_sms, long long n_units);
-cudaError_t launch_gram_i8(const uint8_t* Xt, const float* ys, const uint8_t* Zt, long long n, int d, int m_pad,
-                           int n_slices, const I8Direct& direct, double* Gpart, double* bpart, double C, float* dbg_T,
-                           uint32_t* dbg_w, cudaStream_t s);
+cudaError_t launch_i8_planes(const uint8_t* Xt, const float* ys, const uint8_t* Zt, long long n_units, int d, int m_pad,
+                             int n_slices, const I8Direct& direct, double C, bool accumulate, uint8_t* planes,
+                             double* bpart, float* dbg_T, uint32_t* dbg_w, cudaStream_t s);
+cudaError_t launch_gram_i8(const uint8_t* planes, long long n_units, int m_pad, int n_slices, double C, bool accumulate,
+                           double* Gpart, cudaStream_t s);
 
 // K_nm sweep (kmn_sweep.cu): fp32 cross kernel of a block of points, row-major n x m
 cudaError_t launch_kmn_sweep(const uint8_t* Xt, const uint8_t* Zt, long long n, int d, int m, int m_pad, int num_sms, double C,
