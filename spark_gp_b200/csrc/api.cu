@@ -211,7 +211,7 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   const int i8_n_slices = c->i8_direct_ok ? i8_slices(c->m_pad, c->num_sms, win_units) : 1;
   const int max_slices = n_slices > i8_n_slices ? n_slices : i8_n_slices;
   int rc = ctx_scratch(c, c->gpart_ws, static_cast<size_t>(max_slices) * c->m_pad * c->m_pad * sizeof(double));
-  if (rc == SGP_OK) rc = ctx_scratch(c, c->bpart_ws, static_cast<size_t>(max_slices) * c->m_pad * sizeof(double));
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->bpart_ws, static_cast<size_t>(n_slices) * c->m_pad * sizeof(double));
   if (rc != SGP_OK) return rc;
 
   // AUTO: the int8 kernel inside its measured parity envelope -- accumulate calls of >= 32768 points (posterior
@@ -295,7 +295,6 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   SGP_CUDA(c, cudaEventRecord(e0, c->stream));
   const size_t mm = static_cast<size_t>(c->m) * c->m;
   double* Gpart = c->gpart_ws.as<double>();
-  double* bpart = c->bpart_ws.as<double>();
   if (path != 0) {
     I8Direct direct;
     if (path == 2) {
@@ -307,6 +306,12 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
     }
     const double C = (path == 2) ? direct.csum : c->kf.scale[0];
     const uint8_t* zop = (path == 2) ? c->i8_zd_ws.as<uint8_t>() : c->dI8Zt;
+    // the producer's own point slices (its b partials): a grid that fills the SMs at the variant's occupancy
+    int plane_slices = 1;
+    SGP_CUDA(c, i8_plane_slices(c->m_pad, c->num_sms, win_units, c->d, direct, &plane_slices));
+    rc = ctx_scratch(c, c->bpart_ws, static_cast<size_t>(plane_slices) * c->m_pad * sizeof(double));
+    if (rc != SGP_OK) return rc;
+    double* bpart = c->bpart_ws.as<double>();
     // per window: digit planes + b partials, then the Gram over them; the first window stores the slice partials,
     // later ones add to them, and one deterministic slice reduction follows
     for (long long w = 0; w < n_windows; ++w) {
@@ -314,15 +319,15 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
       const long long nu = std::min(win_units, n_units - u0);
       SGP_CUDA(c, launch_i8_planes(c->i8_xt_ws.as<uint8_t>() + static_cast<size_t>(u0) * x_unit,
                                    c->i8_ys_ws.as<float>() + static_cast<size_t>(u0) * 64, zop, nu, c->d, c->m_pad,
-                                   i8_n_slices, direct, C, w > 0, c->i8_planes_ws.as<uint8_t>(), bpart,
+                                   plane_slices, direct, C, w > 0, c->i8_planes_ws.as<uint8_t>(), bpart,
                                    w == 0 ? c->dbgT : nullptr, w == 0 ? c->dbgW : nullptr, c->stream));
       SGP_CUDA(c, launch_gram_i8(c->i8_planes_ws.as<uint8_t>(), nu, c->m_pad, i8_n_slices, C, w > 0, Gpart, c->stream));
       c->launches += 2;
     }
     SGP_CUDA(c, cudaEventRecord(e1, c->stream));
     // deterministic slice reduction (partial tiles at the mirror position: upper block triangle)
-    SGP_CUDA(c, launch_gram_reduce_upper(c->dGb, c->dGb + mm, Gpart, bpart, i8_n_slices, c->m, c->m_pad, 0, c->m,
-                                         c->stream));
+    SGP_CUDA(c, launch_gram_reduce_upper(c->dGb, c->dGb + mm, Gpart, bpart, i8_n_slices, plane_slices, c->m, c->m_pad, 0,
+                                         c->m, c->stream));
     c->launches += 1;
     return SGP_OK;
   }
@@ -332,6 +337,7 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   p.n_terms = c->kf.n_terms;
   for (int t = 0; t < kMaxTerms; ++t) p.scale[t] = c->kf.scale[t];
   p.Zs = c->dZc; p.beta = c->dBeta;
+  double* bpart = c->bpart_ws.as<double>();
   p.Gpart = Gpart; p.bpart = bpart;
   p.n_slices = n_slices; p.n_tiles_1d = nt1;
   SGP_CUDA(c, launch_gram_f64(p, c->precision == SGP_PREC_F64_STRICT, c->stream));

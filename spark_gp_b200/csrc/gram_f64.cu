@@ -403,35 +403,35 @@ __global__ void gram_reduce_kernel(double* __restrict__ G, double* __restrict__ 
 
 // Same for partial tiles stored at the MIRROR position (upper block triangle; the int8 kernel folds its accumulators
 // transposed so that its global writes coalesce): G[i][j] (+ mirror) += sum_s Gpart[s][i][j] for rows i in [row_lo, row_hi),
-// j >= i.
+// j >= i.  The int8 Gram and its digit-plane producer split the points into different slice counts.
 __global__ void gram_reduce_upper_kernel(double* __restrict__ G, double* __restrict__ b,
                                          const double* __restrict__ Gpart, const double* __restrict__ bpart,
-                                         int n_slices, int m, int m_pad, int row_lo, int row_hi) {
+                                         int g_slices, int b_slices, int m, int m_pad, int row_lo, int row_hi) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const int i = row_lo + blockIdx.y * blockDim.y + threadIdx.y;
   if (i < row_hi && j < m && j >= i) {
     double v = 0.0;
     const size_t stride = static_cast<size_t>(m_pad) * m_pad;
-    for (int s = 0; s < n_slices; ++s) v += Gpart[s * stride + static_cast<size_t>(i) * m_pad + j];
+    for (int s = 0; s < g_slices; ++s) v += Gpart[s * stride + static_cast<size_t>(i) * m_pad + j];
     G[static_cast<size_t>(i) * m + j] += v;
     if (i != j) G[static_cast<size_t>(j) * m + i] += v;
   }
   if (blockIdx.y == 0 && threadIdx.y == 0 && j >= row_lo && j < row_hi) {
     double v = 0.0;
-    for (int s = 0; s < n_slices; ++s) v += bpart[static_cast<size_t>(s) * m_pad + j];
+    for (int s = 0; s < b_slices; ++s) v += bpart[static_cast<size_t>(s) * m_pad + j];
     b[j] += v;
   }
 }
 
 }  // namespace
 
-cudaError_t launch_gram_reduce_upper(double* G, double* b, const double* Gpart, const double* bpart, int n_slices, int m,
-                                     int m_pad, int row_lo, int row_hi, cudaStream_t s) {
+cudaError_t launch_gram_reduce_upper(double* G, double* b, const double* Gpart, const double* bpart, int g_slices,
+                                     int b_slices, int m, int m_pad, int row_lo, int row_hi, cudaStream_t s) {
   if (row_hi > m) row_hi = m;
   if (row_hi <= row_lo) return cudaSuccess;
   dim3 block(32, 8);
   dim3 grid((m + 31) / 32, (row_hi - row_lo + 7) / 8);
-  gram_reduce_upper_kernel<<<grid, block, 0, s>>>(G, b, Gpart, bpart, n_slices, m, m_pad, row_lo, row_hi);
+  gram_reduce_upper_kernel<<<grid, block, 0, s>>>(G, b, Gpart, bpart, g_slices, b_slices, m, m_pad, row_lo, row_hi);
   return cudaGetLastError();
 }
 

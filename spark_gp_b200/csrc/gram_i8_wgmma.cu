@@ -30,6 +30,8 @@
 //              the accumulators are folded into the fp64 partial tile (no overflow possible).
 #include <cuda_fp16.h>
 
+#include <algorithm>
+
 #include "hopper.cuh"
 #include "sgp_internal.h"
 
@@ -72,7 +74,7 @@ __device__ __forceinline__ void store_digits(uint8_t* planes, int plane_bytes, i
   *reinterpret_cast<uint16_t*>(planes + 2 * plane_bytes + off) = static_cast<uint16_t>(prmt(w0, w1, 0x0062));         // P2
 }
 
-// units [u_lo, u_lo + nu) of point slice `slice` (the producer and the Gram split a launch identically)
+// units [u_lo, u_lo + nu) of point slice `slice` of n_slices (the producer and the Gram each split a launch their own way)
 __device__ __forceinline__ long long slice_units(long long n_units, int n_slices, int slice, long long* u_lo) {
   const long long ups = (n_units + n_slices - 1) / n_slices;
   *u_lo = ups * slice;
@@ -387,7 +389,7 @@ __global__ void __launch_bounds__(GTHREADS, 1) gram_i8_kernel(const GramI8Params
 
 }  // namespace
 
-// Point slices of one launch: pick the slice count (<= 16) that minimises (waves x units per slice), counting two CTA
+// Point slices of the Gram: pick the slice count (<= 16) that minimises (waves x units per slice), counting two CTA
 // slots per tile of the upper block triangle.  The Gram kernel runs one CTA per tile, so its grid is half that count:
 // configs[1] (m_pad = 1024) gets 11 slices x 36 tiles = 396 CTAs, three full waves on 132 SMs.
 int i8_slices(int m_pad, int num_sms, long long n_units) {
@@ -403,32 +405,61 @@ int i8_slices(int m_pad, int num_sms, long long n_units) {
   return best;
 }
 
+namespace {
+// the producer variant of a launch: its kernel, point and active-tile image bytes, and dynamic shared memory
+const void* plane_kernel(int d, const I8Direct& direct, uint32_t* xbytes, uint32_t* zbytes, size_t* smem) {
+  const int nchunks = i8_nchunks(d);    // 64-column K chunks of the distance contraction (1 or 2)
+  *xbytes = static_cast<uint32_t>(nchunks * XIMG_BYTES);
+  *zbytes = static_cast<uint32_t>(nchunks * ZPANEL_BYTES);
+  if (direct.on) {
+    *xbytes = static_cast<uint32_t>(direct.n_terms * UP * direct.dpad4 * sizeof(float));
+    *zbytes = static_cast<uint32_t>(direct.n_terms * kTile * direct.dpad4 * sizeof(float));
+  }
+  *smem = 1024 + 2 * TILE_PLANES + *zbytes + XSTAGES * (*xbytes + UP * 4) + 8 * (XSTAGES + 1);
+  const int dp = (d + 15) / 16 * 16;
+  return direct.on ? reinterpret_cast<const void*>(kmn_i8_planes_kernel<true, 0>)
+         : (3 * dp + 16) / 16 == 4 ? reinterpret_cast<const void*>(kmn_i8_planes_kernel<false, 4>)
+                                   : reinterpret_cast<const void*>(kmn_i8_planes_kernel<false, 7>);
+}
+}  // namespace
+
+// Point slices of the producer: the planes are indexed by global unit, so its split need not match the Gram's.  The
+// grid (active tiles x slices) is the largest that runs in one wave at the occupancy the variant's shared memory allows:
+// configs[1] (8 tiles, d = 16: two CTAs per SM) gets 33 slices = 264 CTAs on 132 SMs, where the Gram's split gave 88.
+cudaError_t i8_plane_slices(int m_pad, int num_sms, long long n_units, int d, const I8Direct& direct, int* n_slices) {
+  uint32_t xbytes, zbytes;
+  size_t smem;
+  const void* fn = plane_kernel(d, direct, &xbytes, &zbytes, &smem);
+  if (smem > kSmemOptInMax) return cudaErrorInvalidConfiguration;
+  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  if (e != cudaSuccess) return e;
+  int per_sm = 0;
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, NTHREADS, smem);
+  if (e != cudaSuccess) return e;
+  if (per_sm < 1) return cudaErrorInvalidConfiguration;
+  const long long s = std::min<long long>(static_cast<long long>(num_sms) * per_sm / (m_pad / kTile), n_units);
+  *n_slices = static_cast<int>(std::max<long long>(s, 1));
+  return cudaSuccess;
+}
+
 cudaError_t launch_i8_planes(const uint8_t* Xt, const float* ys, const uint8_t* Zt, long long n_units, int d, int m_pad,
                              int n_slices, const I8Direct& direct, double C, bool accumulate, uint8_t* planes,
                              double* bpart, float* dbg_T, uint32_t* dbg_w, cudaStream_t s) {
   PlaneParams p{};
-  const int dp = (d + 15) / 16 * 16;
   p.Xt = Xt; p.ys = ys; p.Zt = Zt;
   p.n_units = n_units;
-  const int nchunks = i8_nchunks(d);    // 64-column K chunks of the distance contraction (1 or 2)
   p.m_pad = m_pad; p.nt = m_pad / kTile; p.n_slices = n_slices;
   p.planes = planes; p.bpart = bpart;
   p.bscale = C;
   p.accumulate = accumulate ? 1 : 0;
   p.dbg_T = dbg_T; p.dbg_w = dbg_w;
-  p.xbytes = static_cast<uint32_t>(nchunks * XIMG_BYTES);
-  p.zbytes = static_cast<uint32_t>(nchunks * ZPANEL_BYTES);
   if (direct.on) {
     p.n_terms = direct.n_terms; p.dpad4 = direct.dpad4;
     for (int t = 0; t < 4; ++t) p.w[t] = direct.w[t];
-    p.xbytes = static_cast<uint32_t>(direct.n_terms * UP * direct.dpad4 * sizeof(float));
-    p.zbytes = static_cast<uint32_t>(direct.n_terms * kTile * direct.dpad4 * sizeof(float));
   }
-  const size_t smem = 1024 + 2 * TILE_PLANES + p.zbytes + XSTAGES * (p.xbytes + UP * 4) + 8 * (XSTAGES + 1);
+  size_t smem;
+  const void* fn = plane_kernel(d, direct, &p.xbytes, &p.zbytes, &smem);
   if (smem > kSmemOptInMax) return cudaErrorInvalidConfiguration;
-  const void* fn = direct.on ? reinterpret_cast<const void*>(kmn_i8_planes_kernel<true, 0>)
-                   : (3 * dp + 16) / 16 == 4 ? reinterpret_cast<const void*>(kmn_i8_planes_kernel<false, 4>)
-                                             : reinterpret_cast<const void*>(kmn_i8_planes_kernel<false, 7>);
   // per-device attribute: set on every launch (contexts on several GPUs may live in one process)
   cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;

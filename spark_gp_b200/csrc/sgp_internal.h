@@ -165,8 +165,8 @@ int fail(Ctx* c, int code, const std::string& msg);
 cudaError_t launch_gram_f64(const GramParams& p, bool strict_elements, cudaStream_t s);
 cudaError_t launch_gram_reduce(double* G /*m x m*/, double* b, const double* Gpart, const double* bpart,
                                int n_slices, int m, int m_pad, cudaStream_t s);
-cudaError_t launch_gram_reduce_upper(double* G, double* b, const double* Gpart, const double* bpart, int n_slices, int m,
-                                     int m_pad, int row_lo, int row_hi, cudaStream_t s);
+cudaError_t launch_gram_reduce_upper(double* G, double* b, const double* Gpart, const double* bpart, int g_slices,
+                                     int b_slices, int m, int m_pad, int row_lo, int row_hi, cudaStream_t s);
 // same, restricted to the G columns / b entries [col_lo, col_hi) (one int8 launch covers whole tile columns)
 cudaError_t launch_gram_reduce_cols(double* G, double* b, const double* Gpart, const double* bpart, int n_slices, int m,
                                     int m_pad, int col_lo, int col_hi, cudaStream_t s);
@@ -219,8 +219,10 @@ struct I8Direct {
 // (kernel elements, their fixed-point digit planes in the workspace [n_units][m_pad / kTile][kI8PlaneBytes], and the
 // b partials) and the int8 Gram over the workspace (partial tiles of the upper block triangle).  accumulate = false:
 // the window stores its partials (first window of a call); true: it adds to them.  C: the fixed-point scale (the term
-// scale, or the sum of the term scales in direct mode).
+// scale, or the sum of the term scales in direct mode).  The two kernels split a window into point slices of their own:
+// i8_slices for the Gram (its G partials), i8_plane_slices for the producer (its b partials).
 int i8_slices(int m_pad, int num_sms, long long n_units);
+cudaError_t i8_plane_slices(int m_pad, int num_sms, long long n_units, int d, const I8Direct& direct, int* n_slices);
 cudaError_t launch_i8_planes(const uint8_t* Xt, const float* ys, const uint8_t* Zt, long long n_units, int d, int m_pad,
                              int n_slices, const I8Direct& direct, double C, bool accumulate, uint8_t* planes,
                              double* bpart, float* dbg_T, uint32_t* dbg_w, cudaStream_t s);

@@ -4,19 +4,23 @@
 Workloads: bench.py's configs[1] shard (1M x 16, m = 1000) in both int8 modes and configs[3]'s per-GPU shard
 (1.25M x 32, m = 2000).  Bounds: the producer against HBM (planes written + point images read, 3.35 TB/s), the Gram
 against the int8 tensor rate (6 products of 128 x 128 x 64 per tile pair and unit, 1979 TOPS dense); both are H100 SXM
-data-sheet figures for a 700 W card."""
+data-sheet figures for a 700 W card.  producer_ctas: the producer's grid, tiles x its own point slices
+(tests/test_host_i8_launch.py mirrors the rule)."""
 import json
 import os
 import subprocess
 import sys
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np
 import torch
 from torch.profiler import ProfilerActivity, profile
 
 import spark_gp_b200 as sg
 from spark_gp_b200 import _native as N
+from test_host_i8_launch import plane_slices, plane_smem
 
 HBM_GBS, I8_TOPS = 3350.0, 1979.0
 PLANE_BYTES = 3 * 128 * 64
@@ -59,9 +63,12 @@ def run(name, n, d, m, mode, steps=3):
     prod_bytes = units * nt * PLANE_BYTES + xbytes + n * 4
     gram_ops = nt * (nt + 1) // 2 * units * 6 * 2.0 * 128 * 128 * 64
     l2_bytes = units * (nt * (nt - 1) // 2 * 2 + nt) * PLANE_BYTES
+    smem = plane_smem(d) if mode == N.SGP_PREC_I8 else plane_smem(d, (1, -(-d // 4) * 4))
+    producer_ctas = nt * plane_slices(nt * 128, torch.cuda.get_device_properties(0).multi_processor_count, units, smem)
     out = {"name": name, "n": n, "d": d, "m": m, "mode": {N.SGP_PREC_I8: "i8", N.SGP_PREC_I8_DIRECT: "i8_direct"}[mode],
            "producer_ms": t.get("producer"), "gram_ms": t.get("gram"), "device_bytes_held_by_library": held,
-           "producer_hbm_bytes": prod_bytes, "gram_int8_ops": gram_ops, "gram_l2_to_sm_bytes": l2_bytes}
+           "producer_hbm_bytes": prod_bytes, "gram_int8_ops": gram_ops, "gram_l2_to_sm_bytes": l2_bytes,
+           "producer_ctas": producer_ctas}
     if t.get("producer"):
         out["producer_GBs"] = prod_bytes / t["producer"] / 1e6
         out["producer_frac_of_hbm"] = out["producer_GBs"] / HBM_GBS
