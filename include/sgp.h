@@ -223,6 +223,23 @@ int sgp_debug_i8_tile(sgp_ctx* ctx, float* T_out /* 128*64 */, uint32_t* w_out /
 int sgp_greedy_active_set(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const double* X, const double* y, int64_t n,
                           int32_t d, int64_t n_experts, int64_t first_index, int32_t m_target, int64_t* indices_out);
 
+/* KMeansActiveSetProvider (commons/ActiveSetProvider.scala:22-46): Spark 3.1 MLlib KMeans with the reference's settings
+ * (k-means|| seeding with 2 steps, Euclidean distance, unit weights; DESIGN.md 4.7 restates the algorithm).  X: n x d
+ * row-major in HOST memory, fp64 or fp32 (x_is_f32 != 0), uploaded once.  init_centers (k x d fp64) replaces the seeding
+ * (mllib's setInitialModel); NULL: k-means|| from `seed` through the library's counter-based generator (Spark's
+ * XORShift streams depend on the partitioning and are not reproduced).  Lloyd runs until max_iter iterations or until
+ * every non-empty cluster moved by at most tol (squared distance <= tol^2); an empty cluster keeps its centre.
+ * Outputs (host): centers_out (k_out x d; k_out < k when the data have fewer distinct points), labels_out (n, or NULL)
+ * and cost_out (sum of squared distances) of the last assignment pass -- against the centres before the last update, as
+ * Spark's trainingCost --, iterations_out.  Distances are fp32 direct form on points and centres shifted by a common
+ * origin in fp64; centre sums are fp64 in point order: two calls return identical bits.  Errors: SGP_E_BADARG for k < 2,
+ * max_iter < 0, tol < 0 or NaN, n < 1, d < 1, n > 2^31 - 1 and NaN / infinity in X.  Works outside any begin..finish
+ * window and leaves an open window's statistics untouched; rank-local (no communicator). */
+int sgp_kmeans(sgp_ctx* ctx, const void* X, int32_t x_is_f32, int64_t n, int32_t d, int32_t k, int32_t max_iter,
+               double tol, int64_t seed, const double* init_centers /* k x d, or NULL: k-means|| */,
+               double* centers_out /* k x d */, int32_t* k_out, int32_t* labels_out /* n, or NULL */,
+               int32_t* iterations_out, double* cost_out);
+
 /* Evaluate K(X_test, Z) (n x m row-major fp64 out) with the current kernel -- the `crossKernel`
  * contract of kernel/Kernel.scala:69-74 (used by the golden-vector tests). */
 int sgp_cross_kernel(sgp_ctx* ctx, const double* X, int64_t n, double* K_out);

@@ -230,5 +230,25 @@ JNIEXPORT jlongArray JNICALL Java_org_apache_spark_ml_commons_NativeProjectedPro
   return res;
 }
 
+// KMeansActiveSetProvider (ActiveSetProvider.scala:22-46) on the collected points x (n x d row-major): Spark 3.1 MLlib KMeans
+// (k-means|| + Lloyd, tol 1e-4) on the device, sgp_kmeans.  Returns k_out x d centres row-major (k_out < k when the data
+// have fewer distinct points).
+JNIEXPORT jdoubleArray JNICALL Java_org_apache_spark_ml_commons_NativeProjectedProcess_kmeansActiveSet(
+    JNIEnv* env, jclass, jlong h, jdoubleArray X, jlong n, jint d, jint k, jint maxIter, jlong seed) {
+  sgp_ctx* ctx = reinterpret_cast<sgp_ctx*>(h);
+  jdouble* xx = env->GetDoubleArrayElements(X, nullptr);
+  std::vector<double> centres(static_cast<size_t>(k > 0 ? k : 0) * (d > 0 ? d : 0));
+  int32_t k_out = 0, iterations = 0;
+  double cost = 0.0;
+  const int rc = sgp_kmeans(ctx, xx, /*x_is_f32=*/0, n, d, k, maxIter, 1e-4, seed, nullptr, centres.data(), &k_out, nullptr,
+                            &iterations, &cost);
+  env->ReleaseDoubleArrayElements(X, xx, JNI_ABORT);
+  if (rc != SGP_OK) { throw_for(env, ctx, rc); return nullptr; }
+  const jsize len = static_cast<jsize>(k_out) * d;
+  jdoubleArray res = env->NewDoubleArray(len);
+  env->SetDoubleArrayRegion(res, 0, len, centres.data());
+  return res;
+}
+
 }  // extern "C"
 #endif  // __has_include(<jni.h>)

@@ -34,6 +34,9 @@ private[ml] object NativeProjectedProcess {
   @native def greedyActiveSet(ctx: Long, types: Array[Int], scales: Array[Double], sigmas: Array[Double],
                               betas: Array[Double], x: Array[Double], y: Array[Double], n: Long, d: Int, nExperts: Long,
                               firstIndex: Long, activeSetSize: Int): Array[Long]
+  /** Centres (k_out x d row-major) of Spark 3.1 MLlib KMeans with the reference's settings (k-means||, tol 1e-4) over the
+    * n points of x (row-major, d columns), computed on the device (sgp_kmeans). */
+  @native def kmeansActiveSet(ctx: Long, x: Array[Double], n: Long, d: Int, k: Int, maxIter: Int, seed: Long): Array[Double]
 
   /** Flattens the kernel DSL tree into (type, scale, sigma, beta) terms; `scale` multiplies down the tree
     * (ScalarTimesKernel.scala:20-28), Eye terms are kept (they carry whiteNoiseVar / the K_mm diagonal). */
@@ -75,6 +78,26 @@ private[ml] object NativeProjectedProcess {
       terms.flatMap(_._4).toArray, d, hs.map(_.kind).toArray, hs.map(_.term).toArray, hs.map(_.dim).toArray,
       hs.map(_.value).toArray, coef, tol)
     (out(0), new BDV(out.drop(1)))
+  }
+}
+
+/** Drop-in for KMeansActiveSetProvider (ActiveSetProvider.scala:22-46): the points are collected to the driver and
+  * clustered on its GPU in one native call instead of Spark MLlib's distributed KMeans (same algorithm and settings;
+  * Spark's partition-dependent RNG streams are replaced by the library's counter-based generator). */
+class NativeKMeansActiveSetProvider(private val maxIter: Int = 20, device: Int = 0) extends ActiveSetProvider {
+  override def apply(activeSetSize: Int,
+                     expertLabelsAndKernels: RDD[(BDV[Double], Kernel)],
+                     points: RDD[org.apache.spark.ml.feature.LabeledPoint],
+                     kernel: () => Kernel,
+                     optimalHyperparameter: BDV[Double],
+                     seed: Long): Array[Vector] = {
+    val rows = points.map(_.features.toArray).collect()
+    val d = rows.head.length
+    val ctx = NativeProjectedProcess.create(device)
+    try {
+      val c = NativeProjectedProcess.kmeansActiveSet(ctx, rows.flatten, rows.length.toLong, d, activeSetSize, maxIter, seed)
+      c.grouped(d).map(r => org.apache.spark.ml.linalg.Vectors.dense(r): Vector).toArray
+    } finally NativeProjectedProcess.destroy(ctx)
   }
 }
 

@@ -22,7 +22,7 @@ EXPORTS = ["sgp_ctx_create", "sgp_ctx_destroy", "sgp_last_error", "sgp_set_preci
            "sgp_stats_accumulate_device", "sgp_stats_finish", "sgp_sync", "sgp_magic", "sgp_predict",
            "sgp_launch_count", "sgp_gram_kernel_time", "sgp_cross_kernel", "sgp_event_record",
            "sgp_event_elapsed_ms", "sgp_debug_i8_tile", "sgp_last_path", "sgp_experts_upload",
-           "sgp_bcm_nll", "sgp_laplace_nll", "sgp_experts_get_f", "sgp_set_magic", "sgp_last_tail_path", "sgp_last_bcm_path", "sgp_experts_upload_grouped", "sgp_kmn_sweep", "sgp_kmn_sweep_device", "sgp_greedy_active_set"]
+           "sgp_bcm_nll", "sgp_laplace_nll", "sgp_experts_get_f", "sgp_set_magic", "sgp_last_tail_path", "sgp_last_bcm_path", "sgp_experts_upload_grouped", "sgp_kmn_sweep", "sgp_kmn_sweep_device", "sgp_greedy_active_set", "sgp_kmeans"]
 
 
 class KernelTerm(C.Structure):
@@ -75,6 +75,7 @@ def load() -> C.CDLL:
     lib.sgp_gram_kernel_time.argtypes = [vp, dp, C.POINTER(i64)]
     lib.sgp_cross_kernel.argtypes = [vp, vp, i64, vp]
     lib.sgp_greedy_active_set.argtypes = [vp, vp, vp, vp, i64, C.c_int32, i64, i64, C.c_int32, vp]
+    lib.sgp_kmeans.argtypes = [vp, vp, i32, i64, i32, i32, i32, C.c_double, i64, vp, vp, vp, vp, vp, vp]
     lib.sgp_event_record.argtypes = [vp, C.c_int]
     lib.sgp_debug_i8_tile.argtypes = [vp, vp, vp]
     lib.sgp_last_path.argtypes = [vp]

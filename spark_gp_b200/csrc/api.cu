@@ -416,7 +416,8 @@ int sgp_ctx_destroy(sgp_ctx* h) {
   }
   if (c->comm && nccl().ok) nccl().CommDestroy(c->comm);
   for (DevScratch* s : {&c->gpart_ws, &c->bpart_ws, &c->i8_zd_ws, &c->i8_xt_ws, &c->i8_ys_ws, &c->i8_planes_ws,
-                        &c->nll_per_ws, &c->hyper_ws, &c->greedy_ws, &c->sweep_ws, &c->bcm_ws, &c->tail_ws, &c->tail_ws2,
+                        &c->nll_per_ws, &c->hyper_ws, &c->greedy_ws, &c->kmeans_pts_ws, &c->kmeans_cen_ws, &c->kmeans_new_ws,
+                        &c->kmeans_cand_ws, &c->sweep_ws, &c->bcm_ws, &c->tail_ws, &c->tail_ws2,
                         &c->predict_ws, &c->cross_ws})
     cudaFree(s->p);
   if (c->tail_fork) cudaEventDestroy(c->tail_fork);
@@ -1057,6 +1058,27 @@ int sgp_greedy_active_set(sgp_ctx* h, const sgp_kernel_desc* k, const double* X,
   if (rc != SGP_OK) return rc;
   static_assert(sizeof(long long) == sizeof(int64_t), "index type");
   return run_greedy(c, kf, beta, X, y, n, d, n_experts, first_index, m_target, reinterpret_cast<long long*>(indices_out));
+}
+
+int sgp_kmeans(sgp_ctx* h, const void* X, int32_t x_is_f32, int64_t n, int32_t d, int32_t k, int32_t max_iter, double tol,
+               int64_t seed, const double* init_centers, double* centers_out, int32_t* k_out, int32_t* labels_out,
+               int32_t* iterations_out, double* cost_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!X || !centers_out || !k_out || !iterations_out || !cost_out)
+    return fail(c, SGP_E_BADARG, "sgp_kmeans: null argument");
+  if (k < 2) return fail(c, SGP_E_BADARG, "requirement failed: k must be > 1");
+  if (max_iter < 0) return fail(c, SGP_E_BADARG, "requirement failed: maxIter must be >= 0");
+  if (!(tol >= 0.0)) return fail(c, SGP_E_BADARG, "requirement failed: tol must be >= 0");
+  if (n < 1 || d < 1) return fail(c, SGP_E_BADARG, "sgp_kmeans: no points or no features");
+  if (n > 2147483647LL) return fail(c, SGP_E_BADARG, "sgp_kmeans: n too large for one device");
+  if (init_centers)
+    for (size_t i = 0; i < static_cast<size_t>(k) * d; ++i)
+      if (!std::isfinite(init_centers[i])) return fail(c, SGP_E_BADARG, "sgp_kmeans: initial centres contain NaN or infinity");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  static_assert(sizeof(int) == sizeof(int32_t), "label type");
+  return run_kmeans(c, X, x_is_f32, n, d, k, max_iter, tol, static_cast<uint64_t>(seed), init_centers, centers_out, k_out,
+                    labels_out, iterations_out, cost_out);
 }
 
 int sgp_cross_kernel(sgp_ctx* h, const double* X, int64_t n, double* K_out) {

@@ -94,6 +94,7 @@ struct Ctx {
   cublasHandle_t blas = nullptr;
   cudaEvent_t tail_fork = nullptr, tail_join = nullptr;
   DevScratch tail_ws, tail_ws2, predict_ws, cross_ws, bcm_ws, sweep_ws, greedy_ws;
+  DevScratch kmeans_pts_ws, kmeans_cen_ws, kmeans_new_ws, kmeans_cand_ws;   // sgp_kmeans: point-, centre-, candidate-sized
   bool has_magic_run = false;
   bool tail_fast = false;              // last sgp_magic took the Cholesky path for both matrices
   ncclComm_t comm = nullptr;
@@ -280,6 +281,10 @@ int ctx_scratch(Ctx* c, DevScratch& s, size_t bytes);
 // csrc/greedy.cu: forward selection with rank-1 updates (ActiveSetProvider.scala:58-139); beta_flat = [n_terms][d]
 int run_greedy(Ctx* c, const KernelFlat& kf, const std::vector<double>& beta_flat, const double* X, const double* y,
                long long n, int d, long long n_experts, long long first_index, int m_target, long long* indices_out);
+// csrc/kmeans.cu: Spark 3.1 MLlib KMeans (k-means|| + Lloyd) for KMeansActiveSetProvider (ActiveSetProvider.scala:22-46)
+int run_kmeans(Ctx* c, const void* X, int x_is_f32, long long n, int d, int k, int max_iter, double tol, uint64_t seed,
+               const double* init_centers, double* centers_out, int* k_out, int* labels_out, int* iterations_out,
+               double* cost_out);
 int run_tail(Ctx* c, double* magic_vector, double* magic_matrix);
 int run_predict(Ctx* c, const double* X, long long n, double* mean_out, double* var_out);
 

@@ -299,6 +299,32 @@ class ProjectedProcessEngine:
         del keep
         return idx
 
+    def kmeans(self, X, k: int, max_iter: int = 20, tol: float = 1e-4, seed: int = 0, init_centers=None):
+        """Spark 3.1 MLlib KMeans (k-means|| seeding, Lloyd iterations) on the device (`sgp_kmeans`): returns
+        (centres [k_out x d] fp64, labels [n] int32, iterations, cost).  X: n x d, float32 (used without a copy) or
+        float64.  init_centers (k x d) replaces the seeding, as mllib's setInitialModel."""
+        X = np.asarray(X)
+        if X.dtype != np.float32:
+            X = np.asarray(X, dtype=np.float64)
+        X = np.ascontiguousarray(X)
+        if X.ndim != 2:
+            raise ValueError("X must be n x d")
+        n, d = X.shape
+        k = int(k)
+        init = None
+        if init_centers is not None:
+            init = np.ascontiguousarray(init_centers, dtype=np.float64)
+            if init.shape != (k, d):
+                raise ValueError("init_centers must be k x d")
+        centres = np.empty((max(k, 1), max(d, 1)))
+        labels = np.empty(max(n, 1), dtype=np.int32)
+        k_out, iters, cost = C.c_int32(), C.c_int32(), C.c_double()
+        seed = C.c_int64(int(seed) & 0xFFFFFFFFFFFFFFFF).value
+        self._check(self._lib.sgp_kmeans(self._h, N.ptr(X), int(X.dtype == np.float32), n, d, k, int(max_iter), float(tol),
+                                         seed, N.ptr(init) if init is not None else None, N.ptr(centres), C.byref(k_out),
+                                         N.ptr(labels), C.byref(iters), C.byref(cost)))
+        return np.ascontiguousarray(centres[:k_out.value]), labels[:n], iters.value, cost.value
+
     def kmn_sweep(self, X):
         """fp32 K[i][j] = k(x_i, z_j) (n x m) through the tensor-core sweep kernel (one non-Eye term, d <= 32)."""
         X = np.asarray(X)

@@ -47,12 +47,24 @@ class KMeansActiveSetProvider(ActiveSetProvider):
     (`new KMeans().setK(activeSetSize).setSeed(seed).setMaxIter(maxIter)`, Spark defaults otherwise: tol 1e-4).
     Host-side only: the clustering is a library call in the reference too (Spark MLlib); here scikit-learn's Lloyd
     iterations with k-means++ seeding stand in for Spark's k-means|| -- same objective and stopping rule, but Spark's
-    initialisation RNG stream is unpinned, so results are comparable on metrics (RMSE), not centroid by centroid."""
+    initialisation RNG stream is unpinned, so results are comparable on metrics (RMSE), not centroid by centroid.
 
-    def __init__(self, maxIter: int = 20):
+    `on_gpu=True` runs Spark's own algorithm on the device instead (`ProjectedProcessEngine.kmeans`, `sgp_kmeans`): k-means||
+    seeding, empty clusters keep their centre, absolute centre-movement tolerance; float32 X is used without a copy.  May
+    return fewer than activeSetSize centres when the data have fewer distinct points, as Spark does."""
+
+    def __init__(self, maxIter: int = 20, on_gpu: bool = False):
         self.maxIter = int(maxIter)
+        self.on_gpu = bool(on_gpu)
 
     def __call__(self, activeSetSize, X, y, kernel_factory, optimalHyperparameter, seed, gp=None):
+        if self.on_gpu:
+            eng = ProjectedProcessEngine.acquire(gp._device if gp is not None else 0)
+            try:
+                centres, _, _, _ = eng.kmeans(X, int(activeSetSize), max_iter=self.maxIter, tol=1e-4, seed=int(seed))
+            finally:
+                eng.release()
+            return centres
         from sklearn.cluster import KMeans
         km = KMeans(n_clusters=int(activeSetSize), init="k-means++", n_init=1, max_iter=self.maxIter, tol=1e-4,
                     random_state=int(seed) % (2 ** 32), algorithm="lloyd")
