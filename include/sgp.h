@@ -106,7 +106,9 @@ int sgp_comm_unique_id(void* out128);                                   /* rank 
 int sgp_comm_init(sgp_ctx* ctx, const void* id128, int rank, int nranks);
 
 /* ---- the hot path:  PGPH:20-36 ------------------------------------------------------------- */
-/* Active set Z: m x d row-major fp64 (activeSet: Array[Vector]).  Resets G, b to zero. */
+/* Active set Z: m x d row-major fp64 (activeSet: Array[Vector]).  Resets G, b to zero.  Every begin closes the previous
+ * window first: after a failed begin, the calls that need one (accumulate, finish, magic, set_magic, predict,
+ * cross_kernel, kmn_sweep) return SGP_E_STATE until a begin succeeds. */
 int sgp_stats_begin(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const double* Z, int32_t m, int32_t d);
 
 /* One shard / partition / expert group of points in HOST memory: X is n x d row-major (fp64, or fp32

@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstring>
 #include <new>
+#include <utility>
 
 namespace sgp {
 
@@ -47,15 +48,6 @@ int fail(Ctx* c, int code, const std::string& msg) {
     g_create_err = msg;
   }
   return code;
-}
-
-static void free_active_set(Ctx* c) {
-  cudaFree(c->dZ); cudaFree(c->dZs); cudaFree(c->dZc); cudaFree(c->dBeta); cudaFree(c->dGb);
-  cudaFree(c->dMagicVec); cudaFree(c->dMagicMat);
-  cudaFree(c->dI8Scale); cudaFree(c->dI8Flags); cudaFree(c->dI8Zt); cudaFree(c->dI8NormSum);
-  c->dZ = c->dZs = c->dZc = c->dBeta = c->dGb = c->dMagicVec = c->dMagicMat = nullptr;
-  c->dI8Scale = c->dI8NormSum = nullptr; c->dI8Flags = nullptr; c->dI8Zt = nullptr;
-  c->i8_ok = c->i8_direct_ok = c->i8d_prepared = false;
 }
 
 // Flattens a kernel description: Eye terms drop out of the cross kernel (kernel/Kernel.scala:157) and only sum their
@@ -180,177 +172,192 @@ static int direct_prepare(Ctx* c) {
   const size_t zd_bytes = static_cast<size_t>(c->m_pad / kTile) * c->kf.n_terms * kTile * c->dpad * sizeof(float);
   const int rc = ctx_scratch(c, c->i8_zd_ws, zd_bytes);
   if (rc != SGP_OK) return rc;
-  SGP_CUDA(c, launch_i8_prep_active_direct(c->i8_zd_ws.as<float>(), c->dZ, c->m, c->m_pad, c->d, c->dpad, c->kf.n_terms,
-                                           c->dI8Scale, c->dI8Scale + static_cast<size_t>(kMaxTerms) * c->dpad,
-                                           c->dI8Flags, kI8DirectR2Max, c->stream));
+  const double* scale = c->dI8Scale.as<double>();
+  SGP_CUDA(c, launch_i8_prep_active_direct(c->i8_zd_ws.as<float>(), c->dZ.as<double>(), c->m, c->m_pad, c->d, c->dpad,
+                                           c->kf.n_terms, scale, scale + static_cast<size_t>(kMaxTerms) * c->dpad,
+                                           c->dI8Flags.as<int>(), kI8DirectR2Max, c->stream));
   c->launches += 1;
   c->i8d_prepared = true;
   return SGP_OK;
 }
 
-// The statistics of n device-resident points: the fp64 kernel, or the int8 digit-plane producer and Gram (per launch
-// window), then the deterministic slice reduction.
-static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, long long n, long long n_call,
-                        bool first_of_call) {
-  // n: points of this launch; n_call: points of the whole accumulate call.  AUTO decides per CALL -- the size gate
-  // looks at n_call and the magnitude gate at the first chunk -- so the chunks of one shard never mix kernels (and
-  // only the first chunk pays the device->host round trip of the gate)
-  if (n <= 0) return SGP_OK;
-  const int nt1 = c->m_pad / kTile;
-  const int ntiles = nt1 * (nt1 + 1) / 2;
-  int n_slices = c->num_sms / ntiles;            // fp64 kernel: fill the SMs with tiles x point-slices
-  if (n_slices < 1) n_slices = 1;
-  const long long blocks = (n + 15) / 16;
-  if (n_slices > blocks) n_slices = static_cast<int>(blocks);
-  // int8 path: the digit planes of a launch window take kI8PlaneBytes per unit and active tile, so a launch covers at
-  // most kI8PlaneCapBytes of them; larger launches split into equal windows, all run with the first window's slices
-  const long long n_units = (n + 63) / 64;
-  const long long cap_units = std::max<long long>(1, kI8PlaneCapBytes / (kI8PlaneBytes * nt1));
-  const long long n_windows = (n_units + cap_units - 1) / cap_units;
-  const long long win_units = (n_units + n_windows - 1) / n_windows;
-  const int i8_n_slices = c->i8_direct_ok ? i8_slices(c->m_pad, c->num_sms, win_units) : 1;
-  const int max_slices = n_slices > i8_n_slices ? n_slices : i8_n_slices;
-  int rc = ctx_scratch(c, c->gpart_ws, static_cast<size_t>(max_slices) * c->m_pad * c->m_pad * sizeof(double));
-  if (rc == SGP_OK) rc = ctx_scratch(c, c->bpart_ws, static_cast<size_t>(n_slices) * c->m_pad * sizeof(double));
-  if (rc != SGP_OK) return rc;
-
-  // AUTO: the int8 kernel inside its measured parity envelope -- accumulate calls of >= 32768 points (posterior
-  // mean within a few 1e-6 of the all-fp64 kernel from N = 16k up; the limit is the two dropped low-order digit
-  // products, tools/i8_error_model.py,
-  // and does not grow towards small N) and small scaled norms (gate below).  Smaller calls stay on the fp64 DMMA kernel
-  // (2e-7), which needs < 2 ms at that size.
-  // Path of this launch: 0 = fp64 DMMA kernel, 1 = int8 Gram with tensor-core distances (one term, d <= 32, benign norms),
-  // 2 = int8 Gram with direct fp32 distances (up to 4 terms, d <= 72; AUTO: same magnitude budget as path 1).
-  int path = 0;
+// The path of one statistics launch: SGP_PREC_F64 / _F64_STRICT (fp64 DMMA kernel), SGP_PREC_I8 (int8 Gram with
+// tensor-core distances: one term, d <= 32) or SGP_PREC_I8_DIRECT (int8 Gram with direct fp32 distances: up to 4 terms,
+// n_terms * d <= 72).  AUTO: the int8 kernel inside its measured parity envelope -- accumulate calls (n_call points) of
+// >= 32768 points (posterior mean within a few 1e-6 of the all-fp64 kernel from N = 16k up; the limit is the two dropped
+// low-order digit products, tools/i8_error_model.py, and does not grow towards small N) and small scaled norms (the gate
+// of launch_stats_i8).  Smaller calls stay on the fp64 DMMA kernel (2e-7), which needs < 2 ms at that size.  AUTO
+// decides per CALL, on its first chunk, so the chunks of one shard never mix kernels (and only the first chunk pays the
+// device->host round trip of the gate).
+static int stats_path(Ctx* c, long long n_call, bool first_of_call, int* path) {
+  const int i8_mode = c->i8_ok ? SGP_PREC_I8 : c->i8_direct_ok ? SGP_PREC_I8_DIRECT : SGP_PREC_F64;
+  *path = c->precision == SGP_PREC_F64_STRICT ? SGP_PREC_F64_STRICT : SGP_PREC_F64;
   if (c->precision == SGP_PREC_I8) {
-    if (c->i8_ok) path = 1;
-    else if (c->i8_direct_ok) path = 2;
-    else return fail(c, SGP_E_BADARG, "SGP_PREC_I8 needs a kernel with 1..4 non-Eye terms and n_terms * d <= 72 "
-                                      "(tensor-core distances: exactly one term and d <= 32)");
+    if (i8_mode == SGP_PREC_F64)
+      return fail(c, SGP_E_BADARG, "SGP_PREC_I8 needs a kernel with 1..4 non-Eye terms and n_terms * d <= 72 "
+                                   "(tensor-core distances: exactly one term and d <= 32)");
+    *path = i8_mode;
   } else if (c->precision == SGP_PREC_I8_DIRECT) {
     if (!c->i8_direct_ok) return fail(c, SGP_E_BADARG, "SGP_PREC_I8_DIRECT needs a kernel with 1..4 non-Eye terms and n_terms * d <= 72");
-    path = 2;
+    *path = SGP_PREC_I8_DIRECT;
   } else if (c->precision == SGP_PREC_AUTO && n_call >= kAutoI8MinPoints) {
-    path = !first_of_call ? c->call_path : c->i8_ok ? 1 : c->i8_direct_ok ? 2 : 0;
+    *path = first_of_call ? i8_mode : c->call_path;
   }
-  // bytes of one 64-point unit of the int8 point operands: fp16 images (path 1) or fp32 coordinate tiles (path 2)
-  const size_t x_unit = (path == 1) ? i8_points_scratch_bytes(64, i8_nchunks(c->d))
-                                    : static_cast<size_t>(c->kf.n_terms) * 64 * c->dpad * sizeof(float);
-  if (path != 0) {
-    const bool autop = c->precision == SGP_PREC_AUTO;
-    const bool gate = autop && first_of_call;
-    rc = ctx_scratch(c, c->i8_ys_ws, static_cast<size_t>(n_units) * 64 * sizeof(float));
-    if (rc == SGP_OK) rc = ctx_scratch(c, c->i8_xt_ws, static_cast<size_t>(n_units) * x_unit);
-    if (rc == SGP_OK && path == 2) rc = direct_prepare(c);
-    if (rc != SGP_OK) return rc;
-    // the scaled squared norms of EVERY chunk are summed on the device (dI8NormSum[0]: whole begin..finish window,
-    // checked against the budget at finish so that an unrepresentative first chunk cannot silently degrade the
-    // statistics; dI8NormSum[1]: this call's first chunk, read back here for the kernel choice).  The direct mode sums
-    // the WIDEST term's scaled squared norms: they set the size of the kernel values.
-    double* call_sum = gate ? c->dI8NormSum + 1 : nullptr;
-    if (gate) SGP_CUDA(c, cudaMemsetAsync(call_sum, 0, sizeof(double), c->stream));
-    if (path == 1)
-      SGP_CUDA(c, launch_i8_prep_points(c->i8_xt_ws.as<uint8_t>(), c->i8_ys_ws.as<float>(), dX, x_is_f32, dy, n, c->d,
-                                        c->dI8Scale, c->dI8Scale + static_cast<size_t>(kMaxTerms) * c->dpad, c->dI8Flags,
-                                        c->dI8NormSum, call_sum, c->stream));
-    else
-      SGP_CUDA(c, launch_i8_prep_points_direct(c->i8_xt_ws.as<float>(), c->i8_ys_ws.as<float>(), dX, x_is_f32, dy, n, c->d,
-                                               c->dpad, c->kf.n_terms, c->dI8Scale,
-                                               c->dI8Scale + static_cast<size_t>(kMaxTerms) * c->dpad, c->dI8Flags,
-                                               kI8DirectR2Max, autop ? c->dI8NormSum : nullptr, call_sum, c->stream));
-    c->launches += 1;
-    if (gate) {
-      // AUTO's magnitude gate.  The distance contraction accumulates 2 x^.z^ - |x^|^2 - |z^|^2 in fp32 in tensor
-      // memory; its rounding (toward zero, measured) scales with those magnitudes: at mean|x^|^2 + mean|z^|^2 ~ 4.4
-      // the elements are good to 2.7e-7 rms (parity holds, tests), at ~12 (airfoil: norms up to 40) they are not
-      // (posterior mean off by 5e-4).  Large scaled norms also mean tiny kernel values, and the fixed-point digits carry
-      // an ABSOLUTE error of 2^-24: on such shards the int8 Gram -- with either distance form -- loses the posterior
-      // mean (airfoil-like data: 1.5e-4 to 1.5e-2 against 7e-7 .. 7e-6 of the fp64 kernel).  Above the budget the
-      // shard goes to the fp64 DMMA kernel instead.
-      double xsum = 0.0;
-      SGP_CUDA(c, cudaMemcpyAsync(&xsum, call_sum, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-      SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-      if (xsum / static_cast<double>(n) + c->i8_z_norm_mean > kI8NormBudget) path = 0;
-    }
-  }
-  if (first_of_call) c->call_path = path;
-  if (path != 0) {
-    c->i8_points += n;
-    c->i8_flag_mask |= (path == 1) ? 1 : 4;
-  }
-  c->last_path = (path == 1) ? SGP_PREC_I8 : (path == 2) ? SGP_PREC_I8_DIRECT
-                 : (c->precision == SGP_PREC_F64_STRICT ? SGP_PREC_F64_STRICT : SGP_PREC_F64);
-  if (path != 0) {
-    rc = ctx_scratch(c, c->i8_planes_ws, static_cast<size_t>(win_units) * nt1 * kI8PlaneBytes);
-    if (rc != SGP_OK) return rc;
-  }
-  if (c->gram_events_used == c->gram_events.size()) {          // grow the event pool (steady state: no creation)
+  return SGP_OK;
+}
+
+// Records the start of one Gram timing interval (sgp_gram_kernel_time) on the compute stream and returns the event that
+// ends it.  The event pool grows on first use only.
+static int gram_timer_start(Ctx* c, cudaEvent_t* stop) {
+  if (c->gram_events_used == c->gram_events.size()) {
     cudaEvent_t a, b;
     SGP_CUDA(c, cudaEventCreate(&a));
     SGP_CUDA(c, cudaEventCreate(&b));
     c->gram_events.emplace_back(a, b);
   }
-  cudaEvent_t e0 = c->gram_events[c->gram_events_used].first, e1 = c->gram_events[c->gram_events_used].second;
-  c->gram_events_used += 1;
-  SGP_CUDA(c, cudaEventRecord(e0, c->stream));
-  const size_t mm = static_cast<size_t>(c->m) * c->m;
-  double* Gpart = c->gpart_ws.as<double>();
-  if (path != 0) {
-    I8Direct direct;
-    if (path == 2) {
-      direct.on = 1; direct.n_terms = c->kf.n_terms; direct.dpad4 = c->dpad;
-      double csum = 0.0;
-      for (int t = 0; t < c->kf.n_terms; ++t) csum += c->kf.scale[t];
-      for (int t = 0; t < c->kf.n_terms; ++t) direct.w[t] = static_cast<float>(c->kf.scale[t] / csum);
-      direct.csum = csum;
-    }
-    const double C = (path == 2) ? direct.csum : c->kf.scale[0];
-    const uint8_t* zop = (path == 2) ? c->i8_zd_ws.as<uint8_t>() : c->dI8Zt;
-    // the producer's own point slices (its b partials): a grid that fills the SMs at the variant's occupancy
-    int plane_slices = 1;
-    SGP_CUDA(c, i8_plane_slices(c->m_pad, c->num_sms, win_units, c->d, direct, &plane_slices));
-    rc = ctx_scratch(c, c->bpart_ws, static_cast<size_t>(plane_slices) * c->m_pad * sizeof(double));
-    if (rc != SGP_OK) return rc;
-    double* bpart = c->bpart_ws.as<double>();
-    // per window: digit planes + b partials, then the Gram over them; the first window stores the slice partials,
-    // later ones add to them, and one deterministic slice reduction follows
-    for (long long w = 0; w < n_windows; ++w) {
-      const long long u0 = w * win_units;
-      const long long nu = std::min(win_units, n_units - u0);
-      SGP_CUDA(c, launch_i8_planes(c->i8_xt_ws.as<uint8_t>() + static_cast<size_t>(u0) * x_unit,
-                                   c->i8_ys_ws.as<float>() + static_cast<size_t>(u0) * 64, zop, nu, c->d, c->m_pad,
-                                   plane_slices, direct, C, w > 0, c->i8_planes_ws.as<uint8_t>(), bpart,
-                                   w == 0 ? c->dbgT : nullptr, w == 0 ? c->dbgW : nullptr, c->stream));
-      SGP_CUDA(c, launch_gram_i8(c->i8_planes_ws.as<uint8_t>(), nu, c->m_pad, i8_n_slices, C, w > 0, Gpart, c->stream));
-      c->launches += 2;
-    }
-    SGP_CUDA(c, cudaEventRecord(e1, c->stream));
-    // deterministic slice reduction (partial tiles at the mirror position: upper block triangle)
-    SGP_CUDA(c, launch_gram_reduce_upper(c->dGb, c->dGb + mm, Gpart, bpart, i8_n_slices, plane_slices, c->m, c->m_pad, 0,
-                                         c->m, c->stream));
-    c->launches += 1;
-    return SGP_OK;
-  }
+  const auto& ev = c->gram_events[c->gram_events_used++];
+  *stop = ev.second;
+  SGP_CUDA(c, cudaEventRecord(ev.first, c->stream));
+  return SGP_OK;
+}
+
+// The fp64 DMMA kernel over n device-resident points, then the deterministic slice reduction.
+static int launch_stats_f64(Ctx* c, bool strict, const void* dX, int x_is_f32, const double* dy, long long n) {
+  const int nt1 = c->m_pad / kTile;
+  const int ntiles = nt1 * (nt1 + 1) / 2;
+  int n_slices = c->num_sms / ntiles;            // fill the SMs with tiles x point-slices
+  if (n_slices < 1) n_slices = 1;
+  const long long blocks = (n + 15) / 16;
+  if (n_slices > blocks) n_slices = static_cast<int>(blocks);
+  int rc = ctx_scratch(c, c->gpart_ws, static_cast<size_t>(n_slices) * c->m_pad * c->m_pad * sizeof(double));
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->bpart_ws, static_cast<size_t>(n_slices) * c->m_pad * sizeof(double));
+  cudaEvent_t stop = nullptr;
+  if (rc == SGP_OK) rc = gram_timer_start(c, &stop);
+  if (rc != SGP_OK) return rc;
   GramParams p{};
   p.X = dX; p.y = dy; p.n = n; p.x_is_f32 = x_is_f32;
   p.d = c->d; p.dpad = c->dpad; p.m = c->m; p.m_pad = c->m_pad;
   p.n_terms = c->kf.n_terms;
   for (int t = 0; t < kMaxTerms; ++t) p.scale[t] = c->kf.scale[t];
-  p.Zs = c->dZc; p.beta = c->dBeta;
-  double* bpart = c->bpart_ws.as<double>();
-  p.Gpart = Gpart; p.bpart = bpart;
+  p.Zs = c->dZc.as<double>(); p.beta = c->dBeta.as<double>();
+  p.Gpart = c->gpart_ws.as<double>(); p.bpart = c->bpart_ws.as<double>();
   p.n_slices = n_slices; p.n_tiles_1d = nt1;
-  SGP_CUDA(c, launch_gram_f64(p, c->precision == SGP_PREC_F64_STRICT, c->stream));
-  SGP_CUDA(c, cudaEventRecord(e1, c->stream));
-  SGP_CUDA(c, launch_gram_reduce(c->dGb, c->dGb + mm, Gpart, bpart, n_slices, c->m, c->m_pad, c->stream));
+  SGP_CUDA(c, launch_gram_f64(p, strict, c->stream));
+  SGP_CUDA(c, cudaEventRecord(stop, c->stream));
+  double* G = c->dGb.as<double>();
+  SGP_CUDA(c, launch_gram_reduce(G, G + static_cast<size_t>(c->m) * c->m, p.Gpart, p.bpart, n_slices, c->m, c->m_pad,
+                                 c->stream));
   c->launches += 2;
   return SGP_OK;
 }
 
-static void drop_gram_events(Ctx* c) {
-  for (auto& e : c->gram_events) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
-  c->gram_events.clear();
-  c->gram_events_used = 0;
+// The int8 path (*path: SGP_PREC_I8 or _I8_DIRECT): the point operands, AUTO's magnitude gate (above it *path becomes
+// SGP_PREC_F64 and nothing more runs here), the producer and Gram per launch window, the deterministic slice reduction.
+static int launch_stats_i8(Ctx* c, int* path, const void* dX, int x_is_f32, const double* dy, long long n,
+                           bool first_of_call) {
+  const bool direct_mode = *path == SGP_PREC_I8_DIRECT;
+  const bool autop = c->precision == SGP_PREC_AUTO, gate = autop && first_of_call;
+  const long long n_units = (n + 63) / 64;
+  // bytes of one 64-point unit of the point operands: fp16 images (tensor-core distances) or fp32 coordinate tiles
+  const size_t x_unit = direct_mode ? static_cast<size_t>(c->kf.n_terms) * 64 * c->dpad * sizeof(float)
+                                    : i8_points_scratch_bytes(64, i8_nchunks(c->d));
+  int rc = ctx_scratch(c, c->i8_ys_ws, static_cast<size_t>(n_units) * 64 * sizeof(float));
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->i8_xt_ws, static_cast<size_t>(n_units) * x_unit);
+  if (rc == SGP_OK && direct_mode) rc = direct_prepare(c);
+  if (rc != SGP_OK) return rc;
+  // the scaled squared norms of EVERY chunk are summed on the device (dI8NormSum[0]: whole begin..finish window,
+  // checked against the budget at finish so that an unrepresentative first chunk cannot silently degrade the
+  // statistics; dI8NormSum[1]: this call's first chunk, read back here for the kernel choice).  The direct mode sums
+  // the WIDEST term's scaled squared norms: they set the size of the kernel values.
+  const double* scale = c->dI8Scale.as<double>();
+  const double* centre = scale + static_cast<size_t>(kMaxTerms) * c->dpad;
+  double* norm_sum = c->dI8NormSum.as<double>();
+  double* call_sum = gate ? norm_sum + 1 : nullptr;
+  if (gate) SGP_CUDA(c, cudaMemsetAsync(call_sum, 0, sizeof(double), c->stream));
+  if (direct_mode)
+    SGP_CUDA(c, launch_i8_prep_points_direct(c->i8_xt_ws.as<float>(), c->i8_ys_ws.as<float>(), dX, x_is_f32, dy, n, c->d,
+                                             c->dpad, c->kf.n_terms, scale, centre, c->dI8Flags.as<int>(), kI8DirectR2Max,
+                                             autop ? norm_sum : nullptr, call_sum, c->stream));
+  else
+    SGP_CUDA(c, launch_i8_prep_points(c->i8_xt_ws.as<uint8_t>(), c->i8_ys_ws.as<float>(), dX, x_is_f32, dy, n, c->d, scale,
+                                      centre, c->dI8Flags.as<int>(), norm_sum, call_sum, c->stream));
+  c->launches += 1;
+  if (gate) {
+    // AUTO's magnitude gate.  The distance contraction accumulates 2 x^.z^ - |x^|^2 - |z^|^2 in fp32 in tensor
+    // memory; its rounding (toward zero, measured) scales with those magnitudes: at mean|x^|^2 + mean|z^|^2 ~ 4.4
+    // the elements are good to 2.7e-7 rms (parity holds, tests), at ~12 (airfoil: norms up to 40) they are not
+    // (posterior mean off by 5e-4).  Large scaled norms also mean tiny kernel values, and the fixed-point digits carry
+    // an ABSOLUTE error of 2^-24: on such shards the int8 Gram -- with either distance form -- loses the posterior
+    // mean (airfoil-like data: 1.5e-4 to 1.5e-2 against 7e-7 .. 7e-6 of the fp64 kernel).  Above the budget the
+    // shard goes to the fp64 DMMA kernel instead.
+    double xsum = 0.0;
+    SGP_CUDA(c, cudaMemcpyAsync(&xsum, call_sum, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (xsum / static_cast<double>(n) + c->i8_z_norm_mean > kI8NormBudget) {
+      *path = SGP_PREC_F64;
+      return SGP_OK;
+    }
+  }
+  // the digit planes of a launch window take kI8PlaneBytes per unit and active tile, so a launch covers at most
+  // kI8PlaneCapBytes of them; larger launches split into equal windows, all run with the first window's slices: the
+  // Gram's (its G partials) and the producer's own (its b partials), a grid that fills the SMs at the variant's occupancy
+  const int nt1 = c->m_pad / kTile;
+  const long long cap_units = std::max<long long>(1, kI8PlaneCapBytes / (kI8PlaneBytes * nt1));
+  const long long n_windows = (n_units + cap_units - 1) / cap_units;
+  const long long win_units = (n_units + n_windows - 1) / n_windows;
+  const I8Direct direct = direct_mode ? c->i8_direct : I8Direct{};
+  const double C = direct_mode ? direct.csum : c->kf.scale[0];
+  const uint8_t* zop = direct_mode ? c->i8_zd_ws.as<uint8_t>() : c->dI8Zt.as<uint8_t>();
+  const int g_slices = i8_slices(c->m_pad, c->num_sms, win_units);
+  int b_slices = 1;
+  SGP_CUDA(c, i8_plane_slices(c->m_pad, c->num_sms, win_units, c->d, direct, &b_slices));
+  rc = ctx_scratch(c, c->i8_planes_ws, static_cast<size_t>(win_units) * nt1 * kI8PlaneBytes);
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->gpart_ws, static_cast<size_t>(g_slices) * c->m_pad * c->m_pad * sizeof(double));
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->bpart_ws, static_cast<size_t>(b_slices) * c->m_pad * sizeof(double));
+  cudaEvent_t stop = nullptr;
+  if (rc == SGP_OK) rc = gram_timer_start(c, &stop);
+  if (rc != SGP_OK) return rc;
+  uint8_t* planes = c->i8_planes_ws.as<uint8_t>();
+  double* Gpart = c->gpart_ws.as<double>();
+  double* bpart = c->bpart_ws.as<double>();
+  // per window: digit planes + b partials, then the Gram over them; the first window stores the slice partials,
+  // later ones add to them, and one deterministic slice reduction follows
+  for (long long w = 0; w < n_windows; ++w) {
+    const long long u0 = w * win_units;
+    const long long nu = std::min(win_units, n_units - u0);
+    SGP_CUDA(c, launch_i8_planes(c->i8_xt_ws.as<uint8_t>() + static_cast<size_t>(u0) * x_unit,
+                                 c->i8_ys_ws.as<float>() + static_cast<size_t>(u0) * 64, zop, nu, c->d, c->m_pad, b_slices,
+                                 direct, C, w > 0, planes, bpart, w == 0 ? c->dbgT.as<float>() : nullptr,
+                                 w == 0 ? c->dbgW.as<uint32_t>() : nullptr, c->stream));
+    SGP_CUDA(c, launch_gram_i8(planes, nu, c->m_pad, g_slices, C, w > 0, Gpart, c->stream));
+    c->launches += 2;
+  }
+  SGP_CUDA(c, cudaEventRecord(stop, c->stream));
+  // partial tiles at the mirror position: upper block triangle
+  double* G = c->dGb.as<double>();
+  SGP_CUDA(c, launch_gram_reduce_upper(G, G + static_cast<size_t>(c->m) * c->m, Gpart, bpart, g_slices, b_slices, c->m,
+                                       c->m_pad, c->stream));
+  c->launches += 1;
+  return SGP_OK;
+}
+
+// The statistics of n device-resident points (n_call: the whole accumulate call's) on the path stats_path picks.
+static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, long long n, long long n_call,
+                        bool first_of_call) {
+  if (n <= 0) return SGP_OK;
+  const auto int8 = [](int p) { return p == SGP_PREC_I8 || p == SGP_PREC_I8_DIRECT; };
+  int path = SGP_PREC_F64;
+  int rc = stats_path(c, n_call, first_of_call, &path);
+  if (rc == SGP_OK && int8(path)) rc = launch_stats_i8(c, &path, dX, x_is_f32, dy, n, first_of_call);
+  if (rc == SGP_OK && !int8(path)) rc = launch_stats_f64(c, path == SGP_PREC_F64_STRICT, dX, x_is_f32, dy, n);
+  if (rc != SGP_OK) return rc;
+  if (first_of_call) c->call_path = path;
+  c->last_path = path;
+  if (int8(path)) {
+    c->i8_points += n;
+    c->i8_flag_mask |= (path == SGP_PREC_I8) ? 1 : 4;
+  }
+  return SGP_OK;
 }
 
 }  // namespace sgp
@@ -404,22 +411,13 @@ int sgp_ctx_destroy(sgp_ctx* h) {
   if (!c) return SGP_OK;
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
-  drop_gram_events(c);
+  for (auto& e : c->gram_events) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
   for (auto& e : c->user_events) if (e) cudaEventDestroy(e);
-  free_active_set(c);
-  cudaFree(c->ex.X); cudaFree(c->ex.y); cudaFree(c->ex.off); cudaFree(c->ex.f);
-  cudaFree(c->dbgT); cudaFree(c->dbgW);
   for (int i = 0; i < 2; ++i) {
-    cudaFree(c->stage_x[i].p); cudaFree(c->stage_y[i].p);
     if (c->stage_free[i]) cudaEventDestroy(c->stage_free[i]);
     if (c->stage_ready[i]) cudaEventDestroy(c->stage_ready[i]);
   }
   if (c->comm && nccl().ok) nccl().CommDestroy(c->comm);
-  for (DevScratch* s : {&c->gpart_ws, &c->bpart_ws, &c->i8_zd_ws, &c->i8_xt_ws, &c->i8_ys_ws, &c->i8_planes_ws,
-                        &c->nll_per_ws, &c->hyper_ws, &c->greedy_ws, &c->kmeans_pts_ws, &c->kmeans_cen_ws, &c->kmeans_new_ws,
-                        &c->kmeans_cand_ws, &c->sweep_ws, &c->bcm_ws, &c->tail_ws, &c->tail_ws2,
-                        &c->predict_ws, &c->cross_ws})
-    cudaFree(s->p);
   if (c->tail_fork) cudaEventDestroy(c->tail_fork);
   if (c->tail_join) cudaEventDestroy(c->tail_join);
   if (c->tail_stream) cudaStreamDestroy(c->tail_stream);
@@ -428,7 +426,7 @@ int sgp_ctx_destroy(sgp_ctx* h) {
   if (c->blas) cublasDestroy(c->blas);
   if (c->stream) cudaStreamDestroy(c->stream);
   if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
-  delete c;
+  delete c;                                         // the device buffers free themselves
   return SGP_OK;
 }
 
@@ -472,6 +470,7 @@ int sgp_comm_init(sgp_ctx* h, const void* id128, int rank, int nranks) {
 int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32_t m, int32_t d) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
+  c->begun = c->finished = c->has_magic = false;   // a begin that fails leaves no window open
   if (!k || !Z || m <= 0 || d <= 0 || k->n_terms <= 0 || !k->terms)
     return fail(c, SGP_E_BADARG, "sgp_stats_begin: null or empty argument");
   SGP_CUDA(c, cudaSetDevice(c->device));
@@ -480,58 +479,54 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
   const int dpad = (d + 3) & ~3;
   int rc = flatten_kernel(c, k, d, dpad, kf, beta, nullptr);
   if (rc != SGP_OK) return rc;
-  // device buffers are kept across begin() calls with the same (m, d, term count): cudaMalloc/cudaFree are
-  // synchronising and cost milliseconds -- more than the whole statistics pass on the GPU
-  const int nt = kf.n_terms > 0 ? kf.n_terms : 1;
-  const bool same_shape = c->dZ && c->m == m && c->d == d && c->alloc_terms == nt;
-  if (!same_shape) {
-    SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-    free_active_set(c);
-  }
   c->m = m; c->d = d; c->dpad = dpad; c->m_pad = (m + kTile - 1) / kTile * kTile; c->kf = kf;
   // int8 Gram: direct distances for 1..4 non-Eye terms with n_terms * dpad <= 72 (shared memory); tensor-core distances
   // for one term and d <= 32 (two 64-column K chunks)
   c->i8_direct_ok = kf.n_terms >= 1 && kf.n_terms * dpad <= 72;
   c->i8_ok = kf.n_terms == 1 && d <= 32;
+  I8Direct& dm = c->i8_direct;     // the direct mode's term weights C_t / sum C; sum C is its fixed-point scale
+  dm = I8Direct{1, kf.n_terms, dpad};
+  for (int t = 0; t < kf.n_terms; ++t) dm.csum += kf.scale[t];
+  for (int t = 0; t < kf.n_terms; ++t) dm.w[t] = static_cast<float>(kf.scale[t] / dm.csum);
+  // the device buffers only grow: cudaMalloc/cudaFree are synchronising and cost milliseconds -- more than the whole
+  // statistics pass on the GPU
   const size_t mm = static_cast<size_t>(m) * m;
-  if (!same_shape) {
-    c->alloc_terms = nt;
-    SGP_CUDA(c, cudaMalloc(&c->dZ, static_cast<size_t>(m) * d * 8));
-    SGP_CUDA(c, cudaMalloc(&c->dZs, static_cast<size_t>(nt) * c->m_pad * dpad * 8));
-    SGP_CUDA(c, cudaMalloc(&c->dZc, static_cast<size_t>(nt) * c->m_pad * dpad * 8));
-    SGP_CUDA(c, cudaMalloc(&c->dBeta, static_cast<size_t>(kMaxTerms + 1) * dpad * 8));
-    SGP_CUDA(c, cudaMalloc(&c->dGb, (mm + m + 1) * 8));     // [G ; b ; status] -- one all-reduce
-    SGP_CUDA(c, cudaMalloc(&c->dMagicVec, static_cast<size_t>(m) * 8));
-    SGP_CUDA(c, cudaMalloc(&c->dMagicMat, mm * 8));
-    SGP_CUDA(c, cudaMalloc(&c->dI8Flags, 3 * sizeof(int)));
-    SGP_CUDA(c, cudaMalloc(&c->dI8NormSum, 2 * sizeof(double)));
-    SGP_CUDA(c, cudaMalloc(&c->dI8Scale, static_cast<size_t>(kMaxTerms + 1) * dpad * 8));
-  }
-  if (c->i8_ok && !c->dI8Zt)          // same_shape does not tell 0 from 1 non-Eye term
-    SGP_CUDA(c, cudaMalloc(&c->dI8Zt, i8_active_scratch_bytes(c->m_pad, i8_nchunks(d))));
-  SGP_CUDA(c, cudaMemcpyAsync(c->dZ, Z, static_cast<size_t>(m) * d * 8, cudaMemcpyHostToDevice, c->stream));
+  const size_t z_bytes = static_cast<size_t>(std::max(kf.n_terms, 1)) * c->m_pad * dpad * 8;
+  const size_t dim_bytes = static_cast<size_t>(kMaxTerms + 1) * dpad * 8;
+  const std::pair<DevScratch*, size_t> bufs[] = {
+      {&c->dZ, static_cast<size_t>(m) * d * 8}, {&c->dZs, z_bytes}, {&c->dZc, z_bytes}, {&c->dBeta, dim_bytes},
+      {&c->dGb, (mm + m + 1) * 8}, {&c->dMagicVec, static_cast<size_t>(m) * 8}, {&c->dMagicMat, mm * 8},
+      {&c->dI8Flags, 3 * sizeof(int)}, {&c->dI8NormSum, 2 * sizeof(double)}, {&c->dI8Scale, dim_bytes},
+      {&c->dI8Zt, c->i8_ok ? i8_active_scratch_bytes(c->m_pad, i8_nchunks(d)) : 0}};   // 0: not needed
+  for (const auto& [buf, bytes] : bufs)
+    if (bytes > 0 && (rc = ctx_scratch(c, *buf, bytes)) != SGP_OK) return rc;
+  double* dZ = c->dZ.as<double>();
+  double* dBeta = c->dBeta.as<double>();
+  double* dScale = c->dI8Scale.as<double>();
+  int* dFlags = c->dI8Flags.as<int>();
+  SGP_CUDA(c, cudaMemcpyAsync(dZ, Z, static_cast<size_t>(m) * d * 8, cudaMemcpyHostToDevice, c->stream));
   std::vector<double> sc;                          // live until the synchronisation at the end of this function
   beta.resize(static_cast<size_t>(kMaxTerms + 1) * dpad, 0.0);
   c->i8_z_norm_mean = stats_scales(Z, m, d, dpad, kf.n_terms, beta, c->i8_direct_ok, sc,
                                    beta.data() + static_cast<size_t>(kMaxTerms) * dpad);
-  SGP_CUDA(c, cudaMemcpyAsync(c->dBeta, beta.data(), beta.size() * 8, cudaMemcpyHostToDevice, c->stream));
-  SGP_CUDA(c, cudaMemsetAsync(c->dGb, 0, (mm + m + 1) * 8, c->stream));
-  SGP_CUDA(c, cudaMemcpyAsync(c->dI8Scale, sc.data(), sc.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(dBeta, beta.data(), beta.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, cudaMemsetAsync(c->dGb.p, 0, (mm + m + 1) * 8, c->stream));      // [G ; b ; status] -- one all-reduce
+  SGP_CUDA(c, cudaMemcpyAsync(dScale, sc.data(), sc.size() * 8, cudaMemcpyHostToDevice, c->stream));
   for (int t = 0; t < kf.n_terms; ++t) {
     const size_t off = static_cast<size_t>(t) * c->m_pad * dpad;
-    SGP_CUDA(c, launch_scale_rows(c->dZs + off, c->dZc + off, c->dZ, c->dBeta + static_cast<size_t>(t) * dpad,
-                                  c->dBeta + static_cast<size_t>(kMaxTerms) * dpad, m, c->m_pad, d, dpad,
-                                  c->stream));
+    SGP_CUDA(c, launch_scale_rows(c->dZs.as<double>() + off, c->dZc.as<double>() + off, dZ,
+                                  dBeta + static_cast<size_t>(t) * dpad, dBeta + static_cast<size_t>(kMaxTerms) * dpad, m,
+                                  c->m_pad, d, dpad, c->stream));
     c->launches += 1;
   }
-  SGP_CUDA(c, cudaMemsetAsync(c->dI8Flags, 0, 3 * sizeof(int), c->stream));
-  SGP_CUDA(c, cudaMemsetAsync(c->dI8NormSum, 0, 2 * sizeof(double), c->stream));
+  SGP_CUDA(c, cudaMemsetAsync(dFlags, 0, 3 * sizeof(int), c->stream));
+  SGP_CUDA(c, cudaMemsetAsync(c->dI8NormSum.p, 0, 2 * sizeof(double), c->stream));
   if (c->i8_ok) {
     // the tensor-core operand images are built here, the direct mode's active-set tiles on its first launch
     // the active set's range status goes to its own word; the window's status starts from it
-    SGP_CUDA(c, launch_i8_prep_active(c->dI8Zt, c->dZ, m, c->m_pad, d, c->dI8Scale,
-                                      c->dI8Scale + static_cast<size_t>(kMaxTerms) * dpad, c->dI8Flags + 1, c->stream));
-    SGP_CUDA(c, cudaMemcpyAsync(c->dI8Flags, c->dI8Flags + 1, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
+    SGP_CUDA(c, launch_i8_prep_active(c->dI8Zt.as<uint8_t>(), dZ, m, c->m_pad, d, dScale,
+                                      dScale + static_cast<size_t>(kMaxTerms) * dpad, dFlags + 1, c->stream));
+    SGP_CUDA(c, cudaMemcpyAsync(dFlags, dFlags + 1, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
     c->launches += 1;
   }
   c->i8d_prepared = false;
@@ -539,7 +534,7 @@ int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32
   c->gram_events_used = 0;
   c->i8_points = 0;
   c->i8_flag_mask = 0;
-  c->begun = true; c->finished = false; c->has_magic = false;
+  c->begun = true;
   return SGP_OK;
 }
 
@@ -594,6 +589,7 @@ int sgp_stats_finish(sgp_ctx* h, double* G_out, double* b_out) {
   if (!c->begun) return fail(c, SGP_E_STATE, "sgp_stats_begin should have been called first");
   SGP_CUDA(c, cudaSetDevice(c->device));
   const size_t mm = static_cast<size_t>(c->m) * c->m;
+  double* G = c->dGb.as<double>();
   double status = 0.0;
   if (!c->finished) {
     // The rank-local status of the int8 path (operand range exceeded; AUTO's magnitude budget exceeded over the
@@ -603,21 +599,21 @@ int sgp_stats_finish(sgp_ctx* h, double* G_out, double* b_out) {
     const int mask = c->i8_flag_mask;
     const bool budget = mask != 0 && c->precision == SGP_PREC_AUTO;
     const double limit = (kI8NormBudget - c->i8_z_norm_mean) * static_cast<double>(c->i8_points) * 1.25;
-    SGP_CUDA(c, launch_status_to_double(c->dGb + mm + c->m, mask ? c->dI8Flags : nullptr, mask,
-                                        budget ? c->dI8NormSum : nullptr, limit, c->stream));
+    SGP_CUDA(c, launch_status_to_double(G + mm + c->m, mask ? c->dI8Flags.as<int>() : nullptr, mask,
+                                        budget ? c->dI8NormSum.as<double>() : nullptr, limit, c->stream));
     c->launches += 1;
     if (c->comm && c->nranks > 1) {
       // PGPH:31-35 combOp: one all-reduce of the packed [G;b;status] over NVLink
-      ncclResult_t r = nccl().AllReduce(c->dGb, c->dGb, mm + c->m + 1, ncclDouble, ncclSum, c->comm, c->stream);
+      ncclResult_t r = nccl().AllReduce(G, G, mm + c->m + 1, ncclDouble, ncclSum, c->comm, c->stream);
       if (r != ncclSuccess) return fail(c, SGP_E_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
       c->launches += 1;
     }
-    SGP_CUDA(c, cudaMemcpyAsync(&status, c->dGb + mm + c->m, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    SGP_CUDA(c, cudaMemcpyAsync(&status, G + mm + c->m, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   }
   c->finished = true;
-  if (G_out) SGP_CUDA(c, cudaMemcpyAsync(G_out, c->dGb, mm * 8, cudaMemcpyDeviceToHost, c->stream));
+  if (G_out) SGP_CUDA(c, cudaMemcpyAsync(G_out, G, mm * 8, cudaMemcpyDeviceToHost, c->stream));
   if (b_out)
-    SGP_CUDA(c, cudaMemcpyAsync(b_out, c->dGb + mm, static_cast<size_t>(c->m) * 8, cudaMemcpyDeviceToHost, c->stream));
+    SGP_CUDA(c, cudaMemcpyAsync(b_out, G + mm, static_cast<size_t>(c->m) * 8, cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   if (status != 0.0)
     return fail(c, SGP_E_RANGE, "the int8 path cannot represent this shard on some rank (scaled squared norms outside the "
@@ -644,8 +640,8 @@ int sgp_magic(sgp_ctx* h, const double* G_in, const double* b_in, double* magic_
   SGP_CUDA(c, cudaSetDevice(c->device));
   const size_t mm = static_cast<size_t>(c->m) * c->m;
   if (G_in) {
-    SGP_CUDA(c, cudaMemcpyAsync(c->dGb, G_in, mm * 8, cudaMemcpyHostToDevice, c->stream));
-    SGP_CUDA(c, cudaMemcpyAsync(c->dGb + mm, b_in, static_cast<size_t>(c->m) * 8, cudaMemcpyHostToDevice, c->stream));
+    SGP_CUDA(c, cudaMemcpyAsync(c->dGb.p, G_in, mm * 8, cudaMemcpyHostToDevice, c->stream));
+    SGP_CUDA(c, cudaMemcpyAsync(c->dGb.as<double>() + mm, b_in, static_cast<size_t>(c->m) * 8, cudaMemcpyHostToDevice, c->stream));
     c->finished = true;
   } else if (!c->finished) {
     return fail(c, SGP_E_STATE, "sgp_stats_finish should have been called first");
@@ -660,8 +656,8 @@ int sgp_set_magic(sgp_ctx* h, const double* v, const double* M) {
   if (!v || !M) return fail(c, SGP_E_BADARG, "sgp_set_magic: null argument");
   SGP_CUDA(c, cudaSetDevice(c->device));
   const size_t mm = static_cast<size_t>(c->m) * c->m;
-  SGP_CUDA(c, cudaMemcpyAsync(c->dMagicVec, v, static_cast<size_t>(c->m) * 8, cudaMemcpyHostToDevice, c->stream));
-  SGP_CUDA(c, cudaMemcpyAsync(c->dMagicMat, M, mm * 8, cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(c->dMagicVec.p, v, static_cast<size_t>(c->m) * 8, cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(c->dMagicMat.p, M, mm * 8, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));          // the caller may reuse v, M as soon as we return
   c->has_magic = true;
   return SGP_OK;
@@ -699,18 +695,19 @@ int sgp_gram_kernel_time(sgp_ctx* h, double* total_ms, int64_t* launches) {
 }
 
 namespace {
-// Replaces the context's experts by buffers of exactly this size, with f = zeros (GPCls:54).
+// Drops the context's experts and sizes its expert buffers for E experts of n points in total, with f = zeros
+// (GPCls:54).  The caller fills X, y and off, then sets ex.E: the experts count as uploaded only from then on.
 int experts_alloc(Ctx* c, long long E, long long n, int d, int n_max) {
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   ExpertSet& ex = c->ex;
-  cudaFree(ex.X); cudaFree(ex.y); cudaFree(ex.off); cudaFree(ex.f);
   ex = ExpertSet{};
-  SGP_CUDA(c, cudaMalloc(&ex.X, static_cast<size_t>(n) * d * 8));
-  SGP_CUDA(c, cudaMalloc(&ex.y, static_cast<size_t>(n) * 8));
-  SGP_CUDA(c, cudaMalloc(&ex.off, static_cast<size_t>(E + 1) * 8));
-  SGP_CUDA(c, cudaMalloc(&ex.f, static_cast<size_t>(n) * 8));
+  int rc = ctx_scratch(c, c->ex_X, static_cast<size_t>(n) * d * 8);
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_y, static_cast<size_t>(n) * 8);
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_off, static_cast<size_t>(E + 1) * 8);
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_f, static_cast<size_t>(n) * 8);
+  if (rc != SGP_OK) return rc;
+  ex.X = c->ex_X.as<double>(); ex.y = c->ex_y.as<double>(); ex.off = c->ex_off.as<long long>(); ex.f = c->ex_f.as<double>();
   SGP_CUDA(c, cudaMemsetAsync(ex.f, 0, static_cast<size_t>(n) * 8, c->stream));
-  ex.E = E; ex.n = n; ex.d = d; ex.n_max = n_max;
+  ex.n = n; ex.d = d; ex.n_max = n_max;
   return SGP_OK;
 }
 }  // namespace
@@ -735,6 +732,7 @@ int sgp_experts_upload(sgp_ctx* h, const double* X, const double* y, const int64
   SGP_CUDA(c, cudaMemcpyAsync(c->ex.y, y, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaMemcpyAsync(c->ex.off, offsets, static_cast<size_t>(E + 1) * 8, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->ex.E = E;
   return SGP_OK;
 }
 
@@ -764,6 +762,7 @@ int sgp_experts_upload_grouped(sgp_ctx* h, const void* X, int32_t x_is_f32, cons
   });
   if (rc != SGP_OK) return rc;
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->ex.E = E;
   return SGP_OK;
 }
 
@@ -772,7 +771,7 @@ namespace {
 // the flattened terms and uploads them, with zeroed totals and flags, into the context's descriptor block.
 int objective_setup(Ctx* c, const sgp_kernel_desc* k, const sgp_hyper* hypers, int nh, HyperView& hv, double*& dTotal,
                     int*& dFlags) {
-  if (!c->ex.X) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
+  if (c->ex.E == 0) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
   if (!k || !k->terms || k->n_terms <= 0 || nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, "null argument");
   if (nh > kMaxHypers) return fail(c, SGP_E_BADARG, "too many hyper-parameters");
   const int d = c->ex.d;
@@ -919,7 +918,7 @@ int sgp_laplace_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hyper
 int sgp_experts_get_f(sgp_ctx* h, double* f_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
-  if (!c->ex.f || !f_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
+  if (c->ex.E == 0 || !f_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
   SGP_CUDA(c, cudaSetDevice(c->device));
   SGP_CUDA(c, cudaMemcpyAsync(f_out, c->ex.f, static_cast<size_t>(c->ex.n) * 8, cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -946,15 +945,16 @@ int sgp_debug_i8_tile(sgp_ctx* h, float* T_out, uint32_t* w_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
   SGP_CUDA(c, cudaSetDevice(c->device));
-  if (!c->dbgT) {   // arm: the next I8 launches dump the first distance tile of CTA (0,0)
-    SGP_CUDA(c, cudaMalloc(&c->dbgT, 128 * 64 * 4));
-    SGP_CUDA(c, cudaMalloc(&c->dbgW, 128 * 64 * 4));
-    SGP_CUDA(c, cudaMemset(c->dbgT, 0, 128 * 64 * 4));
-    SGP_CUDA(c, cudaMemset(c->dbgW, 0, 128 * 64 * 4));
+  if (!c->dbgW.p) {   // arm: the next I8 launches dump the first distance tile of CTA (0,0)
+    int rc = ctx_scratch(c, c->dbgT, 128 * 64 * 4);
+    if (rc == SGP_OK) rc = ctx_scratch(c, c->dbgW, 128 * 64 * 4);
+    if (rc != SGP_OK) return rc;
+    SGP_CUDA(c, cudaMemset(c->dbgT.p, 0, 128 * 64 * 4));
+    SGP_CUDA(c, cudaMemset(c->dbgW.p, 0, 128 * 64 * 4));
   }
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (T_out) SGP_CUDA(c, cudaMemcpy(T_out, c->dbgT, 128 * 64 * 4, cudaMemcpyDeviceToHost));
-  if (w_out) SGP_CUDA(c, cudaMemcpy(w_out, c->dbgW, 128 * 64 * 4, cudaMemcpyDeviceToHost));
+  if (T_out) SGP_CUDA(c, cudaMemcpy(T_out, c->dbgT.p, 128 * 64 * 4, cudaMemcpyDeviceToHost));
+  if (w_out) SGP_CUDA(c, cudaMemcpy(w_out, c->dbgW.p, 128 * 64 * 4, cudaMemcpyDeviceToHost));
   return SGP_OK;
 }
 
@@ -988,11 +988,12 @@ static int sweep_device(Ctx* c, const void* dX, int x_is_f32, long long n, float
   int rc = ctx_scratch(c, c->i8_xt_ws, i8_points_scratch_bytes(n, i8_nchunks(c->d)));
   if (rc == SGP_OK) rc = ctx_scratch(c, c->i8_ys_ws, static_cast<size_t>((n + 63) / 64) * 64 * sizeof(float));
   if (rc != SGP_OK) return rc;
+  const double* scale = c->dI8Scale.as<double>();
   SGP_CUDA(c, launch_i8_prep_points(c->i8_xt_ws.as<uint8_t>(), c->i8_ys_ws.as<float>(), dX, x_is_f32, nullptr, n, c->d,
-                                    c->dI8Scale, c->dI8Scale + static_cast<size_t>(kMaxTerms) * c->dpad, c->dI8Flags + 2,
+                                    scale, scale + static_cast<size_t>(kMaxTerms) * c->dpad, c->dI8Flags.as<int>() + 2,
                                     nullptr, nullptr, c->stream));
-  SGP_CUDA(c, launch_kmn_sweep(c->i8_xt_ws.as<uint8_t>(), c->dI8Zt, n, c->d, c->m, c->m_pad, c->num_sms, c->kf.scale[0], dK,
-                               c->stream));
+  SGP_CUDA(c, launch_kmn_sweep(c->i8_xt_ws.as<uint8_t>(), c->dI8Zt.as<uint8_t>(), n, c->d, c->m, c->m_pad, c->num_sms,
+                               c->kf.scale[0], dK, c->stream));
   c->launches += 2;
   return SGP_OK;
 }
@@ -1022,7 +1023,7 @@ int sgp_kmn_sweep(sgp_ctx* h, const void* X, int32_t x_is_f32, int64_t n, float*
   float* dK = static_cast<float*>(c->sweep_ws.p);
   void* dX = dK + static_cast<size_t>(cn0) * c->m;
   // this call's status: the active set's range bit from begin, then the bits of this call's points
-  SGP_CUDA(c, cudaMemcpyAsync(c->dI8Flags + 2, c->dI8Flags + 1, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(c->dI8Flags.as<int>() + 2, c->dI8Flags.as<int>() + 1, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
   for (long long p0 = 0; p0 < n; p0 += chunk) {
     const long long cn = (n - p0 < chunk) ? (n - p0) : chunk;
     SGP_CUDA(c, cudaMemcpyAsync(dX, static_cast<const char*>(X) + static_cast<size_t>(p0) * c->d * esz,
@@ -1034,7 +1035,7 @@ int sgp_kmn_sweep(sgp_ctx* h, const void* X, int32_t x_is_f32, int64_t n, float*
     SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   }
   int flags = 0;
-  SGP_CUDA(c, cudaMemcpyAsync(&flags, c->dI8Flags + 2, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(&flags, c->dI8Flags.as<int>() + 2, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   if (flags & 1)
     return fail(c, SGP_E_RANGE, "scaled squared norms exceed the operand range of the tensor-core distance contraction (4096); "
@@ -1094,7 +1095,8 @@ int sgp_cross_kernel(sgp_ctx* h, const double* X, int64_t n, double* K_out) {
   double* dK = dX + static_cast<size_t>(n) * c->d;
   SGP_CUDA(c, cudaMemcpyAsync(dX, X, static_cast<size_t>(n) * c->d * 8, cudaMemcpyHostToDevice, c->stream));
   if (c->kf.n_terms > 0) {
-    SGP_CUDA(c, launch_cross_kernel(dK, dX, c->dZs, c->dBeta, c->kf, n, c->d, c->dpad, c->m, c->m_pad, c->stream));
+    SGP_CUDA(c, launch_cross_kernel(dK, dX, c->dZs.as<double>(), c->dBeta.as<double>(), c->kf, n, c->d, c->dpad, c->m,
+                                    c->m_pad, c->stream));
     c->launches += 1;
   } else {
     SGP_CUDA(c, cudaMemsetAsync(dK, 0, static_cast<size_t>(n) * c->m * 8, c->stream));

@@ -383,10 +383,10 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
 // G[i][j] (+ mirror) += sum_s Gpart[s][i][j] for i >= j ;  b[i] += sum_s bpart[s][i]
 __global__ void gram_reduce_kernel(double* __restrict__ G, double* __restrict__ b,
                                    const double* __restrict__ Gpart, const double* __restrict__ bpart,
-                                   int n_slices, int m, int m_pad, int col_lo, int col_hi) {
-  const int j = col_lo + blockIdx.x * blockDim.x + threadIdx.x;
+                                   int n_slices, int m, int m_pad) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const int i = blockIdx.y * blockDim.y + threadIdx.y;
-  if (j >= col_hi) return;
+  if (j >= m) return;
   if (i < m && j <= i) {
     double v = 0.0;
     const size_t stride = static_cast<size_t>(m_pad) * m_pad;
@@ -394,7 +394,7 @@ __global__ void gram_reduce_kernel(double* __restrict__ G, double* __restrict__ 
     G[static_cast<size_t>(i) * m + j] += v;
     if (i != j) G[static_cast<size_t>(j) * m + i] += v;
   }
-  if (blockIdx.y == 0 && threadIdx.y == 0 && j < m) {
+  if (blockIdx.y == 0 && threadIdx.y == 0) {
     double v = 0.0;
     for (int s = 0; s < n_slices; ++s) v += bpart[static_cast<size_t>(s) * m_pad + j];
     b[j] += v;
@@ -402,21 +402,21 @@ __global__ void gram_reduce_kernel(double* __restrict__ G, double* __restrict__ 
 }
 
 // Same for partial tiles stored at the MIRROR position (upper block triangle; the int8 kernel folds its accumulators
-// transposed so that its global writes coalesce): G[i][j] (+ mirror) += sum_s Gpart[s][i][j] for rows i in [row_lo, row_hi),
-// j >= i.  The int8 Gram and its digit-plane producer split the points into different slice counts.
+// transposed so that its global writes coalesce): G[i][j] (+ mirror) += sum_s Gpart[s][i][j] for j >= i.  The int8 Gram
+// and its digit-plane producer split the points into different slice counts.
 __global__ void gram_reduce_upper_kernel(double* __restrict__ G, double* __restrict__ b,
                                          const double* __restrict__ Gpart, const double* __restrict__ bpart,
-                                         int g_slices, int b_slices, int m, int m_pad, int row_lo, int row_hi) {
+                                         int g_slices, int b_slices, int m, int m_pad) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  const int i = row_lo + blockIdx.y * blockDim.y + threadIdx.y;
-  if (i < row_hi && j < m && j >= i) {
+  const int i = blockIdx.y * blockDim.y + threadIdx.y;
+  if (i < m && j < m && j >= i) {
     double v = 0.0;
     const size_t stride = static_cast<size_t>(m_pad) * m_pad;
     for (int s = 0; s < g_slices; ++s) v += Gpart[s * stride + static_cast<size_t>(i) * m_pad + j];
     G[static_cast<size_t>(i) * m + j] += v;
     if (i != j) G[static_cast<size_t>(j) * m + i] += v;
   }
-  if (blockIdx.y == 0 && threadIdx.y == 0 && j >= row_lo && j < row_hi) {
+  if (blockIdx.y == 0 && threadIdx.y == 0 && j < m) {
     double v = 0.0;
     for (int s = 0; s < b_slices; ++s) v += bpart[static_cast<size_t>(s) * m_pad + j];
     b[j] += v;
@@ -426,12 +426,10 @@ __global__ void gram_reduce_upper_kernel(double* __restrict__ G, double* __restr
 }  // namespace
 
 cudaError_t launch_gram_reduce_upper(double* G, double* b, const double* Gpart, const double* bpart, int g_slices,
-                                     int b_slices, int m, int m_pad, int row_lo, int row_hi, cudaStream_t s) {
-  if (row_hi > m) row_hi = m;
-  if (row_hi <= row_lo) return cudaSuccess;
+                                     int b_slices, int m, int m_pad, cudaStream_t s) {
   dim3 block(32, 8);
-  dim3 grid((m + 31) / 32, (row_hi - row_lo + 7) / 8);
-  gram_reduce_upper_kernel<<<grid, block, 0, s>>>(G, b, Gpart, bpart, g_slices, b_slices, m, m_pad, row_lo, row_hi);
+  dim3 grid((m + 31) / 32, (m + 7) / 8);
+  gram_reduce_upper_kernel<<<grid, block, 0, s>>>(G, b, Gpart, bpart, g_slices, b_slices, m, m_pad);
   return cudaGetLastError();
 }
 
@@ -460,19 +458,12 @@ cudaError_t launch_gram_f64(const GramParams& p, bool strict_elements, cudaStrea
   return cudaGetLastError();
 }
 
-cudaError_t launch_gram_reduce_cols(double* G, double* b, const double* Gpart, const double* bpart, int n_slices,
-                                    int m, int m_pad, int col_lo, int col_hi, cudaStream_t s) {
-  if (col_hi > m) col_hi = m;
-  if (col_hi <= col_lo) return cudaSuccess;
-  dim3 block(32, 8);
-  dim3 grid((col_hi - col_lo + 31) / 32, (m + 7) / 8);
-  gram_reduce_kernel<<<grid, block, 0, s>>>(G, b, Gpart, bpart, n_slices, m, m_pad, col_lo, col_hi);
-  return cudaGetLastError();
-}
-
 cudaError_t launch_gram_reduce(double* G, double* b, const double* Gpart, const double* bpart, int n_slices,
                                int m, int m_pad, cudaStream_t s) {
-  return launch_gram_reduce_cols(G, b, Gpart, bpart, n_slices, m, m_pad, 0, m, s);
+  dim3 block(32, 8);
+  dim3 grid((m + 31) / 32, (m + 7) / 8);
+  gram_reduce_kernel<<<grid, block, 0, s>>>(G, b, Gpart, bpart, n_slices, m, m_pad);
+  return cudaGetLastError();
 }
 
 }  // namespace sgp

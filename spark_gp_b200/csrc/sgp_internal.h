@@ -64,10 +64,22 @@ struct GramParams {
   int n_tiles_1d;       // m_pad / kTile
 };
 
-// Grow-only device scratch block owned by a context (no cudaMalloc / cudaFree in steady state).
+// Direct-distance mode of the int8 digit-plane producer (launch_i8_planes).
+struct I8Direct {
+  int on = 0;            // 1: exponents from fp32 direct-form distances on the CUDA cores (any norms, up to 4 terms)
+  int n_terms = 0, dpad4 = 0;
+  float w[4] = {0, 0, 0, 0};   // C_t / sum C
+  double csum = 0.0;     // sum of the term scales = the fixed-point scale
+};
+
+// Grow-only device buffer owned by a context (no cudaMalloc / cudaFree in steady state); freed by its destructor.
 struct DevScratch {
   void* p = nullptr;
   size_t cap = 0;
+  DevScratch() = default;
+  DevScratch(const DevScratch&) = delete;
+  DevScratch& operator=(const DevScratch&) = delete;
+  ~DevScratch() { if (p) cudaFree(p); }
   template <class T> T* as() const { return static_cast<T*>(p); }
 };
 
@@ -84,7 +96,7 @@ struct ExpertSet {
 struct Ctx {
   int device = 0;
   int precision = SGP_PREC_AUTO;
-  int last_path = -1;    // arithmetic path of the last statistics launch (SGP_PREC_F64 / _STRICT / _I8)
+  int last_path = -1;    // path of the last statistics launch (SGP_PREC_F64 / _F64_STRICT / _I8 / _I8_DIRECT)
   std::string err;
   cudaStream_t stream = nullptr;       // compute
   cudaStream_t copy_stream = nullptr;  // H2D staging
@@ -101,45 +113,45 @@ struct Ctx {
   int rank = 0, nranks = 1;
   int num_sms = kSMsH100;
 
-  // active set / kernel (valid after begin)
+  // active set / kernel (valid after a successful begin; the buffers are grow-only and may be larger than the shape)
   bool begun = false, finished = false, has_magic = false;
   int m = 0, d = 0, dpad = 0, m_pad = 0;
-  int alloc_terms = 0;   // term count the active-set buffers were sized for
   KernelFlat kf;
-  double* dZ = nullptr;      // m x d raw active set (fp64)
-  double* dZs = nullptr;     // [n_terms][m_pad][dpad]  Z * beta (K_mm, cross kernel, prediction)
-  double* dZc = nullptr;     // [n_terms][m_pad][dpad]  (Z - centre) * beta (fp64 statistics kernel)
-  double* dBeta = nullptr;   // [kMaxTerms][dpad], then [dpad] the centre of the fp64 statistics kernel
-  double* dGb = nullptr;     // packed [G (m*m) ; b (m)] -- one all-reduce
+  DevScratch dZ;      // m x d raw active set (fp64)
+  DevScratch dZs;     // [n_terms][m_pad][dpad]  Z * beta (K_mm, cross kernel, prediction)
+  DevScratch dZc;     // [n_terms][m_pad][dpad]  (Z - centre) * beta (fp64 statistics kernel)
+  DevScratch dBeta;   // [kMaxTerms][dpad], then [dpad] the centre of the fp64 statistics kernel
+  DevScratch dGb;     // packed [G (m*m) ; b (m) ; status] -- one all-reduce
   DevScratch gpart_ws, bpart_ws;   // per-slice partial tiles of the statistics kernels
   // int8 exact-accumulation path (gram_i8.cu operand preparation, gram_i8_wgmma.cu Gram kernel).  Two modes:
   // tensor-core distances (one non-Eye term, d <= 32) and direct fp32 distances (1..4 non-Eye terms, n_terms * dpad <= 72);
   // the first qualifies only where the second does, and both use the same scales, centre and active-set norm.
   bool i8_ok = false;            // the kernel/shape qualifies for tensor-core distances
   bool i8_direct_ok = false;     // ... for direct distances
-  double* dI8Scale = nullptr;    // [kMaxTerms][dpad] sqrt(log2 e) * beta_tk, then [dpad] centre (active-set mean)
+  DevScratch dI8Scale;           // [kMaxTerms][dpad] sqrt(log2 e) * beta_tk, then [dpad] centre (active-set mean)
   double i8_z_norm_mean = 0.0;   // mean scaled squared norm of the active set (widest term), for AUTO's budget
-  uint8_t* dI8Zt = nullptr;      // tensor-core mode: active-set operand images
+  I8Direct i8_direct;            // direct mode's term weights and fixed-point scale (used where i8_direct_ok)
+  DevScratch dI8Zt;              // tensor-core mode: active-set operand images
   DevScratch i8_zd_ws;           // direct mode: active-set tiles [tile][term][dpad][128] fp32
   bool i8d_prepared = false;     // ... built in this begin() window (on the first direct-mode launch)
   DevScratch i8_xt_ws, i8_ys_ws; // point operand images / tiles and fp32 y (scratch)
   DevScratch i8_planes_ws;       // digit planes of one launch window (at most kI8PlaneCapBytes)
-  int* dI8Flags = nullptr;       // [0] the window's int8 status, [1] the active set's (begin), [2] the K_nm sweep's
+  DevScratch dI8Flags;           // int [0] the window's int8 status, [1] the active set's (begin), [2] the K_nm sweep's
                                  // (reset to [1] by each host-form call); bit 0: scaled squared norm above
                                  // kI8TensorR2Max; bit 2: above kI8DirectR2Max
-  double* dI8NormSum = nullptr;  // [0]: sum of |x^|^2 over every int8 chunk since begin; [1]: first chunk of this call
-  int call_path = 0;             // AUTO's decision for the current accumulate call (taken on its first chunk): 0 fp64,
-                                 // 1 int8 Gram with tensor-core distances, 2 int8 Gram with direct fp32 distances
+  DevScratch dI8NormSum;         // [0]: sum of |x^|^2 over every int8 chunk since begin; [1]: first chunk of this call
+  int call_path = SGP_PREC_F64;  // path of the current accumulate call (AUTO decides on its first chunk: stats_path)
   int i8_flag_mask = 0;          // dI8Flags bits the int8 launches since begin can have set (0: no int8 launch)
   long long i8_points = 0;       // points that went through the int8 kernel since begin
   // per-expert objective state
-  ExpertSet ex;
+  ExpertSet ex;                  // view of ex_X, ex_y, ex_off, ex_f; E > 0 once an upload has completed
+  DevScratch ex_X, ex_y, ex_off, ex_f;
   DevScratch nll_per_ws;         // per-expert objective rows
   DevScratch hyper_ws;           // hyper-parameter descriptors + totals + flags of one evaluation
   bool bcm_general = false;      // the last sgp_bcm_nll took the global-memory LU path
   // tail / predict state
-  double* dMagicVec = nullptr;   // m
-  double* dMagicMat = nullptr;   // m x m
+  DevScratch dMagicVec;          // m
+  DevScratch dMagicMat;          // m x m
   // host->device staging (double buffered)
   DevScratch stage_x[2], stage_y[2];
   cudaEvent_t stage_free[2] = {nullptr, nullptr};   // recorded when the kernel consuming buffer i is done
@@ -149,8 +161,7 @@ struct Ctx {
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> gram_events;   // event POOL (created once, reused)
   size_t gram_events_used = 0;                                    // pairs recorded since the last begin
   cudaEvent_t user_events[8] = {nullptr};
-  float* dbgT = nullptr;       // sgp_debug_i8_tile
-  uint32_t* dbgW = nullptr;
+  DevScratch dbgT, dbgW;       // sgp_debug_i8_tile: fp32 T and uint32 words
 };
 
 // error helpers ---------------------------------------------------------------------------------
@@ -166,11 +177,9 @@ int fail(Ctx* c, int code, const std::string& msg);
 cudaError_t launch_gram_f64(const GramParams& p, bool strict_elements, cudaStream_t s);
 cudaError_t launch_gram_reduce(double* G /*m x m*/, double* b, const double* Gpart, const double* bpart,
                                int n_slices, int m, int m_pad, cudaStream_t s);
+// same for partial tiles at the mirror position (int8 Gram), with separate slice counts for G and b
 cudaError_t launch_gram_reduce_upper(double* G, double* b, const double* Gpart, const double* bpart, int g_slices,
-                                     int b_slices, int m, int m_pad, int row_lo, int row_hi, cudaStream_t s);
-// same, restricted to the G columns / b entries [col_lo, col_hi) (one int8 launch covers whole tile columns)
-cudaError_t launch_gram_reduce_cols(double* G, double* b, const double* Gpart, const double* bpart, int n_slices, int m,
-                                    int m_pad, int col_lo, int col_hi, cudaStream_t s);
+                                     int b_slices, int m, int m_pad, cudaStream_t s);
 // out = in * beta; out_centred (optional) = (in - centre) * beta; both zero padded to [rows_out][dpad]
 cudaError_t launch_scale_rows(double* out /*[rows][dpad]*/, double* out_centred, const double* in /*rows x d*/,
                               const double* beta, const double* centre, int rows_in, int rows_out, int d, int dpad,
@@ -209,12 +218,6 @@ cudaError_t launch_i8_prep_active_direct(float* Zd, const double* dZ, int m, int
 cudaError_t launch_i8_prep_points_direct(float* Xd, float* ys, const void* dX, int x_is_f32, const double* dy, long long n,
                                          int d, int dpad4, int n_terms, const double* dScale, const double* dCentre, int* flags,
                                          float r2max, double* dNormSum, double* dNormSumCall, cudaStream_t s);
-struct I8Direct {
-  int on = 0;            // 1: exponents from fp32 direct-form distances on the CUDA cores (any norms, up to 4 terms)
-  int n_terms = 0, dpad4 = 0;
-  float w[4] = {0, 0, 0, 0};   // C_t / sum C
-  double csum = 0.0;     // sum of the term scales = the fixed-point scale
-};
 
 // int8 Gram (gram_i8_wgmma.cu).  A launch window over n_units 64-point units is two kernels: the digit-plane producer
 // (kernel elements, their fixed-point digit planes in the workspace [n_units][m_pad / kTile][kI8PlaneBytes], and the

@@ -71,13 +71,17 @@ int run_tail(Ctx* c, double* magic_vector, double* magic_matrix) {
   const int m = c->m;
   const size_t mm = static_cast<size_t>(m) * m;
   cudaStream_t s = c->stream, s2 = c->tail_stream;
+  double* G = c->dGb.as<double>();
+  const double* b = G + mm;
+  double* mvec = c->dMagicVec.as<double>();
+  double* mmat = c->dMagicMat.as<double>();
   SGP_SOLVER(c, cusolverDnSetStream(c->solver, s));
   SGP_SOLVER(c, cusolverDnSetStream(c->solver2, s2));
 
   // ---- persistent workspaces -------------------------------------------------------------------------------
   int lw_potrf = 0, lw_eig = 0, lw_lu = 0;
-  SGP_SOLVER(c, cusolverDnDpotrf_bufferSize(c->solver, CUBLAS_FILL_MODE_LOWER, m, c->dGb, m, &lw_potrf));
-  SGP_SOLVER(c, cusolverDnDgetrf_bufferSize(c->solver, m, m, c->dGb, m, &lw_lu));
+  SGP_SOLVER(c, cusolverDnDpotrf_bufferSize(c->solver, CUBLAS_FILL_MODE_LOWER, m, G, m, &lw_potrf));
+  SGP_SOLVER(c, cusolverDnDgetrf_bufferSize(c->solver, m, m, G, m, &lw_lu));
   int lwork = lw_potrf > lw_lu ? lw_potrf : lw_lu;
   // layout of the one scratch block: [Kmm | A | invA | invK | Acopy] (mm doubles each) [work | work2] [ipiv] [info x 4]
   const size_t need = (5 * mm + 2 * static_cast<size_t>(lwork)) * 8 + static_cast<size_t>(m) * sizeof(int) + 64;
@@ -94,11 +98,9 @@ int run_tail(Ctx* c, double* magic_vector, double* magic_matrix) {
   int* info = ipiv + m;                                               // info[0]: A chain, info[1]: K_mm chain
 
   const double wn = c->kf.eye_sum;                                   // kernel.whiteNoiseVar
-  const double* G = c->dGb;
-  const double* b = c->dGb + mm;
 
   // K_mm = trainingKernel (PGPH:54) on the main stream; both chains need it
-  SGP_CUDA(c, launch_kmm_build(Kmm, c->dZs, nullptr, c->kf, m, c->m_pad, c->dpad, s));
+  SGP_CUDA(c, launch_kmm_build(Kmm, c->dZs.as<double>(), nullptr, c->kf, m, c->m_pad, c->dpad, s));
   SGP_CUDA(c, launch_axpby_diag(A, Kmm, G, wn, m, s));                                                 // PGPH:55-56
   c->launches += 2;
   SGP_CUDA(c, cudaMemcpyAsync(Acopy, A, mm * 8, cudaMemcpyDeviceToDevice, s));     // kept for the slow path
@@ -114,12 +116,12 @@ int run_tail(Ctx* c, double* magic_vector, double* magic_matrix) {
 
   // ---- chain 1 (main stream): Cholesky of A = PD check; magicVector = A \ b -----------------------------------
   SGP_SOLVER(c, cusolverDnDpotrf(c->solver, CUBLAS_FILL_MODE_LOWER, m, A, m, work, lwork, info));
-  SGP_CUDA(c, cudaMemcpyAsync(c->dMagicVec, b, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToDevice, s));
-  SGP_SOLVER(c, cusolverDnDpotrs(c->solver, CUBLAS_FILL_MODE_LOWER, m, 1, A, m, c->dMagicVec, m, info + 3));
+  SGP_CUDA(c, cudaMemcpyAsync(mvec, b, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToDevice, s));
+  SGP_SOLVER(c, cusolverDnDpotrs(c->solver, CUBLAS_FILL_MODE_LOWER, m, 1, A, m, mvec, m, info + 3));
   c->launches += 1;
-  // inv(A) goes into c->dMagicMat (finished in place below): invA is still K_mm's factor buffer on the other stream
-  SGP_CUDA(c, launch_set_identity(c->dMagicMat, m, s));
-  SGP_SOLVER(c, cusolverDnDpotrs(c->solver, CUBLAS_FILL_MODE_LOWER, m, m, A, m, c->dMagicMat, m, info + 3));
+  // inv(A) goes into mmat (finished in place below): invA is still K_mm's factor buffer on the other stream
+  SGP_CUDA(c, launch_set_identity(mmat, m, s));
+  SGP_SOLVER(c, cusolverDnDpotrs(c->solver, CUBLAS_FILL_MODE_LOWER, m, m, A, m, mmat, m, info + 3));
   c->launches += 1;
 
   int hinfo[2] = {0, 0};
@@ -153,8 +155,8 @@ int run_tail(Ctx* c, double* magic_vector, double* magic_matrix) {
       if (ev[i] < 0.0 || ev[i] != ev[i]) return fail(c, SGP_E_NOT_PD, kNotPdMsg);        // PGPH:62-65
     // semi-definite (or PD only to rounding): carry on with LU like the reference                      PGPH:59
     SGP_CUDA(c, cudaMemcpyAsync(A, Acopy, mm * 8, cudaMemcpyDeviceToDevice, s));
-    SGP_CUDA(c, cudaMemcpyAsync(c->dMagicVec, b, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToDevice, s));
-    rc = lu_inverse(c, c->solver, s, m, A, c->dMagicMat, c->dMagicVec, wk, ipiv, info);
+    SGP_CUDA(c, cudaMemcpyAsync(mvec, b, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToDevice, s));
+    rc = lu_inverse(c, c->solver, s, m, A, mmat, mvec, wk, ipiv, info);
     if (rc != SGP_OK) return rc;
   }
   if (!k_done) {
@@ -165,12 +167,12 @@ int run_tail(Ctx* c, double* magic_vector, double* magic_matrix) {
     if (rc != SGP_OK) return rc;
   }
   // magicMatrix = inv(A) * whiteNoiseVar - inv(K_mm)                                                    PGPH:59
-  SGP_CUDA(c, launch_magic_matrix(c->dMagicMat, c->dMagicMat, invK, wn, m, s));
+  SGP_CUDA(c, launch_magic_matrix(mmat, mmat, invK, wn, m, s));
   c->launches += 1;
 
   if (magic_vector)
-    SGP_CUDA(c, cudaMemcpyAsync(magic_vector, c->dMagicVec, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToHost, s));
-  if (magic_matrix) SGP_CUDA(c, cudaMemcpyAsync(magic_matrix, c->dMagicMat, mm * 8, cudaMemcpyDeviceToHost, s));
+    SGP_CUDA(c, cudaMemcpyAsync(magic_vector, mvec, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToHost, s));
+  if (magic_matrix) SGP_CUDA(c, cudaMemcpyAsync(magic_matrix, mmat, mm * 8, cudaMemcpyDeviceToHost, s));
   SGP_CUDA(c, cudaStreamSynchronize(s));
   c->has_magic = true;
   return SGP_OK;
@@ -195,17 +197,18 @@ int run_predict(Ctx* c, const double* X, long long n, double* mean_out, double* 
     const long long rn = (n - r0 < chunk) ? (n - r0) : chunk;
     SGP_CUDA(c, cudaMemcpyAsync(dX, X + static_cast<size_t>(r0) * d, static_cast<size_t>(rn) * d * 8,
                                 cudaMemcpyHostToDevice, s));
-    SGP_CUDA(c, launch_cross_kernel(dK, dX, c->dZs, c->dBeta, c->kf, rn, d, c->dpad, m, c->m_pad, s));
+    SGP_CUDA(c, launch_cross_kernel(dK, dX, c->dZs.as<double>(), c->dBeta.as<double>(), c->kf, rn, d, c->dpad, m,
+                                    c->m_pad, s));
     c->launches += 1;
     if (var_out) {
       // W (rn x m, row-major) = K * magicMatrix  ==  column-major  W^T = M * K^T     (plain library GEMM)
       const double one = 1.0, zero = 0.0;
       cublasStatus_t st = cublasDgemm(c->blas, CUBLAS_OP_N, CUBLAS_OP_N, m, static_cast<int>(rn), m, &one,
-                                      c->dMagicMat, m, dK, m, &zero, dW, m);
+                                      c->dMagicMat.as<double>(), m, dK, m, &zero, dW, m);
       if (st != CUBLAS_STATUS_SUCCESS) return fail(c, SGP_E_CUDA, "cublasDgemm status " + std::to_string((int)st));
     }
-    SGP_CUDA(c, launch_predict_finish(dMean, var_out ? dVar : nullptr, dK, var_out ? dW : nullptr, c->dMagicVec,
-                                      c->kf.self_kernel, rn, m, s));
+    SGP_CUDA(c, launch_predict_finish(dMean, var_out ? dVar : nullptr, dK, var_out ? dW : nullptr,
+                                      c->dMagicVec.as<double>(), c->kf.self_kernel, rn, m, s));
     c->launches += 1;
     SGP_CUDA(c, cudaMemcpyAsync(mean_out + r0, dMean, static_cast<size_t>(rn) * 8, cudaMemcpyDeviceToHost, s));
     if (var_out) SGP_CUDA(c, cudaMemcpyAsync(var_out + r0, dVar, static_cast<size_t>(rn) * 8, cudaMemcpyDeviceToHost, s));

@@ -672,7 +672,7 @@ def test_fixed_point_breaks_just_above_margin():
 
 
 # ---- the fp64 DMMA statistics kernel (kmn_gram_f64_kernel, csrc/gram_f64.cu) and the int8 direct-mode gate ----------
-# launch_stats (csrc/api.cu) runs one of four loop variants of the kernel and splits the points into slices:
+# launch_stats_f64 (csrc/api.cu) runs one of four loop variants of the kernel and splits the points into slices:
 #   SGP_PREC_F64 (and AUTO's fp64 path): fp32 elements on a 128 x 64 staircase of tiles (two CTAs per SM), the
 #     pipelined loop for one non-Eye term with dpad <= DC, else the generic loop (z reloaded per term and per DC-dim
 #     chunk, the terms summed into the panel);
