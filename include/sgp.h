@@ -179,16 +179,25 @@ int sgp_laplace_nll(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper
 /* The latent modes f (same packed expert-major order as the uploaded points): the `y := f` of GPCls:62-65. */
 int sgp_experts_get_f(sgp_ctx* ctx, double* f_out);
 
-/* Installs a caller-supplied (vector v, SYMMETRIC matrix M) in place of the pair sgp_magic computes, so that sgp_predict
- * returns  mean_t = k(x_t, Z) . v  and  var_t = selfKernel + k(x_t, Z) M k(x_t, Z)^T  for them.  This is the per-point
- * part of GreedilyOptimizingActiveSetProvider.getNext (commons/ActiveSetProvider.scala:109-113: p_i, q_i, mu_i are
- * exactly such forms with M = inv(K_mm), inv(sigma2 K_mm + G) and v = magicVector).  Needs sgp_stats_begin. */
+/* Installs a caller-supplied (vector v, m x m matrix M, row-major) in place of the pair sgp_magic computes, so that
+ * sgp_predict returns  mean_t = k(x_t, Z) . v  and  var_t = selfKernel + k(x_t, Z) M k(x_t, Z)^T  for them.  M need not be
+ * bit-symmetric: the variance is the quadratic form of M itself.  This is the per-point part of
+ * GreedilyOptimizingActiveSetProvider.getNext (commons/ActiveSetProvider.scala:109-113: p_i, q_i, mu_i are exactly such
+ * forms with M = inv(K_mm), inv(sigma2 K_mm + G) and v = magicVector).  Needs sgp_stats_begin. */
 int sgp_set_magic(sgp_ctx* ctx, const double* v, const double* M);
 
 /* ---- prediction:  GPC:121-125 for a block of test vectors ----------------------------------- */
-/* mean_t = k(x_t, Z) . magicVector ;  var_t = selfKernel + k(x_t,Z) magicMatrix k(x_t,Z)^T.
- * X: n x d row-major fp64 host.  var_out may be NULL. */
+/* mean_t = k(x_t, Z) . magicVector ;  var_t = selfKernel + k(x_t,Z) magicMatrix k(x_t,Z)^T, all in fp64 (kernel
+ * elements on the CUDA cores, the quadratic form on fp64 tensor cores over the packed triangle of M + M^T).
+ * X: n x d row-major fp64 host.  var_out may be NULL (mean only: the cross kernel never reaches device memory).
+ * SGP_E_STATE before sgp_magic / sgp_set_magic; n = 0 is a no-op.  A point's outputs do not depend on the call it
+ * arrives in: host and device entry, fp32 input and its fp64 upcast, one call or a split, with or without var_out (the
+ * mean) give the same bits.  Neither entry changes the statistics of an open begin..finish window. */
 int sgp_predict(sgp_ctx* ctx, const double* X, int64_t n, double* mean_out, double* var_out);
+/* Same, points already resident in device memory: dX is n x d row-major (fp64, or fp32 when x_is_f32 != 0), dMean and
+ * dVar (may be NULL) are device pointers.  Asynchronous on the context's stream: synchronise with sgp_sync before reading
+ * the outputs. */
+int sgp_predict_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n, double* dMean, double* dVar);
 
 /* ---- introspection (tests / bench) ---------------------------------------------------------- */
 /* Number of kernels this library launched on ctx since creation. */

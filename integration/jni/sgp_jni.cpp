@@ -105,6 +105,33 @@ JNIEXPORT void JNICALL Java_org_apache_spark_ml_commons_NativeProjectedProcess_m
   if (rc != SGP_OK) throw_for(env, ctx, rc);
 }
 
+// ---- prediction (GaussianProcessCommons.scala:121-125) ---------------------------------------------------------------
+// M may come in Breeze's column-major order: k M k^T = k M^T k^T, and the library reads M through its symmetric part.
+JNIEXPORT void JNICALL Java_org_apache_spark_ml_commons_NativeProjectedProcess_setMagic(
+    JNIEnv* env, jclass, jlong h, jdoubleArray magicVector, jdoubleArray magicMatrix) {
+  sgp_ctx* ctx = reinterpret_cast<sgp_ctx*>(h);
+  jdouble* mv = env->GetDoubleArrayElements(magicVector, nullptr);
+  jdouble* mm = env->GetDoubleArrayElements(magicMatrix, nullptr);
+  const int rc = sgp_set_magic(ctx, mv, mm);          // copies both before returning
+  env->ReleaseDoubleArrayElements(magicVector, mv, JNI_ABORT);
+  env->ReleaseDoubleArrayElements(magicMatrix, mm, JNI_ABORT);
+  if (rc != SGP_OK) throw_for(env, ctx, rc);
+}
+
+// a block of rows packed row-major by the Scala side: X (n*d doubles); var may be null (mean only)
+JNIEXPORT void JNICALL Java_org_apache_spark_ml_commons_NativeProjectedProcess_predict(
+    JNIEnv* env, jclass, jlong h, jdoubleArray X, jlong n, jdoubleArray mean, jdoubleArray var) {
+  sgp_ctx* ctx = reinterpret_cast<sgp_ctx*>(h);
+  jdouble* x = env->GetDoubleArrayElements(X, nullptr);   // not a critical region: sgp_predict copies and synchronises
+  jdouble* mo = env->GetDoubleArrayElements(mean, nullptr);
+  jdouble* vo = var ? env->GetDoubleArrayElements(var, nullptr) : nullptr;
+  const int rc = sgp_predict(ctx, x, n, mo, vo);
+  env->ReleaseDoubleArrayElements(X, x, JNI_ABORT);
+  env->ReleaseDoubleArrayElements(mean, mo, 0);
+  if (vo) env->ReleaseDoubleArrayElements(var, vo, 0);
+  if (rc != SGP_OK) throw_for(env, ctx, rc);
+}
+
 // ---- hyper-parameter objective (GaussianProcessCommons.scala:73-78 treeAggregate of likelihoodAndGradient) ----------
 // experts of this executor, packed expert-major by the Scala side: X (n*d), y (n), offsets (E+1)
 JNIEXPORT void JNICALL Java_org_apache_spark_ml_commons_NativeProjectedProcess_expertsUpload(

@@ -21,6 +21,34 @@ private[ml] object NativeProjectedProcess {
   @native def finish(ctx: Long, g: Array[Double], b: Array[Double]): Unit
   @native def magic(ctx: Long, g: Array[Double], b: Array[Double], magicVector: Array[Double],
                     magicMatrix: Array[Double]): Unit
+  /** Installs (magicVector, magicMatrix) for predict; the matrix may be Breeze's column-major array (same quadratic form). */
+  @native def setMagic(ctx: Long, magicVector: Array[Double], magicMatrix: Array[Double]): Unit
+  /** mean (and var, unless null) of n rows of x (row-major): GaussianProjectedProcessRawPredictor.predict, GPC:121-125. */
+  @native def predict(ctx: Long, x: Array[Double], n: Long, mean: Array[Double], variance: Array[Double]): Unit
+
+  /** Scores one partition's rows with the model (kernel, activeSet, magicVector, magicMatrix): one native context per
+    * task (device = partitionId % nGPUs), rows in blocks of `block`.  What a model's `transform` maps over its partitions
+    * (`dataset.rdd.mapPartitionsWithIndex`), instead of one Breeze row at a time (GPC:121-125). */
+  def scorePartition(partitionId: Int, rows: Iterator[Vector], kernel: Kernel, activeSet: Array[Vector],
+                     magicVector: BDV[Double], magicMatrix: BDM[Double], withVariance: Boolean,
+                     nGPUs: Int = 8, block: Int = 32768): Iterator[(Double, Double)] = {
+    val m = activeSet.length
+    val d = activeSet.head.size
+    val terms = flatten(kernel)
+    val ctx = create(partitionId % nGPUs)
+    try {
+      begin(ctx, terms.map(_._1).toArray, terms.map(_._2).toArray, terms.map(_._3).toArray, terms.flatMap(_._4).toArray,
+        activeSet.flatMap(_.toArray), m, d)
+      setMagic(ctx, magicVector.toArray, magicMatrix.toArray)
+      rows.grouped(block).flatMap { blk =>
+        val n = blk.length
+        val mean = new Array[Double](n)
+        val variance = if (withVariance) new Array[Double](n) else null
+        predict(ctx, blk.flatMap(_.toArray).toArray, n.toLong, mean, variance)
+        mean.indices.iterator.map(i => (mean(i), if (withVariance) variance(i) else Double.NaN))
+      }.toVector.iterator                                   // materialised: the context is destroyed below
+    } finally destroy(ctx)
+  }
   // hyper-parameter objective: experts resident on the GPU, one native call per objective evaluation
   @native def expertsUpload(ctx: Long, x: Array[Double], y: Array[Double], offsets: Array[Long], d: Int): Unit
   /** [value, gradient...]; tol <= 0: regression NLL (GPR:55-68), tol > 0: the classifier's Laplace objective. */

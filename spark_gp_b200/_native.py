@@ -19,7 +19,7 @@ SGP_UNIQUE_ID_BYTES = 128
 # every symbol include/sgp.h declares (tests/test_abi.py checks the .so exports each of them)
 EXPORTS = ["sgp_ctx_create", "sgp_ctx_destroy", "sgp_last_error", "sgp_set_precision", "sgp_version",
            "sgp_comm_unique_id", "sgp_comm_init", "sgp_stats_begin", "sgp_stats_accumulate",
-           "sgp_stats_accumulate_device", "sgp_stats_finish", "sgp_sync", "sgp_magic", "sgp_predict",
+           "sgp_stats_accumulate_device", "sgp_stats_finish", "sgp_sync", "sgp_magic", "sgp_predict", "sgp_predict_device",
            "sgp_launch_count", "sgp_gram_kernel_time", "sgp_cross_kernel", "sgp_event_record",
            "sgp_event_elapsed_ms", "sgp_debug_i8_tile", "sgp_last_path", "sgp_experts_upload",
            "sgp_bcm_nll", "sgp_laplace_nll", "sgp_experts_get_f", "sgp_set_magic", "sgp_last_tail_path", "sgp_last_bcm_path", "sgp_experts_upload_grouped", "sgp_kmn_sweep", "sgp_kmn_sweep_device", "sgp_greedy_active_set", "sgp_kmeans"]
@@ -69,6 +69,7 @@ def load() -> C.CDLL:
     lib.sgp_sync.argtypes = [vp]
     lib.sgp_magic.argtypes = [vp, vp, vp, vp, vp]
     lib.sgp_predict.argtypes = [vp, vp, i64, vp, vp]
+    lib.sgp_predict_device.argtypes = [vp, vp, i32, i64, vp, vp]
     lib.sgp_set_magic.argtypes = [vp, vp, vp]
     lib.sgp_launch_count.argtypes = [vp]
     lib.sgp_launch_count.restype = i64

@@ -5,7 +5,7 @@ from __future__ import annotations
 import numpy as np
 from scipy.optimize import minimize
 
-from .engine import ProjectedProcessEngine
+from .engine import ProjectedProcessEngine, is_cuda_tensor
 from .hyperopt import pack_experts, group_for_experts
 from .regression import GaussianProcessParams, GaussianProjectedProcessRawPredictor
 
@@ -18,7 +18,11 @@ class GaussianProcessClassificationModel:
         self.numClasses = 2
 
     def predictRaw(self, features):
-        """(-f, f) per row (GPCls:153-156)."""
+        """(-f, f) per row (GPCls:153-156).  A CUDA torch tensor stays on the device (CUDA float64 result)."""
+        if is_cuda_tensor(features):
+            import torch
+            f, _ = self.rawPredictor._engine.predict_tensor(features, with_variance=False)
+            return torch.stack([-f, f], dim=-1)
         f, _ = self.rawPredictor._engine.predict(np.asarray(features, dtype=np.float64), with_variance=False)
         return np.stack([-f, f], axis=-1)
 
@@ -26,6 +30,10 @@ class GaussianProcessClassificationModel:
         """raw2probabilityInPlace (GPCls:140-148), quirk included: values(0) = sigmoid(-values(0)) = sigmoid(f), so the
         probability column puts sigmoid(f) on class 0 although f > 0 votes for class 1."""
         raw = self.predictRaw(features)
+        if is_cuda_tensor(raw):
+            import torch
+            p0 = 1.0 / (1.0 + torch.exp(raw[..., 0]))
+            return torch.stack([p0, 1.0 - p0], dim=-1)
         p0 = 1.0 / (1.0 + np.exp(raw[..., 0]))          # sigmoid(-(-f))
         return np.stack([p0, 1.0 - p0], axis=-1)
 
@@ -33,7 +41,11 @@ class GaussianProcessClassificationModel:
         """ClassificationModel.predict = raw2prediction(predictRaw(x)); with no thresholds set (the reference sets none)
         Spark's ProbabilisticClassificationModel.raw2prediction is `rawPrediction.argmax`, i.e. class 1 iff f > 0 (first
         maximum on a tie) -- NOT the argmax of the (quirky) probability vector."""
-        return np.argmax(self.predictRaw(features), axis=-1).astype(np.float64)
+        raw = self.predictRaw(features)
+        if is_cuda_tensor(raw):
+            import torch
+            return torch.argmax(raw, dim=-1).to(torch.float64)
+        return np.argmax(raw, axis=-1).astype(np.float64)
 
 
 class GaussianProcessClassifier(GaussianProcessParams):

@@ -84,17 +84,18 @@ static int flatten_kernel(Ctx* c, const sgp_kernel_desc* k, int d, int beta_stri
 // Streams the host rows X (n rows of `row` bytes) and y through the two staging buffers, so that the copy of one chunk
 // (copy_stream) overlaps the kernels of the previous one (compute stream).  The first chunk has `first` points, the
 // others `chunk` (first <= chunk); launch(dX, dy, p0, cn) enqueues the consumer of points [p0, p0 + cn) on the compute
-// stream.  Returns when every copy is done: the caller may reuse X and y.
+// stream.  y may be NULL (points without labels: dy is then NULL).  Returns when every copy is done: the caller may
+// reuse X and y.
 template <class Launch>
 static int stage_rows(Ctx* c, const void* X, const double* y, long long n, size_t row, long long first, long long chunk,
                       Launch&& launch) {
-  const size_t xb = row * chunk, yb = static_cast<size_t>(chunk) * 8;
+  const size_t xb = row * chunk, yb = y ? static_cast<size_t>(chunk) * 8 : 0;
   if (xb > c->stage_x[0].cap || yb > c->stage_y[0].cap) {
     SGP_CUDA(c, cudaStreamSynchronize(c->stream));
     SGP_CUDA(c, cudaStreamSynchronize(c->copy_stream));
     for (int i = 0; i < 2; ++i) {
       int rc = ctx_scratch(c, c->stage_x[i], xb);
-      if (rc == SGP_OK) rc = ctx_scratch(c, c->stage_y[i], yb);
+      if (rc == SGP_OK && yb > 0) rc = ctx_scratch(c, c->stage_y[i], yb);
       if (rc != SGP_OK) return rc;
       SGP_CUDA(c, cudaEventRecord(c->stage_free[i], c->stream));
     }
@@ -104,10 +105,10 @@ static int stage_rows(Ctx* c, const void* X, const double* y, long long n, size_
   for (long long p0 = 0, step = first; p0 < n; p0 += step, step = chunk, buf ^= 1) {
     const long long cn = (n - p0 < step) ? (n - p0) : step;
     void* sx = c->stage_x[buf].p;
-    double* sy = c->stage_y[buf].as<double>();
+    double* sy = y ? c->stage_y[buf].as<double>() : nullptr;
     SGP_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->stage_free[buf], 0));
     SGP_CUDA(c, cudaMemcpyAsync(sx, Xb + static_cast<size_t>(p0) * row, row * cn, cudaMemcpyHostToDevice, c->copy_stream));
-    SGP_CUDA(c, cudaMemcpyAsync(sy, y + p0, static_cast<size_t>(cn) * 8, cudaMemcpyHostToDevice, c->copy_stream));
+    if (y) SGP_CUDA(c, cudaMemcpyAsync(sy, y + p0, static_cast<size_t>(cn) * 8, cudaMemcpyHostToDevice, c->copy_stream));
     SGP_CUDA(c, cudaEventRecord(c->stage_ready[buf], c->copy_stream));
     SGP_CUDA(c, cudaStreamWaitEvent(c->stream, c->stage_ready[buf], 0));
     const int rc = launch(sx, sy, p0, cn);
@@ -394,6 +395,8 @@ int sgp_ctx_create(sgp_ctx** out, int device) {
   for (int i = 0; i < 2; ++i) {
     cudaEventCreateWithFlags(&c->stage_free[i], cudaEventDisableTiming);
     cudaEventCreateWithFlags(&c->stage_ready[i], cudaEventDisableTiming);
+    cudaEventCreateWithFlags(&c->out_ready[i], cudaEventDisableTiming);
+    cudaEventCreateWithFlags(&c->out_free[i], cudaEventDisableTiming);
   }
   if ((e = cudaStreamCreateWithFlags(&c->tail_stream, cudaStreamNonBlocking)) != cudaSuccess ||
       (e = cudaEventCreateWithFlags(&c->tail_fork, cudaEventDisableTiming)) != cudaSuccess ||
@@ -416,6 +419,8 @@ int sgp_ctx_destroy(sgp_ctx* h) {
   for (int i = 0; i < 2; ++i) {
     if (c->stage_free[i]) cudaEventDestroy(c->stage_free[i]);
     if (c->stage_ready[i]) cudaEventDestroy(c->stage_ready[i]);
+    if (c->out_ready[i]) cudaEventDestroy(c->out_ready[i]);
+    if (c->out_free[i]) cudaEventDestroy(c->out_free[i]);
   }
   if (c->comm && nccl().ok) nccl().CommDestroy(c->comm);
   if (c->tail_fork) cudaEventDestroy(c->tail_fork);
@@ -470,7 +475,7 @@ int sgp_comm_init(sgp_ctx* h, const void* id128, int rank, int nranks) {
 int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32_t m, int32_t d) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
-  c->begun = c->finished = c->has_magic = false;   // a begin that fails leaves no window open
+  c->begun = c->finished = c->has_magic = c->magic_packed = false;   // a begin that fails leaves no window open
   if (!k || !Z || m <= 0 || d <= 0 || k->n_terms <= 0 || !k->terms)
     return fail(c, SGP_E_BADARG, "sgp_stats_begin: null or empty argument");
   SGP_CUDA(c, cudaSetDevice(c->device));
@@ -660,9 +665,13 @@ int sgp_set_magic(sgp_ctx* h, const double* v, const double* M) {
   SGP_CUDA(c, cudaMemcpyAsync(c->dMagicMat.p, M, mm * 8, cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));          // the caller may reuse v, M as soon as we return
   c->has_magic = true;
+  c->magic_packed = false;
   return SGP_OK;
 }
 
+// The host rows stream in through the statistics path's double-buffered staging; each window's mean / variance go to one
+// of two device output buffers and are copied out (copy stream) once the NEXT window is queued, so that the copies in
+// both directions overlap the kernels.
 int sgp_predict(sgp_ctx* h, const double* X, int64_t n, double* mean_out, double* var_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
@@ -670,7 +679,64 @@ int sgp_predict(sgp_ctx* h, const double* X, int64_t n, double* mean_out, double
   if (n < 0 || (n > 0 && (!X || !mean_out))) return fail(c, SGP_E_BADARG, "null argument");
   if (n == 0) return SGP_OK;
   SGP_CUDA(c, cudaSetDevice(c->device));
-  return run_predict(c, X, n, mean_out, var_out);
+  // staged chunks of ~32 MB of X (at least 4096 points), never more than one kernel window
+  const size_t row = static_cast<size_t>(c->d) * sizeof(double);
+  const long long win = predict_window_points(c->m_pad);
+  long long chunk = std::max<long long>(4096, static_cast<long long>((size_t(32) << 20) / row));
+  chunk = std::min(std::min(chunk, win), static_cast<long long>(n));
+  int rc = predict_prepare(c, var_out != nullptr);
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->predict_out_ws, 4 * static_cast<size_t>(chunk) * sizeof(double));
+  if (rc != SGP_OK) return rc;
+  double* out = c->predict_out_ws.as<double>();      // [2][mean (chunk) | var (chunk)]
+  auto copy_out = [&](int b, long long p0, long long cn) -> int {
+    const double* dm = out + 2 * static_cast<size_t>(chunk) * b;
+    SGP_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->out_ready[b], 0));
+    SGP_CUDA(c, cudaMemcpyAsync(mean_out + p0, dm, static_cast<size_t>(cn) * 8, cudaMemcpyDeviceToHost, c->copy_stream));
+    if (var_out)
+      SGP_CUDA(c, cudaMemcpyAsync(var_out + p0, dm + chunk, static_cast<size_t>(cn) * 8, cudaMemcpyDeviceToHost,
+                                  c->copy_stream));
+    SGP_CUDA(c, cudaEventRecord(c->out_free[b], c->copy_stream));
+    return SGP_OK;
+  };
+  long long windows = 0, pending_p0 = 0, pending_n = 0;
+  rc = stage_rows(c, X, nullptr, n, row, chunk, chunk,
+                  [&](const void* dX, const double*, long long p0, long long cn) -> int {
+                    const int b = static_cast<int>(windows & 1);
+                    double* dm = out + 2 * static_cast<size_t>(chunk) * b;
+                    SGP_CUDA(c, cudaStreamWaitEvent(c->stream, c->out_free[b], 0));
+                    int r = predict_window(c, dX, 0, cn, dm, var_out ? dm + chunk : nullptr);
+                    if (r != SGP_OK) return r;
+                    SGP_CUDA(c, cudaEventRecord(c->out_ready[b], c->stream));
+                    if (windows > 0 && (r = copy_out(b ^ 1, pending_p0, pending_n)) != SGP_OK) return r;
+                    ++windows;
+                    pending_p0 = p0;
+                    pending_n = cn;
+                    return SGP_OK;
+                  });
+  if (rc == SGP_OK) rc = copy_out(static_cast<int>((windows - 1) & 1), pending_p0, pending_n);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaStreamSynchronize(c->copy_stream));
+  return SGP_OK;
+}
+
+int sgp_predict_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, int64_t n, double* dMean, double* dVar) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!c->has_magic) return fail(c, SGP_E_STATE, "sgp_magic should have been called first");
+  if (n < 0 || (n > 0 && (!dX || !dMean))) return fail(c, SGP_E_BADARG, "null argument");
+  if (n == 0) return SGP_OK;
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  int rc = predict_prepare(c, dVar != nullptr);
+  if (rc != SGP_OK) return rc;
+  const long long win = predict_window_points(c->m_pad);
+  const size_t row = static_cast<size_t>(c->d) * (x_is_f32 ? sizeof(float) : sizeof(double));
+  for (long long p0 = 0; p0 < n; p0 += win) {
+    const long long cn = (n - p0 < win) ? (n - p0) : win;
+    rc = predict_window(c, static_cast<const char*>(dX) + static_cast<size_t>(p0) * row, x_is_f32, cn, dMean + p0,
+                        dVar ? dVar + p0 : nullptr);
+    if (rc != SGP_OK) return rc;
+  }
+  return SGP_OK;
 }
 
 int64_t sgp_launch_count(const sgp_ctx* h) {

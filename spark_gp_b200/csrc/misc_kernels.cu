@@ -1,5 +1,5 @@
 // Small fp64 kernels around the hot path: active-set pre-scaling, K_mm (trainingKernel), the dense
-// cross kernel K(X*, Z) used by prediction and by the golden-vector tests, and element-wise pieces of
+// cross kernel K(X*, Z) of sgp_cross_kernel (golden-vector tests, greedy cross-check), and element-wise pieces of
 // the m x m tail.  All of these are O(m^2) or O(n_test * m) -- negligible next to the Gram kernel.
 #include "sgp_internal.h"
 
@@ -83,41 +83,6 @@ __global__ void magic_matrix_kernel(double* out, const double* invA, const doubl
                                     size_t n) {
   const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
   if (i < n) out[i] = invA[i] * wn - invK[i];   // PGPH:59
-}
-
-// mean_r = K[r,:] . mv ; var_r = self + K[r,:] . W[r,:]     (W = K * magicMatrix)      GPC:124
-__global__ void predict_finish_kernel(double* __restrict__ mean, double* __restrict__ var,
-                                      const double* __restrict__ K, const double* __restrict__ W,
-                                      const double* __restrict__ mv, double self_k, long long n, int m) {
-  const long long r = blockIdx.x;
-  if (r >= n) return;
-  double sm = 0.0, sv = 0.0;
-  for (int j = threadIdx.x; j < m; j += blockDim.x) {
-    const double k = K[static_cast<size_t>(r) * m + j];
-    sm = fma(k, mv[j], sm);
-    if (W) sv = fma(k, W[static_cast<size_t>(r) * m + j], sv);
-  }
-  __shared__ double red[2][32];
-  for (int o = 16; o > 0; o >>= 1) {
-    sm += __shfl_xor_sync(0xffffffffu, sm, o);
-    sv += __shfl_xor_sync(0xffffffffu, sv, o);
-  }
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) { red[0][w] = sm; red[1][w] = sv; }
-  __syncthreads();
-  if (w == 0) {
-    const int nw = blockDim.x >> 5;
-    sm = (l < nw) ? red[0][l] : 0.0;
-    sv = (l < nw) ? red[1][l] : 0.0;
-    for (int o = 16; o > 0; o >>= 1) {
-      sm += __shfl_xor_sync(0xffffffffu, sm, o);
-      sv += __shfl_xor_sync(0xffffffffu, sv, o);
-    }
-    if (l == 0) {
-      mean[r] = sm;
-      if (var) var[r] = self_k + sv;
-    }
-  }
 }
 
 // status words that must be agreed on by every rank travel inside the all-reduced buffers as doubles
@@ -221,12 +186,6 @@ cudaError_t launch_expert_offsets(long long* off, long long n, long long E, cuda
 cudaError_t launch_status_to_double(double* dst, const int* flags, int mask, const double* norm_sum, double norm_limit,
                                     cudaStream_t s) {
   status_to_double_kernel<<<1, 1, 0, s>>>(dst, flags, mask, norm_sum, norm_limit);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_predict_finish(double* mean, double* var, const double* K, const double* W, const double* mv,
-                                  double self_k, long long n, int m, cudaStream_t s) {
-  predict_finish_kernel<<<static_cast<unsigned>(n), 256, 0, s>>>(mean, var, K, W, mv, self_k, n, m);
   return cudaGetLastError();
 }
 

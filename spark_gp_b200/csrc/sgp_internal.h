@@ -36,6 +36,9 @@ constexpr int kMaxHypers = 72;     // hyper-parameters of one objective evaluati
 // launch window (3 bytes per point and padded active row: configs[1] 3.1 GB in one window, configs[3] 7.7 GB in two)
 constexpr size_t kI8PlaneBytes = 3 * kTile * 64;
 constexpr size_t kI8PlaneCapBytes = size_t(4) << 30;
+// prediction: the fp64 cross kernel of one window of points takes at most this much device memory (configs[1]'s m = 1000:
+// 32768 points per window)
+constexpr size_t kPredictKBytes = size_t(256) << 20;
 
 // Flattened, device-ready kernel description (built by sgp_stats_begin).
 struct KernelFlat {
@@ -152,10 +155,15 @@ struct Ctx {
   // tail / predict state
   DevScratch dMagicVec;          // m
   DevScratch dMagicMat;          // m x m
+  DevScratch dMagicPacked;       // m_pad x m_pad  triu(M + M^T, 1) + diag(M), built by the first variance call
+  bool magic_packed = false;     // dMagicPacked holds the installed magicMatrix
+  DevScratch predict_out_ws;     // sgp_predict: [2][mean | var] per window (double buffered)
   // host->device staging (double buffered)
   DevScratch stage_x[2], stage_y[2];
   cudaEvent_t stage_free[2] = {nullptr, nullptr};   // recorded when the kernel consuming buffer i is done
   cudaEvent_t stage_ready[2] = {nullptr, nullptr};  // recorded when the H2D into buffer i is done
+  cudaEvent_t out_ready[2] = {nullptr, nullptr};    // sgp_predict: the window writing output buffer i is done
+  cudaEvent_t out_free[2] = {nullptr, nullptr};     // sgp_predict: the device->host copy out of buffer i is done
   // instrumentation
   int64_t launches = 0;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> gram_events;   // event POOL (created once, reused)
@@ -198,9 +206,26 @@ cudaError_t launch_group_experts(double* Xe, double* ye, const void* dX, int x_i
 cudaError_t launch_expert_offsets(long long* off, long long n, long long E, cudaStream_t s);
 cudaError_t launch_status_to_double(double* dst, const int* flags, int mask, const double* norm_sum, double norm_limit,
                                     cudaStream_t s);
-cudaError_t launch_predict_finish(double* mean, double* var, const double* K /*n x m*/,
-                                  const double* W /*n x m = K*M*/, const double* mv, double self_k,
-                                  long long n, int m, cudaStream_t s);
+
+// Prediction (predict.cu) over one window of device-resident points.
+struct PredictArgs {
+  const void* X;         // n x d row-major, fp32 or fp64
+  int x_is_f32;
+  long long n;           // <= predict_window_points(m_pad)
+  int d, dpad, m, m_pad;
+  const KernelFlat* kf;
+  const double* Zc;      // [n_terms][m_pad][dpad] (Z - c) * beta
+  const double* beta;    // [kMaxTerms][dpad] beta, then [dpad] c
+  const double* v;       // m: magic vector
+  const double* B;       // m_pad x m_pad packed magic matrix (launch_pack_magic); variance only
+  double* ws;            // predict_ws_bytes(window, m_pad); variance only
+  double* mean;          // n
+  double* var;           // n, or nullptr: mean only
+};
+long long predict_window_points(int m_pad);
+size_t predict_ws_bytes(long long window, int m_pad);
+cudaError_t launch_pack_magic(double* B /*m_pad x m_pad*/, const double* M /*m x m*/, int m, int m_pad, cudaStream_t s);
+cudaError_t launch_predict(const PredictArgs& a, cudaStream_t s);
 
 // int8 exact-accumulation path
 size_t i8_points_scratch_bytes(long long n, int nchunks);
@@ -289,6 +314,9 @@ int run_kmeans(Ctx* c, const void* X, int x_is_f32, long long n, int d, int k, i
                const double* init_centers, double* centers_out, int* k_out, int* labels_out, int* iterations_out,
                double* cost_out);
 int run_tail(Ctx* c, double* magic_vector, double* magic_matrix);
-int run_predict(Ctx* c, const double* X, long long n, double* mean_out, double* var_out);
+// Prediction (tail.cu): predict_prepare sizes the workspace and packs the installed magic matrix (once per pair) for the
+// windows that follow; predict_window enqueues one window of at most predict_window_points(m_pad) device-resident points.
+int predict_prepare(Ctx* c, bool with_var);
+int predict_window(Ctx* c, const void* dX, int x_is_f32, long long n, double* dMean, double* dVar);
 
 }  // namespace sgp

@@ -1,4 +1,4 @@
-// The m x m tail (fp64, one GPU) and block prediction.
+// The m x m tail (fp64, one GPU) and the per-window launch of block prediction (kernels in predict.cu).
 //
 //   commons/ProjectedGaussianProcessHelper.scala:49-65   getMagicVector + assertSymPositiveDefinite
 //   commons/GaussianProcessCommons.scala:118-126         GaussianProjectedProcessRawPredictor.predict
@@ -175,45 +175,32 @@ int run_tail(Ctx* c, double* magic_vector, double* magic_matrix) {
   if (magic_matrix) SGP_CUDA(c, cudaMemcpyAsync(magic_matrix, mmat, mm * 8, cudaMemcpyDeviceToHost, s));
   SGP_CUDA(c, cudaStreamSynchronize(s));
   c->has_magic = true;
+  c->magic_packed = false;
   return SGP_OK;
 }
 
-int run_predict(Ctx* c, const double* X, long long n, double* mean_out, double* var_out) {
-  const int m = c->m, d = c->d;
-  cudaStream_t s = c->stream;
-  const long long chunk = 32768;
-  const long long cn = n < chunk ? n : chunk;
-  // one grow-only block: [X | K | W | mean | var]
-  const size_t xb = static_cast<size_t>(cn) * d, kb = static_cast<size_t>(cn) * m;
-  int rc = ctx_scratch(c, c->predict_ws, (xb + 2 * kb + 2 * static_cast<size_t>(cn)) * 8);
+int predict_prepare(Ctx* c, bool with_var) {
+  if (!with_var) return SGP_OK;                       // the mean-only kernel needs no workspace
+  int rc = ctx_scratch(c, c->predict_ws, predict_ws_bytes(predict_window_points(c->m_pad), c->m_pad));
+  if (rc != SGP_OK || c->magic_packed) return rc;
+  rc = ctx_scratch(c, c->dMagicPacked, static_cast<size_t>(c->m_pad) * c->m_pad * sizeof(double));
   if (rc != SGP_OK) return rc;
-  double* dX = static_cast<double*>(c->predict_ws.p);
-  double* dK = dX + xb;
-  double* dW = dK + kb;
-  double* dMean = dW + kb;
-  double* dVar = dMean + cn;
-  if (cublasSetStream(c->blas, s) != CUBLAS_STATUS_SUCCESS) return fail(c, SGP_E_CUDA, "cublasSetStream");
-  for (long long r0 = 0; r0 < n; r0 += chunk) {
-    const long long rn = (n - r0 < chunk) ? (n - r0) : chunk;
-    SGP_CUDA(c, cudaMemcpyAsync(dX, X + static_cast<size_t>(r0) * d, static_cast<size_t>(rn) * d * 8,
-                                cudaMemcpyHostToDevice, s));
-    SGP_CUDA(c, launch_cross_kernel(dK, dX, c->dZs.as<double>(), c->dBeta.as<double>(), c->kf, rn, d, c->dpad, m,
-                                    c->m_pad, s));
-    c->launches += 1;
-    if (var_out) {
-      // W (rn x m, row-major) = K * magicMatrix  ==  column-major  W^T = M * K^T     (plain library GEMM)
-      const double one = 1.0, zero = 0.0;
-      cublasStatus_t st = cublasDgemm(c->blas, CUBLAS_OP_N, CUBLAS_OP_N, m, static_cast<int>(rn), m, &one,
-                                      c->dMagicMat.as<double>(), m, dK, m, &zero, dW, m);
-      if (st != CUBLAS_STATUS_SUCCESS) return fail(c, SGP_E_CUDA, "cublasDgemm status " + std::to_string((int)st));
-    }
-    SGP_CUDA(c, launch_predict_finish(dMean, var_out ? dVar : nullptr, dK, var_out ? dW : nullptr,
-                                      c->dMagicVec.as<double>(), c->kf.self_kernel, rn, m, s));
-    c->launches += 1;
-    SGP_CUDA(c, cudaMemcpyAsync(mean_out + r0, dMean, static_cast<size_t>(rn) * 8, cudaMemcpyDeviceToHost, s));
-    if (var_out) SGP_CUDA(c, cudaMemcpyAsync(var_out + r0, dVar, static_cast<size_t>(rn) * 8, cudaMemcpyDeviceToHost, s));
-    SGP_CUDA(c, cudaStreamSynchronize(s));
-  }
+  SGP_CUDA(c, launch_pack_magic(c->dMagicPacked.as<double>(), c->dMagicMat.as<double>(), c->m, c->m_pad, c->stream));
+  c->launches += 1;
+  c->magic_packed = true;
+  return SGP_OK;
+}
+
+int predict_window(Ctx* c, const void* dX, int x_is_f32, long long n, double* dMean, double* dVar) {
+  PredictArgs a{};
+  a.X = dX; a.x_is_f32 = x_is_f32; a.n = n;
+  a.d = c->d; a.dpad = c->dpad; a.m = c->m; a.m_pad = c->m_pad;
+  a.kf = &c->kf;
+  a.Zc = c->dZc.as<double>(); a.beta = c->dBeta.as<double>(); a.v = c->dMagicVec.as<double>();
+  a.B = c->dMagicPacked.as<double>(); a.ws = c->predict_ws.as<double>();
+  a.mean = dMean; a.var = dVar;
+  SGP_CUDA(c, launch_predict(a, c->stream));
+  c->launches += dVar ? 3 : 1;
   return SGP_OK;
 }
 

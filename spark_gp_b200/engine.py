@@ -35,6 +35,11 @@ class OperandRangeError(SgpError):
     """SGP_E_RANGE: the int8 path cannot represent these coordinates; rerun in SGP_PREC_F64."""
 
 
+def is_cuda_tensor(x) -> bool:
+    """A CUDA torch tensor (checked without importing torch: the package has no hard torch dependency)."""
+    return type(x).__module__.partition(".")[0] == "torch" and bool(getattr(x, "is_cuda", False))
+
+
 def _make_desc(kernel: Kernel, d: int):
     terms = kernel.flatten()
     arr = (N.KernelTerm * len(terms))()
@@ -260,7 +265,7 @@ class ProjectedProcessEngine:
 
     # ---- predict --------------------------------------------------------------------------------------
     def set_magic(self, vector, matrix):
-        """Installs a caller-supplied (vector, symmetric matrix) for `predict`:  mean = k.v,  var = selfKernel + k M k^T
+        """Installs a caller-supplied (vector, matrix) for `predict`:  mean = k.v,  var = selfKernel + k M k^T
         (the per-point quadratic forms of the greedy active-set provider, ActiveSetProvider.scala:109-113)."""
         v = np.ascontiguousarray(vector, dtype=np.float64)
         M = np.ascontiguousarray(matrix, dtype=np.float64)
@@ -276,6 +281,33 @@ class ProjectedProcessEngine:
         var = np.empty(len(X)) if with_variance else None
         self._check(self._lib.sgp_predict(self._h, N.ptr(X), len(X), N.ptr(mean),
                                           N.ptr(var) if with_variance else None))
+        return mean, var
+
+    def predict_device(self, x_ptr: int, x_is_f32: bool, n: int, mean_ptr: int, var_ptr: int = 0):
+        """`sgp_predict_device` on device pointers (var_ptr 0: mean only); asynchronous on the context's stream (`sync`)."""
+        self._check(self._lib.sgp_predict_device(self._h, C.c_void_p(x_ptr), int(x_is_f32), n, C.c_void_p(mean_ptr),
+                                                 C.c_void_p(var_ptr) if var_ptr else None))
+
+    def predict_tensor(self, X, with_variance: bool = True):
+        """`predict` for a CUDA torch tensor on this context's device (n x d or d; float32 is read as it is, other dtypes
+        are converted to float64): (mean, var or None) as CUDA float64 tensors of n entries, without a host round trip."""
+        import torch
+        if X.device.type != "cuda" or X.device.index != self._device:
+            raise ValueError("predict: the tensor is on %s, the model on cuda:%d" % (X.device, self._device))
+        if X.dtype not in (torch.float32, torch.float64):
+            X = X.to(torch.float64)
+        X = X.contiguous()
+        if X.ndim == 1:
+            X = X[None, :]
+        if X.ndim != 2 or X.shape[1] != self.d:
+            raise ValueError("predict: features must be n x %d" % self.d)
+        n = X.shape[0]
+        mean = torch.empty(n, dtype=torch.float64, device=X.device)
+        var = torch.empty(n, dtype=torch.float64, device=X.device) if with_variance else None
+        torch.cuda.current_stream(X.device).synchronize()       # X may still be written on torch's stream
+        self.predict_device(X.data_ptr(), X.dtype == torch.float32, n, mean.data_ptr(),
+                            var.data_ptr() if var is not None else 0)
+        self.sync()
         return mean, var
 
     def cross_kernel(self, X):

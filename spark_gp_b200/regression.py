@@ -10,7 +10,7 @@ from __future__ import annotations
 import numpy as np
 
 from . import _native as N
-from .engine import ProjectedProcessEngine, OperandRangeError, NotPositiveDefiniteException
+from .engine import ProjectedProcessEngine, OperandRangeError, NotPositiveDefiniteException, is_cuda_tensor
 from .kernels import Kernel, RBFKernel, EyeKernel, const
 
 
@@ -208,7 +208,11 @@ class GaussianProjectedProcessRawPredictor:
             pass
 
     def predict(self, features):
-        """(mean, variance) for one vector or a block of vectors."""
+        """(mean, variance) for one vector or a block of vectors.  A CUDA torch tensor stays on the device: the results
+        are CUDA float64 tensors (0-dim for one vector)."""
+        if is_cuda_tensor(features):
+            mean, var = self._engine.predict_tensor(features, with_variance=True)
+            return (mean[0], var[0]) if features.ndim == 1 else (mean, var)
         f = np.asarray(features, dtype=np.float64)
         mean, var = self._engine.predict(f, with_variance=True)
         if f.ndim == 1:
@@ -224,6 +228,9 @@ class GaussianProcessRegressionModel:
         self.hyperparameters = hyperparameters
 
     def predict(self, features):
+        if is_cuda_tensor(features):                 # CUDA torch tensor in, CUDA float64 tensor out
+            mean, _ = self.rawPredictor._engine.predict_tensor(features, with_variance=False)
+            return mean[0] if features.ndim == 1 else mean
         f = np.asarray(features, dtype=np.float64)
         mean, _ = self.rawPredictor._engine.predict(f, with_variance=False)
         return float(mean[0]) if f.ndim == 1 else mean
