@@ -149,9 +149,8 @@ static double stats_scales(const double* Z, int m, int d, int dpad, int n_terms,
     ctr64[j] = sd > 0.0 ? std::nearbyint(ctr[j] / sd) * sd : ctr[j];
   }
   if (!with_scales) return 0.0;
-  const double s2 = std::sqrt(1.4426950408889634074);          // sqrt(log2 e): exponent in base 2
   for (int t = 0; t < n_terms; ++t)
-    for (int j = 0; j < d; ++j) sc[static_cast<size_t>(t) * dpad + j] = s2 * beta[static_cast<size_t>(t) * dpad + j];
+    for (int j = 0; j < d; ++j) sc[static_cast<size_t>(t) * dpad + j] = kSqrtLog2e * beta[static_cast<size_t>(t) * dpad + j];
   double best = 1e300;
   for (int t = 0; t < n_terms; ++t) {
     const double* st = sc.data() + static_cast<size_t>(t) * dpad;
@@ -239,8 +238,8 @@ static int launch_stats_f64(Ctx* c, bool strict, const void* dX, int x_is_f32, c
   p.X = dX; p.y = dy; p.n = n; p.x_is_f32 = x_is_f32;
   p.d = c->d; p.dpad = c->dpad; p.m = c->m; p.m_pad = c->m_pad;
   p.n_terms = c->kf.n_terms;
-  for (int t = 0; t < kMaxTerms; ++t) p.scale[t] = c->kf.scale[t];
-  p.Zs = c->dZc.as<double>(); p.beta = c->dBeta.as<double>();
+  std::copy(c->kf.scale, c->kf.scale + kMaxTerms, p.scale);
+  p.Zc = c->dZc.as<double>(); p.beta = c->dBeta.as<double>();
   p.Gpart = c->gpart_ws.as<double>(); p.bpart = c->bpart_ws.as<double>();
   p.n_slices = n_slices; p.n_tiles_1d = nt1;
   SGP_CUDA(c, launch_gram_f64(p, strict, c->stream));
@@ -847,8 +846,7 @@ int objective_setup(Ctx* c, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   int rc = flatten_kernel(c, k, d, d, kf, beta, &flat_of);
   if (rc != SGP_OK) return rc;
   hv = HyperView{};
-  hv.d = d; hv.n_terms = kf.n_terms; hv.eye_sum = kf.eye_sum; hv.n_hypers = nh;
-  std::copy(kf.scale, kf.scale + kMaxTerms, hv.scale);
+  hv.d = d; hv.kf = kf; hv.n_hypers = nh;
   std::vector<int> kind(nh), hterm(nh, 0), hdim(nh, 0);
   std::vector<double> coef(static_cast<size_t>(nh) * (kMaxTerms + 1), 0.0), value(nh, 0.0);
   for (int i = 0; i < nh; ++i) {
@@ -937,14 +935,14 @@ int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   // reference's own arithmetic, LU with partial pivoting and log|det| with the sign dropped (logDetAndInv.scala:36-63,
   // GPR:59), on kernel matrices staged in global memory.  The choice is rank-local; the one all-reduce per evaluation
   // happens afterwards on every rank.
-  ObjectivePlan plan = plan_objective(Objective::kBcm, c->ex, hv.n_terms);
+  ObjectivePlan plan = plan_objective(Objective::kBcm, c->ex, hv.kf.n_terms);
   if (plan.variant != ObjectiveVariant::kLu) {
     SGP_CUDA(c, launch_bcm_nll(plan, c->ex, hv, rows, dTotal, dFlags, c->stream));
     c->launches += 2;
     int flags = 0;
     SGP_CUDA(c, cudaMemcpyAsync(&flags, dFlags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-    if (flags & 1) plan = plan_objective(Objective::kBcmLu, c->ex, hv.n_terms);
+    if (flags & 1) plan = plan_objective(Objective::kBcmLu, c->ex, hv.kf.n_terms);
   }
   c->bcm_general = plan.variant == ObjectiveVariant::kLu;
   if (c->bcm_general) {
@@ -972,7 +970,7 @@ int sgp_laplace_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hyper
   int* dFlags = nullptr;
   int rc = objective_setup(c, k, hypers, nh, hv, dTotal, dFlags);
   if (rc != SGP_OK) return rc;
-  const ObjectivePlan plan = plan_objective(Objective::kLaplace, c->ex, hv.n_terms);
+  const ObjectivePlan plan = plan_objective(Objective::kLaplace, c->ex, hv.kf.n_terms);
   if (plan.variant == ObjectiveVariant::kRefused)
     return fail(c, SGP_E_BADARG, "datasetSizeForExpert too large for the on-chip Laplace kernel (max ~115 points per expert)");
   SGP_CUDA(c, launch_laplace(plan, c->ex, hv, tol, c->nll_per_ws.as<double>(), dTotal, dFlags, c->stream));

@@ -155,14 +155,14 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
     double* kp = Ks + a * NP + b;
     *kp = (a < n && b < n) ? exp(-*kp) : 0.0;
   }
-  const double scale0 = p.hv.scale[0];
+  const double scale0 = p.hv.kf.term_scale(0);
 #pragma unroll
   for (int r = 0; r < RBR; ++r)
 #pragma unroll
     for (int c = 0; c < RBC; ++c) {
       const int a = ty + 32 * r, b = tx + 16 * c;
       const bool real = a < n && b < n;
-      A[r][c] = real ? fma(scale0, Ks[a * NP + b], (a == b) ? p.hv.eye_sum : 0.0) : ((a == b) ? 1.0 : 0.0);
+      A[r][c] = real ? fma(scale0, Ks[a * NP + b], (a == b) ? p.hv.kf.eye_sum : 0.0) : ((a == b) ? 1.0 : 0.0);
     }
   // ---- n sweeps: A -> -K^-1.  Pivot k = 16 ck + kx sits in row block rk = ck / 2 (ty == 16 (ck % 2) + kx) ------------------
   bool bad = false;

@@ -52,16 +52,16 @@ __device__ __forceinline__ void ex_build_kernel(const HyperView& hv, const doubl
   for (int a = warp; a < n; a += EX_WARPS) {
     for (int b = lane; b <= a; b += 32) {
       double v = 0.0;
-      for (int t = 0; t < hv.n_terms; ++t) {
+      for (int t = 0; t < hv.kf.n_terms; ++t) {
         const double* bt = hv.beta + t * hv.d;
         double q = 0.0;
         for (int k = 0; k < hv.d; ++k) {
           const double df = (Xe[a * xld + k] - Xe[b * xld + k]) * bt[k];
           q = fma(df, df, q);
         }
-        v += hv.scale[t] * exp(-q);
+        v = hv.kf.fold_term(v, t, q);
       }
-      if (a == b) v += hv.eye_sum;
+      if (a == b) v += hv.kf.eye_sum;
       K[a * ld + b] = v;
       if (MIRROR) K[b * ld + a] = v;
     }
@@ -164,7 +164,7 @@ __device__ __forceinline__ void ex_gradient_emit(const HyperView& hv, int sw, in
     if (sw == 0) {
 #pragma unroll
     for (int t = 0; t < kMaxTerms; ++t) {
-      if (t < hv.n_terms) {
+      if (t < hv.kf.n_terms) {
         const double s_ = ex_block_sum<NW>(S[t], red), q_ = ex_block_sum<NW>(Q[t], red);
         if (tid == 0) { sS[t] = s_; sQ[t] = q_; }
       }
@@ -187,15 +187,15 @@ __device__ __forceinline__ void ex_gradient_emit(const HyperView& hv, int sw, in
     if (kind == 0) {                                                 // trainable scalar above a sub-tree
       const double* cf = hv.h_coef + static_cast<size_t>(i) * (kMaxTerms + 1);
       g = cf[kMaxTerms] * sTr[0];
-      for (int t = 0; t < hv.n_terms; ++t) g = fma(cf[t], sS[t], g);
+      for (int t = 0; t < hv.kf.n_terms; ++t) g = fma(cf[t], sS[t], g);
     } else if (kind == 1) {                                          // ARD beta_k
       const int t = hv.h_term[i], k = hv.h_dim[i];
       mine = (t == ts && k >= k0 && k < k0 + kn);
-      if (mine) g = hv.scale[t] * (-2.0 * hv.h_value[i]) * sD[k - k0];
+      if (mine) g = hv.kf.term_scale(t) * (-2.0 * hv.h_value[i]) * sD[k - k0];
     } else {                                                         // RBF sigma
       const int t = hv.h_term[i];
       const double sg = hv.h_value[i];
-      g = hv.scale[t] * sQ[t] / (sg * sg * sg);
+      g = hv.kf.term_scale(t) * sQ[t] / (sg * sg * sg);
     }
     if (mine) out[i] = factor * g;
   }
@@ -209,7 +209,7 @@ __device__ __forceinline__ void ex_descriptor_gradient(const HyperView& hv, cons
                                                        double factor, double* out, double* sums, double* red) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int chunks = (hv.d + DCH - 1) / DCH;
-  const int n_sweeps = hv.any_ard ? hv.n_terms * chunks : 1;
+  const int n_sweeps = hv.any_ard ? hv.kf.n_terms * chunks : 1;
   for (int sw = 0; sw < n_sweeps; ++sw) {
     const int ts = hv.any_ard ? sw / chunks : -1;
     const int k0 = hv.any_ard ? (sw % chunks) * DCH : 0;
@@ -226,7 +226,7 @@ __device__ __forceinline__ void ex_descriptor_gradient(const HyperView& hv, cons
         double kws = 0.0;
 #pragma unroll
         for (int t = 0; t < kMaxTerms; ++t) {
-          if (t < hv.n_terms && (sw == 0 || t == ts)) {
+          if (t < hv.kf.n_terms && (sw == 0 || t == ts)) {
             const double* bt = hv.beta + t * hv.d;
             double q = 0.0, s2 = 0.0;
             for (int k = 0; k < hv.d; ++k) {

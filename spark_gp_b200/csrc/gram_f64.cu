@@ -48,7 +48,7 @@ constexpr int NT = 256;           // threads per CTA (8 warps: 4 x 2 grid of 32x
 template <typename ET> struct ElemOps;
 template <> struct ElemOps<float> {
   // coordinates are pre-scaled by sqrt(log2 e) at staging time, so exp(-q) = 2^(-q'): one MUFU.EX2 (2 ulp)
-  static constexpr double kPrescale = 1.2011224087864498;     // sqrt(log2(e))
+  static constexpr double kPrescale = kSqrtLog2e;
   static __device__ __forceinline__ float ex(float q) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(-q));
@@ -134,7 +134,7 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
 
   // Both operands are centred on c (the row after the kMaxTerms beta rows of p.beta; within half a standard deviation of
   // the active-set mean) in fp64 before they are rounded to ET: x~ = (x - c) beta here, z~ = (Z - c) beta once per
-  // begin() (p.Zs).  Uncentred, the rounding error of every staged coordinate would grow with |x| beta -- the distance
+  // begin() (p.Zc).  Uncentred, the rounding error of every staged coordinate would grow with |x| beta -- the distance
   // from the origin in length scales -- instead of with the spread of the data.
   static_assert(NT % DC == 0, "a thread stages the same feature dim of every point it stages");
   const double* centre = p.beta + kMaxTerms * p.dpad;
@@ -142,7 +142,7 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
   auto load_z_chunk = [&](int term, int c0, int clen) {
     // (threads 192..255 of a 128x64 tile have no column: their zrow may point past the padded active set)
     const bool in_range = zrow < p.m_pad;
-    const double* src = p.Zs + (static_cast<size_t>(term) * p.m_pad + (in_range ? zrow : 0)) * p.dpad + c0;
+    const double* src = p.Zc + (static_cast<size_t>(term) * p.m_pad + (in_range ? zrow : 0)) * p.dpad + c0;
     for (int k = 0; k < clen; ++k) zs[((k >> 2) * 256 + tid) * 4 + (k & 3)] = in_range ? static_cast<ET>(kZSign * ElemOps<ET>::kPrescale * src[k]) : ET(0);
   };
   auto load_x_chunk = [&](long long pt0, int term, int c0, int clen) {

@@ -20,27 +20,22 @@
 namespace sgp {
 namespace {
 
-struct GreedyTerms {
-  int n_terms;
-  double scale[kMaxTerms];
-};
-
 // out[i] = sum_t C_t exp(-sum_k ((x_ik - x_jk) beta_tk)^2): the cross kernel of every point against point j (Eye terms add
 // nothing to a cross kernel, kernel/Kernel.scala:157)
 __global__ void greedy_column_kernel(double* __restrict__ out, const double* __restrict__ X, long long n, int d,
-                                     long long j, const double* __restrict__ beta /*[n_terms][d]*/, GreedyTerms tm) {
+                                     long long j, const double* __restrict__ beta /*[n_terms][d]*/, const KernelFlat kf) {
   const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   if (i >= n) return;
   const double* xi = X + static_cast<size_t>(i) * d;
   const double* xj = X + static_cast<size_t>(j) * d;
   double v = 0.0;
-  for (int t = 0; t < tm.n_terms; ++t) {
+  for (int t = 0; t < kf.n_terms; ++t) {
     double q = 0.0;
     for (int k = 0; k < d; ++k) {
       const double df = xi[k] * beta[t * d + k] - xj[k] * beta[t * d + k];      // same form as cross_kernel_kernel
       q = fma(df, df, q);
     }
-    v += tm.scale[t] * exp(-q);
+    v = kf.fold_term(v, t, q);
   }
   out[i] = v;
 }
@@ -192,9 +187,6 @@ int run_greedy(Ctx* c, const KernelFlat& kf, const std::vector<double>& beta_fla
   SGP_BLAS(c, cublasSetStream(c->blas, s));
   SGP_BLAS(c, cublasSetPointerMode(c->blas, CUBLAS_POINTER_MODE_HOST));
 
-  GreedyTerms tm;
-  tm.n_terms = kf.n_terms;
-  for (int t = 0; t < kMaxTerms; ++t) tm.scale[t] = t < kf.n_terms ? kf.scale[t] : 0.0;
   const double kii = kf.self_kernel, s2n = kf.eye_sum;    // trainingKernelDiag (Kernel.scala:111-114), whiteNoiseVar (ASP:76)
 
   // ---- host state: inv(K_mm), inv(A), b, magic vector --------------------------------------------------------------------
@@ -208,7 +200,7 @@ int run_greedy(Ctx* c, const KernelFlat& kf, const std::vector<double>& beta_fla
     indices_out[m] = idx;
     if (m == M - 1) break;                                  // the last point needs no scores
     double* krow = Kt + static_cast<size_t>(m) * N;
-    greedy_column_kernel<<<nblk, 256, 0, s>>>(krow, dX, n, d, idx, dbeta, tm);
+    greedy_column_kernel<<<nblk, 256, 0, s>>>(krow, dX, n, d, idx, dbeta, kf);
     SGP_CUDA(c, cudaGetLastError());
     c->launches += 1;
     // g = K_mn k* over the m + 1 rows (the last entry is k*.k*), beta = k*.y;  c = K_mn[:, idx]

@@ -20,17 +20,15 @@ __global__ void scale_rows_kernel(double* __restrict__ out, double* __restrict__
   if (out_centred) out_centred[idx] = in_range ? (v - centre[k]) * beta[k] : 0.0;
 }
 
-struct Scales { double s[kMaxTerms]; };
-
 // K_mm[i][j] = sum_t C_t exp(-|z~_ti - z~_tj|^2) + (i==j) * eye_sum        kernel/Kernel.scala:151,
 // kernel/ARDRBFKernel.scala:48-59, kernel/SumOfKernels.scala:45
-__global__ void kmm_build_kernel(double* __restrict__ Kmm, const double* __restrict__ Zs, Scales sc, int n_terms,
-                                 double eye_sum, int m, int m_pad, int dpad) {
+__global__ void kmm_build_kernel(double* __restrict__ Kmm, const double* __restrict__ Zs, const KernelFlat kf, int m,
+                                 int m_pad, int dpad) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const int i = blockIdx.y * blockDim.y + threadIdx.y;
   if (i >= m || j >= m) return;
   double v = 0.0;
-  for (int t = 0; t < n_terms; ++t) {
+  for (int t = 0; t < kf.n_terms; ++t) {
     const double* zi = Zs + (static_cast<size_t>(t) * m_pad + i) * dpad;
     const double* zj = Zs + (static_cast<size_t>(t) * m_pad + j) * dpad;
     double q = 0.0;
@@ -38,22 +36,22 @@ __global__ void kmm_build_kernel(double* __restrict__ Kmm, const double* __restr
       const double df = zi[k] - zj[k];
       q = fma(df, df, q);
     }
-    v += sc.s[t] * exp(-q);
+    v = kf.fold_term(v, t, q);
   }
-  if (i == j) v += eye_sum;
+  if (i == j) v += kf.eye_sum;
   Kmm[static_cast<size_t>(i) * m + j] = v;
 }
 
 // K[r][j] = sum_t C_t exp(-sum_k ((x_rk * beta_tk) - z~_tjk)^2)        kernel/Kernel.scala:69-74 contract:
 // rows = test vectors, cols = training (here: active-set) vectors.  Eye terms add nothing (Kernel.scala:157).
 __global__ void cross_kernel_kernel(double* __restrict__ K, const double* __restrict__ X,
-                                    const double* __restrict__ Zs, const double* __restrict__ beta, Scales sc,
-                                    int n_terms, long long n, int d, int dpad, int m, int m_pad) {
+                                    const double* __restrict__ Zs, const double* __restrict__ beta, const KernelFlat kf,
+                                    long long n, int d, int dpad, int m, int m_pad) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const long long r = blockIdx.y * static_cast<long long>(blockDim.y) + threadIdx.y;
   if (r >= n || j >= m) return;
   double v = 0.0;
-  for (int t = 0; t < n_terms; ++t) {
+  for (int t = 0; t < kf.n_terms; ++t) {
     const double* zj = Zs + (static_cast<size_t>(t) * m_pad + j) * dpad;
     const double* bt = beta + t * dpad;
     const double* xr = X + static_cast<size_t>(r) * d;
@@ -62,7 +60,7 @@ __global__ void cross_kernel_kernel(double* __restrict__ K, const double* __rest
       const double df = xr[k] * bt[k] - zj[k];
       q = fma(df, df, q);
     }
-    v += sc.s[t] * exp(-q);
+    v = kf.fold_term(v, t, q);
   }
   K[static_cast<size_t>(r) * m + j] = v;
 }
@@ -121,12 +119,6 @@ __global__ void expert_offsets_kernel(long long* __restrict__ off, long long n, 
   off[e] = e * kq + (e < r ? e : r);
 }
 
-Scales to_scales(const KernelFlat& kf) {
-  Scales s;
-  for (int t = 0; t < kMaxTerms; ++t) s.s[t] = kf.scale[t];
-  return s;
-}
-
 }  // namespace
 
 cudaError_t launch_scale_rows(double* out, double* out_centred, const double* in, const double* beta, const double* centre,
@@ -137,10 +129,10 @@ cudaError_t launch_scale_rows(double* out, double* out_centred, const double* in
   return cudaGetLastError();
 }
 
-cudaError_t launch_kmm_build(double* Kmm, const double* Zs, const double*, const KernelFlat& kf, int m, int m_pad,
-                             int dpad, cudaStream_t s) {
+cudaError_t launch_kmm_build(double* Kmm, const double* Zs, const KernelFlat& kf, int m, int m_pad, int dpad,
+                             cudaStream_t s) {
   dim3 block(32, 8), grid((m + 31) / 32, (m + 7) / 8);
-  kmm_build_kernel<<<grid, block, 0, s>>>(Kmm, Zs, to_scales(kf), kf.n_terms, kf.eye_sum, m, m_pad, dpad);
+  kmm_build_kernel<<<grid, block, 0, s>>>(Kmm, Zs, kf, m, m_pad, dpad);
   return cudaGetLastError();
 }
 
@@ -148,7 +140,7 @@ cudaError_t launch_cross_kernel(double* K, const double* X, const double* Zs, co
                                 const KernelFlat& kf, long long n, int d, int dpad, int m, int m_pad,
                                 cudaStream_t s) {
   dim3 block(32, 8), grid((m + 31) / 32, static_cast<unsigned>((n + 7) / 8));
-  cross_kernel_kernel<<<grid, block, 0, s>>>(K, X, Zs, beta, to_scales(kf), kf.n_terms, n, d, dpad, m, m_pad);
+  cross_kernel_kernel<<<grid, block, 0, s>>>(K, X, Zs, beta, kf, n, d, dpad, m, m_pad);
   return cudaGetLastError();
 }
 

@@ -33,8 +33,8 @@ struct ElemParams {
   int x_is_f32;
   long long n;            // points of the window
   long long rows_out;     // rows of K to write (>= n, padded rows get zeros)
-  int d, dpad, m, m_pad, n_terms;
-  double scale[kMaxTerms];
+  int d, dpad, m, m_pad;
+  KernelFlat kf;
   const double* Zc;       // [n_terms][m_pad][dpad] (Z - c) * beta (zero padded)
   const double* beta;     // [kMaxTerms][dpad] beta, then [dpad] the centre c
   const double* v;        // m: magic vector
@@ -60,7 +60,7 @@ __global__ void __launch_bounds__(kElemThreads, 1) predict_elements_kernel(const
     double e[kElemPts];
 #pragma unroll
     for (int i = 0; i < kElemPts; ++i) e[i] = 0.0;
-    for (int t = 0; t < p.n_terms; ++t) {
+    for (int t = 0; t < p.kf.n_terms; ++t) {
       double q[kElemPts];
 #pragma unroll
       for (int i = 0; i < kElemPts; ++i) q[i] = 0.0;
@@ -99,9 +99,8 @@ __global__ void __launch_bounds__(kElemThreads, 1) predict_elements_kernel(const
           }
         }
       }
-      const double sc = t == 0 ? p.scale[0] : t == 1 ? p.scale[1] : t == 2 ? p.scale[2] : p.scale[3];  // no local copy
 #pragma unroll
-      for (int pp = 0; pp < kElemPts; ++pp) e[pp] = fma(sc, exp(-q[pp]), e[pp]);
+      for (int pp = 0; pp < kElemPts; ++pp) e[pp] = p.kf.fold_term(e[pp], t, q[pp]);
     }
     const int j = ct * kElemCols + col;
     const bool zvalid = j < p.m;
@@ -296,8 +295,7 @@ cudaError_t launch_predict(const PredictArgs& a, cudaStream_t s) {
   double* K = a.var ? a.ws : nullptr;
   ElemParams p{};
   p.X = a.X; p.x_is_f32 = a.x_is_f32; p.n = a.n; p.rows_out = rows;
-  p.d = a.d; p.dpad = a.dpad; p.m = a.m; p.m_pad = a.m_pad; p.n_terms = a.kf->n_terms;
-  for (int t = 0; t < kMaxTerms; ++t) p.scale[t] = a.kf->scale[t];
+  p.d = a.d; p.dpad = a.dpad; p.m = a.m; p.m_pad = a.m_pad; p.kf = a.kf;
   p.Zc = a.Zc; p.beta = a.beta; p.v = a.v; p.K = K; p.mean = a.mean;
   const long long cta_rows = a.var ? rows : a.n;
   predict_elements_kernel<<<static_cast<unsigned>((cta_rows + kElemCtaPts - 1) / kElemCtaPts), kElemThreads, 0, s>>>(p);
@@ -312,7 +310,7 @@ cudaError_t launch_predict(const PredictArgs& a, cudaStream_t s) {
   predict_var_kernel<<<static_cast<unsigned>(n_rt) * n_ct, kVarThreads, kVarSmem, s>>>(K, a.B, a.n, a.m_pad, n_rt, n_ct,
                                                                                      vpart);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  predict_var_reduce_kernel<<<static_cast<unsigned>((a.n + 255) / 256), 256, 0, s>>>(vpart, a.n, n_ct, a.kf->self_kernel,
+  predict_var_reduce_kernel<<<static_cast<unsigned>((a.n + 255) / 256), 256, 0, s>>>(vpart, a.n, n_ct, a.kf.self_kernel,
                                                                                     a.var);
   return cudaGetLastError();
 }

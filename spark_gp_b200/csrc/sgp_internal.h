@@ -40,12 +40,23 @@ constexpr size_t kI8PlaneCapBytes = size_t(4) << 30;
 // 32768 points per window)
 constexpr size_t kPredictKBytes = size_t(256) << 20;
 
-// Flattened, device-ready kernel description (built by sgp_stats_begin).
+// sqrt(log2 e): coordinates scaled by it turn exp(-q) into 2^(-q'), one ex2 (int8 modes, fp32 element of the fp64 Gram)
+constexpr double kSqrtLog2e = 0x1.337cc2183b050p+0;
+
+// Flattened kernel description (flatten_kernel in api.cu): k(x, z) = sum_t C_t exp(-q_t(x, z)) + [x == z] eye_sum over
+// the non-Eye terms t.  Kernels take it by value, as a parameter or inside their parameter struct.
 struct KernelFlat {
   int n_terms = 0;                 // non-Eye terms
   double scale[kMaxTerms] = {0};   // C_t
   double eye_sum = 0.0;            // sum of Eye coefficients = whiteNoiseVar
   double self_kernel = 0.0;        // sum of all scales (every leaf has k(x,x) = 1)
+
+  // C_t.  A select chain: a kernel parameter array indexed at run time would be copied to local memory.
+  __host__ __device__ double term_scale(int t) const {
+    return t == 0 ? scale[0] : t == 1 ? scale[1] : t == 2 ? scale[2] : scale[3];
+  }
+  // acc + C_t exp(-q) in fp64, one rounding for the product and the sum
+  __device__ double fold_term(double acc, int t, double q) const { return fma(term_scale(t), exp(-q), acc); }
 };
 
 // Launch parameters of the fused K_mn + Gram kernel (gram_f64.cu).
@@ -56,9 +67,11 @@ struct GramParams {
   int x_is_f32;
   int d, dpad;          // dpad = d rounded up to a multiple of 4
   int m, m_pad;         // m_pad = m rounded up to a multiple of kTile
+  // KernelFlat's n_terms and scale[], not the whole struct: the fp32-element kernel runs at its 128-register cap, and a
+  // larger parameter block moves its spills (1M x 16, m = 1000: 3 % slower, H100 SXM at 400 W)
   int n_terms;
   double scale[kMaxTerms];
-  const double* Zs;     // [n_terms][m_pad][dpad]  centred, beta-scaled active set (Z - centre) * beta (zero padded)
+  const double* Zc;    // [n_terms][m_pad][dpad]  centred, beta-scaled active set (Z - centre) * beta (zero padded)
   const double* beta;   // [kMaxTerms + 1][dpad]   per-term feature scales (zero padded), then the centre c of the
                         //                         staged coordinates (v - c) * beta (stats_scales in api.cu)
   double* Gpart;        // [n_slices][m_pad*m_pad] per-slice partial tiles (lower block triangle)
@@ -192,8 +205,8 @@ cudaError_t launch_gram_reduce_upper(double* G, double* b, const double* Gpart, 
 cudaError_t launch_scale_rows(double* out /*[rows][dpad]*/, double* out_centred, const double* in /*rows x d*/,
                               const double* beta, const double* centre, int rows_in, int rows_out, int d, int dpad,
                               cudaStream_t s);
-cudaError_t launch_kmm_build(double* Kmm /*m x m*/, const double* Zs, const double* scale_dev_or_null,
-                             const KernelFlat& kf, int m, int m_pad, int dpad, cudaStream_t s);
+cudaError_t launch_kmm_build(double* Kmm /*m x m*/, const double* Zs, const KernelFlat& kf, int m, int m_pad, int dpad,
+                             cudaStream_t s);
 cudaError_t launch_cross_kernel(double* K /*n x m*/, const double* X /*n x d*/, const double* Zs,
                                 const double* beta, const KernelFlat& kf, long long n, int d, int dpad,
                                 int m, int m_pad, cudaStream_t s);
@@ -213,7 +226,7 @@ struct PredictArgs {
   int x_is_f32;
   long long n;           // <= predict_window_points(m_pad)
   int d, dpad, m, m_pad;
-  const KernelFlat* kf;
+  KernelFlat kf;
   const double* Zc;      // [n_terms][m_pad][dpad] (Z - c) * beta
   const double* beta;    // [kMaxTerms][dpad] beta, then [dpad] c
   const double* v;       // m: magic vector
@@ -265,10 +278,9 @@ cudaError_t launch_kmn_sweep(const uint8_t* Xt, const uint8_t* Zt, long long n, 
 // Per-expert objectives (bcm_nll.cu, laplace.cu) ----------------------------------------------------------------------
 // Device-side view of the flattened kernel and the hyper-parameter descriptors of one evaluation.
 struct HyperView {
-  int d, n_terms;
-  double scale[kMaxTerms];
+  int d;
+  KernelFlat kf;
   const double* beta;        // [n_terms][d]  per-term coordinate scales (ARD betas; RBF: 1/(sqrt2 sigma))
-  double eye_sum;
   int n_hypers, any_ard;
   const int* h_kind;         // [n_hypers] 0 = SCALE, 1 = ARD_BETA, 2 = RBF_SIGMA
   const int* h_term;         // [n_hypers] flattened term index (ARD_BETA / RBF_SIGMA)

@@ -100,7 +100,7 @@ int run_tail(Ctx* c, double* magic_vector, double* magic_matrix) {
   const double wn = c->kf.eye_sum;                                   // kernel.whiteNoiseVar
 
   // K_mm = trainingKernel (PGPH:54) on the main stream; both chains need it
-  SGP_CUDA(c, launch_kmm_build(Kmm, c->dZs.as<double>(), nullptr, c->kf, m, c->m_pad, c->dpad, s));
+  SGP_CUDA(c, launch_kmm_build(Kmm, c->dZs.as<double>(), c->kf, m, c->m_pad, c->dpad, s));
   SGP_CUDA(c, launch_axpby_diag(A, Kmm, G, wn, m, s));                                                 // PGPH:55-56
   c->launches += 2;
   SGP_CUDA(c, cudaMemcpyAsync(Acopy, A, mm * 8, cudaMemcpyDeviceToDevice, s));     // kept for the slow path
@@ -195,7 +195,7 @@ int predict_window(Ctx* c, const void* dX, int x_is_f32, long long n, double* dM
   PredictArgs a{};
   a.X = dX; a.x_is_f32 = x_is_f32; a.n = n;
   a.d = c->d; a.dpad = c->dpad; a.m = c->m; a.m_pad = c->m_pad;
-  a.kf = &c->kf;
+  a.kf = c->kf;
   a.Zc = c->dZc.as<double>(); a.beta = c->dBeta.as<double>(); a.v = c->dMagicVec.as<double>();
   a.B = c->dMagicPacked.as<double>(); a.ws = c->predict_ws.as<double>();
   a.mean = dMean; a.var = dVar;
