@@ -214,3 +214,61 @@ def test_greedy_provider_deltas_and_selection():
     assert sel.shape == (6, d) and np.array_equal(sel[0], X[5])
     assert len({tuple(r) for r in sel}) == 6                               # distinct points on this data
     assert np.array_equal(sel, greedy_active_set(6, experts, fac, theta, X[5]))
+
+
+def test_greedy_vectorised_fold_matches_scalar_fold():
+    """fold_experts (all experts at once, what round_scores selects with) against _fold_expert per expert followed by
+    filter(!isNaN).max() (ASP:108-135), on coarse-rounded scores (plenty of ties) with NaNs, up to every expert poisoned."""
+    from oracle.active_set import _fold_expert, fold_experts
+    rng = np.random.default_rng(12)
+    for trial in range(300):
+        n = int(rng.integers(1, 120)); E = int(rng.integers(1, n + 1))
+        delta = np.round(rng.standard_normal(n), 1)
+        if trial % 3 == 0:
+            delta[rng.integers(n, size=int(rng.integers(1, 4)))] = np.nan
+        if trial % 17 == 0:
+            delta[:] = np.nan
+        best, best_idx, pick = fold_experts(delta, E)
+        want = None
+        for e in range(E):
+            md, mi = _fold_expert(delta[e::E])
+            assert (np.isnan(md) and np.isnan(best[e])) or md == best[e]
+            assert best_idx[e] == mi * E + e
+            if not np.isnan(md) and (want is None or not (want[0] >= md)):
+                want = (md, mi * E + e)
+        assert pick == (-1 if want is None else want[1])
+
+
+def test_greedy_round_scores_matches_get_next():
+    """round_scores (all N points at once, BLAS-3) against the oracle's per-expert candidate_deltas and get_next: the
+    deltas in both of its formulations, and the pick, for prefixes of 1 to 12 points; a NaN label poisons every expert."""
+    from oracle.active_set import candidate_deltas, get_next, round_scores
+    rng = np.random.default_rng(31)
+    for trial, (n, d, E) in enumerate([(150, 3, 7), (97, 2, 97), (240, 5, 1), (301, 4, 13)]):
+        X = rng.random((n, d)); y = np.sin(3 * X.sum(1)) + 0.1 * rng.standard_normal(n)
+        beta = rng.uniform(1.0, 3.0, d)
+        fac = oracle.get_kernel(lambda: 1.1 * oracle.ARDRBFKernel(beta) + oracle.const(0.5) * oracle.RBFKernel(0.7)
+                                + oracle.const(1) * oracle.EyeKernel(), 1e-2)
+        theta = fac().get_hyperparameters()
+        experts = [(y[e::E], fac().set_hyperparameters(theta).set_training_vectors(X[e::E])) for e in range(E)]
+        for r in (1, 2, 5, 12):
+            active_idx = rng.permutation(n)[:r]
+            rs = round_scores(X, y, active_idx, fac, theta, E)
+            inst = fac().set_hyperparameters(theta).set_training_vectors(X[active_idx])
+            kmm, s2 = inst.training_kernel(), inst.white_noise_var
+            g = sum(k.cross_kernel(X[active_idx]) @ k.cross_kernel(X[active_idx]).T for _, k in experts)
+            b = sum(k.cross_kernel(X[active_idx]) @ ye for ye, k in experts)
+            pdm = s2 * kmm + g
+            kinv, pinv, mv = np.linalg.inv(kmm), np.linalg.inv(pdm), np.linalg.solve(pdm, b)
+            for e, (ye, k) in enumerate(experts):
+                dv = candidate_deltas(k.cross_kernel(X[active_idx]), ye, k.training_kernel_diag(), kinv, pinv, mv, s2)
+                assert np.allclose(rs.delta[e::E], dv, rtol=1e-10, atol=1e-12)
+            assert np.allclose(rs.delta_chol, rs.delta, rtol=1e-9, atol=1e-11)
+            assert rs.min_eig_a > 0
+            assert np.array_equal(X[rs.pick], get_next(kmm, experts, X[active_idx], s2))
+        y_bad = y.copy(); y_bad[trial] = np.nan
+        rs = round_scores(X, y_bad, [0], fac, theta, E)
+        assert rs.pick == -1 and np.all(np.isnan(rs.best))
+        bad = [(y_bad[e::E], k) for e, (_, k) in enumerate(experts)]
+        with pytest.raises(ValueError, match="empty.max"):
+            get_next(fac().set_hyperparameters(theta).set_training_vectors(X[[0]]).training_kernel(), bad, X[[0]], s2)
