@@ -121,7 +121,9 @@ int sgp_stats_accumulate_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, 
 
 /* Sum over ranks (one ncclAllReduce of the packed [G;b], if a communicator exists), then copy out.
  * G_out: m x m fp64 (symmetric, so row-/column-major are the same bytes), b_out: m.  Either may be NULL
- * (statistics stay on the device for sgp_magic). */
+ * (statistics stay on the device for sgp_magic).  The first finish closes the window and decides its status; a repeated
+ * finish only copies out again and returns the same status.  A window whose finish returned SGP_E_RANGE keeps that
+ * status until the next begin: G_out / b_out are still copied out, but sgp_magic without G_in returns SGP_E_STATE. */
 int sgp_stats_finish(sgp_ctx* ctx, double* G_out, double* b_out);
 
 /* Block until the context's stream is idle (timing hygiene for callers using the _device entry). */
@@ -133,7 +135,11 @@ int sgp_sync(sgp_ctx* ctx);
  * A = whiteNoiseVar*K_mm + G; SGP_E_NOT_PD if any eigenvalue of A < 0; magicVector = A \ b;
  * magicMatrix = whiteNoiseVar*inv(A) - inv(K_mm).  Outputs may be NULL (kept on device for predict).
  * A successful Cholesky factorization of A proves "no eigenvalue < 0" and supplies the solves (SPD: same result as
- * the reference's LU to rounding); only if it breaks down does the call run the reference's literal dsyevd + LU sequence. */
+ * the reference's LU to rounding); only if it breaks down does the call run the reference's literal dsyevd + LU sequence.
+ * SGP_E_STATE without G_in before finish, or after a finish that returned SGP_E_RANGE.  Once its arguments and the
+ * window's state are accepted, the call uninstalls the pair of any earlier sgp_magic / sgp_set_magic: if it then fails
+ * (SGP_E_NOT_PD, SGP_E_SINGULAR, ...), sgp_predict and sgp_predict_device return SGP_E_STATE until a pair is installed
+ * again.  With G_in on a window that is still open, the window is closed and its accumulated statistics are replaced. */
 int sgp_magic(sgp_ctx* ctx, const double* G_in, const double* b_in,
               double* magic_vector /* m */, double* magic_matrix /* m x m */);
 

@@ -31,7 +31,7 @@ Versions are unpinned in the reference (transitive deps of spark-mllib 3.1.1,
 from .kernels import (Kernel, ARDRBFKernel, RBFKernel, EyeKernel, ConstantTimesKernel,
                       TrainableScalarTimesKernel, SumOfKernels, Scalar, WhiteNoiseKernel,
                       TrainingVectorsNotInitializedException, const)
-from .ppa import (get_matrix_kmn_knm_and_vector_kmny, get_magic_vector,
+from .ppa import (get_matrix_kmn_knm_and_vector_kmny, get_magic_vector, tail_errors,
                   NotPositiveDefiniteException, GaussianProjectedProcessRawPredictor,
                   get_kernel, group_for_experts, get_expert_labels_and_kernels,
                   projected_process)

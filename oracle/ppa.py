@@ -80,6 +80,39 @@ def get_magic_vector(kernel: Kernel, matrix_kmn_knm: np.ndarray, vector_kmny: np
     return magic_vector, magic_matrix
 
 
+def tail_errors(kernel: Kernel, matrix_kmn_knm: np.ndarray, vector_kmny: np.ndarray, magic_vector: np.ndarray,
+                magic_matrix: np.ndarray) -> dict:
+    """How far a computed pair (v, M) is from `get_magic_vector`'s, in units of the fp64 unit roundoff u = 2^-53.
+    `kernel` has the active set as training vectors; A0 = whiteNoiseVar K0 + G is built here in fp64.
+      omega : componentwise backward error of v, max_i |A0 v - b|_i / (|A0| |v| + |b|)_i, over u;
+      fwd_v : |v - v0|_inf / |v0|_inf over kappa_inf(A0) u, v0 the LU solution;
+      fwd_M : max |M - M0| over u (wn kappa_inf(A0) max|inv A0| + kappa_inf(K0) max|inv K0|),
+              M0 = wn inv(A0) - inv(K0).
+    A backward-stable tail keeps each of them at a small multiple of 1 whatever the conditioning."""
+    u = np.finfo(np.float64).eps / 2
+    K0 = kernel.training_kernel()
+    wn = kernel.white_noise_var
+    A0 = wn * K0 + matrix_kmn_knm
+    b = np.asarray(vector_kmny, dtype=np.float64)
+    v = np.asarray(magic_vector, dtype=np.float64)
+    M = np.asarray(magic_matrix, dtype=np.float64)
+    r = np.abs(A0 @ v - b)
+    den = np.abs(A0) @ np.abs(v) + np.abs(b)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        omega = float(np.max(np.where(r == 0, 0.0, r / den)))      # r > 0 over den = 0 counts as infinite
+    v0 = sla.lu_solve(sla.lu_factor(A0), b)
+    inv_a, inv_k = sla.inv(A0), sla.inv(K0)
+    kappa_a = np.linalg.norm(A0, np.inf) * np.linalg.norm(inv_a, np.inf)
+    kappa_k = np.linalg.norm(K0, np.inf) * np.linalg.norm(inv_k, np.inf)
+    v_scale = max(float(np.max(np.abs(v0))), np.finfo(np.float64).tiny)
+    M0 = inv_a * wn - inv_k
+    m_scale = u * (wn * kappa_a * np.max(np.abs(inv_a)) + kappa_k * np.max(np.abs(inv_k)))
+    return {"omega": omega / u,
+            "fwd_v": float(np.max(np.abs(v - v0))) / v_scale / (kappa_a * u),
+            "fwd_M": float(np.max(np.abs(M - M0))) / m_scale,
+            "kappa_A": float(kappa_a), "kappa_K": float(kappa_k)}
+
+
 class GaussianProjectedProcessRawPredictor:
     """GPC:118-126."""
 

@@ -474,7 +474,7 @@ int sgp_comm_init(sgp_ctx* h, const void* id128, int rank, int nranks) {
 int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32_t m, int32_t d) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
-  c->begun = c->finished = c->has_magic = c->magic_packed = false;   // a begin that fails leaves no window open
+  c->begun = c->finished = c->range_failed = c->has_magic = c->magic_packed = false;   // a failed begin leaves no window
   if (!k || !Z || m <= 0 || d <= 0 || k->n_terms <= 0 || !k->terms)
     return fail(c, SGP_E_BADARG, "sgp_stats_begin: null or empty argument");
   SGP_CUDA(c, cudaSetDevice(c->device));
@@ -614,12 +614,14 @@ int sgp_stats_finish(sgp_ctx* h, double* G_out, double* b_out) {
     }
     SGP_CUDA(c, cudaMemcpyAsync(&status, G + mm + c->m, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   }
+  const bool first = !c->finished;
   c->finished = true;
   if (G_out) SGP_CUDA(c, cudaMemcpyAsync(G_out, G, mm * 8, cudaMemcpyDeviceToHost, c->stream));
   if (b_out)
     SGP_CUDA(c, cudaMemcpyAsync(b_out, G + mm, static_cast<size_t>(c->m) * 8, cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (status != 0.0)
+  if (first) c->range_failed = status != 0.0;      // the window keeps its status: a repeated finish reports it again
+  if (c->range_failed)
     return fail(c, SGP_E_RANGE, "the int8 path cannot represent this shard on some rank (scaled squared norms outside the "
                                 "tensor-core operand range, scaled squared norms above AUTO's magnitude budget for tensor-core "
                                 "distances, or above the fp32 direct-distance limit); rerun the statistics with "
@@ -641,14 +643,19 @@ int sgp_magic(sgp_ctx* h, const double* G_in, const double* b_in, double* magic_
   if (!c) return SGP_E_BADARG;
   if (!c->begun) return fail(c, SGP_E_STATE, "sgp_stats_begin should have been called first");
   if ((G_in == nullptr) != (b_in == nullptr)) return fail(c, SGP_E_BADARG, "G_in and b_in must be given together");
+  if (!G_in && !c->finished) return fail(c, SGP_E_STATE, "sgp_stats_finish should have been called first");
+  if (!G_in && c->range_failed)
+    return fail(c, SGP_E_STATE, "the statistics of this window could not be represented (sgp_stats_finish returned "
+                                "SGP_E_RANGE): rerun them, or pass G_in and b_in");
+  // the installed pair is gone from here on: only a tail that succeeds installs one again
+  c->has_magic = c->magic_packed = false;
   SGP_CUDA(c, cudaSetDevice(c->device));
   const size_t mm = static_cast<size_t>(c->m) * c->m;
   if (G_in) {
     SGP_CUDA(c, cudaMemcpyAsync(c->dGb.p, G_in, mm * 8, cudaMemcpyHostToDevice, c->stream));
     SGP_CUDA(c, cudaMemcpyAsync(c->dGb.as<double>() + mm, b_in, static_cast<size_t>(c->m) * 8, cudaMemcpyHostToDevice, c->stream));
     c->finished = true;
-  } else if (!c->finished) {
-    return fail(c, SGP_E_STATE, "sgp_stats_finish should have been called first");
+    c->range_failed = false;
   }
   return run_tail(c, magic_vector, magic_matrix);
 }

@@ -131,6 +131,7 @@ struct Ctx {
 
   // active set / kernel (valid after a successful begin; the buffers are grow-only and may be larger than the shape)
   bool begun = false, finished = false, has_magic = false;
+  bool range_failed = false;           // the window's finish reported SGP_E_RANGE: its statistics are not a model's
   int m = 0, d = 0, dpad = 0, m_pad = 0;
   KernelFlat kf;
   DevScratch dZ;      // m x d raw active set (fp64)
