@@ -185,6 +185,24 @@ int sgp_laplace_nll(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper
 /* The latent modes f (same packed expert-major order as the uploaded points): the `y := f` of GPCls:62-65. */
 int sgp_experts_get_f(sgp_ctx* ctx, double* f_out);
 
+/* One-vs-rest (Spark's OneVsRest over the binary classifier): the uploaded y holds class indices 0 .. n_classes-1, and
+ * class c's binary problem has the labels (y == c).  Evaluates the Laplace objective of sgp_laplace_nll for the n_eval
+ * distinct classes listed in `classes`, each at its own hyper-parameters (kernels[i] and hypers[i * n_hypers ...]: the
+ * same kernel structure and descriptor layout for every class), in one launch over experts x classes.  Every class keeps
+ * its own latent modes on the device, [n_classes][n], allocated on first use and zero after every sgp_experts_upload* and
+ * whenever n_classes changes; the modes of classes not listed are left as they are.  Outputs per listed class, in the
+ * order of `classes`: neg_log_z_out[i], grad_out[i * n_hypers ...].  Class c's value, gradient and modes equal, bit for
+ * bit, what sgp_laplace_nll returns on an upload of the labels (y == c) with the same modes, whichever other classes are
+ * in the call.  With a communicator: one ncclAllReduce of the n_eval rows and n_eval status words.
+ * Errors: SGP_E_BADARG for bad or repeated class indices, a structure that differs between classes, and experts above the
+ * on-chip limit (as sgp_laplace_nll); SGP_E_NOT_PD naming the first listed class whose B broke down. */
+int sgp_laplace_nll_classes(sgp_ctx* ctx, int32_t n_classes, const int32_t* classes, int32_t n_eval,
+                            const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t n_hypers, double tol,
+                            double* neg_log_z_out /* n_eval */, double* grad_out /* n_eval x n_hypers */);
+/* Class cls's latent modes (packed expert-major order, n entries).  SGP_E_STATE before the first sgp_laplace_nll_classes
+ * after an upload; SGP_E_BADARG for cls outside [0, n_classes). */
+int sgp_experts_get_f_class(sgp_ctx* ctx, int32_t cls, double* f_out);
+
 /* Installs a caller-supplied (vector v, m x m matrix M, row-major) in place of the pair sgp_magic computes, so that
  * sgp_predict returns  mean_t = k(x_t, Z) . v  and  var_t = selfKernel + k(x_t, Z) M k(x_t, Z)^T  for them.  M need not be
  * bit-symmetric: the variance is the quadratic form of M itself.  This is the per-point part of

@@ -8,5 +8,5 @@ from .engine import (ProjectedProcessEngine, NotPositiveDefiniteException, Train
                      MatrixSingularException, SgpError, OperandRangeError)
 from .regression import (GaussianProcessRegression, GaussianProcessRegressionModel, RandomActiveSetProvider,
                          GreedilyOptimizingActiveSetProvider, KMeansActiveSetProvider)
-from .classification import GaussianProcessClassifier, GaussianProcessClassificationModel
+from .classification import GaussianProcessClassifier, GaussianProcessClassificationModel, OneVsRest, OneVsRestModel
 from .utils import scale

@@ -3,10 +3,10 @@ approximation per expert + the same projected-process model as regression with y
 from __future__ import annotations
 
 import numpy as np
-from scipy.optimize import minimize
 
+from . import _native as N
 from .engine import ProjectedProcessEngine, is_cuda_tensor
-from .hyperopt import pack_experts, group_for_experts
+from .hyperopt import group_for_experts, lbfgsb, lbfgsb_bounds, lbfgsb_lockstep
 from .regression import GaussianProcessParams, GaussianProjectedProcessRawPredictor
 
 
@@ -65,24 +65,18 @@ class GaussianProcessClassifier(GaussianProcessParams):
         groups = group_for_experts(len(X), self._datasetSizeForExpert)
         order = np.concatenate(groups)
         eng.experts_upload_grouped(X, y, self._datasetSizeForExpert)  # grouping on the device; f = zeros per expert (GPCls:53-55)
-        memo = {}
-
-        def objective(theta):                                       # memoised like DiffFunctionMemoized; f warm-starts
-            key = tuple(theta)
-            if key not in memo:
-                memo[key] = eng.laplace_nll(self.getKernel().setHyperparameters(np.asarray(theta)), self._tol)
-            return memo[key]
+        launches0 = eng.launch_count()
 
         if hyperparameters is None:
             k0 = self.getKernel()
             theta = k0.getHyperparameters()
-            if self._maxIter > 0 and len(theta) > 0:
-                lo, up = k0.hyperparameterBoundaries()
-                bounds = [(float(l), None if np.isinf(u) else float(u)) for l, u in zip(lo, up)]
-                res = minimize(objective, theta, jac=True, method="L-BFGS-B", bounds=bounds,
-                               options=dict(maxiter=self._maxIter, ftol=self._tol, gtol=self._tol))
+            if self._maxIter > 0 and len(theta) > 0:                # memoised like DiffFunctionMemoized; f warm-starts
+                res, evaluations = lbfgsb(
+                    lambda t: eng.laplace_nll(self.getKernel().setHyperparameters(t), self._tol),
+                    theta, lbfgsb_bounds(k0), self._maxIter, self._tol)
                 theta = np.asarray(res.x, dtype=np.float64)
-                self.last_objective = dict(value=float(res.fun), evaluations=len(memo), iterations=int(res.nit))
+                self.last_objective = dict(value=float(res.fun), evaluations=evaluations, iterations=int(res.nit),
+                                           launches=eng.launch_count() - launches0)
         else:
             theta = np.asarray(hyperparameters, dtype=np.float64)
         # GPCls:60: run the Laplace loop once more at the optimum so every expert's f is the mode at theta*
@@ -92,9 +86,150 @@ class GaussianProcessClassifier(GaussianProcessParams):
         f[order] = f_packed
         self.last_latent = f
         # GPCls:62-65 -> produceModel with (f, kernel): the same projected-process path as regression
-        active_set = self._activeSetProvider(self._activeSetSize, X, f, self.getKernel, theta, self._seed, gp=self)
-        kernel = self.getKernel().setHyperparameters(theta)
-        G, b = eng.statistics(kernel, active_set, X, f)             # same helper as regression (fp64-kernel fallback)
-        mv, mm = eng.magic()
-        self.last_stats = (G, b)
+        kernel, active_set, mv, mm, self.last_stats = _produce_model(self, eng, X, f, theta)
         return GaussianProcessClassificationModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, active_set), theta)
+
+
+def _produce_model(gp, eng, X, f, theta):
+    """GPCls:62-65: the active set, the statistics with y := f and the tail, on eng.  Returns (kernel, active set, magic
+    vector, magic matrix, (G, b))."""
+    active_set = gp._activeSetProvider(gp._activeSetSize, X, f, gp.getKernel, theta, gp._seed, gp=gp)
+    kernel = gp.getKernel().setHyperparameters(theta)
+    G, b = eng.statistics(kernel, active_set, X, f)                 # same helper as regression (fp64-kernel fallback)
+    mv, mm = eng.magic()
+    return kernel, active_set, mv, mm, (G, b)
+
+
+# ---- one-vs-rest ------------------------------------------------------------------------------------------------------
+# Spark 3.1's ml/classification/OneVsRest.scala (not part of the reference project; restated here from Spark's
+# documented behaviour, as the reference's own Iris example uses it: classification/examples/Iris.scala wraps the binary
+# classifier in `new OneVsRest().setClassifier(...)`):
+#   - numClasses = max(label) + 1; class c is trained on the labels (y == c) ? 1 : 0 with the wrapped classifier's params;
+#   - OneVsRestModel's rawPrediction is the vector over classes of each class model's rawPrediction(1) (here f_c(x)), its
+#     prediction the argmax with the first maximum winning a tie; there is no probability column.
+# One deviation: a label that is not a non-negative integer raises ValueError, where Spark would silently leave the row
+# out of every class's positives.
+#
+# All classes share X and the expert grouping (GPC:26-31), so the points are uploaded and grouped once, and each round of
+# the C hyper-parameter optimisations is one `sgp_laplace_nll_classes` launch over experts x classes.  Each class runs the
+# binary pipeline: f_c from 0, its own L-BFGS-B from the same x0 and bounds, the Laplace loop once more at theta*_c
+# (GPCls:60), then produceModel with y := f_c.  The results are the binary classifier's on (y == c), bit for bit.
+
+
+def one_vs_rest_labels(y):
+    """Validated class labels and numClasses = max(label) + 1 (Spark's OneVsRest)."""
+    y = np.asarray(y, dtype=np.float64)
+    if y.ndim != 1 or len(y) == 0:
+        raise ValueError("OneVsRest: labels must be a non-empty vector")
+    if not np.all(np.isfinite(y) & (y >= 0.0) & (y == np.floor(y))):
+        raise ValueError("OneVsRest: labels must be non-negative integers (class indices)")
+    return y, int(y.max()) + 1
+
+
+def one_vs_rest_prediction(raw):
+    """OneVsRestModel's prediction from the n x C raw matrix: the argmax over classes, the first maximum winning a tie, as
+    float64 class indices."""
+    if is_cuda_tensor(raw):
+        import torch
+        # torch.argmax does not promise the first maximum on ties: compare against the row maximum instead
+        hit = raw == raw.max(dim=-1, keepdim=True).values
+        first = torch.arange(raw.shape[-1], 0, -1, device=raw.device, dtype=torch.int64) * hit
+        return torch.argmax(first, dim=-1).to(torch.float64)
+    return np.argmax(raw, axis=-1).astype(np.float64)
+
+
+class OneVsRestModel:
+    """Spark's OneVsRestModel over GaussianProcessClassificationModel: one binary model per class."""
+
+    def __init__(self, models, hyperparameters):
+        self.models = list(models)
+        self.numClasses = len(self.models)
+        self.hyperparameters = hyperparameters          # numClasses x n_hypers
+
+    def predictRaw(self, features):
+        """n x numClasses: column c is class c's latent prediction f_c(x) (its model's rawPrediction(1)).  A CUDA torch
+        tensor stays on the device (CUDA float64 result)."""
+        cols = [m.predictRaw(features)[..., 1] for m in self.models]
+        if is_cuda_tensor(features):
+            import torch
+            return torch.stack(cols, dim=-1)
+        return np.stack(cols, axis=-1)
+
+    def predict(self, features):
+        """The class index (float64) of the largest raw value, the first class winning a tie."""
+        return one_vs_rest_prediction(self.predictRaw(features))
+
+    transform = predict
+
+
+class OneVsRest:
+    """Spark's OneVsRest estimator over the binary GaussianProcessClassifier: `OneVsRest().setClassifier(gp).fit(X, y)`."""
+
+    def __init__(self):
+        self._classifier = None
+        self.last_objective = None
+        self.last_latent = None
+
+    def setClassifier(self, value):
+        if not isinstance(value, GaussianProcessClassifier):
+            raise TypeError("OneVsRest: the classifier must be a GaussianProcessClassifier, not %s" % type(value).__name__)
+        self._classifier = value
+        return self
+
+    def getClassifier(self):
+        return self._classifier
+
+    def fit(self, X, y, hyperparameters=None) -> OneVsRestModel:
+        """hyperparameters: None (optimise every class, as the binary fit does) or numClasses x n_hypers fixed values."""
+        gp = self._classifier
+        if not isinstance(gp, GaussianProcessClassifier):
+            raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
+        X = np.asarray(X, dtype=np.float64)
+        y, C = one_vs_rest_labels(y)
+        eng = ProjectedProcessEngine.acquire(gp._device)
+        try:
+            return self._fit(gp, eng, X, y, C, hyperparameters)
+        finally:
+            eng.release()
+
+    def _fit(self, gp, eng, X, y, C, hyperparameters):
+        groups = group_for_experts(len(X), gp._datasetSizeForExpert)
+        order = np.concatenate(groups)
+        eng.experts_upload_grouped(X, y, gp._datasetSizeForExpert)  # once for every class; all modes start at 0
+        launches0 = eng.launch_count()
+        k0 = gp.getKernel()
+        x0 = k0.getHyperparameters()
+        kernel_at = lambda t: gp.getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
+        if hyperparameters is not None:
+            thetas = np.array(hyperparameters, dtype=np.float64).reshape(C, len(x0))
+        else:
+            thetas = np.tile(np.asarray(x0, dtype=np.float64), (C, 1))
+            if gp._maxIter > 0 and len(x0) > 0:
+                def evaluate(batch):
+                    vals, grads = eng.laplace_nll_classes(C, [c for c, _ in batch], [kernel_at(t) for _, t in batch],
+                                                          gp._tol)
+                    return [(float(v), g) for v, g in zip(vals, grads)]
+
+                results, rounds = lbfgsb_lockstep(evaluate, [x0] * C, lbfgsb_bounds(k0), gp._maxIter, gp._tol)
+                thetas = np.array([np.asarray(res.x, dtype=np.float64) for res, _ in results]).reshape(C, len(x0))
+                self.last_objective = dict(
+                    classes=[dict(value=float(res.fun), evaluations=ev, iterations=int(res.nit)) for res, ev in results],
+                    rounds=rounds, launches=eng.launch_count() - launches0)
+        # GPCls:60 for every class at once: each class's f is its mode at theta*_c
+        eng.laplace_nll_classes(C, np.arange(C), [kernel_at(t) for t in thetas], gp._tol)
+        latent = np.empty((C, len(X)))
+        models = []
+        for c in range(C):
+            latent[c, order] = eng.experts_f_class(c, len(X))
+            # produceModel in the fit's context; each class starts from the default precision, as a freshly acquired
+            # context would (a fallback to F64 in one class's statistics must not decide the next class's path)
+            eng.set_precision(N.SGP_PREC_AUTO)
+            kernel, active_set, mv, mm, _ = _produce_model(gp, eng, X, latent[c], thetas[c])
+            # the model's own small context: never runs statistics, so it holds no statistics workspace
+            model_eng = ProjectedProcessEngine(gp._device)
+            model_eng.begin(kernel, active_set)
+            model_eng.set_magic(mv, mm)
+            models.append(GaussianProcessClassificationModel(
+                GaussianProjectedProcessRawPredictor(model_eng, mv, mm, kernel, active_set), thetas[c]))
+        self.last_latent = latent
+        return OneVsRestModel(models, thetas)

@@ -780,6 +780,7 @@ int experts_alloc(Ctx* c, long long E, long long n, int d, int n_max) {
   ex.X = c->ex_X.as<double>(); ex.y = c->ex_y.as<double>(); ex.off = c->ex_off.as<long long>(); ex.f = c->ex_f.as<double>();
   SGP_CUDA(c, cudaMemsetAsync(ex.f, 0, static_cast<size_t>(n) * 8, c->stream));
   ex.n = n; ex.d = d; ex.n_max = n_max;
+  c->ex_classes = 0;                                      // one-vs-rest modes restart at zero on their next use
   return SGP_OK;
 }
 }  // namespace
@@ -839,88 +840,137 @@ int sgp_experts_upload_grouped(sgp_ctx* h, const void* X, int32_t x_is_f32, cons
 }
 
 namespace {
-// Flattens the kernel (flatten_kernel: Eye terms only add to the diagonal), maps the hyper-parameter descriptors onto
-// the flattened terms and uploads them, with zeroed totals and flags, into the context's descriptor block.
-int objective_setup(Ctx* c, const sgp_kernel_desc* k, const sgp_hyper* hypers, int nh, HyperView& hv, double*& dTotal,
-                    int*& dFlags) {
+// Device state of one objective evaluation over n_slots hyper-parameter blocks (one per one-vs-rest class; the BCM and
+// binary Laplace objectives use one), in the context's descriptor block.
+struct ObjectiveSetup {
+  HyperView hv;                    // slot 0
+  int n_slots = 1;
+  long long slot_stride = 0;       // doubles between two slots' [beta | coef | value] blocks
+  const KernelFlat* kf = nullptr;  // [n_slots]
+  const int* cls = nullptr;        // [n_slots] the classes list (or zeros)
+  double* total = nullptr;         // [n_slots][1 + n_hypers] totals, then [n_slots] status words
+  int* flags = nullptr;            // [n_slots]
+};
+
+// Flattens each slot's kernel (flatten_kernel: Eye terms only add to the diagonal), maps the hyper-parameter descriptors
+// (hypers + s * nh for slot s) onto the flattened terms and uploads everything, with zeroed totals and flags, into the
+// context's descriptor block in one copy.  Every slot must have slot 0's kernel structure and descriptor kinds.
+int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int nh,
+                    const int* classes, ObjectiveSetup& o) {
   if (c->ex.E == 0) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
-  if (!k || !k->terms || k->n_terms <= 0 || nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, "null argument");
+  if (!kernels || nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, "null argument");
+  for (int s = 0; s < n_slots; ++s)
+    if (!kernels[s].terms || kernels[s].n_terms <= 0) return fail(c, SGP_E_BADARG, "null argument");
   if (nh > kMaxHypers) return fail(c, SGP_E_BADARG, "too many hyper-parameters");
   const int d = c->ex.d;
-  KernelFlat kf;
+  const sgp_kernel_desc* k = kernels;
+  std::vector<KernelFlat> kfs(n_slots);
   std::vector<int> flat_of;
-  std::vector<double> beta;
-  int rc = flatten_kernel(c, k, d, d, kf, beta, &flat_of);
-  if (rc != SGP_OK) return rc;
-  hv = HyperView{};
-  hv.d = d; hv.kf = kf; hv.n_hypers = nh;
+  std::vector<double> block;       // [n_slots][beta | coef | value]
   std::vector<int> kind(nh), hterm(nh, 0), hdim(nh, 0);
-  std::vector<double> coef(static_cast<size_t>(nh) * (kMaxTerms + 1), 0.0), value(nh, 0.0);
-  for (int i = 0; i < nh; ++i) {
-    kind[i] = hypers[i].kind;
-    value[i] = hypers[i].value;
-    if (hypers[i].kind == SGP_HYPER_SCALE) {
-      if (!hypers[i].coef) return fail(c, SGP_E_BADARG, "SCALE hyper-parameter without coef");
-      for (int t = 0; t < k->n_terms; ++t) {
-        const size_t col = (flat_of[t] >= 0) ? static_cast<size_t>(flat_of[t]) : static_cast<size_t>(kMaxTerms);
-        coef[static_cast<size_t>(i) * (kMaxTerms + 1) + col] += hypers[i].coef[t];
-      }
-    } else if (hypers[i].kind == SGP_HYPER_ARD_BETA || hypers[i].kind == SGP_HYPER_RBF_SIGMA) {
-      if (hypers[i].term < 0 || hypers[i].term >= k->n_terms || flat_of[hypers[i].term] < 0)
-        return fail(c, SGP_E_BADARG, "hyper-parameter refers to a bad term");
-      hterm[i] = flat_of[hypers[i].term];
-      hdim[i] = hypers[i].dim;
-      if (hypers[i].kind == SGP_HYPER_ARD_BETA) hv.any_ard = 1;
-      if (hypers[i].kind == SGP_HYPER_ARD_BETA && (hdim[i] < 0 || hdim[i] >= d)) return fail(c, SGP_E_BADARG, "bad ARD dim");
-    } else {
-      return fail(c, SGP_E_BADARG, "unknown hyper-parameter kind");
+  size_t nb = 0;                   // beta doubles of one slot
+  o = ObjectiveSetup{};
+  o.n_slots = n_slots;
+  HyperView& hv = o.hv;
+  hv.d = d; hv.n_hypers = nh;
+  for (int s = 0; s < n_slots; ++s) {
+    const sgp_kernel_desc* ks = kernels + s;
+    const sgp_hyper* hs = hypers ? hypers + static_cast<size_t>(s) * nh : nullptr;
+    if (s > 0) {
+      bool same = ks->n_terms == k->n_terms;
+      for (int t = 0; same && t < k->n_terms; ++t) same = ks->terms[t].type == k->terms[t].type;
+      for (int i = 0; same && i < nh; ++i)
+        same = hs[i].kind == kind[i] && (hs[i].kind == SGP_HYPER_SCALE || (hs[i].term == hypers[i].term && hs[i].dim == hdim[i]));
+      if (!same) return fail(c, SGP_E_BADARG, "every class needs the same kernel structure and hyper-parameter layout");
     }
+    std::vector<double> beta;
+    int rc = flatten_kernel(c, ks, d, d, kfs[s], beta, &flat_of);
+    if (rc != SGP_OK) return rc;
+    std::vector<double> coef(static_cast<size_t>(nh) * (kMaxTerms + 1), 0.0), value(nh, 0.0);
+    for (int i = 0; i < nh; ++i) {
+      kind[i] = hs[i].kind;
+      value[i] = hs[i].value;
+      if (hs[i].kind == SGP_HYPER_SCALE) {
+        if (!hs[i].coef) return fail(c, SGP_E_BADARG, "SCALE hyper-parameter without coef");
+        for (int t = 0; t < ks->n_terms; ++t) {
+          const size_t col = (flat_of[t] >= 0) ? static_cast<size_t>(flat_of[t]) : static_cast<size_t>(kMaxTerms);
+          coef[static_cast<size_t>(i) * (kMaxTerms + 1) + col] += hs[i].coef[t];
+        }
+      } else if (hs[i].kind == SGP_HYPER_ARD_BETA || hs[i].kind == SGP_HYPER_RBF_SIGMA) {
+        if (hs[i].term < 0 || hs[i].term >= ks->n_terms || flat_of[hs[i].term] < 0)
+          return fail(c, SGP_E_BADARG, "hyper-parameter refers to a bad term");
+        hterm[i] = flat_of[hs[i].term];
+        hdim[i] = hs[i].dim;
+        if (hs[i].kind == SGP_HYPER_ARD_BETA) hv.any_ard = 1;
+        if (hs[i].kind == SGP_HYPER_ARD_BETA && (hdim[i] < 0 || hdim[i] >= d)) return fail(c, SGP_E_BADARG, "bad ARD dim");
+      } else {
+        return fail(c, SGP_E_BADARG, "unknown hyper-parameter kind");
+      }
+    }
+    if (s == 0) {
+      hv.kf = kfs[0];
+      nb = beta.size();
+      o.slot_stride = static_cast<long long>(beta.size() + coef.size() + value.size());
+    }
+    block.insert(block.end(), beta.begin(), beta.end());
+    block.insert(block.end(), coef.begin(), coef.end());
+    block.insert(block.end(), value.begin(), value.end());
   }
-  // [beta | coef | value | totals | status] doubles, then [kind | term | dim | flags] ints
-  const size_t n_dbl = beta.size() + coef.size() + value.size() + (1 + nh) + 1;
-  const size_t n_int = 3 * static_cast<size_t>(nh) + 1;
-  std::vector<double> hd(n_dbl, 0.0);
-  std::vector<int> hi(n_int, 0);
-  std::copy(beta.begin(), beta.end(), hd.begin());
-  std::copy(coef.begin(), coef.end(), hd.begin() + beta.size());
-  std::copy(value.begin(), value.end(), hd.begin() + beta.size() + coef.size());
-  std::copy(kind.begin(), kind.end(), hi.begin());
-  std::copy(hterm.begin(), hterm.end(), hi.begin() + nh);
-  std::copy(hdim.begin(), hdim.end(), hi.begin() + 2 * nh);
-  rc = ctx_scratch(c, c->hyper_ws, n_dbl * 8 + n_int * 4);
+  // [KernelFlat n_slots] then doubles [slot blocks | totals | status], then ints [kind | term | dim | flags | classes]
+  const int W = 1 + nh;
+  const size_t kf_bytes = sizeof(KernelFlat) * n_slots;
+  const size_t n_dbl = block.size() + static_cast<size_t>(n_slots) * (W + 1);
+  const size_t n_int = 3 * static_cast<size_t>(nh) + 2 * static_cast<size_t>(n_slots);
+  std::vector<char> host(kf_bytes + n_dbl * 8 + n_int * 4, 0);
+  std::memcpy(host.data(), kfs.data(), kf_bytes);
+  std::memcpy(host.data() + kf_bytes, block.data(), block.size() * 8);
+  int* hi = reinterpret_cast<int*>(host.data() + kf_bytes + n_dbl * 8);
+  std::copy(kind.begin(), kind.end(), hi);
+  std::copy(hterm.begin(), hterm.end(), hi + nh);
+  std::copy(hdim.begin(), hdim.end(), hi + 2 * nh);
+  if (classes) std::copy(classes, classes + n_slots, hi + 3 * nh + n_slots);
+  int rc = ctx_scratch(c, c->hyper_ws, host.size());
   if (rc != SGP_OK) return rc;
-  double* dD = c->hyper_ws.as<double>();
+  char* dev = c->hyper_ws.as<char>();
+  SGP_CUDA(c, cudaMemcpyAsync(dev, host.data(), host.size(), cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));          // host is a local
+  rc = ctx_scratch(c, c->nll_per_ws, static_cast<size_t>(n_slots) * c->ex.E * W * 8);
+  if (rc != SGP_OK) return rc;
+  o.kf = reinterpret_cast<const KernelFlat*>(dev);
+  double* dD = reinterpret_cast<double*>(dev + kf_bytes);
   int* dI = reinterpret_cast<int*>(dD + n_dbl);
-  SGP_CUDA(c, cudaMemcpyAsync(dD, hd.data(), n_dbl * 8, cudaMemcpyHostToDevice, c->stream));
-  SGP_CUDA(c, cudaMemcpyAsync(dI, hi.data(), n_int * 4, cudaMemcpyHostToDevice, c->stream));
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));          // hd / hi are locals
-  rc = ctx_scratch(c, c->nll_per_ws, static_cast<size_t>(c->ex.E) * (1 + nh) * 8);
-  if (rc != SGP_OK) return rc;
-  hv.beta = dD; hv.h_coef = dD + beta.size(); hv.h_value = hv.h_coef + coef.size();
-  dTotal = dD + beta.size() + coef.size() + value.size();
+  hv.beta = dD; hv.h_coef = dD + nb; hv.h_value = hv.h_coef + static_cast<size_t>(nh) * (kMaxTerms + 1);
+  o.total = dD + block.size();
   hv.h_kind = dI; hv.h_term = dI + nh; hv.h_dim = dI + 2 * nh;
-  dFlags = dI + 3 * nh;
+  o.flags = dI + 3 * nh;
+  o.cls = dI + 3 * nh + n_slots;
   return SGP_OK;
 }
 
-// all-reduce over ranks, copy the (objective, gradient) row back, map a bad pivot to SGP_E_NOT_PD
-int objective_finish(Ctx* c, int nh, double* dTotal, const int* dFlags, double* val_out, double* grad_out, int mask,
-                     int err_code, const char* err_msg) {
-  const int W = 1 + nh;
-  // the rank-local status flag is all-reduced WITH the totals so that every rank raises (or none does)
-  SGP_CUDA(c, launch_status_to_double(dTotal + W, dFlags, mask, nullptr, 0.0, c->stream));
+// all-reduce over ranks, copy the (objective, gradient) rows of every slot back, map a bad pivot to err_code.  With a
+// classes list, the message names the first failing slot's class.
+int objective_finish(Ctx* c, const ObjectiveSetup& o, int nh, double* val_out, double* grad_out, int mask, int err_code,
+                     const char* err_msg, const int* classes = nullptr) {
+  const int W = 1 + nh, S = o.n_slots;
+  // the rank-local status flags are all-reduced WITH the totals so that every rank raises (or none does)
+  SGP_CUDA(c, launch_flags_to_double(o.total + static_cast<size_t>(S) * W, o.flags, mask, S, c->stream));
   c->launches += 1;
+  const size_t len = static_cast<size_t>(S) * (W + 1);
   if (c->comm && c->nranks > 1) {
-    ncclResult_t r = nccl().AllReduce(dTotal, dTotal, W + 1, ncclDouble, ncclSum, c->comm, c->stream);
+    ncclResult_t r = nccl().AllReduce(o.total, o.total, len, ncclDouble, ncclSum, c->comm, c->stream);
     if (r != ncclSuccess) return fail(c, SGP_E_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
     c->launches += 1;
   }
-  std::vector<double> tot(W + 1);
-  SGP_CUDA(c, cudaMemcpyAsync(tot.data(), dTotal, static_cast<size_t>(W + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+  std::vector<double> tot(len);
+  SGP_CUDA(c, cudaMemcpyAsync(tot.data(), o.total, len * 8, cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  if (tot[W] != 0.0) return fail(c, err_code, err_msg);
-  *val_out = tot[0];
-  for (int i = 1; i < W; ++i) grad_out[i - 1] = tot[i];
+  for (int s = 0; s < S; ++s)
+    if (tot[static_cast<size_t>(S) * W + s] != 0.0)
+      return fail(c, err_code, classes ? "class " + std::to_string(classes[s]) + ": " + err_msg : std::string(err_msg));
+  for (int s = 0; s < S; ++s) {
+    val_out[s] = tot[static_cast<size_t>(s) * W];
+    for (int i = 1; i < W; ++i) grad_out[static_cast<size_t>(s) * nh + i - 1] = tot[static_cast<size_t>(s) * W + i];
+  }
   return SGP_OK;
 }
 }  // namespace
@@ -931,11 +981,12 @@ int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   if (!c) return SGP_E_BADARG;
   if (!nll_out || (nh > 0 && !grad_out)) return fail(c, SGP_E_BADARG, "sgp_bcm_nll: null output");
   SGP_CUDA(c, cudaSetDevice(c->device));
-  HyperView hv;
-  double* dTotal = nullptr;
-  int* dFlags = nullptr;
-  int rc = objective_setup(c, k, hypers, nh, hv, dTotal, dFlags);
+  ObjectiveSetup o;
+  int rc = objective_setup(c, 1, k, hypers, nh, nullptr, o);
   if (rc != SGP_OK) return rc;
+  const HyperView& hv = o.hv;
+  double* dTotal = o.total;
+  int* dFlags = o.flags;
   double* rows = c->nll_per_ws.as<double>();
   // fast path: on-chip Cholesky per expert (SPD kernel matrices of <= ~165 points -- every default configuration).
   // general path: experts of any size, or a kernel matrix on which Cholesky broke down (not positive definite): the
@@ -962,9 +1013,13 @@ int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
     if (blas_status != 0) return fail(c, SGP_E_CUDA, "cuBLAS batched LU failed, status " + std::to_string(blas_status));
     c->launches += 5;
   }
-  return objective_finish(c, nh, dTotal, dFlags, nll_out, grad_out, 2, SGP_E_SINGULAR,
+  return objective_finish(c, o, nh, nll_out, grad_out, 2, SGP_E_SINGULAR,
                           "an expert's kernel matrix is singular (MatrixSingularException, logDetAndInv.scala:27-28)");
 }
+
+const char* const kLaplaceRefused =
+    "datasetSizeForExpert too large for the on-chip Laplace kernel (max ~115 points per expert)";
+const char* const kLaplaceNotPd = "an expert's B = I + sqrt(W) K sqrt(W) is not positive definite (increase sigma2)";
 
 int sgp_laplace_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh, double tol,
                     double* neg_log_z_out, double* grad_out) {
@@ -972,18 +1027,60 @@ int sgp_laplace_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hyper
   if (!c) return SGP_E_BADARG;
   if (!neg_log_z_out || (nh > 0 && !grad_out) || !(tol > 0.0)) return fail(c, SGP_E_BADARG, "sgp_laplace_nll: bad argument");
   SGP_CUDA(c, cudaSetDevice(c->device));
-  HyperView hv;
-  double* dTotal = nullptr;
-  int* dFlags = nullptr;
-  int rc = objective_setup(c, k, hypers, nh, hv, dTotal, dFlags);
+  ObjectiveSetup o;
+  int rc = objective_setup(c, 1, k, hypers, nh, nullptr, o);
   if (rc != SGP_OK) return rc;
-  const ObjectivePlan plan = plan_objective(Objective::kLaplace, c->ex, hv.kf.n_terms);
-  if (plan.variant == ObjectiveVariant::kRefused)
-    return fail(c, SGP_E_BADARG, "datasetSizeForExpert too large for the on-chip Laplace kernel (max ~115 points per expert)");
-  SGP_CUDA(c, launch_laplace(plan, c->ex, hv, tol, c->nll_per_ws.as<double>(), dTotal, dFlags, c->stream));
+  const ObjectivePlan plan = plan_objective(Objective::kLaplace, c->ex, o.hv.kf.n_terms);
+  if (plan.variant == ObjectiveVariant::kRefused) return fail(c, SGP_E_BADARG, kLaplaceRefused);
+  SGP_CUDA(c, launch_laplace(plan, c->ex, o.hv, tol, c->nll_per_ws.as<double>(), o.total, o.flags, c->stream));
   c->launches += 2;
-  return objective_finish(c, nh, dTotal, dFlags, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD,
-                          "an expert's B = I + sqrt(W) K sqrt(W) is not positive definite (increase sigma2)");
+  return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd);
+}
+
+int sgp_laplace_nll_classes(sgp_ctx* h, int32_t n_classes, const int32_t* classes, int32_t n_eval,
+                            const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t nh, double tol,
+                            double* neg_log_z_out, double* grad_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!neg_log_z_out || (nh > 0 && !grad_out) || !(tol > 0.0) || !classes)
+    return fail(c, SGP_E_BADARG, "sgp_laplace_nll_classes: bad argument");
+  if (n_classes < 1 || n_eval < 1 || n_eval > n_classes || n_eval > 65535)
+    return fail(c, SGP_E_BADARG, "sgp_laplace_nll_classes: need 1 <= n_eval <= n_classes and n_eval <= 65535");
+  std::vector<int> sorted(classes, classes + n_eval);
+  std::sort(sorted.begin(), sorted.end());
+  if (sorted.front() < 0 || sorted.back() >= n_classes || std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+    return fail(c, SGP_E_BADARG, "sgp_laplace_nll_classes: class indices must be distinct and in [0, n_classes)");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  ObjectiveSetup o;
+  int rc = objective_setup(c, n_eval, kernels, hypers, nh, classes, o);
+  if (rc != SGP_OK) return rc;
+  const ObjectivePlan plan = plan_objective(Objective::kLaplace, c->ex, o.hv.kf.n_terms);
+  if (plan.variant == ObjectiveVariant::kRefused) return fail(c, SGP_E_BADARG, kLaplaceRefused);
+  if (c->ex_classes != n_classes) {                       // first use after an upload, or another class count
+    const size_t bytes = static_cast<size_t>(n_classes) * c->ex.n * 8;
+    rc = ctx_scratch(c, c->ex_fc, bytes);
+    if (rc != SGP_OK) return rc;
+    SGP_CUDA(c, cudaMemsetAsync(c->ex_fc.p, 0, bytes, c->stream));
+    c->ex_classes = n_classes;
+  }
+  LaplaceClasses lc;
+  lc.n_slots = n_eval; lc.cls = o.cls; lc.kf = o.kf; lc.slot_stride = o.slot_stride; lc.f = c->ex_fc.as<double>();
+  SGP_CUDA(c, launch_laplace(plan, c->ex, o.hv, tol, c->nll_per_ws.as<double>(), o.total, o.flags, c->stream, &lc));
+  c->launches += 2;
+  return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd, classes);
+}
+
+int sgp_experts_get_f_class(sgp_ctx* h, int32_t cls, double* f_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (c->ex.E == 0 || !f_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
+  if (c->ex_classes == 0) return fail(c, SGP_E_STATE, "no class modes: sgp_laplace_nll_classes has not run since the upload");
+  if (cls < 0 || cls >= c->ex_classes) return fail(c, SGP_E_BADARG, "sgp_experts_get_f_class: class index out of range");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  SGP_CUDA(c, cudaMemcpyAsync(f_out, c->ex_fc.as<double>() + static_cast<size_t>(cls) * c->ex.n,
+                              static_cast<size_t>(c->ex.n) * 8, cudaMemcpyDeviceToHost, c->stream));
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  return SGP_OK;
 }
 
 int sgp_experts_get_f(sgp_ctx* h, double* f_out) {

@@ -296,12 +296,15 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
 }
 
 // Sum the per-expert rows: one CTA per column, thread t adds experts t, t+256, ... and the 256 partials are combined by
-// a fixed tree -- the order never depends on timing, so the result is deterministic.
+// a fixed tree -- the order never depends on timing, so the result is deterministic.  blockIdx.y: the slot (one-vs-rest
+// class) whose rows [E][width] are summed.
 __global__ void __launch_bounds__(EX_THREADS) rows_reduce_kernel(double* __restrict__ total,
                                                                    const double* __restrict__ per_expert, long long E,
                                                                    int width) {
   __shared__ double part[EX_THREADS];
   const int c = blockIdx.x;
+  total += static_cast<size_t>(blockIdx.y) * width;
+  per_expert += static_cast<size_t>(blockIdx.y) * E * width;
   double s = 0.0;
   for (long long e = threadIdx.x; e < E; e += EX_THREADS) s += per_expert[e * width + c];
   part[threadIdx.x] = s;
@@ -449,8 +452,9 @@ ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms) {
   return stage_rows(ObjectiveVariant::kSmem, bcm_nll_smem_bytes(ex.n_max), kStageTwoCtas);
 }
 
-cudaError_t launch_rows_reduce(double* dTotal, const double* dPerExpert, long long E, int width, cudaStream_t s) {
-  rows_reduce_kernel<<<width, EX_THREADS, 0, s>>>(dTotal, dPerExpert, E, width);
+cudaError_t launch_rows_reduce(double* dTotal, const double* dPerExpert, long long E, int width, cudaStream_t s,
+                               int n_slots) {
+  rows_reduce_kernel<<<dim3(width, n_slots), EX_THREADS, 0, s>>>(dTotal, dPerExpert, E, width);
   return cudaGetLastError();
 }
 

@@ -22,8 +22,10 @@ constexpr int EX_WARPS = EX_THREADS / 32;
 constexpr int DCH = 16;                                   // ARD dimensions per sweep
 constexpr int EX_SUMS = 2 * kMaxTerms + 1 + DCH;          // doubles of shared memory the sweep needs
 
-// host side (bcm_nll.cu): total[c] = sum_e per_expert[e][c], deterministic
-cudaError_t launch_rows_reduce(double* dTotal, const double* dPerExpert, long long E, int width, cudaStream_t s);
+// host side (bcm_nll.cu): total[s][c] = sum_e per_expert[s][e][c] for each of n_slots slots, deterministic; a slot's sums
+// do not depend on the other slots
+cudaError_t launch_rows_reduce(double* dTotal, const double* dPerExpert, long long E, int width, cudaStream_t s,
+                               int n_slots = 1);
 
 template <int NW = EX_WARPS>
 __device__ __forceinline__ double ex_block_sum(double v, double* red) {

@@ -7,6 +7,11 @@
 // post-loop quantities (pi, W, L, a, grad log p) are the ones of the LAST Newton iteration, i.e. computed from the f
 // before that iteration's update, while d3logP (GPCls:118, sign as in the reference) uses exp(-f) of the final f.
 // Summed over experts like commons/GaussianProcessCommons.scala:73-78.
+//
+// One-vs-rest (sgp_laplace_nll_classes): a second grid dimension runs several binary problems over the same experts in
+// one launch.  Block (e, s) evaluates expert e for the s-th listed class c: labels (y == c), modes f + c * n, its own
+// flattened kernel and hyper-parameter block, output row [s][e].  The arithmetic is the single-class body's, so class
+// c's rows equal, bit for bit, those of a single-class launch on an upload of the labels (y == c).
 #include "expert_common.cuh"
 
 namespace sgp {
@@ -17,10 +22,14 @@ constexpr int LT = EX_THREADS;     // threads per CTA
 struct LapParams {
   const double* X; const double* y; double* f; const long long* off;
   int n_max, x_in_smem;
-  HyperView hv;
+  HyperView hv;              // slot 0's view; slot s reads kf[s] and the descriptor values s * slot_stride doubles on
+  const int* cls;            // [n_slots] class of each slot (one-vs-rest), or nullptr: one slot, labels as uploaded
+  const KernelFlat* kf;      // [n_slots] flattened kernel of each slot (with cls)
+  long long slot_stride;     // doubles between two slots' [beta | coef | value] blocks (with cls)
+  long long n;               // uploaded points: the stride of the per-class modes f (with cls)
   double tol;
-  double* out;               // [E][1 + n_hypers]  (-logZ, -gradLogZ)
-  int* flags;                // bit 0: Cholesky pivot not positive
+  double* out;               // [n_slots][E][1 + n_hypers]  (-logZ, -gradLogZ)
+  int* flags;                // [n_slots]  bit 0: Cholesky pivot not positive
 };
 
 __device__ __forceinline__ double sigmoid(double x) { return 1.0 / (1.0 + exp(-x)); }
@@ -51,9 +60,20 @@ __device__ void bwd_solve(const double* L, int n, int ld, double* x) {
 __global__ void __launch_bounds__(LT, 1) laplace_kernel(const LapParams p) {
   extern __shared__ double sm[];
   const long long e = blockIdx.x;
+  const int slot = blockIdx.y;
   const long long r0 = p.off[e];
   const int n = static_cast<int>(p.off[e + 1] - r0);
   const int ld = p.n_max + 1;
+  HyperView hv = p.hv;
+  double* fg = p.f;
+  double cls = -1.0;                                     // < 0: labels as uploaded
+  if (p.cls) {
+    const int c = p.cls[slot];
+    cls = c;
+    fg += static_cast<size_t>(c) * p.n;
+    hv.kf = p.kf[slot];
+    hv.beta += slot * p.slot_stride; hv.h_coef += slot * p.slot_stride; hv.h_value += slot * p.slot_stride;
+  }
   double* K = sm;                                        // full symmetric
   double* M = K + static_cast<size_t>(p.n_max) * ld;     // B -> L -> L^-1 -> B^-1 (lower)
   double* v = M + static_cast<size_t>(p.n_max) * ld;     // vectors, n_max each
@@ -65,11 +85,14 @@ __global__ void __launch_bounds__(LT, 1) laplace_kernel(const LapParams p) {
   double* Xs = sums + EX_SUMS;                           // staged rows (if they fit)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int xld;
-  const double* Xe = ex_stage_rows(p.X + static_cast<size_t>(r0) * p.hv.d, n, p.hv.d, p.x_in_smem, Xs, xld);
+  const double* Xe = ex_stage_rows(p.X + static_cast<size_t>(r0) * hv.d, n, hv.d, p.x_in_smem, Xs, xld);
 
-  for (int i = tid; i < n; i += LT) { f[i] = p.f[r0 + i]; yv[i] = p.y[r0 + i]; }
+  for (int i = tid; i < n; i += LT) {
+    f[i] = fg[r0 + i];
+    yv[i] = (cls < 0.0) ? p.y[r0 + i] : (p.y[r0 + i] == cls ? 1.0 : 0.0);
+  }
   __syncthreads();
-  ex_build_kernel<true>(p.hv, Xe, xld, n, K, ld);        // K, both triangles
+  ex_build_kernel<true>(hv, Xe, xld, n, K, ld);        // K, both triangles
   __syncthreads();
 
   // ---- Newton iteration for the mode (GPCls:79-111) ------------------------------------------------------------------
@@ -118,11 +141,11 @@ __global__ void __launch_bounds__(LT, 1) laplace_kernel(const LapParams p) {
     }
     __syncthreads();
   }
-  if (bad && tid == 0) atomicOr(p.flags, 1);
-  for (int i = tid; i < n; i += LT) p.f[r0 + i] = f[i];   // the mode persists (warm start of the next evaluation)
+  if (bad && tid == 0) atomicOr(p.flags + slot, 1);
+  for (int i = tid; i < n; i += LT) fg[r0 + i] = f[i];   // the mode persists (warm start of the next evaluation)
 
   // ---- log Z and gradient (GPCls:114-128) --------------------------------------------------------------------------
-  double* out = p.out + static_cast<size_t>(e) * (1 + p.hv.n_hypers);
+  double* out = p.out + (static_cast<size_t>(slot) * gridDim.x + e) * (1 + hv.n_hypers);
   if (tid == 0) out[0] = -(new_obj - sumlogL);
   ex_invert_lower(M, n, ld, t1);                         // L^-1 in place
   // diag(C^T C), C = L^-1 (sqrtW K):  cc_i = | L^-1 (sw o K[:,i]) |^2   (GPCls:117,119)
@@ -161,7 +184,7 @@ __global__ void __launch_bounds__(LT, 1) laplace_kernel(const LapParams p) {
   }
   __syncthreads();
   ex_descriptor_gradient(
-      p.hv, Xe, xld, n,
+      hv, Xe, xld, n,
       [&](int a, int b) {
         return 0.5 * (av[a] * av[b] - sw[a] * sw[b] * M[a * ld + b]) + 0.5 * (t2[a] * glp[b] + t2[b] * glp[a]);
       },
@@ -175,16 +198,21 @@ size_t laplace_smem_bytes(int n_max) {
 }
 
 cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol, double* rows,
-                           double* total, int* flags, cudaStream_t s) {
+                           double* total, int* flags, cudaStream_t s, const LaplaceClasses* classes) {
   LapParams p{};
   p.X = ex.X; p.y = ex.y; p.f = ex.f; p.off = ex.off; p.n_max = ex.n_max; p.x_in_smem = plan.x_in_smem;
-  p.hv = hv; p.tol = tol; p.out = rows; p.flags = flags;
+  p.hv = hv; p.n = ex.n; p.tol = tol; p.out = rows; p.flags = flags;
+  int n_slots = 1;
+  if (classes) {
+    p.f = classes->f; p.cls = classes->cls; p.kf = classes->kf; p.slot_stride = classes->slot_stride;
+    n_slots = classes->n_slots;
+  }
   cudaError_t e = cudaFuncSetAttribute(laplace_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(plan.smem));
   if (e != cudaSuccess) return e;
-  laplace_kernel<<<static_cast<unsigned>(ex.E), LT, plan.smem, s>>>(p);
+  laplace_kernel<<<dim3(static_cast<unsigned>(ex.E), static_cast<unsigned>(n_slots)), LT, plan.smem, s>>>(p);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  return launch_rows_reduce(total, rows, ex.E, 1 + hv.n_hypers, s);
+  return launch_rows_reduce(total, rows, ex.E, 1 + hv.n_hypers, s, n_slots);
 }
 
 }  // namespace sgp

@@ -91,6 +91,11 @@ __global__ void status_to_double_kernel(double* __restrict__ dst, const int* __r
   *dst = v;
 }
 
+__global__ void flags_to_double_kernel(double* __restrict__ dst, const int* __restrict__ flags, int mask, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = (flags[i] & mask) ? 1.0 : 0.0;
+}
+
 // Expert grouping on the device (GPC:26-31): E = Math.round(N / n_e); point i (zipWithIndex order) belongs to expert
 // i % E and is its (i / E)-th point.  With k = N / E and r = N % E, experts < r own k+1 points: expert e starts at
 // e*k + min(e, r).  One thread per (point, feature): a strided gather from the row-major input into the expert-major
@@ -178,6 +183,11 @@ cudaError_t launch_expert_offsets(long long* off, long long n, long long E, cuda
 cudaError_t launch_status_to_double(double* dst, const int* flags, int mask, const double* norm_sum, double norm_limit,
                                     cudaStream_t s) {
   status_to_double_kernel<<<1, 1, 0, s>>>(dst, flags, mask, norm_sum, norm_limit);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_flags_to_double(double* dst, const int* flags, int mask, int n, cudaStream_t s) {
+  flags_to_double_kernel<<<(n + 255) / 256, 256, 0, s>>>(dst, flags, mask, n);
   return cudaGetLastError();
 }
 

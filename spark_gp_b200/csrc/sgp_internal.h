@@ -163,6 +163,8 @@ struct Ctx {
   // per-expert objective state
   ExpertSet ex;                  // view of ex_X, ex_y, ex_off, ex_f; E > 0 once an upload has completed
   DevScratch ex_X, ex_y, ex_off, ex_f;
+  DevScratch ex_fc;              // one-vs-rest latent modes [ex_classes][n] (sgp_laplace_nll_classes)
+  int ex_classes = 0;            // classes ex_fc holds modes for; 0: none since the last upload
   DevScratch nll_per_ws;         // per-expert objective rows
   DevScratch hyper_ws;           // hyper-parameter descriptors + totals + flags of one evaluation
   bool bcm_general = false;      // the last sgp_bcm_nll took the global-memory LU path
@@ -220,6 +222,8 @@ cudaError_t launch_group_experts(double* Xe, double* ye, const void* dX, int x_i
 cudaError_t launch_expert_offsets(long long* off, long long n, long long E, cudaStream_t s);
 cudaError_t launch_status_to_double(double* dst, const int* flags, int mask, const double* norm_sum, double norm_limit,
                                     cudaStream_t s);
+// dst[i] = (flags[i] & mask) ? 1 : 0 for i < n: the per-slot status words of an objective evaluation
+cudaError_t launch_flags_to_double(double* dst, const int* flags, int mask, int n, cudaStream_t s);
 
 // Prediction (predict.cu) over one window of device-resident points.
 struct PredictArgs {
@@ -315,8 +319,19 @@ cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const
 cudaError_t launch_bcm_nll_general(const ObjectivePlan& plan, cublasHandle_t blas, int* blas_status, void* ws,
                                    const ExpertSet& ex, const HyperView& hv, double* rows, double* total, int* flags,
                                    cudaStream_t s);
+// One-vs-rest slots of a Laplace launch (sgp_laplace_nll_classes): slot s evaluates class cls[s] with the labels
+// (y == cls[s]), the modes f + cls[s] * n, the flattened kernel kf[s] and the descriptor values slot_stride doubles per
+// slot after hv's.  rows: [n_slots][E][1 + n_hypers], total: [n_slots][1 + n_hypers], flags: [n_slots].
+struct LaplaceClasses {
+  int n_slots = 0;
+  const int* cls = nullptr;           // device, [n_slots]
+  const KernelFlat* kf = nullptr;     // device, [n_slots]
+  long long slot_stride = 0;
+  double* f = nullptr;                // device, [n_classes][n]
+};
+// classes == nullptr: one slot on the labels and modes as uploaded (sgp_laplace_nll)
 cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol, double* rows,
-                           double* total, int* flags, cudaStream_t s);
+                           double* total, int* flags, cudaStream_t s, const LaplaceClasses* classes = nullptr);
 
 int ctx_scratch(Ctx* c, DevScratch& s, size_t bytes);
 // csrc/greedy.cu: forward selection with rank-1 updates (ActiveSetProvider.scala:58-139); beta_flat = [n_terms][d]

@@ -213,9 +213,8 @@ class ProjectedProcessEngine:
         self._experts_d = X.shape[1]
         return int(np.floor(len(X) / dataset_size_for_expert + 0.5))
 
-    def _objective(self, fn, kernel: Kernel, *args):
-        """Runs one per-expert objective of the library over the uploaded experts: (value, gradient w.r.t.
-        kernel.getHyperparameters())."""
+    def _descriptors(self, kernel: Kernel):
+        """(kernel desc, hyper-parameter descriptors, their count, the buffers both point into)."""
         desc, keep = _make_desc(kernel, self._experts_d)
         hd = kernel.hyper_descriptors()
         arr = (N.Hyper * max(len(hd), 1))()
@@ -231,16 +230,55 @@ class ProjectedProcessEngine:
                     cf[t] = v
                 coefs.append(cf)
                 arr[i].coef = cf.ctypes.data_as(C.POINTER(C.c_double))
+        return desc, arr, len(hd), (keep, coefs)
+
+    def _objective(self, fn, kernel: Kernel, *args):
+        """Runs one per-expert objective of the library over the uploaded experts: (value, gradient w.r.t.
+        kernel.getHyperparameters())."""
+        desc, arr, nh, keep = self._descriptors(kernel)
         val = C.c_double()
-        grad = np.zeros(max(len(hd), 1))
-        self._check(fn(self._h, C.byref(desc), arr, len(hd), *args, C.byref(val), N.ptr(grad)))
-        del keep, coefs
-        return val.value, grad[:len(hd)]
+        grad = np.zeros(max(nh, 1))
+        self._check(fn(self._h, C.byref(desc), arr, nh, *args, C.byref(val), N.ptr(grad)))
+        del keep
+        return val.value, grad[:nh]
 
     def laplace_nll(self, kernel: Kernel, tol: float):
         """Binary classification: (-log Z summed over experts, its gradient).  Updates the device-resident latent
         modes f of the uploaded experts (warm start), as GaussianProcessClassifier.likelihoodAndGradient does."""
         return self._objective(self._lib.sgp_laplace_nll, kernel, float(tol))
+
+    def laplace_nll_classes(self, n_classes: int, classes, kernels, tol: float):
+        """One-vs-rest over uploaded class indices: the binary Laplace objective of each listed class c (labels y == c)
+        at its own kernels[i], all in one launch (`sgp_laplace_nll_classes`).  Returns (values [n_eval], gradients
+        [n_eval x n_hypers]); each class's device-resident modes warm-start its next evaluation."""
+        cls = np.ascontiguousarray(classes, dtype=np.int32)
+        if cls.ndim != 1 or len(cls) == 0 or len(cls) != len(kernels):
+            raise ValueError("laplace_nll_classes: one kernel per listed class")
+        descs = (N.KernelDesc * len(cls))()
+        keep, hyp, nh = [], None, None
+        for i, k in enumerate(kernels):
+            desc, arr, n_i, kp = self._descriptors(k)
+            if nh is None:
+                nh = n_i
+                hyp = (N.Hyper * max(len(cls) * nh, 1))()
+            elif n_i != nh:
+                raise ValueError("laplace_nll_classes: every class needs the same hyper-parameter layout")
+            descs[i] = desc
+            for j in range(nh):
+                hyp[i * nh + j] = arr[j]
+            keep.append(kp)
+        vals = np.zeros(len(cls))
+        grads = np.zeros((len(cls), max(nh, 1)))
+        self._check(self._lib.sgp_laplace_nll_classes(self._h, int(n_classes), N.ptr(cls), len(cls), descs, hyp, nh,
+                                                      float(tol), N.ptr(vals), N.ptr(grads)))
+        del keep
+        return vals, np.ascontiguousarray(grads[:, :nh])
+
+    def experts_f_class(self, cls: int, n: int):
+        """Class cls's latent modes after `laplace_nll_classes` (packed expert-major order)."""
+        f = np.empty(n)
+        self._check(self._lib.sgp_experts_get_f_class(self._h, int(cls), N.ptr(f)))
+        return f
 
     def experts_f(self, n: int):
         f = np.empty(n)

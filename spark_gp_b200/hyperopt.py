@@ -7,10 +7,110 @@ tolerance = tol)` -- the reference pins no test on the iterate trajectory, so re
 value and on predictive metrics, not on theta."""
 from __future__ import annotations
 
+import threading
+
 import numpy as np
 from scipy.optimize import minimize
 
 from .engine import ProjectedProcessEngine
+
+
+def lbfgsb_bounds(kernel):
+    """Kernel.hyperparameterBoundaries as SciPy bounds (an infinite upper bound is None)."""
+    lo, up = kernel.hyperparameterBoundaries()
+    return [(float(l), None if np.isinf(u) else float(u)) for l, u in zip(lo, up)]
+
+
+def lbfgsb(objective, x0, bounds, max_iter: int, tol: float):
+    """The optimisation step of GaussianProcessClassifier (GPC:66-92 with GPCls's objective): SciPy's L-BFGS-B in place of
+    Breeze's LBFGSB(lower, upper, maxIter, tolerance = tol), on `objective(theta) -> (value, gradient)` memoised like
+    DiffFunctionMemoized (a point L-BFGS-B visits again is not evaluated again, so the latent modes it warm-starts from
+    only move on new points).  Returns (SciPy result, number of evaluations)."""
+    memo = {}
+
+    def f(theta):
+        key = tuple(theta)
+        if key not in memo:
+            memo[key] = objective(np.asarray(theta))
+        return memo[key]
+
+    res = minimize(f, x0, jac=True, method="L-BFGS-B", bounds=bounds, options=dict(maxiter=max_iter, ftol=tol, gtol=tol))
+    return res, len(memo)
+
+
+class _Aborted(Exception):
+    """Raised inside a class's optimisation when another class's evaluation failed."""
+
+
+def lbfgsb_lockstep(evaluate, x0s, bounds, max_iter: int, tol: float):
+    """C independent `lbfgsb` optimisations advanced together.  SciPy's minimize has no reverse-communication interface,
+    so each runs in a thread of its own; a round waits until every class still iterating has asked for a new point, then
+    `evaluate([(c, theta_c), ...]) -> [(value, gradient), ...]` answers them all at once.  Each class sees exactly the
+    values an independent `lbfgsb` would, so its trajectory is the independent one.  An exception in `evaluate` or in a
+    class's optimisation stops every class and is raised here.  Returns ([(result, evaluations)] per class, rounds)."""
+    n = len(x0s)
+    cv = threading.Condition()
+    pending, answers, active = {}, {}, set(range(n))
+    out, errors = [None] * n, []
+
+    def ask(c, theta):
+        with cv:
+            pending[c] = theta
+            cv.notify_all()
+            while c not in answers and not errors:
+                cv.wait()
+            if c not in answers:
+                raise _Aborted()
+            return answers.pop(c)
+
+    def run(c):
+        try:
+            out[c] = lbfgsb(lambda theta: ask(c, theta), x0s[c], bounds, max_iter, tol)
+        except _Aborted:
+            pass
+        except BaseException as e:          # noqa: BLE001 -- handed to the caller below
+            with cv:
+                errors.append(e)
+        finally:
+            with cv:
+                active.discard(c)
+                cv.notify_all()
+
+    threads = [threading.Thread(target=run, args=(c,), daemon=True) for c in range(n)]
+    for t in threads:
+        t.start()
+    rounds = 0
+    try:
+        while True:
+            with cv:
+                while active and not errors and not active <= set(pending):
+                    cv.wait()
+                if errors or not active:
+                    break
+                batch = sorted(pending.items())
+                pending.clear()
+            try:
+                values = evaluate(batch)
+            except BaseException as e:      # noqa: BLE001
+                with cv:
+                    errors.append(e)
+                    cv.notify_all()
+                break
+            rounds += 1
+            with cv:
+                for (c, _), v in zip(batch, values):
+                    answers[c] = v
+                cv.notify_all()
+    finally:
+        with cv:
+            if not errors and active:
+                errors.append(RuntimeError("lock-step optimisation stopped early"))
+            cv.notify_all()
+        for t in threads:
+            t.join()
+    if errors:
+        raise errors[0]
+    return out, rounds
 
 
 def group_for_experts(n_points: int, dataset_size_for_expert: int):
