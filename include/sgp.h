@@ -176,6 +176,38 @@ typedef struct {
 int sgp_bcm_nll(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper* hypers, int32_t n_hypers,
                 double* nll_out, double* grad_out);
 
+/* ---- cross-validation (Spark's CrossValidator over the regression estimator) ------------------------------------ */
+/* Uploads the n_folds training sets of a k-fold split at once.  fold_of[i] in [0, n_folds) is the fold of point i
+ * (n_folds >= 2).  Set k is fold k's training split: the points with fold_of[i] != k, in index order (Spark keeps the
+ * row order).  It is grouped as sgp_experts_upload_grouped groups a shard: E_k = Math.round(N_k / dataset_size_for_expert),
+ * the j-th training point goes to expert j % E_k.  The sets are stored one after another: X and y cross PCIe once, and
+ * each staged chunk is gathered on the device into every set that holds its points.  Needs (n_folds - 1) n (d + 2) * 8
+ * bytes of device memory (rows, labels and latent modes of every set): SGP_E_NOMEM past what the device has free.
+ * SGP_E_BADARG for n_folds < 2, a fold index outside [0, n_folds), or a set with E_k == 0 (the reference's / by zero).
+ * As every upload, it resets the latent modes and the one-vs-rest modes.  The other objectives (sgp_bcm_nll,
+ * sgp_laplace_nll*) see a fold upload as one expert set: the union of every set's experts. */
+int sgp_experts_upload_folds(sgp_ctx* ctx, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
+                             const int32_t* fold_of, int32_t n_folds, int32_t dataset_size_for_expert);
+
+/* The BCM objective of sgp_bcm_nll on several training sets of the last sgp_experts_upload_folds, in one launch over
+ * experts x slots.  Slot s evaluates set sets[s] at its own kernels[s] and hypers[s * n_hypers ...] (the same kernel
+ * structure and descriptor layout in every slot).  A set may be listed more than once, for several parameter maps on
+ * one fold.  Outputs per slot: nll_out[s], grad_out[s * n_hypers ...].
+ * Contract: slot s's value and gradient equal, bit for bit, what sgp_bcm_nll returns on
+ * sgp_experts_upload_grouped(X[fold_of != k], y[fold_of != k], dataset_size_for_expert) with k = sets[s] and the same
+ * kernel, whenever that single-set call runs the same kernel family (register, shared-memory or LU).  The call plans its
+ * kernel once, on the largest expert over the listed sets; the register kernel's padded shapes add exact zeros only, so
+ * within the register family the shape does not matter.
+ * A slot whose on-chip Cholesky breaks down is evaluated again on the LU path, on its own set alone.  Experts too large for
+ * the on-chip kernels put every slot on the LU path, one slot after another: 5 launches per slot instead of 2 per call.
+ * sgp_last_bcm_path is 1 if any slot ran LU.  With a communicator: one ncclAllReduce of the n_eval rows and n_eval status
+ * words.  Errors: SGP_E_STATE without a fold upload; SGP_E_BADARG for a set index outside [0, n_folds), a structure that
+ * differs between slots, or n_eval outside [1, 65535]; SGP_E_SINGULAR naming the first slot's set whose matrix is
+ * exactly singular. */
+int sgp_bcm_nll_folds(sgp_ctx* ctx, const int32_t* sets, int32_t n_eval, const sgp_kernel_desc* kernels,
+                      const sgp_hyper* hypers, int32_t n_hypers, double* nll_out /* n_eval */,
+                      double* grad_out /* n_eval x n_hypers */);
+
 /* Binary classification (labels 0/1 in the uploaded y): per-expert Laplace approximation,
  * classification/GaussianProcessClassifier.scala:74-129 -- Newton iteration for the mode with the reference's step
  * halving, tolerance `tol` and warm start (the latent f of every uploaded point lives on the device, starts at zero

@@ -10,3 +10,4 @@ from .regression import (GaussianProcessRegression, GaussianProcessRegressionMod
                          GreedilyOptimizingActiveSetProvider, KMeansActiveSetProvider)
 from .classification import GaussianProcessClassifier, GaussianProcessClassificationModel, OneVsRest, OneVsRestModel
 from .utils import scale
+from .tuning import CrossValidator, CrossValidatorModel, ParamGridBuilder, RegressionEvaluator

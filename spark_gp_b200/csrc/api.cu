@@ -781,7 +781,16 @@ int experts_alloc(Ctx* c, long long E, long long n, int d, int n_max) {
   SGP_CUDA(c, cudaMemsetAsync(ex.f, 0, static_cast<size_t>(n) * 8, c->stream));
   ex.n = n; ex.d = d; ex.n_max = n_max;
   c->ex_classes = 0;                                      // one-vs-rest modes restart at zero on their next use
+  c->fold_first.clear();
+  c->fold_nmax.clear();
   return SGP_OK;
+}
+
+// Chunks of ~32 MB of rows (at least 64k points) for the grouped uploads' staging
+long long group_chunk(long long n, size_t row) {
+  long long chunk = static_cast<long long>((32u << 20) / row);
+  if (chunk < 65536) chunk = 65536;
+  return chunk > n ? n : chunk;
 }
 }  // namespace
 
@@ -821,20 +830,90 @@ int sgp_experts_upload_grouped(sgp_ctx* h, const void* X, int32_t x_is_f32, cons
   if (E <= 0) return fail(c, SGP_E_BADARG, "numberOfExperts == 0 (N < datasetSizeForExpert / 2): the reference fails with / by zero");
   int rc = experts_alloc(c, E, n, d, static_cast<int>(n / E + ((n % E) ? 1 : 0)));
   if (rc != SGP_OK) return rc;
-  SGP_CUDA(c, launch_expert_offsets(c->ex.off, n, E, c->stream));
+  SGP_CUDA(c, launch_expert_offsets(c->ex.off, n, E, 0, c->stream));
   // stream the row-major input through the double-buffered staging area of the statistics path, gather on the device
-  const size_t esz = x_is_f32 ? 4 : 8;
-  const size_t row = static_cast<size_t>(d) * esz;
-  long long chunk = static_cast<long long>((32u << 20) / row);
-  if (chunk < 65536) chunk = 65536;
-  if (chunk > n) chunk = n;
+  const size_t row = static_cast<size_t>(d) * (x_is_f32 ? 4 : 8);
+  const long long chunk = group_chunk(n, row);
   rc = stage_rows(c, X, y, n, row, chunk, chunk, [&](const void* dX, const double* dy, long long p0, long long cn) -> int {
-    SGP_CUDA(c, launch_group_experts(c->ex.X, c->ex.y, dX, x_is_f32, dy, n, d, E, p0, cn, c->stream));
+    SGP_CUDA(c, launch_group_experts(c->ex.X, c->ex.y, dX, x_is_f32, dy, n, d, E, p0, cn, nullptr, 0, c->stream));
     c->launches += 1;
     return SGP_OK;
   });
   if (rc != SGP_OK) return rc;
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->ex.E = E;
+  return SGP_OK;
+}
+
+int sgp_experts_upload_folds(sgp_ctx* h, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
+                             const int32_t* fold_of, int32_t n_folds, int32_t dataset_size_for_expert) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!X || !y || !fold_of || n <= 0 || d <= 0 || dataset_size_for_expert <= 0)
+    return fail(c, SGP_E_BADARG, "sgp_experts_upload_folds: null or empty argument");
+  if (n_folds < 2) return fail(c, SGP_E_BADARG, "sgp_experts_upload_folds: n_folds must be >= 2");
+  // the points of each fold in index order: set k leaves out pos[fstart[k] .. fstart[k+1]-1]
+  std::vector<long long> fstart(static_cast<size_t>(n_folds) + 1, 0);
+  for (int64_t i = 0; i < n; ++i) {
+    if (fold_of[i] < 0 || fold_of[i] >= n_folds)
+      return fail(c, SGP_E_BADARG, "sgp_experts_upload_folds: fold index of point " + std::to_string(i) + " outside [0, n_folds)");
+    ++fstart[fold_of[i] + 1];
+  }
+  for (int k = 0; k < n_folds; ++k) fstart[k + 1] += fstart[k];
+  std::vector<long long> pos(static_cast<size_t>(n)), next(fstart.begin(), fstart.end() - 1);
+  for (int64_t i = 0; i < n; ++i) pos[next[fold_of[i]]++] = i;
+  // set k: N_k = n - |fold k| training points in E_k = round(N_k / n_e) experts (GPC:26-31), stored after set k-1
+  std::vector<long long> first(static_cast<size_t>(n_folds) + 1, 0), row0(static_cast<size_t>(n_folds) + 1, 0);
+  std::vector<int> nmax(n_folds);
+  for (int k = 0; k < n_folds; ++k) {
+    const long long Nk = n - (fstart[k + 1] - fstart[k]);
+    const long long Ek = static_cast<long long>(std::floor(static_cast<double>(Nk) / dataset_size_for_expert + 0.5));
+    if (Ek <= 0)
+      return fail(c, SGP_E_BADARG, "fold " + std::to_string(k) + ": numberOfExperts == 0 (N < datasetSizeForExpert / 2): "
+                                   "the reference fails with / by zero");
+    first[k + 1] = first[k] + Ek;
+    row0[k + 1] = row0[k] + Nk;
+    nmax[k] = static_cast<int>(Nk / Ek + ((Nk % Ek) ? 1 : 0));
+  }
+  const long long n_rows = row0[n_folds], E = first[n_folds];
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  {                                           // the sets' rows, labels and modes, (n_folds - 1) n (d + 2) doubles
+    size_t free_b = 0, total_b = 0;
+    SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+    const size_t held = c->ex_X.cap + c->ex_y.cap + c->ex_f.cap;
+    const size_t need = static_cast<size_t>(n_rows) * (static_cast<size_t>(d) + 2) * 8;
+    if (need > free_b + held)
+      return fail(c, SGP_E_NOMEM, "sgp_experts_upload_folds: the training sets need " + std::to_string(need >> 20) +
+                                      " MiB of device memory, " + std::to_string((free_b + held) >> 20) + " MiB available");
+  }
+  int rc = experts_alloc(c, E, n_rows, d, *std::max_element(nmax.begin(), nmax.end()));
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->fold_pos_ws, static_cast<size_t>(n) * 8);
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_set_first, first.size() * 8);
+  if (rc != SGP_OK) return rc;
+  const long long* dpos = c->fold_pos_ws.as<long long>();
+  SGP_CUDA(c, cudaMemcpyAsync(c->fold_pos_ws.p, pos.data(), pos.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(c->ex_set_first.p, first.data(), first.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  for (int k = 0; k < n_folds; ++k) {
+    SGP_CUDA(c, launch_expert_offsets(c->ex.off + first[k], row0[k + 1] - row0[k], first[k + 1] - first[k], row0[k],
+                                      c->stream));
+    c->launches += 1;
+  }
+  // X and y cross PCIe once; each staged chunk is gathered into every training set that holds its points
+  const size_t row = static_cast<size_t>(d) * (x_is_f32 ? 4 : 8);
+  const long long chunk = group_chunk(n, row);
+  rc = stage_rows(c, X, y, n, row, chunk, chunk, [&](const void* dX, const double* dy, long long p0, long long cn) -> int {
+    for (int k = 0; k < n_folds; ++k) {
+      SGP_CUDA(c, launch_group_experts(c->ex.X + static_cast<size_t>(row0[k]) * d, c->ex.y + row0[k], dX, x_is_f32, dy,
+                                       row0[k + 1] - row0[k], d, first[k + 1] - first[k], p0, cn, dpos + fstart[k],
+                                       fstart[k + 1] - fstart[k], c->stream));
+      c->launches += 1;
+    }
+    return SGP_OK;
+  });
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->fold_first = first;
+  c->fold_nmax = nmax;
   c->ex.E = E;
   return SGP_OK;
 }
@@ -847,7 +926,8 @@ struct ObjectiveSetup {
   int n_slots = 1;
   long long slot_stride = 0;       // doubles between two slots' [beta | coef | value] blocks
   const KernelFlat* kf = nullptr;  // [n_slots]
-  const int* cls = nullptr;        // [n_slots] the classes list (or zeros)
+  std::vector<KernelFlat> kf_host; // [n_slots]
+  const int* cls = nullptr;        // [n_slots] the classes (fold sets) list, or zeros
   double* total = nullptr;         // [n_slots][1 + n_hypers] totals, then [n_slots] status words
   int* flags = nullptr;            // [n_slots]
 };
@@ -855,8 +935,9 @@ struct ObjectiveSetup {
 // Flattens each slot's kernel (flatten_kernel: Eye terms only add to the diagonal), maps the hyper-parameter descriptors
 // (hypers + s * nh for slot s) onto the flattened terms and uploads everything, with zeroed totals and flags, into the
 // context's descriptor block in one copy.  Every slot must have slot 0's kernel structure and descriptor kinds.
+// rows_per_slot: the per-expert rows a slot writes (0: every uploaded expert).
 int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int nh,
-                    const int* classes, ObjectiveSetup& o) {
+                    const int* classes, ObjectiveSetup& o, long long rows_per_slot = 0) {
   if (c->ex.E == 0) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
   if (!kernels || nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, "null argument");
   for (int s = 0; s < n_slots; ++s)
@@ -881,7 +962,7 @@ int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const s
       for (int t = 0; same && t < k->n_terms; ++t) same = ks->terms[t].type == k->terms[t].type;
       for (int i = 0; same && i < nh; ++i)
         same = hs[i].kind == kind[i] && (hs[i].kind == SGP_HYPER_SCALE || (hs[i].term == hypers[i].term && hs[i].dim == hdim[i]));
-      if (!same) return fail(c, SGP_E_BADARG, "every class needs the same kernel structure and hyper-parameter layout");
+      if (!same) return fail(c, SGP_E_BADARG, "every class or fold slot needs the same kernel structure and hyper-parameter layout");
     }
     std::vector<double> beta;
     int rc = flatten_kernel(c, ks, d, d, kfs[s], beta, &flat_of);
@@ -934,9 +1015,10 @@ int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const s
   char* dev = c->hyper_ws.as<char>();
   SGP_CUDA(c, cudaMemcpyAsync(dev, host.data(), host.size(), cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));          // host is a local
-  rc = ctx_scratch(c, c->nll_per_ws, static_cast<size_t>(n_slots) * c->ex.E * W * 8);
+  rc = ctx_scratch(c, c->nll_per_ws, static_cast<size_t>(n_slots) * (rows_per_slot > 0 ? rows_per_slot : c->ex.E) * W * 8);
   if (rc != SGP_OK) return rc;
   o.kf = reinterpret_cast<const KernelFlat*>(dev);
+  o.kf_host = std::move(kfs);
   double* dD = reinterpret_cast<double*>(dev + kf_bytes);
   int* dI = reinterpret_cast<int*>(dD + n_dbl);
   hv.beta = dD; hv.h_coef = dD + nb; hv.h_value = hv.h_coef + static_cast<size_t>(nh) * (kMaxTerms + 1);
@@ -948,9 +1030,9 @@ int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const s
 }
 
 // all-reduce over ranks, copy the (objective, gradient) rows of every slot back, map a bad pivot to err_code.  With a
-// classes list, the message names the first failing slot's class.
+// classes (fold sets) list, the message names the first failing slot's class (set), `what` saying which.
 int objective_finish(Ctx* c, const ObjectiveSetup& o, int nh, double* val_out, double* grad_out, int mask, int err_code,
-                     const char* err_msg, const int* classes = nullptr) {
+                     const char* err_msg, const int* classes = nullptr, const char* what = "class") {
   const int W = 1 + nh, S = o.n_slots;
   // the rank-local status flags are all-reduced WITH the totals so that every rank raises (or none does)
   SGP_CUDA(c, launch_flags_to_double(o.total + static_cast<size_t>(S) * W, o.flags, mask, S, c->stream));
@@ -966,7 +1048,8 @@ int objective_finish(Ctx* c, const ObjectiveSetup& o, int nh, double* val_out, d
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   for (int s = 0; s < S; ++s)
     if (tot[static_cast<size_t>(S) * W + s] != 0.0)
-      return fail(c, err_code, classes ? "class " + std::to_string(classes[s]) + ": " + err_msg : std::string(err_msg));
+      return fail(c, err_code, classes ? std::string(what) + " " + std::to_string(classes[s]) + ": " + err_msg
+                                       : std::string(err_msg));
   for (int s = 0; s < S; ++s) {
     val_out[s] = tot[static_cast<size_t>(s) * W];
     for (int i = 1; i < W; ++i) grad_out[static_cast<size_t>(s) * nh + i - 1] = tot[static_cast<size_t>(s) * W + i];
@@ -974,6 +1057,9 @@ int objective_finish(Ctx* c, const ObjectiveSetup& o, int nh, double* val_out, d
   return SGP_OK;
 }
 }  // namespace
+
+const char* const kBcmSingular =
+    "an expert's kernel matrix is singular (MatrixSingularException, logDetAndInv.scala:27-28)";
 
 int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh, double* nll_out,
                 double* grad_out) {
@@ -1013,8 +1099,74 @@ int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
     if (blas_status != 0) return fail(c, SGP_E_CUDA, "cuBLAS batched LU failed, status " + std::to_string(blas_status));
     c->launches += 5;
   }
-  return objective_finish(c, o, nh, nll_out, grad_out, 2, SGP_E_SINGULAR,
-                          "an expert's kernel matrix is singular (MatrixSingularException, logDetAndInv.scala:27-28)");
+  return objective_finish(c, o, nh, nll_out, grad_out, 2, SGP_E_SINGULAR, kBcmSingular);
+}
+
+int sgp_bcm_nll_folds(sgp_ctx* h, const int32_t* sets, int32_t n_eval, const sgp_kernel_desc* kernels,
+                      const sgp_hyper* hypers, int32_t nh, double* nll_out, double* grad_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!nll_out || (nh > 0 && !grad_out) || !sets) return fail(c, SGP_E_BADARG, "sgp_bcm_nll_folds: null argument");
+  if (c->ex.E == 0 || c->fold_first.empty())
+    return fail(c, SGP_E_STATE, "sgp_experts_upload_folds should have been called first");
+  const int n_sets = static_cast<int>(c->fold_first.size()) - 1;
+  if (n_eval < 1 || n_eval > 65535) return fail(c, SGP_E_BADARG, "sgp_bcm_nll_folds: need 1 <= n_eval <= 65535");
+  for (int s = 0; s < n_eval; ++s)
+    if (sets[s] < 0 || sets[s] >= n_sets)
+      return fail(c, SGP_E_BADARG, "sgp_bcm_nll_folds: set index " + std::to_string(sets[s]) + " outside [0, n_folds)");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  const std::vector<long long>& first = c->fold_first;
+  // one plan for the call, on the largest expert over the listed sets; the kernel lays out its shared memory from the
+  // same n_max, so it launches on this view
+  ExpertSet listed = c->ex;
+  long long E_max = 0;
+  listed.n_max = 0;
+  for (int s = 0; s < n_eval; ++s) {
+    listed.n_max = std::max(listed.n_max, c->fold_nmax[sets[s]]);
+    E_max = std::max(E_max, first[sets[s] + 1] - first[sets[s]]);
+  }
+  ObjectiveSetup o;
+  int rc = objective_setup(c, n_eval, kernels, hypers, nh, sets, o, E_max);
+  if (rc != SGP_OK) return rc;
+  const int W = 1 + nh;
+  double* rows = c->nll_per_ws.as<double>();
+  const ObjectivePlan plan = plan_objective(Objective::kBcm, listed, o.hv.kf.n_terms);
+  std::vector<int> flags(n_eval, 1);          // bit 0: the slot goes to the LU path
+  if (plan.variant != ObjectiveVariant::kLu) {
+    BcmFolds f;
+    f.n_slots = n_eval; f.E_max = E_max; f.sets = o.cls; f.first = c->ex_set_first.as<long long>(); f.kf = o.kf;
+    f.slot_stride = o.slot_stride;
+    SGP_CUDA(c, launch_bcm_nll(plan, listed, o.hv, rows, o.total, o.flags, c->stream, &f));
+    c->launches += 2;
+    SGP_CUDA(c, cudaMemcpyAsync(flags.data(), o.flags, sizeof(int) * n_eval, cudaMemcpyDeviceToHost, c->stream));
+    SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  }
+  // a slot whose Cholesky broke down, or every slot when the experts do not fit on chip: the LU path on that slot's set
+  // alone (its experts, its own largest expert), one slot after another
+  c->bcm_general = false;
+  for (int s = 0; s < n_eval; ++s) {
+    if (!(flags[s] & 1)) continue;
+    c->bcm_general = true;
+    const int k = sets[s];
+    ExpertSet set = c->ex;
+    set.off = c->ex.off + first[k];
+    set.E = first[k + 1] - first[k];
+    set.n_max = c->fold_nmax[k];
+    HyperView hv = o.hv;
+    hv.kf = o.kf_host[s];
+    hv.beta += s * o.slot_stride; hv.h_coef += s * o.slot_stride; hv.h_value += s * o.slot_stride;
+    const ObjectivePlan lu = plan_objective(Objective::kBcmLu, set, hv.kf.n_terms);
+    rc = ctx_scratch(c, c->bcm_ws, lu.lu_ws);
+    if (rc != SGP_OK) return rc;
+    SGP_CUDA(c, cudaMemsetAsync(o.flags + s, 0, sizeof(int), c->stream));
+    int blas_status = 0;
+    SGP_CUDA(c, launch_bcm_nll_general(lu, c->blas, &blas_status, c->bcm_ws.p, set, hv,
+                                       rows + static_cast<size_t>(s) * E_max * W, o.total + static_cast<size_t>(s) * W,
+                                       o.flags + s, c->stream));
+    if (blas_status != 0) return fail(c, SGP_E_CUDA, "cuBLAS batched LU failed, status " + std::to_string(blas_status));
+    c->launches += 5;
+  }
+  return objective_finish(c, o, nh, nll_out, grad_out, 2, SGP_E_SINGULAR, kBcmSingular, sets, "fold set");
 }
 
 const char* const kLaplaceRefused =

@@ -14,6 +14,10 @@
 // The reference factors K with LU; K is symmetric positive definite here (the sigma2 Eye term is always present,
 // GPC:18), so Cholesky gives the same log-determinant and inverse (up to rounding) at a third of the work.  A
 // non-positive pivot is reported (the reference would return a negative-determinant "logdet" of |det| instead).
+//
+// Cross-validation (sgp_bcm_nll_folds): a second grid dimension runs several fold training sets of one fold upload in one
+// launch.  Block (x, s) evaluates expert x of the set listed in slot s with slot s's flattened kernel and hyper-parameter
+// block, output row [s][x]; the arithmetic is the single-set body's.
 #include <cstdlib>
 #include <string>
 
@@ -28,14 +32,38 @@ struct NllParams {
   const long long* off;     // [E+1]
   int n_max;                // largest expert
   int x_in_smem;            // the expert's rows are staged in shared memory
-  HyperView hv;
-  double* out;              // [E][1 + n_hypers]   per-expert (nll, gradient)
-  int* flags;               // bit 0: a pivot was not positive
+  HyperView hv;             // slot 0's view; fold slot s reads kf[s] and the descriptor values s * slot_stride doubles on
+  const int* sets;          // [n_slots] fold set of each slot, or nullptr: one slot over every expert
+  const long long* first;   // [n_sets + 1] first expert of each fold set (with sets)
+  const KernelFlat* kf;     // [n_slots] (with sets)
+  long long slot_stride;    // (with sets)
+  double* out;              // [n_slots][gridDim.x][1 + n_hypers]   per-expert (nll, gradient)
+  int* flags;               // [n_slots]  bit 0: a pivot was not positive
 };
+
+// Block (x, s): expert x of slot s's fold set, at slot s's kernel and hyper-parameters (one slot: expert x at p.hv).
+// False when the set has no expert x; the block then returns before its first barrier.
+__device__ __forceinline__ bool nll_block(const NllParams& p, HyperView& hv, long long& e, double*& out) {
+  const int slot = blockIdx.y;
+  e = blockIdx.x;
+  if (p.sets) {
+    const int k = p.sets[slot];
+    const long long first = p.first[k];
+    if (e >= p.first[k + 1] - first) return false;
+    e += first;
+    hv.kf = p.kf[slot];
+    hv.beta += slot * p.slot_stride; hv.h_coef += slot * p.slot_stride; hv.h_value += slot * p.slot_stride;
+  }
+  out = p.out + (static_cast<size_t>(slot) * gridDim.x + blockIdx.x) * (1 + hv.n_hypers);
+  return true;
+}
 
 __global__ void __launch_bounds__(EX_THREADS, 2) bcm_nll_kernel(const NllParams p) {
   extern __shared__ double sm[];
-  const long long e = blockIdx.x;
+  HyperView hv = p.hv;
+  long long e;
+  double* out;
+  if (!nll_block(p, hv, e, out)) return;
   const long long r0 = p.off[e];
   const int n = static_cast<int>(p.off[e + 1] - r0);
   const int ld = p.n_max + 1;                 // padded leading dimension
@@ -48,14 +76,14 @@ __global__ void __launch_bounds__(EX_THREADS, 2) bcm_nll_kernel(const NllParams 
   double* Xs = sums + EX_SUMS;                // [n_max][d|1] staged copy of the expert's rows (if it fits)
   const int tid = threadIdx.x;
   int xld;
-  const double* Xe = ex_stage_rows(p.X + static_cast<size_t>(r0) * p.hv.d, n, p.hv.d, p.x_in_smem, Xs, xld);
+  const double* Xe = ex_stage_rows(p.X + static_cast<size_t>(r0) * hv.d, n, hv.d, p.x_in_smem, Xs, xld);
   for (int i = tid; i < n; i += EX_THREADS) yv[i] = p.y[r0 + i];
   __syncthreads();
-  ex_build_kernel<false>(p.hv, Xe, xld, n, K, ld);
+  ex_build_kernel<false>(hv, Xe, xld, n, K, ld);
   __syncthreads();
   bool bad = false;
   const double logdet = 2.0 * ex_cholesky(K, n, ld, rowbuf, red, bad);
-  if (bad && tid == 0) atomicOr(p.flags, 1);
+  if (bad && tid == 0) atomicOr(p.flags + blockIdx.y, 1);
   ex_invert_lower(K, n, ld, rowbuf);
   ex_ltl_inplace(K, n, ld, rowbuf);           // K now holds K^-1 (lower)
   // ---- alpha = K^-1 y ;  nll ----------------------------------------------------------------------------------------
@@ -68,10 +96,9 @@ __global__ void __launch_bounds__(EX_THREADS, 2) bcm_nll_kernel(const NllParams 
   double part = 0.0;
   for (int a = tid; a < n; a += EX_THREADS) part += yv[a] * alpha[a];
   const double yay = ex_block_sum(part, red);
-  double* out = p.out + static_cast<size_t>(e) * (1 + p.hv.n_hypers);
   if (tid == 0) out[0] = 0.5 * yay + 0.5 * logdet;
   // ---- gradient: -1/2 sum_ab dK_i[a,b] (alpha_a alpha_b - K^-1[a,b])   (GPR:63-66) -----------------------------------
-  ex_descriptor_gradient(p.hv, Xe, xld, n, [&](int a, int b) { return alpha[a] * alpha[b] - K[a * ld + b]; }, -0.5,
+  ex_descriptor_gradient(hv, Xe, xld, n, [&](int a, int b) { return alpha[a] * alpha[b] - K[a * ld + b]; }, -0.5,
                          out + 1, sums, red);
 }
 
@@ -99,10 +126,13 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
   constexpr int NP = 16 * RBC;                // padded order of the matrix (rows beyond NP are never touched)
   constexpr int NR = 32 * RBR;                // >= NP
   extern __shared__ double sm[];
-  const long long e = blockIdx.x;
+  HyperView hv = p.hv;
+  long long e;
+  double* out;
+  if (!nll_block(p, hv, e, out)) return;
   const long long r0 = p.off[e];
   const int n = static_cast<int>(p.off[e + 1] - r0);
-  const int d = p.hv.d, xld = d | 1;
+  const int d = hv.d, xld = d | 1;
   double* ys = sm;                            // [NR]
   double* alpha = ys + NR;                    // [NR]
   double* colbuf = alpha + NR;                // [2][NR]  column of the current sweep (double buffered by sweep parity)
@@ -128,7 +158,7 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
 #pragma unroll
     for (int c = 0; c < RBC; ++c) A[r][c] = 0.0;
   for (int k = 0; k < d; ++k) {
-    const double bk = p.hv.beta[k];
+    const double bk = hv.beta[k];
     double xa[RBR], xb[RBC];
 #pragma unroll
     for (int r = 0; r < RBR; ++r) xa[r] = Xs[(ty + 32 * r) * xld + k] * bk;
@@ -155,14 +185,14 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
     double* kp = Ks + a * NP + b;
     *kp = (a < n && b < n) ? exp(-*kp) : 0.0;
   }
-  const double scale0 = p.hv.kf.term_scale(0);
+  const double scale0 = hv.kf.term_scale(0);
 #pragma unroll
   for (int r = 0; r < RBR; ++r)
 #pragma unroll
     for (int c = 0; c < RBC; ++c) {
       const int a = ty + 32 * r, b = tx + 16 * c;
       const bool real = a < n && b < n;
-      A[r][c] = real ? fma(scale0, Ks[a * NP + b], (a == b) ? p.hv.kf.eye_sum : 0.0) : ((a == b) ? 1.0 : 0.0);
+      A[r][c] = real ? fma(scale0, Ks[a * NP + b], (a == b) ? hv.kf.eye_sum : 0.0) : ((a == b) ? 1.0 : 0.0);
     }
   // ---- n sweeps: A -> -K^-1.  Pivot k = 16 ck + kx sits in row block rk = ck / 2 (ty == 16 (ck % 2) + kx) ------------------
   bool bad = false;
@@ -207,7 +237,7 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
       }
     }
   }
-  if (bad && tid == 0) atomicOr(p.flags, 1);
+  if (bad && tid == 0) atomicOr(p.flags + blockIdx.y, 1);
   __syncthreads();
   // ---- log|det K| = sum log pivot;  alpha = K^-1 y ------------------------------------------------------------------------
   double part = 0.0;
@@ -230,7 +260,6 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
   part = 0.0;
   for (int a = tid; a < n; a += REG_THREADS) part += ys[a] * alpha[a];
   const double yay = ex_block_sum<REG_WARPS>(part, red);
-  double* out = p.out + static_cast<size_t>(e) * (1 + p.hv.n_hypers);
   if (tid == 0) out[0] = 0.5 * yay + 0.5 * logdet;
   // ---- gradient: M = k o (alpha alpha^T - K^-1) in place of A --------------------------------------------------------------
   double S[kMaxTerms], Q[kMaxTerms], D[DCH], trW = 0.0;
@@ -273,40 +302,42 @@ __global__ void __launch_bounds__(REG_THREADS, 1) bcm_nll_reg_kernel(const NllPa
     return acc;
   };
   const int chunks = (d + DCH - 1) / DCH;
-  const int n_sweeps = p.hv.any_ard ? chunks : 1;
-  if (!(p.hv.any_ard && chunks == 1)) {       // Q = sum_ab |x_a - x_b|^2 M_ab = sum_k D_k (RBF sigma); one ARD chunk: below
+  const int n_sweeps = hv.any_ard ? chunks : 1;
+  if (!(hv.any_ard && chunks == 1)) {         // Q = sum_ab |x_a - x_b|^2 M_ab = sum_k D_k (RBF sigma); one ARD chunk: below
     double qsum = 0.0;
     for (int k = 0; k < d; ++k) qsum += dim_sum(k);
     Q[0] = qsum;
   }
   for (int sw = 0; sw < n_sweeps; ++sw) {
-    const int ts = p.hv.any_ard ? 0 : -1;
-    const int k0 = p.hv.any_ard ? sw * DCH : 0;
-    const int kn = p.hv.any_ard ? ((d - k0 < DCH) ? (d - k0) : DCH) : 0;
+    const int ts = hv.any_ard ? 0 : -1;
+    const int k0 = hv.any_ard ? sw * DCH : 0;
+    const int kn = hv.any_ard ? ((d - k0 < DCH) ? (d - k0) : DCH) : 0;
 #pragma unroll
     for (int k = 0; k < DCH; ++k) D[k] = (k < kn) ? dim_sum(k0 + k) : 0.0;
-    if (p.hv.any_ard && chunks == 1) {
+    if (hv.any_ard && chunks == 1) {
       double qsum = 0.0;
 #pragma unroll
       for (int k = 0; k < DCH; ++k) qsum += D[k];
       Q[0] = qsum;
     }
-    ex_gradient_emit<REG_WARPS>(p.hv, sw, ts, k0, kn, S, Q, D, trW, -0.5, out + 1, sums, red);
+    ex_gradient_emit<REG_WARPS>(hv, sw, ts, k0, kn, S, Q, D, trW, -0.5, out + 1, sums, red);
   }
 }
 
 // Sum the per-expert rows: one CTA per column, thread t adds experts t, t+256, ... and the 256 partials are combined by
 // a fixed tree -- the order never depends on timing, so the result is deterministic.  blockIdx.y: the slot (one-vs-rest
-// class) whose rows [E][width] are summed.
+// class, fold slot) whose rows [E][width] are summed; a fold slot sums only its set's experts.
 __global__ void __launch_bounds__(EX_THREADS) rows_reduce_kernel(double* __restrict__ total,
                                                                    const double* __restrict__ per_expert, long long E,
-                                                                   int width) {
+                                                                   int width, const int* __restrict__ sets,
+                                                                   const long long* __restrict__ first) {
   __shared__ double part[EX_THREADS];
   const int c = blockIdx.x;
   total += static_cast<size_t>(blockIdx.y) * width;
   per_expert += static_cast<size_t>(blockIdx.y) * E * width;
+  const long long n_rows = sets ? first[sets[blockIdx.y] + 1] - first[sets[blockIdx.y]] : E;
   double s = 0.0;
-  for (long long e = threadIdx.x; e < E; e += EX_THREADS) s += per_expert[e * width + c];
+  for (long long e = threadIdx.x; e < n_rows; e += EX_THREADS) s += per_expert[e * width + c];
   part[threadIdx.x] = s;
   __syncthreads();
   for (int o = EX_THREADS / 2; o > 0; o >>= 1) {
@@ -453,24 +484,31 @@ ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms) {
 }
 
 cudaError_t launch_rows_reduce(double* dTotal, const double* dPerExpert, long long E, int width, cudaStream_t s,
-                               int n_slots) {
-  rows_reduce_kernel<<<dim3(width, n_slots), EX_THREADS, 0, s>>>(dTotal, dPerExpert, E, width);
+                               int n_slots, const int* sets, const long long* first) {
+  rows_reduce_kernel<<<dim3(width, n_slots), EX_THREADS, 0, s>>>(dTotal, dPerExpert, E, width, sets, first);
   return cudaGetLastError();
 }
 
 cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double* rows, double* total,
-                           int* flags, cudaStream_t s) {
+                           int* flags, cudaStream_t s, const BcmFolds* folds) {
   NllParams p{};
   p.X = ex.X; p.y = ex.y; p.off = ex.off; p.n_max = ex.n_max; p.x_in_smem = plan.x_in_smem;
   p.hv = hv; p.out = rows; p.flags = flags;
+  long long E = ex.E;
+  int n_slots = 1;
+  if (folds) {
+    p.sets = folds->sets; p.first = folds->first; p.kf = folds->kf; p.slot_stride = folds->slot_stride;
+    E = folds->E_max;
+    n_slots = folds->n_slots;
+  }
   const bool reg = plan.variant < ObjectiveVariant::kSmem;
   void (*kernel)(NllParams) = reg ? kRegShapes[static_cast<int>(plan.variant)].kernel : bcm_nll_kernel;
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(plan.smem));
   if (e != cudaSuccess) return e;
-  kernel<<<static_cast<unsigned>(ex.E), reg ? REG_THREADS : EX_THREADS, plan.smem, s>>>(p);
+  kernel<<<dim3(static_cast<unsigned>(E), static_cast<unsigned>(n_slots)), reg ? REG_THREADS : EX_THREADS, plan.smem, s>>>(p);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  return launch_rows_reduce(total, rows, ex.E, 1 + hv.n_hypers, s);
+  return launch_rows_reduce(total, rows, E, 1 + hv.n_hypers, s, n_slots, p.sets, p.first);
 }
 
 cudaError_t launch_bcm_nll_general(const ObjectivePlan& plan, cublasHandle_t blas, int* blas_status, void* ws,

@@ -23,9 +23,10 @@ constexpr int DCH = 16;                                   // ARD dimensions per 
 constexpr int EX_SUMS = 2 * kMaxTerms + 1 + DCH;          // doubles of shared memory the sweep needs
 
 // host side (bcm_nll.cu): total[s][c] = sum_e per_expert[s][e][c] for each of n_slots slots, deterministic; a slot's sums
-// do not depend on the other slots
+// do not depend on the other slots.  E: the slots' row stride and expert count; with sets (device, [n_slots]) and first
+// (device, fold sets' first experts), slot s sums only the first[sets[s] + 1] - first[sets[s]] rows of its stride E.
 cudaError_t launch_rows_reduce(double* dTotal, const double* dPerExpert, long long E, int width, cudaStream_t s,
-                               int n_slots = 1);
+                               int n_slots = 1, const int* sets = nullptr, const long long* first = nullptr);
 
 template <int NW = EX_WARPS>
 __device__ __forceinline__ double ex_block_sum(double v, double* red) {

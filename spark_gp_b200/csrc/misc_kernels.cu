@@ -100,14 +100,27 @@ __global__ void flags_to_double_kernel(double* __restrict__ dst, const int* __re
 // i % E and is its (i / E)-th point.  With k = N / E and r = N % E, experts < r own k+1 points: expert e starts at
 // e*k + min(e, r).  One thread per (point, feature): a strided gather from the row-major input into the expert-major
 // fp64 layout the objective kernels read.
+// A fold's training set (sgp_experts_upload_folds) leaves out the points listed in skip_pos (sorted): point i is then the
+// training set's point i - (left-out points before i), found by a binary search over skip_pos.  Each of a point's d
+// threads runs the same search; the threads of a warp read the same entries.
 __global__ void group_experts_kernel(double* __restrict__ Xe, double* __restrict__ ye, const void* __restrict__ X,
                                      int x_is_f32, const double* __restrict__ y, long long n, int d, long long E,
-                                     long long p0, long long cn) {
+                                     long long p0, long long cn, const long long* __restrict__ skip_pos,
+                                     long long n_skip) {
   const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   if (idx >= cn * d) return;
   const long long li = idx / d;                 // point inside this chunk
   const int k = static_cast<int>(idx % d);
-  const long long i = p0 + li;                  // global point index
+  long long i = p0 + li;                        // global point index, then its training rank
+  if (skip_pos) {
+    long long lo = 0, hi = n_skip;              // lo = number of left-out points before i
+    while (lo < hi) {
+      const long long mid = (lo + hi) >> 1;
+      if (skip_pos[mid] < i) lo = mid + 1; else hi = mid;
+    }
+    if (lo < n_skip && skip_pos[lo] == i) return;
+    i -= lo;
+  }
   const long long e = i % E, pos = i / E;
   const long long kq = n / E, r = n % E;
   const long long dst = e * kq + (e < r ? e : r) + pos;
@@ -117,11 +130,11 @@ __global__ void group_experts_kernel(double* __restrict__ Xe, double* __restrict
   if (k == 0) ye[dst] = y[li];
 }
 
-__global__ void expert_offsets_kernel(long long* __restrict__ off, long long n, long long E) {
+__global__ void expert_offsets_kernel(long long* __restrict__ off, long long n, long long E, long long base) {
   const long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   if (e > E) return;
   const long long kq = n / E, r = n % E;
-  off[e] = e * kq + (e < r ? e : r);
+  off[e] = base + e * kq + (e < r ? e : r);
 }
 
 }  // namespace
@@ -169,14 +182,16 @@ cudaError_t launch_magic_matrix(double* out, const double* invA, const double* i
 }
 
 cudaError_t launch_group_experts(double* Xe, double* ye, const void* dX, int x_is_f32, const double* dy, long long n, int d,
-                                 long long E, long long p0, long long cn, cudaStream_t s) {
+                                 long long E, long long p0, long long cn, const long long* skip_pos, long long n_skip,
+                                 cudaStream_t s) {
   const long long total = cn * d;
-  group_experts_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(Xe, ye, dX, x_is_f32, dy, n, d, E, p0, cn);
+  group_experts_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(Xe, ye, dX, x_is_f32, dy, n, d, E, p0, cn,
+                                                                                  skip_pos, n_skip);
   return cudaGetLastError();
 }
 
-cudaError_t launch_expert_offsets(long long* off, long long n, long long E, cudaStream_t s) {
-  expert_offsets_kernel<<<static_cast<unsigned>((E + 1 + 255) / 256), 256, 0, s>>>(off, n, E);
+cudaError_t launch_expert_offsets(long long* off, long long n, long long E, long long base, cudaStream_t s) {
+  expert_offsets_kernel<<<static_cast<unsigned>((E + 1 + 255) / 256), 256, 0, s>>>(off, n, E, base);
   return cudaGetLastError();
 }
 

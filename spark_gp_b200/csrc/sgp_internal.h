@@ -165,6 +165,12 @@ struct Ctx {
   DevScratch ex_X, ex_y, ex_off, ex_f;
   DevScratch ex_fc;              // one-vs-rest latent modes [ex_classes][n] (sgp_laplace_nll_classes)
   int ex_classes = 0;            // classes ex_fc holds modes for; 0: none since the last upload
+  // fold upload (sgp_experts_upload_folds): the training sets lie one after another in ex; set k owns the experts
+  // fold_first[k] .. fold_first[k+1]-1.  Empty after any other upload.
+  std::vector<long long> fold_first;   // [n_sets + 1]
+  std::vector<int> fold_nmax;          // [n_sets] largest expert of each set
+  DevScratch ex_set_first;             // device copy of fold_first
+  DevScratch fold_pos_ws;              // upload scratch: the point indices grouped by fold, ascending in each fold
   DevScratch nll_per_ws;         // per-expert objective rows
   DevScratch hyper_ws;           // hyper-parameter descriptors + totals + flags of one evaluation
   bool bcm_general = false;      // the last sgp_bcm_nll took the global-memory LU path
@@ -217,9 +223,14 @@ cudaError_t launch_axpby_diag(double* A, const double* K, const double* G, doubl
 cudaError_t launch_set_identity(double* I, int m, cudaStream_t s);
 cudaError_t launch_magic_matrix(double* out, const double* invA, const double* invK, double wn, int m,
                                 cudaStream_t s);
+// Gathers the staged points [p0, p0 + cn) of a training set of n points into E experts.  skip_pos (optional): the sorted
+// indices of the n_skip points left out of the set (a validation fold); a kept point's training rank is its index minus
+// the left-out points before it.  Without skip_pos every point is kept at its own index.
 cudaError_t launch_group_experts(double* Xe, double* ye, const void* dX, int x_is_f32, const double* dy, long long n, int d,
-                                 long long E, long long p0, long long cn, cudaStream_t s);
-cudaError_t launch_expert_offsets(long long* off, long long n, long long E, cudaStream_t s);
+                                 long long E, long long p0, long long cn, const long long* skip_pos, long long n_skip,
+                                 cudaStream_t s);
+// off[e] = base + start of expert e of n points grouped into E experts, e = 0 .. E
+cudaError_t launch_expert_offsets(long long* off, long long n, long long E, long long base, cudaStream_t s);
 cudaError_t launch_status_to_double(double* dst, const int* flags, int mask, const double* norm_sum, double norm_limit,
                                     cudaStream_t s);
 // dst[i] = (flags[i] & mask) ? 1 : 0 for i < n: the per-slot status words of an objective evaluation
@@ -312,9 +323,21 @@ struct ObjectivePlan {
 ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms);
 size_t laplace_smem_bytes(int n_max);   // laplace_kernel without the staged rows (laplace.cu)
 
+// Fold slots of a BCM launch (sgp_bcm_nll_folds): slot s evaluates the experts first[sets[s]] .. first[sets[s] + 1] - 1
+// of a fold upload with the flattened kernel kf[s] and the descriptor values slot_stride doubles per slot after hv's.
+// rows: [n_slots][E_max][1 + n_hypers], total: [n_slots][1 + n_hypers], flags: [n_slots].
+struct BcmFolds {
+  int n_slots = 0;
+  long long E_max = 0;                // the largest expert count over the listed sets
+  const int* sets = nullptr;          // device, [n_slots]
+  const long long* first = nullptr;   // device, [n_sets + 1]
+  const KernelFlat* kf = nullptr;     // device, [n_slots]
+  long long slot_stride = 0;
+};
 // Each launcher runs the planned kernel and sums the per-expert rows [E][1 + n_hypers] into total.
+// folds == nullptr: one slot over every uploaded expert (sgp_bcm_nll)
 cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double* rows, double* total,
-                           int* flags, cudaStream_t s);
+                           int* flags, cudaStream_t s, const BcmFolds* folds = nullptr);
 // ws: plan.lu_ws bytes.  cuBLAS failures are reported through *blas_status.
 cudaError_t launch_bcm_nll_general(const ObjectivePlan& plan, cublasHandle_t blas, int* blas_status, void* ws,
                                    const ExpertSet& ex, const HyperView& hv, double* rows, double* total, int* flags,

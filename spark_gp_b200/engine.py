@@ -247,6 +247,57 @@ class ProjectedProcessEngine:
         modes f of the uploaded experts (warm start), as GaussianProcessClassifier.likelihoodAndGradient does."""
         return self._objective(self._lib.sgp_laplace_nll, kernel, float(tol))
 
+    def experts_upload_folds(self, X, y, fold_of, n_folds: int, dataset_size_for_expert: int):
+        """Uploads the training set of every fold of a k-fold split (`sgp_experts_upload_folds`): set k holds the points
+        with fold_of != k in index order, grouped into experts as `experts_upload_grouped` groups them.  X may be float32
+        or float64.  Returns the number of experts of each set."""
+        X = np.asarray(X)
+        if X.dtype != np.float32:
+            X = np.asarray(X, dtype=np.float64)
+        X = np.ascontiguousarray(X)
+        y = np.ascontiguousarray(y, dtype=np.float64)
+        folds = np.ascontiguousarray(fold_of, dtype=np.int32)
+        if X.ndim != 2 or len(y) != len(X) or folds.shape != (len(X),):
+            raise ValueError("experts_upload_folds: X must be n x d, y and fold_of n entries")
+        self._check(self._lib.sgp_experts_upload_folds(self._h, N.ptr(X), int(X.dtype == np.float32), N.ptr(y), len(X),
+                                                       X.shape[1], N.ptr(folds), int(n_folds),
+                                                       int(dataset_size_for_expert)))
+        self._experts_d = X.shape[1]
+        n_k = len(X) - np.bincount(folds, minlength=int(n_folds))
+        return np.floor(n_k / dataset_size_for_expert + 0.5).astype(np.int64)
+
+    def _slot_descriptors(self, kernels):
+        """Per-slot kernel descriptors and hyper-parameter descriptors of a batched objective: (descs, hypers, n_hypers,
+        the buffers both point into)."""
+        descs = (N.KernelDesc * len(kernels))()
+        keep, hyp, nh = [], None, None
+        for i, k in enumerate(kernels):
+            desc, arr, n_i, kp = self._descriptors(k)
+            if nh is None:
+                nh = n_i
+                hyp = (N.Hyper * max(len(kernels) * nh, 1))()
+            elif n_i != nh:
+                raise ValueError("every slot needs the same hyper-parameter layout")
+            descs[i] = desc
+            for j in range(nh):
+                hyp[i * nh + j] = arr[j]
+            keep.append(kp)
+        return descs, hyp, nh, keep
+
+    def bcm_nll_folds(self, sets, kernels):
+        """The BCM objective of each listed fold set at its own kernels[i], all in one launch (`sgp_bcm_nll_folds`) over
+        the last `experts_upload_folds`.  A set may be listed several times.  Returns (values [n_eval], gradients
+        [n_eval x n_hypers])."""
+        st = np.ascontiguousarray(sets, dtype=np.int32)
+        if st.ndim != 1 or len(st) == 0 or len(st) != len(kernels):
+            raise ValueError("bcm_nll_folds: one kernel per listed set")
+        descs, hyp, nh, keep = self._slot_descriptors(kernels)
+        vals = np.zeros(len(st))
+        grads = np.zeros((len(st), max(nh, 1)))
+        self._check(self._lib.sgp_bcm_nll_folds(self._h, N.ptr(st), len(st), descs, hyp, nh, N.ptr(vals), N.ptr(grads)))
+        del keep
+        return vals, np.ascontiguousarray(grads[:, :nh])
+
     def laplace_nll_classes(self, n_classes: int, classes, kernels, tol: float):
         """One-vs-rest over uploaded class indices: the binary Laplace objective of each listed class c (labels y == c)
         at its own kernels[i], all in one launch (`sgp_laplace_nll_classes`).  Returns (values [n_eval], gradients
@@ -254,19 +305,7 @@ class ProjectedProcessEngine:
         cls = np.ascontiguousarray(classes, dtype=np.int32)
         if cls.ndim != 1 or len(cls) == 0 or len(cls) != len(kernels):
             raise ValueError("laplace_nll_classes: one kernel per listed class")
-        descs = (N.KernelDesc * len(cls))()
-        keep, hyp, nh = [], None, None
-        for i, k in enumerate(kernels):
-            desc, arr, n_i, kp = self._descriptors(k)
-            if nh is None:
-                nh = n_i
-                hyp = (N.Hyper * max(len(cls) * nh, 1))()
-            elif n_i != nh:
-                raise ValueError("laplace_nll_classes: every class needs the same hyper-parameter layout")
-            descs[i] = desc
-            for j in range(nh):
-                hyp[i * nh + j] = arr[j]
-            keep.append(kp)
+        descs, hyp, nh, keep = self._slot_descriptors(kernels)
         vals = np.zeros(len(cls))
         grads = np.zeros((len(cls), max(nh, 1)))
         self._check(self._lib.sgp_laplace_nll_classes(self._h, int(n_classes), N.ptr(cls), len(cls), descs, hyp, nh,

@@ -180,14 +180,12 @@ def optimize_hypers(gp, X, y, engine: ProjectedProcessEngine | None = None):
     engine = engine or ProjectedProcessEngine.acquire(gp._device)
     try:
         obj = BcmObjective(engine, gp.getKernel, X, y, gp._datasetSizeForExpert)
+        launches0 = engine.launch_count()
         k0 = gp.getKernel()
-        x0 = k0.getHyperparameters()
-        lo, up = k0.hyperparameterBoundaries()
-        bounds = [(float(l), None if np.isinf(u) else float(u)) for l, u in zip(lo, up)]
-        res = minimize(lambda t: obj(t), x0, jac=True, method="L-BFGS-B", bounds=bounds,
-                       options=dict(maxiter=gp._maxIter, ftol=gp._tol, gtol=gp._tol))
+        # the same L-BFGS-B call as the cross-validator's lock-step slots, so that a fold slot follows this trajectory
+        res, _ = lbfgsb(obj, k0.getHyperparameters(), lbfgsb_bounds(k0), gp._maxIter, gp._tol)
         gp.last_objective = dict(value=float(res.fun), evaluations=obj.evaluations, iterations=int(res.nit),
-                                 n_experts=obj.n_experts)
+                                 n_experts=obj.n_experts, launches=engine.launch_count() - launches0)
         return np.asarray(res.x, dtype=np.float64)
     finally:
         if own:

@@ -7,6 +7,8 @@ Spark `Dataset` plumbing (label/features columns, RDD caching) has no meaning he
 feature matrix and the labels directly."""
 from __future__ import annotations
 
+import copy
+
 import numpy as np
 
 from . import _native as N
@@ -191,6 +193,24 @@ class GaussianProcessParams:
     def getKernel(self) -> Kernel:
         """commons/GaussianProcessCommons.scala:18: user kernel + sigma2.const * EyeKernel."""
         return self._kernel() + const(self._sigma2) * EyeKernel()
+
+    # the params a ParamMap may set: the setter names without "set"
+    PARAMS = ("sigma2", "datasetSizeForExpert", "activeSetSize", "maxIter", "tol", "seed", "kernel", "activeSetProvider")
+
+    def copy(self, extra=None):
+        """Spark's Params.copy(extra): a new estimator with this one's params (and device and shard size), then the
+        params of `extra` ({name: value}, names as in PARAMS) set through their setters."""
+        extra = dict(extra or {})
+        unknown = sorted(set(extra) - set(self.PARAMS))
+        if unknown:
+            raise ValueError("unknown param(s) %s; the params are %s" % (", ".join(unknown), ", ".join(self.PARAMS)))
+        new = copy.copy(self)
+        for name in ("last_stats", "last_objective"):
+            if hasattr(new, name):
+                setattr(new, name, None)
+        for name, value in extra.items():
+            getattr(new, "set" + name[0].upper() + name[1:])(value)
+        return new
 
 
 class GaussianProjectedProcessRawPredictor:

@@ -14,3 +14,33 @@ def scale(X) -> np.ndarray:
     centered = X - mean
     variance = (centered * centered).sum(axis=0) / n
     return centered / np.sqrt(np.where(variance > 0.0, variance, 1.0))
+
+
+_M64 = (1 << 64) - 1
+
+
+def _mix(z):
+    """SplitMix64's finaliser on Python ints (scalar) or uint64 arrays."""
+    if isinstance(z, np.ndarray):
+        with np.errstate(over="ignore"):
+            z = z + np.uint64(0x9E3779B97F4A7C15)
+            z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+            z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        return z ^ (z >> np.uint64(31))
+    z = (z + 0x9E3779B97F4A7C15) & _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def uniform(seed: int, stream: int, i) -> np.ndarray:
+    """The counter-based generator the library's K-means draws from (DESIGN.md 4.7):
+    u(seed, stream, i) = (mix(mix(mix(seed) ^ stream) ^ i) >> 11) * 2^-53 in [0, 1), for an integer array i."""
+    base = _mix(_mix(int(seed) & _M64) ^ int(stream))
+    z = _mix(np.uint64(base) ^ np.asarray(i, dtype=np.uint64))
+    return (z >> np.uint64(11)).astype(np.float64) * 2.0 ** -53
+
+
+def kfold_assignment(n: int, num_folds: int, seed: int) -> np.ndarray:
+    """CrossValidator's default split: point i goes to fold floor(u(seed, 200, i) * numFolds) (int32)."""
+    return np.floor(uniform(seed, 200, np.arange(int(n))) * int(num_folds)).astype(np.int32)
