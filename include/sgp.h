@@ -211,9 +211,21 @@ int sgp_bcm_nll_folds(sgp_ctx* ctx, const int32_t* sets, int32_t n_eval, const s
 /* Binary classification (labels 0/1 in the uploaded y): per-expert Laplace approximation,
  * classification/GaussianProcessClassifier.scala:74-129 -- Newton iteration for the mode with the reference's step
  * halving, tolerance `tol` and warm start (the latent f of every uploaded point lives on the device, starts at zero
- * and persists across calls), then -log Z and its gradient, summed over experts and ranks. */
+ * and persists across calls), then -log Z and its gradient, summed over experts and ranks.
+ * The on-chip form: every expert's matrices live in shared memory, so an upload whose largest expert has more than 117
+ * points is refused with SGP_E_BADARG.  sgp_laplace_nll_any_size takes any size. */
 int sgp_laplace_nll(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper* hypers, int32_t n_hypers, double tol,
                     double* neg_log_z_out, double* grad_out);
+/* sgp_laplace_nll for experts of any size (GaussianProcessParams.scala:36 puts no bound on datasetSizeForExpert): same
+ * arguments, outputs, modes, warm start and all-reduce.  When the largest uploaded expert fits on chip (<= 117 points)
+ * it makes exactly sgp_laplace_nll's launch, so the results are the same bits.  Otherwise a global-memory kernel runs:
+ * a persistent grid over the experts, each CTA with a workspace slice of 8 ld (2 ld + 44) bytes, ld = the largest
+ * expert rounded up to 32 (the grid is bounded by the experts, the resident CTAs and 4 GiB of workspace), the Cholesky
+ * of B and the cubic post-loop steps blocked on fp64 tensor cores.  Its bits do not depend on the grid or on the other
+ * experts of the upload.  SGP_E_NOMEM, before the launch, when one slice exceeds the device's free memory;
+ * SGP_E_BADARG above 46336 points per expert.  sgp_last_laplace_path tells which kernel ran. */
+int sgp_laplace_nll_any_size(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper* hypers, int32_t n_hypers,
+                             double tol, double* neg_log_z_out, double* grad_out);
 /* The latent modes f (same packed expert-major order as the uploaded points): the `y := f` of GPCls:62-65. */
 int sgp_experts_get_f(sgp_ctx* ctx, double* f_out);
 
@@ -227,10 +239,17 @@ int sgp_experts_get_f(sgp_ctx* ctx, double* f_out);
  * bit, what sgp_laplace_nll returns on an upload of the labels (y == c) with the same modes, whichever other classes are
  * in the call.  With a communicator: one ncclAllReduce of the n_eval rows and n_eval status words.
  * Errors: SGP_E_BADARG for bad or repeated class indices, a structure that differs between classes, and experts above the
- * on-chip limit (as sgp_laplace_nll); SGP_E_NOT_PD naming the first listed class whose B broke down. */
+ * on-chip limit (as sgp_laplace_nll: the on-chip form); SGP_E_NOT_PD naming the first listed class whose B broke down. */
 int sgp_laplace_nll_classes(sgp_ctx* ctx, int32_t n_classes, const int32_t* classes, int32_t n_eval,
                             const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t n_hypers, double tol,
                             double* neg_log_z_out /* n_eval */, double* grad_out /* n_eval x n_hypers */);
+/* sgp_laplace_nll_classes for experts of any size, as sgp_laplace_nll_any_size: on chip (the same launch and bits as
+ * sgp_laplace_nll_classes) when the largest expert fits, else the global-memory kernel over experts x listed classes.
+ * On either path class c's value, gradient and modes equal, bit for bit, what sgp_laplace_nll_any_size returns on an
+ * upload of the labels (y == c) with the same modes. */
+int sgp_laplace_nll_classes_any_size(sgp_ctx* ctx, int32_t n_classes, const int32_t* classes, int32_t n_eval,
+                                     const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t n_hypers, double tol,
+                                     double* neg_log_z_out /* n_eval */, double* grad_out /* n_eval x n_hypers */);
 /* Class cls's latent modes (packed expert-major order, n entries).  SGP_E_STATE before the first sgp_laplace_nll_classes
  * after an upload; SGP_E_BADARG for cls outside [0, n_classes). */
 int sgp_experts_get_f_class(sgp_ctx* ctx, int32_t cls, double* f_out);
@@ -274,6 +293,9 @@ int sgp_last_path(const sgp_ctx* ctx);
 int sgp_last_tail_path(const sgp_ctx* ctx);
 /* Which path the last sgp_bcm_nll took: 0 = on-chip Cholesky kernel, 1 = global-memory LU (reference arithmetic). */
 int sgp_last_bcm_path(const sgp_ctx* ctx);
+/* Which kernel the last sgp_laplace_nll* call ran: 0 = on chip (laplace_kernel), 1 = global memory (experts above the
+ * on-chip limit, *_any_size entries only), -1 = none has run on this context. */
+int sgp_last_laplace_path(const sgp_ctx* ctx);
 /* Debug aid for SGP_PREC_I8: the first call arms a dump; later calls return, for the first 64-point unit of
  * the first CTA of the last launch, T = -q*log2(e) (128 active rows x 64 points, fp32) and the fixed-point words
  * (0x4B000000 | (u + 0x4040)), u = s2*2^15 + s1*2^7 + s0 in balanced digits. */

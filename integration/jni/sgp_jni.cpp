@@ -195,7 +195,7 @@ JNIEXPORT jdoubleArray JNICALL Java_org_apache_spark_ml_commons_NativeProjectedP
   Objective o;
   build_objective(o, nt, ty, sc, sg, be, d, nh, hk, ht, hd, hv, hc);
   std::vector<double> out(1 + nh, 0.0);
-  const int rc = (tol > 0.0) ? sgp_laplace_nll(ctx, &o.desc, o.hypers.data(), nh, tol, &out[0], out.data() + 1)
+  const int rc = (tol > 0.0) ? sgp_laplace_nll_any_size(ctx, &o.desc, o.hypers.data(), nh, tol, &out[0], out.data() + 1)
                              : sgp_bcm_nll(ctx, &o.desc, o.hypers.data(), nh, &out[0], out.data() + 1);
   env->ReleaseIntArrayElements(types, ty, JNI_ABORT);
   env->ReleaseDoubleArrayElements(scales, sc, JNI_ABORT);

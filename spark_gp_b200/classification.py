@@ -72,7 +72,7 @@ class GaussianProcessClassifier(GaussianProcessParams):
             theta = k0.getHyperparameters()
             if self._maxIter > 0 and len(theta) > 0:                # memoised like DiffFunctionMemoized; f warm-starts
                 res, evaluations = lbfgsb(
-                    lambda t: eng.laplace_nll(self.getKernel().setHyperparameters(t), self._tol),
+                    lambda t: eng.laplace_nll_any_size(self.getKernel().setHyperparameters(t), self._tol),
                     theta, lbfgsb_bounds(k0), self._maxIter, self._tol)
                 theta = np.asarray(res.x, dtype=np.float64)
                 self.last_objective = dict(value=float(res.fun), evaluations=evaluations, iterations=int(res.nit),
@@ -80,7 +80,7 @@ class GaussianProcessClassifier(GaussianProcessParams):
         else:
             theta = np.asarray(hyperparameters, dtype=np.float64)
         # GPCls:60: run the Laplace loop once more at the optimum so every expert's f is the mode at theta*
-        eng.laplace_nll(self.getKernel().setHyperparameters(theta), self._tol)
+        eng.laplace_nll_any_size(self.getKernel().setHyperparameters(theta), self._tol)
         f_packed = eng.experts_f(len(X))
         f = np.empty(len(X))
         f[order] = f_packed
@@ -111,7 +111,7 @@ def _produce_model(gp, eng, X, f, theta):
 # out of every class's positives.
 #
 # All classes share X and the expert grouping (GPC:26-31), so the points are uploaded and grouped once, and each round of
-# the C hyper-parameter optimisations is one `sgp_laplace_nll_classes` launch over experts x classes.  Each class runs the
+# the C hyper-parameter optimisations is one `sgp_laplace_nll_classes_any_size` launch over experts x classes.  Each class runs the
 # binary pipeline: f_c from 0, its own L-BFGS-B from the same x0 and bounds, the Laplace loop once more at theta*_c
 # (GPCls:60), then produceModel with y := f_c.  The results are the binary classifier's on (y == c), bit for bit.
 
@@ -206,8 +206,8 @@ class OneVsRest:
             thetas = np.tile(np.asarray(x0, dtype=np.float64), (C, 1))
             if gp._maxIter > 0 and len(x0) > 0:
                 def evaluate(batch):
-                    vals, grads = eng.laplace_nll_classes(C, [c for c, _ in batch], [kernel_at(t) for _, t in batch],
-                                                          gp._tol)
+                    vals, grads = eng.laplace_nll_classes_any_size(C, [c for c, _ in batch],
+                                                                   [kernel_at(t) for _, t in batch], gp._tol)
                     return [(float(v), g) for v, g in zip(vals, grads)]
 
                 results, rounds = lbfgsb_lockstep(evaluate, [x0] * C, lbfgsb_bounds(k0), gp._maxIter, gp._tol)
@@ -216,7 +216,7 @@ class OneVsRest:
                     classes=[dict(value=float(res.fun), evaluations=ev, iterations=int(res.nit)) for res, ev in results],
                     rounds=rounds, launches=eng.launch_count() - launches0)
         # GPCls:60 for every class at once: each class's f is its mode at theta*_c
-        eng.laplace_nll_classes(C, np.arange(C), [kernel_at(t) for t in thetas], gp._tol)
+        eng.laplace_nll_classes_any_size(C, np.arange(C), [kernel_at(t) for t in thetas], gp._tol)
         latent = np.empty((C, len(X)))
         models = []
         for c in range(C):

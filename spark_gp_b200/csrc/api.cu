@@ -1173,27 +1173,56 @@ const char* const kLaplaceRefused =
     "datasetSizeForExpert too large for the on-chip Laplace kernel (max ~115 points per expert)";
 const char* const kLaplaceNotPd = "an expert's B = I + sqrt(W) K sqrt(W) is not positive definite (increase sigma2)";
 
-int sgp_laplace_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh, double tol,
-                    double* neg_log_z_out, double* grad_out) {
-  Ctx* c = reinterpret_cast<Ctx*>(h);
-  if (!c) return SGP_E_BADARG;
+namespace {
+// The Laplace objective of the set-up slots (classes: the one-vs-rest slots, or nullptr), on the kernel plan_objective
+// picks for `kind`: laplace_kernel when the largest expert fits on chip, laplace_global_kernel otherwise (any size only).
+int laplace_run(Ctx* c, Objective kind, const ObjectiveSetup& o, double tol, const LaplaceClasses* classes) {
+  const ObjectivePlan plan = plan_objective(kind, c->ex, o.hv.kf.n_terms);
+  if (plan.variant == ObjectiveVariant::kRefused) return fail(c, SGP_E_BADARG, kLaplaceRefused);
+  if (plan.variant == ObjectiveVariant::kLaplace) {
+    SGP_CUDA(c, launch_laplace(plan, c->ex, o.hv, tol, c->nll_per_ws.as<double>(), o.total, o.flags, c->stream, classes));
+    c->laplace_path = 0;
+    c->launches += 2;
+    return SGP_OK;
+  }
+  // global-memory kernel: one workspace slice per CTA; the grid is bounded by the work items, the resident CTAs and the
+  // workspace that fits under kLaplaceGlobalCapBytes and the device's free memory (what this context holds included)
+  size_t free_b = 0, total_b = 0;
+  SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+  const size_t avail = free_b + c->laplace_ws.cap;
+  if (plan.cta_ws > avail)
+    return fail(c, SGP_E_NOMEM, "the global-memory Laplace kernel needs " + std::to_string(plan.cta_ws >> 20) +
+                                    " MiB of device memory for one expert of " + std::to_string(c->ex.n_max) +
+                                    " points, " + std::to_string(avail >> 20) + " MiB available");
+  if (c->ex.n_max > kLaplaceGlobalMaxPoints)
+    return fail(c, SGP_E_BADARG, "datasetSizeForExpert above " + std::to_string(kLaplaceGlobalMaxPoints) +
+                                     " points (32-bit indexing of the per-expert kernel build)");
+  const long long items = c->ex.E * (classes ? classes->n_slots : 1);
+  const long long resident = static_cast<long long>(laplace_global_ctas_per_sm()) * c->num_sms;
+  const long long grid = laplace_global_grid(items, resident, plan.cta_ws, std::min(kLaplaceGlobalCapBytes, avail));
+  int rc = ctx_scratch(c, c->laplace_ws, static_cast<size_t>(grid) * plan.cta_ws);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, launch_laplace_global(c->ex, o.hv, tol, c->laplace_ws.as<double>(), grid, c->nll_per_ws.as<double>(),
+                                    o.total, o.flags, c->stream, classes));
+  c->laplace_path = 1;
+  c->launches += 2;
+  return SGP_OK;
+}
+
+int laplace_nll(Ctx* c, Objective kind, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh, double tol,
+                double* neg_log_z_out, double* grad_out) {
   if (!neg_log_z_out || (nh > 0 && !grad_out) || !(tol > 0.0)) return fail(c, SGP_E_BADARG, "sgp_laplace_nll: bad argument");
   SGP_CUDA(c, cudaSetDevice(c->device));
   ObjectiveSetup o;
   int rc = objective_setup(c, 1, k, hypers, nh, nullptr, o);
+  if (rc == SGP_OK) rc = laplace_run(c, kind, o, tol, nullptr);
   if (rc != SGP_OK) return rc;
-  const ObjectivePlan plan = plan_objective(Objective::kLaplace, c->ex, o.hv.kf.n_terms);
-  if (plan.variant == ObjectiveVariant::kRefused) return fail(c, SGP_E_BADARG, kLaplaceRefused);
-  SGP_CUDA(c, launch_laplace(plan, c->ex, o.hv, tol, c->nll_per_ws.as<double>(), o.total, o.flags, c->stream));
-  c->launches += 2;
   return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd);
 }
 
-int sgp_laplace_nll_classes(sgp_ctx* h, int32_t n_classes, const int32_t* classes, int32_t n_eval,
-                            const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t nh, double tol,
-                            double* neg_log_z_out, double* grad_out) {
-  Ctx* c = reinterpret_cast<Ctx*>(h);
-  if (!c) return SGP_E_BADARG;
+int laplace_nll_classes(Ctx* c, Objective kind, int32_t n_classes, const int32_t* classes, int32_t n_eval,
+                        const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t nh, double tol,
+                        double* neg_log_z_out, double* grad_out) {
   if (!neg_log_z_out || (nh > 0 && !grad_out) || !(tol > 0.0) || !classes)
     return fail(c, SGP_E_BADARG, "sgp_laplace_nll_classes: bad argument");
   if (n_classes < 1 || n_eval < 1 || n_eval > n_classes || n_eval > 65535)
@@ -1206,8 +1235,8 @@ int sgp_laplace_nll_classes(sgp_ctx* h, int32_t n_classes, const int32_t* classe
   ObjectiveSetup o;
   int rc = objective_setup(c, n_eval, kernels, hypers, nh, classes, o);
   if (rc != SGP_OK) return rc;
-  const ObjectivePlan plan = plan_objective(Objective::kLaplace, c->ex, o.hv.kf.n_terms);
-  if (plan.variant == ObjectiveVariant::kRefused) return fail(c, SGP_E_BADARG, kLaplaceRefused);
+  if (plan_objective(kind, c->ex, o.hv.kf.n_terms).variant == ObjectiveVariant::kRefused)
+    return fail(c, SGP_E_BADARG, kLaplaceRefused);
   if (c->ex_classes != n_classes) {                       // first use after an upload, or another class count
     const size_t bytes = static_cast<size_t>(n_classes) * c->ex.n * 8;
     rc = ctx_scratch(c, c->ex_fc, bytes);
@@ -1217,9 +1246,42 @@ int sgp_laplace_nll_classes(sgp_ctx* h, int32_t n_classes, const int32_t* classe
   }
   LaplaceClasses lc;
   lc.n_slots = n_eval; lc.cls = o.cls; lc.kf = o.kf; lc.slot_stride = o.slot_stride; lc.f = c->ex_fc.as<double>();
-  SGP_CUDA(c, launch_laplace(plan, c->ex, o.hv, tol, c->nll_per_ws.as<double>(), o.total, o.flags, c->stream, &lc));
-  c->launches += 2;
+  rc = laplace_run(c, kind, o, tol, &lc);
+  if (rc != SGP_OK) return rc;
   return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd, classes);
+}
+}  // namespace
+
+int sgp_laplace_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh, double tol,
+                    double* neg_log_z_out, double* grad_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return laplace_nll(c, Objective::kLaplace, k, hypers, nh, tol, neg_log_z_out, grad_out);
+}
+
+int sgp_laplace_nll_any_size(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh, double tol,
+                             double* neg_log_z_out, double* grad_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return laplace_nll(c, Objective::kLaplaceAnySize, k, hypers, nh, tol, neg_log_z_out, grad_out);
+}
+
+int sgp_laplace_nll_classes(sgp_ctx* h, int32_t n_classes, const int32_t* classes, int32_t n_eval,
+                            const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t nh, double tol,
+                            double* neg_log_z_out, double* grad_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return laplace_nll_classes(c, Objective::kLaplace, n_classes, classes, n_eval, kernels, hypers, nh, tol, neg_log_z_out,
+                             grad_out);
+}
+
+int sgp_laplace_nll_classes_any_size(sgp_ctx* h, int32_t n_classes, const int32_t* classes, int32_t n_eval,
+                                     const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t nh, double tol,
+                                     double* neg_log_z_out, double* grad_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return laplace_nll_classes(c, Objective::kLaplaceAnySize, n_classes, classes, n_eval, kernels, hypers, nh, tol,
+                             neg_log_z_out, grad_out);
 }
 
 int sgp_experts_get_f_class(sgp_ctx* h, int32_t cls, double* f_out) {
@@ -1253,6 +1315,11 @@ int sgp_last_path(const sgp_ctx* h) {
 int sgp_last_bcm_path(const sgp_ctx* h) {
   const Ctx* c = reinterpret_cast<const Ctx*>(h);
   return c ? (c->bcm_general ? 1 : 0) : -1;
+}
+
+int sgp_last_laplace_path(const sgp_ctx* h) {
+  const Ctx* c = reinterpret_cast<const Ctx*>(h);
+  return c ? c->laplace_path : -1;
 }
 
 int sgp_last_tail_path(const sgp_ctx* h) {

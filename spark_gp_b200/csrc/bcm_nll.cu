@@ -458,8 +458,13 @@ ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms) {
     plan.smem = plan.x_in_smem ? with_x : smem;
     return plan;
   };
-  if (kind == Objective::kLaplace) {
-    if (laplace_smem_bytes(ex.n_max) > kSmemOptInMax) return plan;      // kRefused
+  if (kind == Objective::kLaplace || kind == Objective::kLaplaceAnySize) {
+    if (laplace_smem_bytes(ex.n_max) > kSmemOptInMax) {
+      if (kind == Objective::kLaplace) return plan;                      // kRefused
+      plan.variant = ObjectiveVariant::kLaplaceGlobal;
+      plan.cta_ws = laplace_global_cta_bytes(ex.n_max);
+      return plan;
+    }
     return stage_rows(ObjectiveVariant::kLaplace, laplace_smem_bytes(ex.n_max), kSmemOptInMax);
   }
   // experts whose shared-memory Cholesky does not fit, or a kernel matrix on which it broke down: the LU path

@@ -36,6 +36,10 @@ constexpr int kMaxHypers = 72;     // hyper-parameters of one objective evaluati
 // launch window (3 bytes per point and padded active row: configs[1] 3.1 GB in one window, configs[3] 7.7 GB in two)
 constexpr size_t kI8PlaneBytes = 3 * kTile * 64;
 constexpr size_t kI8PlaneCapBytes = size_t(4) << 30;
+// global-memory Laplace path: the largest workspace of one launch (one slice per CTA of the persistent grid)
+constexpr size_t kLaplaceGlobalCapBytes = size_t(4) << 30;
+// ... and its largest expert: the kernel build shared with the on-chip kernels indexes rows of the n x n matrix in int
+constexpr int kLaplaceGlobalMaxPoints = 46336;
 // prediction: the fp64 cross kernel of one window of points takes at most this much device memory (configs[1]'s m = 1000:
 // 32768 points per window)
 constexpr size_t kPredictKBytes = size_t(256) << 20;
@@ -174,6 +178,8 @@ struct Ctx {
   DevScratch nll_per_ws;         // per-expert objective rows
   DevScratch hyper_ws;           // hyper-parameter descriptors + totals + flags of one evaluation
   bool bcm_general = false;      // the last sgp_bcm_nll took the global-memory LU path
+  int laplace_path = -1;         // the last sgp_laplace_nll*: 0 on chip, 1 global memory, -1 none yet
+  DevScratch laplace_ws;         // laplace_global_kernel: one workspace slice per CTA
   // tail / predict state
   DevScratch dMagicVec;          // m
   DevScratch dMagicMat;          // m x m
@@ -305,11 +311,14 @@ struct HyperView {
   const double* h_value;     // [n_hypers] current value of the hyper-parameter (beta_k or sigma)
 };
 
-enum class Objective { kBcm, kBcmLu, kLaplace };   // kBcmLu: the BCM objective after its Cholesky broke down
+// kBcmLu: the BCM objective after its Cholesky broke down.  kLaplace: on chip only (refused past the shared-memory
+// limit); kLaplaceAnySize: on chip when the largest expert fits, else the global-memory kernel.
+enum class Objective { kBcm, kBcmLu, kLaplace, kLaplaceAnySize };
 enum class ObjectiveVariant {
   kReg24, kReg36, kReg47, kReg48,   // BCM: bcm_nll_reg_kernel<RBR, RBC>
   kSmem,                            // BCM: bcm_nll_kernel (shared-memory Cholesky)
   kLu,                              // BCM: global-memory LU path (cuBLAS batched LU / inverse)
+  kLaplaceGlobal,                   // laplace_global_kernel (matrices in global memory, persistent grid)
   kLaplace,                         // laplace_kernel
   kRefused                          // Laplace: the expert does not fit on chip
 };
@@ -319,9 +328,11 @@ struct ObjectivePlan {
   int x_in_smem = 0;   // the kernel stages the expert's rows in shared memory
   size_t smem = 0;     // dynamic shared memory per CTA
   size_t lu_ws = 0;    // kLu: global-memory workspace
+  size_t cta_ws = 0;   // kLaplaceGlobal: global-memory workspace of one CTA (the launch takes one per CTA)
 };
 ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms);
 size_t laplace_smem_bytes(int n_max);   // laplace_kernel without the staged rows (laplace.cu)
+size_t laplace_global_cta_bytes(int n_max);   // laplace_global_kernel's workspace per CTA (laplace_global.cu)
 
 // Fold slots of a BCM launch (sgp_bcm_nll_folds): slot s evaluates the experts first[sets[s]] .. first[sets[s] + 1] - 1
 // of a fold upload with the flattened kernel kf[s] and the descriptor values slot_stride doubles per slot after hv's.
@@ -355,6 +366,13 @@ struct LaplaceClasses {
 // classes == nullptr: one slot on the labels and modes as uploaded (sgp_laplace_nll)
 cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol, double* rows,
                            double* total, int* flags, cudaStream_t s, const LaplaceClasses* classes = nullptr);
+// The global-memory kernel (plan kLaplaceGlobal) on `grid` CTAs, CTA b on the slice ws + b * plan.cta_ws.  The grid
+// is laplace_global_grid(E * n_slots, laplace_global_ctas_per_sm() * SMs, plan.cta_ws, workspace budget).
+int laplace_global_ctas_per_sm();
+long long laplace_global_grid(long long items, long long resident, size_t cta_bytes, size_t budget);
+cudaError_t launch_laplace_global(const ExpertSet& ex, const HyperView& hv, double tol, double* ws, long long grid,
+                                  double* rows, double* total, int* flags, cudaStream_t s,
+                                  const LaplaceClasses* classes = nullptr);
 
 int ctx_scratch(Ctx* c, DevScratch& s, size_t bytes);
 // csrc/greedy.cu: forward selection with rank-1 updates (ActiveSetProvider.scala:58-139); beta_flat = [n_terms][d]

@@ -247,6 +247,15 @@ class ProjectedProcessEngine:
         modes f of the uploaded experts (warm start), as GaussianProcessClassifier.likelihoodAndGradient does."""
         return self._objective(self._lib.sgp_laplace_nll, kernel, float(tol))
 
+    def laplace_nll_any_size(self, kernel: Kernel, tol: float):
+        """`laplace_nll` for experts of any size (`sgp_laplace_nll_any_size`): the same launch and bits while the largest
+        expert fits on chip (117 points), the global-memory kernel above."""
+        return self._objective(self._lib.sgp_laplace_nll_any_size, kernel, float(tol))
+
+    def last_laplace_path(self) -> int:
+        """Which kernel the last Laplace objective ran: 0 on chip, 1 global memory, -1 none yet."""
+        return int(self._lib.sgp_last_laplace_path(self._h))
+
     def experts_upload_folds(self, X, y, fold_of, n_folds: int, dataset_size_for_expert: int):
         """Uploads the training set of every fold of a k-fold split (`sgp_experts_upload_folds`): set k holds the points
         with fold_of != k in index order, grouped into experts as `experts_upload_grouped` groups them.  X may be float32
@@ -302,14 +311,21 @@ class ProjectedProcessEngine:
         """One-vs-rest over uploaded class indices: the binary Laplace objective of each listed class c (labels y == c)
         at its own kernels[i], all in one launch (`sgp_laplace_nll_classes`).  Returns (values [n_eval], gradients
         [n_eval x n_hypers]); each class's device-resident modes warm-start its next evaluation."""
+        return self._laplace_classes(self._lib.sgp_laplace_nll_classes, n_classes, classes, kernels, tol)
+
+    def laplace_nll_classes_any_size(self, n_classes: int, classes, kernels, tol: float):
+        """`laplace_nll_classes` for experts of any size (`sgp_laplace_nll_classes_any_size`)."""
+        return self._laplace_classes(self._lib.sgp_laplace_nll_classes_any_size, n_classes, classes, kernels, tol)
+
+    def _laplace_classes(self, fn, n_classes, classes, kernels, tol):
         cls = np.ascontiguousarray(classes, dtype=np.int32)
         if cls.ndim != 1 or len(cls) == 0 or len(cls) != len(kernels):
             raise ValueError("laplace_nll_classes: one kernel per listed class")
         descs, hyp, nh, keep = self._slot_descriptors(kernels)
         vals = np.zeros(len(cls))
         grads = np.zeros((len(cls), max(nh, 1)))
-        self._check(self._lib.sgp_laplace_nll_classes(self._h, int(n_classes), N.ptr(cls), len(cls), descs, hyp, nh,
-                                                      float(tol), N.ptr(vals), N.ptr(grads)))
+        self._check(fn(self._h, int(n_classes), N.ptr(cls), len(cls), descs, hyp, nh, float(tol), N.ptr(vals),
+                       N.ptr(grads)))
         del keep
         return vals, np.ascontiguousarray(grads[:, :nh])
 
