@@ -213,7 +213,10 @@ int sgp_bcm_nll_folds(sgp_ctx* ctx, const int32_t* sets, int32_t n_eval, const s
  * halving, tolerance `tol` and warm start (the latent f of every uploaded point lives on the device, starts at zero
  * and persists across calls), then -log Z and its gradient, summed over experts and ranks.
  * The on-chip form: every expert's matrices live in shared memory, so an upload whose largest expert has more than 117
- * points is refused with SGP_E_BADARG.  sgp_laplace_nll_any_size takes any size. */
+ * points is refused with SGP_E_BADARG.  sgp_laplace_nll_any_size takes any size.
+ * tol must be > 0 (SGP_E_BADARG otherwise).  tol >= 1 returns SGP_E_SINGULAR before any launch, with the modes left as
+ * they were: the loop runs while step > tol and step starts at 1, so no Newton iteration runs, the reference's L stays
+ * zero and `L \ sqrtW` throws MatrixSingularException. */
 int sgp_laplace_nll(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper* hypers, int32_t n_hypers, double tol,
                     double* neg_log_z_out, double* grad_out);
 /* sgp_laplace_nll for experts of any size (GaussianProcessParams.scala:36 puts no bound on datasetSizeForExpert): same
@@ -223,7 +226,8 @@ int sgp_laplace_nll(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper
  * expert rounded up to 32 (the grid is bounded by the experts, the resident CTAs and 4 GiB of workspace), the Cholesky
  * of B and the cubic post-loop steps blocked on fp64 tensor cores.  Its bits do not depend on the grid or on the other
  * experts of the upload.  SGP_E_NOMEM, before the launch, when one slice exceeds the device's free memory;
- * SGP_E_BADARG above 46336 points per expert.  sgp_last_laplace_path tells which kernel ran. */
+ * SGP_E_BADARG above 46336 points per expert; SGP_E_SINGULAR for tol >= 1, as sgp_laplace_nll.  sgp_last_laplace_path
+ * tells which kernel ran. */
 int sgp_laplace_nll_any_size(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper* hypers, int32_t n_hypers,
                              double tol, double* neg_log_z_out, double* grad_out);
 /* The latent modes f (same packed expert-major order as the uploaded points): the `y := f` of GPCls:62-65. */
@@ -239,14 +243,16 @@ int sgp_experts_get_f(sgp_ctx* ctx, double* f_out);
  * bit, what sgp_laplace_nll returns on an upload of the labels (y == c) with the same modes, whichever other classes are
  * in the call.  With a communicator: one ncclAllReduce of the n_eval rows and n_eval status words.
  * Errors: SGP_E_BADARG for bad or repeated class indices, a structure that differs between classes, and experts above the
- * on-chip limit (as sgp_laplace_nll: the on-chip form); SGP_E_NOT_PD naming the first listed class whose B broke down. */
+ * on-chip limit (as sgp_laplace_nll: the on-chip form); SGP_E_NOT_PD naming the first listed class whose B broke down;
+ * SGP_E_SINGULAR for tol >= 1 (no Newton iteration runs, as sgp_laplace_nll), before any launch, every class's modes
+ * left as they were. */
 int sgp_laplace_nll_classes(sgp_ctx* ctx, int32_t n_classes, const int32_t* classes, int32_t n_eval,
                             const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t n_hypers, double tol,
                             double* neg_log_z_out /* n_eval */, double* grad_out /* n_eval x n_hypers */);
 /* sgp_laplace_nll_classes for experts of any size, as sgp_laplace_nll_any_size: on chip (the same launch and bits as
  * sgp_laplace_nll_classes) when the largest expert fits, else the global-memory kernel over experts x listed classes.
  * On either path class c's value, gradient and modes equal, bit for bit, what sgp_laplace_nll_any_size returns on an
- * upload of the labels (y == c) with the same modes. */
+ * upload of the labels (y == c) with the same modes.  SGP_E_SINGULAR for tol >= 1, as sgp_laplace_nll_classes. */
 int sgp_laplace_nll_classes_any_size(sgp_ctx* ctx, int32_t n_classes, const int32_t* classes, int32_t n_eval,
                                      const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t n_hypers, double tol,
                                      double* neg_log_z_out /* n_eval */, double* grad_out /* n_eval x n_hypers */);

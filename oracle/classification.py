@@ -15,8 +15,13 @@ def _sigmoid(x):
     return 1.0 / (1.0 + np.exp(-x))
 
 
-def classification_likelihood_and_gradient(y: np.ndarray, f: np.ndarray, kernel, x: np.ndarray, tol: float):
-    """GPCls:74-129.  Mutates `f` in place (the expert's latent mode).  Returns (-logZ, -gradLogZ)."""
+def classification_likelihood_and_gradient(y: np.ndarray, f: np.ndarray, kernel, x: np.ndarray, tol: float,
+                                           trace=None):
+    """GPCls:74-129.  Mutates `f` in place (the expert's latent mode).  Returns (-logZ, -gradLogZ).
+
+    `trace`, when a list, receives one dict per Newton iteration -- step, cand, old_obj and new_obj (before the
+    comparison), accepted, and max_abs_f (max |f| after the iteration) -- and then one {"exit": reason}: "converged"
+    (|old_obj - new_obj| <= tol), "step" (step <= tol) or "none" (no iteration ran).  It changes no result."""
     kernel.set_hyperparameters(x)
     K, derivatives = kernel.training_kernel_and_derivative()
     n = len(y)
@@ -29,6 +34,7 @@ def classification_likelihood_and_gradient(y: np.ndarray, f: np.ndarray, kernel,
     grad_log_p = np.zeros(n)
     I = np.eye(n)
     step = 1.0
+    iterations = 0
     while abs(old_obj - new_obj) > tol and step > tol:                      # :91
         pi = _sigmoid(f)
         W = np.diag(pi * (1.0 - pi))
@@ -45,12 +51,20 @@ def classification_likelihood_and_gradient(y: np.ndarray, f: np.ndarray, kernel,
         a = b - sqrtW @ sla.solve_triangular(L.T, inner, lower=False)
         new_f = (1.0 - step) * f + step * (K @ a)                            # :102
         new_obj_cand = -float(a @ new_f) / 2.0 + float(np.sum(np.log(_sigmoid((y * 2.0 - 1.0) * new_f))))
+        if trace is not None:
+            trace.append(dict(step=step, cand=new_obj_cand, old_obj=old_obj, new_obj=new_obj,
+                              accepted=bool(new_obj_cand > old_obj)))
+            iterations += 1
         if new_obj_cand > old_obj:                                          # :104-107
             f[:] = new_f
             old_obj = new_obj
             new_obj = new_obj_cand
         else:
             step /= 2.0
+        if trace is not None:
+            trace[-1]["max_abs_f"] = float(np.abs(f).max()) if n else 0.0
+    if trace is not None:
+        trace.append({"exit": "none" if iterations == 0 else "converged" if not abs(old_obj - new_obj) > tol else "step"})
     logZ = new_obj - float(np.sum(np.log(np.diag(L))))                      # :114
     # :116  R = sqrtW * L.t \ (L \ sqrtW)  -> sqrtW * (L.t \ (L \ sqrtW))  (same precedence argument)
     R = sqrtW @ sla.solve_triangular(L.T, sla.solve_triangular(L, sqrtW, lower=True), lower=False)

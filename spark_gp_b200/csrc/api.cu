@@ -1172,6 +1172,9 @@ int sgp_bcm_nll_folds(sgp_ctx* h, const int32_t* sets, int32_t n_eval, const sgp
 const char* const kLaplaceRefused =
     "datasetSizeForExpert too large for the on-chip Laplace kernel (max ~115 points per expert)";
 const char* const kLaplaceNotPd = "an expert's B = I + sqrt(W) K sqrt(W) is not positive definite (increase sigma2)";
+const char* const kLaplaceNoIteration =
+    "tol >= 1: no Newton iteration runs (the loop needs step = 1 > tol), so L stays zero and L \\ sqrtW throws "
+    "MatrixSingularException (GaussianProcessClassifier.scala:91,116)";
 
 namespace {
 // The Laplace objective of the set-up slots (classes: the one-vs-rest slots, or nullptr), on the kernel plan_objective
@@ -1212,6 +1215,7 @@ int laplace_run(Ctx* c, Objective kind, const ObjectiveSetup& o, double tol, con
 int laplace_nll(Ctx* c, Objective kind, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh, double tol,
                 double* neg_log_z_out, double* grad_out) {
   if (!neg_log_z_out || (nh > 0 && !grad_out) || !(tol > 0.0)) return fail(c, SGP_E_BADARG, "sgp_laplace_nll: bad argument");
+  if (tol >= 1.0) return fail(c, SGP_E_SINGULAR, kLaplaceNoIteration);
   SGP_CUDA(c, cudaSetDevice(c->device));
   ObjectiveSetup o;
   int rc = objective_setup(c, 1, k, hypers, nh, nullptr, o);
@@ -1231,6 +1235,7 @@ int laplace_nll_classes(Ctx* c, Objective kind, int32_t n_classes, const int32_t
   std::sort(sorted.begin(), sorted.end());
   if (sorted.front() < 0 || sorted.back() >= n_classes || std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
     return fail(c, SGP_E_BADARG, "sgp_laplace_nll_classes: class indices must be distinct and in [0, n_classes)");
+  if (tol >= 1.0) return fail(c, SGP_E_SINGULAR, kLaplaceNoIteration);
   SGP_CUDA(c, cudaSetDevice(c->device));
   ObjectiveSetup o;
   int rc = objective_setup(c, n_eval, kernels, hypers, nh, classes, o);
