@@ -172,7 +172,10 @@ typedef struct {
  * Experts of any size (GaussianProcessParams.scala:36 sets no bound).  Fast path: on-chip Cholesky per expert (<= ~165
  * points, SPD).  When an expert is larger, or a Cholesky pivot is not positive, the evaluation runs the reference's own
  * arithmetic instead -- LU with partial pivoting, log|det| with the sign dropped (logDetAndInv.scala:36-63, GPR:59) --
- * and only an exactly singular matrix fails, with SGP_E_SINGULAR (Breeze's MatrixSingularException). */
+ * and only an exactly singular matrix fails, with SGP_E_SINGULAR (Breeze's MatrixSingularException).
+ * The LU path holds every expert's matrix and inverse at once, about 16 E n_max^2 bytes (E experts, n_max the largest):
+ * SGP_E_NOMEM, before any launch, when that exceeds the device's free memory.  SGP_E_BADARG, before any allocation or
+ * launch, above 46340 points per expert (32-bit indexing of the per-expert matrix, as for the Laplace limit below). */
 int sgp_bcm_nll(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper* hypers, int32_t n_hypers,
                 double* nll_out, double* grad_out);
 
@@ -202,8 +205,9 @@ int sgp_experts_upload_folds(sgp_ctx* ctx, const void* X, int32_t x_is_f32, cons
  * the on-chip kernels put every slot on the LU path, one slot after another: 5 launches per slot instead of 2 per call.
  * sgp_last_bcm_path is 1 if any slot ran LU.  With a communicator: one ncclAllReduce of the n_eval rows and n_eval status
  * words.  Errors: SGP_E_STATE without a fold upload; SGP_E_BADARG for a set index outside [0, n_folds), a structure that
- * differs between slots, or n_eval outside [1, 65535]; SGP_E_SINGULAR naming the first slot's set whose matrix is
- * exactly singular. */
+ * differs between slots, or n_eval outside [1, 65535], or more than 46340 points in the largest expert of a listed set
+ * (before any allocation or launch); SGP_E_NOMEM when a slot's LU workspace exceeds the device's free memory, as for
+ * sgp_bcm_nll; SGP_E_SINGULAR naming the first slot's set whose matrix is exactly singular. */
 int sgp_bcm_nll_folds(sgp_ctx* ctx, const int32_t* sets, int32_t n_eval, const sgp_kernel_desc* kernels,
                       const sgp_hyper* hypers, int32_t n_hypers, double* nll_out /* n_eval */,
                       double* grad_out /* n_eval x n_hypers */);

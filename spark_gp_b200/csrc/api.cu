@@ -1061,12 +1061,39 @@ int objective_finish(Ctx* c, const ObjectiveSetup& o, int nh, double* val_out, d
 const char* const kBcmSingular =
     "an expert's kernel matrix is singular (MatrixSingularException, logDetAndInv.scala:27-28)";
 
+namespace {
+// The LU path indexes an expert's n x n matrix in int: refused above kBcmLuMaxPoints, before any allocation or launch.
+int bcm_check_size(Ctx* c, int n_max, const char* fn) {
+  if (n_max <= kBcmLuMaxPoints) return SGP_OK;
+  return fail(c, SGP_E_BADARG, std::string(fn) + ": datasetSizeForExpert above " + std::to_string(kBcmLuMaxPoints) +
+                                   " points (the largest expert has " + std::to_string(n_max) +
+                                   "; 32-bit indexing of the per-expert kernel matrix)");
+}
+
+// c->bcm_ws sized for the LU path's workspace (every expert's K and K^-1 at once).  SGP_E_NOMEM, before allocating, when
+// it exceeds the device's free memory plus what bcm_ws already holds.
+int bcm_lu_workspace(Ctx* c, const ObjectivePlan& plan) {
+  size_t free_b = 0, total_b = 0;
+  SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+  const size_t avail = free_b + c->bcm_ws.cap;
+  if (plan.lu_ws > avail)
+    return fail(c, SGP_E_NOMEM, "the BCM objective's LU path needs " + std::to_string(plan.lu_ws >> 20) +
+                                    " MiB of device memory for the experts' kernel matrices and inverses, " +
+                                    std::to_string(avail >> 20) + " MiB available (lower datasetSizeForExpert)");
+  return ctx_scratch(c, c->bcm_ws, plan.lu_ws);
+}
+}  // namespace
+
 int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh, double* nll_out,
                 double* grad_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
   if (!nll_out || (nh > 0 && !grad_out)) return fail(c, SGP_E_BADARG, "sgp_bcm_nll: null output");
   SGP_CUDA(c, cudaSetDevice(c->device));
+  if (c->ex.E > 0) {
+    const int rc = bcm_check_size(c, c->ex.n_max, "sgp_bcm_nll");
+    if (rc != SGP_OK) return rc;
+  }
   ObjectiveSetup o;
   int rc = objective_setup(c, 1, k, hypers, nh, nullptr, o);
   if (rc != SGP_OK) return rc;
@@ -1090,7 +1117,7 @@ int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   }
   c->bcm_general = plan.variant == ObjectiveVariant::kLu;
   if (c->bcm_general) {
-    rc = ctx_scratch(c, c->bcm_ws, plan.lu_ws);
+    rc = bcm_lu_workspace(c, plan);
     if (rc != SGP_OK) return rc;
     SGP_CUDA(c, cudaMemsetAsync(dFlags, 0, sizeof(int), c->stream));
     int blas_status = 0;
@@ -1125,8 +1152,10 @@ int sgp_bcm_nll_folds(sgp_ctx* h, const int32_t* sets, int32_t n_eval, const sgp
     listed.n_max = std::max(listed.n_max, c->fold_nmax[sets[s]]);
     E_max = std::max(E_max, first[sets[s] + 1] - first[sets[s]]);
   }
+  int rc = bcm_check_size(c, listed.n_max, "sgp_bcm_nll_folds");
+  if (rc != SGP_OK) return rc;
   ObjectiveSetup o;
-  int rc = objective_setup(c, n_eval, kernels, hypers, nh, sets, o, E_max);
+  rc = objective_setup(c, n_eval, kernels, hypers, nh, sets, o, E_max);
   if (rc != SGP_OK) return rc;
   const int W = 1 + nh;
   double* rows = c->nll_per_ws.as<double>();
@@ -1156,7 +1185,7 @@ int sgp_bcm_nll_folds(sgp_ctx* h, const int32_t* sets, int32_t n_eval, const sgp
     hv.kf = o.kf_host[s];
     hv.beta += s * o.slot_stride; hv.h_coef += s * o.slot_stride; hv.h_value += s * o.slot_stride;
     const ObjectivePlan lu = plan_objective(Objective::kBcmLu, set, hv.kf.n_terms);
-    rc = ctx_scratch(c, c->bcm_ws, lu.lu_ws);
+    rc = bcm_lu_workspace(c, lu);
     if (rc != SGP_OK) return rc;
     SGP_CUDA(c, cudaMemsetAsync(o.flags + s, 0, sizeof(int), c->stream));
     int blas_status = 0;

@@ -353,7 +353,8 @@ __global__ void __launch_bounds__(EX_THREADS) rows_reduce_kernel(double* __restr
 // (commons/util/logDetAndInv.scala:58-63 -> LAPACK dgetrf), log|det| = sum log|u_ii| with the SIGN IGNORED (GPR:59 drops
 // it), inverse from the same factors (dgetri).  The kernel matrices live in global memory ([E][n_max][n_max], experts
 // smaller than n_max padded with an identity block); the factorizations are cuBLAS' batched LU / inverse (plain library
-// calls on small dense matrices), the build / objective / gradient kernels are ours.
+// calls on small dense matrices), the build / objective / gradient kernels are ours.  Every index into an n_max x n_max
+// matrix that the build shares with the on-chip kernels is an int: n_max <= kBcmLuMaxPoints.
 // ---------------------------------------------------------------------------------------------------------------------
 struct GenParams {
   const double* X; const double* y; const long long* off;
@@ -361,6 +362,8 @@ struct GenParams {
   HyperView hv;
   double* A;                // [E][n_max][n_max]  K, then its LU factors
   const double* Ainv;       // [E][n_max][n_max]  inverse
+  double* ya;               // [E][2][n_max]  y and alpha of each expert when 2 n_max doubles do not fit in shared memory
+                            // (plan.ya_in_ws), else nullptr: they live in shared memory
   const int* info;          // [E] dgetrf info (> 0: exactly singular)
   double* out;              // [E][1 + n_hypers]
   int* flags;               // bit 1: some expert's matrix is singular (MatrixSingularException)
@@ -385,9 +388,9 @@ __global__ void __launch_bounds__(EX_THREADS) gen_objective_kernel(const GenPara
   const long long e = blockIdx.x;
   const long long r0 = p.off[e];
   const int n = static_cast<int>(p.off[e + 1] - r0), ld = p.n_max;
-  double* yv = sm;                       // [n_max]
+  double* yv = p.ya ? p.ya + static_cast<size_t>(e) * 2 * ld : sm;   // [n_max]
   double* alpha = yv + p.n_max;          // [n_max]
-  double* red = alpha + p.n_max;         // [8]
+  double* red = p.ya ? sm : alpha + p.n_max;                         // [8]
   double* sums = red + 8;                // [EX_SUMS]
   double* Xs = sums + EX_SUMS;
   const int tid = threadIdx.x;
@@ -441,9 +444,12 @@ size_t gen_objective_smem_bytes(int n_max) { return sizeof(double) * (2 * static
 
 }  // namespace
 
+// [E][n_max][n_max] K / LU, [E][n_max][n_max] K^-1, [E][2][n_max] y and alpha, 2 E pointers, E info, E n_max pivots
 size_t bcm_general_workspace_bytes(long long E, int n_max) {
   const size_t mat = static_cast<size_t>(E) * n_max * n_max * sizeof(double);
-  return 2 * mat + static_cast<size_t>(E) * (2 * sizeof(double*) + sizeof(int) * (1 + static_cast<size_t>(n_max))) + 256;
+  const size_t ya = static_cast<size_t>(E) * 2 * n_max * sizeof(double);
+  return 2 * mat + ya + static_cast<size_t>(E) * (2 * sizeof(double*) + sizeof(int) * (1 + static_cast<size_t>(n_max))) +
+         256;
 }
 size_t bcm_nll_smem_bytes(int n_max) {
   return sizeof(double) * (static_cast<size_t>(n_max) * (n_max + 1) + 3 * static_cast<size_t>(n_max) + 8 + EX_SUMS);
@@ -470,7 +476,12 @@ ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms) {
   // experts whose shared-memory Cholesky does not fit, or a kernel matrix on which it broke down: the LU path
   if (kind == Objective::kBcmLu || bcm_nll_smem_bytes(ex.n_max) > kSmemOptInMax) {
     plan.lu_ws = bcm_general_workspace_bytes(ex.E, ex.n_max);
-    return stage_rows(ObjectiveVariant::kLu, gen_objective_smem_bytes(ex.n_max), kStageGeneral);
+    stage_rows(ObjectiveVariant::kLu, gen_objective_smem_bytes(ex.n_max), kStageGeneral);
+    if (plan.smem > kSmemOptInMax) {     // n_max > 14511: y and alpha go to the workspace (the rows are not staged here)
+      plan.ya_in_ws = 1;
+      plan.smem = gen_objective_smem_bytes(0);
+    }
+    return plan;
   }
   // one non-Eye term, experts of <= 128 points: the register-resident kernel (SGP_BCM_IMPL=smem selects the other one)
   static const bool force_smem = [] { const char* e = getenv("SGP_BCM_IMPL"); return e && std::string(e) == "smem"; }();
@@ -525,13 +536,14 @@ cudaError_t launch_bcm_nll_general(const ObjectivePlan& plan, cublasHandle_t bla
   const size_t mat = static_cast<size_t>(E) * n_max * n_max;
   double* A = static_cast<double*>(ws);
   double* Ainv = A + mat;
-  double** Aptr = reinterpret_cast<double**>(Ainv + mat);
+  double* ya = Ainv + mat;
+  double** Aptr = reinterpret_cast<double**>(ya + static_cast<size_t>(E) * 2 * n_max);
   double** Cptr = Aptr + E;
   int* info = reinterpret_cast<int*>(Cptr + E);
   int* piv = info + E;
   GenParams p{};
   p.X = ex.X; p.y = ex.y; p.off = ex.off; p.n_max = n_max; p.x_in_smem = plan.x_in_smem;
-  p.hv = hv; p.A = A; p.Ainv = Ainv; p.info = info; p.out = rows; p.flags = flags;
+  p.hv = hv; p.A = A; p.Ainv = Ainv; p.ya = plan.ya_in_ws ? ya : nullptr; p.info = info; p.out = rows; p.flags = flags;
   gen_build_kernel<<<static_cast<unsigned>(E), EX_THREADS, 0, s>>>(p, Aptr, Cptr, Ainv);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;

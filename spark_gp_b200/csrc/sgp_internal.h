@@ -40,6 +40,9 @@ constexpr size_t kI8PlaneCapBytes = size_t(4) << 30;
 constexpr size_t kLaplaceGlobalCapBytes = size_t(4) << 30;
 // ... and its largest expert: the kernel build shared with the on-chip kernels indexes rows of the n x n matrix in int
 constexpr int kLaplaceGlobalMaxPoints = 46336;
+// BCM LU path (sgp_bcm_nll, sgp_bcm_nll_folds): its largest expert, for the same reason; the n x n matrix has leading
+// dimension n, so n^2 <= 2^31 - 1
+constexpr int kBcmLuMaxPoints = 46340;
 // prediction: the fp64 cross kernel of one window of points takes at most this much device memory (configs[1]'s m = 1000:
 // 32768 points per window)
 constexpr size_t kPredictKBytes = size_t(256) << 20;
@@ -328,6 +331,7 @@ struct ObjectivePlan {
   int x_in_smem = 0;   // the kernel stages the expert's rows in shared memory
   size_t smem = 0;     // dynamic shared memory per CTA
   size_t lu_ws = 0;    // kLu: global-memory workspace
+  int ya_in_ws = 0;    // kLu: y and alpha live in lu_ws (2 n_max doubles do not fit in shared memory)
   size_t cta_ws = 0;   // kLaplaceGlobal: global-memory workspace of one CTA (the launch takes one per CTA)
 };
 ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms);

@@ -32,7 +32,9 @@ namespace sgp {
       return fail((c), SGP_E_CUDA, std::string(#expr) + ": cusolver status " + std::to_string((int)st_)); \
   } while (0)
 
-// Grow-only device scratch owned by the context.
+// Grow-only device scratch owned by the context.  A failed cudaMalloc also records its error as the runtime's last
+// error, which the launch check of the next kernel on this thread would report; it is cleared here, and an
+// out-of-memory failure returns SGP_E_NOMEM.
 int ctx_scratch(Ctx* c, DevScratch& s, size_t bytes) {
   if (bytes <= s.cap && s.p) return SGP_OK;
   if (s.p) {
@@ -41,7 +43,13 @@ int ctx_scratch(Ctx* c, DevScratch& s, size_t bytes) {
     cudaFree(s.p);
     s.p = nullptr; s.cap = 0;
   }
-  SGP_CUDA(c, cudaMalloc(&s.p, bytes ? bytes : 8));
+  const cudaError_t e = cudaMalloc(&s.p, bytes ? bytes : 8);
+  if (e != cudaSuccess) {
+    s.p = nullptr;
+    cudaGetLastError();
+    return fail(c, e == cudaErrorMemoryAllocation ? SGP_E_NOMEM : SGP_E_CUDA,
+                "cudaMalloc of " + std::to_string(bytes >> 20) + " MiB: " + cudaGetErrorString(e));
+  }
   s.cap = bytes ? bytes : 8;
   return SGP_OK;
 }
