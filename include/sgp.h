@@ -264,6 +264,31 @@ int sgp_laplace_nll_classes_any_size(sgp_ctx* ctx, int32_t n_classes, const int3
  * after an upload; SGP_E_BADARG for cls outside [0, n_classes). */
 int sgp_experts_get_f_class(sgp_ctx* ctx, int32_t cls, double* f_out);
 
+/* Model selection over param maps (TrainValidationSplit over the binary classifier or one-vs-rest): the Laplace
+ * objective of n_eval slots in one launch over experts x slots, where slots may share a class and each keeps latent modes
+ * of its own.  Listed slot i evaluates the labels (y == classes[i]) at kernels[i] and hypers[i * n_hypers ...] (the same
+ * kernel structure and descriptor layout for every slot), and reads and writes the modes of mode slot mode_slots[i].
+ * Classes may repeat (the binary classifier passes class 1 over its 0/1 labels: y == 1 is y itself); mode slots are
+ * distinct and in [0, n_mode_slots).  The modes live in a store [n_mode_slots][n] of their own, apart from
+ * sgp_laplace_nll_classes's, so neither entry moves the other's modes: allocated on first use, zero after every
+ * sgp_experts_upload* and whenever n_mode_slots changes; the modes of mode slots not listed are left as they are.
+ * Outputs per listed slot, in list order: neg_log_z_out[i], grad_out[i * n_hypers ...].  Slot i's value, gradient and
+ * modes equal, bit for bit, what sgp_laplace_nll_any_size returns on an upload of the labels (y == classes[i]) with the
+ * same modes, whichever other slots are in the call, on the on-chip and on the global-memory kernel alike (the kernel is
+ * chosen as sgp_laplace_nll_any_size chooses it).  With a communicator: one ncclAllReduce of the n_eval rows and n_eval
+ * status words.  Errors: SGP_E_STATE without an upload; SGP_E_BADARG for a repeated or out-of-range mode slot, a negative
+ * class, n_eval > n_mode_slots, n_eval outside [1, 65535], or a structure that differs between slots; SGP_E_SINGULAR for
+ * tol >= 1, before any launch, every mode left as it was; SGP_E_NOT_PD naming the mode slot of the first listed slot
+ * whose B broke down; SGP_E_NOMEM, before any launch, when the store or one global-memory workspace slice exceeds the
+ * device's free memory. */
+int sgp_laplace_nll_slots_any_size(sgp_ctx* ctx, int32_t n_mode_slots, const int32_t* mode_slots,
+                                   const int32_t* classes, int32_t n_eval, const sgp_kernel_desc* kernels,
+                                   const sgp_hyper* hypers, int32_t n_hypers, double tol,
+                                   double* neg_log_z_out /* n_eval */, double* grad_out /* n_eval x n_hypers */);
+/* Mode slot mode_slot's latent modes (packed expert-major order, n entries).  SGP_E_STATE before the first
+ * sgp_laplace_nll_slots_any_size after an upload; SGP_E_BADARG for mode_slot outside [0, n_mode_slots). */
+int sgp_experts_get_f_slot(sgp_ctx* ctx, int32_t mode_slot, double* f_out);
+
 /* Installs a caller-supplied (vector v, m x m matrix M, row-major) in place of the pair sgp_magic computes, so that
  * sgp_predict returns  mean_t = k(x_t, Z) . v  and  var_t = selfKernel + k(x_t, Z) M k(x_t, Z)^T  for them.  M need not be
  * bit-symmetric: the variance is the quadratic form of M itself.  This is the per-point part of

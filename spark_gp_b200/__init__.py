@@ -10,4 +10,5 @@ from .regression import (GaussianProcessRegression, GaussianProcessRegressionMod
                          GreedilyOptimizingActiveSetProvider, KMeansActiveSetProvider)
 from .classification import GaussianProcessClassifier, GaussianProcessClassificationModel, OneVsRest, OneVsRestModel
 from .utils import scale
-from .tuning import CrossValidator, CrossValidatorModel, ParamGridBuilder, RegressionEvaluator
+from .tuning import (CrossValidator, CrossValidatorModel, ParamGridBuilder, RegressionEvaluator,
+                     MulticlassClassificationEvaluator, TrainValidationSplit, TrainValidationSplitModel)

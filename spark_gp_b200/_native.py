@@ -24,7 +24,8 @@ EXPORTS = ["sgp_ctx_create", "sgp_ctx_destroy", "sgp_last_error", "sgp_set_preci
            "sgp_event_elapsed_ms", "sgp_debug_i8_tile", "sgp_last_path", "sgp_experts_upload",
            "sgp_bcm_nll", "sgp_laplace_nll", "sgp_experts_get_f", "sgp_set_magic", "sgp_last_tail_path", "sgp_last_bcm_path", "sgp_experts_upload_grouped", "sgp_kmn_sweep", "sgp_kmn_sweep_device", "sgp_greedy_active_set", "sgp_kmeans",
            "sgp_laplace_nll_classes", "sgp_experts_get_f_class", "sgp_experts_upload_folds", "sgp_bcm_nll_folds",
-           "sgp_laplace_nll_any_size", "sgp_laplace_nll_classes_any_size", "sgp_last_laplace_path"]
+           "sgp_laplace_nll_any_size", "sgp_laplace_nll_classes_any_size", "sgp_last_laplace_path",
+           "sgp_laplace_nll_slots_any_size", "sgp_experts_get_f_slot"]
 
 
 class KernelTerm(C.Structure):
@@ -96,6 +97,8 @@ def load() -> C.CDLL:
     lib.sgp_laplace_nll_classes_any_size.argtypes = [vp, i32, vp, i32, vp, vp, i32, C.c_double, vp, vp]
     lib.sgp_last_laplace_path.argtypes = [vp]
     lib.sgp_experts_get_f_class.argtypes = [vp, i32, vp]
+    lib.sgp_laplace_nll_slots_any_size.argtypes = [vp, i32, vp, vp, i32, vp, vp, i32, C.c_double, vp, vp]
+    lib.sgp_experts_get_f_slot.argtypes = [vp, i32, vp]
     lib.sgp_experts_upload_folds.argtypes = [vp, vp, i32, vp, i64, i32, vp, i32, i32]
     lib.sgp_bcm_nll_folds.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp]
     lib.sgp_event_elapsed_ms.argtypes = [vp, C.c_int, C.c_int, dp]

@@ -179,6 +179,19 @@ class OneVsRest:
     def getClassifier(self):
         return self._classifier
 
+    def copy(self, extra=None):
+        """Spark's OneVsRest.copy(extra): a OneVsRest over classifier.copy(extra).  The params of `extra` are the wrapped
+        classifier's (GaussianProcessParams.PARAMS)."""
+        extra = dict(extra or {})
+        unknown = sorted(set(extra) - set(GaussianProcessParams.PARAMS))
+        if unknown:
+            raise ValueError("unknown param(s) %s; the params are %s"
+                             % (", ".join(unknown), ", ".join(GaussianProcessParams.PARAMS)))
+        new = OneVsRest()
+        if self._classifier is not None:
+            new.setClassifier(self._classifier.copy(extra))
+        return new
+
     def fit(self, X, y, hyperparameters=None) -> OneVsRestModel:
         """hyperparameters: None (optimise every class, as the binary fit does) or numClasses x n_hypers fixed values."""
         gp = self._classifier

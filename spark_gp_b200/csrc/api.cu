@@ -781,6 +781,7 @@ int experts_alloc(Ctx* c, long long E, long long n, int d, int n_max) {
   SGP_CUDA(c, cudaMemsetAsync(ex.f, 0, static_cast<size_t>(n) * 8, c->stream));
   ex.n = n; ex.d = d; ex.n_max = n_max;
   c->ex_classes = 0;                                      // one-vs-rest modes restart at zero on their next use
+  c->ex_mode_slots = 0;                                   // so do the param-map slots' modes
   c->fold_first.clear();
   c->fold_nmax.clear();
   return SGP_OK;
@@ -928,6 +929,7 @@ struct ObjectiveSetup {
   const KernelFlat* kf = nullptr;  // [n_slots]
   std::vector<KernelFlat> kf_host; // [n_slots]
   const int* cls = nullptr;        // [n_slots] the classes (fold sets) list, or zeros
+  const int* mode = nullptr;       // [n_slots] the mode slots list (sgp_laplace_nll_slots_any_size), else cls
   double* total = nullptr;         // [n_slots][1 + n_hypers] totals, then [n_slots] status words
   int* flags = nullptr;            // [n_slots]
 };
@@ -935,9 +937,10 @@ struct ObjectiveSetup {
 // Flattens each slot's kernel (flatten_kernel: Eye terms only add to the diagonal), maps the hyper-parameter descriptors
 // (hypers + s * nh for slot s) onto the flattened terms and uploads everything, with zeroed totals and flags, into the
 // context's descriptor block in one copy.  Every slot must have slot 0's kernel structure and descriptor kinds.
-// rows_per_slot: the per-expert rows a slot writes (0: every uploaded expert).
+// rows_per_slot: the per-expert rows a slot writes (0: every uploaded expert).  modes: a mode slots list uploaded after
+// the classes (nullptr: o.mode is the classes list).
 int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int nh,
-                    const int* classes, ObjectiveSetup& o, long long rows_per_slot = 0) {
+                    const int* classes, ObjectiveSetup& o, long long rows_per_slot = 0, const int* modes = nullptr) {
   if (c->ex.E == 0) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
   if (!kernels || nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, "null argument");
   for (int s = 0; s < n_slots; ++s)
@@ -997,11 +1000,12 @@ int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const s
     block.insert(block.end(), coef.begin(), coef.end());
     block.insert(block.end(), value.begin(), value.end());
   }
-  // [KernelFlat n_slots] then doubles [slot blocks | totals | status], then ints [kind | term | dim | flags | classes]
+  // [KernelFlat n_slots] then doubles [slot blocks | totals | status], then ints [kind | term | dim | flags | classes
+  // | modes (with modes)]
   const int W = 1 + nh;
   const size_t kf_bytes = sizeof(KernelFlat) * n_slots;
   const size_t n_dbl = block.size() + static_cast<size_t>(n_slots) * (W + 1);
-  const size_t n_int = 3 * static_cast<size_t>(nh) + 2 * static_cast<size_t>(n_slots);
+  const size_t n_int = 3 * static_cast<size_t>(nh) + (modes ? 3 : 2) * static_cast<size_t>(n_slots);
   std::vector<char> host(kf_bytes + n_dbl * 8 + n_int * 4, 0);
   std::memcpy(host.data(), kfs.data(), kf_bytes);
   std::memcpy(host.data() + kf_bytes, block.data(), block.size() * 8);
@@ -1010,6 +1014,7 @@ int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const s
   std::copy(hterm.begin(), hterm.end(), hi + nh);
   std::copy(hdim.begin(), hdim.end(), hi + 2 * nh);
   if (classes) std::copy(classes, classes + n_slots, hi + 3 * nh + n_slots);
+  if (modes) std::copy(modes, modes + n_slots, hi + 3 * nh + 2 * n_slots);
   int rc = ctx_scratch(c, c->hyper_ws, host.size());
   if (rc != SGP_OK) return rc;
   char* dev = c->hyper_ws.as<char>();
@@ -1026,6 +1031,7 @@ int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const s
   hv.h_kind = dI; hv.h_term = dI + nh; hv.h_dim = dI + 2 * nh;
   o.flags = dI + 3 * nh;
   o.cls = dI + 3 * nh + n_slots;
+  o.mode = modes ? o.cls + n_slots : o.cls;
   return SGP_OK;
 }
 
@@ -1253,6 +1259,50 @@ int laplace_nll(Ctx* c, Objective kind, const sgp_kernel_desc* k, const sgp_hype
   return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd);
 }
 
+// The Laplace objective of n_eval slots over a mode store: slot i evaluates the labels (y == classes[i]) at kernels[i]
+// and hypers[i * nh ...], with the modes of store slot modes[i] (nullptr: modes = classes).  The store holds n_store
+// slots of n modes; it is (re)allocated and zeroed when *store_slots, the count it was set up for, differs (0 after every
+// upload).  The callers have checked the lists; `what` names a slot in the SGP_E_NOT_PD message.
+int laplace_slots(Ctx* c, Objective kind, DevScratch& store, int* store_slots, int n_store, const int32_t* classes,
+                  const int32_t* modes, int32_t n_eval, const sgp_kernel_desc* kernels, const sgp_hyper* hypers,
+                  int32_t nh, double tol, double* neg_log_z_out, double* grad_out, const char* what) {
+  if (tol >= 1.0) return fail(c, SGP_E_SINGULAR, kLaplaceNoIteration);
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  ObjectiveSetup o;
+  int rc = objective_setup(c, n_eval, kernels, hypers, nh, classes, o, 0, modes);
+  if (rc != SGP_OK) return rc;
+  if (plan_objective(kind, c->ex, o.hv.kf.n_terms).variant == ObjectiveVariant::kRefused)
+    return fail(c, SGP_E_BADARG, kLaplaceRefused);
+  if (*store_slots != n_store) {                          // first use after an upload, or another slot count
+    const size_t bytes = static_cast<size_t>(n_store) * c->ex.n * 8;
+    size_t free_b = 0, total_b = 0;
+    SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+    if (bytes > free_b + store.cap)
+      return fail(c, SGP_E_NOMEM, "the Laplace modes of " + std::to_string(n_store) + " slots need " +
+                                      std::to_string(bytes >> 20) + " MiB of device memory, " +
+                                      std::to_string((free_b + store.cap) >> 20) + " MiB available");
+    *store_slots = 0;                                     // a failed allocation leaves no store behind
+    rc = ctx_scratch(c, store, bytes);
+    if (rc != SGP_OK) return rc;
+    SGP_CUDA(c, cudaMemsetAsync(store.p, 0, bytes, c->stream));
+    *store_slots = n_store;
+  }
+  LaplaceClasses lc;
+  lc.n_slots = n_eval; lc.cls = o.cls; lc.mode = o.mode; lc.kf = o.kf; lc.slot_stride = o.slot_stride;
+  lc.f = store.as<double>();
+  rc = laplace_run(c, kind, o, tol, &lc);
+  if (rc != SGP_OK) return rc;
+  return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd, modes ? modes : classes,
+                          what);
+}
+
+// true when the n entries of v are distinct and in [0, bound)
+bool distinct_in_range(const int32_t* v, int n, int bound) {
+  std::vector<int> sorted(v, v + n);
+  std::sort(sorted.begin(), sorted.end());
+  return sorted.front() >= 0 && sorted.back() < bound && std::adjacent_find(sorted.begin(), sorted.end()) == sorted.end();
+}
+
 int laplace_nll_classes(Ctx* c, Objective kind, int32_t n_classes, const int32_t* classes, int32_t n_eval,
                         const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t nh, double tol,
                         double* neg_log_z_out, double* grad_out) {
@@ -1260,29 +1310,10 @@ int laplace_nll_classes(Ctx* c, Objective kind, int32_t n_classes, const int32_t
     return fail(c, SGP_E_BADARG, "sgp_laplace_nll_classes: bad argument");
   if (n_classes < 1 || n_eval < 1 || n_eval > n_classes || n_eval > 65535)
     return fail(c, SGP_E_BADARG, "sgp_laplace_nll_classes: need 1 <= n_eval <= n_classes and n_eval <= 65535");
-  std::vector<int> sorted(classes, classes + n_eval);
-  std::sort(sorted.begin(), sorted.end());
-  if (sorted.front() < 0 || sorted.back() >= n_classes || std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+  if (!distinct_in_range(classes, n_eval, n_classes))
     return fail(c, SGP_E_BADARG, "sgp_laplace_nll_classes: class indices must be distinct and in [0, n_classes)");
-  if (tol >= 1.0) return fail(c, SGP_E_SINGULAR, kLaplaceNoIteration);
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  ObjectiveSetup o;
-  int rc = objective_setup(c, n_eval, kernels, hypers, nh, classes, o);
-  if (rc != SGP_OK) return rc;
-  if (plan_objective(kind, c->ex, o.hv.kf.n_terms).variant == ObjectiveVariant::kRefused)
-    return fail(c, SGP_E_BADARG, kLaplaceRefused);
-  if (c->ex_classes != n_classes) {                       // first use after an upload, or another class count
-    const size_t bytes = static_cast<size_t>(n_classes) * c->ex.n * 8;
-    rc = ctx_scratch(c, c->ex_fc, bytes);
-    if (rc != SGP_OK) return rc;
-    SGP_CUDA(c, cudaMemsetAsync(c->ex_fc.p, 0, bytes, c->stream));
-    c->ex_classes = n_classes;
-  }
-  LaplaceClasses lc;
-  lc.n_slots = n_eval; lc.cls = o.cls; lc.kf = o.kf; lc.slot_stride = o.slot_stride; lc.f = c->ex_fc.as<double>();
-  rc = laplace_run(c, kind, o, tol, &lc);
-  if (rc != SGP_OK) return rc;
-  return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd, classes);
+  return laplace_slots(c, kind, c->ex_fc, &c->ex_classes, n_classes, classes, nullptr, n_eval, kernels, hypers, nh, tol,
+                       neg_log_z_out, grad_out, "class");
 }
 }  // namespace
 
@@ -1316,6 +1347,38 @@ int sgp_laplace_nll_classes_any_size(sgp_ctx* h, int32_t n_classes, const int32_
   if (!c) return SGP_E_BADARG;
   return laplace_nll_classes(c, Objective::kLaplaceAnySize, n_classes, classes, n_eval, kernels, hypers, nh, tol,
                              neg_log_z_out, grad_out);
+}
+
+int sgp_laplace_nll_slots_any_size(sgp_ctx* h, int32_t n_mode_slots, const int32_t* mode_slots, const int32_t* classes,
+                                   int32_t n_eval, const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t nh,
+                                   double tol, double* neg_log_z_out, double* grad_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!neg_log_z_out || (nh > 0 && !grad_out) || !(tol > 0.0) || !mode_slots || !classes)
+    return fail(c, SGP_E_BADARG, "sgp_laplace_nll_slots_any_size: bad argument");
+  if (n_mode_slots < 1 || n_eval < 1 || n_eval > n_mode_slots || n_eval > 65535)
+    return fail(c, SGP_E_BADARG, "sgp_laplace_nll_slots_any_size: need 1 <= n_eval <= n_mode_slots and n_eval <= 65535");
+  if (!distinct_in_range(mode_slots, n_eval, n_mode_slots))
+    return fail(c, SGP_E_BADARG, "sgp_laplace_nll_slots_any_size: mode slots must be distinct and in [0, n_mode_slots)");
+  if (*std::min_element(classes, classes + n_eval) < 0)
+    return fail(c, SGP_E_BADARG, "sgp_laplace_nll_slots_any_size: class indices must be >= 0");
+  return laplace_slots(c, Objective::kLaplaceAnySize, c->ex_fm, &c->ex_mode_slots, n_mode_slots, classes, mode_slots,
+                       n_eval, kernels, hypers, nh, tol, neg_log_z_out, grad_out, "mode slot");
+}
+
+int sgp_experts_get_f_slot(sgp_ctx* h, int32_t mode_slot, double* f_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (c->ex.E == 0 || !f_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
+  if (c->ex_mode_slots == 0)
+    return fail(c, SGP_E_STATE, "no slot modes: sgp_laplace_nll_slots_any_size has not run since the upload");
+  if (mode_slot < 0 || mode_slot >= c->ex_mode_slots)
+    return fail(c, SGP_E_BADARG, "sgp_experts_get_f_slot: mode slot outside [0, n_mode_slots)");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  SGP_CUDA(c, cudaMemcpyAsync(f_out, c->ex_fm.as<double>() + static_cast<size_t>(mode_slot) * c->ex.n,
+                              static_cast<size_t>(c->ex.n) * 8, cudaMemcpyDeviceToHost, c->stream));
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  return SGP_OK;
 }
 
 int sgp_experts_get_f_class(sgp_ctx* h, int32_t cls, double* f_out) {

@@ -8,10 +8,11 @@
 // before that iteration's update, while d3logP (GPCls:118, sign as in the reference) uses exp(-f) of the final f.
 // Summed over experts like commons/GaussianProcessCommons.scala:73-78.
 //
-// One-vs-rest (sgp_laplace_nll_classes): a second grid dimension runs several binary problems over the same experts in
-// one launch.  Block (e, s) evaluates expert e for the s-th listed class c: labels (y == c), modes f + c * n, its own
-// flattened kernel and hyper-parameter block, output row [s][e].  The arithmetic is the single-class body's, so class
-// c's rows equal, bit for bit, those of a single-class launch on an upload of the labels (y == c).
+// One-vs-rest (sgp_laplace_nll_classes) and param-map slots (sgp_laplace_nll_slots_any_size): a second grid dimension
+// runs several binary problems over the same experts in one launch.  Block (e, s) evaluates expert e for the s-th listed
+// slot, of class c and mode slot m: labels (y == c), modes f + m * n, its own flattened kernel and hyper-parameter
+// block, output row [s][e].  The classes entry passes m = c.  The arithmetic is the single-class body's, so a slot's
+// rows equal, bit for bit, those of a single-class launch on an upload of the labels (y == c) with the same modes.
 #include "expert_common.cuh"
 
 namespace sgp {
@@ -24,6 +25,7 @@ struct LapParams {
   int n_max, x_in_smem;
   HyperView hv;              // slot 0's view; slot s reads kf[s] and the descriptor values s * slot_stride doubles on
   const int* cls;            // [n_slots] class of each slot (one-vs-rest), or nullptr: one slot, labels as uploaded
+  const int* mode;           // [n_slots] mode slot of each slot: its modes are f + mode[s] * n (with cls)
   const KernelFlat* kf;      // [n_slots] flattened kernel of each slot (with cls)
   long long slot_stride;     // doubles between two slots' [beta | coef | value] blocks (with cls)
   long long n;               // uploaded points: the stride of the per-class modes f (with cls)
@@ -68,9 +70,8 @@ __global__ void __launch_bounds__(LT, 1) laplace_kernel(const LapParams p) {
   double* fg = p.f;
   double cls = -1.0;                                     // < 0: labels as uploaded
   if (p.cls) {
-    const int c = p.cls[slot];
-    cls = c;
-    fg += static_cast<size_t>(c) * p.n;
+    cls = p.cls[slot];
+    fg += static_cast<size_t>(p.mode[slot]) * p.n;
     hv.kf = p.kf[slot];
     hv.beta += slot * p.slot_stride; hv.h_coef += slot * p.slot_stride; hv.h_value += slot * p.slot_stride;
   }
@@ -204,7 +205,7 @@ cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const
   p.hv = hv; p.n = ex.n; p.tol = tol; p.out = rows; p.flags = flags;
   int n_slots = 1;
   if (classes) {
-    p.f = classes->f; p.cls = classes->cls; p.kf = classes->kf; p.slot_stride = classes->slot_stride;
+    p.f = classes->f; p.cls = classes->cls; p.mode = classes->mode; p.kf = classes->kf; p.slot_stride = classes->slot_stride;
     n_slots = classes->n_slots;
   }
   cudaError_t e = cudaFuncSetAttribute(laplace_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(plan.smem));

@@ -40,9 +40,10 @@ struct LapGlobalParams {
   int ldw;                   // workspace row stride: n_max rounded up to NB
   HyperView hv;              // slot 0's view (as laplace_kernel's)
   const int* cls;            // [n_slots] or nullptr
+  const int* mode;           // [n_slots] mode slot of each slot (with cls)
   const KernelFlat* kf;      // [n_slots] (with cls)
   long long slot_stride;     // (with cls)
-  long long n;               // uploaded points: stride of the per-class modes (with cls)
+  long long n;               // uploaded points: stride of the per-slot modes (with cls)
   double tol;
   double* ws;                // [gridDim.x][lg_cta_doubles(ldw)]
   double* out;               // [n_slots][E][1 + n_hypers]
@@ -400,9 +401,8 @@ __global__ void __launch_bounds__(GT, 1) laplace_global_kernel(const LapGlobalPa
     double* fg = p.f;
     double cls = -1.0;                                   // < 0: labels as uploaded
     if (p.cls) {
-      const int c = p.cls[slot];
-      cls = c;
-      fg += static_cast<size_t>(c) * p.n;
+      cls = p.cls[slot];
+      fg += static_cast<size_t>(p.mode[slot]) * p.n;
       hv.kf = p.kf[slot];
       hv.beta += slot * p.slot_stride; hv.h_coef += slot * p.slot_stride; hv.h_value += slot * p.slot_stride;
     }
@@ -529,7 +529,7 @@ cudaError_t launch_laplace_global(const ExpertSet& ex, const HyperView& hv, doub
   p.X = ex.X; p.y = ex.y; p.f = ex.f; p.off = ex.off; p.E = ex.E; p.n_slots = 1; p.ldw = lg_ld(ex.n_max);
   p.hv = hv; p.n = ex.n; p.tol = tol; p.ws = ws; p.out = rows; p.flags = flags;
   if (classes) {
-    p.f = classes->f; p.cls = classes->cls; p.kf = classes->kf; p.slot_stride = classes->slot_stride;
+    p.f = classes->f; p.cls = classes->cls; p.mode = classes->mode; p.kf = classes->kf; p.slot_stride = classes->slot_stride;
     p.n_slots = classes->n_slots;
   }
   laplace_global_kernel<<<static_cast<unsigned>(grid), GT, 0, s>>>(p);

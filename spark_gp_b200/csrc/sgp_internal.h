@@ -172,6 +172,8 @@ struct Ctx {
   DevScratch ex_X, ex_y, ex_off, ex_f;
   DevScratch ex_fc;              // one-vs-rest latent modes [ex_classes][n] (sgp_laplace_nll_classes)
   int ex_classes = 0;            // classes ex_fc holds modes for; 0: none since the last upload
+  DevScratch ex_fm;              // param-map latent modes [ex_mode_slots][n] (sgp_laplace_nll_slots_any_size)
+  int ex_mode_slots = 0;         // mode slots ex_fm holds modes for; 0: none since the last upload
   // fold upload (sgp_experts_upload_folds): the training sets lie one after another in ex; set k owns the experts
   // fold_first[k] .. fold_first[k+1]-1.  Empty after any other upload.
   std::vector<long long> fold_first;   // [n_sets + 1]
@@ -357,15 +359,17 @@ cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const
 cudaError_t launch_bcm_nll_general(const ObjectivePlan& plan, cublasHandle_t blas, int* blas_status, void* ws,
                                    const ExpertSet& ex, const HyperView& hv, double* rows, double* total, int* flags,
                                    cudaStream_t s);
-// One-vs-rest slots of a Laplace launch (sgp_laplace_nll_classes): slot s evaluates class cls[s] with the labels
-// (y == cls[s]), the modes f + cls[s] * n, the flattened kernel kf[s] and the descriptor values slot_stride doubles per
-// slot after hv's.  rows: [n_slots][E][1 + n_hypers], total: [n_slots][1 + n_hypers], flags: [n_slots].
+// Slots of a Laplace launch (sgp_laplace_nll_classes*, sgp_laplace_nll_slots_any_size): slot s evaluates class cls[s]
+// with the labels (y == cls[s]), the modes f + mode[s] * n, the flattened kernel kf[s] and the descriptor values
+// slot_stride doubles per slot after hv's.  The classes entries pass mode = cls.  rows: [n_slots][E][1 + n_hypers],
+// total: [n_slots][1 + n_hypers], flags: [n_slots].
 struct LaplaceClasses {
   int n_slots = 0;
   const int* cls = nullptr;           // device, [n_slots]
+  const int* mode = nullptr;          // device, [n_slots], distinct
   const KernelFlat* kf = nullptr;     // device, [n_slots]
   long long slot_stride = 0;
-  double* f = nullptr;                // device, [n_classes][n]
+  double* f = nullptr;                // device, [n_mode_slots][n]
 };
 // classes == nullptr: one slot on the labels and modes as uploaded (sgp_laplace_nll)
 cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol, double* rows,

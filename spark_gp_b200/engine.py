@@ -329,6 +329,30 @@ class ProjectedProcessEngine:
         del keep
         return vals, np.ascontiguousarray(grads[:, :nh])
 
+    def laplace_nll_slots_any_size(self, n_mode_slots: int, mode_slots, classes, kernels, tol: float):
+        """Param-map slots (`sgp_laplace_nll_slots_any_size`): listed slot i evaluates the binary Laplace objective of the
+        labels (y == classes[i]) at kernels[i], warm-started from and writing the modes of mode slot mode_slots[i], all in
+        one launch.  Classes may repeat; mode slots are distinct in [0, n_mode_slots).  Returns (values [n_eval],
+        gradients [n_eval x n_hypers])."""
+        modes = np.ascontiguousarray(mode_slots, dtype=np.int32)
+        cls = np.ascontiguousarray(classes, dtype=np.int32)
+        if modes.ndim != 1 or len(modes) == 0 or cls.shape != modes.shape or len(modes) != len(kernels):
+            raise ValueError("laplace_nll_slots_any_size: one class and one kernel per listed mode slot")
+        descs, hyp, nh, keep = self._slot_descriptors(kernels)
+        vals = np.zeros(len(modes))
+        grads = np.zeros((len(modes), max(nh, 1)))
+        self._check(self._lib.sgp_laplace_nll_slots_any_size(self._h, int(n_mode_slots), N.ptr(modes), N.ptr(cls),
+                                                             len(modes), descs, hyp, nh, float(tol), N.ptr(vals),
+                                                             N.ptr(grads)))
+        del keep
+        return vals, np.ascontiguousarray(grads[:, :nh])
+
+    def experts_f_slot(self, slot: int, n: int):
+        """Mode slot `slot`'s latent modes after `laplace_nll_slots_any_size` (packed expert-major order)."""
+        f = np.empty(n)
+        self._check(self._lib.sgp_experts_get_f_slot(self._h, int(slot), N.ptr(f)))
+        return f
+
     def experts_f_class(self, cls: int, n: int):
         """Class cls's latent modes after `laplace_nll_classes` (packed expert-major order)."""
         f = np.empty(n)

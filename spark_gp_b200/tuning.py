@@ -1,6 +1,7 @@
-"""Model selection for the regression estimator: Spark 3.1's `ParamGridBuilder`, `RegressionEvaluator` and
-`CrossValidator`, as the reference's own examples use them (regression/examples/GPExample.scala:17-27, Airfoil.scala:18-24,
-Synthetics.scala:25-33: 10-fold cross-validation of the RMSE).
+"""Model selection: Spark 3.1's `ParamGridBuilder`, `RegressionEvaluator`, `MulticlassClassificationEvaluator`,
+`CrossValidator` (regression estimator) and `TrainValidationSplit` (any estimator), as the reference's own examples use
+them (regression/examples/GPExample.scala:17-27, Airfoil.scala:18-24, Synthetics.scala:25-33: 10-fold cross-validation of
+the RMSE; classification/examples/MNIST.scala:34-40, Iris.scala:29-35: a train/validation split scored by accuracy).
 
 Spark's ml/tuning and ml/evaluation are not part of the reference project; they are restated here from Spark 3.1's
 documented behaviour:
@@ -21,16 +22,29 @@ All (map, fold) slots that share datasetSizeForExpert, the kernel's structure an
 maxIter and tol are optimised together: the training sets of every fold are uploaded once
 (`sgp_experts_upload_folds`), and each round of their L-BFGS-B runs is one `sgp_bcm_nll_folds` launch over experts x
 slots.  Each slot's objective values equal the independent fit's bit for bit, so every fold model, prediction and metric
-is the one `estimator.copy(map).fit(X[train], y[train])` gives."""
+is the one `estimator.copy(map).fit(X[train], y[train])` gives.
+
+TrainValidationSplit (Spark 3.1): fit every param map on the training rows (in row order), evaluate each fitted model on
+the validation rows (validationMetrics, in map order), take the first best map and refit it on all rows.  trainRatio
+defaults to 0.75 and lies strictly in (0, 1); there is no default evaluator.  Deviation: Spark's randomSplit depends on the
+partitioning; here row i trains iff u(seed, 201, i) < trainRatio (the K-means generator, stream 201), and
+`fit(X, y, train=mask)` takes a given split.  An empty training or validation side raises ValueError.
+Over the binary classifier and one-vs-rest, the maps are grouped by `slot_group_key` of the classifier; a group's
+training rows are uploaded once, and every (map p, class c) is one slot with mode slot p * C + c (binary: C = 1, class 1)
+in `sgp_laplace_nll_slots_any_size`, so each round of the slots' L-BFGS-B runs is one launch.  Each slot's values and
+modes equal the independent fit's bit for bit, so every validation prediction is that of
+`estimator.copy(map).fit(X[train], y[train])`.  Regression maps are fitted one after another."""
 from __future__ import annotations
 
 import numpy as np
 
 from . import _native as N
+from .classification import GaussianProcessClassifier, OneVsRest, _produce_model, one_vs_rest_labels, \
+    one_vs_rest_prediction
 from .engine import ProjectedProcessEngine
-from .hyperopt import lbfgsb_bounds, lbfgsb_lockstep
+from .hyperopt import group_for_experts, lbfgsb_bounds, lbfgsb_lockstep
 from .regression import GaussianProcessRegression
-from .utils import kfold_assignment
+from .utils import kfold_assignment, train_validation_assignment
 
 
 class ParamGridBuilder:
@@ -94,6 +108,59 @@ class RegressionEvaluator:
         if len(y) == 0 or np.shape(prediction) != y.shape:
             raise ValueError("evaluate: labels and predictions must be non-empty vectors of one length")
         return regression_metric(self._metric, y, prediction)
+
+
+def multiclass_metric(name: str, y, p) -> float:
+    """Spark 3.1's MulticlassMetrics for one metric name, unweighted: per true label l (sorted), n_l rows, tp_l hits and
+    fp_l false predictions of l; precision_l = tp_l / (tp_l + fp_l) (0 if never predicted), recall_l = tp_l / n_l,
+    f1_l = 2 p r / (p + r) (0 if p + r = 0); the weighted metrics sum v_l * n_l / n over the labels in order."""
+    y = np.asarray(y, dtype=np.float64)
+    p = np.asarray(p, dtype=np.float64)
+    n = len(y)
+    if name == "accuracy":
+        return float(np.count_nonzero(y == p)) / n
+    if name not in MulticlassClassificationEvaluator.METRICS:
+        raise ValueError("metricName must be one of %s, not %r" % (", ".join(MulticlassClassificationEvaluator.METRICS),
+                                                                  name))
+    total = 0.0
+    for label in np.unique(y):
+        truth, hit = y == label, p == label
+        nl = int(np.count_nonzero(truth))
+        tp = int(np.count_nonzero(hit & truth))
+        fp = int(np.count_nonzero(hit)) - tp
+        precision = tp / (tp + fp) if tp + fp > 0 else 0.0
+        recall = tp / nl
+        value = {"weightedPrecision": precision, "weightedRecall": recall,
+                 "f1": 2.0 * precision * recall / (precision + recall) if precision + recall > 0.0 else 0.0}[name]
+        total += value * nl / n
+    return total
+
+
+class MulticlassClassificationEvaluator:
+    """Spark's MulticlassClassificationEvaluator over (label, prediction): f1 (default), accuracy, weightedPrecision,
+    weightedRecall, all larger-is-better."""
+    METRICS = ("f1", "accuracy", "weightedPrecision", "weightedRecall")
+
+    def __init__(self, metricName: str = "f1"):
+        self.setMetricName(metricName)
+
+    def setMetricName(self, value: str):
+        if value not in self.METRICS:
+            raise ValueError("metricName must be one of %s, not %r" % (", ".join(self.METRICS), value))
+        self._metric = value
+        return self
+
+    def getMetricName(self) -> str:
+        return self._metric
+
+    def isLargerBetter(self) -> bool:
+        return True
+
+    def evaluate(self, y, prediction) -> float:
+        y = np.asarray(y, dtype=np.float64)
+        if len(y) == 0 or np.shape(prediction) != y.shape:
+            raise ValueError("evaluate: labels and predictions must be non-empty vectors of one length")
+        return multiclass_metric(self._metric, y, prediction)
 
 
 def best_index(metrics, larger_is_better: bool) -> int:
@@ -250,3 +317,184 @@ class CrossValidator:
             for (p, k), (res, _) in zip(slots, results):
                 thetas[p][k] = np.asarray(res.x, dtype=np.float64)
         return thetas, dict(groups=groups)
+
+
+def tvs_slot_groups(classifiers, n_classes: int):
+    """{slot_group_key: [(map index p, class index c, mode slot p * n_classes + c), ...]} over every (map, class) slot of
+    a train/validation split over classifiers (one per map), in map-major order."""
+    groups = {}
+    for p, gp in enumerate(classifiers):
+        groups.setdefault(slot_group_key(gp), []).extend((p, c, p * n_classes + c) for c in range(n_classes))
+    return groups
+
+
+class TrainValidationSplitModel:
+    """Spark's TrainValidationSplitModel: the best map refitted on every row, and each map's validation metric."""
+
+    def __init__(self, bestModel, validationMetrics, bestIndex, last_objective):
+        self.bestModel = bestModel
+        self.validationMetrics = list(validationMetrics)
+        self.bestIndex = bestIndex
+        self.last_objective = last_objective
+
+    def predict(self, features):
+        return self.bestModel.predict(features)
+
+    transform = predict
+
+
+class TrainValidationSplit:
+    ESTIMATORS = (GaussianProcessRegression, GaussianProcessClassifier, OneVsRest)
+    EVALUATORS = (RegressionEvaluator, MulticlassClassificationEvaluator)
+
+    def __init__(self):
+        self._estimator = None
+        self._evaluator = None
+        self._maps = None
+        self._train_ratio = 0.75
+        self._seed = 0
+        self.last_predictions = None      # each map's validation predictions, in map order
+
+    def setEstimator(self, value):
+        if not isinstance(value, self.ESTIMATORS):
+            raise TypeError("TrainValidationSplit: the estimator must be a GaussianProcessRegression, a "
+                            "GaussianProcessClassifier or a OneVsRest, not %s" % type(value).__name__)
+        self._estimator = value
+        return self
+
+    def setEvaluator(self, value):
+        if not isinstance(value, self.EVALUATORS):
+            raise TypeError("TrainValidationSplit: the evaluator must be a RegressionEvaluator or a "
+                            "MulticlassClassificationEvaluator, not %s" % type(value).__name__)
+        self._evaluator = value
+        return self
+
+    def setEstimatorParamMaps(self, value):
+        maps = [dict(m) for m in value]
+        if not maps:
+            raise ValueError("TrainValidationSplit: at least one param map")
+        self._maps = maps
+        return self
+
+    def setTrainRatio(self, value: float):
+        if not 0.0 < float(value) < 1.0:
+            raise ValueError("TrainValidationSplit: trainRatio must lie in (0, 1)")
+        self._train_ratio = float(value)
+        return self
+
+    def setSeed(self, value: int):
+        self._seed = int(value)
+        return self
+
+    def getTrainRatio(self) -> float:
+        return self._train_ratio
+
+    def fit(self, X, y, train=None) -> TrainValidationSplitModel:
+        """train: a bool mask of the training rows; default: the seeded split of the module docstring."""
+        est = self._estimator
+        if est is None:
+            raise TypeError("TrainValidationSplit: setEstimator first")
+        if self._evaluator is None:
+            raise ValueError("TrainValidationSplit: setEvaluator first (there is no default evaluator)")
+        X = np.asarray(X)
+        y = np.asarray(y, dtype=np.float64)
+        if X.ndim != 2 or len(y) != len(X):
+            raise ValueError("TrainValidationSplit: X must be n x d and y n labels")
+        if train is None:
+            mask = train_validation_assignment(len(X), self._train_ratio, self._seed)
+        else:
+            mask = np.asarray(train)
+            if mask.shape != (len(X),) or not np.all((mask == 0) | (mask == 1)):
+                raise ValueError("TrainValidationSplit: train must hold one bool per row")
+            mask = mask.astype(bool)
+        if not mask.any() or mask.all():
+            raise ValueError("TrainValidationSplit: the %s side of the split is empty"
+                             % ("training" if not mask.any() else "validation"))
+        maps = self._maps or [{}]
+        ests = [est.copy(m) for m in maps]
+        if isinstance(est, GaussianProcessRegression):
+            preds, objective = self._fit_regression(ests, X, y, mask)
+        else:
+            preds, objective = self._fit_classifiers(ests, isinstance(est, OneVsRest), X, y, mask)
+        metrics = [self._evaluator.evaluate(y[~mask], p) for p in preds]
+        best = best_index(metrics, self._evaluator.isLargerBetter())
+        self.last_predictions = preds
+        return TrainValidationSplitModel(est.copy(maps[best]).fit(X, y), metrics, best, objective)
+
+    @staticmethod
+    def _fit_regression(ests, X, y, train):
+        """Each map fitted on its own: a batched BCM launch over maps on one upload does not exist (a fold upload would
+        refuse validation sides the independent fit takes)."""
+        preds, maps = [], []
+        for e in ests:
+            model = e.fit(X[train], y[train])
+            preds.append(model.predict(X[~train]))
+            maps.append(e.last_objective)
+            del model
+        return preds, dict(maps=maps)
+
+    @staticmethod
+    def _fit_classifiers(ests, ovr: bool, X, y, train):
+        """Validation predictions of every map of the binary classifier (ovr False) or of one-vs-rest, and what the
+        optimisation took: per group of maps one upload, one lock-step L-BFGS-B over the (map, class) slots, one
+        `sgp_laplace_nll_slots_any_size` call per round and one at every slot's optimum (GPCls:60)."""
+        gps = [e.getClassifier() for e in ests] if ovr else ests
+        if any(not isinstance(gp, GaussianProcessClassifier) for gp in gps):
+            raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
+        X = np.asarray(X, dtype=np.float64)
+        if ovr:
+            one_vs_rest_labels(y)
+            C = one_vs_rest_labels(y[train])[1]           # as an independent OneVsRest.fit(X[train], y[train])
+            label = lambda c: c
+        else:
+            if not np.all((y == 0.0) | (y == 1.0)):         # assertLabelsAre01, GPCls:68-72
+                raise RuntimeError("Only 0 and 1 labels are supported.")
+            C = 1
+            label = lambda c: 1                             # y == 1 is y itself
+        Xt, yt, Xv = X[train], y[train], X[~train]
+        raw = [np.empty((len(Xv), C)) for _ in gps]
+        groups = []
+        for slots in tvs_slot_groups(gps, C).values():
+            g0 = gps[slots[0][0]]
+            kernel_at = lambda p, t: gps[p].getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
+            x0s = [gps[p].getKernel().getHyperparameters() for p, _, _ in slots]
+            eng = ProjectedProcessEngine.acquire(g0._device)
+            try:
+                order = np.concatenate(group_for_experts(len(Xt), g0._datasetSizeForExpert))
+                eng.experts_upload_grouped(Xt, yt, g0._datasetSizeForExpert)
+                launches0 = eng.launch_count()
+                calls = [0]
+
+                def evaluate(batch):
+                    calls[0] += 1
+                    vals, grads = eng.laplace_nll_slots_any_size(
+                        len(gps) * C, [slots[i][2] for i, _ in batch], [label(slots[i][1]) for i, _ in batch],
+                        [kernel_at(slots[i][0], t) for i, t in batch], g0._tol)
+                    return [(float(v), g) for v, g in zip(vals, grads)]
+
+                thetas = [np.asarray(x0, dtype=np.float64) for x0 in x0s]
+                results, rounds = [], 0
+                if g0._maxIter > 0 and len(x0s[0]) > 0:
+                    results, rounds = lbfgsb_lockstep(evaluate, x0s, lbfgsb_bounds(g0.getKernel()), g0._maxIter, g0._tol)
+                    thetas = [np.asarray(res.x, dtype=np.float64) for res, _ in results]
+                evaluate(list(enumerate(thetas)))           # GPCls:60: every slot's f is its mode at theta*
+                groups.append(dict(
+                    slots=[dict(map=p, cls=c, mode_slot=m, theta=theta, value=float(res.fun), evaluations=ev,
+                                iterations=int(res.nit))
+                           for (p, c, m), (res, ev), theta in zip(slots, results, thetas)],
+                    rounds=rounds, calls=calls[0], launches=eng.launch_count() - launches0))
+                f = np.empty(len(Xt))
+                for (p, c, m), theta in zip(slots, thetas):
+                    f[order] = eng.experts_f_slot(m, len(Xt))
+                    # each slot's model starts from the default precision, as the independent fit's fresh context does
+                    eng.set_precision(N.SGP_PREC_AUTO)
+                    _produce_model(gps[p], eng, Xt, f, theta)
+                    raw[p][:, c], _ = eng.predict(Xv, with_variance=False)
+            finally:
+                eng.set_precision(N.SGP_PREC_AUTO)
+                eng.release()
+        if ovr:
+            preds = [one_vs_rest_prediction(r) for r in raw]
+        else:                                               # GaussianProcessClassificationModel.predict
+            preds = [np.argmax(np.stack([-r[:, 0], r[:, 0]], axis=-1), axis=-1).astype(np.float64) for r in raw]
+        return preds, dict(groups=groups)

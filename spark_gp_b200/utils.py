@@ -44,3 +44,8 @@ def uniform(seed: int, stream: int, i) -> np.ndarray:
 def kfold_assignment(n: int, num_folds: int, seed: int) -> np.ndarray:
     """CrossValidator's default split: point i goes to fold floor(u(seed, 200, i) * numFolds) (int32)."""
     return np.floor(uniform(seed, 200, np.arange(int(n))) * int(num_folds)).astype(np.int32)
+
+
+def train_validation_assignment(n: int, train_ratio: float, seed: int) -> np.ndarray:
+    """TrainValidationSplit's default split: row i trains iff u(seed, 201, i) < trainRatio (bool mask)."""
+    return uniform(seed, 201, np.arange(int(n))) < float(train_ratio)

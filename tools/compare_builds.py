@@ -9,7 +9,8 @@ Covered, each on both builds:
   - the magic vector and matrix on the Cholesky tail path and on the eigenvalue + LU path;
   - sgp_predict (mean and variance) and sgp_predict_device (fp32 and fp64 rows); sgp_cross_kernel; sgp_kmn_sweep;
   - sgp_bcm_nll value and gradient on the register, shared-memory and LU variants; sgp_laplace_nll value, gradient and
-    the latent modes f; sgp_greedy_active_set indices.
+    the latent modes f; sgp_laplace_nll_any_size on the global-memory kernel and sgp_laplace_nll_classes_any_size on
+    both kernels (values, gradients and every class's modes over two warm-started calls); sgp_greedy_active_set indices.
 Outputs are compared as bit patterns.  The script prints one line per case and exits with 1 if any case differs.
 --time times the fp64 statistics kernel (both loops) and prediction on both builds, alternated in the same process:
 median of 5 synchronised calls after a warm-up, with the card's name and power limit.  --out writes the report there."""
@@ -33,14 +34,36 @@ from spark_gp_b200.engine import ProjectedProcessEngine   # noqa: E402
 from spark_gp_b200.hyperopt import pack_experts     # noqa: E402
 
 
+class _Absent:
+    """An entry this tree declares and the other build does not export (a later addition to the C-ABI)."""
+
+    def __init__(self, name):
+        self.name = name
+
+    def __call__(self, *args):
+        raise RuntimeError("%s is not in the other build" % self.name)
+
+
+class _OlderLib(C.CDLL):
+    def __getattr__(self, name):
+        try:
+            return super().__getattr__(name)
+        except AttributeError:
+            if name.startswith("__"):
+                raise
+            stub = _Absent(name)
+            setattr(self, name, stub)
+            return stub
+
+
 def load_lib(path):
-    """Another libsgp.so with the ctypes bindings of _native (the C-ABI is the same)."""
-    saved = N.LIB_PATH, N._lib
-    N.LIB_PATH, N._lib = os.path.abspath(path), None
+    """Another libsgp.so with the ctypes bindings of _native (the C-ABI is the same, less the entries added since)."""
+    saved = N.LIB_PATH, N._lib, N.C.CDLL
+    N.LIB_PATH, N._lib, N.C.CDLL = os.path.abspath(path), None, _OlderLib
     try:
         return N.load()
     finally:
-        N.LIB_PATH, N._lib = saved
+        N.LIB_PATH, N._lib, N.C.CDLL = saved
 
 
 def engine_on(lib):
@@ -123,6 +146,42 @@ def laplace_case(e, n_terms, seed):
     return dict(value=np.array([v]), grad=g, f=e.experts_f(len(X)))
 
 
+def laplace_global_case(e, n_terms, seed):
+    """Experts of 150 points: sgp_laplace_nll_any_size on the global-memory kernel, two warm-started evaluations."""
+    rng = np.random.default_rng(seed)
+    X = rng.standard_normal((600, 3))
+    y = (np.sin(2 * X[:, 0]) + 0.3 * rng.standard_normal(len(X)) > 0).astype(np.float64)
+    e.experts_upload(*pack_experts(X, y, 150))
+    k = kernel(n_terms, 3, rng)
+    out = {}
+    for step in range(2):
+        v, g = e.laplace_nll_any_size(k.setHyperparameters(k.getHyperparameters() * (1.0 + 0.1 * step)), 1e-6)
+        out.update({"value%d" % step: np.array([v]), "grad%d" % step: g, "f%d" % step: e.experts_f(len(X))})
+    out["path"] = np.array([e.last_laplace_path()])
+    return out
+
+
+def laplace_classes_case(e, n_terms, n_e, seed):
+    """sgp_laplace_nll_classes_any_size over 3 classes: every class, then a permuted subset warm-started."""
+    rng = np.random.default_rng(seed)
+    X = rng.standard_normal((4 * n_e, 3))
+    s = np.sin(2 * X[:, 0]) + X[:, 2] + 0.3 * rng.standard_normal(len(X))
+    y = np.digitize(s, np.quantile(s, [1 / 3, 2 / 3])).astype(np.float64)
+    e.experts_upload(*pack_experts(X, y, n_e))
+    k = kernel(n_terms, 3, rng)
+    t0 = k.getHyperparameters()
+    out = {}
+    for step, classes in enumerate(([0, 1, 2], [2, 0])):
+        ks = [kernel(n_terms, 3, np.random.default_rng(seed)).setHyperparameters(t0 * (1.0 + 0.07 * c + 0.1 * step))
+              for c in classes]
+        v, g = e.laplace_nll_classes_any_size(3, classes, ks, 1e-6)
+        out.update({"value%d" % step: v, "grad%d" % step: g})
+        for c in range(3):
+            out["f%d_class%d" % (step, c)] = e.experts_f_class(c, len(X))
+    out["path"] = np.array([e.last_laplace_path()])
+    return out
+
+
 def greedy_case(e, n_terms, seed):
     rng = np.random.default_rng(seed)
     X = rng.random((4000, 5))
@@ -143,6 +202,11 @@ def cases():
     for t in (1, 2, 4):
         out.append(("laplace_nll %d terms" % t, lambda e, t=t: laplace_case(e, t, 20 + t)))
         out.append(("greedy_active_set %d terms" % t, lambda e, t=t: greedy_case(e, t, 30 + t)))
+    for t in (1, 2):
+        out.append(("laplace_nll_any_size global, %d terms" % t, lambda e, t=t: laplace_global_case(e, t, 40 + t)))
+        for n_e, label in ((100, "on chip"), (150, "global")):
+            out.append(("laplace_nll_classes_any_size %s, %d terms" % (label, t),
+                        lambda e, t=t, n_e=n_e: laplace_classes_case(e, t, n_e, 50 + t)))
     return out
 
 
