@@ -6,7 +6,7 @@ import numpy as np
 
 from . import _native as N
 from .engine import ProjectedProcessEngine, is_cuda_tensor
-from .hyperopt import group_for_experts, lbfgsb, lbfgsb_bounds, lbfgsb_lockstep
+from .hyperopt import group_for_experts, lbfgsb_bounds, optimise_slots
 from .regression import GaussianProcessParams, GaussianProjectedProcessRawPredictor
 
 
@@ -62,37 +62,52 @@ class GaussianProcessClassifier(GaussianProcessParams):
         if not np.all((y == 0.0) | (y == 1.0)):                     # assertLabelsAre01, GPCls:68-72
             raise RuntimeError("Only 0 and 1 labels are supported.")
         eng = ProjectedProcessEngine.acquire(self._device)
-        groups = group_for_experts(len(X), self._datasetSizeForExpert)
-        order = np.concatenate(groups)
-        eng.experts_upload_grouped(X, y, self._datasetSizeForExpert)  # grouping on the device; f = zeros per expert (GPCls:53-55)
-        launches0 = eng.launch_count()
-
-        if hyperparameters is None:
-            k0 = self.getKernel()
-            theta = k0.getHyperparameters()
-            if self._maxIter > 0 and len(theta) > 0:                # memoised like DiffFunctionMemoized; f warm-starts
-                res, evaluations = lbfgsb(
-                    lambda t: eng.laplace_nll_any_size(self.getKernel().setHyperparameters(t), self._tol),
-                    theta, lbfgsb_bounds(k0), self._maxIter, self._tol)
-                theta = np.asarray(res.x, dtype=np.float64)
-                self.last_objective = dict(value=float(res.fun), evaluations=evaluations, iterations=int(res.nit),
-                                           launches=eng.launch_count() - launches0)
-        else:
-            theta = np.asarray(hyperparameters, dtype=np.float64)
-        # GPCls:60: run the Laplace loop once more at the optimum so every expert's f is the mode at theta*
-        eng.laplace_nll_any_size(self.getKernel().setHyperparameters(theta), self._tol)
-        f_packed = eng.experts_f(len(X))
-        f = np.empty(len(X))
-        f[order] = f_packed
+        objective = lambda batch: [eng.laplace_nll_any_size(self.getKernel().setHyperparameters(t), self._tol)
+                                   for _, t in batch]
+        (theta,), (f,), fit = laplace_fit(
+            self, eng, X, y, objective, lambda _: eng.experts_f(len(X)), [self.getKernel().getHyperparameters()],
+            None if hyperparameters is None else [np.asarray(hyperparameters, dtype=np.float64)])
+        if fit["slots"] is not None:
+            self.last_objective = dict(fit["slots"][0], launches=fit["launches"])
         self.last_latent = f
         # GPCls:62-65 -> produceModel with (f, kernel): the same projected-process path as regression
         kernel, active_set, mv, mm, self.last_stats = _produce_model(self, eng, X, f, theta)
         return GaussianProcessClassificationModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, active_set), theta)
 
 
+def laplace_fit(gp, eng, X, y, objective, modes, x0s, thetas=None):
+    """The Laplace part of the binary fit (GPCls:53-60) for every slot of the caller, on one upload of (X, y) into eng,
+    grouped into experts by gp's datasetSizeForExpert (every slot's modes start at 0).
+      objective([(i, theta_i), ...]) -> [(value, gradient), ...]: slot i's Laplace objective at theta_i, warm-started from
+                                        and moving its device-resident modes;
+      modes(i):                         slot i's modes, packed expert-major.
+    Unless `thetas` are given, every slot is optimised from x0s (`optimise_slots`; skipped when there are no
+    hyper-parameters).  Then the Laplace loop runs once more at every slot's theta (GPCls:60), so that its modes are the
+    modes at theta.  Returns (thetas, modes [slot][row] in row order, dict(slots: each slot's optimisation record or None
+    when nothing was optimised, rounds, launches: the optimisation's, launches_total: with the call at theta))."""
+    order = np.concatenate(group_for_experts(len(X), gp._datasetSizeForExpert))
+    eng.experts_upload_grouped(X, y, gp._datasetSizeForExpert)
+    launches0 = eng.launch_count()
+    records, rounds = None, 0
+    if thetas is None:
+        thetas = [np.asarray(x0, dtype=np.float64) for x0 in x0s]
+        if len(thetas[0]) > 0:
+            thetas, records, rounds = optimise_slots(objective, x0s, lbfgsb_bounds(gp.getKernel()), gp._maxIter, gp._tol)
+    launches = eng.launch_count() - launches0
+    objective(list(enumerate(thetas)))
+    fit = dict(slots=records, rounds=rounds, launches=launches, launches_total=eng.launch_count() - launches0)
+    latent = np.empty((len(thetas), len(X)))
+    for i in range(len(thetas)):
+        latent[i, order] = modes(i)
+    return thetas, latent, fit
+
+
 def _produce_model(gp, eng, X, f, theta):
     """GPCls:62-65: the active set, the statistics with y := f and the tail, on eng.  Returns (kernel, active set, magic
     vector, magic matrix, (G, b))."""
+    # every model starts from the default precision, as on a freshly acquired context: a fallback to F64 in one slot's
+    # statistics must not decide the next slot's path
+    eng.set_precision(N.SGP_PREC_AUTO)
     active_set = gp._activeSetProvider(gp._activeSetSize, X, f, gp.getKernel, theta, gp._seed, gp=gp)
     kernel = gp.getKernel().setHyperparameters(theta)
     G, b = eng.statistics(kernel, active_set, X, f)                 # same helper as regression (fp64-kernel fallback)
@@ -206,37 +221,23 @@ class OneVsRest:
             eng.release()
 
     def _fit(self, gp, eng, X, y, C, hyperparameters):
-        groups = group_for_experts(len(X), gp._datasetSizeForExpert)
-        order = np.concatenate(groups)
-        eng.experts_upload_grouped(X, y, gp._datasetSizeForExpert)  # once for every class; all modes start at 0
-        launches0 = eng.launch_count()
-        k0 = gp.getKernel()
-        x0 = k0.getHyperparameters()
         kernel_at = lambda t: gp.getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
-        if hyperparameters is not None:
-            thetas = np.array(hyperparameters, dtype=np.float64).reshape(C, len(x0))
-        else:
-            thetas = np.tile(np.asarray(x0, dtype=np.float64), (C, 1))
-            if gp._maxIter > 0 and len(x0) > 0:
-                def evaluate(batch):
-                    vals, grads = eng.laplace_nll_classes_any_size(C, [c for c, _ in batch],
-                                                                   [kernel_at(t) for _, t in batch], gp._tol)
-                    return [(float(v), g) for v, g in zip(vals, grads)]
 
-                results, rounds = lbfgsb_lockstep(evaluate, [x0] * C, lbfgsb_bounds(k0), gp._maxIter, gp._tol)
-                thetas = np.array([np.asarray(res.x, dtype=np.float64) for res, _ in results]).reshape(C, len(x0))
-                self.last_objective = dict(
-                    classes=[dict(value=float(res.fun), evaluations=ev, iterations=int(res.nit)) for res, ev in results],
-                    rounds=rounds, launches=eng.launch_count() - launches0)
-        # GPCls:60 for every class at once: each class's f is its mode at theta*_c
-        eng.laplace_nll_classes_any_size(C, np.arange(C), [kernel_at(t) for t in thetas], gp._tol)
-        latent = np.empty((C, len(X)))
+        def objective(batch):
+            vals, grads = eng.laplace_nll_classes_any_size(C, [c for c, _ in batch], [kernel_at(t) for _, t in batch],
+                                                           gp._tol)
+            return [(float(v), g) for v, g in zip(vals, grads)]
+
+        x0 = gp.getKernel().getHyperparameters()
+        given = None if hyperparameters is None else np.array(hyperparameters, dtype=np.float64).reshape(C, len(x0))
+        thetas, latent, fit = laplace_fit(gp, eng, X, y, objective, lambda c: eng.experts_f_class(c, len(X)), [x0] * C,
+                                          given)
+        thetas = np.array(thetas).reshape(C, len(x0))
+        if fit["slots"] is not None:
+            self.last_objective = dict(classes=fit["slots"], rounds=fit["rounds"], launches=fit["launches"])
         models = []
         for c in range(C):
-            latent[c, order] = eng.experts_f_class(c, len(X))
-            # produceModel in the fit's context; each class starts from the default precision, as a freshly acquired
-            # context would (a fallback to F64 in one class's statistics must not decide the next class's path)
-            eng.set_precision(N.SGP_PREC_AUTO)
+            # produceModel in the fit's context
             kernel, active_set, mv, mm, _ = _produce_model(gp, eng, X, latent[c], thetas[c])
             # the model's own small context: never runs statistics, so it holds no statistics workspace
             model_eng = ProjectedProcessEngine(gp._device)

@@ -40,6 +40,13 @@ def is_cuda_tensor(x) -> bool:
     return type(x).__module__.partition(".")[0] == "torch" and bool(getattr(x, "is_cuda", False))
 
 
+def _rows(X):
+    """Points as the library reads them: float32 stays as it is (no copy when already contiguous), anything else becomes
+    float64; C-contiguous."""
+    X = np.asarray(X)
+    return np.ascontiguousarray(X if X.dtype == np.float32 else np.asarray(X, dtype=np.float64))
+
+
 def _make_desc(kernel: Kernel, d: int):
     terms = kernel.flatten()
     arr = (N.KernelTerm * len(terms))()
@@ -149,11 +156,8 @@ class ProjectedProcessEngine:
 
     def accumulate(self, X, y):
         """One shard of points in host memory.  X: n x d (float32 or float64), y: n."""
-        X = np.asarray(X)
-        if X.dtype != np.float32:
-            X = np.asarray(X, dtype=np.float64)
-        X = np.ascontiguousarray(X)
-        y = np.ascontiguousarray(y, dtype=np.float64)
+        X = _rows(X)
+        y =np.ascontiguousarray(y, dtype=np.float64)
         if X.ndim != 2 or X.shape[1] != self.d or len(y) != len(X):
             raise ValueError("shard shape mismatch")
         self._check(self._lib.sgp_stats_accumulate(self._h, N.ptr(X), int(X.dtype == np.float32), N.ptr(y), len(X)))
@@ -203,11 +207,8 @@ class ProjectedProcessEngine:
     def experts_upload_grouped(self, X, y, dataset_size_for_expert: int):
         """Groups the points into experts ON THE DEVICE (GPC:26-31: point i -> expert i % E) while they stream in; X may be
         float32 or float64, row-major as given.  Returns the number of experts."""
-        X = np.asarray(X)
-        if X.dtype != np.float32:
-            X = np.asarray(X, dtype=np.float64)
-        X = np.ascontiguousarray(X)
-        y = np.ascontiguousarray(y, dtype=np.float64)
+        X = _rows(X)
+        y =np.ascontiguousarray(y, dtype=np.float64)
         self._check(self._lib.sgp_experts_upload_grouped(self._h, N.ptr(X), int(X.dtype == np.float32), N.ptr(y), len(X),
                                                          X.shape[1], int(dataset_size_for_expert)))
         self._experts_d = X.shape[1]
@@ -260,11 +261,8 @@ class ProjectedProcessEngine:
         """Uploads the training set of every fold of a k-fold split (`sgp_experts_upload_folds`): set k holds the points
         with fold_of != k in index order, grouped into experts as `experts_upload_grouped` groups them.  X may be float32
         or float64.  Returns the number of experts of each set."""
-        X = np.asarray(X)
-        if X.dtype != np.float32:
-            X = np.asarray(X, dtype=np.float64)
-        X = np.ascontiguousarray(X)
-        y = np.ascontiguousarray(y, dtype=np.float64)
+        X = _rows(X)
+        y =np.ascontiguousarray(y, dtype=np.float64)
         folds = np.ascontiguousarray(fold_of, dtype=np.int32)
         if X.ndim != 2 or len(y) != len(X) or folds.shape != (len(X),):
             raise ValueError("experts_upload_folds: X must be n x d, y and fold_of n entries")
@@ -275,9 +273,9 @@ class ProjectedProcessEngine:
         n_k = len(X) - np.bincount(folds, minlength=int(n_folds))
         return np.floor(n_k / dataset_size_for_expert + 0.5).astype(np.int64)
 
-    def _slot_descriptors(self, kernels):
-        """Per-slot kernel descriptors and hyper-parameter descriptors of a batched objective: (descs, hypers, n_hypers,
-        the buffers both point into)."""
+    def _batched_objective(self, fn, head, kernels, tail=()):
+        """Runs one batched per-expert objective of the library, `fn(ctx, *head, descs, hypers, n_hypers, *tail, values,
+        gradients)`, with one evaluation per kernel.  Returns (values [n_eval], gradients [n_eval x n_hypers])."""
         descs = (N.KernelDesc * len(kernels))()
         keep, hyp, nh = [], None, None
         for i, k in enumerate(kernels):
@@ -291,7 +289,11 @@ class ProjectedProcessEngine:
             for j in range(nh):
                 hyp[i * nh + j] = arr[j]
             keep.append(kp)
-        return descs, hyp, nh, keep
+        vals = np.zeros(len(kernels))
+        grads = np.zeros((len(kernels), max(nh, 1)))
+        self._check(fn(self._h, *head, descs, hyp, nh, *tail, N.ptr(vals), N.ptr(grads)))
+        del keep
+        return vals, np.ascontiguousarray(grads[:, :nh])
 
     def bcm_nll_folds(self, sets, kernels):
         """The BCM objective of each listed fold set at its own kernels[i], all in one launch (`sgp_bcm_nll_folds`) over
@@ -300,12 +302,7 @@ class ProjectedProcessEngine:
         st = np.ascontiguousarray(sets, dtype=np.int32)
         if st.ndim != 1 or len(st) == 0 or len(st) != len(kernels):
             raise ValueError("bcm_nll_folds: one kernel per listed set")
-        descs, hyp, nh, keep = self._slot_descriptors(kernels)
-        vals = np.zeros(len(st))
-        grads = np.zeros((len(st), max(nh, 1)))
-        self._check(self._lib.sgp_bcm_nll_folds(self._h, N.ptr(st), len(st), descs, hyp, nh, N.ptr(vals), N.ptr(grads)))
-        del keep
-        return vals, np.ascontiguousarray(grads[:, :nh])
+        return self._batched_objective(self._lib.sgp_bcm_nll_folds, (N.ptr(st), len(st)), kernels)
 
     def laplace_nll_classes(self, n_classes: int, classes, kernels, tol: float):
         """One-vs-rest over uploaded class indices: the binary Laplace objective of each listed class c (labels y == c)
@@ -321,13 +318,7 @@ class ProjectedProcessEngine:
         cls = np.ascontiguousarray(classes, dtype=np.int32)
         if cls.ndim != 1 or len(cls) == 0 or len(cls) != len(kernels):
             raise ValueError("laplace_nll_classes: one kernel per listed class")
-        descs, hyp, nh, keep = self._slot_descriptors(kernels)
-        vals = np.zeros(len(cls))
-        grads = np.zeros((len(cls), max(nh, 1)))
-        self._check(fn(self._h, int(n_classes), N.ptr(cls), len(cls), descs, hyp, nh, float(tol), N.ptr(vals),
-                       N.ptr(grads)))
-        del keep
-        return vals, np.ascontiguousarray(grads[:, :nh])
+        return self._batched_objective(fn, (int(n_classes), N.ptr(cls), len(cls)), kernels, (float(tol),))
 
     def laplace_nll_slots_any_size(self, n_mode_slots: int, mode_slots, classes, kernels, tol: float):
         """Param-map slots (`sgp_laplace_nll_slots_any_size`): listed slot i evaluates the binary Laplace objective of the
@@ -338,31 +329,25 @@ class ProjectedProcessEngine:
         cls = np.ascontiguousarray(classes, dtype=np.int32)
         if modes.ndim != 1 or len(modes) == 0 or cls.shape != modes.shape or len(modes) != len(kernels):
             raise ValueError("laplace_nll_slots_any_size: one class and one kernel per listed mode slot")
-        descs, hyp, nh, keep = self._slot_descriptors(kernels)
-        vals = np.zeros(len(modes))
-        grads = np.zeros((len(modes), max(nh, 1)))
-        self._check(self._lib.sgp_laplace_nll_slots_any_size(self._h, int(n_mode_slots), N.ptr(modes), N.ptr(cls),
-                                                             len(modes), descs, hyp, nh, float(tol), N.ptr(vals),
-                                                             N.ptr(grads)))
-        del keep
-        return vals, np.ascontiguousarray(grads[:, :nh])
+        return self._batched_objective(self._lib.sgp_laplace_nll_slots_any_size,
+                                       (int(n_mode_slots), N.ptr(modes), N.ptr(cls), len(modes)), kernels, (float(tol),))
+
+    def _modes(self, fn, n: int, *which):
+        """n latent modes (packed expert-major order) read back by `fn(ctx, *which, out)`."""
+        f = np.empty(n)
+        self._check(fn(self._h, *which, N.ptr(f)))
+        return f
 
     def experts_f_slot(self, slot: int, n: int):
         """Mode slot `slot`'s latent modes after `laplace_nll_slots_any_size` (packed expert-major order)."""
-        f = np.empty(n)
-        self._check(self._lib.sgp_experts_get_f_slot(self._h, int(slot), N.ptr(f)))
-        return f
+        return self._modes(self._lib.sgp_experts_get_f_slot, n, int(slot))
 
     def experts_f_class(self, cls: int, n: int):
         """Class cls's latent modes after `laplace_nll_classes` (packed expert-major order)."""
-        f = np.empty(n)
-        self._check(self._lib.sgp_experts_get_f_class(self._h, int(cls), N.ptr(f)))
-        return f
+        return self._modes(self._lib.sgp_experts_get_f_class, n, int(cls))
 
     def experts_f(self, n: int):
-        f = np.empty(n)
-        self._check(self._lib.sgp_experts_get_f(self._h, N.ptr(f)))
-        return f
+        return self._modes(self._lib.sgp_experts_get_f, n)
 
     def bcm_nll(self, kernel: Kernel):
         """(sum over experts of 1/2 y'K^-1 y + 1/2 log|K|, gradient w.r.t. kernel.getHyperparameters())."""
@@ -452,10 +437,7 @@ class ProjectedProcessEngine:
         """Spark 3.1 MLlib KMeans (k-means|| seeding, Lloyd iterations) on the device (`sgp_kmeans`): returns
         (centres [k_out x d] fp64, labels [n] int32, iterations, cost).  X: n x d, float32 (used without a copy) or
         float64.  init_centers (k x d) replaces the seeding, as mllib's setInitialModel."""
-        X = np.asarray(X)
-        if X.dtype != np.float32:
-            X = np.asarray(X, dtype=np.float64)
-        X = np.ascontiguousarray(X)
+        X = _rows(X)
         if X.ndim != 2:
             raise ValueError("X must be n x d")
         n, d = X.shape
@@ -476,11 +458,8 @@ class ProjectedProcessEngine:
 
     def kmn_sweep(self, X):
         """fp32 K[i][j] = k(x_i, z_j) (n x m) through the tensor-core sweep kernel (one non-Eye term, d <= 32)."""
-        X = np.asarray(X)
-        if X.dtype != np.float32:
-            X = np.asarray(X, dtype=np.float64)
-        X = np.ascontiguousarray(X)
-        K = np.empty((len(X), self.m), dtype=np.float32)
+        X = _rows(X)
+        K =np.empty((len(X), self.m), dtype=np.float32)
         self._check(self._lib.sgp_kmn_sweep(self._h, N.ptr(X), int(X.dtype == np.float32), len(X), N.ptr(K)))
         return K
 

@@ -4,7 +4,8 @@ Expert grouping as the reference (GPC:26-31: E = Math.round(N / n_e), point i ->
 (sum over experts of the negative log marginal likelihood, GPR:55-68, + gradient) runs on the GPU (`sgp_bcm_nll`);
 the bound-constrained quasi-Newton loop is SciPy's L-BFGS-B in place of Breeze's `LBFGSB(lower, upper, maxIter,
 tolerance = tol)` -- the reference pins no test on the iterate trajectory, so results are compared on the objective
-value and on predictive metrics, not on theta."""
+value and on predictive metrics, not on theta.  `optimise_slots` runs that loop for every estimator and model selector
+here, over one slot or several in lock-step."""
 from __future__ import annotations
 
 import threading
@@ -113,6 +114,24 @@ def lbfgsb_lockstep(evaluate, x0s, bounds, max_iter: int, tol: float):
     return out, rounds
 
 
+def optimise_slots(evaluate, x0s, bounds, max_iter: int, tol: float):
+    """The hyper-parameter optimisation of every estimator here: one `lbfgsb` per slot, from x0s[i], with
+    `evaluate([(i, theta_i), ...]) -> [(value, gradient), ...]` as the objective of the listed slots.  One slot runs
+    `lbfgsb` on the calling thread; several run in lock-step (`lbfgsb_lockstep`), each on the trajectory of its
+    independent run.  maxIter <= 0 evaluates nothing (SciPy's L-BFGS-B would still evaluate x0).  Returns (each slot's
+    theta, each slot's record dict(value, evaluations, iterations) or None when nothing was optimised, rounds: the
+    number of `evaluate` calls)."""
+    if max_iter <= 0:
+        return [np.asarray(x0, dtype=np.float64) for x0 in x0s], None, 0
+    if len(x0s) == 1:
+        res, evaluations = lbfgsb(lambda theta: evaluate([(0, theta)])[0], x0s[0], bounds, max_iter, tol)
+        results, rounds = [(res, evaluations)], evaluations
+    else:
+        results, rounds = lbfgsb_lockstep(evaluate, x0s, bounds, max_iter, tol)
+    return ([np.asarray(res.x, dtype=np.float64) for res, _ in results],
+            [dict(value=float(res.fun), evaluations=ev, iterations=int(res.nit)) for res, ev in results], rounds)
+
+
 def group_for_experts(n_points: int, dataset_size_for_expert: int):
     """GPC:26-31."""
     n_experts = int(np.floor(n_points / dataset_size_for_expert + 0.5))
@@ -154,39 +173,22 @@ def pack_experts(X, y, dataset_size_for_expert: int):
     return Xp, yp, offsets
 
 
-class BcmObjective:
-    """f(theta) and its gradient, memoised like commons/util/DiffFunctionMemoized.scala."""
-
-    def __init__(self, engine: ProjectedProcessEngine, kernel_factory, X, y, dataset_size_for_expert: int):
-        self.engine, self.kernel_factory = engine, kernel_factory
-        # expert grouping (GPC:26-31) as a strided gather on the device while the points stream in (the host-side
-        # pack_experts below is the same permutation, kept for callers that hold expert-major data and for the tests)
-        self.n_experts = engine.experts_upload_grouped(X, y, dataset_size_for_expert)
-        self._memo = {}
-        self.evaluations = 0
-
-    def __call__(self, theta):
-        key = tuple(np.asarray(theta, dtype=np.float64))
-        if key not in self._memo:
-            kernel = self.kernel_factory().setHyperparameters(np.asarray(theta, dtype=np.float64))
-            self._memo[key] = self.engine.bcm_nll(kernel)
-            self.evaluations += 1
-        return self._memo[key]
-
-
 def optimize_hypers(gp, X, y, engine: ProjectedProcessEngine | None = None):
     """Returns the optimal hyper-parameter vector (layout of Kernel.getHyperparameters)."""
     own = engine is None
     engine = engine or ProjectedProcessEngine.acquire(gp._device)
     try:
-        obj = BcmObjective(engine, gp.getKernel, X, y, gp._datasetSizeForExpert)
+        # expert grouping (GPC:26-31) as a strided gather on the device while the points stream in (the host-side
+        # pack_experts above is the same permutation, kept for callers that hold expert-major data and for the tests)
+        n_experts = engine.experts_upload_grouped(X, y, gp._datasetSizeForExpert)
         launches0 = engine.launch_count()
         k0 = gp.getKernel()
-        # the same L-BFGS-B call as the cross-validator's lock-step slots, so that a fold slot follows this trajectory
-        res, _ = lbfgsb(obj, k0.getHyperparameters(), lbfgsb_bounds(k0), gp._maxIter, gp._tol)
-        gp.last_objective = dict(value=float(res.fun), evaluations=obj.evaluations, iterations=int(res.nit),
-                                 n_experts=obj.n_experts, launches=engine.launch_count() - launches0)
-        return np.asarray(res.x, dtype=np.float64)
+        evaluate = lambda batch: [engine.bcm_nll(gp.getKernel().setHyperparameters(t)) for _, t in batch]
+        (theta,), records, _ = optimise_slots(evaluate, [k0.getHyperparameters()], lbfgsb_bounds(k0), gp._maxIter,
+                                              gp._tol)
+        if records is not None:
+            gp.last_objective = dict(records[0], n_experts=n_experts, launches=engine.launch_count() - launches0)
+        return theta
     finally:
         if own:
             engine.release()

@@ -38,11 +38,10 @@ from __future__ import annotations
 
 import numpy as np
 
-from . import _native as N
-from .classification import GaussianProcessClassifier, OneVsRest, _produce_model, one_vs_rest_labels, \
+from .classification import GaussianProcessClassifier, OneVsRest, _produce_model, laplace_fit, one_vs_rest_labels, \
     one_vs_rest_prediction
 from .engine import ProjectedProcessEngine
-from .hyperopt import group_for_experts, lbfgsb_bounds, lbfgsb_lockstep
+from .hyperopt import lbfgsb_bounds, optimise_slots
 from .regression import GaussianProcessRegression
 from .utils import kfold_assignment, train_validation_assignment
 
@@ -85,11 +84,10 @@ def regression_metric(name: str, y, p) -> float:
     raise ValueError("metricName must be one of rmse, mse, r2, mae, var, not %r" % (name,))
 
 
-class RegressionEvaluator:
-    METRICS = ("rmse", "mse", "r2", "mae", "var")
-
-    def __init__(self, metricName: str = "rmse"):
-        self.setMetricName(metricName)
+class _Evaluator:
+    """What the evaluators share: the metric name, one of METRICS, and `evaluate`, which checks its arguments and hands
+    them to `_metric_of(name, y, prediction)`."""
+    METRICS = ()
 
     def setMetricName(self, value: str):
         if value not in self.METRICS:
@@ -100,14 +98,22 @@ class RegressionEvaluator:
     def getMetricName(self) -> str:
         return self._metric
 
-    def isLargerBetter(self) -> bool:
-        return self._metric in ("r2", "var")
-
     def evaluate(self, y, prediction) -> float:
         y = np.asarray(y, dtype=np.float64)
         if len(y) == 0 or np.shape(prediction) != y.shape:
             raise ValueError("evaluate: labels and predictions must be non-empty vectors of one length")
-        return regression_metric(self._metric, y, prediction)
+        return self._metric_of(self._metric, y, prediction)
+
+
+class RegressionEvaluator(_Evaluator):
+    METRICS = ("rmse", "mse", "r2", "mae", "var")
+    _metric_of = staticmethod(regression_metric)
+
+    def __init__(self, metricName: str = "rmse"):
+        self.setMetricName(metricName)
+
+    def isLargerBetter(self) -> bool:
+        return self._metric in ("r2", "var")
 
 
 def multiclass_metric(name: str, y, p) -> float:
@@ -136,31 +142,17 @@ def multiclass_metric(name: str, y, p) -> float:
     return total
 
 
-class MulticlassClassificationEvaluator:
+class MulticlassClassificationEvaluator(_Evaluator):
     """Spark's MulticlassClassificationEvaluator over (label, prediction): f1 (default), accuracy, weightedPrecision,
     weightedRecall, all larger-is-better."""
     METRICS = ("f1", "accuracy", "weightedPrecision", "weightedRecall")
+    _metric_of = staticmethod(multiclass_metric)
 
     def __init__(self, metricName: str = "f1"):
         self.setMetricName(metricName)
 
-    def setMetricName(self, value: str):
-        if value not in self.METRICS:
-            raise ValueError("metricName must be one of %s, not %r" % (", ".join(self.METRICS), value))
-        self._metric = value
-        return self
-
-    def getMetricName(self) -> str:
-        return self._metric
-
     def isLargerBetter(self) -> bool:
         return True
-
-    def evaluate(self, y, prediction) -> float:
-        y = np.asarray(y, dtype=np.float64)
-        if len(y) == 0 or np.shape(prediction) != y.shape:
-            raise ValueError("evaluate: labels and predictions must be non-empty vectors of one length")
-        return multiclass_metric(self._metric, y, prediction)
 
 
 def best_index(metrics, larger_is_better: bool) -> int:
@@ -178,21 +170,28 @@ def slot_group_key(est: GaussianProcessRegression):
     return (est._datasetSizeForExpert, terms, layout, tuple(lbfgsb_bounds(k)), est._maxIter, est._tol)
 
 
-def group_slots(estimators, n_folds: int):
-    """{key: [(map index, fold), ...]} over every (map, fold) slot, in map-major order."""
+def group_slots(estimators, n: int):
+    """{slot_group_key: [(map index p, j), ...]} over every slot (p, j), j in [0, n), of one estimator per map, in
+    map-major order; j is the fold of a cross-validation or the class of a train/validation split."""
     groups = {}
     for p, est in enumerate(estimators):
-        key = slot_group_key(est)
-        groups.setdefault(key, []).extend((p, k) for k in range(n_folds))
+        groups.setdefault(slot_group_key(est), []).extend((p, j) for j in range(n))
     return groups
 
 
-class CrossValidatorModel:
-    """Spark's CrossValidatorModel: the best map refitted on every row, and each map's metric averaged over the folds."""
+def tvs_slot_groups(classifiers, n_classes: int):
+    """`group_slots` over the (map p, class c) slots of a train/validation split over classifiers (one per map), each
+    with the device mode slot it owns: {slot_group_key: [(p, c, p * n_classes + c), ...]}.  The one place that numbers
+    mode slots."""
+    return {key: [(p, c, p * n_classes + c) for p, c in slots]
+            for key, slots in group_slots(classifiers, n_classes).items()}
 
-    def __init__(self, bestModel, avgMetrics, bestIndex, last_objective):
+
+class _SelectedModel:
+    """What the model selectors' models share: the best map refitted on every row predicts."""
+
+    def __init__(self, bestModel, bestIndex, last_objective):
         self.bestModel = bestModel
-        self.avgMetrics = list(avgMetrics)
         self.bestIndex = bestIndex
         self.last_objective = last_objective
 
@@ -202,7 +201,40 @@ class CrossValidatorModel:
     transform = predict
 
 
-class CrossValidator:
+class _Validator:
+    """What the model selectors share: the param maps, the seed and the check of the data; NAME prefixes the errors."""
+    NAME = ""
+
+    def setEstimatorParamMaps(self, value):
+        maps = [dict(m) for m in value]
+        if not maps:
+            raise ValueError("%s: at least one param map" % self.NAME)
+        self._maps = maps
+        return self
+
+    def setSeed(self, value: int):
+        self._seed = int(value)
+        return self
+
+    def _data(self, X, y):
+        X = np.asarray(X)
+        y = np.asarray(y, dtype=np.float64)
+        if X.ndim != 2 or len(y) != len(X):
+            raise ValueError("%s: X must be n x d and y n labels" % self.NAME)
+        return X, y
+
+
+class CrossValidatorModel(_SelectedModel):
+    """Spark's CrossValidatorModel: the best map refitted on every row, and each map's metric averaged over the folds."""
+
+    def __init__(self, bestModel, avgMetrics, bestIndex, last_objective):
+        super().__init__(bestModel, bestIndex, last_objective)
+        self.avgMetrics = list(avgMetrics)
+
+
+class CrossValidator(_Validator):
+    NAME = "CrossValidator"
+
     def __init__(self):
         self._estimator = None
         self._evaluator = RegressionEvaluator()
@@ -224,21 +256,10 @@ class CrossValidator:
         self._evaluator = value
         return self
 
-    def setEstimatorParamMaps(self, value):
-        maps = [dict(m) for m in value]
-        if not maps:
-            raise ValueError("CrossValidator: at least one param map")
-        self._maps = maps
-        return self
-
     def setNumFolds(self, value: int):
         if int(value) < 2:
             raise ValueError("CrossValidator: numFolds must be >= 2")
         self._num_folds = int(value)
-        return self
-
-    def setSeed(self, value: int):
-        self._seed = int(value)
         return self
 
     def getNumFolds(self) -> int:
@@ -249,10 +270,7 @@ class CrossValidator:
         est = self._estimator
         if est is None:
             raise TypeError("CrossValidator: setEstimator(GaussianProcessRegression) first")
-        X = np.asarray(X)
-        y = np.asarray(y, dtype=np.float64)
-        if X.ndim != 2 or len(y) != len(X):
-            raise ValueError("CrossValidator: X must be n x d and y n labels")
+        X, y = self._data(X, y)
         K = self._num_folds
         if folds is None:
             fold_of = kfold_assignment(len(X), K, self._seed)
@@ -304,46 +322,27 @@ class CrossValidator:
                                                     [kernel_at(slots[i][0], t) for i, t in batch])
                     return [(float(v), g) for v, g in zip(vals, grads)]
 
-                k0 = e0.getKernel()
-                results, rounds = lbfgsb_lockstep(evaluate, [x0s[p] for p, _ in slots], lbfgsb_bounds(k0), e0._maxIter,
-                                                  e0._tol)
-                groups.append(dict(
-                    slots=[dict(map=p, fold=k, value=float(res.fun), evaluations=ev, iterations=int(res.nit))
-                           for (p, k), (res, ev) in zip(slots, results)],
-                    rounds=rounds, launches=eng.launch_count() - launches0))
+                fitted, records, rounds = optimise_slots(evaluate, [x0s[p] for p, _ in slots],
+                                                         lbfgsb_bounds(e0.getKernel()), e0._maxIter, e0._tol)
+                groups.append(dict(slots=[dict(map=p, fold=k, **r) for (p, k), r in zip(slots, records)],
+                                   rounds=rounds, launches=eng.launch_count() - launches0))
             finally:
-                eng.set_precision(N.SGP_PREC_AUTO)
                 eng.release()
-            for (p, k), (res, _) in zip(slots, results):
-                thetas[p][k] = np.asarray(res.x, dtype=np.float64)
+            for (p, k), theta in zip(slots, fitted):
+                thetas[p][k] = theta
         return thetas, dict(groups=groups)
 
 
-def tvs_slot_groups(classifiers, n_classes: int):
-    """{slot_group_key: [(map index p, class index c, mode slot p * n_classes + c), ...]} over every (map, class) slot of
-    a train/validation split over classifiers (one per map), in map-major order."""
-    groups = {}
-    for p, gp in enumerate(classifiers):
-        groups.setdefault(slot_group_key(gp), []).extend((p, c, p * n_classes + c) for c in range(n_classes))
-    return groups
-
-
-class TrainValidationSplitModel:
+class TrainValidationSplitModel(_SelectedModel):
     """Spark's TrainValidationSplitModel: the best map refitted on every row, and each map's validation metric."""
 
     def __init__(self, bestModel, validationMetrics, bestIndex, last_objective):
-        self.bestModel = bestModel
+        super().__init__(bestModel, bestIndex, last_objective)
         self.validationMetrics = list(validationMetrics)
-        self.bestIndex = bestIndex
-        self.last_objective = last_objective
-
-    def predict(self, features):
-        return self.bestModel.predict(features)
-
-    transform = predict
 
 
-class TrainValidationSplit:
+class TrainValidationSplit(_Validator):
+    NAME = "TrainValidationSplit"
     ESTIMATORS = (GaussianProcessRegression, GaussianProcessClassifier, OneVsRest)
     EVALUATORS = (RegressionEvaluator, MulticlassClassificationEvaluator)
 
@@ -369,21 +368,10 @@ class TrainValidationSplit:
         self._evaluator = value
         return self
 
-    def setEstimatorParamMaps(self, value):
-        maps = [dict(m) for m in value]
-        if not maps:
-            raise ValueError("TrainValidationSplit: at least one param map")
-        self._maps = maps
-        return self
-
     def setTrainRatio(self, value: float):
         if not 0.0 < float(value) < 1.0:
             raise ValueError("TrainValidationSplit: trainRatio must lie in (0, 1)")
         self._train_ratio = float(value)
-        return self
-
-    def setSeed(self, value: int):
-        self._seed = int(value)
         return self
 
     def getTrainRatio(self) -> float:
@@ -396,10 +384,7 @@ class TrainValidationSplit:
             raise TypeError("TrainValidationSplit: setEstimator first")
         if self._evaluator is None:
             raise ValueError("TrainValidationSplit: setEvaluator first (there is no default evaluator)")
-        X = np.asarray(X)
-        y = np.asarray(y, dtype=np.float64)
-        if X.ndim != 2 or len(y) != len(X):
-            raise ValueError("TrainValidationSplit: X must be n x d and y n labels")
+        X, y = self._data(X, y)
         if train is None:
             mask = train_validation_assignment(len(X), self._train_ratio, self._seed)
         else:
@@ -456,42 +441,28 @@ class TrainValidationSplit:
         groups = []
         for slots in tvs_slot_groups(gps, C).values():
             g0 = gps[slots[0][0]]
+            modes = [m for _, _, m in slots]
             kernel_at = lambda p, t: gps[p].getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
-            x0s = [gps[p].getKernel().getHyperparameters() for p, _, _ in slots]
             eng = ProjectedProcessEngine.acquire(g0._device)
             try:
-                order = np.concatenate(group_for_experts(len(Xt), g0._datasetSizeForExpert))
-                eng.experts_upload_grouped(Xt, yt, g0._datasetSizeForExpert)
-                launches0 = eng.launch_count()
-                calls = [0]
-
-                def evaluate(batch):
-                    calls[0] += 1
+                def objective(batch):
                     vals, grads = eng.laplace_nll_slots_any_size(
-                        len(gps) * C, [slots[i][2] for i, _ in batch], [label(slots[i][1]) for i, _ in batch],
+                        len(gps) * C, [modes[i] for i, _ in batch], [label(slots[i][1]) for i, _ in batch],
                         [kernel_at(slots[i][0], t) for i, t in batch], g0._tol)
                     return [(float(v), g) for v, g in zip(vals, grads)]
 
-                thetas = [np.asarray(x0, dtype=np.float64) for x0 in x0s]
-                results, rounds = [], 0
-                if g0._maxIter > 0 and len(x0s[0]) > 0:
-                    results, rounds = lbfgsb_lockstep(evaluate, x0s, lbfgsb_bounds(g0.getKernel()), g0._maxIter, g0._tol)
-                    thetas = [np.asarray(res.x, dtype=np.float64) for res, _ in results]
-                evaluate(list(enumerate(thetas)))           # GPCls:60: every slot's f is its mode at theta*
+                thetas, latent, fit = laplace_fit(g0, eng, Xt, yt, objective,
+                                                  lambda i: eng.experts_f_slot(modes[i], len(Xt)),
+                                                  [gps[p].getKernel().getHyperparameters() for p, _, _ in slots])
+                # every objective call is one round, and one more runs at the slots' thetas
                 groups.append(dict(
-                    slots=[dict(map=p, cls=c, mode_slot=m, theta=theta, value=float(res.fun), evaluations=ev,
-                                iterations=int(res.nit))
-                           for (p, c, m), (res, ev), theta in zip(slots, results, thetas)],
-                    rounds=rounds, calls=calls[0], launches=eng.launch_count() - launches0))
-                f = np.empty(len(Xt))
-                for (p, c, m), theta in zip(slots, thetas):
-                    f[order] = eng.experts_f_slot(m, len(Xt))
-                    # each slot's model starts from the default precision, as the independent fit's fresh context does
-                    eng.set_precision(N.SGP_PREC_AUTO)
+                    slots=[dict(map=p, cls=c, mode_slot=m, theta=theta, **r)
+                           for (p, c, m), r, theta in zip(slots, fit["slots"] or [], thetas)],
+                    rounds=fit["rounds"], calls=fit["rounds"] + 1, launches=fit["launches_total"]))
+                for (p, c, _), f, theta in zip(slots, latent, thetas):
                     _produce_model(gps[p], eng, Xt, f, theta)
                     raw[p][:, c], _ = eng.predict(Xv, with_variance=False)
             finally:
-                eng.set_precision(N.SGP_PREC_AUTO)
                 eng.release()
         if ovr:
             preds = [one_vs_rest_prediction(r) for r in raw]

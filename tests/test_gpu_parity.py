@@ -451,11 +451,10 @@ def test_fit_with_hyperparameter_optimisation():
     rmse = float(np.sqrt(np.mean((model.predict(X[te]) - y[te]) ** 2)))
     assert rmse < 0.11
     assert gp.last_objective["evaluations"] >= 2
-    from spark_gp_b200.hyperopt import BcmObjective
     eng = sg.ProjectedProcessEngine(0)
-    obj = BcmObjective(eng, gp.getKernel, X[tr], y[tr], 100)
-    f0, _ = obj(gp.getKernel().getHyperparameters())
-    f1, _ = obj(model.hyperparameters)
+    eng.experts_upload_grouped(X[tr], y[tr], 100)
+    f0, _ = eng.bcm_nll(gp.getKernel().setHyperparameters(gp.getKernel().getHyperparameters()))
+    f1, _ = eng.bcm_nll(gp.getKernel().setHyperparameters(model.hyperparameters))
     eng.close()
     assert f1 <= f0
 

@@ -1,12 +1,14 @@
 """Host side of cross-validation (no GPU): the fold split, the grid, the metrics, best-index selection, the slot grouping,
-`copy`, and the lock-step optimiser driving slots that share a fold."""
+`copy`, the lock-step optimiser driving slots that share a fold, and the slot optimiser every estimator uses."""
+import threading
+
 import numpy as np
 import pytest
 
 import spark_gp_b200 as sg
 from oracle import cross_validation as ocv
 from oracle.kmeans import u
-from spark_gp_b200.hyperopt import lbfgsb, lbfgsb_lockstep
+from spark_gp_b200.hyperopt import lbfgsb, lbfgsb_lockstep, optimise_slots
 from spark_gp_b200.tuning import best_index, group_slots, regression_metric
 from spark_gp_b200.utils import kfold_assignment
 
@@ -116,3 +118,42 @@ def test_lockstep_slots_sharing_a_fold_follow_their_independent_runs():
         assert np.array_equal(res.x, ref.x)
         assert res.nit == ref.nit and ev_l == ev
     assert rounds == len(calls) and rounds < sum(ev for _, ev in results)
+
+
+@pytest.mark.parametrize("n_slots", [1, 4])
+def test_optimise_slots_equals_independent_lbfgsb_runs(n_slots):
+    """One slot is `lbfgsb` itself on the calling thread (no thread is started); several run in lock-step.  Either way
+    every slot's theta, value, evaluations and iterations are those of its independent `lbfgsb`."""
+    x0s = [np.full(3, 0.5 + 0.2 * i) for i in range(n_slots)]
+    bounds = [(0.1, None), (0.1, 5.0), (0.0, None)]
+    threads_alive, calls = threading.active_count(), []
+
+    def evaluate(batch):
+        calls.append(threading.active_count())
+        return [_quadratic(i, t) for i, t in batch]
+
+    thetas, records, rounds = optimise_slots(evaluate, x0s, bounds, 30, 1e-9)
+    evaluations = []
+    for i in range(n_slots):
+        ref, ev = lbfgsb(lambda t: _quadratic(i, t), x0s[i], bounds, 30, 1e-9)
+        assert thetas[i].dtype == np.float64 and np.array_equal(thetas[i], ref.x)
+        assert records[i] == dict(value=float(ref.fun), evaluations=ev, iterations=int(ref.nit))
+        evaluations.append(ev)
+    assert rounds == len(calls) == max(evaluations)
+    if n_slots == 1:
+        assert all(n == threads_alive for n in calls)
+    else:
+        assert all(n > threads_alive for n in calls) and rounds < sum(evaluations)
+
+
+@pytest.mark.parametrize("n_slots", [1, 3])
+@pytest.mark.parametrize("max_iter", [0, -1])
+def test_optimise_slots_without_iterations_evaluates_nothing(n_slots, max_iter):
+    def evaluate(batch):
+        raise AssertionError("evaluated at maxIter %d" % max_iter)
+
+    x0s = [np.arange(3) + i for i in range(n_slots)]
+    thetas, records, rounds = optimise_slots(evaluate, x0s, [(None, None)] * 3, max_iter, 1e-9)
+    assert records is None and rounds == 0
+    for theta, x0 in zip(thetas, x0s):
+        assert theta.dtype == np.float64 and np.array_equal(theta, x0)

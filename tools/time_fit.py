@@ -9,7 +9,6 @@ import sys, time
 sys.path.insert(0, ".")
 import numpy as np
 import spark_gp_b200 as sg
-from spark_gp_b200.hyperopt import BcmObjective
 
 N_ = int(sys.argv[1]) if len(sys.argv) > 1 else 1_000_000
 max_iter = int(sys.argv[2]) if len(sys.argv) > 2 else 20
