@@ -154,6 +154,14 @@ int sgp_experts_upload(sgp_ctx* ctx, const double* X, const double* y, const int
  * the copy streams in -- the reference's zipWithIndex / groupByKey shuffle, here a strided gather.  Latent modes start at 0. */
 int sgp_experts_upload_grouped(sgp_ctx* ctx, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
                                int32_t dataset_size_for_expert);
+/* sgp_experts_upload_grouped on points already in device memory: the same refusals, allocation, offsets and gather, read
+ * in place instead of staged, so the experts are the same bits as the host upload's (the gather is a permutation and an
+ * exact fp32 -> fp64 conversion).  The library's stream does not wait for other streams: dX and dy must be written
+ * before the call.  They are read before it returns.  The same holds for every _device entry below. dX and dy must be device (or managed) memory on the
+ * context's device: anything else is refused with SGP_E_BADARG (checked with cudaPointerGetAttributes) before any
+ * allocation or launch. */
+int sgp_experts_upload_grouped_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, const double* dy, int64_t n,
+                                      int32_t d, int32_t dataset_size_for_expert);
 
 /* One hyper-parameter, in the order of Kernel.getHyperparameters (depth first, trainable scalar prepended). */
 enum { SGP_HYPER_SCALE = 0, SGP_HYPER_ARD_BETA = 1, SGP_HYPER_RBF_SIGMA = 2 };
@@ -191,6 +199,12 @@ int sgp_bcm_nll(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper* hy
  * sgp_laplace_nll*) see a fold upload as one expert set: the union of every set's experts. */
 int sgp_experts_upload_folds(sgp_ctx* ctx, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
                              const int32_t* fold_of, int32_t n_folds, int32_t dataset_size_for_expert);
+/* sgp_experts_upload_folds on points already in device memory: every set is the same bits as the host upload's.  fold_of
+ * (the split, not the data) stays in host memory. dX and dy must be device (or managed) memory on the
+ * context's device: anything else is refused with SGP_E_BADARG (checked with cudaPointerGetAttributes) before any
+ * allocation or launch. */
+int sgp_experts_upload_folds_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, const double* dy, int64_t n,
+                                    int32_t d, const int32_t* fold_of, int32_t n_folds, int32_t dataset_size_for_expert);
 
 /* The BCM objective of sgp_bcm_nll on several training sets of the last sgp_experts_upload_folds, in one launch over
  * experts x slots.  Slot s evaluates set sets[s] at its own kernels[s] and hypers[s * n_hypers ...] (the same kernel
@@ -289,6 +303,16 @@ int sgp_laplace_nll_slots_any_size(sgp_ctx* ctx, int32_t n_mode_slots, const int
  * sgp_laplace_nll_slots_any_size after an upload; SGP_E_BADARG for mode_slot outside [0, n_mode_slots). */
 int sgp_experts_get_f_slot(sgp_ctx* ctx, int32_t mode_slot, double* f_out);
 
+/* One stored mode vector in ROW order, written to device memory: dF_out[i] = the mode of point i, which the grouped
+ * upload put at position i / E of expert i % E (the first n % E experts one longer).  store: SGP_MODES_BINARY (the modes
+ * of sgp_experts_get_f; index ignored), SGP_MODES_CLASS (class `index`, as sgp_experts_get_f_class) or SGP_MODES_SLOT
+ * (mode slot `index`, as sgp_experts_get_f_slot).  The same refusals as those three getters, with their codes; besides,
+ * SGP_E_BADARG for an unknown store and SGP_E_STATE when the experts did not come from sgp_experts_upload_grouped or its
+ * _device form (other uploads have no row order to restore).  dF_out (n doubles) must be device memory on the context's
+ * device (SGP_E_BADARG otherwise, before the launch).  Returns when the modes are written. */
+enum { SGP_MODES_BINARY = 0, SGP_MODES_CLASS = 1, SGP_MODES_SLOT = 2 };
+int sgp_experts_get_f_rows_device(sgp_ctx* ctx, int32_t store, int32_t index, double* dF_out);
+
 /* Installs a caller-supplied (vector v, m x m matrix M, row-major) in place of the pair sgp_magic computes, so that
  * sgp_predict returns  mean_t = k(x_t, Z) . v  and  var_t = selfKernel + k(x_t, Z) M k(x_t, Z)^T  for them.  M need not be
  * bit-symmetric: the variance is the quadratic form of M itself.  This is the per-point part of
@@ -346,6 +370,14 @@ int sgp_debug_i8_tile(sgp_ctx* ctx, float* T_out /* 128*64 */, uint32_t* w_out /
  * Errors: SGP_E_NOT_PD as assertSymPositiveDefinite (PGPH:62-65), SGP_E_BADARG "empty.max" when every expert is poisoned. */
 int sgp_greedy_active_set(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const double* X, const double* y, int64_t n,
                           int32_t d, int64_t n_experts, int64_t first_index, int32_t m_target, int64_t* indices_out);
+/* sgp_greedy_active_set on dX (n x d fp64) and dy (n fp64) in device memory, read in place instead of copied in: the same
+ * selection, indices and errors; 8 n (d + 1) bytes less device memory.  indices_out stays host memory. dX and dy
+ * must be device (or managed) memory on the
+ * context's device: anything else is refused with SGP_E_BADARG (checked with cudaPointerGetAttributes) before any
+ * allocation or launch. */
+int sgp_greedy_active_set_device(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const double* dX, const double* dy,
+                                 int64_t n, int32_t d, int64_t n_experts, int64_t first_index, int32_t m_target,
+                                 int64_t* indices_out);
 
 /* KMeansActiveSetProvider (commons/ActiveSetProvider.scala:22-46): Spark 3.1 MLlib KMeans with the reference's settings
  * (k-means|| seeding with 2 steps, Euclidean distance, unit weights; DESIGN.md 4.7 restates the algorithm).  X: n x d
@@ -363,6 +395,14 @@ int sgp_kmeans(sgp_ctx* ctx, const void* X, int32_t x_is_f32, int64_t n, int32_t
                double tol, int64_t seed, const double* init_centers /* k x d, or NULL: k-means|| */,
                double* centers_out /* k x d */, int32_t* k_out, int32_t* labels_out /* n, or NULL */,
                int32_t* iterations_out, double* cost_out);
+/* sgp_kmeans on dX in device memory (fp64, or fp32 when x_is_f32 != 0), read in place instead of copied in: the same
+ * algorithm and the same bits in every output; the few rows the host reads (the seeding's candidates) are gathered on
+ * the device.  init_centers and every output stay host memory.  dX must be device (or managed) memory on the context's
+ * device: SGP_E_BADARG otherwise, before any allocation or launch. */
+int sgp_kmeans_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n, int32_t d, int32_t k, int32_t max_iter,
+                      double tol, int64_t seed, const double* init_centers /* k x d, or NULL: k-means|| */,
+                      double* centers_out /* k x d */, int32_t* k_out, int32_t* labels_out /* n, or NULL */,
+                      int32_t* iterations_out, double* cost_out);
 
 /* Evaluate K(X_test, Z) (n x m row-major fp64 out) with the current kernel -- the `crossKernel`
  * contract of kernel/Kernel.scala:69-74 (used by the golden-vector tests). */

@@ -25,7 +25,9 @@ EXPORTS = ["sgp_ctx_create", "sgp_ctx_destroy", "sgp_last_error", "sgp_set_preci
            "sgp_bcm_nll", "sgp_laplace_nll", "sgp_experts_get_f", "sgp_set_magic", "sgp_last_tail_path", "sgp_last_bcm_path", "sgp_experts_upload_grouped", "sgp_kmn_sweep", "sgp_kmn_sweep_device", "sgp_greedy_active_set", "sgp_kmeans",
            "sgp_laplace_nll_classes", "sgp_experts_get_f_class", "sgp_experts_upload_folds", "sgp_bcm_nll_folds",
            "sgp_laplace_nll_any_size", "sgp_laplace_nll_classes_any_size", "sgp_last_laplace_path",
-           "sgp_laplace_nll_slots_any_size", "sgp_experts_get_f_slot"]
+           "sgp_laplace_nll_slots_any_size", "sgp_experts_get_f_slot", "sgp_experts_upload_grouped_device",
+           "sgp_experts_upload_folds_device", "sgp_experts_get_f_rows_device", "sgp_kmeans_device",
+           "sgp_greedy_active_set_device"]
 
 
 class KernelTerm(C.Structure):
@@ -39,6 +41,7 @@ class Hyper(C.Structure):
 
 
 SGP_HYPER_SCALE, SGP_HYPER_ARD_BETA, SGP_HYPER_RBF_SIGMA = 0, 1, 2
+SGP_MODES_BINARY, SGP_MODES_CLASS, SGP_MODES_SLOT = 0, 1, 2
 
 
 class KernelDesc(C.Structure):
@@ -101,6 +104,11 @@ def load() -> C.CDLL:
     lib.sgp_experts_get_f_slot.argtypes = [vp, i32, vp]
     lib.sgp_experts_upload_folds.argtypes = [vp, vp, i32, vp, i64, i32, vp, i32, i32]
     lib.sgp_bcm_nll_folds.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp]
+    lib.sgp_experts_upload_grouped_device.argtypes = lib.sgp_experts_upload_grouped.argtypes
+    lib.sgp_experts_upload_folds_device.argtypes = lib.sgp_experts_upload_folds.argtypes
+    lib.sgp_experts_get_f_rows_device.argtypes = [vp, i32, i32, vp]
+    lib.sgp_kmeans_device.argtypes = lib.sgp_kmeans.argtypes
+    lib.sgp_greedy_active_set_device.argtypes = lib.sgp_greedy_active_set.argtypes
     lib.sgp_event_elapsed_ms.argtypes = [vp, C.c_int, C.c_int, dp]
     for name in EXPORTS:
         if name not in ("sgp_last_error", "sgp_launch_count"):

@@ -5,7 +5,7 @@ from __future__ import annotations
 import numpy as np
 
 from . import _native as N
-from .engine import ProjectedProcessEngine, is_cuda_tensor
+from .engine import ProjectedProcessEngine, device_fit_data, is_cuda_tensor
 from .hyperopt import group_for_experts, lbfgsb_bounds, optimise_slots
 from .regression import GaussianProcessParams, GaussianProjectedProcessRawPredictor
 
@@ -57,15 +57,15 @@ class GaussianProcessClassifier(GaussianProcessParams):
         self.last_objective = None
 
     def fit(self, X, y, hyperparameters=None) -> GaussianProcessClassificationModel:
-        X = np.asarray(X, dtype=np.float64)
-        y = np.asarray(y, dtype=np.float64)
-        if not np.all((y == 0.0) | (y == 1.0)):                     # assertLabelsAre01, GPCls:68-72
-            raise RuntimeError("Only 0 and 1 labels are supported.")
+        """X may be a CUDA tensor on the classifier's device (y a CUDA tensor there too, or a host vector): X, the labels
+        and the latent modes then stay on the device, and `last_latent` is a CUDA float64 tensor."""
+        X, y = fit_data(X, y, self._device, "GaussianProcessClassifier.fit")
+        assert_labels_are_01(y)
         eng = ProjectedProcessEngine.acquire(self._device)
         objective = lambda batch: [eng.laplace_nll_any_size(self.getKernel().setHyperparameters(t), self._tol)
                                    for _, t in batch]
         (theta,), (f,), fit = laplace_fit(
-            self, eng, X, y, objective, lambda _: eng.experts_f(len(X)), [self.getKernel().getHyperparameters()],
+            self, eng, X, y, objective, N.SGP_MODES_BINARY, lambda _: 0, [self.getKernel().getHyperparameters()],
             None if hyperparameters is None else [np.asarray(hyperparameters, dtype=np.float64)])
         if fit["slots"] is not None:
             self.last_objective = dict(fit["slots"][0], launches=fit["launches"])
@@ -75,16 +75,33 @@ class GaussianProcessClassifier(GaussianProcessParams):
         return GaussianProcessClassificationModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, active_set), theta)
 
 
-def laplace_fit(gp, eng, X, y, objective, modes, x0s, thetas=None):
+def fit_data(X, y, device: int, what: str):
+    """The (X, y) of a classifier fit: X as float64 (the classifiers read float64 points) and y float64, on the host, or on
+    the device for a CUDA tensor X (`device_fit_data`)."""
+    if is_cuda_tensor(X):
+        import torch
+        X, y = device_fit_data(X, y, device, what)
+        return X.to(torch.float64), y
+    return np.asarray(X, dtype=np.float64), np.asarray(y, dtype=np.float64)
+
+
+def assert_labels_are_01(y):
+    """assertLabelsAre01 (GPCls:68-72), on a host array or on the device (only the verdict crosses PCIe)."""
+    if not bool(((y == 0.0) | (y == 1.0)).all()):
+        raise RuntimeError("Only 0 and 1 labels are supported.")
+
+
+def laplace_fit(gp, eng, X, y, objective, store, index, x0s, thetas=None):
     """The Laplace part of the binary fit (GPCls:53-60) for every slot of the caller, on one upload of (X, y) into eng,
     grouped into experts by gp's datasetSizeForExpert (every slot's modes start at 0).
       objective([(i, theta_i), ...]) -> [(value, gradient), ...]: slot i's Laplace objective at theta_i, warm-started from
                                         and moving its device-resident modes;
-      modes(i):                         slot i's modes, packed expert-major.
+      store, index(i):                  where slot i's modes live (N.SGP_MODES_*, and the class or mode slot).
     Unless `thetas` are given, every slot is optimised from x0s (`optimise_slots`; skipped when there are no
     hyper-parameters).  Then the Laplace loop runs once more at every slot's theta (GPCls:60), so that its modes are the
-    modes at theta.  Returns (thetas, modes [slot][row] in row order, dict(slots: each slot's optimisation record or None
-    when nothing was optimised, rounds, launches: the optimisation's, launches_total: with the call at theta))."""
+    modes at theta.  Returns (thetas, modes [slot][row] in row order -- a CUDA float64 tensor, ungrouped on the device,
+    when X is a CUDA tensor --, dict(slots: each slot's optimisation record or None when nothing was optimised, rounds,
+    launches: the optimisation's, launches_total: with the call at theta))."""
     order = np.concatenate(group_for_experts(len(X), gp._datasetSizeForExpert))
     eng.experts_upload_grouped(X, y, gp._datasetSizeForExpert)
     launches0 = eng.launch_count()
@@ -96,9 +113,12 @@ def laplace_fit(gp, eng, X, y, objective, modes, x0s, thetas=None):
     launches = eng.launch_count() - launches0
     objective(list(enumerate(thetas)))
     fit = dict(slots=records, rounds=rounds, launches=launches, launches_total=eng.launch_count() - launches0)
+    if is_cuda_tensor(X):
+        import torch
+        return thetas, torch.stack([eng.experts_modes_rows(store, index(i), len(X)) for i in range(len(thetas))]), fit
     latent = np.empty((len(thetas), len(X)))
     for i in range(len(thetas)):
-        latent[i, order] = modes(i)
+        latent[i, order] = eng.experts_modes(store, index(i), len(X))
     return thetas, latent, fit
 
 
@@ -132,11 +152,16 @@ def _produce_model(gp, eng, X, f, theta):
 
 
 def one_vs_rest_labels(y):
-    """Validated class labels and numClasses = max(label) + 1 (Spark's OneVsRest)."""
-    y = np.asarray(y, dtype=np.float64)
+    """Validated class labels and numClasses = max(label) + 1 (Spark's OneVsRest).  A CUDA tensor is checked on the
+    device (only the verdict and the maximum cross PCIe) and returned as a CUDA float64 tensor."""
+    if is_cuda_tensor(y):
+        import torch
+        y, fin, floor = y.to(torch.float64), torch.isfinite, torch.floor
+    else:
+        y, fin, floor = np.asarray(y, dtype=np.float64), np.isfinite, np.floor
     if y.ndim != 1 or len(y) == 0:
         raise ValueError("OneVsRest: labels must be a non-empty vector")
-    if not np.all(np.isfinite(y) & (y >= 0.0) & (y == np.floor(y))):
+    if not bool((fin(y) & (y >= 0.0) & (y == floor(y))).all()):
         raise ValueError("OneVsRest: labels must be non-negative integers (class indices)")
     return y, int(y.max()) + 1
 
@@ -212,7 +237,7 @@ class OneVsRest:
         gp = self._classifier
         if not isinstance(gp, GaussianProcessClassifier):
             raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
-        X = np.asarray(X, dtype=np.float64)
+        X, y = fit_data(X, y, gp._device, "OneVsRest.fit")
         y, C = one_vs_rest_labels(y)
         eng = ProjectedProcessEngine.acquire(gp._device)
         try:
@@ -230,8 +255,7 @@ class OneVsRest:
 
         x0 = gp.getKernel().getHyperparameters()
         given = None if hyperparameters is None else np.array(hyperparameters, dtype=np.float64).reshape(C, len(x0))
-        thetas, latent, fit = laplace_fit(gp, eng, X, y, objective, lambda c: eng.experts_f_class(c, len(X)), [x0] * C,
-                                          given)
+        thetas, latent, fit = laplace_fit(gp, eng, X, y, objective, N.SGP_MODES_CLASS, lambda c: c, [x0] * C, given)
         thetas = np.array(thetas).reshape(C, len(x0))
         if fit["slots"] is not None:
             self.last_objective = dict(classes=fit["slots"], rounds=fit["rounds"], launches=fit["launches"])

@@ -119,6 +119,31 @@ static int stage_rows(Ctx* c, const void* X, const double* y, long long n, size_
   return SGP_OK;
 }
 
+// stage_rows for rows that are host memory, or the same chunks read in place where X and y are device memory already
+template <class Launch>
+static int feed_rows(Ctx* c, bool on_device, const void* X, const double* y, long long n, size_t row, long long chunk,
+                     Launch&& launch) {
+  if (!on_device) return stage_rows(c, X, y, n, row, chunk, chunk, launch);
+  for (long long p0 = 0; p0 < n; p0 += chunk) {
+    const long long cn = (n - p0 < chunk) ? (n - p0) : chunk;
+    const int rc = launch(static_cast<const char*>(X) + static_cast<size_t>(p0) * row, y ? y + p0 : nullptr, p0, cn);
+    if (rc != SGP_OK) return rc;
+  }
+  return SGP_OK;
+}
+
+// The pointer check of the _device entries: p must be device (or managed) memory on the context's device.  Refused
+// before any allocation or launch, so that a host pointer never reaches a kernel.
+static int device_ptr_ok(Ctx* c, const void* p, const char* entry, const char* what) {
+  cudaPointerAttributes a{};
+  const cudaError_t e = cudaPointerGetAttributes(&a, p);
+  if (e != cudaSuccess) cudaGetLastError();
+  if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != c->device)
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": " + what + " is not device memory on device " +
+                                     std::to_string(c->device));
+  return SGP_OK;
+}
+
 // Host state of the statistics kernels for the active set Z (m x d) and the flattened beta ([kMaxTerms][dpad]):
 // sc = [kMaxTerms][dpad] sqrt(log2 e) * beta_tk (int8 modes only, with_scales), then the [dpad] centre of the int8 modes,
 // the active-set mean; ctr64 = [dpad] the centre of the fp64 kernel.  Distances are translation invariant, and centred
@@ -780,6 +805,7 @@ int experts_alloc(Ctx* c, long long E, long long n, int d, int n_max) {
   ex.X = c->ex_X.as<double>(); ex.y = c->ex_y.as<double>(); ex.off = c->ex_off.as<long long>(); ex.f = c->ex_f.as<double>();
   SGP_CUDA(c, cudaMemsetAsync(ex.f, 0, static_cast<size_t>(n) * 8, c->stream));
   ex.n = n; ex.d = d; ex.n_max = n_max;
+  c->ex_grouped = false;
   c->ex_classes = 0;                                      // one-vs-rest modes restart at zero on their next use
   c->ex_mode_slots = 0;                                   // so do the param-map slots' modes
   c->fold_first.clear();
@@ -819,23 +845,29 @@ int sgp_experts_upload(sgp_ctx* h, const double* X, const double* y, const int64
   return SGP_OK;
 }
 
-int sgp_experts_upload_grouped(sgp_ctx* h, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
-                               int32_t dataset_size_for_expert) {
-  Ctx* c = reinterpret_cast<Ctx*>(h);
-  if (!c) return SGP_E_BADARG;
+namespace {
+// sgp_experts_upload_grouped and its _device form: X and y are host memory (staged) or device memory (read in place)
+int upload_grouped(Ctx* c, bool on_device, const void* X, int x_is_f32, const double* y, long long n, int d,
+                   int dataset_size_for_expert, const char* entry) {
   if (!X || !y || n <= 0 || d <= 0 || dataset_size_for_expert <= 0)
-    return fail(c, SGP_E_BADARG, "sgp_experts_upload_grouped: null or empty argument");
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": null or empty argument");
   SGP_CUDA(c, cudaSetDevice(c->device));
+  if (on_device) {
+    int rc = device_ptr_ok(c, X, entry, "X");
+    if (rc == SGP_OK) rc = device_ptr_ok(c, y, entry, "y");
+    if (rc != SGP_OK) return rc;
+  }
   // GPC:27  numberOfExperts = Math.round(points.count() / datasetSizeForExpert)  (round half up on a positive double)
   const long long E = static_cast<long long>(std::floor(static_cast<double>(n) / dataset_size_for_expert + 0.5));
   if (E <= 0) return fail(c, SGP_E_BADARG, "numberOfExperts == 0 (N < datasetSizeForExpert / 2): the reference fails with / by zero");
   int rc = experts_alloc(c, E, n, d, static_cast<int>(n / E + ((n % E) ? 1 : 0)));
   if (rc != SGP_OK) return rc;
   SGP_CUDA(c, launch_expert_offsets(c->ex.off, n, E, 0, c->stream));
-  // stream the row-major input through the double-buffered staging area of the statistics path, gather on the device
+  // host input streams through the double-buffered staging area of the statistics path; either way the gather is on the
+  // device, chunk by chunk
   const size_t row = static_cast<size_t>(d) * (x_is_f32 ? 4 : 8);
   const long long chunk = group_chunk(n, row);
-  rc = stage_rows(c, X, y, n, row, chunk, chunk, [&](const void* dX, const double* dy, long long p0, long long cn) -> int {
+  rc = feed_rows(c, on_device, X, y, n, row, chunk, [&](const void* dX, const double* dy, long long p0, long long cn) -> int {
     SGP_CUDA(c, launch_group_experts(c->ex.X, c->ex.y, dX, x_is_f32, dy, n, d, E, p0, cn, nullptr, 0, c->stream));
     c->launches += 1;
     return SGP_OK;
@@ -843,21 +875,27 @@ int sgp_experts_upload_grouped(sgp_ctx* h, const void* X, int32_t x_is_f32, cons
   if (rc != SGP_OK) return rc;
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   c->ex.E = E;
+  c->ex_grouped = true;
   return SGP_OK;
 }
 
-int sgp_experts_upload_folds(sgp_ctx* h, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
-                             const int32_t* fold_of, int32_t n_folds, int32_t dataset_size_for_expert) {
-  Ctx* c = reinterpret_cast<Ctx*>(h);
-  if (!c) return SGP_E_BADARG;
+// sgp_experts_upload_folds and its _device form; fold_of is host memory in both
+int upload_folds(Ctx* c, bool on_device, const void* X, int x_is_f32, const double* y, long long n, int d,
+                 const int32_t* fold_of, int n_folds, int dataset_size_for_expert, const char* entry) {
   if (!X || !y || !fold_of || n <= 0 || d <= 0 || dataset_size_for_expert <= 0)
-    return fail(c, SGP_E_BADARG, "sgp_experts_upload_folds: null or empty argument");
-  if (n_folds < 2) return fail(c, SGP_E_BADARG, "sgp_experts_upload_folds: n_folds must be >= 2");
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": null or empty argument");
+  if (n_folds < 2) return fail(c, SGP_E_BADARG, std::string(entry) + ": n_folds must be >= 2");
+  if (on_device) {
+    SGP_CUDA(c, cudaSetDevice(c->device));
+    int rc = device_ptr_ok(c, X, entry, "X");
+    if (rc == SGP_OK) rc = device_ptr_ok(c, y, entry, "y");
+    if (rc != SGP_OK) return rc;
+  }
   // the points of each fold in index order: set k leaves out pos[fstart[k] .. fstart[k+1]-1]
   std::vector<long long> fstart(static_cast<size_t>(n_folds) + 1, 0);
   for (int64_t i = 0; i < n; ++i) {
     if (fold_of[i] < 0 || fold_of[i] >= n_folds)
-      return fail(c, SGP_E_BADARG, "sgp_experts_upload_folds: fold index of point " + std::to_string(i) + " outside [0, n_folds)");
+      return fail(c, SGP_E_BADARG, std::string(entry) + ": fold index of point " + std::to_string(i) + " outside [0, n_folds)");
     ++fstart[fold_of[i] + 1];
   }
   for (int k = 0; k < n_folds; ++k) fstart[k + 1] += fstart[k];
@@ -884,7 +922,7 @@ int sgp_experts_upload_folds(sgp_ctx* h, const void* X, int32_t x_is_f32, const 
     const size_t held = c->ex_X.cap + c->ex_y.cap + c->ex_f.cap;
     const size_t need = static_cast<size_t>(n_rows) * (static_cast<size_t>(d) + 2) * 8;
     if (need > free_b + held)
-      return fail(c, SGP_E_NOMEM, "sgp_experts_upload_folds: the training sets need " + std::to_string(need >> 20) +
+      return fail(c, SGP_E_NOMEM, std::string(entry) + ": the training sets need " + std::to_string(need >> 20) +
                                       " MiB of device memory, " + std::to_string((free_b + held) >> 20) + " MiB available");
   }
   int rc = experts_alloc(c, E, n_rows, d, *std::max_element(nmax.begin(), nmax.end()));
@@ -899,10 +937,11 @@ int sgp_experts_upload_folds(sgp_ctx* h, const void* X, int32_t x_is_f32, const 
                                       c->stream));
     c->launches += 1;
   }
-  // X and y cross PCIe once; each staged chunk is gathered into every training set that holds its points
+  // X and y are read once (host input: cross PCIe once); each chunk is gathered into every training set that holds its
+  // points
   const size_t row = static_cast<size_t>(d) * (x_is_f32 ? 4 : 8);
   const long long chunk = group_chunk(n, row);
-  rc = stage_rows(c, X, y, n, row, chunk, chunk, [&](const void* dX, const double* dy, long long p0, long long cn) -> int {
+  rc = feed_rows(c, on_device, X, y, n, row, chunk, [&](const void* dX, const double* dy, long long p0, long long cn) -> int {
     for (int k = 0; k < n_folds; ++k) {
       SGP_CUDA(c, launch_group_experts(c->ex.X + static_cast<size_t>(row0[k]) * d, c->ex.y + row0[k], dX, x_is_f32, dy,
                                        row0[k + 1] - row0[k], d, first[k + 1] - first[k], p0, cn, dpos + fstart[k],
@@ -917,6 +956,37 @@ int sgp_experts_upload_folds(sgp_ctx* h, const void* X, int32_t x_is_f32, const 
   c->fold_nmax = nmax;
   c->ex.E = E;
   return SGP_OK;
+}
+}  // namespace
+
+int sgp_experts_upload_grouped(sgp_ctx* h, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
+                               int32_t dataset_size_for_expert) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return upload_grouped(c, false, X, x_is_f32, y, n, d, dataset_size_for_expert, "sgp_experts_upload_grouped");
+}
+
+int sgp_experts_upload_grouped_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, const double* dy, int64_t n, int32_t d,
+                                      int32_t dataset_size_for_expert) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return upload_grouped(c, true, dX, x_is_f32, dy, n, d, dataset_size_for_expert, "sgp_experts_upload_grouped_device");
+}
+
+int sgp_experts_upload_folds(sgp_ctx* h, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
+                             const int32_t* fold_of, int32_t n_folds, int32_t dataset_size_for_expert) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return upload_folds(c, false, X, x_is_f32, y, n, d, fold_of, n_folds, dataset_size_for_expert,
+                      "sgp_experts_upload_folds");
+}
+
+int sgp_experts_upload_folds_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, const double* dy, int64_t n, int32_t d,
+                                    const int32_t* fold_of, int32_t n_folds, int32_t dataset_size_for_expert) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return upload_folds(c, true, dX, x_is_f32, dy, n, d, fold_of, n_folds, dataset_size_for_expert,
+                      "sgp_experts_upload_folds_device");
 }
 
 namespace {
@@ -1404,6 +1474,38 @@ int sgp_experts_get_f(sgp_ctx* h, double* f_out) {
   return SGP_OK;
 }
 
+int sgp_experts_get_f_rows_device(sgp_ctx* h, int32_t store, int32_t index, double* dF_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (store != SGP_MODES_BINARY && store != SGP_MODES_CLASS && store != SGP_MODES_SLOT)
+    return fail(c, SGP_E_BADARG, "sgp_experts_get_f_rows_device: unknown mode store");
+  // the host getters' refusals, in their order and with their codes
+  if (c->ex.E == 0 || !dF_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
+  const double* f = c->ex.f;
+  if (store == SGP_MODES_CLASS) {
+    if (c->ex_classes == 0) return fail(c, SGP_E_STATE, "no class modes: sgp_laplace_nll_classes has not run since the upload");
+    if (index < 0 || index >= c->ex_classes)
+      return fail(c, SGP_E_BADARG, "sgp_experts_get_f_rows_device: class index out of range");
+    f = c->ex_fc.as<double>() + static_cast<size_t>(index) * c->ex.n;
+  } else if (store == SGP_MODES_SLOT) {
+    if (c->ex_mode_slots == 0)
+      return fail(c, SGP_E_STATE, "no slot modes: sgp_laplace_nll_slots_any_size has not run since the upload");
+    if (index < 0 || index >= c->ex_mode_slots)
+      return fail(c, SGP_E_BADARG, "sgp_experts_get_f_rows_device: mode slot outside [0, n_mode_slots)");
+    f = c->ex_fm.as<double>() + static_cast<size_t>(index) * c->ex.n;
+  }
+  if (!c->ex_grouped)
+    return fail(c, SGP_E_STATE, "sgp_experts_get_f_rows_device: the experts were not uploaded by sgp_experts_upload_grouped "
+                                "or its _device form, so their rows have no row order");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  const int rc = device_ptr_ok(c, dF_out, "sgp_experts_get_f_rows_device", "f_out");
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, launch_ungroup_experts(dF_out, f, c->ex.n, c->ex.E, c->stream));
+  c->launches += 1;
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  return SGP_OK;
+}
+
 int sgp_last_path(const sgp_ctx* h) {
   const Ctx* c = reinterpret_cast<const Ctx*>(h);
   return c ? c->last_path : -1;
@@ -1527,22 +1629,68 @@ int sgp_kmn_sweep(sgp_ctx* h, const void* X, int32_t x_is_f32, int64_t n, float*
   return SGP_OK;
 }
 
-int sgp_greedy_active_set(sgp_ctx* h, const sgp_kernel_desc* k, const double* X, const double* y, int64_t n, int32_t d,
-                          int64_t n_experts, int64_t first_index, int32_t m_target, int64_t* indices_out) {
-  Ctx* c = reinterpret_cast<Ctx*>(h);
-  if (!c) return SGP_E_BADARG;
+namespace {
+int greedy_active_set(Ctx* c, bool on_device, const sgp_kernel_desc* k, const double* X, const double* y, int64_t n,
+                      int32_t d, int64_t n_experts, int64_t first_index, int32_t m_target, int64_t* indices_out,
+                      const char* entry) {
   if (!k || !X || !y || !indices_out || n <= 0 || d <= 0 || m_target <= 0 || k->n_terms <= 0 || !k->terms)
-    return fail(c, SGP_E_BADARG, "sgp_greedy_active_set: null or empty argument");
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": null or empty argument");
   if (n_experts <= 0) return fail(c, SGP_E_BADARG, "numberOfExperts == 0 (N < datasetSizeForExpert / 2)");
   if (first_index < 0 || first_index >= n) return fail(c, SGP_E_BADARG, "first_index out of range");
-  if (n > 2147483647LL) return fail(c, SGP_E_BADARG, "sgp_greedy_active_set: n too large for one device");
+  if (n > 2147483647LL) return fail(c, SGP_E_BADARG, std::string(entry) + ": n too large for one device");
   SGP_CUDA(c, cudaSetDevice(c->device));
+  if (on_device) {
+    int rc = device_ptr_ok(c, X, entry, "X");
+    if (rc == SGP_OK) rc = device_ptr_ok(c, y, entry, "y");
+    if (rc != SGP_OK) return rc;
+  }
   KernelFlat kf;
   std::vector<double> beta;
   const int rc = flatten_kernel(c, k, d, d, kf, beta, nullptr);
   if (rc != SGP_OK) return rc;
   static_assert(sizeof(long long) == sizeof(int64_t), "index type");
-  return run_greedy(c, kf, beta, X, y, n, d, n_experts, first_index, m_target, reinterpret_cast<long long*>(indices_out));
+  return run_greedy(c, kf, beta, X, y, on_device, n, d, n_experts, first_index, m_target,
+                    reinterpret_cast<long long*>(indices_out));
+}
+
+int kmeans(Ctx* c, bool on_device, const void* X, int32_t x_is_f32, int64_t n, int32_t d, int32_t k, int32_t max_iter,
+           double tol, int64_t seed, const double* init_centers, double* centers_out, int32_t* k_out, int32_t* labels_out,
+           int32_t* iterations_out, double* cost_out, const char* entry) {
+  if (!X || !centers_out || !k_out || !iterations_out || !cost_out)
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": null argument");
+  if (k < 2) return fail(c, SGP_E_BADARG, "requirement failed: k must be > 1");
+  if (max_iter < 0) return fail(c, SGP_E_BADARG, "requirement failed: maxIter must be >= 0");
+  if (!(tol >= 0.0)) return fail(c, SGP_E_BADARG, "requirement failed: tol must be >= 0");
+  if (n < 1 || d < 1) return fail(c, SGP_E_BADARG, std::string(entry) + ": no points or no features");
+  if (n > 2147483647LL) return fail(c, SGP_E_BADARG, std::string(entry) + ": n too large for one device");
+  if (init_centers)
+    for (size_t i = 0; i < static_cast<size_t>(k) * d; ++i)
+      if (!std::isfinite(init_centers[i]))
+        return fail(c, SGP_E_BADARG, std::string(entry) + ": initial centres contain NaN or infinity");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  if (on_device) {
+    const int rc = device_ptr_ok(c, X, entry, "X");
+    if (rc != SGP_OK) return rc;
+  }
+  static_assert(sizeof(int) == sizeof(int32_t), "label type");
+  return run_kmeans(c, X, x_is_f32, on_device, n, d, k, max_iter, tol, static_cast<uint64_t>(seed), init_centers,
+                    centers_out, k_out, labels_out, iterations_out, cost_out);
+}
+}  // namespace
+
+int sgp_greedy_active_set(sgp_ctx* h, const sgp_kernel_desc* k, const double* X, const double* y, int64_t n, int32_t d,
+                          int64_t n_experts, int64_t first_index, int32_t m_target, int64_t* indices_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return greedy_active_set(c, false, k, X, y, n, d, n_experts, first_index, m_target, indices_out, "sgp_greedy_active_set");
+}
+
+int sgp_greedy_active_set_device(sgp_ctx* h, const sgp_kernel_desc* k, const double* dX, const double* dy, int64_t n,
+                                 int32_t d, int64_t n_experts, int64_t first_index, int32_t m_target, int64_t* indices_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return greedy_active_set(c, true, k, dX, dy, n, d, n_experts, first_index, m_target, indices_out,
+                           "sgp_greedy_active_set_device");
 }
 
 int sgp_kmeans(sgp_ctx* h, const void* X, int32_t x_is_f32, int64_t n, int32_t d, int32_t k, int32_t max_iter, double tol,
@@ -1550,20 +1698,17 @@ int sgp_kmeans(sgp_ctx* h, const void* X, int32_t x_is_f32, int64_t n, int32_t d
                int32_t* iterations_out, double* cost_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
-  if (!X || !centers_out || !k_out || !iterations_out || !cost_out)
-    return fail(c, SGP_E_BADARG, "sgp_kmeans: null argument");
-  if (k < 2) return fail(c, SGP_E_BADARG, "requirement failed: k must be > 1");
-  if (max_iter < 0) return fail(c, SGP_E_BADARG, "requirement failed: maxIter must be >= 0");
-  if (!(tol >= 0.0)) return fail(c, SGP_E_BADARG, "requirement failed: tol must be >= 0");
-  if (n < 1 || d < 1) return fail(c, SGP_E_BADARG, "sgp_kmeans: no points or no features");
-  if (n > 2147483647LL) return fail(c, SGP_E_BADARG, "sgp_kmeans: n too large for one device");
-  if (init_centers)
-    for (size_t i = 0; i < static_cast<size_t>(k) * d; ++i)
-      if (!std::isfinite(init_centers[i])) return fail(c, SGP_E_BADARG, "sgp_kmeans: initial centres contain NaN or infinity");
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  static_assert(sizeof(int) == sizeof(int32_t), "label type");
-  return run_kmeans(c, X, x_is_f32, n, d, k, max_iter, tol, static_cast<uint64_t>(seed), init_centers, centers_out, k_out,
-                    labels_out, iterations_out, cost_out);
+  return kmeans(c, false, X, x_is_f32, n, d, k, max_iter, tol, seed, init_centers, centers_out, k_out, labels_out,
+                iterations_out, cost_out, "sgp_kmeans");
+}
+
+int sgp_kmeans_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, int64_t n, int32_t d, int32_t k, int32_t max_iter,
+                      double tol, int64_t seed, const double* init_centers, double* centers_out, int32_t* k_out,
+                      int32_t* labels_out, int32_t* iterations_out, double* cost_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return kmeans(c, true, dX, x_is_f32, n, d, k, max_iter, tol, seed, init_centers, centers_out, k_out, labels_out,
+                iterations_out, cost_out, "sgp_kmeans_device");
 }
 
 int sgp_cross_kernel(sgp_ctx* h, const double* X, int64_t n, double* K_out) {

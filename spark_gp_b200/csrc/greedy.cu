@@ -152,11 +152,12 @@ bool chol_inverse(const std::vector<double>& A, int n, int ld, std::vector<doubl
 }  // namespace
 
 int run_greedy(Ctx* c, const KernelFlat& kf, const std::vector<double>& beta_flat /*[n_terms][d]*/, const double* X,
-               const double* y, long long n, int d, long long E, long long first_index, int m_target,
+               const double* y, bool x_on_device, long long n, int d, long long E, long long first_index, int m_target,
                long long* indices_out) {
   const size_t N = static_cast<size_t>(n);
-  // ---- device state: X, y, K_mn (row per selected point), p, q, mu, delta, [t~ t], per-expert folds --------------------
-  const size_t bytes = (N * d + N + static_cast<size_t>(m_target) * N + 4 * N + 2 * N) * 8 +
+  // ---- device state: X, y (host input only), K_mn (row per selected point), p, q, mu, delta, [t~ t], per-expert folds --
+  const size_t xy = x_on_device ? 0 : N * d + N;
+  const size_t bytes = (xy + static_cast<size_t>(m_target) * N + 4 * N + 2 * N) * 8 +
                        static_cast<size_t>(E) * 16 + static_cast<size_t>(kMaxTerms) * d * 8 +
                        static_cast<size_t>(m_target) * 2 * 8 + static_cast<size_t>(m_target + 1) * 8 + 64;
   size_t free_b = 0, total_b = 0;
@@ -165,9 +166,10 @@ int run_greedy(Ctx* c, const KernelFlat& kf, const std::vector<double>& beta_fla
     return fail(c, SGP_E_NOMEM, "sgp_greedy_active_set: the N x m cross kernel does not fit in device memory");
   int rc = ctx_scratch(c, c->greedy_ws, bytes);
   if (rc != SGP_OK) return rc;
-  double* dX = static_cast<double*>(c->greedy_ws.p);
-  double* dy = dX + N * d;
-  double* Kt = dy + N;                                   // [m_target][N]
+  double* ws = static_cast<double*>(c->greedy_ws.p);
+  const double* dX = x_on_device ? X : ws;
+  const double* dy = x_on_device ? y : ws + N * d;
+  double* Kt = ws + xy;                                  // [m_target][N]
   double* dp = Kt + static_cast<size_t>(m_target) * N;
   double* dq = dp + N;
   double* dmu = dq + N;
@@ -180,8 +182,10 @@ int run_greedy(Ctx* c, const KernelFlat& kf, const std::vector<double>& beta_fla
   double* dg = dU + static_cast<size_t>(m_target) * 2;   // [m_target + 1]
   long long* dsel = reinterpret_cast<long long*>(dg + m_target + 1);
   cudaStream_t s = c->stream;
-  SGP_CUDA(c, cudaMemcpyAsync(dX, X, N * d * 8, cudaMemcpyHostToDevice, s));
-  SGP_CUDA(c, cudaMemcpyAsync(dy, y, N * 8, cudaMemcpyHostToDevice, s));
+  if (!x_on_device) {
+    SGP_CUDA(c, cudaMemcpyAsync(ws, X, N * d * 8, cudaMemcpyHostToDevice, s));
+    SGP_CUDA(c, cudaMemcpyAsync(ws + N * d, y, N * 8, cudaMemcpyHostToDevice, s));
+  }
   SGP_CUDA(c, cudaMemcpyAsync(dbeta, beta_flat.data(), beta_flat.size() * 8, cudaMemcpyHostToDevice, s));
   SGP_CUDA(c, cudaMemsetAsync(dp, 0, 3 * N * 8, s));      // p, q, mu
   SGP_BLAS(c, cublasSetStream(c->blas, s));

@@ -328,6 +328,17 @@ __global__ void __launch_bounds__(kPPThreads) kmeans_pp_kernel(const double* __r
 
 unsigned blocks(long long n, int t) { return static_cast<unsigned>((n + t - 1) / t); }
 
+// out[q][j] = X[idx[q]][j] as fp64: the rows the host reads (candidates, the origin's fallback) when X is device memory
+template <typename T>
+__global__ void __launch_bounds__(256) kmeans_gather_rows_kernel(const T* __restrict__ X, int d,
+                                                                 const long long* __restrict__ idx, int m,
+                                                                 double* __restrict__ out) {
+  const long long t = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  if (t >= static_cast<long long>(m) * d) return;
+  const int q = static_cast<int>(t / d), j = static_cast<int>(t % d);
+  out[t] = static_cast<double>(X[static_cast<size_t>(idx[q]) * d + j]);
+}
+
 // bump allocator over one scratch block (256-byte aligned pieces)
 struct Carve {
   char* base;
@@ -348,7 +359,8 @@ int label_bits(int k) {
 template <typename T>
 struct KMeansRun {
   Ctx* c;
-  const T* X;      // host
+  const T* X;      // host, or device memory where on_device
+  bool on_device;
   int n, d, k;
   uint64_t seed;
   cudaStream_t s;
@@ -415,7 +427,7 @@ struct KMeansRun {
     rows_per_slice = (n + slices - 1) / slices;
     const size_t N = static_cast<size_t>(n);
     auto carve = [&](Carve& cv) {
-      dX = cv.take<T>(N * d);
+      dX = cv.take<T>(on_device ? 0 : N * d);
       label = cv.take<int>(N); iota = cv.take<int>(N); sel = cv.take<int>(N); keys = cv.take<int>(N); vals = cv.take<int>(N);
       dist = cv.take<double>(N); cost = cv.take<double>(N); flag = cv.take<unsigned char>(N);
       part = cv.take<double>(std::max<size_t>(static_cast<size_t>(slices) * 2 * d, kSumBlocks));
@@ -428,6 +440,7 @@ struct KMeansRun {
     if (rc != SGP_OK) return rc;
     Carve real{static_cast<char*>(c->kmeans_pts_ws.p)};
     carve(real);
+    if (on_device) dX = const_cast<T*>(X);     // read in place, never written
     const size_t K = static_cast<size_t>(k);
     auto carve_c = [&](Carve& cv) {
       Cc = cv.take<double>(K * d); wsum = cv.take<double>(K);
@@ -446,7 +459,7 @@ struct KMeansRun {
   // the data's origin: per column the fp64 mean rounded to a multiple of the largest power of two not above the column's
   // standard deviation (so that the shift is exact for integer data), or the first point's coordinate for a constant column
   int origin() {
-    SGP_CUDA(c, cudaMemcpyAsync(dX, X, static_cast<size_t>(n) * d * sizeof(T), cudaMemcpyHostToDevice, s));
+    if (!on_device) SGP_CUDA(c, cudaMemcpyAsync(dX, X, static_cast<size_t>(n) * d * sizeof(T), cudaMemcpyHostToDevice, s));
     SGP_CUDA(c, cudaMemsetAsync(ints, 0, 8 * sizeof(int), s));
     kmeans_colstats_kernel<T><<<slices, 256, 0, s>>>(dX, n, d, rows_per_slice, part, ints);
     SGP_CUDA(c, cudaGetLastError());
@@ -457,7 +470,9 @@ struct KMeansRun {
     SGP_CUDA(c, cudaMemcpyAsync(&bad, ints, sizeof(int), cudaMemcpyDeviceToHost, s));
     SGP_CUDA(c, cudaStreamSynchronize(s));
     if (bad) return fail(c, SGP_E_BADARG, "sgp_kmeans: X contains NaN or infinity");
-    std::vector<double> oh(d);
+    std::vector<double> oh(d), x0(d);
+    const int rc = rows({0}, x0.data());
+    if (rc != SGP_OK) return rc;
     for (int j = 0; j < d; ++j) {
       double a = 0.0, b = 0.0;
       for (int q = 0; q < slices; ++q) { a += h[static_cast<size_t>(q) * 2 * d + j]; b += h[static_cast<size_t>(q) * 2 * d + d + j]; }
@@ -466,15 +481,32 @@ struct KMeansRun {
         const double q = std::ldexp(1.0, std::ilogb(sd));
         oh[j] = std::nearbyint(mean / q) * q;
       } else {
-        oh[j] = static_cast<double>(X[j]);
+        oh[j] = x0[j];
       }
     }
     SGP_CUDA(c, cudaMemcpyAsync(o, oh.data(), static_cast<size_t>(d) * 8, cudaMemcpyHostToDevice, s));
     return SGP_OK;
   }
 
-  void row(long long i, double* out) const {
-    for (int j = 0; j < d; ++j) out[j] = static_cast<double>(X[static_cast<size_t>(i) * d + j]);
+  // the rows idx of X as fp64, row after row, into host memory
+  int rows(const std::vector<long long>& idx, double* out) {
+    if (!on_device) {
+      for (size_t q = 0; q < idx.size(); ++q)
+        for (int j = 0; j < d; ++j) out[q * d + j] = static_cast<double>(X[static_cast<size_t>(idx[q]) * d + j]);
+      return SGP_OK;
+    }
+    const size_t m = idx.size(), ib = (m * 8 + 255) / 256 * 256;
+    int rc = ctx_scratch(c, c->kmeans_rows_ws, ib + m * d * 8);
+    if (rc != SGP_OK) return rc;
+    long long* didx = static_cast<long long*>(c->kmeans_rows_ws.p);
+    double* drows = reinterpret_cast<double*>(static_cast<char*>(c->kmeans_rows_ws.p) + ib);
+    SGP_CUDA(c, cudaMemcpyAsync(didx, idx.data(), m * 8, cudaMemcpyHostToDevice, s));
+    kmeans_gather_rows_kernel<T><<<blocks(static_cast<long long>(m) * d, 256), 256, 0, s>>>(X, d, didx, static_cast<int>(m),
+                                                                                          drows);
+    SGP_CUDA(c, cudaGetLastError());
+    c->launches += 1;
+    SGP_CUDA(c, cudaMemcpyAsync(out, drows, m * d * 8, cudaMemcpyDeviceToHost, s));
+    return sync();
   }
 
   // k-means|| (KMeans.initKMeansParallel) then, for more than k distinct candidates, the local weighted k-means++ and its
@@ -491,9 +523,10 @@ struct KMeansRun {
       const int m = static_cast<int>(new_idx.size());
       if (m > 0) {
         rows.resize(static_cast<size_t>(m) * d);
-        for (int q = 0; q < m; ++q) row(new_idx[q], rows.data() + static_cast<size_t>(q) * d);
+        int rc = this->rows(new_idx, rows.data());
+        if (rc != SGP_OK) return rc;
         const size_t img = (static_cast<size_t>(rows_pad(m)) * cstride(d) * 4 + 255) / 256 * 256;
-        int rc = ctx_scratch(c, c->kmeans_new_ws, img + rows.size() * 8);
+        rc = ctx_scratch(c, c->kmeans_new_ws, img + rows.size() * 8);
         if (rc != SGP_OK) return rc;
         float* F = static_cast<float*>(c->kmeans_new_ws.p);
         double* R = reinterpret_cast<double*>(static_cast<char*>(c->kmeans_new_ws.p) + img);
@@ -521,10 +554,12 @@ struct KMeansRun {
       cand_idx.insert(cand_idx.end(), new_idx.begin(), new_idx.end());
     }
     // distinct candidates, first occurrence kept (-0.0 and 0.0 are equal)
-    std::vector<double> cand, r(d);
+    std::vector<double> cand, all(cand_idx.size() * d), r(d);
     std::unordered_set<std::string> seen;
-    for (long long i : cand_idx) {
-      row(i, r.data());
+    int rc = this->rows(cand_idx, all.data());
+    if (rc != SGP_OK) return rc;
+    for (size_t q = 0; q < cand_idx.size(); ++q) {
+      std::copy(all.begin() + q * d, all.begin() + (q + 1) * d, r.begin());
       std::string key(reinterpret_cast<const char*>(r.data()), static_cast<size_t>(d) * 8);
       for (int j = 0; j < d; ++j) {
         const double z = r[j] + 0.0;
@@ -555,7 +590,7 @@ struct KMeansRun {
     };
     Carve probe{nullptr};
     carve(probe);
-    int rc = ctx_scratch(c, c->kmeans_cand_ws, probe.off);
+    rc = ctx_scratch(c, c->kmeans_cand_ws, probe.off);
     if (rc != SGP_OK) return rc;
     Carve real{static_cast<char*>(c->kmeans_cand_ws.p)};
     carve(real);
@@ -639,14 +674,14 @@ struct KMeansRun {
 
 }  // namespace
 
-int run_kmeans(Ctx* c, const void* X, int x_is_f32, long long n, int d, int k, int max_iter, double tol, uint64_t seed,
-               const double* init_centers, double* centers_out, int* k_out, int* labels_out, int* iterations_out,
-               double* cost_out) {
+int run_kmeans(Ctx* c, const void* X, int x_is_f32, bool x_on_device, long long n, int d, int k, int max_iter, double tol,
+               uint64_t seed, const double* init_centers, double* centers_out, int* k_out, int* labels_out,
+               int* iterations_out, double* cost_out) {
   if (x_is_f32) {
-    KMeansRun<float> r{c, static_cast<const float*>(X), static_cast<int>(n), d, k, seed, c->stream};
+    KMeansRun<float> r{c, static_cast<const float*>(X), x_on_device, static_cast<int>(n), d, k, seed, c->stream};
     return r.run(max_iter, tol, init_centers, centers_out, k_out, labels_out, iterations_out, cost_out);
   }
-  KMeansRun<double> r{c, static_cast<const double*>(X), static_cast<int>(n), d, k, seed, c->stream};
+  KMeansRun<double> r{c, static_cast<const double*>(X), x_on_device, static_cast<int>(n), d, k, seed, c->stream};
   return r.run(max_iter, tol, init_centers, centers_out, k_out, labels_out, iterations_out, cost_out);
 }
 

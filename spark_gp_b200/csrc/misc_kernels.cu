@@ -130,6 +130,15 @@ __global__ void group_experts_kernel(double* __restrict__ Xe, double* __restrict
   if (k == 0) ye[dst] = y[li];
 }
 
+// One thread per point: the inverse of group_experts_kernel's permutation (without skipped points).
+__global__ void ungroup_experts_kernel(double* __restrict__ out, const double* __restrict__ f, long long n, long long E) {
+  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const long long e = i % E, pos = i / E;
+  const long long kq = n / E, r = n % E;
+  out[i] = f[e * kq + (e < r ? e : r) + pos];
+}
+
 __global__ void expert_offsets_kernel(long long* __restrict__ off, long long n, long long E, long long base) {
   const long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   if (e > E) return;
@@ -187,6 +196,11 @@ cudaError_t launch_group_experts(double* Xe, double* ye, const void* dX, int x_i
   const long long total = cn * d;
   group_experts_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(Xe, ye, dX, x_is_f32, dy, n, d, E, p0, cn,
                                                                                   skip_pos, n_skip);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_ungroup_experts(double* out, const double* f, long long n, long long E, cudaStream_t s) {
+  ungroup_experts_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(out, f, n, E);
   return cudaGetLastError();
 }
 

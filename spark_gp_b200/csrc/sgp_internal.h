@@ -130,6 +130,7 @@ struct Ctx {
   cudaEvent_t tail_fork = nullptr, tail_join = nullptr;
   DevScratch tail_ws, tail_ws2, predict_ws, cross_ws, bcm_ws, sweep_ws, greedy_ws;
   DevScratch kmeans_pts_ws, kmeans_cen_ws, kmeans_new_ws, kmeans_cand_ws;   // sgp_kmeans: point-, centre-, candidate-sized
+  DevScratch kmeans_rows_ws;           // sgp_kmeans_device: indices and fp64 copies of the rows the host reads
   bool has_magic_run = false;
   bool tail_fast = false;              // last sgp_magic took the Cholesky path for both matrices
   ncclComm_t comm = nullptr;
@@ -174,6 +175,7 @@ struct Ctx {
   int ex_classes = 0;            // classes ex_fc holds modes for; 0: none since the last upload
   DevScratch ex_fm;              // param-map latent modes [ex_mode_slots][n] (sgp_laplace_nll_slots_any_size)
   int ex_mode_slots = 0;         // mode slots ex_fm holds modes for; 0: none since the last upload
+  bool ex_grouped = false;       // ex came from a grouped upload (point i -> expert i % E): its modes can be ungrouped
   // fold upload (sgp_experts_upload_folds): the training sets lie one after another in ex; set k owns the experts
   // fold_first[k] .. fold_first[k+1]-1.  Empty after any other upload.
   std::vector<long long> fold_first;   // [n_sets + 1]
@@ -240,6 +242,8 @@ cudaError_t launch_magic_matrix(double* out, const double* invA, const double* i
 cudaError_t launch_group_experts(double* Xe, double* ye, const void* dX, int x_is_f32, const double* dy, long long n, int d,
                                  long long E, long long p0, long long cn, const long long* skip_pos, long long n_skip,
                                  cudaStream_t s);
+// The inverse of the grouping: out[i] = f[row of point i], point i being expert i % E's (i / E)-th point.
+cudaError_t launch_ungroup_experts(double* out, const double* f, long long n, long long E, cudaStream_t s);
 // off[e] = base + start of expert e of n points grouped into E experts, e = 0 .. E
 cudaError_t launch_expert_offsets(long long* off, long long n, long long E, long long base, cudaStream_t s);
 cudaError_t launch_status_to_double(double* dst, const int* flags, int mask, const double* norm_sum, double norm_limit,
@@ -383,13 +387,15 @@ cudaError_t launch_laplace_global(const ExpertSet& ex, const HyperView& hv, doub
                                   const LaplaceClasses* classes = nullptr);
 
 int ctx_scratch(Ctx* c, DevScratch& s, size_t bytes);
+// X and y below are host memory, or device memory on the context's device where x_on_device is set (the _device entries)
 // csrc/greedy.cu: forward selection with rank-1 updates (ActiveSetProvider.scala:58-139); beta_flat = [n_terms][d]
 int run_greedy(Ctx* c, const KernelFlat& kf, const std::vector<double>& beta_flat, const double* X, const double* y,
-               long long n, int d, long long n_experts, long long first_index, int m_target, long long* indices_out);
+               bool x_on_device, long long n, int d, long long n_experts, long long first_index, int m_target,
+               long long* indices_out);
 // csrc/kmeans.cu: Spark 3.1 MLlib KMeans (k-means|| + Lloyd) for KMeansActiveSetProvider (ActiveSetProvider.scala:22-46)
-int run_kmeans(Ctx* c, const void* X, int x_is_f32, long long n, int d, int k, int max_iter, double tol, uint64_t seed,
-               const double* init_centers, double* centers_out, int* k_out, int* labels_out, int* iterations_out,
-               double* cost_out);
+int run_kmeans(Ctx* c, const void* X, int x_is_f32, bool x_on_device, long long n, int d, int k, int max_iter, double tol,
+               uint64_t seed, const double* init_centers, double* centers_out, int* k_out, int* labels_out,
+               int* iterations_out, double* cost_out);
 int run_tail(Ctx* c, double* magic_vector, double* magic_matrix);
 // Prediction (tail.cu): predict_prepare sizes the workspace and packs the installed magic matrix (once per pair) for the
 // windows that follow; predict_window enqueues one window of at most predict_window_points(m_pad) device-resident points.

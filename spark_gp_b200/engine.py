@@ -40,6 +40,66 @@ def is_cuda_tensor(x) -> bool:
     return type(x).__module__.partition(".")[0] == "torch" and bool(getattr(x, "is_cuda", False))
 
 
+def device_tensor(X, device: int, what: str, dtype=None):
+    """A CUDA torch tensor as the library reads it on cuda:`device`: float32 and float64 as given (or `dtype` when given),
+    other dtypes converted to float64, contiguous.  Synchronises torch's current stream, so that whatever torch still has
+    queued for the tensor is written before the library's stream reads it.  ValueError for a tensor on another device."""
+    import torch
+    if X.device.type != "cuda" or X.device.index != device:
+        raise ValueError("%s: the tensor is on %s, the model on cuda:%d" % (what, X.device, device))
+    if dtype is not None:
+        X = X.to(dtype)
+    elif X.dtype not in (torch.float32, torch.float64):
+        X = X.to(torch.float64)
+    X = X.contiguous()
+    torch.cuda.current_stream(X.device).synchronize()
+    return X
+
+
+def device_fit_data(X, y, device: int, what: str):
+    """The (X, y) of a fit from a CUDA tensor X: ValueError, before anything runs on the device, for X on another device
+    than cuda:`device` or not n x d, and for y on another device than X or not n entries.  y may be a host vector; it
+    becomes a CUDA float64 vector.  X keeps its dtype (`device_tensor` converts it where the library reads it)."""
+    import torch
+    if X.device.type != "cuda" or X.device.index != device:
+        raise ValueError("%s: X is on %s, the estimator on cuda:%d" % (what, X.device, device))
+    if X.ndim != 2:
+        raise ValueError("%s: X must be n x d" % what)
+    if isinstance(y, torch.Tensor):
+        if y.device != X.device:
+            raise ValueError("%s: y is on %s, X on %s" % (what, y.device, X.device))
+        y = y.to(torch.float64)
+    else:
+        y = torch.as_tensor(np.asarray(y, dtype=np.float64), device=X.device)
+    if y.ndim != 1 or len(y) != len(X):
+        raise ValueError("%s: y must hold one label per row of X (%d), not shape %s" % (what, len(X), tuple(y.shape)))
+    return X, y
+
+
+def take_rows(X, idx):
+    """X[idx] on X's side: a numpy array, or a CUDA tensor gathered on the device (nothing crosses PCIe but idx)."""
+    if is_cuda_tensor(X):
+        import torch
+        return X[torch.as_tensor(np.asarray(idx, dtype=np.int64), device=X.device)]
+    return np.asarray(X)[idx]
+
+
+def rows_to_host(X, idx):
+    """X[idx] as a float64 host array: for a CUDA tensor only these rows cross PCIe."""
+    if is_cuda_tensor(X):
+        import torch
+        return take_rows(X, idx).to(torch.float64).cpu().numpy()
+    return np.asarray(np.asarray(X)[idx], dtype=np.float64)
+
+
+def host_copy(x):
+    """An explicit float64 host copy of a CUDA tensor, for the algorithms that run on the host; host arrays pass as they
+    are."""
+    if is_cuda_tensor(x):
+        return np.asarray(x.cpu().numpy(), dtype=np.float64)
+    return x
+
+
 def _rows(X):
     """Points as the library reads them: float32 stays as it is (no copy when already contiguous), anything else becomes
     float64; C-contiguous."""
@@ -179,13 +239,27 @@ class ProjectedProcessEngine:
         self._check(self._lib.sgp_sync(self._h))
 
     def statistics(self, kernel: Kernel, active_set, X, y, shard_points: int = 1 << 22):
-        """`getMatrixKmnKnmAndVectorKmny` over host data in shards (PGPH:23 broadcast, PGPH:25-35 seqOp over shards).
-        When the int8 path reports SGP_E_RANGE (coordinates outside its operand range, or AUTO's magnitude
-        budget exceeded over the whole window) the pass is repeated on the fp64 DMMA kernel -- still on the GPU."""
+        """`getMatrixKmnKnmAndVectorKmny` over host data in shards (PGPH:23 broadcast, PGPH:25-35 seqOp over shards), or
+        over a CUDA tensor X (and y) in one `sgp_stats_accumulate_device` call: the library cuts its own launch windows,
+        so shard_points applies to host data only.  When the int8 path reports SGP_E_RANGE (coordinates outside its
+        operand range, or AUTO's magnitude budget exceeded over the whole window) the pass is repeated on the fp64 DMMA
+        kernel -- still on the GPU."""
+        if is_cuda_tensor(X):
+            import torch
+            X = device_tensor(X, self._device, "statistics")
+            y = device_tensor(y, self._device, "statistics", torch.float64)
+            if X.ndim != 2 or y.shape != (len(X),):
+                raise ValueError("statistics: X must be n x d and y n entries")
+
         def run():
             self.begin(kernel, active_set)
-            for s in range(0, len(X), shard_points):
-                self.accumulate(X[s:s + shard_points], y[s:s + shard_points])
+            if is_cuda_tensor(X):
+                if X.shape[1] != self.d:
+                    raise ValueError("shard shape mismatch")
+                self.accumulate_ptr(X.data_ptr(), X.dtype == torch.float32, y.data_ptr(), len(X), device=True)
+            else:
+                for s in range(0, len(X), shard_points):
+                    self.accumulate(X[s:s + shard_points], y[s:s + shard_points])
             return self.finish()
         try:
             return run()
@@ -204,13 +278,26 @@ class ProjectedProcessEngine:
         self._check(self._lib.sgp_experts_upload(self._h, N.ptr(X), N.ptr(y), N.ptr(off), len(off) - 1, X.shape[1]))
         self._experts_d = X.shape[1]
 
+    def _device_xy(self, X, y, what):
+        """(X, y) of a device entry: X as `device_tensor` reads it, y float64, each with its pointer."""
+        import torch
+        X = device_tensor(X, self._device, what)
+        y = device_tensor(y, self._device, what, torch.float64)
+        return X, y, C.c_void_p(X.data_ptr()), C.c_void_p(y.data_ptr()), int(X.dtype == torch.float32)
+
     def experts_upload_grouped(self, X, y, dataset_size_for_expert: int):
         """Groups the points into experts ON THE DEVICE (GPC:26-31: point i -> expert i % E) while they stream in; X may be
-        float32 or float64, row-major as given.  Returns the number of experts."""
-        X = _rows(X)
-        y =np.ascontiguousarray(y, dtype=np.float64)
-        self._check(self._lib.sgp_experts_upload_grouped(self._h, N.ptr(X), int(X.dtype == np.float32), N.ptr(y), len(X),
-                                                         X.shape[1], int(dataset_size_for_expert)))
+        float32 or float64, row-major as given.  A CUDA tensor X (and y) is read in place
+        (`sgp_experts_upload_grouped_device`): the same experts, bit for bit.  Returns the number of experts."""
+        if is_cuda_tensor(X):
+            X, y, px, py, f32 = self._device_xy(X, y, "experts_upload_grouped")
+            self._check(self._lib.sgp_experts_upload_grouped_device(self._h, px, f32, py, len(X), X.shape[1],
+                                                                    int(dataset_size_for_expert)))
+        else:
+            X = _rows(X)
+            y =np.ascontiguousarray(y, dtype=np.float64)
+            self._check(self._lib.sgp_experts_upload_grouped(self._h, N.ptr(X), int(X.dtype == np.float32), N.ptr(y),
+                                                             len(X), X.shape[1], int(dataset_size_for_expert)))
         self._experts_d = X.shape[1]
         return int(np.floor(len(X) / dataset_size_for_expert + 0.5))
 
@@ -260,15 +347,19 @@ class ProjectedProcessEngine:
     def experts_upload_folds(self, X, y, fold_of, n_folds: int, dataset_size_for_expert: int):
         """Uploads the training set of every fold of a k-fold split (`sgp_experts_upload_folds`): set k holds the points
         with fold_of != k in index order, grouped into experts as `experts_upload_grouped` groups them.  X may be float32
-        or float64.  Returns the number of experts of each set."""
-        X = _rows(X)
-        y =np.ascontiguousarray(y, dtype=np.float64)
+        or float64; a CUDA tensor X (and y) is read in place (`sgp_experts_upload_folds_device`), fold_of stays a host
+        array.  Returns the number of experts of each set."""
         folds = np.ascontiguousarray(fold_of, dtype=np.int32)
+        if is_cuda_tensor(X):
+            X, y, px, py, f32 = self._device_xy(X, y, "experts_upload_folds")
+            fn = self._lib.sgp_experts_upload_folds_device
+        else:
+            X = _rows(X)
+            y =np.ascontiguousarray(y, dtype=np.float64)
+            px, py, f32, fn = N.ptr(X), N.ptr(y), int(X.dtype == np.float32), self._lib.sgp_experts_upload_folds
         if X.ndim != 2 or len(y) != len(X) or folds.shape != (len(X),):
             raise ValueError("experts_upload_folds: X must be n x d, y and fold_of n entries")
-        self._check(self._lib.sgp_experts_upload_folds(self._h, N.ptr(X), int(X.dtype == np.float32), N.ptr(y), len(X),
-                                                       X.shape[1], N.ptr(folds), int(n_folds),
-                                                       int(dataset_size_for_expert)))
+        self._check(fn(self._h, px, f32, py, len(X), X.shape[1], N.ptr(folds), int(n_folds), int(dataset_size_for_expert)))
         self._experts_d = X.shape[1]
         n_k = len(X) - np.bincount(folds, minlength=int(n_folds))
         return np.floor(n_k / dataset_size_for_expert + 0.5).astype(np.int64)
@@ -349,6 +440,23 @@ class ProjectedProcessEngine:
     def experts_f(self, n: int):
         return self._modes(self._lib.sgp_experts_get_f, n)
 
+    def experts_modes(self, store: int, index: int, n: int):
+        """The n modes of one store (N.SGP_MODES_BINARY / _CLASS / _SLOT, index: the class or mode slot), packed
+        expert-major, in host memory."""
+        if store == N.SGP_MODES_CLASS:
+            return self.experts_f_class(index, n)
+        if store == N.SGP_MODES_SLOT:
+            return self.experts_f_slot(index, n)
+        return self.experts_f(n)
+
+    def experts_modes_rows(self, store: int, index: int, n: int):
+        """`experts_modes` in ROW order as a CUDA float64 tensor on this context's device, ungrouped on the device
+        (`sgp_experts_get_f_rows_device`): the modes never leave it.  Needs a grouped upload of n points."""
+        import torch
+        f = torch.empty(n, dtype=torch.float64, device="cuda:%d" % self._device)
+        self._check(self._lib.sgp_experts_get_f_rows_device(self._h, int(store), int(index), C.c_void_p(f.data_ptr())))
+        return f
+
     def bcm_nll(self, kernel: Kernel):
         """(sum over experts of 1/2 y'K^-1 y + 1/2 log|K|, gradient w.r.t. kernel.getHyperparameters())."""
         return self._objective(self._lib.sgp_bcm_nll, kernel)
@@ -394,11 +502,7 @@ class ProjectedProcessEngine:
         """`predict` for a CUDA torch tensor on this context's device (n x d or d; float32 is read as it is, other dtypes
         are converted to float64): (mean, var or None) as CUDA float64 tensors of n entries, without a host round trip."""
         import torch
-        if X.device.type != "cuda" or X.device.index != self._device:
-            raise ValueError("predict: the tensor is on %s, the model on cuda:%d" % (X.device, self._device))
-        if X.dtype not in (torch.float32, torch.float64):
-            X = X.to(torch.float64)
-        X = X.contiguous()
+        X = device_tensor(X, self._device, "predict")       # X may still be written on torch's stream
         if X.ndim == 1:
             X = X[None, :]
         if X.ndim != 2 or X.shape[1] != self.d:
@@ -406,7 +510,6 @@ class ProjectedProcessEngine:
         n = X.shape[0]
         mean = torch.empty(n, dtype=torch.float64, device=X.device)
         var = torch.empty(n, dtype=torch.float64, device=X.device) if with_variance else None
-        torch.cuda.current_stream(X.device).synchronize()       # X may still be written on torch's stream
         self.predict_device(X.data_ptr(), X.dtype == torch.float32, n, mean.data_ptr(),
                             var.data_ptr() if var is not None else 0)
         self.sync()
@@ -423,21 +526,36 @@ class ProjectedProcessEngine:
 
     def greedy_active_set(self, kernel: Kernel, X, y, n_experts: int, first_index: int, m_target: int):
         """Row indices of the points GreedilyOptimizingActiveSetProvider selects (ActiveSetProvider.scala:58-139), computed
-        with rank-1 updates on the device (`sgp_greedy_active_set`): O(n m) per round instead of a statistics pass."""
-        X = np.ascontiguousarray(X, dtype=np.float64)
-        y = np.ascontiguousarray(y, dtype=np.float64)
+        with rank-1 updates on the device (`sgp_greedy_active_set`): O(n m) per round instead of a statistics pass.  A
+        CUDA tensor X (and y) is converted to float64 on the device and read in place (`sgp_greedy_active_set_device`)."""
+        if is_cuda_tensor(X):
+            import torch
+            X = device_tensor(X, self._device, "greedy_active_set", torch.float64)
+            y = device_tensor(y, self._device, "greedy_active_set", torch.float64)
+            px, py, fn = C.c_void_p(X.data_ptr()), C.c_void_p(y.data_ptr()), self._lib.sgp_greedy_active_set_device
+        else:
+            X = np.ascontiguousarray(X, dtype=np.float64)
+            y = np.ascontiguousarray(y, dtype=np.float64)
+            px, py, fn = N.ptr(X), N.ptr(y), self._lib.sgp_greedy_active_set
         desc, keep = _make_desc(kernel, X.shape[1])
         idx = np.empty(int(m_target), dtype=np.int64)
-        self._check(self._lib.sgp_greedy_active_set(self._h, C.byref(desc), N.ptr(X), N.ptr(y), len(X), X.shape[1],
-                                                    int(n_experts), int(first_index), int(m_target), N.ptr(idx)))
+        self._check(fn(self._h, C.byref(desc), px, py, len(X), X.shape[1], int(n_experts), int(first_index),
+                       int(m_target), N.ptr(idx)))
         del keep
         return idx
 
     def kmeans(self, X, k: int, max_iter: int = 20, tol: float = 1e-4, seed: int = 0, init_centers=None):
         """Spark 3.1 MLlib KMeans (k-means|| seeding, Lloyd iterations) on the device (`sgp_kmeans`): returns
         (centres [k_out x d] fp64, labels [n] int32, iterations, cost).  X: n x d, float32 (used without a copy) or
-        float64.  init_centers (k x d) replaces the seeding, as mllib's setInitialModel."""
-        X = _rows(X)
+        float64.  init_centers (k x d) replaces the seeding, as mllib's setInitialModel.  A CUDA tensor X is read in place
+        (`sgp_kmeans_device`): the same outputs, bit for bit."""
+        if is_cuda_tensor(X):
+            import torch
+            X = device_tensor(X, self._device, "kmeans")
+            px, f32, fn = C.c_void_p(X.data_ptr()), int(X.dtype == torch.float32), self._lib.sgp_kmeans_device
+        else:
+            X = _rows(X)
+            px, f32, fn = N.ptr(X), int(X.dtype == np.float32), self._lib.sgp_kmeans
         if X.ndim != 2:
             raise ValueError("X must be n x d")
         n, d = X.shape
@@ -451,9 +569,8 @@ class ProjectedProcessEngine:
         labels = np.empty(max(n, 1), dtype=np.int32)
         k_out, iters, cost = C.c_int32(), C.c_int32(), C.c_double()
         seed = C.c_int64(int(seed) & 0xFFFFFFFFFFFFFFFF).value
-        self._check(self._lib.sgp_kmeans(self._h, N.ptr(X), int(X.dtype == np.float32), n, d, k, int(max_iter), float(tol),
-                                         seed, N.ptr(init) if init is not None else None, N.ptr(centres), C.byref(k_out),
-                                         N.ptr(labels), C.byref(iters), C.byref(cost)))
+        self._check(fn(self._h, px, f32, n, d, k, int(max_iter), float(tol), seed, N.ptr(init) if init is not None else None,
+                       N.ptr(centres), C.byref(k_out), N.ptr(labels), C.byref(iters), C.byref(cost)))
         return np.ascontiguousarray(centres[:k_out.value]), labels[:n], iters.value, cost.value
 
     def kmn_sweep(self, X):

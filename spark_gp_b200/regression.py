@@ -12,7 +12,8 @@ import copy
 import numpy as np
 
 from . import _native as N
-from .engine import ProjectedProcessEngine, OperandRangeError, NotPositiveDefiniteException, is_cuda_tensor
+from .engine import ProjectedProcessEngine, OperandRangeError, NotPositiveDefiniteException, device_fit_data, host_copy, \
+    is_cuda_tensor, rows_to_host
 from .kernels import Kernel, RBFKernel, EyeKernel, const
 
 
@@ -26,11 +27,12 @@ class ActiveSetProvider:
 class _RandomActiveSetProvider(ActiveSetProvider):
     """commons/ActiveSetProvider.scala:48-56: uniform sample without replacement.  (Spark's `takeSample`
     RNG stream is not reproduced -- the reference pins no test on it; pass an explicit active set through
-    `ExplicitActiveSetProvider` when results must be compared.)"""
+    `ExplicitActiveSetProvider` when results must be compared.)  A CUDA tensor X gives the same rows, gathered on the
+    device: only they cross PCIe."""
     def __call__(self, activeSetSize, X, y, kernel_factory, optimalHyperparameter, seed, gp=None):
         rng = np.random.default_rng(seed)
         idx = rng.choice(len(X), size=min(activeSetSize, len(X)), replace=False)
-        return np.asarray(np.asarray(X)[idx], dtype=np.float64)     # index first: no fp64 copy of the whole shard
+        return rows_to_host(X, idx)                                 # index first: no fp64 copy of the whole shard
 
 
 RandomActiveSetProvider = _RandomActiveSetProvider()
@@ -53,7 +55,8 @@ class KMeansActiveSetProvider(ActiveSetProvider):
 
     `on_gpu=True` runs Spark's own algorithm on the device instead (`ProjectedProcessEngine.kmeans`, `sgp_kmeans`): k-means||
     seeding, empty clusters keep their centre, absolute centre-movement tolerance; float32 X is used without a copy.  May
-    return fewer than activeSetSize centres when the data have fewer distinct points, as Spark does."""
+    return fewer than activeSetSize centres when the data have fewer distinct points, as Spark does.  It reads a CUDA tensor
+    X in place (`sgp_kmeans_device`); scikit-learn runs on the host, on an explicit host copy of such an X."""
 
     def __init__(self, maxIter: int = 20, on_gpu: bool = False):
         self.maxIter = int(maxIter)
@@ -70,7 +73,7 @@ class KMeansActiveSetProvider(ActiveSetProvider):
         from sklearn.cluster import KMeans
         km = KMeans(n_clusters=int(activeSetSize), init="k-means++", n_init=1, max_iter=self.maxIter, tol=1e-4,
                     random_state=int(seed) % (2 ** 32), algorithm="lloyd")
-        km.fit(np.asarray(X, dtype=np.float64))
+        km.fit(np.asarray(host_copy(X), dtype=np.float64))
         return np.ascontiguousarray(km.cluster_centers_, dtype=np.float64)
 
 
@@ -89,7 +92,9 @@ class GreedilyOptimizingActiveSetProvider(ActiveSetProvider):
     `incremental=True` (default) runs the whole selection in `sgp_greedy_active_set`: the N x m cross kernel stays on the
     device and p_i, q_i, mu_i and the two inverses follow from rank-1 (bordered-matrix) updates -- O(N m) per round, all
     in fp64; `incremental=False` is the round-by-round form above (kept as the cross-check: both must select the points
-    the CPU restatement selects)."""
+    the CPU restatement selects).  On a CUDA tensor X the incremental selection converts X to float64 on the device and
+    reads it in place (`sgp_greedy_active_set_device`), only the selected rows cross PCIe; the round-by-round form runs on
+    an explicit host copy."""
 
     def __init__(self, first_index=None, precision=None, incremental=True):
         self.first_index = first_index
@@ -97,22 +102,25 @@ class GreedilyOptimizingActiveSetProvider(ActiveSetProvider):
         self.incremental = incremental
 
     def __call__(self, activeSetSize, X, y, kernel_factory, optimalHyperparameter, seed, gp=None):
-        X64 = np.ascontiguousarray(X, dtype=np.float64)
-        y = np.asarray(y, dtype=np.float64)
+        if is_cuda_tensor(X) and not self.incremental:
+            X, y = host_copy(X), host_copy(y)
+        on_device = is_cuda_tensor(X)
+        X64 = X if on_device else np.ascontiguousarray(X, dtype=np.float64)
+        y = y if on_device else np.asarray(y, dtype=np.float64)
         n = len(X64)
         n_e = gp._datasetSizeForExpert if gp is not None else 100
         E = int(np.floor(n / n_e + 0.5))
         if E <= 0:
             raise ZeroDivisionError("numberOfExperts == 0 (N < datasetSizeForExpert / 2)")
         first = self.first_index if self.first_index is not None else int(np.random.default_rng(seed).integers(n))
-        active = X64[[first]].copy()
         theta = np.asarray(optimalHyperparameter, dtype=np.float64)
         eng = ProjectedProcessEngine.acquire(gp._device if gp is not None else 0)
         eng.set_precision(N.SGP_PREC_F64 if self.precision is None else self.precision)
         try:
             if self.incremental:
                 kernel = kernel_factory().setHyperparameters(theta)
-                return X64[eng.greedy_active_set(kernel, X64, y, E, first, activeSetSize)]
+                return rows_to_host(X64, eng.greedy_active_set(kernel, X64, y, E, first, activeSetSize))
+            active = X64[[first]].copy()
             while len(active) < activeSetSize:
                 kernel = kernel_factory().setHyperparameters(theta)
                 active = np.vstack([active, self._get_next(eng, kernel, X64, y, active, E)])
@@ -269,9 +277,14 @@ class GaussianProcessRegression(GaussianProcessParams):
 
     def fit(self, X, y, hyperparameters=None) -> GaussianProcessRegressionModel:
         """GPR.train (:43-53).  `hyperparameters` short-circuits optimizeHypers (:48) with a given theta;
-        otherwise the BCM objective is optimised when maxIter > 0."""
-        X = np.asarray(X)
-        y = np.asarray(y, dtype=np.float64)
+        otherwise the BCM objective is optimised when maxIter > 0.
+        X may be a CUDA tensor on the estimator's device (y a CUDA tensor there too, or a host vector): X then never
+        leaves the device; only the active set's rows and the small outputs cross PCIe."""
+        if is_cuda_tensor(X):
+            X, y = device_fit_data(X, y, self._device, "GaussianProcessRegression.fit")
+        else:
+            X = np.asarray(X)
+            y = np.asarray(y, dtype=np.float64)
         if hyperparameters is None:
             if self._maxIter > 0:
                 from .hyperopt import optimize_hypers     # per-expert BCM NLL on the GPU + L-BFGS-B on the host

@@ -33,14 +33,20 @@ Over the binary classifier and one-vs-rest, the maps are grouped by `slot_group_
 training rows are uploaded once, and every (map p, class c) is one slot with mode slot p * C + c (binary: C = 1, class 1)
 in `sgp_laplace_nll_slots_any_size`, so each round of the slots' L-BFGS-B runs is one launch.  Each slot's values and
 modes equal the independent fit's bit for bit, so every validation prediction is that of
-`estimator.copy(map).fit(X[train], y[train])`.  Regression maps are fitted one after another."""
+`estimator.copy(map).fit(X[train], y[train])`.  Regression maps are fitted one after another.
+
+Both selectors take X (and y) as CUDA tensors on the estimator's device as well: the fold upload reads them in place
+(`sgp_experts_upload_folds_device`), the training and validation rows are gathered on the device and predicted there, and
+only the validation labels and predictions go to the host, for the evaluator.  `folds=` and `train=` stay host arrays.
+The results are the host fit's, bit for bit."""
 from __future__ import annotations
 
 import numpy as np
 
-from .classification import GaussianProcessClassifier, OneVsRest, _produce_model, laplace_fit, one_vs_rest_labels, \
-    one_vs_rest_prediction
-from .engine import ProjectedProcessEngine
+from . import _native as N
+from .classification import GaussianProcessClassifier, OneVsRest, _produce_model, assert_labels_are_01, laplace_fit, \
+    one_vs_rest_labels, one_vs_rest_prediction
+from .engine import ProjectedProcessEngine, device_fit_data, host_copy, is_cuda_tensor, take_rows
 from .hyperopt import lbfgsb_bounds, optimise_slots
 from .regression import GaussianProcessRegression
 from .utils import kfold_assignment, train_validation_assignment
@@ -216,12 +222,24 @@ class _Validator:
         self._seed = int(value)
         return self
 
-    def _data(self, X, y):
+    def _data(self, X, y, device: int):
+        if is_cuda_tensor(X):
+            return device_fit_data(X, y, device, self.NAME + ".fit")
         X = np.asarray(X)
         y = np.asarray(y, dtype=np.float64)
         if X.ndim != 2 or len(y) != len(X):
             raise ValueError("%s: X must be n x d and y n labels" % self.NAME)
         return X, y
+
+
+def _rows(X, mask):
+    """The rows of X where the host bool mask is set, on X's side."""
+    return take_rows(X, np.flatnonzero(mask))
+
+
+def _host_predictions(p):
+    """A model's predictions as the evaluator reads them (host float64)."""
+    return np.asarray(host_copy(p), dtype=np.float64)
 
 
 class CrossValidatorModel(_SelectedModel):
@@ -270,7 +288,7 @@ class CrossValidator(_Validator):
         est = self._estimator
         if est is None:
             raise TypeError("CrossValidator: setEstimator(GaussianProcessRegression) first")
-        X, y = self._data(X, y)
+        X, y = self._data(X, y, est._device)
         K = self._num_folds
         if folds is None:
             fold_of = kfold_assignment(len(X), K, self._seed)
@@ -290,10 +308,10 @@ class CrossValidator(_Validator):
         for p, e in enumerate(ests):
             for k in range(K):
                 train, val = fold_of != k, fold_of == k
-                model = e._produce_model(X[train], y[train], thetas[p][k])
-                pred = model.predict(X[val])
+                model = e._produce_model(_rows(X, train), _rows(y, train), thetas[p][k])
+                pred = _host_predictions(model.predict(_rows(X, val)))
                 folds_out[p, k] = dict(theta=thetas[p][k], magicVector=model.rawPredictor.magicVector, prediction=pred)
-                metrics[p, k] = self._evaluator.evaluate(y[val], pred)
+                metrics[p, k] = self._evaluator.evaluate(host_copy(_rows(y, val)), pred)
                 del model                         # its context goes back to the pool before the next slot
         avg = [sum(metrics[p, k] for k in range(K)) / K for p in range(len(maps))]
         best = best_index(avg, self._evaluator.isLargerBetter())
@@ -384,7 +402,8 @@ class TrainValidationSplit(_Validator):
             raise TypeError("TrainValidationSplit: setEstimator first")
         if self._evaluator is None:
             raise ValueError("TrainValidationSplit: setEvaluator first (there is no default evaluator)")
-        X, y = self._data(X, y)
+        gp = est.getClassifier() if isinstance(est, OneVsRest) else est
+        X, y = self._data(X, y, getattr(gp, "_device", 0))           # a OneVsRest without a classifier fails below
         if train is None:
             mask = train_validation_assignment(len(X), self._train_ratio, self._seed)
         else:
@@ -401,7 +420,8 @@ class TrainValidationSplit(_Validator):
             preds, objective = self._fit_regression(ests, X, y, mask)
         else:
             preds, objective = self._fit_classifiers(ests, isinstance(est, OneVsRest), X, y, mask)
-        metrics = [self._evaluator.evaluate(y[~mask], p) for p in preds]
+        y_val = host_copy(_rows(y, ~mask))
+        metrics = [self._evaluator.evaluate(y_val, p) for p in preds]
         best = best_index(metrics, self._evaluator.isLargerBetter())
         self.last_predictions = preds
         return TrainValidationSplitModel(est.copy(maps[best]).fit(X, y), metrics, best, objective)
@@ -412,8 +432,8 @@ class TrainValidationSplit(_Validator):
         refuse validation sides the independent fit takes)."""
         preds, maps = [], []
         for e in ests:
-            model = e.fit(X[train], y[train])
-            preds.append(model.predict(X[~train]))
+            model = e.fit(_rows(X, train), _rows(y, train))
+            preds.append(_host_predictions(model.predict(_rows(X, ~train))))
             maps.append(e.last_objective)
             del model
         return preds, dict(maps=maps)
@@ -426,17 +446,20 @@ class TrainValidationSplit(_Validator):
         gps = [e.getClassifier() for e in ests] if ovr else ests
         if any(not isinstance(gp, GaussianProcessClassifier) for gp in gps):
             raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
-        X = np.asarray(X, dtype=np.float64)
+        if is_cuda_tensor(X):
+            import torch
+            X = X.to(torch.float64)
+        else:
+            X = np.asarray(X, dtype=np.float64)
         if ovr:
             one_vs_rest_labels(y)
-            C = one_vs_rest_labels(y[train])[1]           # as an independent OneVsRest.fit(X[train], y[train])
+            C = one_vs_rest_labels(_rows(y, train))[1]    # as an independent OneVsRest.fit(X[train], y[train])
             label = lambda c: c
         else:
-            if not np.all((y == 0.0) | (y == 1.0)):         # assertLabelsAre01, GPCls:68-72
-                raise RuntimeError("Only 0 and 1 labels are supported.")
+            assert_labels_are_01(y)
             C = 1
             label = lambda c: 1                             # y == 1 is y itself
-        Xt, yt, Xv = X[train], y[train], X[~train]
+        Xt, yt, Xv = _rows(X, train), _rows(y, train), _rows(X, ~train)
         raw = [np.empty((len(Xv), C)) for _ in gps]
         groups = []
         for slots in tvs_slot_groups(gps, C).values():
@@ -451,8 +474,7 @@ class TrainValidationSplit(_Validator):
                         [kernel_at(slots[i][0], t) for i, t in batch], g0._tol)
                     return [(float(v), g) for v, g in zip(vals, grads)]
 
-                thetas, latent, fit = laplace_fit(g0, eng, Xt, yt, objective,
-                                                  lambda i: eng.experts_f_slot(modes[i], len(Xt)),
+                thetas, latent, fit = laplace_fit(g0, eng, Xt, yt, objective, N.SGP_MODES_SLOT, lambda i: modes[i],
                                                   [gps[p].getKernel().getHyperparameters() for p, _, _ in slots])
                 # every objective call is one round, and one more runs at the slots' thetas
                 groups.append(dict(
@@ -461,7 +483,10 @@ class TrainValidationSplit(_Validator):
                     rounds=fit["rounds"], calls=fit["rounds"] + 1, launches=fit["launches_total"]))
                 for (p, c, _), f, theta in zip(slots, latent, thetas):
                     _produce_model(gps[p], eng, Xt, f, theta)
-                    raw[p][:, c], _ = eng.predict(Xv, with_variance=False)
+                    if is_cuda_tensor(Xv):
+                        raw[p][:, c] = _host_predictions(eng.predict_tensor(Xv, with_variance=False)[0])
+                    else:
+                        raw[p][:, c], _ = eng.predict(Xv, with_variance=False)
             finally:
                 eng.release()
         if ovr:
