@@ -196,7 +196,8 @@ int sgp_bcm_nll(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper* hy
  * bytes of device memory (rows, labels and latent modes of every set): SGP_E_NOMEM past what the device has free.
  * SGP_E_BADARG for n_folds < 2, a fold index outside [0, n_folds), or a set with E_k == 0 (the reference's / by zero).
  * As every upload, it resets the latent modes and the one-vs-rest modes.  The other objectives (sgp_bcm_nll,
- * sgp_laplace_nll*) see a fold upload as one expert set: the union of every set's experts. */
+ * sgp_laplace_nll* but sgp_laplace_nll_fold_slots_any_size) see a fold upload as one expert set: the union of every
+ * set's experts. */
 int sgp_experts_upload_folds(sgp_ctx* ctx, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
                              const int32_t* fold_of, int32_t n_folds, int32_t dataset_size_for_expert);
 /* sgp_experts_upload_folds on points already in device memory: every set is the same bits as the host upload's.  fold_of
@@ -312,6 +313,42 @@ int sgp_experts_get_f_slot(sgp_ctx* ctx, int32_t mode_slot, double* f_out);
  * device (SGP_E_BADARG otherwise, before the launch).  Returns when the modes are written. */
 enum { SGP_MODES_BINARY = 0, SGP_MODES_CLASS = 1, SGP_MODES_SLOT = 2 };
 int sgp_experts_get_f_rows_device(sgp_ctx* ctx, int32_t store, int32_t index, double* dF_out);
+
+/* Cross-validation over one-vs-rest (Spark's CrossValidator over OneVsRest): the Laplace objective of n_eval slots over
+ * the training sets of the last sgp_experts_upload_folds, in one launch per kernel family.  Listed slot i evaluates, with
+ * no other inputs, the training set sets[i], the labels (y == classes[i]), kernels[i] with hypers[i * n_hypers ...] (the
+ * same kernel structure and descriptor layout for every slot), and the latent modes of mode slot mode_slots[i], which it
+ * warm-starts from and writes back.  Sets and classes may repeat; mode slots are distinct and in [0, n_mode_slots).  The
+ * binary classifier is class 1 over 0/1 labels.
+ * Contract: slot i's value, gradient and modes equal, bit for bit, what sgp_laplace_nll_any_size returns after
+ * sgp_experts_upload_grouped(X[fold_of != k], y[fold_of != k] == c, dataset_size_for_expert), k = sets[i] and
+ * c = classes[i], with the same modes, on either kernel and whichever other slots share the call.  The kernel is chosen
+ * per set, by sgp_laplace_nll_any_size's rule on the set's largest expert (on chip up to 117 points, else global memory),
+ * so a call whose sets straddle that edge makes two launches, one per family; each slot's results land in its list
+ * position.  sgp_last_laplace_path is 1 if the global-memory kernel ran.
+ * The modes live in a store of their own, [n_mode_slots][rows of the largest set], indexed from each set's first row
+ * (apart from the stores of sgp_laplace_nll_classes and sgp_laplace_nll_slots_any_size: no entry moves another's modes):
+ * allocated on first use, zero after every sgp_experts_upload* and whenever n_mode_slots changes; the modes of mode slots
+ * not listed are left as they are.  With a communicator: one ncclAllReduce of the n_eval rows and n_eval status words.
+ * Errors, all before any allocation or launch: SGP_E_STATE without a fold upload; SGP_E_BADARG for a set outside
+ * [0, n_folds), a repeated or out-of-range mode slot, a negative class, n_eval outside [1, 65535] or above n_mode_slots,
+ * a structure that differs between slots, or a listed set's expert above 46336 points; SGP_E_SINGULAR for tol >= 1,
+ * every mode left as it was; SGP_E_NOMEM when the store or one global-memory workspace slice exceeds the device's free
+ * memory.  SGP_E_NOT_PD names the mode slot of the first listed slot whose B broke down. */
+int sgp_laplace_nll_fold_slots_any_size(sgp_ctx* ctx, int32_t n_mode_slots, const int32_t* mode_slots,
+                                        const int32_t* sets, const int32_t* classes, int32_t n_eval,
+                                        const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t n_hypers,
+                                        double tol, double* neg_log_z_out /* n_eval */,
+                                        double* grad_out /* n_eval x n_hypers */);
+/* Mode slot mode_slot's latent modes on fold set `set` (its N_k rows, in the set's packed expert-major order).
+ * SGP_E_STATE without a fold upload or before the first sgp_laplace_nll_fold_slots_any_size after it; SGP_E_BADARG for a
+ * set outside [0, n_folds) or a mode slot outside [0, n_mode_slots). */
+int sgp_experts_get_f_fold_slot(sgp_ctx* ctx, int32_t set, int32_t mode_slot, double* f_out);
+/* The same modes in the set's training-row order (the order of X[fold_of != set]), written to device memory dF_out (N_k
+ * doubles on the context's device: SGP_E_BADARG otherwise, before the launch).  The refusals of
+ * sgp_experts_get_f_fold_slot.  Returns when the modes are written.  (sgp_experts_get_f_rows_device refuses a fold
+ * upload.) */
+int sgp_experts_get_f_fold_rows_device(sgp_ctx* ctx, int32_t set, int32_t mode_slot, double* dF_out);
 
 /* Installs a caller-supplied (vector v, m x m matrix M, row-major) in place of the pair sgp_magic computes, so that
  * sgp_predict returns  mean_t = k(x_t, Z) . v  and  var_t = selfKernel + k(x_t, Z) M k(x_t, Z)^T  for them.  M need not be

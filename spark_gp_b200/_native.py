@@ -27,7 +27,8 @@ EXPORTS = ["sgp_ctx_create", "sgp_ctx_destroy", "sgp_last_error", "sgp_set_preci
            "sgp_laplace_nll_any_size", "sgp_laplace_nll_classes_any_size", "sgp_last_laplace_path",
            "sgp_laplace_nll_slots_any_size", "sgp_experts_get_f_slot", "sgp_experts_upload_grouped_device",
            "sgp_experts_upload_folds_device", "sgp_experts_get_f_rows_device", "sgp_kmeans_device",
-           "sgp_greedy_active_set_device"]
+           "sgp_greedy_active_set_device", "sgp_laplace_nll_fold_slots_any_size", "sgp_experts_get_f_fold_slot",
+           "sgp_experts_get_f_fold_rows_device"]
 
 
 class KernelTerm(C.Structure):
@@ -107,6 +108,9 @@ def load() -> C.CDLL:
     lib.sgp_experts_upload_grouped_device.argtypes = lib.sgp_experts_upload_grouped.argtypes
     lib.sgp_experts_upload_folds_device.argtypes = lib.sgp_experts_upload_folds.argtypes
     lib.sgp_experts_get_f_rows_device.argtypes = [vp, i32, i32, vp]
+    lib.sgp_laplace_nll_fold_slots_any_size.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp, i32, C.c_double, vp, vp]
+    lib.sgp_experts_get_f_fold_slot.argtypes = [vp, i32, i32, vp]
+    lib.sgp_experts_get_f_fold_rows_device.argtypes = [vp, i32, i32, vp]
     lib.sgp_kmeans_device.argtypes = lib.sgp_kmeans.argtypes
     lib.sgp_greedy_active_set_device.argtypes = lib.sgp_greedy_active_set.argtypes
     lib.sgp_event_elapsed_ms.argtypes = [vp, C.c_int, C.c_int, dp]

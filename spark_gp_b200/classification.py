@@ -97,13 +97,26 @@ def laplace_fit(gp, eng, X, y, objective, store, index, x0s, thetas=None):
       objective([(i, theta_i), ...]) -> [(value, gradient), ...]: slot i's Laplace objective at theta_i, warm-started from
                                         and moving its device-resident modes;
       store, index(i):                  where slot i's modes live (N.SGP_MODES_*, and the class or mode slot).
-    Unless `thetas` are given, every slot is optimised from x0s (`optimise_slots`; skipped when there are no
-    hyper-parameters).  Then the Laplace loop runs once more at every slot's theta (GPCls:60), so that its modes are the
-    modes at theta.  Returns (thetas, modes [slot][row] in row order -- a CUDA float64 tensor, ungrouped on the device,
-    when X is a CUDA tensor --, dict(slots: each slot's optimisation record or None when nothing was optimised, rounds,
-    launches: the optimisation's, launches_total: with the call at theta))."""
+    The slots are fitted by `laplace_optimise`.  Returns (thetas, modes [slot][row] in row order -- a CUDA float64 tensor,
+    ungrouped on the device, when X is a CUDA tensor --, the fit record of `laplace_optimise`)."""
     order = np.concatenate(group_for_experts(len(X), gp._datasetSizeForExpert))
     eng.experts_upload_grouped(X, y, gp._datasetSizeForExpert)
+    thetas, fit = laplace_optimise(gp, eng, objective, x0s, thetas)
+    if is_cuda_tensor(X):
+        import torch
+        return thetas, torch.stack([eng.experts_modes_rows(store, index(i), len(X)) for i in range(len(thetas))]), fit
+    latent = np.empty((len(thetas), len(X)))
+    for i in range(len(thetas)):
+        latent[i, order] = eng.experts_modes(store, index(i), len(X))
+    return thetas, latent, fit
+
+
+def laplace_optimise(gp, eng, objective, x0s, thetas=None):
+    """The slots' hyper-parameters on the experts already uploaded into eng (`objective` as for `laplace_fit`).  Unless
+    `thetas` are given, every slot is optimised from x0s (`optimise_slots`; skipped when there are no hyper-parameters).
+    Then the Laplace loop runs once more at every slot's theta (GPCls:60), so that its modes are the modes at theta.
+    Returns (thetas, dict(slots: each slot's optimisation record or None when nothing was optimised, rounds, launches:
+    the optimisation's, launches_total: with the call at theta))."""
     launches0 = eng.launch_count()
     records, rounds = None, 0
     if thetas is None:
@@ -112,14 +125,7 @@ def laplace_fit(gp, eng, X, y, objective, store, index, x0s, thetas=None):
             thetas, records, rounds = optimise_slots(objective, x0s, lbfgsb_bounds(gp.getKernel()), gp._maxIter, gp._tol)
     launches = eng.launch_count() - launches0
     objective(list(enumerate(thetas)))
-    fit = dict(slots=records, rounds=rounds, launches=launches, launches_total=eng.launch_count() - launches0)
-    if is_cuda_tensor(X):
-        import torch
-        return thetas, torch.stack([eng.experts_modes_rows(store, index(i), len(X)) for i in range(len(thetas))]), fit
-    latent = np.empty((len(thetas), len(X)))
-    for i in range(len(thetas)):
-        latent[i, order] = eng.experts_modes(store, index(i), len(X))
-    return thetas, latent, fit
+    return thetas, dict(slots=records, rounds=rounds, launches=launches, launches_total=eng.launch_count() - launches0)
 
 
 def _produce_model(gp, eng, X, f, theta):

@@ -808,8 +808,10 @@ int experts_alloc(Ctx* c, long long E, long long n, int d, int n_max) {
   c->ex_grouped = false;
   c->ex_classes = 0;                                      // one-vs-rest modes restart at zero on their next use
   c->ex_mode_slots = 0;                                   // so do the param-map slots' modes
+  c->ex_fold_mode_slots = 0;                              // and the fold slots' modes
   c->fold_first.clear();
   c->fold_nmax.clear();
+  c->fold_row0.clear();
   return SGP_OK;
 }
 
@@ -954,6 +956,7 @@ int upload_folds(Ctx* c, bool on_device, const void* X, int x_is_f32, const doub
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   c->fold_first = first;
   c->fold_nmax = nmax;
+  c->fold_row0 = row0;
   c->ex.E = E;
   return SGP_OK;
 }
@@ -1000,6 +1003,7 @@ struct ObjectiveSetup {
   std::vector<KernelFlat> kf_host; // [n_slots]
   const int* cls = nullptr;        // [n_slots] the classes (fold sets) list, or zeros
   const int* mode = nullptr;       // [n_slots] the mode slots list (sgp_laplace_nll_slots_any_size), else cls
+  const int* sets = nullptr;       // [n_slots] the fold sets list (sgp_laplace_nll_fold_slots_any_size), else nullptr
   double* total = nullptr;         // [n_slots][1 + n_hypers] totals, then [n_slots] status words
   int* flags = nullptr;            // [n_slots]
 };
@@ -1008,9 +1012,10 @@ struct ObjectiveSetup {
 // (hypers + s * nh for slot s) onto the flattened terms and uploads everything, with zeroed totals and flags, into the
 // context's descriptor block in one copy.  Every slot must have slot 0's kernel structure and descriptor kinds.
 // rows_per_slot: the per-expert rows a slot writes (0: every uploaded expert).  modes: a mode slots list uploaded after
-// the classes (nullptr: o.mode is the classes list).
+// the classes (nullptr: o.mode is the classes list).  sets: a fold sets list uploaded after the modes (nullptr: none).
 int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int nh,
-                    const int* classes, ObjectiveSetup& o, long long rows_per_slot = 0, const int* modes = nullptr) {
+                    const int* classes, ObjectiveSetup& o, long long rows_per_slot = 0, const int* modes = nullptr,
+                    const int* sets = nullptr) {
   if (c->ex.E == 0) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
   if (!kernels || nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, "null argument");
   for (int s = 0; s < n_slots; ++s)
@@ -1071,11 +1076,11 @@ int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const s
     block.insert(block.end(), value.begin(), value.end());
   }
   // [KernelFlat n_slots] then doubles [slot blocks | totals | status], then ints [kind | term | dim | flags | classes
-  // | modes (with modes)]
+  // | modes (with modes) | sets (with sets)]
   const int W = 1 + nh;
   const size_t kf_bytes = sizeof(KernelFlat) * n_slots;
   const size_t n_dbl = block.size() + static_cast<size_t>(n_slots) * (W + 1);
-  const size_t n_int = 3 * static_cast<size_t>(nh) + (modes ? 3 : 2) * static_cast<size_t>(n_slots);
+  const size_t n_int = 3 * static_cast<size_t>(nh) + ((modes ? 3 : 2) + (sets ? 1 : 0)) * static_cast<size_t>(n_slots);
   std::vector<char> host(kf_bytes + n_dbl * 8 + n_int * 4, 0);
   std::memcpy(host.data(), kfs.data(), kf_bytes);
   std::memcpy(host.data() + kf_bytes, block.data(), block.size() * 8);
@@ -1085,6 +1090,7 @@ int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const s
   std::copy(hdim.begin(), hdim.end(), hi + 2 * nh);
   if (classes) std::copy(classes, classes + n_slots, hi + 3 * nh + n_slots);
   if (modes) std::copy(modes, modes + n_slots, hi + 3 * nh + 2 * n_slots);
+  if (sets) std::copy(sets, sets + n_slots, hi + 3 * nh + (modes ? 3 : 2) * n_slots);
   int rc = ctx_scratch(c, c->hyper_ws, host.size());
   if (rc != SGP_OK) return rc;
   char* dev = c->hyper_ws.as<char>();
@@ -1102,13 +1108,16 @@ int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const s
   o.flags = dI + 3 * nh;
   o.cls = dI + 3 * nh + n_slots;
   o.mode = modes ? o.cls + n_slots : o.cls;
+  if (sets) o.sets = o.cls + (modes ? 2 : 1) * n_slots;
   return SGP_OK;
 }
 
 // all-reduce over ranks, copy the (objective, gradient) rows of every slot back, map a bad pivot to err_code.  With a
-// classes (fold sets) list, the message names the first failing slot's class (set), `what` saying which.
+// classes (fold sets) list, the message names the first failing slot's class (set), `what` saying which.  pos (optional):
+// slot s's outputs go to position pos[s], and the first failing slot is the one of the smallest position.
 int objective_finish(Ctx* c, const ObjectiveSetup& o, int nh, double* val_out, double* grad_out, int mask, int err_code,
-                     const char* err_msg, const int* classes = nullptr, const char* what = "class") {
+                     const char* err_msg, const int* classes = nullptr, const char* what = "class",
+                     const int* pos = nullptr) {
   const int W = 1 + nh, S = o.n_slots;
   // the rank-local status flags are all-reduced WITH the totals so that every rank raises (or none does)
   SGP_CUDA(c, launch_flags_to_double(o.total + static_cast<size_t>(S) * W, o.flags, mask, S, c->stream));
@@ -1122,13 +1131,16 @@ int objective_finish(Ctx* c, const ObjectiveSetup& o, int nh, double* val_out, d
   std::vector<double> tot(len);
   SGP_CUDA(c, cudaMemcpyAsync(tot.data(), o.total, len * 8, cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  auto at = [&](int s) { return pos ? pos[s] : s; };
+  int failed = -1;
   for (int s = 0; s < S; ++s)
-    if (tot[static_cast<size_t>(S) * W + s] != 0.0)
-      return fail(c, err_code, classes ? std::string(what) + " " + std::to_string(classes[s]) + ": " + err_msg
-                                       : std::string(err_msg));
+    if (tot[static_cast<size_t>(S) * W + s] != 0.0 && (failed < 0 || at(s) < at(failed))) failed = s;
+  if (failed >= 0)
+    return fail(c, err_code, classes ? std::string(what) + " " + std::to_string(classes[failed]) + ": " + err_msg
+                                     : std::string(err_msg));
   for (int s = 0; s < S; ++s) {
-    val_out[s] = tot[static_cast<size_t>(s) * W];
-    for (int i = 1; i < W; ++i) grad_out[static_cast<size_t>(s) * nh + i - 1] = tot[static_cast<size_t>(s) * W + i];
+    val_out[at(s)] = tot[static_cast<size_t>(s) * W];
+    for (int i = 1; i < W; ++i) grad_out[static_cast<size_t>(at(s)) * nh + i - 1] = tot[static_cast<size_t>(s) * W + i];
   }
   return SGP_OK;
 }
@@ -1329,6 +1341,26 @@ int laplace_nll(Ctx* c, Objective kind, const sgp_kernel_desc* k, const sgp_hype
   return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd);
 }
 
+// A mode store of n_store slots of `stride` modes each, (re)allocated and zeroed when *store_slots, the count it was set
+// up for, differs (0 after every upload).  SGP_E_NOMEM, before allocating, past the device's free memory; a failed
+// allocation leaves no store behind.
+int mode_store(Ctx* c, DevScratch& store, int* store_slots, int n_store, long long stride) {
+  if (*store_slots == n_store) return SGP_OK;
+  const size_t bytes = static_cast<size_t>(n_store) * stride * 8;
+  size_t free_b = 0, total_b = 0;
+  SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+  if (bytes > free_b + store.cap)
+    return fail(c, SGP_E_NOMEM, "the Laplace modes of " + std::to_string(n_store) + " slots need " +
+                                    std::to_string(bytes >> 20) + " MiB of device memory, " +
+                                    std::to_string((free_b + store.cap) >> 20) + " MiB available");
+  *store_slots = 0;
+  const int rc = ctx_scratch(c, store, bytes);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaMemsetAsync(store.p, 0, bytes, c->stream));
+  *store_slots = n_store;
+  return SGP_OK;
+}
+
 // The Laplace objective of n_eval slots over a mode store: slot i evaluates the labels (y == classes[i]) at kernels[i]
 // and hypers[i * nh ...], with the modes of store slot modes[i] (nullptr: modes = classes).  The store holds n_store
 // slots of n modes; it is (re)allocated and zeroed when *store_slots, the count it was set up for, differs (0 after every
@@ -1343,23 +1375,11 @@ int laplace_slots(Ctx* c, Objective kind, DevScratch& store, int* store_slots, i
   if (rc != SGP_OK) return rc;
   if (plan_objective(kind, c->ex, o.hv.kf.n_terms).variant == ObjectiveVariant::kRefused)
     return fail(c, SGP_E_BADARG, kLaplaceRefused);
-  if (*store_slots != n_store) {                          // first use after an upload, or another slot count
-    const size_t bytes = static_cast<size_t>(n_store) * c->ex.n * 8;
-    size_t free_b = 0, total_b = 0;
-    SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
-    if (bytes > free_b + store.cap)
-      return fail(c, SGP_E_NOMEM, "the Laplace modes of " + std::to_string(n_store) + " slots need " +
-                                      std::to_string(bytes >> 20) + " MiB of device memory, " +
-                                      std::to_string((free_b + store.cap) >> 20) + " MiB available");
-    *store_slots = 0;                                     // a failed allocation leaves no store behind
-    rc = ctx_scratch(c, store, bytes);
-    if (rc != SGP_OK) return rc;
-    SGP_CUDA(c, cudaMemsetAsync(store.p, 0, bytes, c->stream));
-    *store_slots = n_store;
-  }
+  rc = mode_store(c, store, store_slots, n_store, c->ex.n);   // first use after an upload, or another slot count
+  if (rc != SGP_OK) return rc;
   LaplaceClasses lc;
   lc.n_slots = n_eval; lc.cls = o.cls; lc.mode = o.mode; lc.kf = o.kf; lc.slot_stride = o.slot_stride;
-  lc.f = store.as<double>();
+  lc.f = store.as<double>(); lc.f_stride = c->ex.n;
   rc = laplace_run(c, kind, o, tol, &lc);
   if (rc != SGP_OK) return rc;
   return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd, modes ? modes : classes,
@@ -1434,6 +1454,179 @@ int sgp_laplace_nll_slots_any_size(sgp_ctx* h, int32_t n_mode_slots, const int32
     return fail(c, SGP_E_BADARG, "sgp_laplace_nll_slots_any_size: class indices must be >= 0");
   return laplace_slots(c, Objective::kLaplaceAnySize, c->ex_fm, &c->ex_mode_slots, n_mode_slots, classes, mode_slots,
                        n_eval, kernels, hypers, nh, tol, neg_log_z_out, grad_out, "mode slot");
+}
+
+namespace {
+// rows of the largest training set of the fold upload: the stride of the fold-slot mode store
+long long fold_rows_max(const Ctx* c) {
+  long long m = 0;
+  for (size_t k = 0; k + 1 < c->fold_row0.size(); ++k) m = std::max(m, c->fold_row0[k + 1] - c->fold_row0[k]);
+  return m;
+}
+
+// The stored modes of mode slot `mode_slot` on fold set `set` (from the set's first row), after the fold-slot getters'
+// refusals; n_k and E_k: the set's rows and experts.
+int fold_slot_modes(Ctx* c, int32_t set, int32_t mode_slot, const void* out, const char* fn, const double** f,
+                    long long* n_k, long long* E_k) {
+  if (c->ex.E == 0 || c->fold_first.empty() || !out)
+    return fail(c, SGP_E_STATE, "sgp_experts_upload_folds should have been called first");
+  if (c->ex_fold_mode_slots == 0)
+    return fail(c, SGP_E_STATE, "no fold slot modes: sgp_laplace_nll_fold_slots_any_size has not run since the upload");
+  const int n_sets = static_cast<int>(c->fold_first.size()) - 1;
+  if (set < 0 || set >= n_sets) return fail(c, SGP_E_BADARG, std::string(fn) + ": set index outside [0, n_folds)");
+  if (mode_slot < 0 || mode_slot >= c->ex_fold_mode_slots)
+    return fail(c, SGP_E_BADARG, std::string(fn) + ": mode slot outside [0, n_mode_slots)");
+  *f = c->ex_ffm.as<double>() + static_cast<size_t>(mode_slot) * fold_rows_max(c);
+  *n_k = c->fold_row0[set + 1] - c->fold_row0[set];
+  *E_k = c->fold_first[set + 1] - c->fold_first[set];
+  return SGP_OK;
+}
+}  // namespace
+
+int sgp_laplace_nll_fold_slots_any_size(sgp_ctx* h, int32_t n_mode_slots, const int32_t* mode_slots,
+                                        const int32_t* sets, const int32_t* classes, int32_t n_eval,
+                                        const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t nh, double tol,
+                                        double* neg_log_z_out, double* grad_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  const std::string fn = "sgp_laplace_nll_fold_slots_any_size";
+  if (!neg_log_z_out || (nh > 0 && !grad_out) || !(tol > 0.0) || !mode_slots || !sets || !classes)
+    return fail(c, SGP_E_BADARG, fn + ": bad argument");
+  if (c->ex.E == 0 || c->fold_first.empty())
+    return fail(c, SGP_E_STATE, "sgp_experts_upload_folds should have been called first");
+  if (n_mode_slots < 1 || n_eval < 1 || n_eval > n_mode_slots || n_eval > 65535)
+    return fail(c, SGP_E_BADARG, fn + ": need 1 <= n_eval <= n_mode_slots and n_eval <= 65535");
+  if (!distinct_in_range(mode_slots, n_eval, n_mode_slots))
+    return fail(c, SGP_E_BADARG, fn + ": mode slots must be distinct and in [0, n_mode_slots)");
+  if (*std::min_element(classes, classes + n_eval) < 0) return fail(c, SGP_E_BADARG, fn + ": class indices must be >= 0");
+  const int n_sets = static_cast<int>(c->fold_first.size()) - 1;
+  int n_max = 0;
+  for (int s = 0; s < n_eval; ++s) {
+    if (sets[s] < 0 || sets[s] >= n_sets)
+      return fail(c, SGP_E_BADARG, fn + ": set index " + std::to_string(sets[s]) + " outside [0, n_folds)");
+    n_max = std::max(n_max, c->fold_nmax[sets[s]]);
+  }
+  if (n_max > kLaplaceGlobalMaxPoints)
+    return fail(c, SGP_E_BADARG, "datasetSizeForExpert above " + std::to_string(kLaplaceGlobalMaxPoints) +
+                                     " points (32-bit indexing of the per-expert kernel build)");
+  if (tol >= 1.0) return fail(c, SGP_E_SINGULAR, kLaplaceNoIteration);
+  if (!kernels || nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, fn + ": null argument");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  // Each slot runs the kernel its own set plans (sgp_laplace_nll_any_size's rule on the set's largest expert): the slots
+  // are set up in the order [on chip | global memory], each family a contiguous range launched on its own; pos[j] is
+  // the list position of set-up slot j.
+  ExpertSet probe = c->ex;
+  std::vector<char> on_chip(n_eval);
+  for (int s = 0; s < n_eval; ++s) {
+    probe.n_max = c->fold_nmax[sets[s]];
+    on_chip[s] = plan_objective(Objective::kLaplaceAnySize, probe, 1).variant == ObjectiveVariant::kLaplace;
+  }
+  std::vector<int> pos;
+  for (int s = 0; s < n_eval; ++s) if (on_chip[s]) pos.push_back(s);
+  const int n_chip = static_cast<int>(pos.size());
+  for (int s = 0; s < n_eval; ++s) if (!on_chip[s]) pos.push_back(s);
+  std::vector<sgp_kernel_desc> kp(n_eval);
+  std::vector<sgp_hyper> hp(static_cast<size_t>(n_eval) * nh);
+  std::vector<int> mp(n_eval), sp(n_eval), cp(n_eval);
+  long long E_max = 0;
+  for (int j = 0; j < n_eval; ++j) {
+    const int s = pos[j];
+    kp[j] = kernels[s];
+    std::copy(hypers + static_cast<size_t>(s) * nh, hypers + static_cast<size_t>(s + 1) * nh,
+              hp.begin() + static_cast<size_t>(j) * nh);
+    mp[j] = mode_slots[s]; sp[j] = sets[s]; cp[j] = classes[s];
+    E_max = std::max(E_max, c->fold_first[sets[s] + 1] - c->fold_first[sets[s]]);
+  }
+  ObjectiveSetup o;
+  int rc = objective_setup(c, n_eval, kp.data(), hp.data(), nh, cp.data(), o, E_max, mp.data(), sp.data());
+  if (rc != SGP_OK) return rc;
+  const long long stride = fold_rows_max(c);
+  rc = mode_store(c, c->ex_ffm, &c->ex_fold_mode_slots, n_mode_slots, stride);
+  if (rc != SGP_OK) return rc;
+  // one view and plan per family: the largest expert and expert count over the family's sets
+  struct Family { int s0, s1; ExpertSet view; long long E; ObjectivePlan plan; };
+  std::vector<Family> fams;
+  for (int f = 0; f < 2; ++f) {
+    Family fam{f == 0 ? 0 : n_chip, f == 0 ? n_chip : n_eval, c->ex, 0, ObjectivePlan{}};
+    if (fam.s0 == fam.s1) continue;
+    fam.view.n_max = 0;
+    for (int j = fam.s0; j < fam.s1; ++j) {
+      fam.view.n_max = std::max(fam.view.n_max, c->fold_nmax[sp[j]]);
+      fam.E = std::max(fam.E, c->fold_first[sp[j] + 1] - c->fold_first[sp[j]]);
+    }
+    fam.plan = plan_objective(Objective::kLaplaceAnySize, fam.view, o.hv.kf.n_terms);
+    fams.push_back(fam);
+  }
+  // the global-memory family's workspace, before anything launches (as laplace_run sizes it)
+  long long grid = 0;
+  for (const Family& fam : fams) {
+    if (fam.plan.variant != ObjectiveVariant::kLaplaceGlobal) continue;
+    size_t free_b = 0, total_b = 0;
+    SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+    const size_t avail = free_b + c->laplace_ws.cap;
+    if (fam.plan.cta_ws > avail)
+      return fail(c, SGP_E_NOMEM, "the global-memory Laplace kernel needs " + std::to_string(fam.plan.cta_ws >> 20) +
+                                      " MiB of device memory for one expert of " + std::to_string(fam.view.n_max) +
+                                      " points, " + std::to_string(avail >> 20) + " MiB available");
+    const long long resident = static_cast<long long>(laplace_global_ctas_per_sm()) * c->num_sms;
+    grid = laplace_global_grid(fam.E * (fam.s1 - fam.s0), resident, fam.plan.cta_ws,
+                               std::min(kLaplaceGlobalCapBytes, avail));
+    rc = ctx_scratch(c, c->laplace_ws, static_cast<size_t>(grid) * fam.plan.cta_ws);
+    if (rc != SGP_OK) return rc;
+  }
+  const int W = 1 + nh;
+  c->laplace_path = 0;
+  for (const Family& fam : fams) {
+    const int s0 = fam.s0;
+    LaplaceClasses lc;
+    lc.n_slots = fam.s1 - s0; lc.cls = o.cls + s0; lc.mode = o.mode + s0; lc.kf = o.kf + s0;
+    lc.slot_stride = o.slot_stride; lc.f = c->ex_ffm.as<double>(); lc.f_stride = stride;
+    lc.sets = o.sets + s0; lc.first = c->ex_set_first.as<long long>(); lc.E_max = fam.E;
+    HyperView hv = o.hv;
+    hv.kf = o.kf_host[s0];
+    hv.beta += s0 * o.slot_stride; hv.h_coef += s0 * o.slot_stride; hv.h_value += s0 * o.slot_stride;
+    double* rows = c->nll_per_ws.as<double>() + static_cast<size_t>(s0) * E_max * W;
+    double* total = o.total + static_cast<size_t>(s0) * W;
+    if (fam.plan.variant == ObjectiveVariant::kLaplace) {
+      SGP_CUDA(c, launch_laplace(fam.plan, fam.view, hv, tol, rows, total, o.flags + s0, c->stream, &lc));
+    } else {
+      SGP_CUDA(c, launch_laplace_global(fam.view, hv, tol, c->laplace_ws.as<double>(), grid, rows, total, o.flags + s0,
+                                        c->stream, &lc));
+      c->laplace_path = 1;
+    }
+    c->launches += 2;
+  }
+  return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd, mp.data(), "mode slot",
+                          pos.data());
+}
+
+int sgp_experts_get_f_fold_slot(sgp_ctx* h, int32_t set, int32_t mode_slot, double* f_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  const double* f = nullptr;
+  long long n_k = 0, E_k = 0;
+  const int rc = fold_slot_modes(c, set, mode_slot, f_out, "sgp_experts_get_f_fold_slot", &f, &n_k, &E_k);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  SGP_CUDA(c, cudaMemcpyAsync(f_out, f, static_cast<size_t>(n_k) * 8, cudaMemcpyDeviceToHost, c->stream));
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  return SGP_OK;
+}
+
+int sgp_experts_get_f_fold_rows_device(sgp_ctx* h, int32_t set, int32_t mode_slot, double* dF_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  const double* f = nullptr;
+  long long n_k = 0, E_k = 0;
+  int rc = fold_slot_modes(c, set, mode_slot, dF_out, "sgp_experts_get_f_fold_rows_device", &f, &n_k, &E_k);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  rc = device_ptr_ok(c, dF_out, "sgp_experts_get_f_fold_rows_device", "f_out");
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, launch_ungroup_experts(dF_out, f, n_k, E_k, c->stream));   // the set is grouped as a grouped upload
+  c->launches += 1;
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  return SGP_OK;
 }
 
 int sgp_experts_get_f_slot(sgp_ctx* h, int32_t mode_slot, double* f_out) {

@@ -13,6 +13,11 @@
 // slot, of class c and mode slot m: labels (y == c), modes f + m * n, its own flattened kernel and hyper-parameter
 // block, output row [s][e].  The classes entry passes m = c.  The arithmetic is the single-class body's, so a slot's
 // rows equal, bit for bit, those of a single-class launch on an upload of the labels (y == c) with the same modes.
+//
+// Fold slots (sgp_laplace_nll_fold_slots_any_size): slot s also names a training set of a fold upload.  Block (x, s) is
+// expert first[sets[s]] + x (a block past the set's expert count returns before its first barrier), its modes are indexed
+// from the set's first row, and its output row is [s][x].  n_max and x_in_smem only move addresses: every loop runs over
+// the expert's own n, so a slot's rows equal those of a launch on an upload of that set alone.
 #include "expert_common.cuh"
 
 namespace sgp {
@@ -28,7 +33,9 @@ struct LapParams {
   const int* mode;           // [n_slots] mode slot of each slot: its modes are f + mode[s] * n (with cls)
   const KernelFlat* kf;      // [n_slots] flattened kernel of each slot (with cls)
   long long slot_stride;     // doubles between two slots' [beta | coef | value] blocks (with cls)
-  long long n;               // uploaded points: the stride of the per-class modes f (with cls)
+  long long n;               // the stride of the per-slot modes f (with cls)
+  const int* sets;           // [n_slots] fold set of each slot (with cls), or nullptr: every slot over every expert
+  const long long* first;    // [n_sets + 1] first expert of each fold set (with sets)
   double tol;
   double* out;               // [n_slots][E][1 + n_hypers]  (-logZ, -gradLogZ)
   int* flags;                // [n_slots]  bit 0: Cholesky pivot not positive
@@ -61,8 +68,15 @@ __device__ void bwd_solve(const double* L, int n, int ld, double* x) {
 
 __global__ void __launch_bounds__(LT, 1) laplace_kernel(const LapParams p) {
   extern __shared__ double sm[];
-  const long long e = blockIdx.x;
+  long long e = blockIdx.x;
   const int slot = blockIdx.y;
+  long long fr = 0;                                      // row of the modes that belong to the set's first row
+  if (p.sets) {
+    const long long first = p.first[p.sets[slot]];
+    if (e >= p.first[p.sets[slot] + 1] - first) return;
+    e += first;
+    fr = p.off[first];
+  }
   const long long r0 = p.off[e];
   const int n = static_cast<int>(p.off[e + 1] - r0);
   const int ld = p.n_max + 1;
@@ -75,6 +89,7 @@ __global__ void __launch_bounds__(LT, 1) laplace_kernel(const LapParams p) {
     hv.kf = p.kf[slot];
     hv.beta += slot * p.slot_stride; hv.h_coef += slot * p.slot_stride; hv.h_value += slot * p.slot_stride;
   }
+  fg += r0 - fr;                                         // the expert's modes
   double* K = sm;                                        // full symmetric
   double* M = K + static_cast<size_t>(p.n_max) * ld;     // B -> L -> L^-1 -> B^-1 (lower)
   double* v = M + static_cast<size_t>(p.n_max) * ld;     // vectors, n_max each
@@ -89,7 +104,7 @@ __global__ void __launch_bounds__(LT, 1) laplace_kernel(const LapParams p) {
   const double* Xe = ex_stage_rows(p.X + static_cast<size_t>(r0) * hv.d, n, hv.d, p.x_in_smem, Xs, xld);
 
   for (int i = tid; i < n; i += LT) {
-    f[i] = fg[r0 + i];
+    f[i] = fg[i];
     yv[i] = (cls < 0.0) ? p.y[r0 + i] : (p.y[r0 + i] == cls ? 1.0 : 0.0);
   }
   __syncthreads();
@@ -143,10 +158,10 @@ __global__ void __launch_bounds__(LT, 1) laplace_kernel(const LapParams p) {
     __syncthreads();
   }
   if (bad && tid == 0) atomicOr(p.flags + slot, 1);
-  for (int i = tid; i < n; i += LT) fg[r0 + i] = f[i];   // the mode persists (warm start of the next evaluation)
+  for (int i = tid; i < n; i += LT) fg[i] = f[i];   // the mode persists (warm start of the next evaluation)
 
   // ---- log Z and gradient (GPCls:114-128) --------------------------------------------------------------------------
-  double* out = p.out + (static_cast<size_t>(slot) * gridDim.x + e) * (1 + hv.n_hypers);
+  double* out = p.out + (static_cast<size_t>(slot) * gridDim.x + blockIdx.x) * (1 + hv.n_hypers);
   if (tid == 0) out[0] = -(new_obj - sumlogL);
   ex_invert_lower(M, n, ld, t1);                         // L^-1 in place
   // diag(C^T C), C = L^-1 (sqrtW K):  cc_i = | L^-1 (sw o K[:,i]) |^2   (GPCls:117,119)
@@ -204,16 +219,19 @@ cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const
   p.X = ex.X; p.y = ex.y; p.f = ex.f; p.off = ex.off; p.n_max = ex.n_max; p.x_in_smem = plan.x_in_smem;
   p.hv = hv; p.n = ex.n; p.tol = tol; p.out = rows; p.flags = flags;
   int n_slots = 1;
+  long long E = ex.E;
   if (classes) {
     p.f = classes->f; p.cls = classes->cls; p.mode = classes->mode; p.kf = classes->kf; p.slot_stride = classes->slot_stride;
+    p.n = classes->f_stride; p.sets = classes->sets; p.first = classes->first;
     n_slots = classes->n_slots;
+    if (classes->sets) E = classes->E_max;
   }
   cudaError_t e = cudaFuncSetAttribute(laplace_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(plan.smem));
   if (e != cudaSuccess) return e;
-  laplace_kernel<<<dim3(static_cast<unsigned>(ex.E), static_cast<unsigned>(n_slots)), LT, plan.smem, s>>>(p);
+  laplace_kernel<<<dim3(static_cast<unsigned>(E), static_cast<unsigned>(n_slots)), LT, plan.smem, s>>>(p);
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  return launch_rows_reduce(total, rows, ex.E, 1 + hv.n_hypers, s, n_slots);
+  return launch_rows_reduce(total, rows, E, 1 + hv.n_hypers, s, n_slots, p.sets, p.first);
 }
 
 }  // namespace sgp

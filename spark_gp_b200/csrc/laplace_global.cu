@@ -15,6 +15,8 @@
 //   - the level-2 steps (K b, the two triangular solves, K a, K s2, R t1) stay on the CUDA cores.
 // Every sum has a fixed order and the tiling depends on the expert's own n only, so a work item's bits do not depend on
 // the CTA that runs it, the grid size, n_max or the other experts and slots of the launch.
+// Fold slots (sgp_laplace_nll_fold_slots_any_size): item (s, x) is expert first[sets[s]] + x of slot s's training set
+// (items past the set's expert count are skipped), its modes are indexed from the set's first row, its row is [s][x].
 #include "expert_common.cuh"
 
 namespace sgp {
@@ -35,7 +37,7 @@ __host__ __device__ constexpr size_t lg_cta_doubles(int ld) {
 
 struct LapGlobalParams {
   const double* X; const double* y; double* f; const long long* off;
-  long long E;               // experts per slot
+  long long E;               // experts per slot (with sets: the largest expert count over the listed sets)
   int n_slots;
   int ldw;                   // workspace row stride: n_max rounded up to NB
   HyperView hv;              // slot 0's view (as laplace_kernel's)
@@ -43,7 +45,9 @@ struct LapGlobalParams {
   const int* mode;           // [n_slots] mode slot of each slot (with cls)
   const KernelFlat* kf;      // [n_slots] (with cls)
   long long slot_stride;     // (with cls)
-  long long n;               // uploaded points: stride of the per-slot modes (with cls)
+  long long n;               // stride of the per-slot modes (with cls)
+  const int* sets;           // [n_slots] fold set of each slot (with cls), or nullptr
+  const long long* first;    // [n_sets + 1] first expert of each fold set (with sets)
   double tol;
   double* ws;                // [gridDim.x][lg_cta_doubles(ldw)]
   double* out;               // [n_slots][E][1 + n_hypers]
@@ -393,7 +397,13 @@ __global__ void __launch_bounds__(GT, 1) laplace_global_kernel(const LapGlobalPa
   const long long items = p.E * p.n_slots;
   for (long long w = blockIdx.x; w < items; w += gridDim.x) {
     const int slot = static_cast<int>(w / p.E);
-    const long long e = w % p.E;
+    long long e = w % p.E, fr = 0;                       // fr: row of the modes that belong to the set's first row
+    if (p.sets) {
+      const long long first = p.first[p.sets[slot]];
+      if (e >= p.first[p.sets[slot] + 1] - first) continue;   // the whole CTA skips the item
+      e += first;
+      fr = p.off[first];
+    }
     const long long r0 = p.off[e];
     const int n = static_cast<int>(p.off[e + 1] - r0);
     const int np = (n + NB - 1) / NB * NB;
@@ -409,7 +419,7 @@ __global__ void __launch_bounds__(GT, 1) laplace_global_kernel(const LapGlobalPa
     const double* Xe = p.X + static_cast<size_t>(r0) * hv.d;
     __syncthreads();                                     // the previous item is done with the workspace
     for (int i = tid; i < np; i += GT) {
-      f[i] = (i < n) ? fg[r0 + i] : 0.0;
+      f[i] = (i < n) ? fg[r0 - fr + i] : 0.0;
       yv[i] = (i >= n) ? 0.0 : (cls < 0.0) ? p.y[r0 + i] : (p.y[r0 + i] == cls ? 1.0 : 0.0);
     }
     ex_build_kernel<true>(hv, Xe, hv.d, n, K, ld);       // K, both triangles (laplace_kernel's elements)
@@ -467,10 +477,10 @@ __global__ void __launch_bounds__(GT, 1) laplace_global_kernel(const LapGlobalPa
       __syncthreads();
     }
     if (bad && tid == 0) atomicOr(p.flags + slot, 1);
-    for (int i = tid; i < n; i += GT) fg[r0 + i] = f[i];   // the mode persists (warm start of the next evaluation)
+    for (int i = tid; i < n; i += GT) fg[r0 - fr + i] = f[i];   // the mode persists (warm start of the next evaluation)
 
     // ---- log Z and gradient (GPCls:114-128) ------------------------------------------------------------------------
-    double* out = p.out + (static_cast<size_t>(slot) * p.E + e) * (1 + hv.n_hypers);
+    double* out = p.out + (static_cast<size_t>(slot) * p.E + w % p.E) * (1 + hv.n_hypers);   // row [slot][x]
     if (tid == 0) out[0] = -(new_obj - sumlogL);
     lg_invert_lower(M, np, ld, P, D, Xs);                // L^-1 in place
     lg_diag_ctc(M, K, sw, np, ld, t2);                   // diag(C^T C), C = L^-1 (sqrtW K)   (GPCls:117,119)
@@ -530,12 +540,13 @@ cudaError_t launch_laplace_global(const ExpertSet& ex, const HyperView& hv, doub
   p.hv = hv; p.n = ex.n; p.tol = tol; p.ws = ws; p.out = rows; p.flags = flags;
   if (classes) {
     p.f = classes->f; p.cls = classes->cls; p.mode = classes->mode; p.kf = classes->kf; p.slot_stride = classes->slot_stride;
-    p.n_slots = classes->n_slots;
+    p.n_slots = classes->n_slots; p.n = classes->f_stride; p.sets = classes->sets; p.first = classes->first;
+    if (classes->sets) p.E = classes->E_max;
   }
   laplace_global_kernel<<<static_cast<unsigned>(grid), GT, 0, s>>>(p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  return launch_rows_reduce(total, rows, ex.E, 1 + hv.n_hypers, s, p.n_slots);
+  return launch_rows_reduce(total, rows, p.E, 1 + hv.n_hypers, s, p.n_slots, p.sets, p.first);
 }
 
 }  // namespace sgp

@@ -175,11 +175,15 @@ struct Ctx {
   int ex_classes = 0;            // classes ex_fc holds modes for; 0: none since the last upload
   DevScratch ex_fm;              // param-map latent modes [ex_mode_slots][n] (sgp_laplace_nll_slots_any_size)
   int ex_mode_slots = 0;         // mode slots ex_fm holds modes for; 0: none since the last upload
+  DevScratch ex_ffm;             // fold-slot latent modes [ex_fold_mode_slots][largest set's rows]
+                                 // (sgp_laplace_nll_fold_slots_any_size), indexed from each set's first row
+  int ex_fold_mode_slots = 0;    // mode slots ex_ffm holds modes for; 0: none since the last upload
   bool ex_grouped = false;       // ex came from a grouped upload (point i -> expert i % E): its modes can be ungrouped
   // fold upload (sgp_experts_upload_folds): the training sets lie one after another in ex; set k owns the experts
   // fold_first[k] .. fold_first[k+1]-1.  Empty after any other upload.
   std::vector<long long> fold_first;   // [n_sets + 1]
   std::vector<int> fold_nmax;          // [n_sets] largest expert of each set
+  std::vector<long long> fold_row0;    // [n_sets + 1] first row of each set
   DevScratch ex_set_first;             // device copy of fold_first
   DevScratch fold_pos_ws;              // upload scratch: the point indices grouped by fold, ascending in each fold
   DevScratch nll_per_ws;         // per-expert objective rows
@@ -363,7 +367,8 @@ cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const
 cudaError_t launch_bcm_nll_general(const ObjectivePlan& plan, cublasHandle_t blas, int* blas_status, void* ws,
                                    const ExpertSet& ex, const HyperView& hv, double* rows, double* total, int* flags,
                                    cudaStream_t s);
-// Slots of a Laplace launch (sgp_laplace_nll_classes*, sgp_laplace_nll_slots_any_size): slot s evaluates class cls[s]
+// Slots of a Laplace launch (sgp_laplace_nll_classes*, sgp_laplace_nll_slots_any_size, sgp_laplace_nll_fold_slots_any_size):
+// slot s evaluates class cls[s]
 // with the labels (y == cls[s]), the modes f + mode[s] * n, the flattened kernel kf[s] and the descriptor values
 // slot_stride doubles per slot after hv's.  The classes entries pass mode = cls.  rows: [n_slots][E][1 + n_hypers],
 // total: [n_slots][1 + n_hypers], flags: [n_slots].
@@ -373,7 +378,13 @@ struct LaplaceClasses {
   const int* mode = nullptr;          // device, [n_slots], distinct
   const KernelFlat* kf = nullptr;     // device, [n_slots]
   long long slot_stride = 0;
-  double* f = nullptr;                // device, [n_mode_slots][n]
+  double* f = nullptr;                // device, [n_mode_slots][f_stride]
+  long long f_stride = 0;             // modes per mode slot: the uploaded points, or the largest fold set's rows
+  // fold slots (sgp_laplace_nll_fold_slots_any_size): slot s evaluates the experts first[sets[s]] .. first[sets[s] + 1] - 1
+  // of a fold upload, its modes indexed from the set's first row; rows [n_slots][E_max][1 + n_hypers]
+  const int* sets = nullptr;          // device, [n_slots], or nullptr: every slot over every uploaded expert
+  const long long* first = nullptr;   // device, [n_sets + 1]
+  long long E_max = 0;                // the largest expert count over the slots' sets
 };
 // classes == nullptr: one slot on the labels and modes as uploaded (sgp_laplace_nll)
 cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol, double* rows,

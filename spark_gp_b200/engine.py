@@ -423,6 +423,35 @@ class ProjectedProcessEngine:
         return self._batched_objective(self._lib.sgp_laplace_nll_slots_any_size,
                                        (int(n_mode_slots), N.ptr(modes), N.ptr(cls), len(modes)), kernels, (float(tol),))
 
+    def laplace_nll_fold_slots_any_size(self, n_mode_slots: int, mode_slots, sets, classes, kernels, tol: float):
+        """Fold slots over the last `experts_upload_folds` (`sgp_laplace_nll_fold_slots_any_size`): listed slot i evaluates
+        the binary Laplace objective of training set sets[i] with the labels (y == classes[i]) at kernels[i], warm-started
+        from and writing the modes of mode slot mode_slots[i].  Sets and classes may repeat; mode slots are distinct in
+        [0, n_mode_slots).  Each slot equals `laplace_nll_any_size` on a grouped upload of that set alone, bit for bit.
+        Returns (values [n_eval], gradients [n_eval x n_hypers])."""
+        modes = np.ascontiguousarray(mode_slots, dtype=np.int32)
+        st = np.ascontiguousarray(sets, dtype=np.int32)
+        cls = np.ascontiguousarray(classes, dtype=np.int32)
+        if modes.ndim != 1 or len(modes) == 0 or st.shape != modes.shape or cls.shape != modes.shape \
+                or len(modes) != len(kernels):
+            raise ValueError("laplace_nll_fold_slots_any_size: one set, class and kernel per listed mode slot")
+        return self._batched_objective(self._lib.sgp_laplace_nll_fold_slots_any_size,
+                                       (int(n_mode_slots), N.ptr(modes), N.ptr(st), N.ptr(cls), len(modes)), kernels,
+                                       (float(tol),))
+
+    def experts_f_fold_slot(self, set_: int, slot: int, n: int):
+        """Mode slot `slot`'s latent modes on fold set `set_` of n training rows, after `laplace_nll_fold_slots_any_size`
+        (the set's packed expert-major order)."""
+        return self._modes(self._lib.sgp_experts_get_f_fold_slot, n, int(set_), int(slot))
+
+    def experts_f_fold_slot_rows(self, set_: int, slot: int, n: int):
+        """`experts_f_fold_slot` in the set's training-row order as a CUDA float64 tensor on this context's device,
+        ungrouped on the device (`sgp_experts_get_f_fold_rows_device`)."""
+        import torch
+        f = torch.empty(n, dtype=torch.float64, device="cuda:%d" % self._device)
+        self._check(self._lib.sgp_experts_get_f_fold_rows_device(self._h, int(set_), int(slot), C.c_void_p(f.data_ptr())))
+        return f
+
     def _modes(self, fn, n: int, *which):
         """n latent modes (packed expert-major order) read back by `fn(ctx, *which, out)`."""
         f = np.empty(n)

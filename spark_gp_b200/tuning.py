@@ -1,7 +1,8 @@
 """Model selection: Spark 3.1's `ParamGridBuilder`, `RegressionEvaluator`, `MulticlassClassificationEvaluator`,
-`CrossValidator` (regression estimator) and `TrainValidationSplit` (any estimator), as the reference's own examples use
-them (regression/examples/GPExample.scala:17-27, Airfoil.scala:18-24, Synthetics.scala:25-33: 10-fold cross-validation of
-the RMSE; classification/examples/MNIST.scala:34-40, Iris.scala:29-35: a train/validation split scored by accuracy).
+`CrossValidator` (regression estimator and one-vs-rest) and `TrainValidationSplit` (any estimator), as the reference's own
+examples use them (regression/examples/GPExample.scala:17-27, Airfoil.scala:18-24, Synthetics.scala:25-33: 10-fold
+cross-validation of the RMSE; classification/examples/Iris.scala: 10-fold cross-validation of one-vs-rest scored by
+accuracy; classification/examples/MNIST.scala:34-40: a train/validation split scored by accuracy).
 
 Spark's ml/tuning and ml/evaluation are not part of the reference project; they are restated here from Spark 3.1's
 documented behaviour:
@@ -23,6 +24,13 @@ maxIter and tol are optimised together: the training sets of every fold are uplo
 (`sgp_experts_upload_folds`), and each round of their L-BFGS-B runs is one `sgp_bcm_nll_folds` launch over experts x
 slots.  Each slot's objective values equal the independent fit's bit for bit, so every fold model, prediction and metric
 is the one `estimator.copy(map).fit(X[train], y[train])` gives.
+Over one-vs-rest, fold k has C_k = max(y[train]) + 1 classes, as an independent `OneVsRest.fit(X[train], y[train])`
+counts them.  The (map p, fold k, class c) slots are grouped by `slot_group_key` of the wrapped classifier; a group uploads
+the fold sets once, and each round of its L-BFGS-B runs is one `sgp_laplace_nll_fold_slots_any_size` call, every slot
+with its own mode slot (`fold_class_slot_groups`), plus one call at every slot's optimum (GPCls:60).  Each fold's class
+models are then produced on its training rows, and its validation prediction is the first argmax over the C_k raw
+columns.  The evaluator is a RegressionEvaluator (the default) or a MulticlassClassificationEvaluator.  The binary
+classifier is refused; the fold-slot entry already serves it (class 1 over 0/1 labels, one mode slot per (map, fold)).
 
 TrainValidationSplit (Spark 3.1): fit every param map on the training rows (in row order), evaluate each fitted model on
 the validation rows (validationMetrics, in map order), take the first best map and refit it on all rows.  trainRatio
@@ -45,9 +53,9 @@ import numpy as np
 
 from . import _native as N
 from .classification import GaussianProcessClassifier, OneVsRest, _produce_model, assert_labels_are_01, laplace_fit, \
-    one_vs_rest_labels, one_vs_rest_prediction
+    laplace_optimise, one_vs_rest_labels, one_vs_rest_prediction
 from .engine import ProjectedProcessEngine, device_fit_data, host_copy, is_cuda_tensor, take_rows
-from .hyperopt import lbfgsb_bounds, optimise_slots
+from .hyperopt import group_for_experts, lbfgsb_bounds, optimise_slots
 from .regression import GaussianProcessRegression
 from .utils import kfold_assignment, train_validation_assignment
 
@@ -185,12 +193,21 @@ def group_slots(estimators, n: int):
     return groups
 
 
+def fold_class_slot_groups(classifiers, n_classes):
+    """`group_slots` over the (map p, fold k, class c) slots of a cross-validation over classifiers (one per map), fold k
+    having n_classes[k] classes, each with the device mode slot it owns: {slot_group_key: [(p, k, c, mode slot), ...]}.
+    Mode slot p * sum(n_classes) + (classes of the folds before k) + c.  The one place that numbers mode slots."""
+    fc = [(k, c) for k, C in enumerate(n_classes) for c in range(C)]
+    return {key: [(p, *fc[j], p * len(fc) + j) for p, j in slots]
+            for key, slots in group_slots(classifiers, len(fc)).items()}
+
+
 def tvs_slot_groups(classifiers, n_classes: int):
-    """`group_slots` over the (map p, class c) slots of a train/validation split over classifiers (one per map), each
-    with the device mode slot it owns: {slot_group_key: [(p, c, p * n_classes + c), ...]}.  The one place that numbers
-    mode slots."""
-    return {key: [(p, c, p * n_classes + c) for p, c in slots]
-            for key, slots in group_slots(classifiers, n_classes).items()}
+    """The (map p, class c) slots of a train/validation split over classifiers (one per map), each with the device mode
+    slot it owns, p * n_classes + c: {slot_group_key: [(p, c, mode slot), ...]} (`fold_class_slot_groups` with one
+    fold)."""
+    return {key: [(p, c, m) for p, _, c, m in slots]
+            for key, slots in fold_class_slot_groups(classifiers, [n_classes]).items()}
 
 
 class _SelectedModel:
@@ -252,6 +269,8 @@ class CrossValidatorModel(_SelectedModel):
 
 class CrossValidator(_Validator):
     NAME = "CrossValidator"
+    ESTIMATORS = (GaussianProcessRegression, OneVsRest)
+    EVALUATORS = (RegressionEvaluator, MulticlassClassificationEvaluator)
 
     def __init__(self):
         self._estimator = None
@@ -262,15 +281,18 @@ class CrossValidator(_Validator):
         self.last_folds = None            # {(map, fold): theta, magicVector and validation prediction of the fold model}
 
     def setEstimator(self, value):
-        if not isinstance(value, GaussianProcessRegression):
-            raise TypeError("CrossValidator: the estimator must be a GaussianProcessRegression, not %s"
+        """A GaussianProcessRegression or a OneVsRest.  The binary GaussianProcessClassifier is refused: the fold-slot
+        objective already serves it (class 1 over 0/1 labels), but its selector path is not built."""
+        if not isinstance(value, self.ESTIMATORS):
+            raise TypeError("CrossValidator: the estimator must be a GaussianProcessRegression or a OneVsRest, not %s"
                             % type(value).__name__)
         self._estimator = value
         return self
 
     def setEvaluator(self, value):
-        if not isinstance(value, RegressionEvaluator):
-            raise TypeError("CrossValidator: the evaluator must be a RegressionEvaluator")
+        if not isinstance(value, self.EVALUATORS):
+            raise TypeError("CrossValidator: the evaluator must be a RegressionEvaluator or a "
+                            "MulticlassClassificationEvaluator, not %s" % type(value).__name__)
         self._evaluator = value
         return self
 
@@ -287,8 +309,11 @@ class CrossValidator(_Validator):
         """folds: the fold of every row (integers in [0, numFolds)); default: the seeded split of the module docstring."""
         est = self._estimator
         if est is None:
-            raise TypeError("CrossValidator: setEstimator(GaussianProcessRegression) first")
-        X, y = self._data(X, y, est._device)
+            raise TypeError("CrossValidator: setEstimator(GaussianProcessRegression or OneVsRest) first")
+        ovr = isinstance(est, OneVsRest)
+        if ovr and not isinstance(est.getClassifier(), GaussianProcessClassifier):
+            raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
+        X, y = self._data(X, y, (est.getClassifier() if ovr else est)._device)
         K = self._num_folds
         if folds is None:
             fold_of = kfold_assignment(len(X), K, self._seed)
@@ -302,6 +327,11 @@ class CrossValidator(_Validator):
             raise ValueError("CrossValidator: fold %d has no rows to validate on" % int(np.argmin(sizes)))
         maps = self._maps or [{}]
         ests = [est.copy(m) for m in maps]
+        if ovr:
+            folds_out, objective = self._fit_one_vs_rest([e.getClassifier() for e in ests], X, y, fold_of, K)
+            metrics = np.array([[self._evaluator.evaluate(host_copy(_rows(y, fold_of == k)), folds_out[p, k]["prediction"])
+                                 for k in range(K)] for p in range(len(maps))])
+            return self._select(est, maps, X, y, K, metrics, folds_out, objective)
         thetas, objective = self._optimise(ests, X, y, fold_of, K)
         metrics = np.empty((len(maps), K))
         folds_out = {}
@@ -313,11 +343,82 @@ class CrossValidator(_Validator):
                 folds_out[p, k] = dict(theta=thetas[p][k], magicVector=model.rawPredictor.magicVector, prediction=pred)
                 metrics[p, k] = self._evaluator.evaluate(host_copy(_rows(y, val)), pred)
                 del model                         # its context goes back to the pool before the next slot
+        return self._select(est, maps, X, y, K, metrics, folds_out, objective)
+
+    def _select(self, est, maps, X, y, K, metrics, folds_out, objective):
+        """avgMetrics, the first best map refitted on every row, and the records of the fit."""
         avg = [sum(metrics[p, k] for k in range(K)) / K for p in range(len(maps))]
         best = best_index(avg, self._evaluator.isLargerBetter())
         self.last_folds = folds_out
         objective["fold_metrics"] = metrics
         return CrossValidatorModel(est.copy(maps[best]).fit(X, y), avg, best, objective)
+
+    @staticmethod
+    def _fit_one_vs_rest(gps, X, y, fold_of, K):
+        """Every (map p, fold k) of one-vs-rest over the classifiers gps (one per map): the fold's C_k class models, as
+        `OneVsRest().setClassifier(gps[p]).fit(X[train], y[train])` fits them, and their validation prediction.  Per
+        group of slots one fold upload, one lock-step L-BFGS-B over the (map, fold, class) slots with one
+        `sgp_laplace_nll_fold_slots_any_size` call per round, and one more call at every slot's optimum (GPCls:60).
+        Returns ({(p, k): theta (C_k x h), magicVector [C_k], prediction}, dict(groups=...))."""
+        if is_cuda_tensor(X):
+            import torch
+            X = X.to(torch.float64)
+        else:
+            X = np.asarray(X, dtype=np.float64)
+        y = one_vs_rest_labels(y)[0]
+        train = [fold_of != k for k in range(K)]
+        n_k = [int(np.count_nonzero(t)) for t in train]
+        C = [one_vs_rest_labels(_rows(y, t))[1] for t in train]   # as an independent OneVsRest.fit(X[train], y[train])
+        thetas, latent, groups = {}, {}, []
+        for slots in fold_class_slot_groups(gps, C).values():
+            g0 = gps[slots[0][0]]
+            kernel_at = lambda p, t: gps[p].getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
+            eng = ProjectedProcessEngine.acquire(g0._device)
+            try:
+                eng.experts_upload_folds(X, y, fold_of, K, g0._datasetSizeForExpert)
+
+                def objective(batch):
+                    vals, grads = eng.laplace_nll_fold_slots_any_size(
+                        len(gps) * sum(C), [slots[i][3] for i, _ in batch], [slots[i][1] for i, _ in batch],
+                        [slots[i][2] for i, _ in batch], [kernel_at(slots[i][0], t) for i, t in batch], g0._tol)
+                    return [(float(v), g) for v, g in zip(vals, grads)]
+
+                fitted, fit = laplace_optimise(g0, eng, objective, [gps[p].getKernel().getHyperparameters()
+                                                                    for p, _, _, _ in slots])
+                # every objective call is one round, and one more runs at the slots' thetas
+                groups.append(dict(
+                    slots=[dict(map=p, fold=k, cls=c, mode_slot=m, theta=theta, **r)
+                           for (p, k, c, m), r, theta in zip(slots, fit["slots"] or [{}] * len(slots), fitted)],
+                    rounds=fit["rounds"], calls=fit["rounds"] + 1, launches=fit["launches_total"]))
+                for (p, k, c, m), theta in zip(slots, fitted):
+                    thetas[p, k, c] = theta
+                    if is_cuda_tensor(X):
+                        latent[p, k, c] = eng.experts_f_fold_slot_rows(k, m, n_k[k])
+                    else:
+                        order = np.concatenate(group_for_experts(n_k[k], g0._datasetSizeForExpert))
+                        latent[p, k, c] = np.empty(n_k[k])
+                        latent[p, k, c][order] = eng.experts_f_fold_slot(k, m, n_k[k])
+            finally:
+                eng.release()
+        folds_out = {}
+        eng = ProjectedProcessEngine.acquire(gps[0]._device)
+        try:
+            for p, gp in enumerate(gps):
+                for k in range(K):
+                    Xt, Xv = _rows(X, train[k]), _rows(X, ~train[k])
+                    raw, mvs = np.empty((len(Xv), C[k])), []
+                    for c in range(C[k]):
+                        _, _, mv, _, _ = _produce_model(gp, eng, Xt, latent[p, k, c], thetas[p, k, c])
+                        mvs.append(mv)
+                        if is_cuda_tensor(Xv):
+                            raw[:, c] = _host_predictions(eng.predict_tensor(Xv, with_variance=False)[0])
+                        else:
+                            raw[:, c], _ = eng.predict(Xv, with_variance=False)
+                    folds_out[p, k] = dict(theta=np.array([thetas[p, k, c] for c in range(C[k])]), magicVector=mvs,
+                                           prediction=one_vs_rest_prediction(raw))
+        finally:
+            eng.release()
+        return folds_out, dict(groups=groups)
 
     @staticmethod
     def _optimise(ests, X, y, fold_of, K):
