@@ -370,6 +370,28 @@ int sgp_predict(sgp_ctx* ctx, const double* X, int64_t n, double* mean_out, doub
  * the outputs. */
 int sgp_predict_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n, double* dMean, double* dVar);
 
+/* ---- averaged predictive probability (GPML eq. 3.25) with commons/util/Integrator.scala's quadrature ---------------- */
+/* The n-node Gauss-Hermite rule for the weight exp(-x^2): sum_i weights[i] f(nodes[i]) ~ int f(x) exp(-x^2) dx.  Nodes
+ * ascending, exactly antisymmetric (nodes[i] == -nodes[n-1-i]); weights exactly symmetric.  Host code, no context, no
+ * GPU.  SGP_E_BADARG for n outside [1, 256] or a NULL output. */
+int sgp_gauss_hermite_rule(int32_t n, double* nodes, double* weights);
+/* p_t = (1/sqrt(pi)) sum_i w_i sigmoid(mean_t + sqrt(2 var_t) x_i), sigmoid(z) = 1/(1 + exp(-z)), with the n_nodes-node
+ * rule (x_i, w_i) of sgp_gauss_hermite_rule and (mean_t, var_t) bit for bit what sgp_predict returns (var_t includes the
+ * white-noise part of selfKernel): Integrator.expectedOfFunctionOfNormal(mean_t, var_t, sigmoid), the probability of
+ * class 1 averaged over the latent posterior.  One deviation: var_t < 0 (rounding, or a caller's sgp_set_magic pair) is
+ * taken as 0, so that p_t = sigmoid(mean_t) times the rule's weight sum / sqrt(pi), where the Integrator would return
+ * NaN; a NaN mean or variance gives NaN.  The quadrature is fused into the variance pass: the call makes the launches of
+ * an sgp_predict with var_out.  mean_out and var_out may be NULL.  Refuses what sgp_predict refuses, with the same codes,
+ * and n_nodes outside [1, 256] (SGP_E_BADARG).  A point's outputs do not depend on the call it arrives in, as for
+ * sgp_predict. */
+int sgp_predict_probability(sgp_ctx* ctx, const double* X, int64_t n, int32_t n_nodes, double* p_out, double* mean_out,
+                            double* var_out);
+/* Same, points and outputs in device memory (dX fp64, or fp32 when x_is_f32 != 0; dMean and dVar may be NULL); every
+ * pointer must be device memory on the context's device (SGP_E_BADARG otherwise, before any launch).  Asynchronous on
+ * the context's stream: synchronise with sgp_sync before reading the outputs. */
+int sgp_predict_probability_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n, int32_t n_nodes,
+                                   double* dP, double* dMean, double* dVar);
+
 /* ---- introspection (tests / bench) ---------------------------------------------------------- */
 /* Number of kernels this library launched on ctx since creation. */
 int64_t sgp_launch_count(const sgp_ctx* ctx);

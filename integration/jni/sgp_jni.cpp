@@ -132,6 +132,24 @@ JNIEXPORT void JNICALL Java_org_apache_spark_ml_commons_NativeProjectedProcess_p
   if (rc != SGP_OK) throw_for(env, ctx, rc);
 }
 
+// the probability of class 1 averaged over the latent posterior (Integrator.scala's Gauss-Hermite rule with `nodes`
+// nodes) of a block of rows; mean and var may be null
+JNIEXPORT void JNICALL Java_org_apache_spark_ml_commons_NativeProjectedProcess_predictProbability(
+    JNIEnv* env, jclass, jlong h, jdoubleArray X, jlong n, jint nodes, jdoubleArray p, jdoubleArray mean,
+    jdoubleArray var) {
+  sgp_ctx* ctx = reinterpret_cast<sgp_ctx*>(h);
+  jdouble* x = env->GetDoubleArrayElements(X, nullptr);
+  jdouble* po = env->GetDoubleArrayElements(p, nullptr);
+  jdouble* mo = mean ? env->GetDoubleArrayElements(mean, nullptr) : nullptr;
+  jdouble* vo = var ? env->GetDoubleArrayElements(var, nullptr) : nullptr;
+  const int rc = sgp_predict_probability(ctx, x, n, nodes, po, mo, vo);
+  env->ReleaseDoubleArrayElements(X, x, JNI_ABORT);
+  env->ReleaseDoubleArrayElements(p, po, 0);
+  if (mo) env->ReleaseDoubleArrayElements(mean, mo, 0);
+  if (vo) env->ReleaseDoubleArrayElements(var, vo, 0);
+  if (rc != SGP_OK) throw_for(env, ctx, rc);
+}
+
 // ---- hyper-parameter objective (GaussianProcessCommons.scala:73-78 treeAggregate of likelihoodAndGradient) ----------
 // experts of this executor, packed expert-major by the Scala side: X (n*d), y (n), offsets (E+1)
 JNIEXPORT void JNICALL Java_org_apache_spark_ml_commons_NativeProjectedProcess_expertsUpload(

@@ -25,6 +25,32 @@ private[ml] object NativeProjectedProcess {
   @native def setMagic(ctx: Long, magicVector: Array[Double], magicMatrix: Array[Double]): Unit
   /** mean (and var, unless null) of n rows of x (row-major): GaussianProjectedProcessRawPredictor.predict, GPC:121-125. */
   @native def predict(ctx: Long, x: Array[Double], n: Long, mean: Array[Double], variance: Array[Double]): Unit
+  /** p (and mean, variance, unless null) of n rows of x (row-major): the probability of class 1 averaged over the latent
+    * posterior, new Integrator(nodes).expectedOfFunctionOfNormal(mean, variance, sigmoid) on the device, a negative
+    * variance taken as 0 (commons/util/Integrator.scala; IntegratorTest uses nodes = 100). */
+  @native def predictProbability(ctx: Long, x: Array[Double], n: Long, nodes: Int, p: Array[Double], mean: Array[Double],
+                                 variance: Array[Double]): Unit
+
+  /** The averaged probability of class 1 for one partition's rows under a binary classification model (kernel,
+    * activeSet, magicVector, magicMatrix), in blocks of `block` rows: what `scorePartition` is for the raw prediction. */
+  def probabilityPartition(partitionId: Int, rows: Iterator[Vector], kernel: Kernel, activeSet: Array[Vector],
+                           magicVector: BDV[Double], magicMatrix: BDM[Double], nodes: Int = 100,
+                           nGPUs: Int = 8, block: Int = 32768): Iterator[Double] = {
+    val m = activeSet.length
+    val d = activeSet.head.size
+    val terms = flatten(kernel)
+    val ctx = create(partitionId % nGPUs)
+    try {
+      begin(ctx, terms.map(_._1).toArray, terms.map(_._2).toArray, terms.map(_._3).toArray, terms.flatMap(_._4).toArray,
+        activeSet.flatMap(_.toArray), m, d)
+      setMagic(ctx, magicVector.toArray, magicMatrix.toArray)
+      rows.grouped(block).flatMap { blk =>
+        val p = new Array[Double](blk.length)
+        predictProbability(ctx, blk.flatMap(_.toArray).toArray, blk.length.toLong, nodes, p, null, null)
+        p.iterator
+      }.toVector.iterator                                   // materialised: the context is destroyed below
+    } finally destroy(ctx)
+  }
 
   /** Scores one partition's rows with the model (kernel, activeSet, magicVector, magicMatrix): one native context per
     * task (device = partitionId % nGPUs), rows in blocks of `block`.  What a model's `transform` maps over its partitions

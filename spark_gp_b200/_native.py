@@ -28,7 +28,8 @@ EXPORTS = ["sgp_ctx_create", "sgp_ctx_destroy", "sgp_last_error", "sgp_set_preci
            "sgp_laplace_nll_slots_any_size", "sgp_experts_get_f_slot", "sgp_experts_upload_grouped_device",
            "sgp_experts_upload_folds_device", "sgp_experts_get_f_rows_device", "sgp_kmeans_device",
            "sgp_greedy_active_set_device", "sgp_laplace_nll_fold_slots_any_size", "sgp_experts_get_f_fold_slot",
-           "sgp_experts_get_f_fold_rows_device"]
+           "sgp_experts_get_f_fold_rows_device", "sgp_gauss_hermite_rule", "sgp_predict_probability",
+           "sgp_predict_probability_device"]
 
 
 class KernelTerm(C.Structure):
@@ -77,6 +78,9 @@ def load() -> C.CDLL:
     lib.sgp_magic.argtypes = [vp, vp, vp, vp, vp]
     lib.sgp_predict.argtypes = [vp, vp, i64, vp, vp]
     lib.sgp_predict_device.argtypes = [vp, vp, i32, i64, vp, vp]
+    lib.sgp_gauss_hermite_rule.argtypes = [i32, vp, vp]
+    lib.sgp_predict_probability.argtypes = [vp, vp, i64, i32, vp, vp, vp]
+    lib.sgp_predict_probability_device.argtypes = [vp, vp, i32, i64, i32, vp, vp, vp]
     lib.sgp_set_magic.argtypes = [vp, vp, vp]
     lib.sgp_launch_count.argtypes = [vp]
     lib.sgp_launch_count.restype = i64

@@ -37,6 +37,20 @@ class GaussianProcessClassificationModel:
         p0 = 1.0 / (1.0 + np.exp(raw[..., 0]))          # sigmoid(-(-f))
         return np.stack([p0, 1.0 - p0], axis=-1)
 
+    def predictAveragedProbability(self, features, numNodes: int = 100):
+        """n x 2 rows [1 - p, p]: p the probability of class 1 averaged over the latent posterior N(f*, var*) of the raw
+        predictor (GPML eq. 3.25), p = E[sigmoid(f)] by the numNodes-node Gauss-Hermite rule, as
+        commons/util/Integrator.scala computes it (IntegratorTest's 100 nodes by default; a negative variance is taken as
+        0, where the Integrator would return NaN).  Class 1 is column 1, unlike `predictProbability`.  One vector gives
+        one row; a CUDA torch tensor stays on the device (CUDA float64 result)."""
+        engine = self.rawPredictor._engine
+        if is_cuda_tensor(features):
+            import torch
+            p, _, _ = engine.predict_probability_tensor(features, nodes=numNodes)
+            return torch.stack([1.0 - p, p], dim=-1)
+        p, _, _ = engine.predict_probability(np.asarray(features, dtype=np.float64), nodes=numNodes)
+        return np.stack([1.0 - p, p], axis=-1)
+
     def predict(self, features):
         """ClassificationModel.predict = raw2prediction(predictRaw(x)); with no thresholds set (the reference sets none)
         Spark's ProbabilisticClassificationModel.raw2prediction is `rawPrediction.argmax`, i.e. class 1 iff f > 0 (first
@@ -196,6 +210,16 @@ class OneVsRestModel:
         """n x numClasses: column c is class c's latent prediction f_c(x) (its model's rawPrediction(1)).  A CUDA torch
         tensor stays on the device (CUDA float64 result)."""
         cols = [m.predictRaw(features)[..., 1] for m in self.models]
+        if is_cuda_tensor(features):
+            import torch
+            return torch.stack(cols, dim=-1)
+        return np.stack(cols, axis=-1)
+
+    def predictAveragedProbability(self, features, numNodes: int = 100):
+        """n x numClasses: column c is class c's binary averaged probability (its model's
+        `predictAveragedProbability` column 1).  These are one-vs-rest scores, each against the rest of the classes: a
+        row is NOT normalised and need not sum to 1.  A CUDA torch tensor stays on the device (CUDA float64 result)."""
+        cols = [m.predictAveragedProbability(features, numNodes)[..., 1] for m in self.models]
         if is_cuda_tensor(features):
             import torch
             return torch.stack(cols, dim=-1)

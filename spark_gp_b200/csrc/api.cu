@@ -700,31 +700,33 @@ int sgp_set_magic(sgp_ctx* h, const double* v, const double* M) {
   return SGP_OK;
 }
 
-// The host rows stream in through the statistics path's double-buffered staging; each window's mean / variance go to one
-// of two device output buffers and are copied out (copy stream) once the NEXT window is queued, so that the copies in
-// both directions overlap the kernels.
-int sgp_predict(sgp_ctx* h, const double* X, int64_t n, double* mean_out, double* var_out) {
-  Ctx* c = reinterpret_cast<Ctx*>(h);
-  if (!c) return SGP_E_BADARG;
-  if (!c->has_magic) return fail(c, SGP_E_STATE, "sgp_magic should have been called first");
-  if (n < 0 || (n > 0 && (!X || !mean_out))) return fail(c, SGP_E_BADARG, "null argument");
-  if (n == 0) return SGP_OK;
+namespace {
+// The host rows stream in through the statistics path's double-buffered staging; each window's mean / variance /
+// probability go to one of two device output buffers and are copied out (copy stream) once the NEXT window is queued, so
+// that the copies in both directions overlap the kernels.  The mean is always computed (the probability reads it); it is
+// copied out only where mean_out is given.  p_out: the averaged probabilities with the n_nodes-node rule, or nullptr.
+int predict_host(Ctx* c, const double* X, long long n, int n_nodes, double* mean_out, double* var_out, double* p_out) {
   SGP_CUDA(c, cudaSetDevice(c->device));
   // staged chunks of ~32 MB of X (at least 4096 points), never more than one kernel window
   const size_t row = static_cast<size_t>(c->d) * sizeof(double);
   const long long win = predict_window_points(c->m_pad);
   long long chunk = std::max<long long>(4096, static_cast<long long>((size_t(32) << 20) / row));
-  chunk = std::min(std::min(chunk, win), static_cast<long long>(n));
-  int rc = predict_prepare(c, var_out != nullptr);
-  if (rc == SGP_OK) rc = ctx_scratch(c, c->predict_out_ws, 4 * static_cast<size_t>(chunk) * sizeof(double));
+  chunk = std::min(std::min(chunk, win), n);
+  int rc = predict_prepare(c, var_out != nullptr || p_out != nullptr, p_out ? n_nodes : 0);
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->predict_out_ws, 6 * static_cast<size_t>(chunk) * sizeof(double));
   if (rc != SGP_OK) return rc;
-  double* out = c->predict_out_ws.as<double>();      // [2][mean (chunk) | var (chunk)]
+  double* out = c->predict_out_ws.as<double>();      // [2][mean (chunk) | var (chunk) | p (chunk)]
   auto copy_out = [&](int b, long long p0, long long cn) -> int {
-    const double* dm = out + 2 * static_cast<size_t>(chunk) * b;
+    const double* dm = out + 3 * static_cast<size_t>(chunk) * b;
     SGP_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->out_ready[b], 0));
-    SGP_CUDA(c, cudaMemcpyAsync(mean_out + p0, dm, static_cast<size_t>(cn) * 8, cudaMemcpyDeviceToHost, c->copy_stream));
+    if (mean_out)
+      SGP_CUDA(c, cudaMemcpyAsync(mean_out + p0, dm, static_cast<size_t>(cn) * 8, cudaMemcpyDeviceToHost,
+                                  c->copy_stream));
     if (var_out)
       SGP_CUDA(c, cudaMemcpyAsync(var_out + p0, dm + chunk, static_cast<size_t>(cn) * 8, cudaMemcpyDeviceToHost,
+                                  c->copy_stream));
+    if (p_out)
+      SGP_CUDA(c, cudaMemcpyAsync(p_out + p0, dm + 2 * chunk, static_cast<size_t>(cn) * 8, cudaMemcpyDeviceToHost,
                                   c->copy_stream));
     SGP_CUDA(c, cudaEventRecord(c->out_free[b], c->copy_stream));
     return SGP_OK;
@@ -733,9 +735,10 @@ int sgp_predict(sgp_ctx* h, const double* X, int64_t n, double* mean_out, double
   rc = stage_rows(c, X, nullptr, n, row, chunk, chunk,
                   [&](const void* dX, const double*, long long p0, long long cn) -> int {
                     const int b = static_cast<int>(windows & 1);
-                    double* dm = out + 2 * static_cast<size_t>(chunk) * b;
+                    double* dm = out + 3 * static_cast<size_t>(chunk) * b;
                     SGP_CUDA(c, cudaStreamWaitEvent(c->stream, c->out_free[b], 0));
-                    int r = predict_window(c, dX, 0, cn, dm, var_out ? dm + chunk : nullptr);
+                    int r = predict_window(c, dX, 0, cn, dm, var_out ? dm + chunk : nullptr,
+                                           p_out ? dm + 2 * chunk : nullptr);
                     if (r != SGP_OK) return r;
                     SGP_CUDA(c, cudaEventRecord(c->out_ready[b], c->stream));
                     if (windows > 0 && (r = copy_out(b ^ 1, pending_p0, pending_n)) != SGP_OK) return r;
@@ -750,23 +753,84 @@ int sgp_predict(sgp_ctx* h, const double* X, int64_t n, double* mean_out, double
   return SGP_OK;
 }
 
+// The device entries' shared body: windows of device-resident points, outputs written in place (dMean may be nullptr
+// with dP: the mean then lands in the workspace).
+int predict_device(Ctx* c, const void* dX, int x_is_f32, long long n, int n_nodes, double* dMean, double* dVar,
+                   double* dP) {
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  int rc = predict_prepare(c, dVar != nullptr || dP != nullptr, dP ? n_nodes : 0);
+  if (rc != SGP_OK) return rc;
+  const long long win = predict_window_points(c->m_pad);
+  const size_t row = static_cast<size_t>(c->d) * (x_is_f32 ? sizeof(float) : sizeof(double));
+  for (long long p0 = 0; p0 < n; p0 += win) {
+    const long long cn = (n - p0 < win) ? (n - p0) : win;
+    rc = predict_window(c, static_cast<const char*>(dX) + static_cast<size_t>(p0) * row, x_is_f32, cn,
+                        dMean ? dMean + p0 : nullptr, dVar ? dVar + p0 : nullptr, dP ? dP + p0 : nullptr);
+    if (rc != SGP_OK) return rc;
+  }
+  return SGP_OK;
+}
+
+int check_nodes(Ctx* c, int32_t n_nodes) {
+  if (n_nodes < 1 || n_nodes > kMaxHermiteNodes)
+    return fail(c, SGP_E_BADARG, "n_nodes must be in [1, " + std::to_string(kMaxHermiteNodes) + "]");
+  return SGP_OK;
+}
+}  // namespace
+
+int sgp_predict(sgp_ctx* h, const double* X, int64_t n, double* mean_out, double* var_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!c->has_magic) return fail(c, SGP_E_STATE, "sgp_magic should have been called first");
+  if (n < 0 || (n > 0 && (!X || !mean_out))) return fail(c, SGP_E_BADARG, "null argument");
+  if (n == 0) return SGP_OK;
+  return predict_host(c, X, n, 0, mean_out, var_out, nullptr);
+}
+
 int sgp_predict_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, int64_t n, double* dMean, double* dVar) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
   if (!c->has_magic) return fail(c, SGP_E_STATE, "sgp_magic should have been called first");
   if (n < 0 || (n > 0 && (!dX || !dMean))) return fail(c, SGP_E_BADARG, "null argument");
   if (n == 0) return SGP_OK;
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  int rc = predict_prepare(c, dVar != nullptr);
+  return predict_device(c, dX, x_is_f32, n, 0, dMean, dVar, nullptr);
+}
+
+int sgp_predict_probability(sgp_ctx* h, const double* X, int64_t n, int32_t n_nodes, double* p_out, double* mean_out,
+                            double* var_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!c->has_magic) return fail(c, SGP_E_STATE, "sgp_magic should have been called first");
+  int rc = check_nodes(c, n_nodes);
   if (rc != SGP_OK) return rc;
-  const long long win = predict_window_points(c->m_pad);
-  const size_t row = static_cast<size_t>(c->d) * (x_is_f32 ? sizeof(float) : sizeof(double));
-  for (long long p0 = 0; p0 < n; p0 += win) {
-    const long long cn = (n - p0 < win) ? (n - p0) : win;
-    rc = predict_window(c, static_cast<const char*>(dX) + static_cast<size_t>(p0) * row, x_is_f32, cn, dMean + p0,
-                        dVar ? dVar + p0 : nullptr);
-    if (rc != SGP_OK) return rc;
-  }
+  if (n < 0 || (n > 0 && (!X || !p_out))) return fail(c, SGP_E_BADARG, "null argument");
+  if (n == 0) return SGP_OK;
+  return predict_host(c, X, n, n_nodes, mean_out, var_out, p_out);
+}
+
+int sgp_predict_probability_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, int64_t n, int32_t n_nodes, double* dP,
+                                   double* dMean, double* dVar) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!c->has_magic) return fail(c, SGP_E_STATE, "sgp_magic should have been called first");
+  int rc = check_nodes(c, n_nodes);
+  if (rc != SGP_OK) return rc;
+  if (n < 0 || (n > 0 && (!dX || !dP))) return fail(c, SGP_E_BADARG, "null argument");
+  if (n == 0) return SGP_OK;
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  const char* entry = "sgp_predict_probability_device";
+  rc = device_ptr_ok(c, dX, entry, "X");
+  if (rc == SGP_OK) rc = device_ptr_ok(c, dP, entry, "p_out");
+  if (rc == SGP_OK && dMean) rc = device_ptr_ok(c, dMean, entry, "mean_out");
+  if (rc == SGP_OK && dVar) rc = device_ptr_ok(c, dVar, entry, "var_out");
+  if (rc != SGP_OK) return rc;
+  return predict_device(c, dX, x_is_f32, n, n_nodes, dMean, dVar, dP);
+}
+
+int sgp_gauss_hermite_rule(int32_t n, double* nodes, double* weights) {
+  if (!gauss_hermite_rule(n, nodes, weights))
+    return fail(nullptr, SGP_E_BADARG, "sgp_gauss_hermite_rule: n must be in [1, " + std::to_string(kMaxHermiteNodes) +
+                                           "] and the outputs non-null");
   return SGP_OK;
 }
 

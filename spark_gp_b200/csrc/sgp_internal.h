@@ -196,7 +196,9 @@ struct Ctx {
   DevScratch dMagicMat;          // m x m
   DevScratch dMagicPacked;       // m_pad x m_pad  triu(M + M^T, 1) + diag(M), built by the first variance call
   bool magic_packed = false;     // dMagicPacked holds the installed magicMatrix
-  DevScratch predict_out_ws;     // sgp_predict: [2][mean | var] per window (double buffered)
+  DevScratch predict_out_ws;     // sgp_predict*: [2][mean | var | p] per window (double buffered)
+  DevScratch dGhRule;            // [nodes | weights] of the gh_nodes-node Gauss-Hermite rule (sgp_predict_probability*)
+  int gh_nodes = 0;              // 0: none uploaded yet
   // host->device staging (double buffered)
   DevScratch stage_x[2], stage_y[2];
   cudaEvent_t stage_free[2] = {nullptr, nullptr};   // recorded when the kernel consuming buffer i is done
@@ -267,11 +269,18 @@ struct PredictArgs {
   const double* v;       // m: magic vector
   const double* B;       // m_pad x m_pad packed magic matrix (launch_pack_magic); variance only
   double* ws;            // predict_ws_bytes(window, m_pad); variance only
-  double* mean;          // n
-  double* var;           // n, or nullptr: mean only
+  double* mean;          // n; nullptr only with prob (the mean then lands in ws)
+  double* var;           // n, or nullptr: mean only (or not returned by a probability call)
+  const double* rule;    // [n_nodes nodes | n_nodes weights] of the Gauss-Hermite rule; probability only
+  int n_nodes;
+  double* prob;          // n averaged probabilities, or nullptr (predict_var_reduce_kernel<true>)
 };
 long long predict_window_points(int m_pad);
 size_t predict_ws_bytes(long long window, int m_pad);
+// The n-node Gauss-Hermite rule for the weight exp(-x^2) (host code): nodes ascending, exactly symmetric.  false for n
+// outside [1, kMaxHermiteNodes] or a null output.
+constexpr int kMaxHermiteNodes = 256;
+bool gauss_hermite_rule(int n, double* nodes, double* weights);
 cudaError_t launch_pack_magic(double* B /*m_pad x m_pad*/, const double* M /*m x m*/, int m, int m_pad, cudaStream_t s);
 cudaError_t launch_predict(const PredictArgs& a, cudaStream_t s);
 
@@ -410,7 +419,9 @@ int run_kmeans(Ctx* c, const void* X, int x_is_f32, bool x_on_device, long long 
 int run_tail(Ctx* c, double* magic_vector, double* magic_matrix);
 // Prediction (tail.cu): predict_prepare sizes the workspace and packs the installed magic matrix (once per pair) for the
 // windows that follow; predict_window enqueues one window of at most predict_window_points(m_pad) device-resident points.
-int predict_prepare(Ctx* c, bool with_var);
-int predict_window(Ctx* c, const void* dX, int x_is_f32, long long n, double* dMean, double* dVar);
+// n_nodes > 0 (a probability call) also makes sure dGhRule holds that rule.  dP: the averaged probabilities (dMean may
+// then be nullptr).
+int predict_prepare(Ctx* c, bool with_var, int n_nodes = 0);
+int predict_window(Ctx* c, const void* dX, int x_is_f32, long long n, double* dMean, double* dVar, double* dP = nullptr);
 
 }  // namespace sgp

@@ -187,9 +187,22 @@ int run_tail(Ctx* c, double* magic_vector, double* magic_matrix) {
   return SGP_OK;
 }
 
-int predict_prepare(Ctx* c, bool with_var) {
+int predict_prepare(Ctx* c, bool with_var, int n_nodes) {
   if (!with_var) return SGP_OK;                       // the mean-only kernel needs no workspace
   int rc = ctx_scratch(c, c->predict_ws, predict_ws_bytes(predict_window_points(c->m_pad), c->m_pad));
+  if (rc == SGP_OK && n_nodes > 0 && n_nodes != c->gh_nodes) {
+    // once per context and rule size: a copy, not a launch, so a probability call launches what a variance call does
+    std::vector<double> rule(2 * static_cast<size_t>(n_nodes));
+    if (!gauss_hermite_rule(n_nodes, rule.data(), rule.data() + n_nodes))
+      return fail(c, SGP_E_BADARG, "n_nodes must be in [1, " + std::to_string(kMaxHermiteNodes) + "]");
+    rc = ctx_scratch(c, c->dGhRule, 2 * static_cast<size_t>(kMaxHermiteNodes) * sizeof(double));
+    if (rc != SGP_OK) return rc;
+    c->gh_nodes = 0;
+    SGP_CUDA(c, cudaMemcpyAsync(c->dGhRule.p, rule.data(), rule.size() * sizeof(double), cudaMemcpyHostToDevice,
+                                c->stream));
+    SGP_CUDA(c, cudaStreamSynchronize(c->stream));    // `rule` goes out of scope here
+    c->gh_nodes = n_nodes;
+  }
   if (rc != SGP_OK || c->magic_packed) return rc;
   rc = ctx_scratch(c, c->dMagicPacked, static_cast<size_t>(c->m_pad) * c->m_pad * sizeof(double));
   if (rc != SGP_OK) return rc;
@@ -199,7 +212,7 @@ int predict_prepare(Ctx* c, bool with_var) {
   return SGP_OK;
 }
 
-int predict_window(Ctx* c, const void* dX, int x_is_f32, long long n, double* dMean, double* dVar) {
+int predict_window(Ctx* c, const void* dX, int x_is_f32, long long n, double* dMean, double* dVar, double* dP) {
   PredictArgs a{};
   a.X = dX; a.x_is_f32 = x_is_f32; a.n = n;
   a.d = c->d; a.dpad = c->dpad; a.m = c->m; a.m_pad = c->m_pad;
@@ -207,8 +220,11 @@ int predict_window(Ctx* c, const void* dX, int x_is_f32, long long n, double* dM
   a.Zc = c->dZc.as<double>(); a.beta = c->dBeta.as<double>(); a.v = c->dMagicVec.as<double>();
   a.B = c->dMagicPacked.as<double>(); a.ws = c->predict_ws.as<double>();
   a.mean = dMean; a.var = dVar;
+  if (dP) {
+    a.rule = c->dGhRule.as<double>(); a.n_nodes = c->gh_nodes; a.prob = dP;
+  }
   SGP_CUDA(c, launch_predict(a, c->stream));
-  c->launches += dVar ? 3 : 1;
+  c->launches += (dVar || dP) ? 3 : 1;
   return SGP_OK;
 }
 

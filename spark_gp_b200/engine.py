@@ -544,6 +544,57 @@ class ProjectedProcessEngine:
         self.sync()
         return mean, var
 
+    def predict_probability(self, X, nodes: int = 100, with_mean_var: bool = False):
+        """`sgp_predict_probability`: (p, mean, var) for n x d or d host features, p the probability of class 1 averaged
+        over the latent posterior N(mean, var) with the `nodes`-node Gauss-Hermite rule (GPML eq. 3.25, as
+        commons/util/Integrator.scala computes it, a negative variance taken as 0); mean and var are those of `predict`,
+        bit for bit, or None unless with_mean_var."""
+        X = np.ascontiguousarray(X, dtype=np.float64)
+        if X.ndim == 1:
+            X = X[None, :]
+        p = np.empty(len(X))
+        mean, var = (np.empty(len(X)), np.empty(len(X))) if with_mean_var else (None, None)
+        self._check(self._lib.sgp_predict_probability(self._h, N.ptr(X), len(X), int(nodes), N.ptr(p),
+                                                      N.ptr(mean) if with_mean_var else None,
+                                                      N.ptr(var) if with_mean_var else None))
+        return p, mean, var
+
+    def predict_probability_device(self, x_ptr: int, x_is_f32: bool, n: int, nodes: int, p_ptr: int, mean_ptr: int = 0,
+                                   var_ptr: int = 0):
+        """`sgp_predict_probability_device` on device pointers (mean_ptr, var_ptr 0: not returned); asynchronous on the
+        context's stream (`sync`)."""
+        self._check(self._lib.sgp_predict_probability_device(
+            self._h, C.c_void_p(x_ptr), int(x_is_f32), n, int(nodes), C.c_void_p(p_ptr),
+            C.c_void_p(mean_ptr) if mean_ptr else None, C.c_void_p(var_ptr) if var_ptr else None))
+
+    def predict_probability_tensor(self, X, nodes: int = 100, with_mean_var: bool = False):
+        """`predict_probability` for a CUDA torch tensor on this context's device (n x d or d; float32 is read as it is,
+        other dtypes are converted to float64): (p, mean, var) as CUDA float64 tensors of n entries (mean and var None
+        unless with_mean_var), without a host round trip."""
+        import torch
+        X = device_tensor(X, self._device, "predict_probability")
+        if X.ndim == 1:
+            X = X[None, :]
+        if X.ndim != 2 or X.shape[1] != self.d:
+            raise ValueError("predict_probability: features must be n x %d" % self.d)
+        n = X.shape[0]
+        new = lambda: torch.empty(n, dtype=torch.float64, device=X.device)
+        p = new()
+        mean, var = (new(), new()) if with_mean_var else (None, None)
+        self.predict_probability_device(X.data_ptr(), X.dtype == torch.float32, n, nodes, p.data_ptr(),
+                                        mean.data_ptr() if with_mean_var else 0, var.data_ptr() if with_mean_var else 0)
+        self.sync()
+        return p, mean, var
+
+    @staticmethod
+    def gauss_hermite_rule(n: int):
+        """`sgp_gauss_hermite_rule`: the n-node Gauss-Hermite (nodes, weights) for the weight exp(-x^2), 1 <= n <= 256."""
+        lib = N.load()
+        x, w = np.empty(max(n, 0)), np.empty(max(n, 0))
+        if lib.sgp_gauss_hermite_rule(int(n), N.ptr(x), N.ptr(w)) != N.SGP_OK:
+            raise ValueError(lib.sgp_last_error(None).decode())
+        return x, w
+
     def cross_kernel(self, X):
         """kernel.crossKernel(test) with the active set as training vectors: len(test) x m."""
         X = np.ascontiguousarray(X, dtype=np.float64)

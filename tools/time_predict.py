@@ -15,12 +15,21 @@ Each is printed as a share of the H100 SXM data-sheet bound (fp64 tensor 67 TFLO
 --dump-outputs writes both builds' mean and variance (host entry) and prints the largest difference between them, relative
 to the summed magnitudes |k| |v| and selfKernel + |k| |M| |k| on a subset of rows.
 --profile runs the device entry once per shape under torch.profiler and prints the kernel times (a separate run: tracing
-slows the host)."""
+slows the host).
+
+  python tools/time_predict.py --probability [--reps 5]
+
+times the averaged probability (`sgp_predict_probability`, 100 nodes) against the mean + variance call on the same
+model, the two alternating in one process, through the device and the host entry, at 1M x 16 / m = 1000 and at the
+11769 x 784 / m = 500 shape.  The magic pair is scaled so that the variances are O(1) and of both signs, as a fitted
+model's are near zero.  It prints the card, the fused reduce kernel's time against the plain one from torch.profiler
+(a separate traced call), and the largest |p - the library's rule applied in fp64 numpy to the call's own (mean, var)|."""
 from __future__ import annotations
 
 import argparse
 import ctypes as C
 import os
+import re
 import subprocess
 import sys
 import time
@@ -108,16 +117,82 @@ def report(label, n, d, m, t, var):
                        dmma, elem, n * m, kbytes))
 
 
+def host_rule_probability(mean, var, nodes):
+    """The library's rule applied in fp64 numpy: (1/sqrt(pi)) sum_i w_i sigmoid(mean + sqrt(2 max(var, 0)) x_i)."""
+    x, w = ProjectedProcessEngine.gauss_hermite_rule(nodes)
+    out = np.empty(len(mean))
+    for s in range(0, len(mean), 65536):
+        mu, v = mean[s:s + 65536], var[s:s + 65536]
+        z = mu[:, None] + np.sqrt(2.0 * np.where(v < 0.0, 0.0, v))[:, None] * x
+        with np.errstate(over="ignore"):
+            out[s:s + 65536] = (1.0 / (1.0 + np.exp(-z))) @ w / np.sqrt(np.pi)
+    return out
+
+
+def probability(eng, reps, nodes=100):
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    for si in (0, 3):
+        n, d, m = SHAPES[si]
+        c = case(n, d, m, seed=si)
+        eng.begin(c["kernel"], c["Z"])
+        eng.set_magic(c["v"], c["M"] * 1e-4)
+        Xd = torch.from_numpy(c["X"]).to(device="cuda")
+        torch.cuda.synchronize()
+        print("n=%d d=%d m=%d, %d nodes" % (n, d, m, nodes))
+        calls = {
+            "device mean+var": lambda: eng.predict_tensor(Xd, with_variance=True),
+            "device probability": lambda: eng.predict_probability_tensor(Xd, nodes=nodes),
+            "host mean+var": lambda: eng.predict(c["X"], with_variance=True),
+            "host probability": lambda: eng.predict_probability(c["X"], nodes=nodes),
+        }
+        for f in calls.values():
+            f()
+        ts = {k: [] for k in calls}
+        for _ in range(reps):                               # alternate, so that both see the same load
+            for k, f in calls.items():
+                t0 = time.perf_counter()
+                f()
+                ts[k].append(time.perf_counter() - t0)
+        for entry in ("device", "host"):
+            mv, pr = np.median(ts[entry + " mean+var"]), np.median(ts[entry + " probability"])
+            print("  %-7s mean+var %9.3f ms   probability %9.3f ms   difference %+8.3f ms (%+.1f %%)   spread: %s / %s" % (
+                entry, mv * 1e3, pr * 1e3, (pr - mv) * 1e3, 100 * (pr - mv) / mv,
+                " ".join("%.2f" % (t * 1e3) for t in ts[entry + " mean+var"]),
+                " ".join("%.2f" % (t * 1e3) for t in ts[entry + " probability"])))
+        for label, f in (("mean+var", calls["device mean+var"]), ("probability", calls["device probability"])):
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                f()
+            for ev in prof.key_averages():
+                name = re.search(r"(predict_\w+|pack_magic_kernel)(<\w+>)?", ev.key)
+                if name:
+                    print("    %-12s kernel %-36s %9.3f ms x %d" % (label, name.group(0), ev.device_time_total / 1e3,
+                                                                  ev.count))
+        p, mean, var = eng.predict_probability(c["X"], nodes=nodes, with_mean_var=True)
+        hm, hv = eng.predict(c["X"])
+        ref = host_rule_probability(mean, var, nodes)
+        print("  mean / var equal to sgp_predict's: %s / %s;  variances < 0: %.1f %%;  max |p - host rule| = %.2e" % (
+            np.array_equal(mean, hm), np.array_equal(var, hv), 100 * np.mean(var < 0), np.abs(p - ref).max()))
+        del Xd
+        sys.stdout.flush()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", help="another libsgp.so (e.g. the parent commit's build) to time against")
     ap.add_argument("--dump-outputs", help="directory for both builds' outputs")
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--probability", action="store_true", help="time the averaged probability (see above)")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--shapes", default="0,1,2,3", help="indices into SHAPES")
     a = ap.parse_args()
     import torch
     print("card: %s" % card())
+    if a.probability:
+        eng = ProjectedProcessEngine(0)
+        probability(eng, a.reps)
+        eng.close()
+        return
     new = ProjectedProcessEngine(0)
     old = engine_on(load_other(a.lib)) if a.lib else None
     for si in [int(s) for s in a.shapes.split(",")]:
