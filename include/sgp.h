@@ -227,6 +227,24 @@ int sgp_bcm_nll_folds(sgp_ctx* ctx, const int32_t* sets, int32_t n_eval, const s
                       const sgp_hyper* hypers, int32_t n_hypers, double* nll_out /* n_eval */,
                       double* grad_out /* n_eval x n_hypers */);
 
+/* The BCM objective of sgp_bcm_nll at several kernels on the last grouped upload (sgp_experts_upload_grouped or its
+ * _device form), in one launch over experts x slots: several param maps on one training set.  Slot s evaluates every
+ * uploaded expert at kernels[s] and hypers[s * n_hypers ...] (the same kernel structure and descriptor layout in every
+ * slot).  Outputs per slot: nll_out[s], grad_out[s * n_hypers ...].
+ * Contract: slot s's value and gradient equal, bit for bit, what sgp_bcm_nll returns on the same upload with the same
+ * kernel, whatever else is in the call.  The call plans its kernel on the upload's largest expert, as sgp_bcm_nll does.
+ * A slot whose on-chip Cholesky breaks down is evaluated again on the LU path, alone; experts too large for the on-chip
+ * kernels put every slot on the LU path, one slot after another (the rules of sgp_bcm_nll_folds, whose code this entry
+ * runs with every slot on one set).  sgp_last_bcm_path is 1 if any slot ran LU.  With a communicator: one ncclAllReduce
+ * of the n_eval rows and n_eval status words.
+ * Errors: SGP_E_STATE without a grouped upload -- a fold upload or an sgp_experts_upload is refused, since neither has
+ * one training set to hand every slot; SGP_E_BADARG for n_eval outside [1, 65535], a structure or descriptor layout that
+ * differs between slots, or more than 46340 points in the largest expert (before any allocation or launch); SGP_E_NOMEM
+ * when a slot's LU workspace exceeds the device's free memory, as for sgp_bcm_nll; SGP_E_SINGULAR naming the first slot
+ * whose matrix is exactly singular. */
+int sgp_bcm_nll_slots(sgp_ctx* ctx, int32_t n_eval, const sgp_kernel_desc* kernels, const sgp_hyper* hypers,
+                      int32_t n_hypers, double* nll_out /* n_eval */, double* grad_out /* n_eval x n_hypers */);
+
 /* Binary classification (labels 0/1 in the uploaded y): per-expert Laplace approximation,
  * classification/GaussianProcessClassifier.scala:74-129 -- Newton iteration for the mode with the reference's step
  * halving, tolerance `tol` and warm start (the latent f of every uploaded point lives on the device, starts at zero

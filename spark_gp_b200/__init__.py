@@ -10,5 +10,6 @@ from .regression import (GaussianProcessRegression, GaussianProcessRegressionMod
                          GreedilyOptimizingActiveSetProvider, KMeansActiveSetProvider)
 from .classification import GaussianProcessClassifier, GaussianProcessClassificationModel, OneVsRest, OneVsRestModel
 from .utils import scale
-from .tuning import (CrossValidator, CrossValidatorModel, ParamGridBuilder, RegressionEvaluator,
-                     MulticlassClassificationEvaluator, TrainValidationSplit, TrainValidationSplitModel)
+from .tuning import (BinaryClassificationEvaluator, CrossValidator, CrossValidatorModel, ParamGridBuilder,
+                     RegressionEvaluator, MulticlassClassificationEvaluator, TrainValidationSplit,
+                     TrainValidationSplitModel)

@@ -29,7 +29,7 @@ EXPORTS = ["sgp_ctx_create", "sgp_ctx_destroy", "sgp_last_error", "sgp_set_preci
            "sgp_experts_upload_folds_device", "sgp_experts_get_f_rows_device", "sgp_kmeans_device",
            "sgp_greedy_active_set_device", "sgp_laplace_nll_fold_slots_any_size", "sgp_experts_get_f_fold_slot",
            "sgp_experts_get_f_fold_rows_device", "sgp_gauss_hermite_rule", "sgp_predict_probability",
-           "sgp_predict_probability_device"]
+           "sgp_predict_probability_device", "sgp_bcm_nll_slots"]
 
 
 class KernelTerm(C.Structure):
@@ -109,6 +109,7 @@ def load() -> C.CDLL:
     lib.sgp_experts_get_f_slot.argtypes = [vp, i32, vp]
     lib.sgp_experts_upload_folds.argtypes = [vp, vp, i32, vp, i64, i32, vp, i32, i32]
     lib.sgp_bcm_nll_folds.argtypes = [vp, vp, i32, vp, vp, i32, vp, vp]
+    lib.sgp_bcm_nll_slots.argtypes = [vp, i32, vp, vp, i32, vp, vp]
     lib.sgp_experts_upload_grouped_device.argtypes = lib.sgp_experts_upload_grouped.argtypes
     lib.sgp_experts_upload_folds_device.argtypes = lib.sgp_experts_upload_folds.argtypes
     lib.sgp_experts_get_f_rows_device.argtypes = [vp, i32, i32, vp]

@@ -927,7 +927,10 @@ int upload_grouped(Ctx* c, bool on_device, const void* X, int x_is_f32, const do
   const long long E = static_cast<long long>(std::floor(static_cast<double>(n) / dataset_size_for_expert + 0.5));
   if (E <= 0) return fail(c, SGP_E_BADARG, "numberOfExperts == 0 (N < datasetSizeForExpert / 2): the reference fails with / by zero");
   int rc = experts_alloc(c, E, n, d, static_cast<int>(n / E + ((n % E) ? 1 : 0)));
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_set_first, 2 * 8);
   if (rc != SGP_OK) return rc;
+  const long long one_set[2] = {0, E};        // the upload as one set, for sgp_bcm_nll_slots (synchronised below)
+  SGP_CUDA(c, cudaMemcpyAsync(c->ex_set_first.p, one_set, sizeof(one_set), cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, launch_expert_offsets(c->ex.off, n, E, 0, c->stream));
   // host input streams through the double-buffered staging area of the statistics path; either way the gather is on the
   // device, chunk by chunk
@@ -1281,30 +1284,25 @@ int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   return objective_finish(c, o, nh, nll_out, grad_out, 2, SGP_E_SINGULAR, kBcmSingular);
 }
 
-int sgp_bcm_nll_folds(sgp_ctx* h, const int32_t* sets, int32_t n_eval, const sgp_kernel_desc* kernels,
-                      const sgp_hyper* hypers, int32_t nh, double* nll_out, double* grad_out) {
-  Ctx* c = reinterpret_cast<Ctx*>(h);
-  if (!c) return SGP_E_BADARG;
-  if (!nll_out || (nh > 0 && !grad_out) || !sets) return fail(c, SGP_E_BADARG, "sgp_bcm_nll_folds: null argument");
-  if (c->ex.E == 0 || c->fold_first.empty())
-    return fail(c, SGP_E_STATE, "sgp_experts_upload_folds should have been called first");
-  const int n_sets = static_cast<int>(c->fold_first.size()) - 1;
-  if (n_eval < 1 || n_eval > 65535) return fail(c, SGP_E_BADARG, "sgp_bcm_nll_folds: need 1 <= n_eval <= 65535");
-  for (int s = 0; s < n_eval; ++s)
-    if (sets[s] < 0 || sets[s] >= n_sets)
-      return fail(c, SGP_E_BADARG, "sgp_bcm_nll_folds: set index " + std::to_string(sets[s]) + " outside [0, n_folds)");
+namespace {
+// The BCM objective of n_eval slots over expert sets of the upload, in one on-chip launch over experts x slots: slot s
+// evaluates set k = sets[s] (the experts first[k] .. first[k+1]-1, the largest of nmax[k] points; c->ex_set_first holds
+// first on the device) at kernels[s] and hypers + s * nh.  The set indices are the caller's to check.  A failing slot is
+// named `what` names[s].
+int bcm_nll_sets(Ctx* c, const char* fn, const int32_t* sets, int n_eval, const std::vector<long long>& first,
+                 const std::vector<int>& nmax, const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int nh,
+                 double* nll_out, double* grad_out, const int* names, const char* what) {
   SGP_CUDA(c, cudaSetDevice(c->device));
-  const std::vector<long long>& first = c->fold_first;
   // one plan for the call, on the largest expert over the listed sets; the kernel lays out its shared memory from the
   // same n_max, so it launches on this view
   ExpertSet listed = c->ex;
   long long E_max = 0;
   listed.n_max = 0;
   for (int s = 0; s < n_eval; ++s) {
-    listed.n_max = std::max(listed.n_max, c->fold_nmax[sets[s]]);
+    listed.n_max = std::max(listed.n_max, nmax[sets[s]]);
     E_max = std::max(E_max, first[sets[s] + 1] - first[sets[s]]);
   }
-  int rc = bcm_check_size(c, listed.n_max, "sgp_bcm_nll_folds");
+  int rc = bcm_check_size(c, listed.n_max, fn);
   if (rc != SGP_OK) return rc;
   ObjectiveSetup o;
   rc = objective_setup(c, n_eval, kernels, hypers, nh, sets, o, E_max);
@@ -1332,7 +1330,7 @@ int sgp_bcm_nll_folds(sgp_ctx* h, const int32_t* sets, int32_t n_eval, const sgp
     ExpertSet set = c->ex;
     set.off = c->ex.off + first[k];
     set.E = first[k + 1] - first[k];
-    set.n_max = c->fold_nmax[k];
+    set.n_max = nmax[k];
     HyperView hv = o.hv;
     hv.kf = o.kf_host[s];
     hv.beta += s * o.slot_stride; hv.h_coef += s * o.slot_stride; hv.h_value += s * o.slot_stride;
@@ -1347,7 +1345,41 @@ int sgp_bcm_nll_folds(sgp_ctx* h, const int32_t* sets, int32_t n_eval, const sgp
     if (blas_status != 0) return fail(c, SGP_E_CUDA, "cuBLAS batched LU failed, status " + std::to_string(blas_status));
     c->launches += 5;
   }
-  return objective_finish(c, o, nh, nll_out, grad_out, 2, SGP_E_SINGULAR, kBcmSingular, sets, "fold set");
+  return objective_finish(c, o, nh, nll_out, grad_out, 2, SGP_E_SINGULAR, kBcmSingular, names, what);
+}
+}  // namespace
+
+int sgp_bcm_nll_folds(sgp_ctx* h, const int32_t* sets, int32_t n_eval, const sgp_kernel_desc* kernels,
+                      const sgp_hyper* hypers, int32_t nh, double* nll_out, double* grad_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!nll_out || (nh > 0 && !grad_out) || !sets) return fail(c, SGP_E_BADARG, "sgp_bcm_nll_folds: null argument");
+  if (c->ex.E == 0 || c->fold_first.empty())
+    return fail(c, SGP_E_STATE, "sgp_experts_upload_folds should have been called first");
+  const int n_sets = static_cast<int>(c->fold_first.size()) - 1;
+  if (n_eval < 1 || n_eval > 65535) return fail(c, SGP_E_BADARG, "sgp_bcm_nll_folds: need 1 <= n_eval <= 65535");
+  for (int s = 0; s < n_eval; ++s)
+    if (sets[s] < 0 || sets[s] >= n_sets)
+      return fail(c, SGP_E_BADARG, "sgp_bcm_nll_folds: set index " + std::to_string(sets[s]) + " outside [0, n_folds)");
+  return bcm_nll_sets(c, "sgp_bcm_nll_folds", sets, n_eval, c->fold_first, c->fold_nmax, kernels, hypers, nh, nll_out,
+                      grad_out, sets, "fold set");
+}
+
+int sgp_bcm_nll_slots(sgp_ctx* h, int32_t n_eval, const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t nh,
+                      double* nll_out, double* grad_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  if (!nll_out || (nh > 0 && !grad_out)) return fail(c, SGP_E_BADARG, "sgp_bcm_nll_slots: null argument");
+  if (c->ex.E == 0 || !c->ex_grouped)
+    return fail(c, SGP_E_STATE, "sgp_experts_upload_grouped should have been called first (sgp_bcm_nll_slots evaluates "
+                                "one grouped training set; a fold upload or sgp_experts_upload has none)");
+  if (n_eval < 1 || n_eval > 65535) return fail(c, SGP_E_BADARG, "sgp_bcm_nll_slots: need 1 <= n_eval <= 65535");
+  // every slot on the upload's one set, {0, E} (in c->ex_set_first since the grouped upload); slots are named by index
+  const std::vector<int32_t> zeros(n_eval, 0);
+  std::vector<int> slot(n_eval);
+  for (int s = 0; s < n_eval; ++s) slot[s] = s;
+  return bcm_nll_sets(c, "sgp_bcm_nll_slots", zeros.data(), n_eval, {0, c->ex.E}, {c->ex.n_max}, kernels, hypers, nh,
+                      nll_out, grad_out, slot.data(), "slot");
 }
 
 const char* const kLaplaceRefused =

@@ -184,7 +184,7 @@ struct Ctx {
   std::vector<long long> fold_first;   // [n_sets + 1]
   std::vector<int> fold_nmax;          // [n_sets] largest expert of each set
   std::vector<long long> fold_row0;    // [n_sets + 1] first row of each set
-  DevScratch ex_set_first;             // device copy of fold_first
+  DevScratch ex_set_first;             // device copy of fold_first; {0, E} after a grouped upload (one set)
   DevScratch fold_pos_ws;              // upload scratch: the point indices grouped by fold, ascending in each fold
   DevScratch nll_per_ws;         // per-expert objective rows
   DevScratch hyper_ws;           // hyper-parameter descriptors + totals + flags of one evaluation
@@ -357,7 +357,7 @@ ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms);
 size_t laplace_smem_bytes(int n_max);   // laplace_kernel without the staged rows (laplace.cu)
 size_t laplace_global_cta_bytes(int n_max);   // laplace_global_kernel's workspace per CTA (laplace_global.cu)
 
-// Fold slots of a BCM launch (sgp_bcm_nll_folds): slot s evaluates the experts first[sets[s]] .. first[sets[s] + 1] - 1
+// Fold slots of a BCM launch (sgp_bcm_nll_folds; sgp_bcm_nll_slots lists set 0 of a grouped upload's {0, E}): slot s evaluates the experts first[sets[s]] .. first[sets[s] + 1] - 1
 // of a fold upload with the flattened kernel kf[s] and the descriptor values slot_stride doubles per slot after hv's.
 // rows: [n_slots][E_max][1 + n_hypers], total: [n_slots][1 + n_hypers], flags: [n_slots].
 struct BcmFolds {

@@ -395,6 +395,14 @@ class ProjectedProcessEngine:
             raise ValueError("bcm_nll_folds: one kernel per listed set")
         return self._batched_objective(self._lib.sgp_bcm_nll_folds, (N.ptr(st), len(st)), kernels)
 
+    def bcm_nll_slots(self, kernels):
+        """The BCM objective of the last `experts_upload_grouped` at each of kernels, all in one launch
+        (`sgp_bcm_nll_slots`): slot i is `bcm_nll(kernels[i])`, bit for bit.  Returns (values [n_eval], gradients
+        [n_eval x n_hypers])."""
+        if len(kernels) == 0:
+            raise ValueError("bcm_nll_slots: at least one kernel")
+        return self._batched_objective(self._lib.sgp_bcm_nll_slots, (len(kernels),), kernels)
+
     def laplace_nll_classes(self, n_classes: int, classes, kernels, tol: float):
         """One-vs-rest over uploaded class indices: the binary Laplace objective of each listed class c (labels y == c)
         at its own kernels[i], all in one launch (`sgp_laplace_nll_classes`).  Returns (values [n_eval], gradients

@@ -1,5 +1,5 @@
 """Model selection: Spark 3.1's `ParamGridBuilder`, `RegressionEvaluator`, `MulticlassClassificationEvaluator`,
-`CrossValidator` (regression estimator and one-vs-rest) and `TrainValidationSplit` (any estimator), as the reference's own
+`BinaryClassificationEvaluator`, `CrossValidator` (regression estimator and one-vs-rest) and `TrainValidationSplit` (any estimator), as the reference's own
 examples use them (regression/examples/GPExample.scala:17-27, Airfoil.scala:18-24, Synthetics.scala:25-33: 10-fold
 cross-validation of the RMSE; classification/examples/Iris.scala: 10-fold cross-validation of one-vs-rest scored by
 accuracy; classification/examples/MNIST.scala:34-40: a train/validation split scored by accuracy).
@@ -41,7 +41,13 @@ Over the binary classifier and one-vs-rest, the maps are grouped by `slot_group_
 training rows are uploaded once, and every (map p, class c) is one slot with mode slot p * C + c (binary: C = 1, class 1)
 in `sgp_laplace_nll_slots_any_size`, so each round of the slots' L-BFGS-B runs is one launch.  Each slot's values and
 modes equal the independent fit's bit for bit, so every validation prediction is that of
-`estimator.copy(map).fit(X[train], y[train])`.  Regression maps are fitted one after another.
+`estimator.copy(map).fit(X[train], y[train])`.  Over regression, the maps are grouped by `slot_group_key` too; a
+group's training rows are uploaded once (`sgp_experts_upload_grouped`), and each round of its maps' L-BFGS-B runs is one
+`sgp_bcm_nll_slots` launch, each map's values equal to the independent fit's bit for bit; each map's model is then
+produced on the training rows at its theta.
+A BinaryClassificationEvaluator (Spark 3.1's, over rawPrediction(1) = f; see `binary_metric`) is accepted over the
+binary classifier only, and scores each map's validation latent mean f; over any other estimator `fit` raises TypeError.
+CrossValidator does not take it, as it does not take the binary classifier.
 
 Both selectors take X (and y) as CUDA tensors on the estimator's device as well: the fold upload reads them in place
 (`sgp_experts_upload_folds_device`), the training and validation rows are gathered on the device and predicted there, and
@@ -164,6 +170,70 @@ class MulticlassClassificationEvaluator(_Evaluator):
 
     def __init__(self, metricName: str = "f1"):
         self.setMetricName(metricName)
+
+    def isLargerBetter(self) -> bool:
+        return True
+
+
+def binary_metric(name: str, y, scores, num_bins: int = 1000) -> float:
+    """Spark 3.1's BinaryClassificationMetrics(scoreAndLabels, numBins) for one metric name, unweighted, on one partition.
+    The distinct scores in descending order are the curve's points, each with its counts of labels 1 and 0.  With
+    numBins > 0 and g = (distinct scores) // numBins >= 2, every g consecutive points are merged into one at the run's
+    last (smallest) score, and the points left over into a last one; Spark merges within each partition, so its curve
+    depends on the partitioning (this is its one-partition curve).  Cumulative counts give each point's recall TP / P
+    (0 when P = 0), false positive rate FP / N (0 when N = 0) and precision TP / (TP + FP).  areaUnderROC is the
+    trapezoidal area under (0, 0), (FPR, recall)..., (1, 1); areaUnderPR under (0, first precision),
+    (recall, precision)...; the trapezoids are summed in curve order."""
+    if name not in BinaryClassificationEvaluator.METRICS:
+        raise ValueError("metricName must be one of %s, not %r" % (", ".join(BinaryClassificationEvaluator.METRICS),
+                                                                  name))
+    y = np.asarray(y, dtype=np.float64)
+    s = np.asarray(scores, dtype=np.float64)
+    if len(y) == 0 or s.shape != y.shape:
+        raise ValueError("BinaryClassificationEvaluator: labels and scores must be non-empty vectors of one length")
+    if not np.all((y == 0.0) | (y == 1.0)):
+        raise ValueError("BinaryClassificationEvaluator: labels must be 0 or 1")
+    if np.isnan(s).any():
+        raise ValueError("BinaryClassificationEvaluator: a score is NaN")
+    distinct, inv = np.unique(s, return_inverse=True)
+    n = len(distinct)
+    pos = np.bincount(inv[y == 1.0], minlength=n)[::-1]          # descending scores
+    neg = np.bincount(inv, minlength=n)[::-1] - pos
+    g = n // num_bins if num_bins > 0 else 0
+    ends = np.arange(n) if g < 2 else np.unique(np.append(np.arange(g - 1, n, g), n - 1))
+    tp, fp = np.cumsum(pos)[ends], np.cumsum(neg)[ends]
+    P, N_ = tp[-1], fp[-1]
+    recall = tp / P if P > 0 else np.zeros(len(ends))
+    if name == "areaUnderROC":
+        fpr = fp / N_ if N_ > 0 else np.zeros(len(ends))
+        x, v = np.concatenate([[0.0], fpr, [1.0]]), np.concatenate([[0.0], recall, [1.0]])
+    else:
+        precision = tp / (tp + fp)                                  # every point holds a row: tp + fp > 0
+        x, v = np.concatenate([[0.0], recall]), np.concatenate([precision[:1], precision])
+    return float(np.cumsum((x[1:] - x[:-1]) * (v[1:] + v[:-1]) / 2.0)[-1])
+
+
+class BinaryClassificationEvaluator(_Evaluator):
+    """Spark's BinaryClassificationEvaluator over (label, rawPrediction(1)): areaUnderROC (default) or areaUnderPR,
+    larger-is-better, with numBins (default 1000; 0 keeps every distinct score) as in `binary_metric`.  `evaluate(y,
+    scores)` takes 0/1 labels and the raw score; for GaussianProcessClassifier that is the latent mean f."""
+    METRICS = ("areaUnderROC", "areaUnderPR")
+
+    def __init__(self, metricName: str = "areaUnderROC", numBins: int = 1000):
+        self.setMetricName(metricName)
+        self.setNumBins(numBins)
+
+    def setNumBins(self, value: int):
+        if int(value) != value or not (value == 0 or value > 1):
+            raise ValueError("BinaryClassificationEvaluator: numBins must be 0 or an integer > 1")
+        self._num_bins = int(value)
+        return self
+
+    def getNumBins(self) -> int:
+        return self._num_bins
+
+    def _metric_of(self, name, y, scores):
+        return binary_metric(name, y, scores, self._num_bins)
 
     def isLargerBetter(self) -> bool:
         return True
@@ -463,7 +533,7 @@ class TrainValidationSplitModel(_SelectedModel):
 class TrainValidationSplit(_Validator):
     NAME = "TrainValidationSplit"
     ESTIMATORS = (GaussianProcessRegression, GaussianProcessClassifier, OneVsRest)
-    EVALUATORS = (RegressionEvaluator, MulticlassClassificationEvaluator)
+    EVALUATORS = (RegressionEvaluator, MulticlassClassificationEvaluator, BinaryClassificationEvaluator)
 
     def __init__(self):
         self._estimator = None
@@ -481,9 +551,12 @@ class TrainValidationSplit(_Validator):
         return self
 
     def setEvaluator(self, value):
+        """A RegressionEvaluator, a MulticlassClassificationEvaluator (on the predictions) or, over the binary
+        GaussianProcessClassifier only, a BinaryClassificationEvaluator (on the validation latent mean f)."""
         if not isinstance(value, self.EVALUATORS):
-            raise TypeError("TrainValidationSplit: the evaluator must be a RegressionEvaluator or a "
-                            "MulticlassClassificationEvaluator, not %s" % type(value).__name__)
+            raise TypeError("TrainValidationSplit: the evaluator must be a RegressionEvaluator, a "
+                            "MulticlassClassificationEvaluator or a BinaryClassificationEvaluator, not %s"
+                            % type(value).__name__)
         self._evaluator = value
         return self
 
@@ -503,6 +576,10 @@ class TrainValidationSplit(_Validator):
             raise TypeError("TrainValidationSplit: setEstimator first")
         if self._evaluator is None:
             raise ValueError("TrainValidationSplit: setEvaluator first (there is no default evaluator)")
+        scored = isinstance(self._evaluator, BinaryClassificationEvaluator)
+        if scored and not isinstance(est, GaussianProcessClassifier):
+            raise TypeError("TrainValidationSplit: a BinaryClassificationEvaluator scores the binary "
+                            "GaussianProcessClassifier only, not a %s" % type(est).__name__)
         gp = est.getClassifier() if isinstance(est, OneVsRest) else est
         X, y = self._data(X, y, getattr(gp, "_device", 0))           # a OneVsRest without a classifier fails below
         if train is None:
@@ -519,31 +596,64 @@ class TrainValidationSplit(_Validator):
         ests = [est.copy(m) for m in maps]
         if isinstance(est, GaussianProcessRegression):
             preds, objective = self._fit_regression(ests, X, y, mask)
+            evaluated = preds
         else:
-            preds, objective = self._fit_classifiers(ests, isinstance(est, OneVsRest), X, y, mask)
+            preds, raw, objective = self._fit_classifiers(ests, isinstance(est, OneVsRest), X, y, mask)
+            evaluated = [r[:, 0] for r in raw] if scored else preds      # rawPrediction(1) = f
         y_val = host_copy(_rows(y, ~mask))
-        metrics = [self._evaluator.evaluate(y_val, p) for p in preds]
+        metrics = [self._evaluator.evaluate(y_val, p) for p in evaluated]
         best = best_index(metrics, self._evaluator.isLargerBetter())
         self.last_predictions = preds
         return TrainValidationSplitModel(est.copy(maps[best]).fit(X, y), metrics, best, objective)
 
     @staticmethod
     def _fit_regression(ests, X, y, train):
-        """Each map fitted on its own: a batched BCM launch over maps on one upload does not exist (a fold upload would
-        refuse validation sides the independent fit takes)."""
-        preds, maps = [], []
-        for e in ests:
-            model = e.fit(_rows(X, train), _rows(y, train))
-            preds.append(_host_predictions(model.predict(_rows(X, ~train))))
-            maps.append(e.last_objective)
-            del model
-        return preds, dict(maps=maps)
+        """Validation predictions of every map of the regression estimator, and what the optimisation took: per group of
+        maps (`group_slots`) one grouped upload of the training rows and one lock-step L-BFGS-B over the maps, each
+        round one `sgp_bcm_nll_slots` launch.  A group with maxIter <= 0 takes its kernels' own hyper-parameters, as
+        GPR.fit does.  Each map's model is then produced on the training rows.  Returns (predictions, dict(maps=[each
+        map's dict(theta, magicVector, evaluations, iterations; value and n_experts when optimised)],
+        groups=[dict(maps, rounds, launches)]))."""
+        Xt, yt, Xv = _rows(X, train), _rows(y, train), _rows(X, ~train)
+        x0s = [e.getKernel().getHyperparameters() for e in ests]
+        thetas = [np.asarray(x0, dtype=np.float64) for x0 in x0s]
+        records, groups = [dict(evaluations=0, iterations=0) for _ in ests], []
+        for slots in group_slots(ests, 1).values():
+            e0 = ests[slots[0][0]]
+            if e0._maxIter <= 0:
+                continue
+            eng = ProjectedProcessEngine.acquire(e0._device)
+            try:
+                n_experts = eng.experts_upload_grouped(Xt, yt, e0._datasetSizeForExpert)
+                launches0 = eng.launch_count()
+                kernel_at = lambda p, t: ests[p].getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
+
+                def evaluate(batch):
+                    vals, grads = eng.bcm_nll_slots([kernel_at(slots[i][0], t) for i, t in batch])
+                    return [(float(v), g) for v, g in zip(vals, grads)]
+
+                fitted, recs, rounds = optimise_slots(evaluate, [x0s[p] for p, _ in slots],
+                                                      lbfgsb_bounds(e0.getKernel()), e0._maxIter, e0._tol)
+                groups.append(dict(maps=[p for p, _ in slots], rounds=rounds, launches=eng.launch_count() - launches0))
+            finally:
+                eng.release()
+            for (p, _), theta, r in zip(slots, fitted, recs):
+                thetas[p] = theta
+                records[p] = dict(r, n_experts=n_experts)
+        preds = []
+        for e, theta, r in zip(ests, thetas, records):
+            model = e._produce_model(Xt, yt, theta)
+            preds.append(_host_predictions(model.predict(Xv)))
+            r.update(theta=theta, magicVector=model.rawPredictor.magicVector)
+            del model                             # its context goes back to the pool before the next map
+        return preds, dict(maps=records, groups=groups)
 
     @staticmethod
     def _fit_classifiers(ests, ovr: bool, X, y, train):
-        """Validation predictions of every map of the binary classifier (ovr False) or of one-vs-rest, and what the
-        optimisation took: per group of maps one upload, one lock-step L-BFGS-B over the (map, class) slots, one
-        `sgp_laplace_nll_slots_any_size` call per round and one at every slot's optimum (GPCls:60)."""
+        """Validation predictions of every map of the binary classifier (ovr False) or of one-vs-rest, their raw
+        columns (each class's latent mean f), and what the optimisation took: per group of maps one upload, one
+        lock-step L-BFGS-B over the (map, class) slots, one `sgp_laplace_nll_slots_any_size` call per round and one at
+        every slot's optimum (GPCls:60)."""
         gps = [e.getClassifier() for e in ests] if ovr else ests
         if any(not isinstance(gp, GaussianProcessClassifier) for gp in gps):
             raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
@@ -594,4 +704,4 @@ class TrainValidationSplit(_Validator):
             preds = [one_vs_rest_prediction(r) for r in raw]
         else:                                               # GaussianProcessClassificationModel.predict
             preds = [np.argmax(np.stack([-r[:, 0], r[:, 0]], axis=-1), axis=-1).astype(np.float64) for r in raw]
-        return preds, dict(groups=groups)
+        return preds, raw, dict(groups=groups)

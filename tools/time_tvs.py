@@ -2,7 +2,7 @@
 wall time, optimisation rounds against evaluations, objective launches (sgp_launch_count over the optimisation),
 validationMetrics, and a check that both ways give the same validation predictions, bit for bit.
 
-  python tools/time_tvs.py [--reps 3] [--out DIR]
+  python tools/time_tvs.py [--reps 3] [--out DIR] [--workloads mnist68 ovr10 reg8]
 
 Workloads:
   mnist68    the 1600 rows of tests/golden/mnist68_case.npz (784 features, classification/examples/MNIST.scala's 6-vs-8
@@ -10,6 +10,8 @@ Workloads:
              100, default maxIter (100), trainRatio 0.8, accuracy
   ovr10      a 10-class one-vs-rest shard, 200 000 x 8, sigma2 in 1, 2, RBFKernel(2.0), datasetSizeForExpert 100,
              activeSetSize 500, maxIter 10 (as tools/time_ovr.py), trainRatio 0.8, f1
+  reg8       a regression shard, 200 000 x 8, sigma2 in 0.5, 1, 2, 1.0 * ARDRBFKernel(8), datasetSizeForExpert
+             100, activeSetSize 500, maxIter 10, trainRatio 0.8, rmse
 Both sides run the whole selection except the refit of the best map on all rows, which is the same call on both.  After
 one untimed run of each, each time is the median of --reps runs, the two ways alternated."""
 from __future__ import annotations
@@ -58,11 +60,25 @@ def ovr10(n=200_000, d=8, C=10):
     return X, lab.astype(np.float64), sg.OneVsRest().setClassifier(gp), maps, sg.MulticlassClassificationEvaluator("f1")
 
 
+def reg8(n=200_000, d=8):
+    rng = np.random.default_rng(8)
+    X = rng.standard_normal((n, d))
+    y = np.sin(X[:, 0]) + 0.5 * X[:, 1] * X[:, 2] + 0.1 * rng.standard_normal(n)
+    gp = (sg.GaussianProcessRegression().setDatasetSizeForExpert(100).setActiveSetSize(500).setMaxIter(10)
+          .setKernel(lambda: 1.0 * sg.ARDRBFKernel(d)))
+    maps = sg.ParamGridBuilder().addGrid("sigma2", [0.5, 1.0, 2.0]).build()
+    return X, y, gp, maps, sg.RegressionEvaluator("rmse")
+
+
 def batched(X, y, est, maps, ev, mask):
     """TrainValidationSplit's selection without the final refit."""
     tvs = sg.TrainValidationSplit().setEstimator(est).setEvaluator(ev).setEstimatorParamMaps(maps)
+    ests = [est.copy(m) for m in maps]
     t = time.perf_counter()
-    preds, objective = tvs._fit_classifiers([est.copy(m) for m in maps], isinstance(est, sg.OneVsRest), X, y, mask)
+    if isinstance(est, sg.GaussianProcessRegression):
+        preds, objective = tvs._fit_regression(ests, X, y, mask)
+    else:
+        preds, _, objective = tvs._fit_classifiers(ests, isinstance(est, sg.OneVsRest), X, y, mask)
     metrics = [ev.evaluate(y[~mask], p) for p in preds]
     wall = time.perf_counter() - t
     g = objective["groups"]
@@ -112,10 +128,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--out", help="directory for the report")
+    ap.add_argument("--workloads", nargs="+", choices=("mnist68", "ovr10", "reg8"), default=["mnist68", "ovr10", "reg8"])
     a = ap.parse_args()
     report = dict(card=card())
     print("card:", report["card"])
-    report["results"] = [run("mnist68", mnist68(), a.reps), run("ovr10", ovr10(), a.reps)]
+    workloads = dict(mnist68=mnist68, ovr10=ovr10, reg8=reg8)
+    report["results"] = [run(name, workloads[name](), a.reps) for name in a.workloads]
     if a.out:
         os.makedirs(a.out, exist_ok=True)
         with open(os.path.join(a.out, "time_tvs.json"), "w") as fh:
