@@ -519,7 +519,7 @@ cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const
   }
   const bool reg = plan.variant < ObjectiveVariant::kSmem;
   void (*kernel)(NllParams) = reg ? kRegShapes[static_cast<int>(plan.variant)].kernel : bcm_nll_kernel;
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(plan.smem));
+  cudaError_t e = allow_dynamic_smem(reinterpret_cast<const void*>(kernel));
   if (e != cudaSuccess) return e;
   kernel<<<dim3(static_cast<unsigned>(E), static_cast<unsigned>(n_slots)), reg ? REG_THREADS : EX_THREADS, plan.smem, s>>>(p);
   e = cudaGetLastError();
@@ -553,7 +553,7 @@ cudaError_t launch_bcm_nll_general(const ObjectivePlan& plan, cublasHandle_t bla
   if (st == CUBLAS_STATUS_SUCCESS)
     st = cublasDgetriBatched(blas, n_max, Aptr, n_max, piv, Cptr, n_max, info + 0, static_cast<int>(E));
   if (st != CUBLAS_STATUS_SUCCESS) { *blas_status = static_cast<int>(st); return cudaSuccess; }
-  e = cudaFuncSetAttribute(gen_objective_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(plan.smem));
+  e = allow_dynamic_smem(reinterpret_cast<const void*>(gen_objective_kernel));
   if (e != cudaSuccess) return e;
   gen_objective_kernel<<<static_cast<unsigned>(E), EX_THREADS, plan.smem, s>>>(p);
   e = cudaGetLastError();

@@ -438,9 +438,9 @@ cudaError_t launch_gram_f64(const GramParams& p, bool strict_elements, cudaStrea
     const int nt = p.n_tiles_1d * (p.n_tiles_1d + 1) / 2;
     dim3 grid(nt, p.n_slices);
     constexpr size_t smem = gram_smem_bytes<double>();
-    {   // the attribute is per DEVICE (one JVM may hold contexts on several GPUs): set it on every launch, it is cheap
-      cudaError_t e = cudaFuncSetAttribute(kmn_gram_f64_kernel<double, 128>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    {   // the cap is per DEVICE and shared by every context on it (one JVM holds one per task thread, on one or several
+        // GPUs): set it on every launch, to the one value allow_dynamic_smem gives this kernel; it is cheap
+      cudaError_t e = allow_dynamic_smem(reinterpret_cast<const void*>(kmn_gram_f64_kernel<double, 128>));
       if (e != cudaSuccess) return e;
     }
     kmn_gram_f64_kernel<double, 128><<<grid, NT, smem, s>>>(p);
@@ -449,8 +449,7 @@ cudaError_t launch_gram_f64(const GramParams& p, bool strict_elements, cudaStrea
     dim3 grid(nt, p.n_slices);
     constexpr size_t smem = gram_smem_bytes<float>();
     {
-      cudaError_t e = cudaFuncSetAttribute(kmn_gram_f64_kernel<float, 64>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      cudaError_t e = allow_dynamic_smem(reinterpret_cast<const void*>(kmn_gram_f64_kernel<float, 64>));
       if (e != cudaSuccess) return e;
     }
     kmn_gram_f64_kernel<float, 64><<<grid, NT, smem, s>>>(p);

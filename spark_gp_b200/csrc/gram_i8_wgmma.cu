@@ -431,7 +431,7 @@ cudaError_t i8_plane_slices(int m_pad, int num_sms, long long n_units, int d, co
   size_t smem;
   const void* fn = plane_kernel(d, direct, &xbytes, &zbytes, &smem);
   if (smem > kSmemOptInMax) return cudaErrorInvalidConfiguration;
-  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  cudaError_t e = allow_dynamic_smem(fn);
   if (e != cudaSuccess) return e;
   int per_sm = 0;
   e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, NTHREADS, smem);
@@ -460,8 +460,9 @@ cudaError_t launch_i8_planes(const uint8_t* Xt, const float* ys, const uint8_t* 
   size_t smem;
   const void* fn = plane_kernel(d, direct, &p.xbytes, &p.zbytes, &smem);
   if (smem > kSmemOptInMax) return cudaErrorInvalidConfiguration;
-  // per-device attribute: set on every launch (contexts on several GPUs may live in one process)
-  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  // the cap is per device and shared by every context on it (one per task thread, on one or several GPUs): set on
+  // every launch, to the one value allow_dynamic_smem gives every launch of this kernel, never to this launch's smem
+  cudaError_t e = allow_dynamic_smem(fn);
   if (e != cudaSuccess) return e;
   dim3 grid(p.nt, n_slices);
   void* args[] = {&p};
@@ -479,7 +480,7 @@ cudaError_t launch_gram_i8(const uint8_t* planes, long long n_units, int m_pad, 
   p.accumulate = accumulate ? 1 : 0;
   const size_t smem = 1024 + GSTAGES * 2 * TILE_PLANES + 16 * GSTAGES;
   const void* fn = reinterpret_cast<const void*>(gram_i8_kernel);
-  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  cudaError_t e = allow_dynamic_smem(fn);
   if (e != cudaSuccess) return e;
   dim3 grid(p.nt * (p.nt + 1) / 2, n_slices);
   void* args[] = {&p};

@@ -120,7 +120,7 @@ cudaError_t launch_kmn_sweep(const uint8_t* Xt, const uint8_t* Zt, long long n, 
   const size_t smem = 1024 + p.nchunks * ZPANEL_BYTES + XSTAGES * p.nchunks * XIMG_BYTES + 8 * (XSTAGES + 1);
   const void* fn = (3 * dp + 16) / 16 == 4 ? reinterpret_cast<const void*>(kmn_sweep_kernel<4>)
                                            : reinterpret_cast<const void*>(kmn_sweep_kernel<7>);
-  cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  cudaError_t e = allow_dynamic_smem(fn);
   if (e != cudaSuccess) return e;
   dim3 grid(p.nt, slices);
   void* args[] = {&p};

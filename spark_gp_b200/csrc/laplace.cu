@@ -226,7 +226,7 @@ cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const
     n_slots = classes->n_slots;
     if (classes->sets) E = classes->E_max;
   }
-  cudaError_t e = cudaFuncSetAttribute(laplace_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(plan.smem));
+  cudaError_t e = allow_dynamic_smem(reinterpret_cast<const void*>(laplace_kernel));
   if (e != cudaSuccess) return e;
   laplace_kernel<<<dim3(static_cast<unsigned>(E), static_cast<unsigned>(n_slots)), LT, plan.smem, s>>>(p);
   e = cudaGetLastError();

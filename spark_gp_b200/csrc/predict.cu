@@ -394,8 +394,8 @@ cudaError_t launch_predict(const PredictArgs& a, cudaStream_t s) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || !with_var) return e;
   const int n_rt = static_cast<int>(rows / kVarRows);
-  // the attribute is per device (one process may hold contexts on several GPUs): set it on every launch, it is cheap
-  e = cudaFuncSetAttribute(predict_var_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kVarSmem));
+  // the cap is per device and shared by every context on it: set on every launch (allow_dynamic_smem), it is cheap
+  e = allow_dynamic_smem(reinterpret_cast<const void*>(predict_var_kernel));
   if (e != cudaSuccess) return e;
   predict_var_kernel<<<static_cast<unsigned>(n_rt) * n_ct, kVarThreads, kVarSmem, s>>>(K, a.B, a.n, a.m_pad, n_rt, n_ct,
                                                                                      vpart);

@@ -213,6 +213,22 @@ struct Ctx {
   DevScratch dbgT, dbgW;       // sgp_debug_i8_tile: fp32 T and uint32 words
 };
 
+// Opts kernel fn in to dynamic shared memory above 48 KiB.  Launchers call it before every launch of such a kernel and
+// pass their own plan's size to the launch itself.  The cap is an attribute of the function on the current device, shared
+// by every context of the process on that device (one per Spark task thread), so it is one value per kernel -- the
+// largest a CTA can opt in to -- never the size of the call at hand: a context that set its small plan's size between
+// another context's set and launch would get that launch refused.  Concurrent sets all write the same value.  Static and
+// dynamic shared memory share the opt-in maximum, so the cap is that maximum less the kernel's static shared memory
+// (predict_var_kernel declares some; a larger cap is refused).  This is the only place in csrc/ that sets
+// cudaFuncAttributeMaxDynamicSharedMemorySize (tests/test_host_concurrent_contexts.py checks it).
+inline cudaError_t allow_dynamic_smem(const void* fn) {
+  cudaFuncAttributes a;
+  const cudaError_t e = cudaFuncGetAttributes(&a, fn);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              static_cast<int>(kSmemOptInMax - a.sharedSizeBytes));
+}
+
 // error helpers ---------------------------------------------------------------------------------
 int fail(Ctx* c, int code, const std::string& msg);
 #define SGP_CUDA(c, expr)                                                                         \

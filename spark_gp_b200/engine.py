@@ -143,12 +143,15 @@ class ProjectedProcessEngine:
 
     @classmethod
     def acquire(cls, device: int = 0):
-        pool = cls._idle.get(device)
-        if pool:
-            eng = pool.pop()
-            eng.set_precision(N.SGP_PREC_AUTO)
-            return eng
-        return cls(device)
+        """An idle context of the pool, or a new one.  Estimators fit from several threads at once (one Spark task each):
+        the pool is popped without a check-then-pop window, so two threads never get the same context and a thread
+        that finds the pool emptied under it creates its own."""
+        try:
+            eng = cls._idle.get(device, []).pop()
+        except IndexError:
+            return cls(device)
+        eng.set_precision(N.SGP_PREC_AUTO)
+        return eng
 
     def release(self):
         """Hand the context back to the pool (or destroy it when the pool is full or it carries a communicator)."""
