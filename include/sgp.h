@@ -500,6 +500,37 @@ int sgp_cross_kernel(sgp_ctx* ctx, const double* X, int64_t n, double* K_out);
 int sgp_kmn_sweep(sgp_ctx* ctx, const void* X, int32_t x_is_f32, int64_t n, float* K_out);
 int sgp_kmn_sweep_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n, float* dK_out);
 
+/* ---- Kernel evaluation: crossKernel, trainingKernel, trainingKernelAndDerivative (kernel/Kernel.scala:12-98) ---------
+ * Evaluates `kernel` on the vectors passed in, in fp64; no context state is read or changed (an open begin..finish
+ * window's statistics and status and an installed magic pair stay as they are).
+ *   SGP_KEVAL_CROSS:    K[i][j] = k(A_i, B_j), n x m row-major.  Eye terms contribute nothing (Kernel.scala:157).  Equal,
+ *                       bit for bit, to sgp_cross_kernel on the same kernel with B as its active set.
+ *   SGP_KEVAL_TRAINING: B must be NULL and m == n: K = k(A, A) plus every Eye term's scale on the diagonal
+ *                       (Kernel.scala:151), exactly symmetric.
+ * dK_out (n_hypers x n x m, or NULL to skip): dK_out[h] = dK / d theta_h, h in the order of `hypers`, which must be the
+ * kernel's descriptors as sgp_bcm_nll takes them: one ARD_BETA per feature of every ARD term and one RBF_SIGMA per RBF
+ * term, each with the term's own value, and any SCALE descriptors.  ARD beta_k of term t: -2 beta_k (a_k - b_k)^2 C_t e_t
+ * (ARDRBFKernel.scala:61-79); RBF sigma: |a - b|^2 / sigma^3 C_t e_t (RBFKernel.scala:56-64); SCALE: sum_t coef_t times
+ * term t's element, Eye terms only on the TRAINING diagonal (ScalarTimesKernel.scala:93-97).  In TRAINING mode every dK
+ * is exactly symmetric too.
+ * A is fp64, or fp32 when a_is_f32 (converted to fp64 first: the same bits as its fp64 upcast).  An element's arithmetic
+ * does not depend on how the rows are split over calls or windows.
+ * SGP_E_BADARG, before any allocation or launch: n, m or d < 1; NULL A or K_out; a mode outside {CROSS, TRAINING}; B
+ * missing in CROSS or given in TRAINING; descriptors that do not match the kernel; a kernel with no terms (or more than
+ * 4 non-Eye terms); an output beyond 64-bit sizes.
+ * Host entry: A, B and the outputs are host memory.  Rows of A go through the device in windows whose K and dK stay
+ * within 256 MiB (at least one row); B (TRAINING: A) is copied to the device once.  SGP_E_NOMEM, before any
+ * allocation, when the windows and that copy do not fit in free device memory.
+ * _device: A, B (fp64) and both outputs are device (or managed) memory on the context's device, SGP_E_BADARG otherwise;
+ * asynchronous on the context's stream (sgp_sync before reading the outputs). */
+enum { SGP_KEVAL_CROSS = 0, SGP_KEVAL_TRAINING = 1 };
+int sgp_kernel_eval(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper* hypers, int32_t n_hypers, const void* A,
+                    int32_t a_is_f32, int64_t n, const double* B, int32_t m, int32_t d, int32_t mode,
+                    double* K_out /* n x m */, double* dK_out /* n_hypers x n x m, or NULL */);
+int sgp_kernel_eval_device(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sgp_hyper* hypers, int32_t n_hypers,
+                           const void* dA, int32_t a_is_f32, int64_t n, const double* dB, int32_t m, int32_t d,
+                           int32_t mode, double* dK_out /* n x m */, double* ddK_out /* n_hypers x n x m, or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

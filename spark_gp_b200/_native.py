@@ -29,7 +29,7 @@ EXPORTS = ["sgp_ctx_create", "sgp_ctx_destroy", "sgp_last_error", "sgp_set_preci
            "sgp_experts_upload_folds_device", "sgp_experts_get_f_rows_device", "sgp_kmeans_device",
            "sgp_greedy_active_set_device", "sgp_laplace_nll_fold_slots_any_size", "sgp_experts_get_f_fold_slot",
            "sgp_experts_get_f_fold_rows_device", "sgp_gauss_hermite_rule", "sgp_predict_probability",
-           "sgp_predict_probability_device", "sgp_bcm_nll_slots"]
+           "sgp_predict_probability_device", "sgp_bcm_nll_slots", "sgp_kernel_eval", "sgp_kernel_eval_device"]
 
 
 class KernelTerm(C.Structure):
@@ -44,6 +44,7 @@ class Hyper(C.Structure):
 
 SGP_HYPER_SCALE, SGP_HYPER_ARD_BETA, SGP_HYPER_RBF_SIGMA = 0, 1, 2
 SGP_MODES_BINARY, SGP_MODES_CLASS, SGP_MODES_SLOT = 0, 1, 2
+SGP_KEVAL_CROSS, SGP_KEVAL_TRAINING = 0, 1
 
 
 class KernelDesc(C.Structure):
@@ -118,6 +119,8 @@ def load() -> C.CDLL:
     lib.sgp_experts_get_f_fold_rows_device.argtypes = [vp, i32, i32, vp]
     lib.sgp_kmeans_device.argtypes = lib.sgp_kmeans.argtypes
     lib.sgp_greedy_active_set_device.argtypes = lib.sgp_greedy_active_set.argtypes
+    lib.sgp_kernel_eval.argtypes = [vp, C.POINTER(KernelDesc), vp, i32, vp, i32, i64, vp, i32, i32, i32, vp, vp]
+    lib.sgp_kernel_eval_device.argtypes = lib.sgp_kernel_eval.argtypes
     lib.sgp_event_elapsed_ms.argtypes = [vp, C.c_int, C.c_int, dp]
     for name in EXPORTS:
         if name not in ("sgp_last_error", "sgp_launch_count"):

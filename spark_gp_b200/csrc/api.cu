@@ -2024,4 +2024,236 @@ int sgp_cross_kernel(sgp_ctx* h, const double* X, int64_t n, double* K_out) {
   return SGP_OK;
 }
 
+namespace {
+// One sgp_kernel_eval* call after its checks: the launch arguments (pointers into the descriptor tables still unset) and
+// the tables themselves, [beta (n_terms x d) | scale coefficients (n_scale x (kMaxTerms + 1))] doubles then
+// [ARD indices (n_terms x d) | scale indices (n_scale)] ints.
+struct KernelEvalSetup {
+  KernelEvalArgs a{};
+  std::vector<char> tables;
+  size_t n_dbl = 0;
+  int nh = 0;            // matrices of dK written (0 without dK_out)
+};
+
+// Every refusal of both entries, before any allocation or launch.  The descriptors must be those of the kernel: one
+// ARD_BETA per feature of every ARD term and one RBF_SIGMA per RBF term, each carrying the term's own value, plus any
+// number of SCALE descriptors (trainable scalars), in any order.
+int kernel_eval_setup(Ctx* c, const char* entry, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh,
+                      const void* A, int64_t n, const double* B, int32_t m, int32_t d, int32_t mode, const double* K_out,
+                      const double* dK_out, KernelEvalSetup& o) {
+  const std::string fn(entry);
+  if (!k || k->n_terms <= 0 || !k->terms) return fail(c, SGP_E_BADARG, fn + ": a kernel with no terms");
+  if (n < 1 || m < 1 || d < 1) return fail(c, SGP_E_BADARG, fn + ": n, m and d must be >= 1");
+  if (!A || !K_out) return fail(c, SGP_E_BADARG, fn + ": null argument");
+  if (mode != SGP_KEVAL_CROSS && mode != SGP_KEVAL_TRAINING) return fail(c, SGP_E_BADARG, fn + ": unknown mode");
+  if (mode == SGP_KEVAL_CROSS && !B) return fail(c, SGP_E_BADARG, fn + ": CROSS needs the training vectors B");
+  if (mode == SGP_KEVAL_TRAINING && (B || m != n))
+    return fail(c, SGP_E_BADARG, fn + ": TRAINING takes no B and m == n");
+  if (nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, fn + ": null hyper-parameter descriptors");
+  const int n_mat = 1 + (dK_out ? nh : 0);
+  if (static_cast<unsigned __int128>(n_mat) * static_cast<unsigned __int128>(n) * static_cast<unsigned __int128>(m) * 8 >
+      static_cast<unsigned __int128>(INT64_MAX))
+    return fail(c, SGP_E_BADARG, fn + ": the output exceeds 64-bit sizes");
+  KernelFlat kf;
+  std::vector<double> beta;
+  std::vector<int> flat_of;
+  int rc = flatten_kernel(c, k, d, d, kf, beta, &flat_of);
+  if (rc != SGP_OK) return rc;
+  const int T = kf.n_terms;
+  std::vector<int> ard_h(static_cast<size_t>(T) * d, -1), scale_h;
+  std::vector<double> scale_coef;
+  KernelEvalArgs& a = o.a;
+  for (int t = 0; t < kMaxTerms; ++t) { a.rbf_h[t] = -1; a.sigma3[t] = 1.0; }
+  const std::string mismatch = fn + ": the hyper-parameter descriptors do not match the kernel";
+  for (int i = 0; i < nh; ++i) {
+    const sgp_hyper& hp = hypers[i];
+    if (hp.kind == SGP_HYPER_SCALE) {
+      if (!hp.coef) return fail(c, SGP_E_BADARG, fn + ": SCALE hyper-parameter without coef");
+      scale_h.push_back(i);
+      scale_coef.resize(scale_coef.size() + kMaxTerms + 1, 0.0);
+      double* cf = scale_coef.data() + scale_coef.size() - (kMaxTerms + 1);
+      for (int t = 0; t < k->n_terms; ++t) cf[flat_of[t] >= 0 ? flat_of[t] : kMaxTerms] += hp.coef[t];
+      continue;
+    }
+    if (hp.term < 0 || hp.term >= k->n_terms) return fail(c, SGP_E_BADARG, mismatch);
+    const sgp_kernel_term& term = k->terms[hp.term];
+    const int t = flat_of[hp.term];
+    if (hp.kind == SGP_HYPER_ARD_BETA && term.type == SGP_TERM_ARD) {
+      if (hp.dim < 0 || hp.dim >= d || ard_h[static_cast<size_t>(t) * d + hp.dim] >= 0 || hp.value != term.beta[hp.dim])
+        return fail(c, SGP_E_BADARG, mismatch);
+      ard_h[static_cast<size_t>(t) * d + hp.dim] = i;
+    } else if (hp.kind == SGP_HYPER_RBF_SIGMA && term.type == SGP_TERM_RBF) {
+      if (a.rbf_h[t] >= 0 || hp.value != term.sigma) return fail(c, SGP_E_BADARG, mismatch);
+      a.rbf_h[t] = i;
+      a.sigma3[t] = term.sigma * term.sigma * term.sigma;
+    } else {
+      return fail(c, SGP_E_BADARG, mismatch);
+    }
+  }
+  for (int t = 0; t < k->n_terms; ++t) {
+    const int ft = flat_of[t];
+    if (ft < 0) continue;
+    bool covered = true;
+    if (k->terms[t].type == SGP_TERM_RBF) covered = a.rbf_h[ft] >= 0;
+    for (int j = 0; covered && k->terms[t].type == SGP_TERM_ARD && j < d; ++j)
+      covered = ard_h[static_cast<size_t>(ft) * d + j] >= 0;
+    if (!covered) return fail(c, SGP_E_BADARG, mismatch);
+  }
+  const int ns = static_cast<int>(scale_h.size());
+  o.n_dbl = static_cast<size_t>(T) * d + scale_coef.size();
+  o.tables.assign(o.n_dbl * 8 + (ard_h.size() + scale_h.size()) * 4 + 8, 0);
+  std::memcpy(o.tables.data(), beta.data(), static_cast<size_t>(T) * d * 8);
+  std::memcpy(o.tables.data() + static_cast<size_t>(T) * d * 8, scale_coef.data(), scale_coef.size() * 8);
+  std::memcpy(o.tables.data() + o.n_dbl * 8, ard_h.data(), ard_h.size() * 4);
+  std::memcpy(o.tables.data() + o.n_dbl * 8 + ard_h.size() * 4, scale_h.data(), scale_h.size() * 4);
+  a.n = n; a.m = m; a.d = d;
+  a.training = mode == SGP_KEVAL_TRAINING;
+  a.kf = kf;
+  a.n_scale = dK_out ? ns : 0;
+  o.nh = dK_out ? nh : 0;
+  return SGP_OK;
+}
+
+// Points the launch arguments at the tables uploaded to dev.
+void kernel_eval_bind(KernelEvalSetup& o, const char* dev) {
+  const double* dd = reinterpret_cast<const double*>(dev);
+  const int* di = reinterpret_cast<const int*>(dev + o.n_dbl * 8);
+  const size_t td = static_cast<size_t>(o.a.kf.n_terms) * o.a.d;
+  o.a.beta = dd;
+  o.a.scale_coef = dd + td;
+  o.a.ard_h = di;
+  o.a.scale_h = di + td;
+}
+
+// Allocations of one call that do not fit in the device's free memory (counting what regrowing a buffer frees):
+// SGP_E_NOMEM before any of them is made.
+int kernel_eval_fits(Ctx* c, const char* entry, std::initializer_list<std::pair<const DevScratch*, size_t>> bufs) {
+  size_t free_b = 0, total_b = 0;
+  SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+  size_t need = 0;
+  for (const auto& [buf, bytes] : bufs)
+    if (bytes > buf->cap) need += bytes - buf->cap;
+  if (need > free_b)
+    return fail(c, SGP_E_NOMEM, std::string(entry) + ": " + std::to_string(need >> 20) + " MiB of device memory needed, " +
+                                    std::to_string(free_b >> 20) + " MiB free");
+  return SGP_OK;
+}
+
+int upload_tables(Ctx* c, const KernelEvalSetup& o) {
+  SGP_CUDA(c, cudaMemcpyAsync(c->keval_ws.p, o.tables.data(), o.tables.size(), cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));   // o.tables is the caller's local
+  return SGP_OK;
+}
+
+size_t align256(size_t b) { return (b + 255) / 256 * 256; }
+}  // namespace
+
+int sgp_kernel_eval(sgp_ctx* h, const sgp_kernel_desc* kernel, const sgp_hyper* hypers, int32_t n_hypers, const void* A,
+                    int32_t a_is_f32, int64_t n, const double* B, int32_t m, int32_t d, int32_t mode, double* K_out,
+                    double* dK_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  KernelEvalSetup o;
+  int rc = kernel_eval_setup(c, "sgp_kernel_eval", kernel, hypers, n_hypers, A, n, B, m, d, mode, K_out, dK_out, o);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  const bool training = mode == SGP_KEVAL_TRAINING;
+  const size_t esz = a_is_f32 ? 4 : 8;
+  const size_t row = static_cast<size_t>(d) * esz;
+  // windows of rows whose K and dK together stay within kPredictKBytes (at least one row)
+  const size_t row_out = static_cast<size_t>(1 + o.nh) * m * 8;
+  const long long win = std::min<long long>(n, std::max<long long>(1, static_cast<long long>(kPredictKBytes / row_out)));
+  const size_t win_out = static_cast<size_t>(win) * row_out;
+  // the training vectors go to the device once, after the tables: B as fp64 (CROSS), or A as given (TRAINING, where the
+  // windows then read their rows from that copy instead of staging them)
+  const size_t tab = align256(o.tables.size());
+  const size_t b_bytes = training ? static_cast<size_t>(n) * row : static_cast<size_t>(m) * d * 8;
+  const size_t stage = training ? 0 : static_cast<size_t>(win) * row;
+  rc = kernel_eval_fits(c, "sgp_kernel_eval", {{&c->keval_ws, tab + b_bytes}, {&c->keval_out_ws, 2 * win_out},
+                                               {&c->stage_x[0], stage}, {&c->stage_x[1], stage}});
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->keval_ws, tab + b_bytes);
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->keval_out_ws, 2 * win_out);
+  if (rc != SGP_OK) return rc;
+  char* dev = c->keval_ws.as<char>();
+  kernel_eval_bind(o, dev);
+  SGP_CUDA(c, cudaMemcpyAsync(dev + tab, training ? A : B, b_bytes, cudaMemcpyHostToDevice, c->stream));
+  if ((rc = upload_tables(c, o)) != SGP_OK) return rc;
+  o.a.B = dev + tab;
+  o.a.b_is_f32 = training ? a_is_f32 : 0;
+  o.a.a_is_f32 = a_is_f32;
+  // each window's K and dK go to one of two output buffers [K | dK_0 | dK_1 ..] of win rows each, and are copied out
+  // (copy stream) once the next window is queued, as sgp_predict does
+  double* out = c->keval_out_ws.as<double>();
+  const size_t mat = static_cast<size_t>(win) * m;
+  const size_t full = static_cast<size_t>(n) * m;
+  auto copy_out = [&](int b, long long p0, long long cn) -> int {
+    const double* src = out + static_cast<size_t>(1 + o.nh) * mat * b;
+    const size_t bytes = static_cast<size_t>(cn) * m * 8, off = static_cast<size_t>(p0) * m;
+    SGP_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->out_ready[b], 0));
+    SGP_CUDA(c, cudaMemcpyAsync(K_out + off, src, bytes, cudaMemcpyDeviceToHost, c->copy_stream));
+    for (int hh = 0; hh < o.nh; ++hh)
+      SGP_CUDA(c, cudaMemcpyAsync(dK_out + hh * full + off, src + (1 + hh) * mat, bytes, cudaMemcpyDeviceToHost,
+                                  c->copy_stream));
+    SGP_CUDA(c, cudaEventRecord(c->out_free[b], c->copy_stream));
+    return SGP_OK;
+  };
+  long long windows = 0, pending_p0 = 0, pending_n = 0;
+  rc = feed_rows(c, training, training ? o.a.B : A, nullptr, n, row, win,
+                 [&](const void* dA, const double*, long long p0, long long cn) -> int {
+                   const int b = static_cast<int>(windows & 1);
+                   double* dst = out + static_cast<size_t>(1 + o.nh) * mat * b;
+                   KernelEvalArgs a = o.a;
+                   a.A = dA; a.n = cn; a.row0 = p0;
+                   a.K = dst;
+                   a.dK = o.nh > 0 ? dst + mat : nullptr;
+                   a.dk_stride = mat;
+                   SGP_CUDA(c, cudaStreamWaitEvent(c->stream, c->out_free[b], 0));
+                   SGP_CUDA(c, launch_kernel_eval(a, c->stream));
+                   c->launches += 1;
+                   SGP_CUDA(c, cudaEventRecord(c->out_ready[b], c->stream));
+                   int r = SGP_OK;
+                   if (windows > 0 && (r = copy_out(b ^ 1, pending_p0, pending_n)) != SGP_OK) return r;
+                   ++windows;
+                   pending_p0 = p0;
+                   pending_n = cn;
+                   return SGP_OK;
+                 });
+  if (rc == SGP_OK) rc = copy_out(static_cast<int>((windows - 1) & 1), pending_p0, pending_n);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaStreamSynchronize(c->copy_stream));
+  return SGP_OK;
+}
+
+int sgp_kernel_eval_device(sgp_ctx* h, const sgp_kernel_desc* kernel, const sgp_hyper* hypers, int32_t n_hypers,
+                           const void* dA, int32_t a_is_f32, int64_t n, const double* dB, int32_t m, int32_t d, int32_t mode,
+                           double* dK_out, double* ddK_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  const char* entry = "sgp_kernel_eval_device";
+  KernelEvalSetup o;
+  int rc = kernel_eval_setup(c, entry, kernel, hypers, n_hypers, dA, n, dB, m, d, mode, dK_out, ddK_out, o);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  rc = device_ptr_ok(c, dA, entry, "A");
+  if (rc == SGP_OK && dB) rc = device_ptr_ok(c, dB, entry, "B");
+  if (rc == SGP_OK) rc = device_ptr_ok(c, dK_out, entry, "K_out");
+  if (rc == SGP_OK && ddK_out) rc = device_ptr_ok(c, ddK_out, entry, "dK_out");
+  if (rc == SGP_OK) rc = kernel_eval_fits(c, entry, {{&c->keval_ws, o.tables.size()}});
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->keval_ws, o.tables.size());
+  if (rc == SGP_OK) rc = upload_tables(c, o);
+  if (rc != SGP_OK) return rc;
+  kernel_eval_bind(o, c->keval_ws.as<char>());
+  KernelEvalArgs& a = o.a;
+  a.A = dA; a.a_is_f32 = a_is_f32;
+  a.B = dB ? static_cast<const void*>(dB) : dA;
+  a.b_is_f32 = dB ? 0 : a_is_f32;
+  a.row0 = 0;
+  a.K = dK_out;
+  a.dK = o.nh > 0 ? ddK_out : nullptr;
+  a.dk_stride = static_cast<size_t>(n) * m;
+  SGP_CUDA(c, launch_kernel_eval(a, c->stream));
+  c->launches += 1;
+  return SGP_OK;
+}
+
 }  // extern "C"

@@ -197,6 +197,8 @@ struct Ctx {
   DevScratch dMagicPacked;       // m_pad x m_pad  triu(M + M^T, 1) + diag(M), built by the first variance call
   bool magic_packed = false;     // dMagicPacked holds the installed magicMatrix
   DevScratch predict_out_ws;     // sgp_predict*: [2][mean | var | p] per window (double buffered)
+  DevScratch keval_ws;           // sgp_kernel_eval*: descriptor tables, then (host entry) the staged training vectors
+  DevScratch keval_out_ws;       // sgp_kernel_eval: [2][K | dK] per window (double buffered)
   DevScratch dGhRule;            // [nodes | weights] of the gh_nodes-node Gauss-Hermite rule (sgp_predict_probability*)
   int gh_nodes = 0;              // 0: none uploaded yet
   // host->device staging (double buffered)
@@ -334,6 +336,31 @@ cudaError_t launch_gram_i8(const uint8_t* planes, long long n_units, int m_pad, 
 // K_nm sweep (kmn_sweep.cu): fp32 cross kernel of a block of points, row-major n x m
 cudaError_t launch_kmn_sweep(const uint8_t* Xt, const uint8_t* Zt, long long n, int d, int m, int m_pad, int num_sms, double C,
                              float* K, cudaStream_t s);
+
+// Kernel evaluation (kernel_eval.cu, sgp_kernel_eval*): K[i][j] = k(a_i, b_j) for n rows of A against m rows of B, and
+// with dK every derivative dK / d theta_h, h in the order of the hyper-parameter descriptors.
+struct KernelEvalArgs {
+  const void* A;            // n x d row-major, fp32 or fp64
+  int a_is_f32;
+  const void* B;            // m x d row-major (TRAINING: the training vectors, of which A is rows row0 ..)
+  int b_is_f32;
+  long long n;
+  int m, d;
+  int training;             // 1: the Eye sum (and the Eye coefficients of trainable scalars) go on the diagonal
+  long long row0;           // A's row i is row row0 + i of the training vectors (the diagonal is row0 + i == j)
+  KernelFlat kf;
+  const double* beta;       // [n_terms][d] flattened feature scales (ARD betas; RBF: 1/(sqrt2 sigma))
+  double* K;                // n x m
+  double* dK;               // [n_hypers][dk_stride] (n x m each), or nullptr: K only
+  size_t dk_stride;
+  const int* ard_h;         // [n_terms][d] hyper-parameter index of (ARD term t, feature k); -1 for an RBF term
+  int rbf_h[kMaxTerms];     // hyper-parameter index of RBF term t's sigma, -1 for an ARD term
+  double sigma3[kMaxTerms]; // RBF term t: sigma^3
+  int n_scale;              // trainable scalars
+  const int* scale_h;       // [n_scale] hyper-parameter index
+  const double* scale_coef; // [n_scale][kMaxTerms + 1] d(C_t)/d(theta) per flattened term, then d(eye_sum)/d(theta)
+};
+cudaError_t launch_kernel_eval(const KernelEvalArgs& a, cudaStream_t s);
 
 // Per-expert objectives (bcm_nll.cu, laplace.cu) ----------------------------------------------------------------------
 // Device-side view of the flattened kernel and the hyper-parameter descriptors of one evaluation.

@@ -304,9 +304,10 @@ class ProjectedProcessEngine:
         self._experts_d = X.shape[1]
         return int(np.floor(len(X) / dataset_size_for_expert + 0.5))
 
-    def _descriptors(self, kernel: Kernel):
-        """(kernel desc, hyper-parameter descriptors, their count, the buffers both point into)."""
-        desc, keep = _make_desc(kernel, self._experts_d)
+    def _descriptors(self, kernel: Kernel, d: int = None):
+        """(kernel desc, hyper-parameter descriptors, their count, the buffers both point into) for d features (default:
+        the uploaded experts')."""
+        desc, keep = _make_desc(kernel, self._experts_d if d is None else d)
         hd = kernel.hyper_descriptors()
         arr = (N.Hyper * max(len(hd), 1))()
         coefs = []
@@ -614,6 +615,44 @@ class ProjectedProcessEngine:
         K = np.empty((len(X), self.m))
         self._check(self._lib.sgp_cross_kernel(self._h, N.ptr(X), len(X), N.ptr(K)))
         return K
+
+    def kernel_eval(self, kernel: Kernel, A, B=None, derivatives: bool = False):
+        """The kernel's matrix on the given vectors (`sgp_kernel_eval`; `sgp_kernel_eval_device` for CUDA tensors on this
+        context's device, read in place): crossKernel K = k(A, B) (n x m), or with B None the training kernel k(A, A)
+        with the Eye terms on the diagonal.  Returns (K, dK): dK [n_hypers x n x m] in kernel.getHyperparameters() order
+        with derivatives, else None.  A may be float32; B is read as float64.  Host arrays give numpy arrays, CUDA
+        tensors CUDA float64 tensors."""
+        on_device = is_cuda_tensor(A)
+        if on_device:
+            import torch
+            A = device_tensor(A, self._device, "kernel_eval")
+            B = None if B is None else device_tensor(B, self._device, "kernel_eval", torch.float64)
+            f32 = int(A.dtype == torch.float32)
+        else:
+            A = _rows(A)
+            B = None if B is None else np.ascontiguousarray(B, dtype=np.float64)
+            f32 = int(A.dtype == np.float32)
+        if A.ndim != 2 or (B is not None and (B.ndim != 2 or B.shape[1] != A.shape[1])):
+            raise ValueError("kernel_eval: A must be n x d and B m x d")
+        n, d = A.shape
+        m = n if B is None else B.shape[0]
+        desc, arr, nh, keep = self._descriptors(kernel, d)
+        mode = N.SGP_KEVAL_TRAINING if B is None else N.SGP_KEVAL_CROSS
+        shape_dk = (nh if derivatives else 0, n, m)
+        if on_device:
+            K = torch.empty((n, m), dtype=torch.float64, device=A.device)
+            dK = torch.empty(shape_dk, dtype=torch.float64, device=A.device)
+            ptr = lambda t: C.c_void_p(t.data_ptr())
+            fn = self._lib.sgp_kernel_eval_device
+        else:
+            K, dK = np.empty((n, m)), np.empty(shape_dk)
+            ptr, fn = N.ptr, self._lib.sgp_kernel_eval
+        self._check(fn(self._h, C.byref(desc), arr, nh, ptr(A), f32, n, None if B is None else ptr(B), m, d, mode, ptr(K),
+                       ptr(dK) if shape_dk[0] > 0 else None))
+        if on_device:
+            self.sync()
+        del keep
+        return K, (dK if derivatives else None)
 
     def greedy_active_set(self, kernel: Kernel, X, y, n_experts: int, first_index: int, m_target: int):
         """Row indices of the points GreedilyOptimizingActiveSetProvider selects (ActiveSetProvider.scala:58-139), computed

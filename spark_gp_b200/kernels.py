@@ -1,7 +1,10 @@
 """Host-side mirror of the reference's kernel DSL (`commons/kernel/*.scala`): same class names, the same
-hyperparameter layout and bounds, the same sugar -- but no numerics.  A kernel object here is a
-*description*; `flatten()` turns the tree into the term list of `sgp_kernel_desc` (include/sgp.h) and
-all arithmetic happens in the CUDA library.
+hyperparameter layout and bounds, the same sugar, and the same evaluation methods (setTrainingVectors, trainingKernel,
+trainingKernelDiag, trainingKernelAndDerivative, crossKernel, selfKernel).  A kernel object here is a *description*:
+`flatten()` turns the tree into the term list of `sgp_kernel_desc` (include/sgp.h), `hyper_descriptors()` says how the
+matrix depends on each hyper-parameter, and the arithmetic runs in the CUDA library (`sgp_kernel_eval`, or
+`sgp_kernel_eval_device` for CUDA tensors).  Only the diagonal quantities (selfKernel, trainingKernelDiag), sums of the
+term scales, are computed here.
 
 Scala                                   Python
   1 * new ARDRBFKernel(5)                 1 * ARDRBFKernel(5)
@@ -17,7 +20,7 @@ from . import _native as N
 
 
 class Kernel:
-    """commons/kernel/Kernel.scala:12-98 -- the parts that are pure bookkeeping."""
+    """commons/kernel/Kernel.scala:12-98."""
 
     def getHyperparameters(self) -> np.ndarray: raise NotImplementedError
     def setHyperparameters(self, value): raise NotImplementedError
@@ -39,6 +42,87 @@ class Kernel:
 
     def __rmul__(self, c):
         return (c if isinstance(c, Scalar) else Scalar(float(c))) * self
+
+    # ---- evaluation (Kernel.scala:37-98) ----------------------------------------------------------------------------
+    def _children(self) -> list: return []
+
+    def setTrainingVectors(self, vectors, device: int = 0):
+        """Kernel.scala:44-49: n x d vectors (one d-vector is one row), a host array or a CUDA tensor.  The kernel is
+        evaluated on the tensor's device, or on cuda:`device` for a host array.  float32 is kept as it is (the library
+        converts it to float64 exactly); other dtypes become float64.  Composite kernels pass the vectors on, as the
+        reference's do."""
+        from .engine import is_cuda_tensor
+        if is_cuda_tensor(vectors):
+            v, dev = (vectors if vectors.ndim == 2 else vectors.reshape(1, -1)), vectors.device.index
+        else:
+            v = np.asarray(vectors)
+            v, dev = np.atleast_2d(v if v.dtype == np.float32 else v.astype(np.float64)), int(device)
+        self._training = (v, dev)
+        for child in self._children():
+            child.setTrainingVectors(vectors, device)
+        return self
+
+    def getTrainingVectors(self):
+        return self._training_vectors()[0]
+
+    def _training_vectors(self):
+        tv = getattr(self, "_training", None)
+        if tv is None:
+            from .engine import TrainingVectorsNotInitializedException
+            raise TrainingVectorsNotInitializedException("setTrainingVectors method should have been called first")
+        return tv
+
+    def _evaluate(self, test, derivatives: bool):
+        """(K, dK or None) from the library on a pooled context: the training kernel (test None) or crossKernel(test).
+        When one side is a CUDA tensor the other goes to its device, and the results are CUDA float64 tensors."""
+        from .engine import ProjectedProcessEngine, is_cuda_tensor
+        train, device = self._training_vectors()
+        if test is not None:
+            if is_cuda_tensor(test) and not is_cuda_tensor(train):
+                import torch
+                device = test.device.index
+                train = torch.as_tensor(train, device=test.device)
+            elif is_cuda_tensor(train) and not is_cuda_tensor(test):
+                import torch
+                test = torch.as_tensor(np.asarray(test), device=train.device)
+        eng = ProjectedProcessEngine.acquire(device)
+        try:
+            if test is None:
+                return eng.kernel_eval(self, train, None, derivatives)
+            return eng.kernel_eval(self, test, train, derivatives)
+        finally:
+            eng.release()
+
+    def trainingKernel(self):
+        """Kernel.scala:51-55: K[i][j] = k(x_i, x_j) over the training vectors, the Eye terms on the diagonal."""
+        return self._evaluate(None, False)[0]
+
+    def trainingKernelDiag(self):
+        """Kernel.scala:57-61: the diagonal of trainingKernel, selfKernel on every row (computed here, no GPU call)."""
+        from .engine import is_cuda_tensor
+        train, _ = self._training_vectors()
+        if is_cuda_tensor(train):
+            import torch
+            return torch.full((len(train),), self.selfKernel(None), dtype=torch.float64, device=train.device)
+        return np.zeros(len(train)) + self.selfKernel(None)
+
+    def trainingKernelAndDerivative(self):
+        """Kernel.scala:63-68: (K, dK) with dK[i] = dK / d getHyperparameters()[i], an n_hypers x n x n array."""
+        return self._evaluate(None, True)
+
+    def crossKernel(self, test):
+        """Kernel.scala:70-84: len(test) x len(trainingVectors) for n x d test vectors; one row for a single d-vector."""
+        from .engine import is_cuda_tensor
+        if not is_cuda_tensor(test):
+            test = np.asarray(test)
+            test = test if test.dtype == np.float32 else test.astype(np.float64)
+        if test.ndim == 1:
+            return self._evaluate(test.reshape(1, -1), False)[0][0]
+        return self._evaluate(test, False)[0]
+
+    def selfKernel(self, test) -> float:
+        """Kernel.scala:86-90: k(x, x), the same for every x -- the sum of the term scales (every leaf has k(x, x) = 1)."""
+        return float(sum(t["scale"] for t in self.flatten()))
 
 
 class EyeKernel(Kernel):
@@ -113,6 +197,7 @@ class ConstantTimesKernel(Kernel):
     def flatten(self, scale=1.0): return self.kernel.flatten(scale * self.C)
     def hyper_descriptors(self, scale=1.0, term_offset=0):
         return self.kernel.hyper_descriptors(scale * self.C, term_offset)
+    def _children(self): return [self.kernel]
     def __str__(self): return ("%1.1e * %s" % (self.C, self.kernel)) if self.C != 0 else ""
 
 
@@ -201,4 +286,5 @@ class SumOfKernels(Kernel):
         n1 = len(self.kernel1.flatten(scale))
         return (self.kernel1.hyper_descriptors(scale, term_offset)
                 + self.kernel2.hyper_descriptors(scale, term_offset + n1))
+    def _children(self): return [self.kernel1, self.kernel2]
     def __str__(self): return " + ".join(s for s in (str(self.kernel1), str(self.kernel2)) if len(s) > 0)
