@@ -103,6 +103,18 @@ int sgp_version(void);
 /* ---- multi-GPU (one process / context per GPU; replaces PGPH:23 broadcast + PGPH:25-35 treeAggregate) */
 #define SGP_UNIQUE_ID_BYTES 128
 int sgp_comm_unique_id(void* out128);                                   /* rank 0, then ship the bytes to all ranks */
+/* Attaches one communicator of nranks ranks to ctx.  SGP_E_BADARG for a null id, nranks < 1, rank < 0 or rank >= nranks;
+ * SGP_E_STATE when ctx already has a communicator (the first one stays attached); SGP_E_NCCL when ncclCommInitRank
+ * fails, leaving ctx without a communicator.  A refused call leaves ctx usable.
+ * With a communicator of nranks > 1, sgp_stats_finish, sgp_bcm_nll, _folds, _slots and sgp_laplace_nll, _any_size,
+ * _classes, _classes_any_size, _slots_any_size, _fold_slots_any_size each make exactly one ncclAllReduce, and a status
+ * decided on one rank (SGP_E_RANGE, SGP_E_SINGULAR, SGP_E_NOT_PD) is returned on every rank.  The other entries are
+ * rank-local.  The caller's obligation: every rank makes the same sequence of these calls, with the same kernel
+ * structure, n_eval and descriptor layout.  Refusals that depend on the rank's own data return BEFORE the collective and
+ * leave the peers blocked in it: the on-chip Laplace limit (117 points in the largest expert), the global-memory Laplace
+ * kernel's limit (SGP_E_BADARG above its per-expert point bound), the 46340-point limit of
+ * the BCM LU path, SGP_E_NOMEM of the LU workspace / Laplace workspace / mode stores, and a rank without experts
+ * (SGP_E_STATE).  The caller must prevent them, e.g. by giving every rank experts that fit the same kernel family. */
 int sgp_comm_init(sgp_ctx* ctx, const void* id128, int rank, int nranks);
 
 /* ---- the hot path:  PGPH:20-36 ------------------------------------------------------------- */

@@ -486,12 +486,16 @@ int sgp_comm_unique_id(void* out128) {
 int sgp_comm_init(sgp_ctx* h, const void* id128, int rank, int nranks) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c || !id128 || nranks < 1 || rank < 0 || rank >= nranks) return fail(c, SGP_E_BADARG, "bad comm arguments");
+  // a second communicator would orphan the first, and its peers with it: the context keeps the one it has
+  if (c->comm) return fail(c, SGP_E_STATE, "sgp_comm_init: the context already has a communicator");
   if (!nccl().ok) return fail(c, SGP_E_NCCL, "libnccl.so.2 could not be loaded");
   SGP_CUDA(c, cudaSetDevice(c->device));
   ncclUniqueId id;
   std::memcpy(&id, id128, sizeof(id));
-  ncclResult_t r = nccl().CommInitRank(&c->comm, nranks, id, rank);
+  ncclComm_t comm = nullptr;
+  ncclResult_t r = nccl().CommInitRank(&comm, nranks, id, rank);
   if (r != ncclSuccess) return fail(c, SGP_E_NCCL, std::string("ncclCommInitRank: ") + nccl().GetErrorString(r));
+  c->comm = comm;                                   // only a communicator that was made: sgp_ctx_destroy destroys it
   c->rank = rank; c->nranks = nranks;
   return SGP_OK;
 }
@@ -1190,12 +1194,33 @@ int objective_finish(Ctx* c, const ObjectiveSetup& o, int nh, double* val_out, d
   SGP_CUDA(c, launch_flags_to_double(o.total + static_cast<size_t>(S) * W, o.flags, mask, S, c->stream));
   c->launches += 1;
   const size_t len = static_cast<size_t>(S) * (W + 1);
+  std::vector<double> tot(len);
+  std::vector<int> listed;
   if (c->comm && c->nranks > 1) {
+    if (pos) {
+      // The row a slot was set up in follows the rank's own experts (the fold slots' on-chip | global-memory split), so
+      // ranks may disagree on it: move every row and status word to its list position before the sum.
+      std::vector<double> set_up(len);
+      SGP_CUDA(c, cudaMemcpyAsync(set_up.data(), o.total, len * 8, cudaMemcpyDeviceToHost, c->stream));
+      SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+      for (int s = 0; s < S; ++s) {
+        std::copy(set_up.begin() + static_cast<size_t>(s) * W, set_up.begin() + static_cast<size_t>(s + 1) * W,
+                  tot.begin() + static_cast<size_t>(pos[s]) * W);
+        tot[static_cast<size_t>(S) * W + pos[s]] = set_up[static_cast<size_t>(S) * W + s];
+      }
+      SGP_CUDA(c, cudaMemcpyAsync(o.total, tot.data(), len * 8, cudaMemcpyHostToDevice, c->stream));
+      SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+      if (classes) {
+        listed.resize(S);
+        for (int s = 0; s < S; ++s) listed[pos[s]] = classes[s];
+        classes = listed.data();
+      }
+      pos = nullptr;                                // from here on, row s is list position s
+    }
     ncclResult_t r = nccl().AllReduce(o.total, o.total, len, ncclDouble, ncclSum, c->comm, c->stream);
     if (r != ncclSuccess) return fail(c, SGP_E_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
     c->launches += 1;
   }
-  std::vector<double> tot(len);
   SGP_CUDA(c, cudaMemcpyAsync(tot.data(), o.total, len * 8, cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
   auto at = [&](int s) { return pos ? pos[s] : s; };

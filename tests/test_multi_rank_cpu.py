@@ -50,7 +50,7 @@ def _worker(rank, world, port, ret):
         ret["db"] = float(np.abs(out[m * m:] - b0).max() / np.abs(b0).max())
     # the hyper-parameter objective (GPC:73-78) is a sum over EXPERTS: rank r owns experts r, r+world, ... of the
     # reference's grouping (point i -> expert i % E) and one all-reduce of the packed [nll; grad] row gives the total --
-    # the contract of sgp_experts_upload + sgp_bcm_nll / sgp_laplace_nll (tools/multi_gpu_check.py runs it on GPUs)
+    # the contract of sgp_experts_upload + sgp_bcm_nll / sgp_laplace_nll (tests/test_gpu_multi_rank.py runs it on GPUs)
     full = oracle.get_expert_labels_and_kernels(X, y, fac, 100)
     mine = full[rank::world]
     v, g = bcm_objective(mine, theta)
