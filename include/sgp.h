@@ -108,8 +108,8 @@ int sgp_comm_unique_id(void* out128);                                   /* rank 
  * fails, leaving ctx without a communicator.  A refused call leaves ctx usable.
  * With a communicator of nranks > 1, sgp_stats_finish, sgp_bcm_nll, _folds, _slots and sgp_laplace_nll, _any_size,
  * _classes, _classes_any_size, _slots_any_size, _fold_slots_any_size each make exactly one ncclAllReduce, and a status
- * decided on one rank (SGP_E_RANGE, SGP_E_SINGULAR, SGP_E_NOT_PD) is returned on every rank.  The other entries are
- * rank-local.  The caller's obligation: every rank makes the same sequence of these calls, with the same kernel
+ * decided on one rank (SGP_E_RANGE, SGP_E_SINGULAR, SGP_E_NOT_PD) is returned on every rank.  sgp_kmeans_sharded[_device]
+ * makes collectives of its own (see there).  The other entries are rank-local.  The caller's obligation: every rank makes the same sequence of these calls, with the same kernel
  * structure, n_eval and descriptor layout.  Refusals that depend on the rank's own data return BEFORE the collective and
  * leave the peers blocked in it: the on-chip Laplace limit (117 points in the largest expert), the global-memory Laplace
  * kernel's limit (SGP_E_BADARG above its per-expert point bound), the 46340-point limit of
@@ -174,6 +174,16 @@ int sgp_experts_upload_grouped(sgp_ctx* ctx, const void* X, int32_t x_is_f32, co
  * allocation or launch. */
 int sgp_experts_upload_grouped_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, const double* dy, int64_t n,
                                       int32_t d, int32_t dataset_size_for_expert);
+
+/* The grouped upload with the number of experts given instead of derived from datasetSizeForExpert: point i of dX -> expert
+ * i % n_experts, the same offsets, gather and bits as sgp_experts_upload_grouped_device with that E.  A rank of a
+ * data-parallel fit uploads with it the rows of its own block of the global experts [e0, e0 + n_experts): taken in global
+ * row order, row e + j E_total of expert e is local row (e - e0) + j n_experts, so each expert is the single-GPU upload's,
+ * row for row.  SGP_E_BADARG for null pointers, n < 1, d < 1, n_experts < 1, n_experts > n (an empty expert), and for
+ * pointers that are not device memory on the context's device, before any allocation or launch.  The modes of such an
+ * upload can be ungrouped (sgp_experts_get_f_rows_device). */
+int sgp_experts_upload_strided_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, const double* dy, int64_t n,
+                                      int32_t d, int64_t n_experts);
 
 /* One hyper-parameter, in the order of Kernel.getHyperparameters (depth first, trainable scalar prepended). */
 enum { SGP_HYPER_SCALE = 0, SGP_HYPER_ARD_BETA = 1, SGP_HYPER_RBF_SIGMA = 2 };
@@ -492,6 +502,31 @@ int sgp_kmeans_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n,
                       double tol, int64_t seed, const double* init_centers /* k x d, or NULL: k-means|| */,
                       double* centers_out /* k x d */, int32_t* k_out, int32_t* labels_out /* n, or NULL */,
                       int32_t* iterations_out, double* cost_out);
+
+/* sgp_kmeans on the concatenation of the ranks' rows over the context's communicator (sgp_comm_init): this rank holds the
+ * global rows [offset, offset + n) of n_total, the ranks' blocks following each other in rank order (n = 0 is allowed).
+ * The algorithm is sgp_kmeans's on the n_total rows: draws at the global row index, the first centre from its owner, the
+ * origin's column sums and the k-means|| cost sums as each rank's fixed-order sum summed over the ranks, the chosen
+ * candidates gathered in global index order (their rows' bit patterns summed as integers, so exact), candidate weights as
+ * int64 counts summed over the ranks, and each Lloyd step's per-cluster fp64 sums (point order on each rank) and counts
+ * summed over the ranks before every rank moves the centres by sum * (1 / count).  Everything that follows from the
+ * summed values (the distinct filter, the local k-means++ and its Lloyd iterations, convergence) runs identically on
+ * every rank, so every rank returns the same centres, k_out, iterations and cost; labels_out gets this rank's n labels.
+ * With one rank, or without a communicator, the outputs are sgp_kmeans's on X bit for bit; on data whose fp32 distances
+ * and fp64 sums are exact (integer coordinates), they are sgp_kmeans's on the concatenation at any number of ranks.
+ * Every rank must make the call with the same d, k, max_iter, tol, seed, n_total and initial centres.  Refusals: those of
+ * sgp_kmeans on every rank alike (the arguments every rank shares are checked first; the layout -- n, offset, a null or
+ * foreign X -- and NaN / infinity are summed over the ranks before any rank refuses, so every rank refuses together).
+ * SGP_E_NOMEM and CUDA errors stay rank-local. */
+int sgp_kmeans_sharded(sgp_ctx* ctx, const void* X, int32_t x_is_f32, int64_t n, int64_t offset, int64_t n_total,
+                       int32_t d, int32_t k, int32_t max_iter, double tol, int64_t seed,
+                       const double* init_centers /* k x d, or NULL */, double* centers_out /* k x d */, int32_t* k_out,
+                       int32_t* labels_out /* n, or NULL */, int32_t* iterations_out, double* cost_out);
+/* sgp_kmeans_sharded on dX in device memory, read in place (as sgp_kmeans_device). */
+int sgp_kmeans_sharded_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n, int64_t offset, int64_t n_total,
+                              int32_t d, int32_t k, int32_t max_iter, double tol, int64_t seed,
+                              const double* init_centers, double* centers_out, int32_t* k_out, int32_t* labels_out,
+                              int32_t* iterations_out, double* cost_out);
 
 /* Evaluate K(X_test, Z) (n x m row-major fp64 out) with the current kernel -- the `crossKernel`
  * contract of kernel/Kernel.scala:69-74 (used by the golden-vector tests). */

@@ -65,14 +65,26 @@ class GaussianProcessClassificationModel:
 class GaussianProcessClassifier(GaussianProcessParams):
     """GPCls:42-135."""
 
-    def __init__(self, device: int = 0):
+    def __init__(self, device: int = 0, process_group=None):
+        """process_group: a torch.distributed process group (one process per GPU, NCCL) to fit over; each rank then
+        passes its own shard to `fit` (`spark_gp_b200.distributed`)."""
         super().__init__()
         self._device = device
+        self._process_group = process_group
         self.last_objective = None
 
     def fit(self, X, y, hyperparameters=None) -> GaussianProcessClassificationModel:
         """X may be a CUDA tensor on the classifier's device (y a CUDA tensor there too, or a host vector): X, the labels
-        and the latent modes then stay on the device, and `last_latent` is a CUDA float64 tensor."""
+        and the latent modes then stay on the device, and `last_latent` is a CUDA float64 tensor.
+        With a process group, (X, y) is this rank's shard (possibly empty, 0 x d) and every rank returns the model of the
+        concatenation of the shards in rank order, the same bits on every rank; `last_latent` then holds the modes of the
+        rows of this rank's experts, in global row order."""
+        if self._process_group is not None:
+            from . import distributed
+            eng, kernel, theta, active_set, mv, mm, self.last_stats, self.last_latent = distributed.fit(
+                self, X, y, hyperparameters, True)
+            return GaussianProcessClassificationModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, active_set),
+                                                      theta)
         X, y = fit_data(X, y, self._device, "GaussianProcessClassifier.fit")
         assert_labels_are_01(y)
         eng = ProjectedProcessEngine.acquire(self._device)

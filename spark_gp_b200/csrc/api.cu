@@ -385,6 +385,15 @@ static int launch_stats(Ctx* c, const void* dX, int x_is_f32, const double* dy, 
   return SGP_OK;
 }
 
+// In-place sum of `count` elements of device memory over the context's communicator, on its stream (a no-op without a
+// communicator of more than one rank).  For the sharded K-means: its few collectives are small and synchronous.
+int comm_sum(Ctx* c, void* buf, size_t count, ncclDataType_t type) {
+  if (!c->comm || c->nranks <= 1 || count == 0) return SGP_OK;
+  const ncclResult_t r = nccl().AllReduce(buf, buf, count, type, ncclSum, c->comm, c->stream);
+  if (r != ncclSuccess) return fail(c, SGP_E_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
+  c->launches += 1;
+  return SGP_OK;
+}
 }  // namespace sgp
 
 using namespace sgp;
@@ -499,6 +508,7 @@ int sgp_comm_init(sgp_ctx* h, const void* id128, int rank, int nranks) {
   c->rank = rank; c->nranks = nranks;
   return SGP_OK;
 }
+
 
 int sgp_stats_begin(sgp_ctx* h, const sgp_kernel_desc* k, const double* Z, int32_t m, int32_t d) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
@@ -917,19 +927,8 @@ int sgp_experts_upload(sgp_ctx* h, const double* X, const double* y, const int64
 
 namespace {
 // sgp_experts_upload_grouped and its _device form: X and y are host memory (staged) or device memory (read in place)
-int upload_grouped(Ctx* c, bool on_device, const void* X, int x_is_f32, const double* y, long long n, int d,
-                   int dataset_size_for_expert, const char* entry) {
-  if (!X || !y || n <= 0 || d <= 0 || dataset_size_for_expert <= 0)
-    return fail(c, SGP_E_BADARG, std::string(entry) + ": null or empty argument");
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  if (on_device) {
-    int rc = device_ptr_ok(c, X, entry, "X");
-    if (rc == SGP_OK) rc = device_ptr_ok(c, y, entry, "y");
-    if (rc != SGP_OK) return rc;
-  }
-  // GPC:27  numberOfExperts = Math.round(points.count() / datasetSizeForExpert)  (round half up on a positive double)
-  const long long E = static_cast<long long>(std::floor(static_cast<double>(n) / dataset_size_for_expert + 0.5));
-  if (E <= 0) return fail(c, SGP_E_BADARG, "numberOfExperts == 0 (N < datasetSizeForExpert / 2): the reference fails with / by zero");
+// E experts, point i -> expert i % E (after the caller's argument checks)
+int upload_strided(Ctx* c, bool on_device, const void* X, int x_is_f32, const double* y, long long n, int d, long long E) {
   int rc = experts_alloc(c, E, n, d, static_cast<int>(n / E + ((n % E) ? 1 : 0)));
   if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_set_first, 2 * 8);
   if (rc != SGP_OK) return rc;
@@ -950,6 +949,22 @@ int upload_grouped(Ctx* c, bool on_device, const void* X, int x_is_f32, const do
   c->ex.E = E;
   c->ex_grouped = true;
   return SGP_OK;
+}
+
+int upload_grouped(Ctx* c, bool on_device, const void* X, int x_is_f32, const double* y, long long n, int d,
+                   int dataset_size_for_expert, const char* entry) {
+  if (!X || !y || n <= 0 || d <= 0 || dataset_size_for_expert <= 0)
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": null or empty argument");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  if (on_device) {
+    int rc = device_ptr_ok(c, X, entry, "X");
+    if (rc == SGP_OK) rc = device_ptr_ok(c, y, entry, "y");
+    if (rc != SGP_OK) return rc;
+  }
+  // GPC:27  numberOfExperts = Math.round(points.count() / datasetSizeForExpert)  (round half up on a positive double)
+  const long long E = static_cast<long long>(std::floor(static_cast<double>(n) / dataset_size_for_expert + 0.5));
+  if (E <= 0) return fail(c, SGP_E_BADARG, "numberOfExperts == 0 (N < datasetSizeForExpert / 2): the reference fails with / by zero");
+  return upload_strided(c, on_device, X, x_is_f32, y, n, d, E);
 }
 
 // sgp_experts_upload_folds and its _device form; fold_of is host memory in both
@@ -1045,6 +1060,21 @@ int sgp_experts_upload_grouped_device(sgp_ctx* h, const void* dX, int32_t x_is_f
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
   return upload_grouped(c, true, dX, x_is_f32, dy, n, d, dataset_size_for_expert, "sgp_experts_upload_grouped_device");
+}
+
+int sgp_experts_upload_strided_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, const double* dy, int64_t n, int32_t d,
+                                      int64_t n_experts) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  const char* entry = "sgp_experts_upload_strided_device";
+  if (!dX || !dy || n <= 0 || d <= 0 || n_experts <= 0)
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": null or empty argument");
+  if (n_experts > n) return fail(c, SGP_E_BADARG, std::string(entry) + ": more experts than points (an empty expert)");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  int rc = device_ptr_ok(c, dX, entry, "X");
+  if (rc == SGP_OK) rc = device_ptr_ok(c, dy, entry, "y");
+  if (rc != SGP_OK) return rc;
+  return upload_strided(c, true, dX, x_is_f32, dy, n, d, n_experts);
 }
 
 int sgp_experts_upload_folds(sgp_ctx* h, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
@@ -1967,6 +1997,57 @@ int greedy_active_set(Ctx* c, bool on_device, const sgp_kernel_desc* k, const do
                     reinterpret_cast<long long*>(indices_out));
 }
 
+// sgp_kmeans_sharded and its _device form: every refusal is taken on every rank together (the layout table and the
+// local argument verdicts are all-reduced before anything else)
+int kmeans_sharded(Ctx* c, bool on_device, const void* X, int32_t x_is_f32, int64_t n, int64_t offset, int64_t n_total,
+                   int32_t d, int32_t k, int32_t max_iter, double tol, int64_t seed, const double* init_centers,
+                   double* centers_out, int32_t* k_out, int32_t* labels_out, int32_t* iterations_out, double* cost_out,
+                   const char* entry) {
+  if (!centers_out || !k_out || !iterations_out || !cost_out)
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": null argument");
+  if (k < 2) return fail(c, SGP_E_BADARG, "requirement failed: k must be > 1");
+  if (max_iter < 0) return fail(c, SGP_E_BADARG, "requirement failed: maxIter must be >= 0");
+  if (!(tol >= 0.0)) return fail(c, SGP_E_BADARG, "requirement failed: tol must be >= 0");
+  if (d < 1) return fail(c, SGP_E_BADARG, std::string(entry) + ": no features");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  int local_bad = (n < 0 || n > 2147483647LL || offset < 0 || (n > 0 && !X)) ? 1 : 0;
+  if (!local_bad && n > 0 && on_device && device_ptr_ok(c, X, entry, "X") != SGP_OK) local_bad = 2;
+  if (init_centers)
+    for (size_t i = 0; i < static_cast<size_t>(k) * d; ++i)
+      if (!std::isfinite(init_centers[i]))
+        return fail(c, SGP_E_BADARG, std::string(entry) + ": initial centres contain NaN or infinity");
+  // the layout table [rank][n, offset, verdict], summed over the ranks: every rank checks every rank's entry
+  const int R = c->comm ? c->nranks : 1, me = c->comm ? c->rank : 0;
+  std::vector<long long> table(static_cast<size_t>(R) * 3, 0);
+  table[static_cast<size_t>(me) * 3] = n;
+  table[static_cast<size_t>(me) * 3 + 1] = offset;
+  table[static_cast<size_t>(me) * 3 + 2] = local_bad;
+  int rc = ctx_scratch(c, c->kmeans_comm_ws, table.size() * 8);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaMemcpyAsync(c->kmeans_comm_ws.p, table.data(), table.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  rc = comm_sum(c, c->kmeans_comm_ws.p, table.size(), ncclInt64);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaMemcpyAsync(table.data(), c->kmeans_comm_ws.p, table.size() * 8, cudaMemcpyDeviceToHost, c->stream));
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  long long next = 0;
+  for (int r = 0; r < R; ++r) {
+    const long long* t = &table[static_cast<size_t>(r) * 3];
+    if (t[2] == 2) return fail(c, SGP_E_BADARG, std::string(entry) + ": X of rank " + std::to_string(r) +
+                                                    " is not device memory on its context's device");
+    if (t[2] != 0 || t[1] != next)
+      return fail(c, SGP_E_BADARG, std::string(entry) + ": rank " + std::to_string(r) + " holds rows [" +
+                                       std::to_string(t[1]) + ", +" + std::to_string(t[0]) + "); the ranks' rows must " +
+                                       "follow each other in rank order from 0");
+    next += t[0];
+  }
+  if (next != n_total || n_total < 1)
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": the ranks hold " + std::to_string(next) + " rows, n_total is " +
+                                     std::to_string(n_total));
+  return run_kmeans_sharded(c, X, x_is_f32, on_device, n, offset, n_total, d, k, max_iter, tol,
+                            static_cast<uint64_t>(seed), init_centers, centers_out, k_out, labels_out, iterations_out,
+                            cost_out);
+}
+
 int kmeans(Ctx* c, bool on_device, const void* X, int32_t x_is_f32, int64_t n, int32_t d, int32_t k, int32_t max_iter,
            double tol, int64_t seed, const double* init_centers, double* centers_out, int32_t* k_out, int32_t* labels_out,
            int32_t* iterations_out, double* cost_out, const char* entry) {
@@ -2023,6 +2104,26 @@ int sgp_kmeans_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, int64_t n, i
   if (!c) return SGP_E_BADARG;
   return kmeans(c, true, dX, x_is_f32, n, d, k, max_iter, tol, seed, init_centers, centers_out, k_out, labels_out,
                 iterations_out, cost_out, "sgp_kmeans_device");
+}
+
+int sgp_kmeans_sharded(sgp_ctx* h, const void* X, int32_t x_is_f32, int64_t n, int64_t offset, int64_t n_total, int32_t d,
+                       int32_t k, int32_t max_iter, double tol, int64_t seed, const double* init_centers,
+                       double* centers_out, int32_t* k_out, int32_t* labels_out, int32_t* iterations_out,
+                       double* cost_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return kmeans_sharded(c, false, X, x_is_f32, n, offset, n_total, d, k, max_iter, tol, seed, init_centers, centers_out,
+                        k_out, labels_out, iterations_out, cost_out, "sgp_kmeans_sharded");
+}
+
+int sgp_kmeans_sharded_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, int64_t n, int64_t offset, int64_t n_total,
+                              int32_t d, int32_t k, int32_t max_iter, double tol, int64_t seed,
+                              const double* init_centers, double* centers_out, int32_t* k_out, int32_t* labels_out,
+                              int32_t* iterations_out, double* cost_out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  return kmeans_sharded(c, true, dX, x_is_f32, n, offset, n_total, d, k, max_iter, tol, seed, init_centers, centers_out,
+                        k_out, labels_out, iterations_out, cost_out, "sgp_kmeans_sharded_device");
 }
 
 int sgp_cross_kernel(sgp_ctx* h, const double* X, int64_t n, double* K_out) {

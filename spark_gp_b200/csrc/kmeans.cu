@@ -176,12 +176,13 @@ __global__ void __launch_bounds__(256) kmeans_sum_kernel(const double* __restric
   if (threadIdx.x == 0) part[blockIdx.x] = sh[0];
 }
 
-// k-means|| step: point i is chosen iff u(seed, stream, i) < (2k cost_i) / S (a NaN threshold chooses nothing)
-__global__ void kmeans_sample_kernel(const double* __restrict__ cost, int n, double two_k, double S, uint64_t seed,
-                                     uint64_t stream, unsigned char* __restrict__ flag) {
+// k-means|| step: point i (global row i0 + i) is chosen iff u(seed, stream, i0 + i) < (2k cost_i) / S (a NaN threshold
+// chooses nothing)
+__global__ void kmeans_sample_kernel(const double* __restrict__ cost, int n, long long i0, double two_k, double S,
+                                     uint64_t seed, uint64_t stream, unsigned char* __restrict__ flag) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  flag[i] = km_u(seed, stream, static_cast<uint64_t>(i)) < (two_k * cost[i]) / S ? 1 : 0;
+  flag[i] = km_u(seed, stream, static_cast<uint64_t>(i0 + i)) < (two_k * cost[i]) / S ? 1 : 0;
 }
 
 __global__ void kmeans_fill_kernel(double* __restrict__ v, int n, double x) {
@@ -249,6 +250,45 @@ __global__ void __launch_bounds__(256) kmeans_update_kernel(const T* __restrict_
   }
   for (int off = 16; off > 0; off >>= 1) moved += __shfl_down_sync(0xffffffffu, moved, off);
   if (lane == 0 && notconv && !(moved <= tol2)) *notconv = 1;
+}
+
+// The sharded Lloyd step's two halves, split at the all-reduce.  kmeans_sums_kernel: one warp per cluster j sums its
+// members on this rank in point-index order, exactly as kmeans_update_kernel without weights does, and counts them.
+template <typename T>
+__global__ void __launch_bounds__(256) kmeans_sums_kernel(const T* __restrict__ X, int d, const int* __restrict__ order,
+                                                          const int* __restrict__ beg, const int* __restrict__ end, int k,
+                                                          double* __restrict__ sums, long long* __restrict__ cnt) {
+  const int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (j >= k) return;
+  const int b = beg[j], e = end[j];
+  if (lane == 0) cnt[j] = e - b;
+  for (int c = lane; c < d; c += 32) {
+    double s = 0.0;
+#pragma unroll 4
+    for (int m = b; m < e; ++m) s = __dadd_rn(s, static_cast<double>(X[static_cast<size_t>(order[m]) * d + c]));
+    sums[static_cast<size_t>(j) * d + c] = s;
+  }
+}
+
+// kmeans_centre_kernel: the summed clusters' centres, sum * (1 / count), and the moved flag, with kmeans_update_kernel's
+// arithmetic; an empty cluster keeps its centre.
+__global__ void __launch_bounds__(256) kmeans_centre_kernel(const double* __restrict__ sums,
+                                                            const long long* __restrict__ cnt, int k, int d,
+                                                            double* __restrict__ Cc, double tol2, int* notconv) {
+  const int j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (j >= k) return;
+  const double ws = static_cast<double>(cnt[j]);
+  if (ws == 0.0) return;
+  const double inv = 1.0 / ws;
+  double moved = 0.0;
+  for (int c = lane; c < d; c += 32) {
+    const double nc = __dmul_rn(sums[static_cast<size_t>(j) * d + c], inv);
+    const double df = nc - Cc[static_cast<size_t>(j) * d + c];
+    moved = fma(df, df, moved);
+    Cc[static_cast<size_t>(j) * d + c] = nc;
+  }
+  for (int off = 16; off > 0; off >>= 1) moved += __shfl_down_sync(0xffffffffu, moved, off);
+  if (lane == 0 && !(moved <= tol2)) *notconv = 1;
 }
 
 // local k-means++ (LocalKMeans.kMeansPlusPlus): a cluster of zero weight gets cand[floor(u * C)], u from stream 101 with a
@@ -364,6 +404,9 @@ struct KMeansRun {
   int n, d, k;
   uint64_t seed;
   cudaStream_t s;
+  // sgp_kmeans_sharded: this rank holds the global rows [off, off + n) of N; the collectives sum over c's communicator
+  bool sharded = false;
+  long long off = 0, N = 0;
   // point-sized workspace
   T* dX = nullptr;
   int *label = nullptr, *iota = nullptr, *sel = nullptr, *keys = nullptr, *vals = nullptr, *ints = nullptr;
@@ -372,12 +415,33 @@ struct KMeansRun {
   void* cub_tmp = nullptr;
   size_t cub_bytes = 0;
   // centre workspace (k rows)
-  double *Cc = nullptr, *wsum = nullptr;
+  double *Cc = nullptr, *wsum = nullptr, *sums = nullptr;
+  long long* cnts = nullptr;
   float* Cf = nullptr;
   int *beg = nullptr, *end = nullptr;
   int slices = 1, rows_per_slice = 1;
 
   int sync() { SGP_CUDA(c, cudaStreamSynchronize(s)); return SGP_OK; }
+
+  // host values summed element-wise over the ranks (sharded only), in place
+  int allsum(void* host, size_t count, ncclDataType_t type) {
+    if (!sharded || count == 0) return SGP_OK;
+    const size_t bytes = count * 8;                            // every type summed here is 8 bytes wide
+    int rc = ctx_scratch(c, c->kmeans_comm_ws, bytes);
+    if (rc != SGP_OK) return rc;
+    SGP_CUDA(c, cudaMemcpyAsync(c->kmeans_comm_ws.p, host, bytes, cudaMemcpyHostToDevice, s));
+    rc = comm_sum(c, c->kmeans_comm_ws.p, count, type);
+    if (rc != SGP_OK) return rc;
+    SGP_CUDA(c, cudaMemcpyAsync(host, c->kmeans_comm_ws.p, bytes, cudaMemcpyDeviceToHost, s));
+    return sync();
+  }
+
+  // fixed_sum over the ranks: each rank's fixed-order sum, then their sum
+  double global_sum(const double* v, int m, int& rc) {
+    double t = fixed_sum(v, m, rc);
+    if (rc == SGP_OK) rc = allsum(&t, 1, ncclDouble);
+    return t;
+  }
 
   double fixed_sum(const double* v, int m, int& rc) {
     const int per = (m + kSumBlocks - 1) / kSumBlocks;
@@ -416,6 +480,49 @@ struct KMeansRun {
     return SGP_OK;
   }
 
+  // the Lloyd update over the ranks: this rank's per-cluster sums (point order) and counts, summed over the ranks, then
+  // every rank moves the centres from the same totals
+  int update_sharded(int kk, double tol2, int* notconv) {
+    SGP_CUDA(c, cudaMemsetAsync(beg, 0, static_cast<size_t>(kk) * sizeof(int), s));
+    SGP_CUDA(c, cudaMemsetAsync(end, 0, static_cast<size_t>(kk) * sizeof(int), s));
+    if (n > 0) {
+      size_t tb = cub_bytes;
+      SGP_CUDA(c, cub::DeviceRadixSort::SortPairs(cub_tmp, tb, label, keys, iota, vals, n, 0, label_bits(kk), s));
+      kmeans_bounds_kernel<<<blocks(n, 256), 256, 0, s>>>(keys, n, beg, end);
+      c->launches += 2;
+    }
+    kmeans_sums_kernel<T><<<blocks(static_cast<long long>(kk) * 32, 256), 256, 0, s>>>(dX, d, vals, beg, end, kk, sums,
+                                                                                      cnts);
+    SGP_CUDA(c, cudaGetLastError());
+    c->launches += 1;
+    int rc = comm_sum(c, sums, static_cast<size_t>(kk) * d, ncclDouble);
+    if (rc == SGP_OK) rc = comm_sum(c, cnts, static_cast<size_t>(kk), ncclInt64);
+    if (rc != SGP_OK) return rc;
+    kmeans_centre_kernel<<<blocks(static_cast<long long>(kk) * 32, 256), 256, 0, s>>>(sums, cnts, kk, d, Cc, tol2, notconv);
+    SGP_CUDA(c, cudaGetLastError());
+    c->launches += 1;
+    return SGP_OK;
+  }
+
+  // this rank's chosen global indices -> every rank's, in rank order (= global index order: the ranks' rows follow each
+  // other in rank order)
+  int gather_chosen(std::vector<long long>& chosen) {
+    if (!sharded) return SGP_OK;
+    const int R = c->comm ? c->nranks : 1, me = c->comm ? c->rank : 0;
+    std::vector<long long> counts(static_cast<size_t>(R), 0);
+    counts[me] = static_cast<long long>(chosen.size());
+    int rc = allsum(counts.data(), counts.size(), ncclInt64);
+    if (rc != SGP_OK) return rc;
+    long long total = 0, mine = 0;
+    for (int r = 0; r < R; ++r) { if (r == me) mine = total; total += counts[r]; }
+    std::vector<long long> all(static_cast<size_t>(total), 0);
+    std::copy(chosen.begin(), chosen.end(), all.begin() + mine);
+    rc = allsum(all.data(), all.size(), ncclInt64);
+    if (rc != SGP_OK) return rc;
+    chosen.swap(all);
+    return SGP_OK;
+  }
+
   int setup() {
     size_t t1 = 0, t2 = 0;
     SGP_CUDA(c, cub::DeviceRadixSort::SortPairs(nullptr, t1, static_cast<int*>(nullptr), static_cast<int*>(nullptr),
@@ -444,6 +551,7 @@ struct KMeansRun {
     const size_t K = static_cast<size_t>(k);
     auto carve_c = [&](Carve& cv) {
       Cc = cv.take<double>(K * d); wsum = cv.take<double>(K);
+      sums = cv.take<double>(sharded ? K * d : 0); cnts = cv.take<long long>(sharded ? K : 0);
       Cf = cv.take<float>(static_cast<size_t>(rows_pad(k)) * cstride(d));
       beg = cv.take<int>(K); end = cv.take<int>(K);
     };
@@ -469,14 +577,24 @@ struct KMeansRun {
     SGP_CUDA(c, cudaMemcpyAsync(h.data(), part, h.size() * 8, cudaMemcpyDeviceToHost, s));
     SGP_CUDA(c, cudaMemcpyAsync(&bad, ints, sizeof(int), cudaMemcpyDeviceToHost, s));
     SGP_CUDA(c, cudaStreamSynchronize(s));
-    if (bad) return fail(c, SGP_E_BADARG, "sgp_kmeans: X contains NaN or infinity");
-    std::vector<double> oh(d), x0(d);
-    const int rc = rows({0}, x0.data());
+    // [column sums; column sums of squares; non-finite flag], the slices folded in order, then summed over the ranks
+    std::vector<double> ab(static_cast<size_t>(2) * d + 1, 0.0);
+    for (int j = 0; j < d; ++j)
+      for (int q = 0; q < slices; ++q) {
+        ab[j] += h[static_cast<size_t>(q) * 2 * d + j];
+        ab[d + j] += h[static_cast<size_t>(q) * 2 * d + d + j];
+      }
+    ab[2 * d] = bad ? 1.0 : 0.0;
+    int rc = allsum(ab.data(), ab.size(), ncclDouble);
     if (rc != SGP_OK) return rc;
+    if (ab[2 * d] != 0.0) return fail(c, SGP_E_BADARG, "sgp_kmeans: X contains NaN or infinity");
+    std::vector<double> oh(d), x0(d);
+    rc = grows({0}, x0.data());
+    if (rc != SGP_OK) return rc;
+    const double nt = static_cast<double>(N);
     for (int j = 0; j < d; ++j) {
-      double a = 0.0, b = 0.0;
-      for (int q = 0; q < slices; ++q) { a += h[static_cast<size_t>(q) * 2 * d + j]; b += h[static_cast<size_t>(q) * 2 * d + d + j]; }
-      const double mean = a / n, sd = std::sqrt(std::max(b / n - mean * mean, 0.0));
+      const double a = ab[j], b = ab[d + j];
+      const double mean = a / nt, sd = std::sqrt(std::max(b / nt - mean * mean, 0.0));
       if (sd > 0.0 && std::isfinite(sd)) {
         const double q = std::ldexp(1.0, std::ilogb(sd));
         oh[j] = std::nearbyint(mean / q) * q;
@@ -509,21 +627,44 @@ struct KMeansRun {
     return sync();
   }
 
+  // the global rows idx as fp64 into host memory: each rank contributes the rows it holds, and the rows' bit patterns are
+  // summed over the ranks as integers (exact: every other rank adds zero)
+  int grows(const std::vector<long long>& idx, double* out) {
+    if (!sharded) return rows(idx, out);
+    std::vector<long long> mine;
+    std::vector<size_t> where;
+    for (size_t q = 0; q < idx.size(); ++q)
+      if (idx[q] >= off && idx[q] < off + n) { mine.push_back(idx[q] - off); where.push_back(q); }
+    std::vector<double> loc(mine.size() * d);
+    if (!mine.empty()) {
+      const int rc = rows(mine, loc.data());
+      if (rc != SGP_OK) return rc;
+    }
+    std::vector<uint64_t> bits(idx.size() * d, 0);
+    for (size_t q = 0; q < mine.size(); ++q) std::memcpy(&bits[where[q] * d], &loc[q * d], static_cast<size_t>(d) * 8);
+    const int rc = allsum(bits.data(), bits.size(), ncclUint64);
+    if (rc != SGP_OK) return rc;
+    std::memcpy(out, bits.data(), bits.size() * 8);
+    return SGP_OK;
+  }
+
   // k-means|| (KMeans.initKMeansParallel) then, for more than k distinct candidates, the local weighted k-means++ and its
   // Lloyd iterations (LocalKMeans.kMeansPlusPlus).  Leaves the kk initial centres in Cc.
   int init_parallel(int* kk_out) {
-    const long long i0 = std::min<long long>(n - 1, static_cast<long long>(std::floor(km_u(seed, 0, 0) * n)));
+    const long long i0 = std::min<long long>(N - 1, static_cast<long long>(std::floor(km_u(seed, 0, 0) * N)));
     std::vector<long long> cand_idx{i0}, new_idx{i0};
-    kmeans_fill_kernel<<<blocks(n, 256), 256, 0, s>>>(cost, n, INFINITY);
-    kmeans_iota_kernel<<<blocks(n, 256), 256, 0, s>>>(iota, n, 0);
-    SGP_CUDA(c, cudaGetLastError());
-    c->launches += 2;
+    if (n > 0) {
+      kmeans_fill_kernel<<<blocks(n, 256), 256, 0, s>>>(cost, n, INFINITY);
+      kmeans_iota_kernel<<<blocks(n, 256), 256, 0, s>>>(iota, n, 0);
+      SGP_CUDA(c, cudaGetLastError());
+      c->launches += 2;
+    }
     std::vector<double> rows;
     for (int step = 0; step < 2; ++step) {
       const int m = static_cast<int>(new_idx.size());
       if (m > 0) {
         rows.resize(static_cast<size_t>(m) * d);
-        int rc = this->rows(new_idx, rows.data());
+        int rc = grows(new_idx, rows.data());
         if (rc != SGP_OK) return rc;
         const size_t img = (static_cast<size_t>(rows_pad(m)) * cstride(d) * 4 + 255) / 256 * 256;
         rc = ctx_scratch(c, c->kmeans_new_ws, img + rows.size() * 8);
@@ -533,30 +674,37 @@ struct KMeansRun {
         SGP_CUDA(c, cudaMemcpyAsync(R, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice, s));
         rc = centre_images(R, m, F);
         if (rc != SGP_OK) return rc;
-        SGP_CUDA(c, launch_assign<T>(dX, n, d, o, F, m, nullptr, cost, 1, nullptr, s));
-        c->launches += 1;
+        if (n > 0) {
+          SGP_CUDA(c, launch_assign<T>(dX, n, d, o, F, m, nullptr, cost, 1, nullptr, s));
+          c->launches += 1;
+        }
       }
       int rc = SGP_OK;
-      const double S = fixed_sum(cost, n, rc);
+      const double S = global_sum(cost, n, rc);
       if (rc != SGP_OK) return rc;
-      kmeans_sample_kernel<<<blocks(n, 256), 256, 0, s>>>(cost, n, 2.0 * k, S, seed, 1 + step, flag);
-      SGP_CUDA(c, cudaGetLastError());
-      size_t tb = cub_bytes;
-      SGP_CUDA(c, cub::DeviceSelect::Flagged(cub_tmp, tb, iota, flag, sel, ints + 1, n, s));
-      c->launches += 2;
       int cnt = 0;
-      SGP_CUDA(c, cudaMemcpyAsync(&cnt, ints + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
-      SGP_CUDA(c, cudaStreamSynchronize(s));
+      if (n > 0) {
+        kmeans_sample_kernel<<<blocks(n, 256), 256, 0, s>>>(cost, n, off, 2.0 * k, S, seed, 1 + step, flag);
+        SGP_CUDA(c, cudaGetLastError());
+        size_t tb = cub_bytes;
+        SGP_CUDA(c, cub::DeviceSelect::Flagged(cub_tmp, tb, iota, flag, sel, ints + 1, n, s));
+        c->launches += 2;
+        SGP_CUDA(c, cudaMemcpyAsync(&cnt, ints + 1, sizeof(int), cudaMemcpyDeviceToHost, s));
+        SGP_CUDA(c, cudaStreamSynchronize(s));
+      }
       std::vector<int> chosen(cnt);
       if (cnt > 0) SGP_CUDA(c, cudaMemcpyAsync(chosen.data(), sel, static_cast<size_t>(cnt) * 4, cudaMemcpyDeviceToHost, s));
       SGP_CUDA(c, cudaStreamSynchronize(s));
       new_idx.assign(chosen.begin(), chosen.end());
+      for (long long& g : new_idx) g += off;
+      rc = gather_chosen(new_idx);
+      if (rc != SGP_OK) return rc;
       cand_idx.insert(cand_idx.end(), new_idx.begin(), new_idx.end());
     }
     // distinct candidates, first occurrence kept (-0.0 and 0.0 are equal)
     std::vector<double> cand, all(cand_idx.size() * d), r(d);
     std::unordered_set<std::string> seen;
-    int rc = this->rows(cand_idx, all.data());
+    int rc = grows(cand_idx, all.data());
     if (rc != SGP_OK) return rc;
     for (size_t q = 0; q < cand_idx.size(); ++q) {
       std::copy(all.begin() + q * d, all.begin() + (q + 1) * d, r.begin());
@@ -598,10 +746,24 @@ struct KMeansRun {
     rc = centre_images(dcand, C, CF);
     if (rc != SGP_OK) return rc;
     // weights: how many points have each candidate as their nearest
-    SGP_CUDA(c, launch_assign<T>(dX, n, d, o, CF, C, label, dist, 0, nullptr, s));
     SGP_CUDA(c, cudaMemsetAsync(cnt, 0, Cz * sizeof(int), s));
-    kmeans_count_kernel<<<blocks(n, 256), 256, 0, s>>>(label, n, cnt);
-    kmeans_to_double_kernel<<<blocks(C, 256), 256, 0, s>>>(cnt, C, w);
+    if (n > 0) {
+      SGP_CUDA(c, launch_assign<T>(dX, n, d, o, CF, C, label, dist, 0, nullptr, s));
+      kmeans_count_kernel<<<blocks(n, 256), 256, 0, s>>>(label, n, cnt);
+    }
+    if (sharded) {                            // int64 counts summed over the ranks
+      std::vector<int> ci(Cz);
+      SGP_CUDA(c, cudaMemcpyAsync(ci.data(), cnt, Cz * sizeof(int), cudaMemcpyDeviceToHost, s));
+      SGP_CUDA(c, cudaStreamSynchronize(s));
+      std::vector<long long> cl(ci.begin(), ci.end());
+      rc = allsum(cl.data(), cl.size(), ncclInt64);
+      if (rc != SGP_OK) return rc;
+      std::vector<double> wh(cl.begin(), cl.end());
+      SGP_CUDA(c, cudaMemcpyAsync(w, wh.data(), Cz * 8, cudaMemcpyHostToDevice, s));
+      SGP_CUDA(c, cudaStreamSynchronize(s));
+    } else {
+      kmeans_to_double_kernel<<<blocks(C, 256), 256, 0, s>>>(cnt, C, w);
+    }
     kmeans_pp_kernel<<<1, kPPThreads, 0, s>>>(dcand, C, d, w, k, seed, ccost, Cc);
     kmeans_iota_kernel<<<blocks(C, 256), 256, 0, s>>>(clab, C, -1);
     SGP_CUDA(c, cudaGetLastError());
@@ -634,9 +796,11 @@ struct KMeansRun {
     int kk = k;
     if (init) {
       SGP_CUDA(c, cudaMemcpyAsync(Cc, init, static_cast<size_t>(k) * d * 8, cudaMemcpyHostToDevice, s));
-      kmeans_iota_kernel<<<blocks(n, 256), 256, 0, s>>>(iota, n, 0);
-      SGP_CUDA(c, cudaGetLastError());
-      c->launches += 1;
+      if (n > 0) {
+        kmeans_iota_kernel<<<blocks(n, 256), 256, 0, s>>>(iota, n, 0);
+        SGP_CUDA(c, cudaGetLastError());
+        c->launches += 1;
+      }
     } else {
       rc = init_parallel(&kk);
       if (rc != SGP_OK) return rc;
@@ -647,11 +811,14 @@ struct KMeansRun {
     int iteration = 0;
     bool converged = false;
     do {
-      SGP_CUDA(c, launch_assign<T>(dX, n, d, o, Cf, kk, label, dist, 0, nullptr, s));
-      c->launches += 1;
+      if (n > 0) {
+        SGP_CUDA(c, launch_assign<T>(dX, n, d, o, Cf, kk, label, dist, 0, nullptr, s));
+        c->launches += 1;
+      }
       if (max_iter == 0) break;
       SGP_CUDA(c, cudaMemsetAsync(ints + 4, 0, sizeof(int), s));
-      rc = update<T>(dX, n, label, nullptr, kk, tol * tol, ints + 4, cub_tmp, cub_bytes, keys, vals);
+      rc = sharded ? update_sharded(kk, tol * tol, ints + 4)
+                   : update<T>(dX, n, label, nullptr, kk, tol * tol, ints + 4, cub_tmp, cub_bytes, keys, vals);
       if (rc == SGP_OK) rc = centre_images(Cc, kk, Cf);
       if (rc != SGP_OK) return rc;
       int notconv = 0;
@@ -660,10 +827,10 @@ struct KMeansRun {
       converged = notconv == 0;
       ++iteration;
     } while (iteration < max_iter && !converged);
-    const double cost_total = fixed_sum(dist, n, rc);
+    const double cost_total = global_sum(dist, n, rc);
     if (rc != SGP_OK) return rc;
     SGP_CUDA(c, cudaMemcpyAsync(centers_out, Cc, static_cast<size_t>(kk) * d * 8, cudaMemcpyDeviceToHost, s));
-    if (labels_out) SGP_CUDA(c, cudaMemcpyAsync(labels_out, label, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, s));
+    if (labels_out && n > 0) SGP_CUDA(c, cudaMemcpyAsync(labels_out, label, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, s));
     SGP_CUDA(c, cudaStreamSynchronize(s));
     *k_out = kk;
     *iters_out = iteration;
@@ -679,9 +846,24 @@ int run_kmeans(Ctx* c, const void* X, int x_is_f32, bool x_on_device, long long 
                int* iterations_out, double* cost_out) {
   if (x_is_f32) {
     KMeansRun<float> r{c, static_cast<const float*>(X), x_on_device, static_cast<int>(n), d, k, seed, c->stream};
+    r.N = n;
     return r.run(max_iter, tol, init_centers, centers_out, k_out, labels_out, iterations_out, cost_out);
   }
   KMeansRun<double> r{c, static_cast<const double*>(X), x_on_device, static_cast<int>(n), d, k, seed, c->stream};
+  r.N = n;
+  return r.run(max_iter, tol, init_centers, centers_out, k_out, labels_out, iterations_out, cost_out);
+}
+
+int run_kmeans_sharded(Ctx* c, const void* X, int x_is_f32, bool x_on_device, long long n, long long offset,
+                       long long n_total, int d, int k, int max_iter, double tol, uint64_t seed, const double* init_centers,
+                       double* centers_out, int* k_out, int* labels_out, int* iterations_out, double* cost_out) {
+  if (x_is_f32) {
+    KMeansRun<float> r{c, static_cast<const float*>(X), x_on_device, static_cast<int>(n), d, k, seed, c->stream};
+    r.sharded = true; r.off = offset; r.N = n_total;
+    return r.run(max_iter, tol, init_centers, centers_out, k_out, labels_out, iterations_out, cost_out);
+  }
+  KMeansRun<double> r{c, static_cast<const double*>(X), x_on_device, static_cast<int>(n), d, k, seed, c->stream};
+  r.sharded = true; r.off = offset; r.N = n_total;
   return r.run(max_iter, tol, init_centers, centers_out, k_out, labels_out, iterations_out, cost_out);
 }
 

@@ -131,6 +131,7 @@ struct Ctx {
   DevScratch tail_ws, tail_ws2, predict_ws, cross_ws, bcm_ws, sweep_ws, greedy_ws;
   DevScratch kmeans_pts_ws, kmeans_cen_ws, kmeans_new_ws, kmeans_cand_ws;   // sgp_kmeans: point-, centre-, candidate-sized
   DevScratch kmeans_rows_ws;           // sgp_kmeans_device: indices and fp64 copies of the rows the host reads
+  DevScratch kmeans_comm_ws;           // sgp_kmeans_sharded: the buffers its collectives sum over the ranks
   bool has_magic_run = false;
   bool tail_fast = false;              // last sgp_magic took the Cholesky path for both matrices
   ncclComm_t comm = nullptr;
@@ -459,6 +460,13 @@ int run_greedy(Ctx* c, const KernelFlat& kf, const std::vector<double>& beta_fla
 int run_kmeans(Ctx* c, const void* X, int x_is_f32, bool x_on_device, long long n, int d, int k, int max_iter, double tol,
                uint64_t seed, const double* init_centers, double* centers_out, int* k_out, int* labels_out,
                int* iterations_out, double* cost_out);
+// the same algorithm on the concatenation of the ranks' rows (this rank: global rows [offset, offset + n) of n_total); its
+// collectives go over c's communicator
+int run_kmeans_sharded(Ctx* c, const void* X, int x_is_f32, bool x_on_device, long long n, long long offset,
+                       long long n_total, int d, int k, int max_iter, double tol, uint64_t seed, const double* init_centers,
+                       double* centers_out, int* k_out, int* labels_out, int* iterations_out, double* cost_out);
+// in-place sum of count elements of device memory over c's communicator, on c's stream (a no-op for one rank)
+int comm_sum(Ctx* c, void* buf, size_t count, ncclDataType_t type);
 int run_tail(Ctx* c, double* magic_vector, double* magic_matrix);
 // Prediction (tail.cu): predict_prepare sizes the workspace and packs the installed magic matrix (once per pair) for the
 // windows that follow; predict_window enqueues one window of at most predict_window_points(m_pad) device-resident points.

@@ -1,0 +1,347 @@
+"""Data-parallel `fit` of `GaussianProcessRegression` and the binary `GaussianProcessClassifier` over a torch.distributed
+process group: one process per GPU, each passing its own shard, every rank returning the model of the concatenation of
+the shards in rank order (DESIGN.md section 5).
+
+The reference's cluster steps, one by one:
+  * `groupForExperts` (GPC:26-31): E = round(N / datasetSizeForExpert) over all N rows, expert e holds the global rows
+    e, e + E, ...  Rank r owns the experts [r E // R, (r + 1) E // R); every row moves to its expert's owner in one
+    all-to-all, and the rows a rank receives, in global row order, are grouped on its device row i -> expert i % E_r
+    (`sgp_experts_upload_strided_device`), which makes each expert the single-GPU upload's, row for row.
+  * `optimizeHypers` (GPC:66-92): every rank runs the same L-BFGS-B on the reducing objective entries
+    (`sgp_bcm_nll`, `sgp_laplace_nll_any_size`), which all-reduce [value; gradient] and the status words, so every rank
+    sees the same bits and takes the same steps.  The classifier's latent modes stay with their expert's owner.
+  * `getMatrixKmnKnmAndVectorKmny` (PGPH:20-36): each rank accumulates its rows -- the regression its own shard, the
+    classifier its experts' rows with the modes as labels -- and `sgp_stats_finish` all-reduces G and b and the int8
+    status, so AUTO's fall-back to fp64 is taken on every rank together.
+
+A rank that returns before a collective leaves its peers blocked in it.  So before the first collective every rank
+states the refusals it can compute (its data, the global sizes), the ranks exchange them, and if any rank would refuse,
+every rank raises the same exception.  The SGP_E_NOMEM checks depend on each rank's free memory and are not agreed.
+
+`engine_factory` is the context class (a test passes a stand-in)."""
+from __future__ import annotations
+
+import numpy as np
+
+from . import _native as N
+from .engine import ProjectedProcessEngine, device_fit_data, is_cuda_tensor, rows_to_host
+
+# per-expert point limits of the library: the BCM LU path (sgp_bcm_nll) and the global-memory Laplace kernel
+BCM_MAX_EXPERT_POINTS = 46340
+LAPLACE_MAX_EXPERT_POINTS = 46336
+
+_EXCEPTIONS = {e.__name__: e for e in (ValueError, RuntimeError, TypeError, ZeroDivisionError)}
+
+
+class ShardPlan:
+    """Where every row and expert lives, from the ranks' shard sizes in rank order (the same on every rank)."""
+
+    def __init__(self, sizes, rank: int, dataset_size_for_expert: int):
+        self.sizes = np.asarray(sizes, dtype=np.int64)
+        self.R, self.rank = len(self.sizes), int(rank)
+        self.offsets = np.concatenate([[0], np.cumsum(self.sizes)]).astype(np.int64)
+        self.N = int(self.offsets[-1])
+        self.E = int(np.floor(self.N / dataset_size_for_expert + 0.5))       # Math.round(N / n_e), GPC:27
+        # rank r owns the experts [first[r], first[r + 1])
+        self.first = np.array([r * self.E // self.R for r in range(self.R + 1)], dtype=np.int64)
+
+    @property
+    def offset(self) -> int:
+        return int(self.offsets[self.rank])
+
+    @property
+    def local_experts(self) -> int:
+        return int(self.first[self.rank + 1] - self.first[self.rank])
+
+    def owner(self, rows):
+        """The rank owning each global row's expert."""
+        return np.searchsorted(self.first, np.asarray(rows) % self.E, side="right") - 1
+
+    def destinations(self, r: int = None):
+        """The destination rank of each row of rank r's shard (default: this rank)."""
+        r = self.rank if r is None else r
+        return self.owner(np.arange(self.offsets[r], self.offsets[r + 1]))
+
+    def send_counts(self):
+        return np.bincount(self.destinations(), minlength=self.R).astype(np.int64)
+
+    def recv_counts(self):
+        return np.array([int((self.destinations(s) == self.rank).sum()) for s in range(self.R)], dtype=np.int64)
+
+    def expert_rows(self):
+        """The global rows this rank receives, in the order it receives them (global row order)."""
+        e0, e1 = self.first[self.rank], self.first[self.rank + 1]
+        g = np.arange(self.N)
+        return g[(g % self.E >= e0) & (g % self.E < e1)]
+
+    def local_order(self):
+        """The expert-major order of the received rows (expert e0 + q holds rows q, q + E_r, ...): the permutation the
+        strided upload applies."""
+        n, E = int(self.recv_counts().sum()), self.local_experts
+        return np.concatenate([np.arange(q, n, E) for q in range(E)]) if E > 0 else np.arange(0)
+
+
+def _dist():
+    import torch.distributed as dist
+    return dist
+
+
+def group_refusal(plan: ShardPlan, infos, classifier: bool, experts: bool):
+    """The refusal every rank takes, from every rank's (n, d, dtype, local refusal) and the plan, or None: the first
+    rank's own refusal, then a disagreement of the ranks' shapes or dtypes, then the expert grouping's limits (only
+    when the fit groups experts).  Returns (exception class name, message)."""
+    for r, (_, _, _, err) in enumerate(infos):
+        if err is not None:
+            return err[0], "rank %d: %s" % (r, err[1])
+    ds = sorted({d for n, d, _, _ in infos if n > 0} or {infos[0][1]})
+    if len(ds) > 1:
+        return "ValueError", "the ranks' shards have different numbers of features: %s" % ds
+    dtypes = sorted({t for n, _, t, _ in infos if n > 0})
+    if len(dtypes) > 1:
+        return "ValueError", "the ranks' shards have different dtypes: %s" % ", ".join(dtypes)
+    if plan.N == 0:
+        return "ValueError", "every rank's shard is empty"
+    if not experts:
+        return None
+    if plan.E <= 0:
+        return "ZeroDivisionError", "numberOfExperts == 0 (N < datasetSizeForExpert / 2)"
+    if plan.E < plan.R:
+        return "ValueError", ("%d experts for %d ranks: every rank needs at least one expert (lower datasetSizeForExpert "
+                              "or use fewer ranks)" % (plan.E, plan.R))
+    largest = -(-plan.N // plan.E)
+    limit = LAPLACE_MAX_EXPERT_POINTS if classifier else BCM_MAX_EXPERT_POINTS
+    if largest > limit:
+        return "ValueError", "datasetSizeForExpert above %d: the largest expert holds %d points" % (limit, largest)
+    return None
+
+
+def agree(group, n: int, d: int, dtype: str, err, dataset_size_for_expert: int, classifier: bool, experts: bool):
+    """The agreement step, the fit's first collective: every rank's (n, d, dtype, refusal) to every rank.  Raises the
+    agreed refusal on every rank; else returns (the plan, the agreed dtype, the agreed number of features): those of the
+    non-empty shards, which an empty shard takes whatever its own shape."""
+    dist = _dist()
+    infos = [None] * dist.get_world_size(group)
+    dist.all_gather_object(infos, (int(n), int(d), str(dtype), err), group=group)
+    plan = ShardPlan([i[0] for i in infos], dist.get_rank(group), dataset_size_for_expert)
+    verdict = group_refusal(plan, infos, classifier, experts)
+    if verdict is not None:
+        raise _EXCEPTIONS.get(verdict[0], RuntimeError)(verdict[1])
+    first = next(i for i in infos if i[0] > 0)
+    return plan, first[2], first[1]
+
+
+def exchange(plan: ShardPlan, X, y, group):
+    """Moves every row of the shard (torch tensors X n x d, y n, on the group's device) to its expert's owner in one
+    all-to-all of the rows' bytes with y appended.  Returns (X, y) of the rows this rank owns, in global row order."""
+    import torch
+    dist = _dist()
+    d, es = X.shape[1], X.element_size()
+    order = torch.as_tensor(np.argsort(plan.destinations(), kind="stable"), device=X.device)
+    rows = torch.empty((0, d * es + 8), dtype=torch.uint8, device=X.device)
+    if len(X):
+        rows = torch.cat([X.contiguous().view(torch.uint8).reshape(len(X), d * es),
+                          y.reshape(len(y), 1).to(torch.float64).view(torch.uint8)], dim=1)[order].contiguous()
+    send, recv = plan.send_counts(), plan.recv_counts()
+    out = torch.empty((int(recv.sum()), d * es + 8), dtype=torch.uint8, device=X.device)
+    dist.all_to_all_single(out, rows, recv.tolist(), send.tolist(), group=group)
+    if len(out) == 0:
+        return X.new_empty((0, d)), y.new_empty(0, dtype=torch.float64)
+    Xr = out[:, :d * es].contiguous().view(X.dtype).reshape(len(out), d)
+    yr = out[:, d * es:].contiguous().view(torch.float64).reshape(len(out))
+    return Xr, yr
+
+
+def gather_rows(plan: ShardPlan, X, idx, group, device):
+    """The global rows idx of the concatenation as a float64 host array on every rank: the owners contribute the rows
+    (`rows_to_host`, the single-GPU provider's conversion) and the rows' bit patterns are summed as int64 (exact: every
+    other rank adds zero)."""
+    import torch
+    dist = _dist()
+    idx = np.asarray(idx, dtype=np.int64)
+    lo, hi = plan.offset, plan.offset + int(plan.sizes[plan.rank])
+    mine = (idx >= lo) & (idx < hi)
+    out = np.zeros((len(idx), X.shape[1]), dtype=np.int64)
+    if mine.any():
+        out[mine] = np.ascontiguousarray(rows_to_host(X, idx[mine] - lo)).view(np.int64)
+    t = torch.as_tensor(out, device=device)
+    dist.all_reduce(t, group=group)
+    return t.cpu().numpy().view(np.float64)
+
+
+def active_set(gp, plan: ShardPlan, eng, X, theta, group, device):
+    """The active set of the concatenation, the same on every rank: the random provider's single-GPU draw over N
+    (gathered from the owners), the explicit provider's rows, or the sharded GPU K-means."""
+    from .regression import KMeansActiveSetProvider, _RandomActiveSetProvider
+    provider = gp._activeSetProvider
+    if type(provider) is _RandomActiveSetProvider:
+        rng = np.random.default_rng(gp._seed)
+        idx = rng.choice(plan.N, size=min(gp._activeSetSize, plan.N), replace=False)
+        return gather_rows(plan, X, idx, group, device)
+    if type(provider) is KMeansActiveSetProvider:
+        centres, _, _, _ = eng.kmeans_sharded(X, plan.offset, plan.N, int(gp._activeSetSize), max_iter=provider.maxIter,
+                                              tol=1e-4, seed=int(gp._seed), d=X.shape[1])
+        return centres
+    return provider(gp._activeSetSize, X, None, gp.getKernel, theta, gp._seed, gp=gp)
+
+
+def check_provider(provider):
+    """ValueError for a provider that cannot run over a process group (its configuration is the same on every rank, so
+    every rank raises, before any collective).  Only the three classes themselves are accepted, not subclasses: a
+    provider called on one rank's shard could give every rank a different active set, and the all-reduced statistics
+    would then sum over different active sets."""
+    from .regression import ExplicitActiveSetProvider, KMeansActiveSetProvider, _RandomActiveSetProvider
+    if type(provider) is KMeansActiveSetProvider and not provider.on_gpu:
+        raise ValueError("a fit over a process group needs KMeansActiveSetProvider(on_gpu=True): scikit-learn's K-means "
+                         "runs on one host's points")
+    if type(provider) not in (_RandomActiveSetProvider, ExplicitActiveSetProvider, KMeansActiveSetProvider):
+        raise ValueError("%s cannot run over a process group: use the random, explicit or GPU K-means provider"
+                         % type(provider).__name__)
+
+
+# One context with a communicator per (member ranks, device, context class), kept for the process's lifetime: the fits
+# over a group reuse it instead of making a communicator each (the models get contexts of their own).  Every rank of
+# the group makes the same sequence of fits, so every rank finds or makes its entry at the same fit.
+_COMM_ENGINES = {}
+
+
+def comm_engine(group, device_index: int, device, engine_factory):
+    """The group's context with a communicator on device_index, made (and its communicator attached) at first use."""
+    dist = _dist()
+    key = (tuple(dist.get_process_group_ranks(group)), device_index, engine_factory)
+    eng = _COMM_ENGINES.get(key)
+    if eng is None:
+        eng = engine_factory(device_index)
+        try:
+            attach_communicator(eng, group, device)
+        except BaseException:
+            eng.close()
+            raise
+        _COMM_ENGINES[key] = eng
+    return key, eng
+
+
+def attach_communicator(eng, group, device):
+    """One NCCL communicator of the group's ranks on eng: rank 0 makes the id, the group broadcasts it."""
+    dist = _dist()
+    obj = [eng.comm_unique_id() if dist.get_rank(group) == 0 else None]
+    dist.broadcast_object_list(obj, src=dist.get_global_rank(group, 0), group=group, device=device)
+    eng.comm_init(obj[0], dist.get_rank(group), dist.get_world_size(group))
+
+
+def _local_data(X, y, device: int, classifier: bool, what: str):
+    """The shard as the single-GPU fit reads it (regression: float32 X kept, others float64; classifier: float64), with
+    the labels checked for the classifier."""
+    if classifier:
+        from .classification import assert_labels_are_01, fit_data
+        X, y = fit_data(X, y, device, what)
+    elif is_cuda_tensor(X):
+        X, y = device_fit_data(X, y, device, what)
+        import torch
+        if X.dtype not in (torch.float32, torch.float64):
+            X = X.to(torch.float64)
+    else:
+        X = np.asarray(X)
+        X = X if X.dtype == np.float32 else np.asarray(X, dtype=np.float64)
+        y = np.asarray(y, dtype=np.float64)
+    if X.ndim != 2 or y.ndim != 1 or len(y) != len(X):
+        raise ValueError("%s: X must be n x d and y n entries" % what)
+    if classifier:
+        assert_labels_are_01(y)
+    return X, y
+
+
+def _tensor(a, device, dtype=None):
+    import torch
+    t = a if is_cuda_tensor(a) else torch.from_numpy(np.ascontiguousarray(a))
+    t = t.to(device)
+    return t if dtype is None else t.to(dtype)
+
+
+def fit(gp, X, y, hyperparameters, classifier: bool, engine_factory=ProjectedProcessEngine):
+    """The data-parallel fit of gp (a GaussianProcessRegression or binary GaussianProcessClassifier with a process
+    group) on this rank's shard.  The fit runs on the group's context with a communicator (`comm_engine`); the model gets
+    a context of its own holding the active set and magic pair.  Returns (model's engine, kernel, theta, active set, magic
+    vector, magic matrix, (G, b), latent modes of this rank's expert rows or None).  Fits over one group must not run
+    concurrently."""
+    import contextlib
+
+    import torch
+    dist = _dist()
+    group = gp._process_group
+    what = "%s.fit" % type(gp).__name__
+    check_provider(gp._activeSetProvider)
+    nccl = dist.get_backend(group) == "nccl"
+    device = torch.device("cuda", gp._device) if nccl else torch.device("cpu")
+    with torch.cuda.device(gp._device) if nccl else contextlib.nullcontext():
+        experts = classifier or (hyperparameters is None and gp._maxIter > 0)
+        err, n, d, dtype = None, 0, -1, ""
+        try:
+            X, y = _local_data(X, y, gp._device, classifier, what)
+            n, d, dtype = len(X), X.shape[1], str(X.dtype).replace("torch.", "")
+        except (ValueError, TypeError, RuntimeError) as e:
+            err = (type(e).__name__, str(e))
+        plan, dtype, d = agree(group, n, d, dtype, err, gp._datasetSizeForExpert, classifier, experts)
+        if len(X) == 0:                                     # an empty shard takes the agreed dtype and width
+            X = np.empty((0, d), dtype=np.float32 if dtype == "float32" else np.float64)
+            y = np.empty(0)
+        key, eng = comm_engine(group, gp._device, device, engine_factory)
+        try:
+            out = _fit(gp, plan, eng, X, y, hyperparameters, classifier, experts, dtype, group, device)
+        except BaseException:
+            # a failure after a collective may leave the ranks out of step: the communicator is not reused
+            _COMM_ENGINES.pop(key, None)
+            eng.close()
+            raise
+        kernel, theta, Z, mv, mm = out[:5]
+        model_eng = engine_factory(gp._device)
+        model_eng.begin(kernel, Z)
+        model_eng.set_magic(mv, mm)
+        return (model_eng,) + out
+
+
+def _fit(gp, plan, eng, X, y, hyperparameters, classifier, experts, dtype, group, device):
+    import torch
+    from .hyperopt import lbfgsb_bounds, optimise_slots
+    eng.set_precision(N.SGP_PREC_AUTO)                      # as on a freshly acquired context
+    k0 = gp.getKernel()
+    theta, Xe, f = None, None, None
+    if experts:
+        Xe, ye = exchange(plan, _tensor(X, device, getattr(torch, dtype)), _tensor(y, device, torch.float64), group)
+        eng.experts_upload_strided(Xe, ye, plan.local_experts)
+    if classifier:
+        from .classification import laplace_optimise
+        objective = lambda batch: [eng.laplace_nll_any_size(gp.getKernel().setHyperparameters(t), gp._tol)
+                                   for _, t in batch]
+        (theta,), fit = laplace_optimise(gp, eng, objective, [k0.getHyperparameters()],
+                                         None if hyperparameters is None else
+                                         [np.asarray(hyperparameters, dtype=np.float64)])
+        if fit["slots"] is not None:
+            gp.last_objective = dict(fit["slots"][0], launches=fit["launches"])
+        n_e = len(Xe)
+        if is_cuda_tensor(X):                               # the modes stay on the device, ungrouped into row order
+            f = eng.experts_modes_rows(N.SGP_MODES_BINARY, 0, n_e)
+        else:
+            f = np.empty(n_e)
+            f[plan.local_order()] = eng.experts_modes(N.SGP_MODES_BINARY, 0, n_e)
+            Xe = Xe.cpu().numpy()
+        stats_X, stats_y = Xe, f
+        eng.set_precision(N.SGP_PREC_AUTO)
+    else:
+        if hyperparameters is not None:
+            theta = np.asarray(hyperparameters, dtype=np.float64)
+        elif gp._maxIter > 0:
+            launches0 = eng.launch_count()
+            evaluate = lambda batch: [eng.bcm_nll(gp.getKernel().setHyperparameters(t)) for _, t in batch]
+            (theta,), records, _ = optimise_slots(evaluate, [k0.getHyperparameters()], lbfgsb_bounds(k0), gp._maxIter,
+                                                  gp._tol)
+            if records is not None:
+                gp.last_objective = dict(records[0], n_experts=plan.E, launches=eng.launch_count() - launches0)
+        else:
+            theta = k0.getHyperparameters()
+        theta = np.asarray(theta, dtype=np.float64)
+        stats_X, stats_y = X, y
+    Z = active_set(gp, plan, eng, X, theta, group, device)
+    kernel = gp.getKernel().setHyperparameters(theta)
+    G, b = eng.statistics(kernel, Z, stats_X, stats_y, getattr(gp, "_shard_points", 1 << 22))
+    mv, mm = eng.magic()
+    return kernel, theta, Z, mv, mm, (G, b), f

@@ -304,6 +304,17 @@ class ProjectedProcessEngine:
         self._experts_d = X.shape[1]
         return int(np.floor(len(X) / dataset_size_for_expert + 0.5))
 
+    def experts_upload_strided(self, X, y, n_experts: int):
+        """Groups CUDA tensor rows into n_experts experts on the device, row i -> expert i % n_experts
+        (`sgp_experts_upload_strided_device`): a data-parallel fit's rank uploads its block of the global experts with it,
+        its rows in global row order.  Returns n_experts."""
+        X, y, px, py, f32 = self._device_xy(X, y, "experts_upload_strided")
+        if X.ndim != 2 or y.shape != (len(X),):
+            raise ValueError("experts_upload_strided: X must be n x d and y n entries")
+        self._check(self._lib.sgp_experts_upload_strided_device(self._h, px, f32, py, len(X), X.shape[1], int(n_experts)))
+        self._experts_d = X.shape[1]
+        return int(n_experts)
+
     def _descriptors(self, kernel: Kernel, d: int = None):
         """(kernel desc, hyper-parameter descriptors, their count, the buffers both point into) for d features (default:
         the uploaded experts')."""
@@ -701,6 +712,38 @@ class ProjectedProcessEngine:
         seed = C.c_int64(int(seed) & 0xFFFFFFFFFFFFFFFF).value
         self._check(fn(self._h, px, f32, n, d, k, int(max_iter), float(tol), seed, N.ptr(init) if init is not None else None,
                        N.ptr(centres), C.byref(k_out), N.ptr(labels), C.byref(iters), C.byref(cost)))
+        return np.ascontiguousarray(centres[:k_out.value]), labels[:n], iters.value, cost.value
+
+    def kmeans_sharded(self, X, offset: int, n_total: int, k: int, max_iter: int = 20, tol: float = 1e-4, seed: int = 0,
+                       init_centers=None, d: int = None):
+        """`kmeans` on the concatenation of every rank's rows over this context's communicator (`sgp_kmeans_sharded`;
+        `sgp_kmeans_sharded_device` for a CUDA tensor X): this rank holds the global rows [offset, offset + len(X)) of
+        n_total.  Every rank gets the same (centres, iterations, cost) and the labels of its own rows.  X may be empty
+        (0 x d; give d when X has no shape)."""
+        if is_cuda_tensor(X):
+            import torch
+            X = device_tensor(X, self._device, "kmeans_sharded")
+            px, f32, fn = C.c_void_p(X.data_ptr() if len(X) else None), int(X.dtype == torch.float32), \
+                self._lib.sgp_kmeans_sharded_device
+        else:
+            X = _rows(X)
+            px, f32, fn = (N.ptr(X) if len(X) else None), int(X.dtype == np.float32), self._lib.sgp_kmeans_sharded
+        if X.ndim != 2:
+            raise ValueError("X must be n x d")
+        n, d = len(X), int(X.shape[1] if d is None else d)
+        k = int(k)
+        init = None
+        if init_centers is not None:
+            init = np.ascontiguousarray(init_centers, dtype=np.float64)
+            if init.shape != (k, d):
+                raise ValueError("init_centers must be k x d")
+        centres = np.empty((max(k, 1), max(d, 1)))
+        labels = np.empty(max(n, 1), dtype=np.int32)
+        k_out, iters, cost = C.c_int32(), C.c_int32(), C.c_double()
+        seed = C.c_int64(int(seed) & 0xFFFFFFFFFFFFFFFF).value
+        self._check(fn(self._h, px, f32, n, int(offset), int(n_total), d, k, int(max_iter), float(tol), seed,
+                       N.ptr(init) if init is not None else None, N.ptr(centres), C.byref(k_out), N.ptr(labels),
+                       C.byref(iters), C.byref(cost)))
         return np.ascontiguousarray(centres[:k_out.value]), labels[:n], iters.value, cost.value
 
     def kmn_sweep(self, X):

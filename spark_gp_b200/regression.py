@@ -269,17 +269,27 @@ class GaussianProcessRegressionModel:
 class GaussianProcessRegression(GaussianProcessParams):
     """regression/GaussianProcessRegression.scala:36-73."""
 
-    def __init__(self, device: int = 0, shard_points: int = 1 << 22):
+    def __init__(self, device: int = 0, shard_points: int = 1 << 22, process_group=None):
+        """process_group: a torch.distributed process group (one process per GPU, NCCL) to fit over; each rank then
+        passes its own shard to `fit` (`spark_gp_b200.distributed`)."""
         super().__init__()
         self._device = device
         self._shard_points = shard_points
+        self._process_group = process_group
         self.last_stats = None
 
     def fit(self, X, y, hyperparameters=None) -> GaussianProcessRegressionModel:
         """GPR.train (:43-53).  `hyperparameters` short-circuits optimizeHypers (:48) with a given theta;
         otherwise the BCM objective is optimised when maxIter > 0.
         X may be a CUDA tensor on the estimator's device (y a CUDA tensor there too, or a host vector): X then never
-        leaves the device; only the active set's rows and the small outputs cross PCIe."""
+        leaves the device; only the active set's rows and the small outputs cross PCIe.
+        With a process group, (X, y) is this rank's shard (possibly empty, 0 x d) and every rank returns the model of the
+        concatenation of the shards in rank order, the same bits on every rank."""
+        if self._process_group is not None:
+            from . import distributed
+            eng, kernel, theta, active_set, mv, mm, self.last_stats, _ = distributed.fit(self, X, y, hyperparameters, False)
+            return GaussianProcessRegressionModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, active_set),
+                                                  theta)
         if is_cuda_tensor(X):
             X, y = device_fit_data(X, y, self._device, "GaussianProcessRegression.fit")
         else:
