@@ -40,7 +40,8 @@ enum {
   SGP_E_SINGULAR = 6, /* MatrixSingularException (commons/util/logDetAndInv.scala:27-28), LU info > 0 */
   SGP_E_NOMEM = 7,
   SGP_E_RANGE = 8     /* int8 modes only: scaled squared norms above 4096 (the tensor-core operand range) / above the
-                         magnitude budget (SGP_PREC_I8), or scaled squared norms above 2048 (SGP_PREC_I8_DIRECT); rerun in SGP_PREC_F64 */
+                         magnitude budget (SGP_PREC_I8), or scaled squared norms above 2048 (SGP_PREC_I8_DIRECT); rerun in SGP_PREC_F64.
+                         sgp_kmeans*: a nearest-centre squared distance beyond the fp32 range after the prescale */
 };
 
 /* Flattened kernel DSL (the files under commons/kernel/).  A kernel is a sum of terms  sum_t scale_t * k_t:
@@ -487,9 +488,15 @@ int sgp_greedy_active_set_device(sgp_ctx* ctx, const sgp_kernel_desc* kernel, co
  * Outputs (host): centers_out (k_out x d; k_out < k when the data have fewer distinct points), labels_out (n, or NULL)
  * and cost_out (sum of squared distances) of the last assignment pass -- against the centres before the last update, as
  * Spark's trainingCost --, iterations_out.  Distances are fp32 direct form on points and centres shifted by a common
- * origin in fp64; centre sums are fp64 in point order: two calls return identical bits.  Errors: SGP_E_BADARG for k < 2,
- * max_iter < 0, tol < 0 or NaN, n < 1, d < 1, n > 2^31 - 1 and NaN / infinity in X.  Works outside any begin..finish
- * window and leaves an open window's statistics untouched; rank-local (no communicator). */
+ * origin and scaled by a common power of two 2^s in fp64 (then returned times 2^-2s, in fp64); centre sums are fp64 in
+ * point order: two calls return identical bits.  s = 0 while the largest column standard deviation sd is within
+ * [2^-16, 2^16]; otherwise s brings it into [1, 2), so data whose largest sd lies in [2^-511, 2^512) (about 1.5e-154 to
+ * 1.3e154) keep their spread in the fp32 distances at any scale.  Errors: SGP_E_BADARG for k < 2, max_iter < 0, tol < 0
+ * or NaN, n < 1, d < 1, n > 2^31 - 1 and NaN / infinity in X; SGP_E_RANGE before any k-means step when the largest sd is
+ * outside [2^-511, 2^512) or a column's sum of squares overflows fp64 (|x| above about 1e154), and at the end when a
+ * point's squared distance to its nearest centre is beyond the fp32 range after the prescale (above about 3.4e38 4^-s:
+ * initial centres far outside the data's spread).  Works outside any begin..finish window and leaves an open window's
+ * statistics untouched; rank-local (no communicator). */
 int sgp_kmeans(sgp_ctx* ctx, const void* X, int32_t x_is_f32, int64_t n, int32_t d, int32_t k, int32_t max_iter,
                double tol, int64_t seed, const double* init_centers /* k x d, or NULL: k-means|| */,
                double* centers_out /* k x d */, int32_t* k_out, int32_t* labels_out /* n, or NULL */,
@@ -516,7 +523,8 @@ int sgp_kmeans_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n,
  * and fp64 sums are exact (integer coordinates), they are sgp_kmeans's on the concatenation at any number of ranks.
  * Every rank must make the call with the same d, k, max_iter, tol, seed, n_total and initial centres.  Refusals: those of
  * sgp_kmeans on every rank alike (the arguments every rank shares are checked first; the layout -- n, offset, a null or
- * foreign X -- and NaN / infinity are summed over the ranks before any rank refuses, so every rank refuses together).
+ * foreign X -- and NaN / infinity are summed over the ranks before any rank refuses, so every rank refuses together;
+ * the prescale comes from the summed statistics, and SGP_E_RANGE from a flag summed over the ranks, so both agree).
  * SGP_E_NOMEM and CUDA errors stay rank-local. */
 int sgp_kmeans_sharded(sgp_ctx* ctx, const void* X, int32_t x_is_f32, int64_t n, int64_t offset, int64_t n_total,
                        int32_t d, int32_t k, int32_t max_iter, double tol, int64_t seed,

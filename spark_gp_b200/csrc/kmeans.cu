@@ -3,8 +3,10 @@
 // centre of an empty cluster and stop on an absolute centre-movement rule (DESIGN.md 4.7 restates the algorithm).
 //   * assignment (the hot path): point-stationary fp32 direct-form distances on the CUDA cores.  Each thread holds its
 //     point's coordinates in registers (chunks of DCH for large d), centre tiles are staged in shared memory, a running
-//     min / argmin keeps the lowest index on ties.  Points and centres are shifted by a common origin o in fp64 BEFORE the
-//     fp32 rounding, so the accuracy does not depend on the data's distance from the origin.
+//     min / argmin keeps the lowest index on ties.  Points and centres are shifted by a common origin o and scaled by a
+//     common power of two 2^s in fp64 BEFORE the fp32 rounding, so the accuracy does not depend on the data's distance
+//     from the origin, and fp32 neither underflows nor overflows at the data's scale; distances are returned times 2^-2s
+//     (exact).
 //   * centre update: fp64 sums over the points as given, in point-index order (stable radix sort of the labels, one warp
 //     per cluster), no floating-point atomics: the result does not depend on scheduling.
 //   * every fp64 reduction the algorithm branches on (the k-means|| cost sum, the k-means++ walk) has a fixed order.
@@ -42,15 +44,17 @@ int dchunk(int d) { return d <= 4 ? 4 : d <= 8 ? 8 : d <= 16 ? 16 : 32; }
 int cstride(int d) { const int c = dchunk(d); return (d + c - 1) / c * c; }
 int rows_pad(int k) { return (k + kRowPad - 1) / kRowPad * kRowPad; }
 
-// label[i] / dist[i] = argmin / min over the k centres of |x_i - c|^2 (fp32, lowest index on ties); min_into: dist[i] =
-// min(dist[i], min) and no label (the k-means|| running cost); changed (optional) is set when a label differs from the
-// one already in label[].  Cf: [rows_pad(k)][cstride(d)] fp32 images (c - o), zero padded.
+// label[i] / dist[i] = argmin / min over the k centres of |x_i - c|^2 (fp32 on the images (x - o) scale, lowest index
+// on ties; dist = min inv2 with inv2 = scale^-2); min_into: dist[i] = min(dist[i], min inv2) and no label (the k-means||
+// running cost); changed (optional) is set when a label differs from the one already in label[]; *range is set when a
+// point's nearest distance is not finite.  Cf: [rows_pad(k)][cstride(d)] fp32 images (c - o) scale, zero padded.
 template <typename T, int DCH, int TC>
 __global__ void __launch_bounds__(kAssignThreads) kmeans_assign_kernel(const T* __restrict__ X, int n, int d,
-                                                                       const double* __restrict__ o,
-                                                                       const float* __restrict__ Cf, int k, int cs,
-                                                                       int* __restrict__ label, double* __restrict__ dist,
-                                                                       int min_into, int* __restrict__ changed) {
+                                                                       const double* __restrict__ o, double scale,
+                                                                       double inv2, const float* __restrict__ Cf, int k,
+                                                                       int cs, int* __restrict__ label,
+                                                                       double* __restrict__ dist, int min_into,
+                                                                       int* __restrict__ changed, int* __restrict__ range) {
   __shared__ __align__(16) float sc[TC][DCH];
   const int i = blockIdx.x * kAssignThreads + threadIdx.x;
   const bool live = i < n;
@@ -60,7 +64,9 @@ __global__ void __launch_bounds__(kAssignThreads) kmeans_assign_kernel(const T* 
 #pragma unroll
     for (int kk = 0; kk < DCH; ++kk) {
       const int j = ch * DCH + kk;
-      xs[kk] = (live && j < d) ? static_cast<float>(static_cast<double>(X[static_cast<size_t>(i) * d + j]) - o[j]) : 0.f;
+      xs[kk] = (live && j < d)
+                   ? static_cast<float>((static_cast<double>(X[static_cast<size_t>(i) * d + j]) - o[j]) * scale)
+                   : 0.f;
     }
   };
   if (nch == 1) load_x(0);
@@ -96,36 +102,48 @@ __global__ void __launch_bounds__(kAssignThreads) kmeans_assign_kernel(const T* 
       if (c0 + c < k && acc[c] < best) { best = acc[c]; bi = c0 + c; }
   }
   if (!live) return;
+  if (!(best < INFINITY)) *range = 1;
   if (min_into) {
-    dist[i] = fmin(dist[i], static_cast<double>(best));
+    dist[i] = fmin(dist[i], static_cast<double>(best) * inv2);
     return;
   }
   if (changed && label[i] != bi) *changed = 1;
   label[i] = bi;
-  dist[i] = static_cast<double>(best);
+  dist[i] = static_cast<double>(best) * inv2;
 }
 
+// the data's frame for the fp32 distances: origin o (device, d entries) and the prescale sc = 2^s, inv2 = 2^-2s
+struct Frame {
+  const double* o;
+  double sc, inv2;
+  int* range;
+};
+
 template <typename T>
-cudaError_t launch_assign(const T* X, int n, int d, const double* o, const float* Cf, int k, int* label, double* dist,
+cudaError_t launch_assign(const T* X, int n, int d, const Frame& f, const float* Cf, int k, int* label, double* dist,
                           int min_into, int* changed, cudaStream_t s) {
   const unsigned grid = static_cast<unsigned>((n + kAssignThreads - 1) / kAssignThreads);
   const int cs = cstride(d);
+#define SGP_KM_ASSIGN(DCH, TC)                                                                                             \
+  kmeans_assign_kernel<T, DCH, TC><<<grid, kAssignThreads, 0, s>>>(X, n, d, f.o, f.sc, f.inv2, Cf, k, cs, label, dist,  \
+                                                                   min_into, changed, f.range)
   switch (dchunk(d)) {
-    case 4: kmeans_assign_kernel<T, 4, 64><<<grid, kAssignThreads, 0, s>>>(X, n, d, o, Cf, k, cs, label, dist, min_into, changed); break;
-    case 8: kmeans_assign_kernel<T, 8, 64><<<grid, kAssignThreads, 0, s>>>(X, n, d, o, Cf, k, cs, label, dist, min_into, changed); break;
-    case 16: kmeans_assign_kernel<T, 16, 64><<<grid, kAssignThreads, 0, s>>>(X, n, d, o, Cf, k, cs, label, dist, min_into, changed); break;
-    default: kmeans_assign_kernel<T, 32, 32><<<grid, kAssignThreads, 0, s>>>(X, n, d, o, Cf, k, cs, label, dist, min_into, changed); break;
+    case 4: SGP_KM_ASSIGN(4, 64); break;
+    case 8: SGP_KM_ASSIGN(8, 64); break;
+    case 16: SGP_KM_ASSIGN(16, 64); break;
+    default: SGP_KM_ASSIGN(32, 32); break;
   }
+#undef SGP_KM_ASSIGN
   return cudaGetLastError();
 }
 
-// Cf[r][j] = fp32(C[r][j] - o[j]) for r < k, j < d; zero elsewhere in [rows_pad(k)][cstride(d)]
+// Cf[r][j] = fp32((C[r][j] - o[j]) sc) for r < k, j < d; zero elsewhere in [rows_pad(k)][cstride(d)]
 __global__ void kmeans_centre_f32_kernel(const double* __restrict__ Cc, int k, int d, const double* __restrict__ o,
-                                         float* __restrict__ Cf, int rows, int cs) {
+                                         double sc, float* __restrict__ Cf, int rows, int cs) {
   const long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   if (e >= static_cast<long long>(rows) * cs) return;
   const int r = static_cast<int>(e / cs), j = static_cast<int>(e % cs);
-  Cf[e] = (r < k && j < d) ? static_cast<float>(Cc[static_cast<size_t>(r) * d + j] - o[j]) : 0.f;
+  Cf[e] = (r < k && j < d) ? static_cast<float>((Cc[static_cast<size_t>(r) * d + j] - o[j]) * sc) : 0.f;
 }
 
 // per-slice column sums and sums of squares (fixed order: 8 row lanes x 32 column lanes, lanes folded in order); any
@@ -420,6 +438,7 @@ struct KMeansRun {
   float* Cf = nullptr;
   int *beg = nullptr, *end = nullptr;
   int slices = 1, rows_per_slice = 1;
+  Frame fr{};                     // o, the prescale and the range flag (ints + 5), set by origin()
 
   int sync() { SGP_CUDA(c, cudaStreamSynchronize(s)); return SGP_OK; }
 
@@ -459,17 +478,18 @@ struct KMeansRun {
 
   int centre_images(const double* C, int kk, float* F) {
     const int rows = rows_pad(kk), cs = cstride(d);
-    kmeans_centre_f32_kernel<<<blocks(static_cast<long long>(rows) * cs, 256), 256, 0, s>>>(C, kk, d, o, F, rows, cs);
+    kmeans_centre_f32_kernel<<<blocks(static_cast<long long>(rows) * cs, 256), 256, 0, s>>>(C, kk, d, o, fr.sc, F, rows,
+                                                                                            cs);
     SGP_CUDA(c, cudaGetLastError());
     c->launches += 1;
     return SGP_OK;
   }
 
-  // stable sort of (label, index), cluster bounds, fixed-order (weighted) means
+  // stable sort of (label, idx) -- idx = 0..m-1 -- cluster bounds, fixed-order (weighted) means
   template <typename P>
-  int update(const P* pts, int m, const int* lab, const double* w, int kk, double tol2, int* notconv, void* tmp,
-             size_t tmp_bytes, int* kout, int* vout) {
-    SGP_CUDA(c, cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, lab, kout, iota, vout, m, 0, label_bits(kk), s));
+  int update(const P* pts, int m, const int* lab, const int* idx, const double* w, int kk, double tol2, int* notconv,
+             void* tmp, size_t tmp_bytes, int* kout, int* vout) {
+    SGP_CUDA(c, cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, lab, kout, idx, vout, m, 0, label_bits(kk), s));
     SGP_CUDA(c, cudaMemsetAsync(beg, 0, static_cast<size_t>(kk) * sizeof(int), s));
     SGP_CUDA(c, cudaMemsetAsync(end, 0, static_cast<size_t>(kk) * sizeof(int), s));
     kmeans_bounds_kernel<<<blocks(m, 256), 256, 0, s>>>(kout, m, beg, end);
@@ -592,16 +612,30 @@ struct KMeansRun {
     rc = grows({0}, x0.data());
     if (rc != SGP_OK) return rc;
     const double nt = static_cast<double>(N);
+    double sdmax = 0.0;
+    bool finite = true;
     for (int j = 0; j < d; ++j) {
       const double a = ab[j], b = ab[d + j];
       const double mean = a / nt, sd = std::sqrt(std::max(b / nt - mean * mean, 0.0));
       if (sd > 0.0 && std::isfinite(sd)) {
         const double q = std::ldexp(1.0, std::ilogb(sd));
         oh[j] = std::nearbyint(mean / q) * q;
+        sdmax = std::max(sdmax, sd);
       } else {
+        finite = finite && std::isfinite(sd);
         oh[j] = x0[j];
       }
     }
+    // the prescale 2^s: none while the largest sd is within [2^-16, 2^16], else the s that brings it into [1, 2), so that
+    // the fp32 squares neither underflow nor overflow at the data's scale.  |s| <= 511 keeps 2^s and 2^-2s normal fp64
+    // numbers; beyond it (or where a column's sum of squares overflows fp64) the data are refused rather than collapsed.
+    // Every rank derives s from the same summed statistics, so every rank refuses together.
+    int sexp = 0;
+    if (sdmax > 0.0 && (sdmax < 0x1.0p-16 || sdmax > 0x1.0p16)) sexp = -std::ilogb(sdmax);
+    if (!finite || sexp < -511 || sexp > 511)
+      return fail(c, SGP_E_RANGE, "sgp_kmeans: the data's spread is outside the range of the fp32 distances (largest "
+                                  "column standard deviation outside [2^-511, 2^512), or sums of squares beyond fp64)");
+    fr = Frame{o, std::ldexp(1.0, sexp), std::ldexp(1.0, -2 * sexp), ints + 5};
     SGP_CUDA(c, cudaMemcpyAsync(o, oh.data(), static_cast<size_t>(d) * 8, cudaMemcpyHostToDevice, s));
     return SGP_OK;
   }
@@ -675,7 +709,7 @@ struct KMeansRun {
         rc = centre_images(R, m, F);
         if (rc != SGP_OK) return rc;
         if (n > 0) {
-          SGP_CUDA(c, launch_assign<T>(dX, n, d, o, F, m, nullptr, cost, 1, nullptr, s));
+          SGP_CUDA(c, launch_assign<T>(dX, n, d, fr, F, m, nullptr, cost, 1, nullptr, s));
           c->launches += 1;
         }
       }
@@ -728,12 +762,13 @@ struct KMeansRun {
     const size_t Cz = static_cast<size_t>(C);
     double *dcand = nullptr, *w = nullptr, *cdist = nullptr, *ccost = nullptr;
     float* CF = nullptr;
-    int *cnt = nullptr, *clab = nullptr, *ckeys = nullptr, *cvals = nullptr;
+    int *cnt = nullptr, *clab = nullptr, *ckeys = nullptr, *cvals = nullptr, *cidx = nullptr;
     void* ctmp = nullptr;
     auto carve = [&](Carve& cv) {
       dcand = cv.take<double>(Cz * d); w = cv.take<double>(Cz); cdist = cv.take<double>(Cz); ccost = cv.take<double>(Cz);
       CF = cv.take<float>(static_cast<size_t>(rows_pad(C)) * cstride(d));
       cnt = cv.take<int>(Cz); clab = cv.take<int>(Cz); ckeys = cv.take<int>(Cz); cvals = cv.take<int>(Cz);
+      cidx = cv.take<int>(Cz);      // the candidates' own 0..C-1 (a shard may hold fewer than C points)
       ctmp = cv.take<char>(tsort);
     };
     Carve probe{nullptr};
@@ -748,7 +783,7 @@ struct KMeansRun {
     // weights: how many points have each candidate as their nearest
     SGP_CUDA(c, cudaMemsetAsync(cnt, 0, Cz * sizeof(int), s));
     if (n > 0) {
-      SGP_CUDA(c, launch_assign<T>(dX, n, d, o, CF, C, label, dist, 0, nullptr, s));
+      SGP_CUDA(c, launch_assign<T>(dX, n, d, fr, CF, C, label, dist, 0, nullptr, s));
       kmeans_count_kernel<<<blocks(n, 256), 256, 0, s>>>(label, n, cnt);
     }
     if (sharded) {                            // int64 counts summed over the ranks
@@ -766,15 +801,16 @@ struct KMeansRun {
     }
     kmeans_pp_kernel<<<1, kPPThreads, 0, s>>>(dcand, C, d, w, k, seed, ccost, Cc);
     kmeans_iota_kernel<<<blocks(C, 256), 256, 0, s>>>(clab, C, -1);
+    kmeans_iota_kernel<<<blocks(C, 256), 256, 0, s>>>(cidx, C, 0);
     SGP_CUDA(c, cudaGetLastError());
     SGP_CUDA(c, cudaMemsetAsync(ints + 2, 0, 2 * sizeof(int), s));   // [2] changed, [3] empty-cluster draw counter
-    c->launches += 5;
+    c->launches += 6;
     for (int it = 0; it < 30; ++it) {
       rc = centre_images(Cc, k, Cf);
       if (rc != SGP_OK) return rc;
       SGP_CUDA(c, cudaMemsetAsync(ints + 2, 0, sizeof(int), s));
-      SGP_CUDA(c, launch_assign<double>(dcand, C, d, o, Cf, k, clab, cdist, 0, ints + 2, s));
-      rc = update<double>(dcand, C, clab, w, k, 0.0, nullptr, ctmp, tsort, ckeys, cvals);
+      SGP_CUDA(c, launch_assign<double>(dcand, C, d, fr, Cf, k, clab, cdist, 0, ints + 2, s));
+      rc = update<double>(dcand, C, clab, cidx, w, k, 0.0, nullptr, ctmp, tsort, ckeys, cvals);
       if (rc != SGP_OK) return rc;
       kmeans_local_empty_kernel<<<1, 1, 0, s>>>(wsum, k, dcand, C, d, Cc, seed, ints + 3);
       SGP_CUDA(c, cudaGetLastError());
@@ -812,13 +848,13 @@ struct KMeansRun {
     bool converged = false;
     do {
       if (n > 0) {
-        SGP_CUDA(c, launch_assign<T>(dX, n, d, o, Cf, kk, label, dist, 0, nullptr, s));
+        SGP_CUDA(c, launch_assign<T>(dX, n, d, fr, Cf, kk, label, dist, 0, nullptr, s));
         c->launches += 1;
       }
       if (max_iter == 0) break;
       SGP_CUDA(c, cudaMemsetAsync(ints + 4, 0, sizeof(int), s));
       rc = sharded ? update_sharded(kk, tol * tol, ints + 4)
-                   : update<T>(dX, n, label, nullptr, kk, tol * tol, ints + 4, cub_tmp, cub_bytes, keys, vals);
+                   : update<T>(dX, n, label, iota, nullptr, kk, tol * tol, ints + 4, cub_tmp, cub_bytes, keys, vals);
       if (rc == SGP_OK) rc = centre_images(Cc, kk, Cf);
       if (rc != SGP_OK) return rc;
       int notconv = 0;
@@ -829,6 +865,17 @@ struct KMeansRun {
     } while (iteration < max_iter && !converged);
     const double cost_total = global_sum(dist, n, rc);
     if (rc != SGP_OK) return rc;
+    // a nearest-centre distance beyond the fp32 range even after the prescale (a centre or point far outside the data's
+    // spread): refused on every rank together, rather than returning a run whose draws and costs were inf
+    int fl = 0;
+    SGP_CUDA(c, cudaMemcpyAsync(&fl, ints + 5, sizeof(int), cudaMemcpyDeviceToHost, s));
+    SGP_CUDA(c, cudaStreamSynchronize(s));
+    double far = fl ? 1.0 : 0.0;
+    rc = allsum(&far, 1, ncclDouble);
+    if (rc != SGP_OK) return rc;
+    if (far != 0.0)
+      return fail(c, SGP_E_RANGE, "sgp_kmeans: a squared distance to the nearest centre is beyond the fp32 range after the "
+                                  "data's power-of-two prescale");
     SGP_CUDA(c, cudaMemcpyAsync(centers_out, Cc, static_cast<size_t>(kk) * d * 8, cudaMemcpyDeviceToHost, s));
     if (labels_out && n > 0) SGP_CUDA(c, cudaMemcpyAsync(labels_out, label, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, s));
     SGP_CUDA(c, cudaStreamSynchronize(s));

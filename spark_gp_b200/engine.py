@@ -32,7 +32,8 @@ class SgpError(RuntimeError):
 
 
 class OperandRangeError(SgpError):
-    """SGP_E_RANGE: the int8 path cannot represent these coordinates; rerun in SGP_PREC_F64."""
+    """SGP_E_RANGE: the int8 path cannot represent these coordinates (rerun in SGP_PREC_F64), or a k-means distance to
+    the nearest centre is beyond the fp32 range after the data's prescale."""
 
 
 def is_cuda_tensor(x) -> bool:

@@ -256,6 +256,24 @@ def kmeans_world(rank, world, group, integer, on_cuda, sizes=None, k=20):
         solo.close()
 
 
+def kmeans_model_world(rank, world, group, sizes):
+    """sgp_kmeans_sharded on real-valued data, this rank's block of `sizes` rows (host fp64)."""
+    import torch
+    import spark_gp_b200 as sg
+    from oracle import kmeans_cases as kc
+    from spark_gp_b200.distributed import attach_communicator
+    X = kc._lattice_mixture(5000, 5, 9)
+    eng = sg.ProjectedProcessEngine(rank)
+    try:
+        attach_communicator(eng, group, torch.device("cuda", rank))
+        cuts = [0] + [int(c) for c in np.cumsum(sizes)]
+        c, lab, it, cost = eng.kmeans_sharded(X[cuts[rank]:cuts[rank + 1]], cuts[rank], len(X), 20, max_iter=20, seed=5,
+                                              d=X.shape[1])
+        return dict(c=c, lab=lab, it=it, cost=cost)
+    finally:
+        eng.close()
+
+
 # ---------------- cases ------------------------------------------------------------------------------------------------
 def same_model(a, b, keys=("theta", "Z", "mv", "mm", "mean", "var")):
     for k in keys:
@@ -368,3 +386,23 @@ def test_multi_rank_sharded_kmeans_on_integer_blobs_equals_kmeans(world, uneven)
         o = got[r]
         assert np.array_equal(bits(o["c"]), bits(o["c0"])) and o["it"] == o["it0"] and np.array_equal(bits(o["cost"]), bits(o["cost0"]))
         assert np.array_equal(o["lab"], o["lab0"])
+
+
+@need_two
+@pytest.mark.parametrize("split", ["rank0_empty", "rank0_seven_rows", "even"])
+def test_two_rank_sharded_kmeans_on_real_data_equals_the_two_rank_model(split):
+    """Real-valued data at two ranks, where every all-reduced value is one addition: the outputs are the model's two-rank
+    form bit for bit (each rank's fixed-order sums added), including a rank with no rows and one with fewer rows than
+    candidates."""
+    from oracle import kmeans_cases as kc
+    from oracle import kmeans_model as km
+    sizes = {"rank0_empty": [0, 5000], "rank0_seven_rows": [7, 4993], "even": [2500, 2500]}[split]
+    X = kc._lattice_mixture(5000, 5, 9)
+    (Cm, labm, itm, costm), info = km.run(X, 20, max_iter=20, seed=5, sizes=sizes)
+    assert info["C"] > 20 and (split == "even" or info["C"] > sizes[0])
+    got = run("kmeans_model_world", 2, sizes=sizes)
+    cuts = [0] + [int(c) for c in np.cumsum(sizes)]
+    for r in range(2):
+        o = got[r]
+        assert np.array_equal(bits(o["c"]), bits(Cm)) and o["it"] == itm and np.array_equal(bits(o["cost"]), bits(costm))
+        assert np.array_equal(o["lab"], labm[cuts[r]:cuts[r + 1]])
