@@ -88,10 +88,9 @@ class GaussianProcessClassifier(GaussianProcessParams):
         X, y = fit_data(X, y, self._device, "GaussianProcessClassifier.fit")
         assert_labels_are_01(y)
         eng = ProjectedProcessEngine.acquire(self._device)
-        objective = lambda batch: [eng.laplace_nll_any_size(self.getKernel().setHyperparameters(t), self._tol)
-                                   for _, t in batch]
         (theta,), (f,), fit = laplace_fit(
-            self, eng, X, y, objective, N.SGP_MODES_BINARY, lambda _: 0, [self.getKernel().getHyperparameters()],
+            self, eng, X, y, binary_objective(self, eng), N.SGP_MODES_BINARY, lambda _: 0,
+            [self.getKernel().getHyperparameters()],
             None if hyperparameters is None else [np.asarray(hyperparameters, dtype=np.float64)])
         if fit["slots"] is not None:
             self.last_objective = dict(fit["slots"][0], launches=fit["launches"])
@@ -115,6 +114,23 @@ def assert_labels_are_01(y):
     """assertLabelsAre01 (GPCls:68-72), on a host array or on the device (only the verdict crosses PCIe)."""
     if not bool(((y == 0.0) | (y == 1.0)).all()):
         raise RuntimeError("Only 0 and 1 labels are supported.")
+
+
+def binary_objective(gp, eng):
+    """The binary classifier's objective for `laplace_optimise`: `laplace_nll_any_size` of each listed slot on eng."""
+    return lambda batch: [eng.laplace_nll_any_size(gp.getKernel().setHyperparameters(t), gp._tol) for _, t in batch]
+
+
+def classes_objective(gp, eng, n_classes: int):
+    """One-vs-rest's objective for `laplace_optimise` (slot c: class c): every listed class in one
+    `laplace_nll_classes_any_size` launch on eng."""
+    kernel_at = lambda t: gp.getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
+
+    def objective(batch):
+        vals, grads = eng.laplace_nll_classes_any_size(n_classes, [c for c, _ in batch], [kernel_at(t) for _, t in batch],
+                                                       gp._tol)
+        return [(float(v), g) for v, g in zip(vals, grads)]
+    return objective
 
 
 def laplace_fit(gp, eng, X, y, objective, store, index, x0s, thetas=None):
@@ -275,10 +291,16 @@ class OneVsRest:
         return new
 
     def fit(self, X, y, hyperparameters=None) -> OneVsRestModel:
-        """hyperparameters: None (optimise every class, as the binary fit does) or numClasses x n_hypers fixed values."""
+        """hyperparameters: None (optimise every class, as the binary fit does) or numClasses x n_hypers fixed values.
+        When the classifier has a process group, (X, y) is this rank's shard (possibly empty, 0 x d) and every rank
+        returns the model of the concatenation of the shards in rank order, the same bits on every rank; numClasses is
+        the concatenation's, and `last_latent[c]` holds class c's modes at the rows of this rank's experts, in global
+        row order (`spark_gp_b200.distributed`)."""
         gp = self._classifier
         if not isinstance(gp, GaussianProcessClassifier):
             raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
+        if gp._process_group is not None:
+            return self._fit_group(gp, X, y, hyperparameters)
         X, y = fit_data(X, y, gp._device, "OneVsRest.fit")
         y, C = one_vs_rest_labels(y)
         eng = ProjectedProcessEngine.acquire(gp._device)
@@ -288,19 +310,12 @@ class OneVsRest:
             eng.release()
 
     def _fit(self, gp, eng, X, y, C, hyperparameters):
-        kernel_at = lambda t: gp.getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
-
-        def objective(batch):
-            vals, grads = eng.laplace_nll_classes_any_size(C, [c for c, _ in batch], [kernel_at(t) for _, t in batch],
-                                                           gp._tol)
-            return [(float(v), g) for v, g in zip(vals, grads)]
-
         x0 = gp.getKernel().getHyperparameters()
         given = None if hyperparameters is None else np.array(hyperparameters, dtype=np.float64).reshape(C, len(x0))
-        thetas, latent, fit = laplace_fit(gp, eng, X, y, objective, N.SGP_MODES_CLASS, lambda c: c, [x0] * C, given)
+        thetas, latent, fit = laplace_fit(gp, eng, X, y, classes_objective(gp, eng, C), N.SGP_MODES_CLASS, lambda c: c,
+                                          [x0] * C, given)
         thetas = np.array(thetas).reshape(C, len(x0))
-        if fit["slots"] is not None:
-            self.last_objective = dict(classes=fit["slots"], rounds=fit["rounds"], launches=fit["launches"])
+        self._record(fit)
         models = []
         for c in range(C):
             # produceModel in the fit's context
@@ -313,3 +328,22 @@ class OneVsRest:
                 GaussianProjectedProcessRawPredictor(model_eng, mv, mm, kernel, active_set), thetas[c]))
         self.last_latent = latent
         return OneVsRestModel(models, thetas)
+
+    def _fit_group(self, gp, X, y, hyperparameters):
+        from . import distributed
+        slots, fit = distributed.group_fit(gp, X, y, hyperparameters, "classes")
+        self._record(fit)
+        thetas = np.array([s[2] for s in slots]).reshape(len(slots), -1)
+        latent = [s[7] for s in slots]
+        if is_cuda_tensor(latent[0]):
+            import torch
+            self.last_latent = torch.stack(latent)
+        else:
+            self.last_latent = np.stack(latent)
+        models = [GaussianProcessClassificationModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, Z), theta)
+                  for (eng, kernel, _, Z, mv, mm, _, _), theta in zip(slots, thetas)]
+        return OneVsRestModel(models, thetas)
+
+    def _record(self, fit):
+        if fit["slots"] is not None:
+            self.last_objective = dict(classes=fit["slots"], rounds=fit["rounds"], launches=fit["launches"])

@@ -1,6 +1,6 @@
-"""Data-parallel `fit` of `GaussianProcessRegression` and the binary `GaussianProcessClassifier` over a torch.distributed
-process group: one process per GPU, each passing its own shard, every rank returning the model of the concatenation of
-the shards in rank order (DESIGN.md section 5).
+"""Data-parallel `fit` of `GaussianProcessRegression`, the binary `GaussianProcessClassifier` and `OneVsRest` over a
+torch.distributed process group: one process per GPU, each passing its own shard, every rank returning the model of the
+concatenation of the shards in rank order (DESIGN.md section 5).
 
 The reference's cluster steps, one by one:
   * `groupForExperts` (GPC:26-31): E = round(N / datasetSizeForExpert) over all N rows, expert e holds the global rows
@@ -8,11 +8,12 @@ The reference's cluster steps, one by one:
     all-to-all, and the rows a rank receives, in global row order, are grouped on its device row i -> expert i % E_r
     (`sgp_experts_upload_strided_device`), which makes each expert the single-GPU upload's, row for row.
   * `optimizeHypers` (GPC:66-92): every rank runs the same L-BFGS-B on the reducing objective entries
-    (`sgp_bcm_nll`, `sgp_laplace_nll_any_size`), which all-reduce [value; gradient] and the status words, so every rank
-    sees the same bits and takes the same steps.  The classifier's latent modes stay with their expert's owner.
+    (`sgp_bcm_nll`, `sgp_laplace_nll_any_size`, and for one-vs-rest `sgp_laplace_nll_classes_any_size` over the classes
+    in lock step), which all-reduce [value; gradient] and the status words, so every rank sees the same bits and takes
+    the same steps.  The classifiers' latent modes stay with their expert's owner.
   * `getMatrixKmnKnmAndVectorKmny` (PGPH:20-36): each rank accumulates its rows -- the regression its own shard, the
-    classifier its experts' rows with the modes as labels -- and `sgp_stats_finish` all-reduces G and b and the int8
-    status, so AUTO's fall-back to fp64 is taken on every rank together.
+    classifiers their experts' rows with each slot's modes as labels -- and `sgp_stats_finish` all-reduces G and b and
+    the int8 status, so AUTO's fall-back to fp64 is taken on every rank together.
 
 A rank that returns before a collective leaves its peers blocked in it.  So before the first collective every rank
 states the refusals it can compute (its data, the global sizes), the ranks exchange them, and if any rank would refuse,
@@ -87,16 +88,16 @@ def _dist():
 
 
 def group_refusal(plan: ShardPlan, infos, classifier: bool, experts: bool):
-    """The refusal every rank takes, from every rank's (n, d, dtype, local refusal) and the plan, or None: the first
-    rank's own refusal, then a disagreement of the ranks' shapes or dtypes, then the expert grouping's limits (only
-    when the fit groups experts).  Returns (exception class name, message)."""
-    for r, (_, _, _, err) in enumerate(infos):
-        if err is not None:
-            return err[0], "rank %d: %s" % (r, err[1])
-    ds = sorted({d for n, d, _, _ in infos if n > 0} or {infos[0][1]})
+    """The refusal every rank takes, from every rank's agreement entry (n, d, dtype, local refusal[, largest label]) and
+    the plan, or None: the first rank's own refusal, then a disagreement of the ranks' shapes or dtypes, then the expert
+    grouping's limits (only when the fit groups experts).  Returns (exception class name, message)."""
+    for r, info in enumerate(infos):
+        if info[3] is not None:
+            return info[3][0], "rank %d: %s" % (r, info[3][1])
+    ds = sorted({i[1] for i in infos if i[0] > 0} or {infos[0][1]})
     if len(ds) > 1:
         return "ValueError", "the ranks' shards have different numbers of features: %s" % ds
-    dtypes = sorted({t for n, _, t, _ in infos if n > 0})
+    dtypes = sorted({i[2] for i in infos if i[0] > 0})
     if len(dtypes) > 1:
         return "ValueError", "the ranks' shards have different dtypes: %s" % ", ".join(dtypes)
     if plan.N == 0:
@@ -115,19 +116,26 @@ def group_refusal(plan: ShardPlan, infos, classifier: bool, experts: bool):
     return None
 
 
-def agree(group, n: int, d: int, dtype: str, err, dataset_size_for_expert: int, classifier: bool, experts: bool):
-    """The agreement step, the fit's first collective: every rank's (n, d, dtype, refusal) to every rank.  Raises the
-    agreed refusal on every rank; else returns (the plan, the agreed dtype, the agreed number of features): those of the
-    non-empty shards, which an empty shard takes whatever its own shape."""
+def num_classes(infos):
+    """One-vs-rest's numClasses of the concatenation from every rank's agreement entry: one more than the largest label
+    of any rank (an empty shard, or a fit without class labels, sends -1)."""
+    return max(i[4] for i in infos) + 1
+
+
+def agree(group, n: int, d: int, dtype: str, err, dataset_size_for_expert: int, classifier: bool, experts: bool,
+          top: int = -1):
+    """The agreement step, the fit's first collective: every rank's (n, d, dtype, refusal, largest label top) to every
+    rank.  Raises the agreed refusal on every rank; else returns (the plan, the agreed dtype, the agreed number of
+    features: those of the non-empty shards, which an empty shard takes whatever its own shape, `num_classes`)."""
     dist = _dist()
     infos = [None] * dist.get_world_size(group)
-    dist.all_gather_object(infos, (int(n), int(d), str(dtype), err), group=group)
+    dist.all_gather_object(infos, (int(n), int(d), str(dtype), err, int(top)), group=group)
     plan = ShardPlan([i[0] for i in infos], dist.get_rank(group), dataset_size_for_expert)
     verdict = group_refusal(plan, infos, classifier, experts)
     if verdict is not None:
         raise _EXCEPTIONS.get(verdict[0], RuntimeError)(verdict[1])
     first = next(i for i in infos if i[0] > 0)
-    return plan, first[2], first[1]
+    return plan, first[2], first[1], num_classes(infos)
 
 
 def exchange(plan: ShardPlan, X, y, group):
@@ -228,11 +236,12 @@ def attach_communicator(eng, group, device):
     eng.comm_init(obj[0], dist.get_rank(group), dist.get_world_size(group))
 
 
-def _local_data(X, y, device: int, classifier: bool, what: str):
-    """The shard as the single-GPU fit reads it (regression: float32 X kept, others float64; classifier: float64), with
-    the labels checked for the classifier."""
-    if classifier:
-        from .classification import assert_labels_are_01, fit_data
+def _local_data(X, y, device: int, kind: str, what: str):
+    """The shard as the single-GPU fit reads it (regression: float32 X kept, others float64; classifiers: float64), with
+    the labels checked for the classifiers.  Returns (X, y, the largest label: one-vs-rest's, -1 for an empty shard and
+    for the other fits)."""
+    if kind != "regression":
+        from .classification import fit_data
         X, y = fit_data(X, y, device, what)
     elif is_cuda_tensor(X):
         X, y = device_fit_data(X, y, device, what)
@@ -245,9 +254,15 @@ def _local_data(X, y, device: int, classifier: bool, what: str):
         y = np.asarray(y, dtype=np.float64)
     if X.ndim != 2 or y.ndim != 1 or len(y) != len(X):
         raise ValueError("%s: X must be n x d and y n entries" % what)
-    if classifier:
+    top = -1
+    if kind == "binary":
+        from .classification import assert_labels_are_01
         assert_labels_are_01(y)
-    return X, y
+    elif kind == "classes" and len(y):
+        from .classification import one_vs_rest_labels
+        y, top = one_vs_rest_labels(y)
+        top -= 1
+    return X, y, top
 
 
 def _tensor(a, device, dtype=None):
@@ -259,77 +274,72 @@ def _tensor(a, device, dtype=None):
 
 def fit(gp, X, y, hyperparameters, classifier: bool, engine_factory=ProjectedProcessEngine):
     """The data-parallel fit of gp (a GaussianProcessRegression or binary GaussianProcessClassifier with a process
-    group) on this rank's shard.  The fit runs on the group's context with a communicator (`comm_engine`); the model gets
-    a context of its own holding the active set and magic pair.  Returns (model's engine, kernel, theta, active set, magic
-    vector, magic matrix, (G, b), latent modes of this rank's expert rows or None).  Fits over one group must not run
-    concurrently."""
+    group) on this rank's shard (`group_fit`).  Returns (model's engine, kernel, theta, active set, magic vector, magic
+    matrix, (G, b), latent modes of this rank's expert rows or None)."""
+    models, record = group_fit(gp, X, y, hyperparameters, "binary" if classifier else "regression", engine_factory)
+    if record is not None and record["slots"] is not None:
+        gp.last_objective = dict(record["slots"][0], launches=record["launches"])
+    return models[0]
+
+
+def group_fit(gp, X, y, hyperparameters, kind: str, engine_factory=ProjectedProcessEngine):
+    """The data-parallel fit over gp's process group on this rank's shard.  kind: "regression", "binary" (gp a binary
+    GaussianProcessClassifier) or "classes" (one-vs-rest over gp: y holds class indices, numClasses agreed by the ranks,
+    and hyperparameters, if given, numClasses x n_hypers).  The fit runs on the group's context with a communicator
+    (`comm_engine`); each model gets a context of its own holding its active set and magic pair.  Returns (per slot --
+    the one model, or one per class -- (model's engine, kernel, theta, active set, magic vector, magic matrix, (G, b),
+    latent modes of this rank's expert rows or None), the Laplace fit record of `laplace_optimise` or None for the
+    regression).  Fits over one group must not run concurrently."""
     import contextlib
 
     import torch
     dist = _dist()
     group = gp._process_group
-    what = "%s.fit" % type(gp).__name__
+    what = "OneVsRest.fit" if kind == "classes" else "%s.fit" % type(gp).__name__
+    classifier = kind != "regression"
     check_provider(gp._activeSetProvider)
     nccl = dist.get_backend(group) == "nccl"
     device = torch.device("cuda", gp._device) if nccl else torch.device("cpu")
     with torch.cuda.device(gp._device) if nccl else contextlib.nullcontext():
         experts = classifier or (hyperparameters is None and gp._maxIter > 0)
-        err, n, d, dtype = None, 0, -1, ""
+        err, n, d, dtype, top = None, 0, -1, "", -1
         try:
-            X, y = _local_data(X, y, gp._device, classifier, what)
+            X, y, top = _local_data(X, y, gp._device, kind, what)
             n, d, dtype = len(X), X.shape[1], str(X.dtype).replace("torch.", "")
         except (ValueError, TypeError, RuntimeError) as e:
             err = (type(e).__name__, str(e))
-        plan, dtype, d = agree(group, n, d, dtype, err, gp._datasetSizeForExpert, classifier, experts)
+        plan, dtype, d, n_classes = agree(group, n, d, dtype, err, gp._datasetSizeForExpert, classifier, experts, top)
         if len(X) == 0:                                     # an empty shard takes the agreed dtype and width
             X = np.empty((0, d), dtype=np.float32 if dtype == "float32" else np.float64)
             y = np.empty(0)
         key, eng = comm_engine(group, gp._device, device, engine_factory)
         try:
-            out = _fit(gp, plan, eng, X, y, hyperparameters, classifier, experts, dtype, group, device)
+            slots, record = _fit(gp, plan, eng, X, y, hyperparameters, kind, n_classes, dtype, group, device)
         except BaseException:
             # a failure after a collective may leave the ranks out of step: the communicator is not reused
             _COMM_ENGINES.pop(key, None)
             eng.close()
             raise
-        kernel, theta, Z, mv, mm = out[:5]
-        model_eng = engine_factory(gp._device)
-        model_eng.begin(kernel, Z)
-        model_eng.set_magic(mv, mm)
-        return (model_eng,) + out
+        models = []
+        for kernel, theta, Z, mv, mm, stats, f in slots:
+            model_eng = engine_factory(gp._device)
+            model_eng.begin(kernel, Z)
+            model_eng.set_magic(mv, mm)
+            models.append((model_eng, kernel, theta, Z, mv, mm, stats, f))
+        return models, record
 
 
-def _fit(gp, plan, eng, X, y, hyperparameters, classifier, experts, dtype, group, device):
+def _fit(gp, plan, eng, X, y, hyperparameters, kind, n_classes, dtype, group, device):
     import torch
     from .hyperopt import lbfgsb_bounds, optimise_slots
     eng.set_precision(N.SGP_PREC_AUTO)                      # as on a freshly acquired context
     k0 = gp.getKernel()
-    theta, Xe, f = None, None, None
-    if experts:
-        Xe, ye = exchange(plan, _tensor(X, device, getattr(torch, dtype)), _tensor(y, device, torch.float64), group)
-        eng.experts_upload_strided(Xe, ye, plan.local_experts)
-    if classifier:
-        from .classification import laplace_optimise
-        objective = lambda batch: [eng.laplace_nll_any_size(gp.getKernel().setHyperparameters(t), gp._tol)
-                                   for _, t in batch]
-        (theta,), fit = laplace_optimise(gp, eng, objective, [k0.getHyperparameters()],
-                                         None if hyperparameters is None else
-                                         [np.asarray(hyperparameters, dtype=np.float64)])
-        if fit["slots"] is not None:
-            gp.last_objective = dict(fit["slots"][0], launches=fit["launches"])
-        n_e = len(Xe)
-        if is_cuda_tensor(X):                               # the modes stay on the device, ungrouped into row order
-            f = eng.experts_modes_rows(N.SGP_MODES_BINARY, 0, n_e)
-        else:
-            f = np.empty(n_e)
-            f[plan.local_order()] = eng.experts_modes(N.SGP_MODES_BINARY, 0, n_e)
-            Xe = Xe.cpu().numpy()
-        stats_X, stats_y = Xe, f
-        eng.set_precision(N.SGP_PREC_AUTO)
-    else:
+    if kind == "regression":
         if hyperparameters is not None:
             theta = np.asarray(hyperparameters, dtype=np.float64)
         elif gp._maxIter > 0:
+            Xe, ye = exchange(plan, _tensor(X, device, getattr(torch, dtype)), _tensor(y, device, torch.float64), group)
+            eng.experts_upload_strided(Xe, ye, plan.local_experts)
             launches0 = eng.launch_count()
             evaluate = lambda batch: [eng.bcm_nll(gp.getKernel().setHyperparameters(t)) for _, t in batch]
             (theta,), records, _ = optimise_slots(evaluate, [k0.getHyperparameters()], lbfgsb_bounds(k0), gp._maxIter,
@@ -338,8 +348,39 @@ def _fit(gp, plan, eng, X, y, hyperparameters, classifier, experts, dtype, group
                 gp.last_objective = dict(records[0], n_experts=plan.E, launches=eng.launch_count() - launches0)
         else:
             theta = k0.getHyperparameters()
-        theta = np.asarray(theta, dtype=np.float64)
-        stats_X, stats_y = X, y
+        return [_model(gp, plan, eng, X, np.asarray(theta, dtype=np.float64), X, y, None, group, device)], None
+    # the Laplace fit of one slot (the binary classifier) or of every class (one-vs-rest), as `laplace_fit` on one GPU
+    from .classification import binary_objective, classes_objective, laplace_optimise
+    x0 = k0.getHyperparameters()
+    if kind == "binary":
+        store, objective, x0s = N.SGP_MODES_BINARY, binary_objective(gp, eng), [x0]
+        given = None if hyperparameters is None else [np.asarray(hyperparameters, dtype=np.float64)]
+    else:
+        store, objective, x0s = N.SGP_MODES_CLASS, classes_objective(gp, eng, n_classes), [x0] * n_classes
+        given = None if hyperparameters is None else \
+            np.array(hyperparameters, dtype=np.float64).reshape(n_classes, len(x0))
+    Xe, ye = exchange(plan, _tensor(X, device, getattr(torch, dtype)), _tensor(y, device, torch.float64), group)
+    eng.experts_upload_strided(Xe, ye, plan.local_experts)
+    thetas, record = laplace_optimise(gp, eng, objective, x0s, given)
+    n_e = len(Xe)
+    if not is_cuda_tensor(X):
+        Xe = Xe.cpu().numpy()
+    slots = []
+    for i, theta in enumerate(thetas):
+        # every model starts from the default precision, as `_produce_model`
+        eng.set_precision(N.SGP_PREC_AUTO)
+        if is_cuda_tensor(X):                               # the modes stay on the device, ungrouped into row order
+            f = eng.experts_modes_rows(store, i, n_e)
+        else:
+            f = np.empty(n_e)
+            f[plan.local_order()] = eng.experts_modes(store, i, n_e)
+        slots.append(_model(gp, plan, eng, X, theta, Xe, f, f, group, device))
+    return slots, record
+
+
+def _model(gp, plan, eng, X, theta, stats_X, stats_y, f, group, device):
+    """One slot's model at theta: the active set of the concatenation, the statistics of (stats_X, stats_y) all-reduced
+    over the group, and the tail.  Returns (kernel, theta, active set, magic vector, magic matrix, (G, b), f)."""
     Z = active_set(gp, plan, eng, X, theta, group, device)
     kernel = gp.getKernel().setHyperparameters(theta)
     G, b = eng.statistics(kernel, Z, stats_X, stats_y, getattr(gp, "_shard_points", 1 << 22))
