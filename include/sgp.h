@@ -69,7 +69,8 @@ typedef struct {
 
 /* Arithmetic modes of the statistics kernel.  All modes accumulate G and b in fp64. */
 enum {
-  SGP_PREC_F64 = 0,        /* fp32-accurate kernel elements (direct-form distances, full-precision expf), fp64 DMMA Gram.
+  SGP_PREC_F64 = 0,        /* fp32 kernel elements (direct-form distances in fp32, exp as ex2.approx within 2 ulp;
+                              elements below 2^-126 C flushed to 0; the term scale C applied in fp64), fp64 DMMA Gram.
                               Points and active set are centred in fp64 before the fp32 rounding (on the active-set
                               mean, rounded to a whole multiple of its standard deviation), so the error does not grow
                               with the data's distance from the origin: G, b <= 1e-6 and mean / variance <= 1e-5 also

@@ -11,8 +11,8 @@
 // triangle of G and one contiguous slice of the shard's points.  Per block of 16 points it
 //   (1) evaluates the two panels P_I[16][128], P_J[16][128] of the cross kernel into shared memory
 //       (direct-form sum_k (x~_k - z~_k)^2 on centred, pre-scaled coordinates x~ = (x - c)*beta with c within half
-//       a standard deviation of the active-set mean, full-precision exp,
-//       fp32 by default / fp64 in strict mode; Eye terms contribute nothing),
+//       a standard deviation of the active-set mean; fp32 with ex2.approx (2 ulp, results below 2^-126 flushed to 0) by
+//       default, fp64 with CUDA's exp in strict mode; the term scale C_t multiplies in fp64; Eye terms contribute nothing),
 //   (2) accumulates  acc += P_I^T P_J  with fp64 tensor-core MMAs (mma.sync m8n8k4 f64), accumulators in
 //       registers for the CTA's whole lifetime, and (diagonal tiles only) b_I += P_I^T y.
 // At the end every CTA stores its tile into its slice's private partial buffer; a second tiny kernel sums
@@ -212,12 +212,12 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
         (void)blk; (void)pbuf;
       };
       auto panel_store = [&](long long blk, double* pbuf, const float2 (&q)[PB]) {
-        const float sc = static_cast<float>(p.scale[0]);
+        const double sc = p.scale[0];                            // applied in fp64: no overflow, no fp32 underflow
         double* dst = pbuf + pan * PB * PS + col;
         const long long pt0 = blk * PB;
 #pragma unroll
         for (int pp = 0; pp < PB; ++pp)
-          dst[pp * PS] = (zvalid && pt0 + pp < p.n) ? static_cast<double>(sc * ElemOps<ET>::ex(q[pp].x + q[pp].y)) : 0.0;
+          dst[pp * PS] = (zvalid && pt0 + pp < p.n) ? static_cast<double>(ElemOps<ET>::ex(q[pp].x + q[pp].y)) * sc : 0.0;
       };
       // ---- prologue: x(blk_lo) -> xs[0]; panel(blk_lo) -> panel[0]; x(blk_lo+1) -> xs[1]
       xs[e0] = fetch_x(blk_lo, e0); xs[e1] = fetch_x(blk_lo, e1);
@@ -330,12 +330,12 @@ __global__ void __launch_bounds__(NT, (TN == 64) ? 2 : 1) kmn_gram_f64_kernel(co
         }
       }
       if (elem_active) {
-        const ET sc = static_cast<ET>(p.scale[term]);
+        const double sc = p.scale[term];                         // the term scale in fp64 after the exponential
 #pragma unroll
         for (int pp = 0; pp < PB; ++pp) {
           ET qq;
           if constexpr (kPacked) qq = q[pp].x + q[pp].y; else qq = q[pp];
-          const double v = (zvalid && pt0 + pp < p.n) ? static_cast<double>(sc * ElemOps<ET>::ex(qq)) : 0.0;
+          const double v = (zvalid && pt0 + pp < p.n) ? static_cast<double>(ElemOps<ET>::ex(qq)) * sc : 0.0;
           dst[pp * PS] = (term == 0) ? v : dst[pp * PS] + v;
         }
       }
