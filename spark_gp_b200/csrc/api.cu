@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstring>
 #include <new>
+#include <numeric>
 #include <utility>
 
 namespace sgp {
@@ -878,15 +879,14 @@ int experts_alloc(Ctx* c, long long E, long long n, int d, int n_max) {
   int rc = ctx_scratch(c, c->ex_X, static_cast<size_t>(n) * d * 8);
   if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_y, static_cast<size_t>(n) * 8);
   if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_off, static_cast<size_t>(E + 1) * 8);
-  if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_f, static_cast<size_t>(n) * 8);
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_f.buf, static_cast<size_t>(n) * 8);
   if (rc != SGP_OK) return rc;
-  ex.X = c->ex_X.as<double>(); ex.y = c->ex_y.as<double>(); ex.off = c->ex_off.as<long long>(); ex.f = c->ex_f.as<double>();
+  ex.X = c->ex_X.as<double>(); ex.y = c->ex_y.as<double>(); ex.off = c->ex_off.as<long long>(); ex.f = c->ex_f.buf.as<double>();
   SGP_CUDA(c, cudaMemsetAsync(ex.f, 0, static_cast<size_t>(n) * 8, c->stream));
   ex.n = n; ex.d = d; ex.n_max = n_max;
   c->ex_grouped = false;
-  c->ex_classes = 0;                                      // one-vs-rest modes restart at zero on their next use
-  c->ex_mode_slots = 0;                                   // so do the param-map slots' modes
-  c->ex_fold_mode_slots = 0;                              // and the fold slots' modes
+  c->ex_f.slots = 1;                                      // the binary objectives' modes: one slot, zero
+  for (ModeStore* m : {&c->ex_fc, &c->ex_fm, &c->ex_ffm}) m->slots = 0;   // the slot stores restart at zero on next use
   c->fold_first.clear();
   c->fold_nmax.clear();
   c->fold_row0.clear();
@@ -930,10 +930,7 @@ namespace {
 // E experts, point i -> expert i % E (after the caller's argument checks)
 int upload_strided(Ctx* c, bool on_device, const void* X, int x_is_f32, const double* y, long long n, int d, long long E) {
   int rc = experts_alloc(c, E, n, d, static_cast<int>(n / E + ((n % E) ? 1 : 0)));
-  if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_set_first, 2 * 8);
   if (rc != SGP_OK) return rc;
-  const long long one_set[2] = {0, E};        // the upload as one set, for sgp_bcm_nll_slots (synchronised below)
-  SGP_CUDA(c, cudaMemcpyAsync(c->ex_set_first.p, one_set, sizeof(one_set), cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, launch_expert_offsets(c->ex.off, n, E, 0, c->stream));
   // host input streams through the double-buffered staging area of the statistics path; either way the gather is on the
   // device, chunk by chunk
@@ -1007,7 +1004,7 @@ int upload_folds(Ctx* c, bool on_device, const void* X, int x_is_f32, const doub
   {                                           // the sets' rows, labels and modes, (n_folds - 1) n (d + 2) doubles
     size_t free_b = 0, total_b = 0;
     SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
-    const size_t held = c->ex_X.cap + c->ex_y.cap + c->ex_f.cap;
+    const size_t held = c->ex_X.cap + c->ex_y.cap + c->ex_f.buf.cap;
     const size_t need = static_cast<size_t>(n_rows) * (static_cast<size_t>(d) + 2) * 8;
     if (need > free_b + held)
       return fail(c, SGP_E_NOMEM, std::string(entry) + ": the training sets need " + std::to_string(need >> 20) +
@@ -1015,11 +1012,9 @@ int upload_folds(Ctx* c, bool on_device, const void* X, int x_is_f32, const doub
   }
   int rc = experts_alloc(c, E, n_rows, d, *std::max_element(nmax.begin(), nmax.end()));
   if (rc == SGP_OK) rc = ctx_scratch(c, c->fold_pos_ws, static_cast<size_t>(n) * 8);
-  if (rc == SGP_OK) rc = ctx_scratch(c, c->ex_set_first, first.size() * 8);
   if (rc != SGP_OK) return rc;
   const long long* dpos = c->fold_pos_ws.as<long long>();
   SGP_CUDA(c, cudaMemcpyAsync(c->fold_pos_ws.p, pos.data(), pos.size() * 8, cudaMemcpyHostToDevice, c->stream));
-  SGP_CUDA(c, cudaMemcpyAsync(c->ex_set_first.p, first.data(), first.size() * 8, cudaMemcpyHostToDevice, c->stream));
   for (int k = 0; k < n_folds; ++k) {
     SGP_CUDA(c, launch_expert_offsets(c->ex.off + first[k], row0[k + 1] - row0[k], first[k + 1] - first[k], row0[k],
                                       c->stream));
@@ -1094,53 +1089,76 @@ int sgp_experts_upload_folds_device(sgp_ctx* h, const void* dX, int32_t x_is_f32
 }
 
 namespace {
-// Device state of one objective evaluation over n_slots hyper-parameter blocks (one per one-vs-rest class; the BCM and
-// binary Laplace objectives use one), in the context's descriptor block.
+// The expert sets an objective call's slots index: set k is the experts first[k] .. first[k+1]-1, the largest of nmax[k]
+// points.  The fold upload's training sets, or the whole upload as the one set {0, E}.
+struct ExpertSets {
+  std::vector<long long> first;    // [n_sets + 1]
+  std::vector<int> nmax;           // [n_sets]
+};
+ExpertSets whole_upload(const Ctx* c) { return {{0, c->ex.E}, {c->ex.n_max}}; }
+ExpertSets fold_sets(const Ctx* c) { return {c->fold_first, c->fold_nmax}; }
+
+// The slots of one objective call, in list order: slot i evaluates expert set sets[i] at kernels[i] and the descriptors
+// hypers + i * nh; the Laplace objective adds the labels (y == cls[i]) (-1: as uploaded) and the modes of mode slot
+// modes[i].  A failing slot is named `what` names[i] (what == nullptr: not named).  The constructor makes n slots on
+// the whole upload with the labels as uploaded and mode slot 0; the entries fill in what differs.
+struct SlotList {
+  const sgp_kernel_desc* kernels;
+  const sgp_hyper* hypers;
+  int nh;
+  std::vector<int> sets, cls, modes, names;
+  const char* what = nullptr;
+  SlotList(const sgp_kernel_desc* k, const sgp_hyper* h, int n_hypers, int n)
+      : kernels(k), hypers(h), nh(n_hypers), sets(n, 0), cls(n, -1), modes(n, 0), names(n, 0) {}
+};
+
+// Device state of one objective evaluation, in the context's descriptor block.  Set-up slot j is list slot pos[j].
 struct ObjectiveSetup {
-  HyperView hv;                    // slot 0
-  int n_slots = 1;
-  long long slot_stride = 0;       // doubles between two slots' [beta | coef | value] blocks
-  const KernelFlat* kf = nullptr;  // [n_slots]
+  HyperView hv;                    // set-up slot 0
+  ObjectiveSlots slots;            // the slot table (f and f_stride: the Laplace objective's to fill)
   std::vector<KernelFlat> kf_host; // [n_slots]
-  const int* cls = nullptr;        // [n_slots] the classes (fold sets) list, or zeros
-  const int* mode = nullptr;       // [n_slots] the mode slots list (sgp_laplace_nll_slots_any_size), else cls
-  const int* sets = nullptr;       // [n_slots] the fold sets list (sgp_laplace_nll_fold_slots_any_size), else nullptr
+  ExpertSets es;                   // the sets the slots index
+  std::vector<int> set, pos;       // [n_slots] set-up slot j's expert set and list position
+  std::vector<int> names;          // [n_slots] list order
+  const char* what = nullptr;
   double* total = nullptr;         // [n_slots][1 + n_hypers] totals, then [n_slots] status words
   int* flags = nullptr;            // [n_slots]
 };
 
-// Flattens each slot's kernel (flatten_kernel: Eye terms only add to the diagonal), maps the hyper-parameter descriptors
-// (hypers + s * nh for slot s) onto the flattened terms and uploads everything, with zeroed totals and flags, into the
-// context's descriptor block in one copy.  Every slot must have slot 0's kernel structure and descriptor kinds.
-// rows_per_slot: the per-expert rows a slot writes (0: every uploaded expert).  modes: a mode slots list uploaded after
-// the classes (nullptr: o.mode is the classes list).  sets: a fold sets list uploaded after the modes (nullptr: none).
-int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int nh,
-                    const int* classes, ObjectiveSetup& o, long long rows_per_slot = 0, const int* modes = nullptr,
-                    const int* sets = nullptr) {
+// Flattens each slot's kernel (flatten_kernel: Eye terms only add to the diagonal), maps its hyper-parameter descriptors
+// onto the flattened terms and uploads everything, with the sets' first experts, the slot list and zeroed totals and
+// flags, into the context's descriptor block in one copy.  The slots are set up in the order pos (empty: list order).
+// Every slot must have the first one's kernel structure and descriptor kinds.
+int objective_setup(Ctx* c, const SlotList& L, ExpertSets es, ObjectiveSetup& o, std::vector<int> pos = {}) {
   if (c->ex.E == 0) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
-  if (!kernels || nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, "null argument");
+  const int nh = L.nh, n_slots = static_cast<int>(L.sets.size());
+  if (!L.kernels || nh < 0 || (nh > 0 && !L.hypers)) return fail(c, SGP_E_BADARG, "null argument");
+  if (pos.empty()) {
+    pos.resize(n_slots);
+    std::iota(pos.begin(), pos.end(), 0);
+  }
   for (int s = 0; s < n_slots; ++s)
-    if (!kernels[s].terms || kernels[s].n_terms <= 0) return fail(c, SGP_E_BADARG, "null argument");
+    if (!L.kernels[pos[s]].terms || L.kernels[pos[s]].n_terms <= 0) return fail(c, SGP_E_BADARG, "null argument");
   if (nh > kMaxHypers) return fail(c, SGP_E_BADARG, "too many hyper-parameters");
   const int d = c->ex.d;
-  const sgp_kernel_desc* k = kernels;
+  const sgp_kernel_desc* k = L.kernels + pos[0];
+  const sgp_hyper* h0 = L.hypers ? L.hypers + static_cast<size_t>(pos[0]) * nh : nullptr;
   std::vector<KernelFlat> kfs(n_slots);
   std::vector<int> flat_of;
   std::vector<double> block;       // [n_slots][beta | coef | value]
   std::vector<int> kind(nh), hterm(nh, 0), hdim(nh, 0);
   size_t nb = 0;                   // beta doubles of one slot
   o = ObjectiveSetup{};
-  o.n_slots = n_slots;
   HyperView& hv = o.hv;
   hv.d = d; hv.n_hypers = nh;
   for (int s = 0; s < n_slots; ++s) {
-    const sgp_kernel_desc* ks = kernels + s;
-    const sgp_hyper* hs = hypers ? hypers + static_cast<size_t>(s) * nh : nullptr;
+    const sgp_kernel_desc* ks = L.kernels + pos[s];
+    const sgp_hyper* hs = L.hypers ? L.hypers + static_cast<size_t>(pos[s]) * nh : nullptr;
     if (s > 0) {
       bool same = ks->n_terms == k->n_terms;
       for (int t = 0; same && t < k->n_terms; ++t) same = ks->terms[t].type == k->terms[t].type;
       for (int i = 0; same && i < nh; ++i)
-        same = hs[i].kind == kind[i] && (hs[i].kind == SGP_HYPER_SCALE || (hs[i].term == hypers[i].term && hs[i].dim == hdim[i]));
+        same = hs[i].kind == kind[i] && (hs[i].kind == SGP_HYPER_SCALE || (hs[i].term == h0[i].term && hs[i].dim == hdim[i]));
       if (!same) return fail(c, SGP_E_BADARG, "every class or fold slot needs the same kernel structure and hyper-parameter layout");
     }
     std::vector<double> beta;
@@ -1170,82 +1188,125 @@ int objective_setup(Ctx* c, int n_slots, const sgp_kernel_desc* kernels, const s
     if (s == 0) {
       hv.kf = kfs[0];
       nb = beta.size();
-      o.slot_stride = static_cast<long long>(beta.size() + coef.size() + value.size());
+      o.slots.slot_stride = static_cast<long long>(beta.size() + coef.size() + value.size());
     }
     block.insert(block.end(), beta.begin(), beta.end());
     block.insert(block.end(), coef.begin(), coef.end());
     block.insert(block.end(), value.begin(), value.end());
   }
-  // [KernelFlat n_slots] then doubles [slot blocks | totals | status], then ints [kind | term | dim | flags | classes
-  // | modes (with modes) | sets (with sets)]
+  o.set.resize(n_slots);
+  std::vector<int> cls(n_slots), modes(n_slots);
+  for (int s = 0; s < n_slots; ++s) {
+    const int k_s = o.set[s] = L.sets[pos[s]];
+    cls[s] = L.cls[pos[s]];
+    modes[s] = L.modes[pos[s]];
+    o.slots.E_max = std::max(o.slots.E_max, es.first[k_s + 1] - es.first[k_s]);
+  }
+  // [KernelFlat n_slots] then doubles [slot blocks | totals | status], long longs [first], then ints [kind | term | dim
+  // | flags | sets | classes | modes]
   const int W = 1 + nh;
   const size_t kf_bytes = sizeof(KernelFlat) * n_slots;
   const size_t n_dbl = block.size() + static_cast<size_t>(n_slots) * (W + 1);
-  const size_t n_int = 3 * static_cast<size_t>(nh) + ((modes ? 3 : 2) + (sets ? 1 : 0)) * static_cast<size_t>(n_slots);
-  std::vector<char> host(kf_bytes + n_dbl * 8 + n_int * 4, 0);
+  const size_t n_first = es.first.size();
+  const size_t n_int = 3 * static_cast<size_t>(nh) + 4 * static_cast<size_t>(n_slots);
+  std::vector<char> host(kf_bytes + (n_dbl + n_first) * 8 + n_int * 4, 0);
   std::memcpy(host.data(), kfs.data(), kf_bytes);
   std::memcpy(host.data() + kf_bytes, block.data(), block.size() * 8);
-  int* hi = reinterpret_cast<int*>(host.data() + kf_bytes + n_dbl * 8);
+  std::memcpy(host.data() + kf_bytes + n_dbl * 8, es.first.data(), n_first * 8);
+  int* hi = reinterpret_cast<int*>(host.data() + kf_bytes + (n_dbl + n_first) * 8);
   std::copy(kind.begin(), kind.end(), hi);
   std::copy(hterm.begin(), hterm.end(), hi + nh);
   std::copy(hdim.begin(), hdim.end(), hi + 2 * nh);
-  if (classes) std::copy(classes, classes + n_slots, hi + 3 * nh + n_slots);
-  if (modes) std::copy(modes, modes + n_slots, hi + 3 * nh + 2 * n_slots);
-  if (sets) std::copy(sets, sets + n_slots, hi + 3 * nh + (modes ? 3 : 2) * n_slots);
+  std::copy(o.set.begin(), o.set.end(), hi + 3 * nh + n_slots);
+  std::copy(cls.begin(), cls.end(), hi + 3 * nh + 2 * n_slots);
+  std::copy(modes.begin(), modes.end(), hi + 3 * nh + 3 * n_slots);
   int rc = ctx_scratch(c, c->hyper_ws, host.size());
   if (rc != SGP_OK) return rc;
   char* dev = c->hyper_ws.as<char>();
   SGP_CUDA(c, cudaMemcpyAsync(dev, host.data(), host.size(), cudaMemcpyHostToDevice, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));          // host is a local
-  rc = ctx_scratch(c, c->nll_per_ws, static_cast<size_t>(n_slots) * (rows_per_slot > 0 ? rows_per_slot : c->ex.E) * W * 8);
+  rc = ctx_scratch(c, c->nll_per_ws, static_cast<size_t>(n_slots) * o.slots.E_max * W * 8);
   if (rc != SGP_OK) return rc;
-  o.kf = reinterpret_cast<const KernelFlat*>(dev);
-  o.kf_host = std::move(kfs);
   double* dD = reinterpret_cast<double*>(dev + kf_bytes);
-  int* dI = reinterpret_cast<int*>(dD + n_dbl);
+  int* dI = reinterpret_cast<int*>(dD + n_dbl + n_first);
   hv.beta = dD; hv.h_coef = dD + nb; hv.h_value = hv.h_coef + static_cast<size_t>(nh) * (kMaxTerms + 1);
-  o.total = dD + block.size();
   hv.h_kind = dI; hv.h_term = dI + nh; hv.h_dim = dI + 2 * nh;
+  o.total = dD + block.size();
   o.flags = dI + 3 * nh;
-  o.cls = dI + 3 * nh + n_slots;
-  o.mode = modes ? o.cls + n_slots : o.cls;
-  if (sets) o.sets = o.cls + (modes ? 2 : 1) * n_slots;
+  o.slots.n_slots = n_slots;
+  o.slots.kf = reinterpret_cast<const KernelFlat*>(dev);
+  o.slots.first = reinterpret_cast<const long long*>(dD + n_dbl);
+  o.slots.sets = o.flags + n_slots;
+  o.slots.cls = o.flags + 2 * n_slots;
+  o.slots.mode = o.flags + 3 * n_slots;
+  o.kf_host = std::move(kfs);
+  o.es = std::move(es);
+  o.pos = std::move(pos);
+  o.names = L.names;
+  o.what = L.what;
   return SGP_OK;
 }
 
-// all-reduce over ranks, copy the (objective, gradient) rows of every slot back, map a bad pivot to err_code.  With a
-// classes (fold sets) list, the message names the first failing slot's class (set), `what` saying which.  pos (optional):
-// slot s's outputs go to position pos[s], and the first failing slot is the one of the smallest position.
+// Set-up slot s's view of the descriptors: its flattened kernel and its [beta | coef | value] block.
+HyperView slot_view(const ObjectiveSetup& o, int s) {
+  HyperView hv = o.hv;
+  hv.kf = o.kf_host[s];
+  const long long shift = s * o.slots.slot_stride;
+  hv.beta += shift; hv.h_coef += shift; hv.h_value += shift;
+  return hv;
+}
+
+// Set-up slots [s0, s1) as one launch: the upload seen with the largest expert over their sets (the kernels lay out
+// their shared memory and workspace from it), their slot table, the first one's view and their outputs.
+struct SlotRange {
+  ExpertSet view;
+  ObjectiveSlots slots;
+  HyperView hv;
+  double* rows;
+  double* total;
+  int* flags;
+};
+SlotRange slot_range(const Ctx* c, const ObjectiveSetup& o, int s0, int s1) {
+  const size_t W = 1 + o.hv.n_hypers;
+  SlotRange r{c->ex, o.slots, slot_view(o, s0), c->nll_per_ws.as<double>() + s0 * o.slots.E_max * W, o.total + s0 * W,
+              o.flags + s0};
+  r.view.n_max = 0;
+  r.slots.E_max = 0;
+  for (int s = s0; s < s1; ++s) {
+    r.view.n_max = std::max(r.view.n_max, o.es.nmax[o.set[s]]);
+    r.slots.E_max = std::max(r.slots.E_max, o.es.first[o.set[s] + 1] - o.es.first[o.set[s]]);
+  }
+  r.slots.n_slots = s1 - s0;
+  r.slots.sets += s0; r.slots.kf += s0; r.slots.cls += s0; r.slots.mode += s0;
+  return r;
+}
+
+// All-reduces over ranks, copies every slot's (objective, gradient) row to its list position and maps a status word to
+// err_code, naming the failing slot of the smallest list position.
 int objective_finish(Ctx* c, const ObjectiveSetup& o, int nh, double* val_out, double* grad_out, int mask, int err_code,
-                     const char* err_msg, const int* classes = nullptr, const char* what = "class",
-                     const int* pos = nullptr) {
-  const int W = 1 + nh, S = o.n_slots;
+                     const char* err_msg) {
+  const int W = 1 + nh, S = o.slots.n_slots;
   // the rank-local status flags are all-reduced WITH the totals so that every rank raises (or none does)
   SGP_CUDA(c, launch_flags_to_double(o.total + static_cast<size_t>(S) * W, o.flags, mask, S, c->stream));
   c->launches += 1;
   const size_t len = static_cast<size_t>(S) * (W + 1);
   std::vector<double> tot(len);
-  std::vector<int> listed;
+  std::vector<int> at = o.pos;                      // the list position of row s
   if (c->comm && c->nranks > 1) {
-    if (pos) {
-      // The row a slot was set up in follows the rank's own experts (the fold slots' on-chip | global-memory split), so
+    if (!std::is_sorted(at.begin(), at.end())) {
+      // The row a slot was set up in follows the rank's own experts (the Laplace [on chip | global memory] split), so
       // ranks may disagree on it: move every row and status word to its list position before the sum.
       std::vector<double> set_up(len);
       SGP_CUDA(c, cudaMemcpyAsync(set_up.data(), o.total, len * 8, cudaMemcpyDeviceToHost, c->stream));
       SGP_CUDA(c, cudaStreamSynchronize(c->stream));
       for (int s = 0; s < S; ++s) {
         std::copy(set_up.begin() + static_cast<size_t>(s) * W, set_up.begin() + static_cast<size_t>(s + 1) * W,
-                  tot.begin() + static_cast<size_t>(pos[s]) * W);
-        tot[static_cast<size_t>(S) * W + pos[s]] = set_up[static_cast<size_t>(S) * W + s];
+                  tot.begin() + static_cast<size_t>(at[s]) * W);
+        tot[static_cast<size_t>(S) * W + at[s]] = set_up[static_cast<size_t>(S) * W + s];
       }
       SGP_CUDA(c, cudaMemcpyAsync(o.total, tot.data(), len * 8, cudaMemcpyHostToDevice, c->stream));
       SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-      if (classes) {
-        listed.resize(S);
-        for (int s = 0; s < S; ++s) listed[pos[s]] = classes[s];
-        classes = listed.data();
-      }
-      pos = nullptr;                                // from here on, row s is list position s
+      std::iota(at.begin(), at.end(), 0);
     }
     ncclResult_t r = nccl().AllReduce(o.total, o.total, len, ncclDouble, ncclSum, c->comm, c->stream);
     if (r != ncclSuccess) return fail(c, SGP_E_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
@@ -1253,16 +1314,15 @@ int objective_finish(Ctx* c, const ObjectiveSetup& o, int nh, double* val_out, d
   }
   SGP_CUDA(c, cudaMemcpyAsync(tot.data(), o.total, len * 8, cudaMemcpyDeviceToHost, c->stream));
   SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  auto at = [&](int s) { return pos ? pos[s] : s; };
   int failed = -1;
   for (int s = 0; s < S; ++s)
-    if (tot[static_cast<size_t>(S) * W + s] != 0.0 && (failed < 0 || at(s) < at(failed))) failed = s;
+    if (tot[static_cast<size_t>(S) * W + s] != 0.0 && (failed < 0 || at[s] < at[failed])) failed = s;
   if (failed >= 0)
-    return fail(c, err_code, classes ? std::string(what) + " " + std::to_string(classes[failed]) + ": " + err_msg
-                                     : std::string(err_msg));
+    return fail(c, err_code, o.what ? std::string(o.what) + " " + std::to_string(o.names[at[failed]]) + ": " + err_msg
+                                    : std::string(err_msg));
   for (int s = 0; s < S; ++s) {
-    val_out[at(s)] = tot[static_cast<size_t>(s) * W];
-    for (int i = 1; i < W; ++i) grad_out[static_cast<size_t>(at(s)) * nh + i - 1] = tot[static_cast<size_t>(s) * W + i];
+    val_out[at[s]] = tot[static_cast<size_t>(s) * W];
+    for (int i = 1; i < W; ++i) grad_out[static_cast<size_t>(at[s]) * nh + i - 1] = tot[static_cast<size_t>(s) * W + i];
   }
   return SGP_OK;
 }
@@ -1292,6 +1352,54 @@ int bcm_lu_workspace(Ctx* c, const ObjectivePlan& plan) {
                                     std::to_string(avail >> 20) + " MiB available (lower datasetSizeForExpert)");
   return ctx_scratch(c, c->bcm_ws, plan.lu_ws);
 }
+
+// The BCM objective of a slot list, in one on-chip launch over experts x slots planned on the largest expert over the
+// listed sets (on-chip Cholesky per expert: SPD kernel matrices of <= ~165 points, every default configuration).  A slot
+// whose Cholesky broke down (not positive definite), or every slot when the experts do not fit on chip, takes the general
+// path on its set alone (its experts, its own largest expert), one slot after another: the reference's own arithmetic,
+// LU with partial pivoting and log|det| with the sign dropped (logDetAndInv.scala:36-63, GPR:59), on kernel matrices
+// staged in global memory.  The choice is rank-local; the one all-reduce per evaluation happens afterwards on every rank.
+int bcm_objective(Ctx* c, const char* fn, const SlotList& L, ExpertSets es, double* nll_out, double* grad_out) {
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  if (c->ex.E > 0) {                          // (without experts, objective_setup refuses)
+    int n_max = 0;
+    for (int k : L.sets) n_max = std::max(n_max, es.nmax[k]);
+    const int rc = bcm_check_size(c, n_max, fn);
+    if (rc != SGP_OK) return rc;
+  }
+  ObjectiveSetup o;
+  int rc = objective_setup(c, L, std::move(es), o);
+  if (rc != SGP_OK) return rc;
+  const int n = o.slots.n_slots;
+  const SlotRange all = slot_range(c, o, 0, n);
+  const ObjectivePlan plan = plan_objective(Objective::kBcm, all.view, o.hv.kf.n_terms);
+  std::vector<int> flags(n, 1);               // bit 0: the slot goes to the LU path
+  if (plan.variant != ObjectiveVariant::kLu) {
+    SGP_CUDA(c, launch_bcm_nll(plan, all.view, all.hv, all.slots, all.rows, all.total, all.flags, c->stream));
+    c->launches += 2;
+    SGP_CUDA(c, cudaMemcpyAsync(flags.data(), o.flags, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
+    SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  }
+  c->bcm_general = false;
+  for (int s = 0; s < n; ++s) {
+    if (!(flags[s] & 1)) continue;
+    c->bcm_general = true;
+    const SlotRange one = slot_range(c, o, s, s + 1);
+    ExpertSet set = one.view;
+    set.off += o.es.first[o.set[s]];
+    set.E = one.slots.E_max;
+    const ObjectivePlan lu = plan_objective(Objective::kBcmLu, set, one.hv.kf.n_terms);
+    rc = bcm_lu_workspace(c, lu);
+    if (rc != SGP_OK) return rc;
+    SGP_CUDA(c, cudaMemsetAsync(one.flags, 0, sizeof(int), c->stream));
+    int blas_status = 0;
+    SGP_CUDA(c, launch_bcm_nll_general(lu, c->blas, &blas_status, c->bcm_ws.p, set, one.hv, one.rows, one.total,
+                                       one.flags, c->stream));
+    if (blas_status != 0) return fail(c, SGP_E_CUDA, "cuBLAS batched LU failed, status " + std::to_string(blas_status));
+    c->launches += 5;
+  }
+  return objective_finish(c, o, L.nh, nll_out, grad_out, 2, SGP_E_SINGULAR, kBcmSingular);
+}
 }  // namespace
 
 int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh, double* nll_out,
@@ -1299,110 +1407,8 @@ int sgp_bcm_nll(sgp_ctx* h, const sgp_kernel_desc* k, const sgp_hyper* hypers, i
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
   if (!nll_out || (nh > 0 && !grad_out)) return fail(c, SGP_E_BADARG, "sgp_bcm_nll: null output");
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  if (c->ex.E > 0) {
-    const int rc = bcm_check_size(c, c->ex.n_max, "sgp_bcm_nll");
-    if (rc != SGP_OK) return rc;
-  }
-  ObjectiveSetup o;
-  int rc = objective_setup(c, 1, k, hypers, nh, nullptr, o);
-  if (rc != SGP_OK) return rc;
-  const HyperView& hv = o.hv;
-  double* dTotal = o.total;
-  int* dFlags = o.flags;
-  double* rows = c->nll_per_ws.as<double>();
-  // fast path: on-chip Cholesky per expert (SPD kernel matrices of <= ~165 points -- every default configuration).
-  // general path: experts of any size, or a kernel matrix on which Cholesky broke down (not positive definite): the
-  // reference's own arithmetic, LU with partial pivoting and log|det| with the sign dropped (logDetAndInv.scala:36-63,
-  // GPR:59), on kernel matrices staged in global memory.  The choice is rank-local; the one all-reduce per evaluation
-  // happens afterwards on every rank.
-  ObjectivePlan plan = plan_objective(Objective::kBcm, c->ex, hv.kf.n_terms);
-  if (plan.variant != ObjectiveVariant::kLu) {
-    SGP_CUDA(c, launch_bcm_nll(plan, c->ex, hv, rows, dTotal, dFlags, c->stream));
-    c->launches += 2;
-    int flags = 0;
-    SGP_CUDA(c, cudaMemcpyAsync(&flags, dFlags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-    if (flags & 1) plan = plan_objective(Objective::kBcmLu, c->ex, hv.kf.n_terms);
-  }
-  c->bcm_general = plan.variant == ObjectiveVariant::kLu;
-  if (c->bcm_general) {
-    rc = bcm_lu_workspace(c, plan);
-    if (rc != SGP_OK) return rc;
-    SGP_CUDA(c, cudaMemsetAsync(dFlags, 0, sizeof(int), c->stream));
-    int blas_status = 0;
-    SGP_CUDA(c, launch_bcm_nll_general(plan, c->blas, &blas_status, c->bcm_ws.p, c->ex, hv, rows, dTotal, dFlags,
-                                       c->stream));
-    if (blas_status != 0) return fail(c, SGP_E_CUDA, "cuBLAS batched LU failed, status " + std::to_string(blas_status));
-    c->launches += 5;
-  }
-  return objective_finish(c, o, nh, nll_out, grad_out, 2, SGP_E_SINGULAR, kBcmSingular);
+  return bcm_objective(c, "sgp_bcm_nll", SlotList(k, hypers, nh, 1), whole_upload(c), nll_out, grad_out);
 }
-
-namespace {
-// The BCM objective of n_eval slots over expert sets of the upload, in one on-chip launch over experts x slots: slot s
-// evaluates set k = sets[s] (the experts first[k] .. first[k+1]-1, the largest of nmax[k] points; c->ex_set_first holds
-// first on the device) at kernels[s] and hypers + s * nh.  The set indices are the caller's to check.  A failing slot is
-// named `what` names[s].
-int bcm_nll_sets(Ctx* c, const char* fn, const int32_t* sets, int n_eval, const std::vector<long long>& first,
-                 const std::vector<int>& nmax, const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int nh,
-                 double* nll_out, double* grad_out, const int* names, const char* what) {
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  // one plan for the call, on the largest expert over the listed sets; the kernel lays out its shared memory from the
-  // same n_max, so it launches on this view
-  ExpertSet listed = c->ex;
-  long long E_max = 0;
-  listed.n_max = 0;
-  for (int s = 0; s < n_eval; ++s) {
-    listed.n_max = std::max(listed.n_max, nmax[sets[s]]);
-    E_max = std::max(E_max, first[sets[s] + 1] - first[sets[s]]);
-  }
-  int rc = bcm_check_size(c, listed.n_max, fn);
-  if (rc != SGP_OK) return rc;
-  ObjectiveSetup o;
-  rc = objective_setup(c, n_eval, kernels, hypers, nh, sets, o, E_max);
-  if (rc != SGP_OK) return rc;
-  const int W = 1 + nh;
-  double* rows = c->nll_per_ws.as<double>();
-  const ObjectivePlan plan = plan_objective(Objective::kBcm, listed, o.hv.kf.n_terms);
-  std::vector<int> flags(n_eval, 1);          // bit 0: the slot goes to the LU path
-  if (plan.variant != ObjectiveVariant::kLu) {
-    BcmFolds f;
-    f.n_slots = n_eval; f.E_max = E_max; f.sets = o.cls; f.first = c->ex_set_first.as<long long>(); f.kf = o.kf;
-    f.slot_stride = o.slot_stride;
-    SGP_CUDA(c, launch_bcm_nll(plan, listed, o.hv, rows, o.total, o.flags, c->stream, &f));
-    c->launches += 2;
-    SGP_CUDA(c, cudaMemcpyAsync(flags.data(), o.flags, sizeof(int) * n_eval, cudaMemcpyDeviceToHost, c->stream));
-    SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  }
-  // a slot whose Cholesky broke down, or every slot when the experts do not fit on chip: the LU path on that slot's set
-  // alone (its experts, its own largest expert), one slot after another
-  c->bcm_general = false;
-  for (int s = 0; s < n_eval; ++s) {
-    if (!(flags[s] & 1)) continue;
-    c->bcm_general = true;
-    const int k = sets[s];
-    ExpertSet set = c->ex;
-    set.off = c->ex.off + first[k];
-    set.E = first[k + 1] - first[k];
-    set.n_max = nmax[k];
-    HyperView hv = o.hv;
-    hv.kf = o.kf_host[s];
-    hv.beta += s * o.slot_stride; hv.h_coef += s * o.slot_stride; hv.h_value += s * o.slot_stride;
-    const ObjectivePlan lu = plan_objective(Objective::kBcmLu, set, hv.kf.n_terms);
-    rc = bcm_lu_workspace(c, lu);
-    if (rc != SGP_OK) return rc;
-    SGP_CUDA(c, cudaMemsetAsync(o.flags + s, 0, sizeof(int), c->stream));
-    int blas_status = 0;
-    SGP_CUDA(c, launch_bcm_nll_general(lu, c->blas, &blas_status, c->bcm_ws.p, set, hv,
-                                       rows + static_cast<size_t>(s) * E_max * W, o.total + static_cast<size_t>(s) * W,
-                                       o.flags + s, c->stream));
-    if (blas_status != 0) return fail(c, SGP_E_CUDA, "cuBLAS batched LU failed, status " + std::to_string(blas_status));
-    c->launches += 5;
-  }
-  return objective_finish(c, o, nh, nll_out, grad_out, 2, SGP_E_SINGULAR, kBcmSingular, names, what);
-}
-}  // namespace
 
 int sgp_bcm_nll_folds(sgp_ctx* h, const int32_t* sets, int32_t n_eval, const sgp_kernel_desc* kernels,
                       const sgp_hyper* hypers, int32_t nh, double* nll_out, double* grad_out) {
@@ -1416,8 +1422,11 @@ int sgp_bcm_nll_folds(sgp_ctx* h, const int32_t* sets, int32_t n_eval, const sgp
   for (int s = 0; s < n_eval; ++s)
     if (sets[s] < 0 || sets[s] >= n_sets)
       return fail(c, SGP_E_BADARG, "sgp_bcm_nll_folds: set index " + std::to_string(sets[s]) + " outside [0, n_folds)");
-  return bcm_nll_sets(c, "sgp_bcm_nll_folds", sets, n_eval, c->fold_first, c->fold_nmax, kernels, hypers, nh, nll_out,
-                      grad_out, sets, "fold set");
+  SlotList L(kernels, hypers, nh, n_eval);
+  L.sets.assign(sets, sets + n_eval);
+  L.names = L.sets;
+  L.what = "fold set";
+  return bcm_objective(c, "sgp_bcm_nll_folds", L, fold_sets(c), nll_out, grad_out);
 }
 
 int sgp_bcm_nll_slots(sgp_ctx* h, int32_t n_eval, const sgp_kernel_desc* kernels, const sgp_hyper* hypers, int32_t nh,
@@ -1429,12 +1438,10 @@ int sgp_bcm_nll_slots(sgp_ctx* h, int32_t n_eval, const sgp_kernel_desc* kernels
     return fail(c, SGP_E_STATE, "sgp_experts_upload_grouped should have been called first (sgp_bcm_nll_slots evaluates "
                                 "one grouped training set; a fold upload or sgp_experts_upload has none)");
   if (n_eval < 1 || n_eval > 65535) return fail(c, SGP_E_BADARG, "sgp_bcm_nll_slots: need 1 <= n_eval <= 65535");
-  // every slot on the upload's one set, {0, E} (in c->ex_set_first since the grouped upload); slots are named by index
-  const std::vector<int32_t> zeros(n_eval, 0);
-  std::vector<int> slot(n_eval);
-  for (int s = 0; s < n_eval; ++s) slot[s] = s;
-  return bcm_nll_sets(c, "sgp_bcm_nll_slots", zeros.data(), n_eval, {0, c->ex.E}, {c->ex.n_max}, kernels, hypers, nh,
-                      nll_out, grad_out, slot.data(), "slot");
+  SlotList L(kernels, hypers, nh, n_eval);    // every slot on the whole upload, named by its index
+  std::iota(L.names.begin(), L.names.end(), 0);
+  L.what = "slot";
+  return bcm_objective(c, "sgp_bcm_nll_slots", L, whole_upload(c), nll_out, grad_out);
 }
 
 const char* const kLaplaceRefused =
@@ -1445,96 +1452,103 @@ const char* const kLaplaceNoIteration =
     "MatrixSingularException (GaussianProcessClassifier.scala:91,116)";
 
 namespace {
-// The Laplace objective of the set-up slots (classes: the one-vs-rest slots, or nullptr), on the kernel plan_objective
-// picks for `kind`: laplace_kernel when the largest expert fits on chip, laplace_global_kernel otherwise (any size only).
-int laplace_run(Ctx* c, Objective kind, const ObjectiveSetup& o, double tol, const LaplaceClasses* classes) {
-  const ObjectivePlan plan = plan_objective(kind, c->ex, o.hv.kf.n_terms);
-  if (plan.variant == ObjectiveVariant::kRefused) return fail(c, SGP_E_BADARG, kLaplaceRefused);
-  if (plan.variant == ObjectiveVariant::kLaplace) {
-    SGP_CUDA(c, launch_laplace(plan, c->ex, o.hv, tol, c->nll_per_ws.as<double>(), o.total, o.flags, c->stream, classes));
-    c->laplace_path = 0;
-    c->launches += 2;
-    return SGP_OK;
-  }
-  // global-memory kernel: one workspace slice per CTA; the grid is bounded by the work items, the resident CTAs and the
-  // workspace that fits under kLaplaceGlobalCapBytes and the device's free memory (what this context holds included)
+// A mode store of n_store slots of `stride` modes each, (re)allocated and zeroed when store.slots, the count it was set
+// up for, differs (0 after every upload).  SGP_E_NOMEM, before allocating, past the device's free memory; a failed
+// allocation leaves no store behind.
+int mode_store(Ctx* c, ModeStore& store, int n_store, long long stride) {
+  if (store.slots == n_store) return SGP_OK;
+  const size_t bytes = static_cast<size_t>(n_store) * stride * 8;
   size_t free_b = 0, total_b = 0;
   SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
-  const size_t avail = free_b + c->laplace_ws.cap;
-  if (plan.cta_ws > avail)
-    return fail(c, SGP_E_NOMEM, "the global-memory Laplace kernel needs " + std::to_string(plan.cta_ws >> 20) +
-                                    " MiB of device memory for one expert of " + std::to_string(c->ex.n_max) +
-                                    " points, " + std::to_string(avail >> 20) + " MiB available");
-  if (c->ex.n_max > kLaplaceGlobalMaxPoints)
-    return fail(c, SGP_E_BADARG, "datasetSizeForExpert above " + std::to_string(kLaplaceGlobalMaxPoints) +
-                                     " points (32-bit indexing of the per-expert kernel build)");
-  const long long items = c->ex.E * (classes ? classes->n_slots : 1);
-  const long long resident = static_cast<long long>(laplace_global_ctas_per_sm()) * c->num_sms;
-  const long long grid = laplace_global_grid(items, resident, plan.cta_ws, std::min(kLaplaceGlobalCapBytes, avail));
-  int rc = ctx_scratch(c, c->laplace_ws, static_cast<size_t>(grid) * plan.cta_ws);
+  if (bytes > free_b + store.buf.cap)
+    return fail(c, SGP_E_NOMEM, "the Laplace modes of " + std::to_string(n_store) + " slots need " +
+                                    std::to_string(bytes >> 20) + " MiB of device memory, " +
+                                    std::to_string((free_b + store.buf.cap) >> 20) + " MiB available");
+  store.slots = 0;
+  const int rc = ctx_scratch(c, store.buf, bytes);
   if (rc != SGP_OK) return rc;
-  SGP_CUDA(c, launch_laplace_global(c->ex, o.hv, tol, c->laplace_ws.as<double>(), grid, c->nll_per_ws.as<double>(),
-                                    o.total, o.flags, c->stream, classes));
-  c->laplace_path = 1;
-  c->launches += 2;
+  SGP_CUDA(c, cudaMemsetAsync(store.buf.p, 0, bytes, c->stream));
+  store.slots = n_store;
   return SGP_OK;
 }
 
+// The Laplace objective of a slot list with the modes of `store` (n_store mode slots of `stride` modes).  Each slot runs
+// the kernel its own set plans (sgp_laplace_nll_any_size's rule on the set's largest expert): the slots are set up in
+// the order [on chip | global memory], each family a contiguous range planned for `kind` and launched on its own.  On
+// one set this is one family, planned on the whole upload.
+int laplace_objective(Ctx* c, Objective kind, const SlotList& L, ExpertSets es, ModeStore& store, int n_store,
+                      long long stride, double tol, double* neg_log_z_out, double* grad_out) {
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  const int n = static_cast<int>(L.sets.size());
+  ExpertSet probe = c->ex;
+  std::vector<char> on_chip(n);
+  for (int s = 0; s < n; ++s) {
+    probe.n_max = es.nmax[L.sets[s]];
+    on_chip[s] = plan_objective(Objective::kLaplaceAnySize, probe, 1).variant == ObjectiveVariant::kLaplace;
+  }
+  std::vector<int> pos;
+  for (int s = 0; s < n; ++s) if (on_chip[s]) pos.push_back(s);
+  const int n_chip = static_cast<int>(pos.size());
+  for (int s = 0; s < n; ++s) if (!on_chip[s]) pos.push_back(s);
+  ObjectiveSetup o;
+  int rc = objective_setup(c, L, std::move(es), o, std::move(pos));
+  if (rc != SGP_OK) return rc;
+  struct Family { SlotRange r; ObjectivePlan plan; };
+  std::vector<Family> fams;
+  for (const auto& [s0, s1] : {std::pair<int, int>{0, n_chip}, std::pair<int, int>{n_chip, n}}) {
+    if (s0 == s1) continue;
+    Family fam{slot_range(c, o, s0, s1), {}};
+    fam.plan = plan_objective(kind, fam.r.view, o.hv.kf.n_terms);
+    if (fam.plan.variant == ObjectiveVariant::kRefused) return fail(c, SGP_E_BADARG, kLaplaceRefused);
+    fams.push_back(fam);
+  }
+  rc = mode_store(c, store, n_store, stride);   // first use after an upload, or another slot count
+  if (rc != SGP_OK) return rc;
+  // the global-memory family: one workspace slice per CTA; the grid is bounded by the work items, the resident CTAs and
+  // the workspace that fits under kLaplaceGlobalCapBytes and the device's free memory (what this context holds included)
+  long long grid = 0;
+  for (const Family& fam : fams) {
+    if (fam.plan.variant != ObjectiveVariant::kLaplaceGlobal) continue;
+    size_t free_b = 0, total_b = 0;
+    SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+    const size_t avail = free_b + c->laplace_ws.cap;
+    if (fam.plan.cta_ws > avail)
+      return fail(c, SGP_E_NOMEM, "the global-memory Laplace kernel needs " + std::to_string(fam.plan.cta_ws >> 20) +
+                                      " MiB of device memory for one expert of " + std::to_string(fam.r.view.n_max) +
+                                      " points, " + std::to_string(avail >> 20) + " MiB available");
+    if (fam.r.view.n_max > kLaplaceGlobalMaxPoints)
+      return fail(c, SGP_E_BADARG, "datasetSizeForExpert above " + std::to_string(kLaplaceGlobalMaxPoints) +
+                                       " points (32-bit indexing of the per-expert kernel build)");
+    const long long resident = static_cast<long long>(laplace_global_ctas_per_sm()) * c->num_sms;
+    grid = laplace_global_grid(fam.r.slots.E_max * fam.r.slots.n_slots, resident, fam.plan.cta_ws,
+                               std::min(kLaplaceGlobalCapBytes, avail));
+    rc = ctx_scratch(c, c->laplace_ws, static_cast<size_t>(grid) * fam.plan.cta_ws);
+    if (rc != SGP_OK) return rc;
+  }
+  c->laplace_path = 0;
+  for (Family& fam : fams) {
+    SlotRange& r = fam.r;
+    r.slots.f = store.buf.as<double>();
+    r.slots.f_stride = stride;
+    if (fam.plan.variant == ObjectiveVariant::kLaplace) {
+      SGP_CUDA(c, launch_laplace(fam.plan, r.view, r.hv, tol, r.slots, r.rows, r.total, r.flags, c->stream));
+    } else {
+      SGP_CUDA(c, launch_laplace_global(r.view, r.hv, tol, c->laplace_ws.as<double>(), grid, r.slots, r.rows, r.total,
+                                        r.flags, c->stream));
+      c->laplace_path = 1;
+    }
+    c->launches += 2;
+  }
+  return objective_finish(c, o, L.nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd);
+}
+
+// sgp_laplace_nll and _any_size: one slot on the whole upload, the labels as uploaded, the binary modes ex.f
 int laplace_nll(Ctx* c, Objective kind, const sgp_kernel_desc* k, const sgp_hyper* hypers, int32_t nh, double tol,
                 double* neg_log_z_out, double* grad_out) {
   if (!neg_log_z_out || (nh > 0 && !grad_out) || !(tol > 0.0)) return fail(c, SGP_E_BADARG, "sgp_laplace_nll: bad argument");
   if (tol >= 1.0) return fail(c, SGP_E_SINGULAR, kLaplaceNoIteration);
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  ObjectiveSetup o;
-  int rc = objective_setup(c, 1, k, hypers, nh, nullptr, o);
-  if (rc == SGP_OK) rc = laplace_run(c, kind, o, tol, nullptr);
-  if (rc != SGP_OK) return rc;
-  return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd);
-}
-
-// A mode store of n_store slots of `stride` modes each, (re)allocated and zeroed when *store_slots, the count it was set
-// up for, differs (0 after every upload).  SGP_E_NOMEM, before allocating, past the device's free memory; a failed
-// allocation leaves no store behind.
-int mode_store(Ctx* c, DevScratch& store, int* store_slots, int n_store, long long stride) {
-  if (*store_slots == n_store) return SGP_OK;
-  const size_t bytes = static_cast<size_t>(n_store) * stride * 8;
-  size_t free_b = 0, total_b = 0;
-  SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
-  if (bytes > free_b + store.cap)
-    return fail(c, SGP_E_NOMEM, "the Laplace modes of " + std::to_string(n_store) + " slots need " +
-                                    std::to_string(bytes >> 20) + " MiB of device memory, " +
-                                    std::to_string((free_b + store.cap) >> 20) + " MiB available");
-  *store_slots = 0;
-  const int rc = ctx_scratch(c, store, bytes);
-  if (rc != SGP_OK) return rc;
-  SGP_CUDA(c, cudaMemsetAsync(store.p, 0, bytes, c->stream));
-  *store_slots = n_store;
-  return SGP_OK;
-}
-
-// The Laplace objective of n_eval slots over a mode store: slot i evaluates the labels (y == classes[i]) at kernels[i]
-// and hypers[i * nh ...], with the modes of store slot modes[i] (nullptr: modes = classes).  The store holds n_store
-// slots of n modes; it is (re)allocated and zeroed when *store_slots, the count it was set up for, differs (0 after every
-// upload).  The callers have checked the lists; `what` names a slot in the SGP_E_NOT_PD message.
-int laplace_slots(Ctx* c, Objective kind, DevScratch& store, int* store_slots, int n_store, const int32_t* classes,
-                  const int32_t* modes, int32_t n_eval, const sgp_kernel_desc* kernels, const sgp_hyper* hypers,
-                  int32_t nh, double tol, double* neg_log_z_out, double* grad_out, const char* what) {
-  if (tol >= 1.0) return fail(c, SGP_E_SINGULAR, kLaplaceNoIteration);
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  ObjectiveSetup o;
-  int rc = objective_setup(c, n_eval, kernels, hypers, nh, classes, o, 0, modes);
-  if (rc != SGP_OK) return rc;
-  if (plan_objective(kind, c->ex, o.hv.kf.n_terms).variant == ObjectiveVariant::kRefused)
-    return fail(c, SGP_E_BADARG, kLaplaceRefused);
-  rc = mode_store(c, store, store_slots, n_store, c->ex.n);   // first use after an upload, or another slot count
-  if (rc != SGP_OK) return rc;
-  LaplaceClasses lc;
-  lc.n_slots = n_eval; lc.cls = o.cls; lc.mode = o.mode; lc.kf = o.kf; lc.slot_stride = o.slot_stride;
-  lc.f = store.as<double>(); lc.f_stride = c->ex.n;
-  rc = laplace_run(c, kind, o, tol, &lc);
-  if (rc != SGP_OK) return rc;
-  return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd, modes ? modes : classes,
-                          what);
+  return laplace_objective(c, kind, SlotList(k, hypers, nh, 1), whole_upload(c), c->ex_f, 1, c->ex.n, tol, neg_log_z_out,
+                           grad_out);
 }
 
 // true when the n entries of v are distinct and in [0, bound)
@@ -1553,8 +1567,12 @@ int laplace_nll_classes(Ctx* c, Objective kind, int32_t n_classes, const int32_t
     return fail(c, SGP_E_BADARG, "sgp_laplace_nll_classes: need 1 <= n_eval <= n_classes and n_eval <= 65535");
   if (!distinct_in_range(classes, n_eval, n_classes))
     return fail(c, SGP_E_BADARG, "sgp_laplace_nll_classes: class indices must be distinct and in [0, n_classes)");
-  return laplace_slots(c, kind, c->ex_fc, &c->ex_classes, n_classes, classes, nullptr, n_eval, kernels, hypers, nh, tol,
-                       neg_log_z_out, grad_out, "class");
+  if (tol >= 1.0) return fail(c, SGP_E_SINGULAR, kLaplaceNoIteration);
+  SlotList L(kernels, hypers, nh, n_eval);    // class c keeps its modes in mode slot c
+  L.cls.assign(classes, classes + n_eval);
+  L.modes = L.names = L.cls;
+  L.what = "class";
+  return laplace_objective(c, kind, L, whole_upload(c), c->ex_fc, n_classes, c->ex.n, tol, neg_log_z_out, grad_out);
 }
 }  // namespace
 
@@ -1603,8 +1621,14 @@ int sgp_laplace_nll_slots_any_size(sgp_ctx* h, int32_t n_mode_slots, const int32
     return fail(c, SGP_E_BADARG, "sgp_laplace_nll_slots_any_size: mode slots must be distinct and in [0, n_mode_slots)");
   if (*std::min_element(classes, classes + n_eval) < 0)
     return fail(c, SGP_E_BADARG, "sgp_laplace_nll_slots_any_size: class indices must be >= 0");
-  return laplace_slots(c, Objective::kLaplaceAnySize, c->ex_fm, &c->ex_mode_slots, n_mode_slots, classes, mode_slots,
-                       n_eval, kernels, hypers, nh, tol, neg_log_z_out, grad_out, "mode slot");
+  if (tol >= 1.0) return fail(c, SGP_E_SINGULAR, kLaplaceNoIteration);
+  SlotList L(kernels, hypers, nh, n_eval);
+  L.cls.assign(classes, classes + n_eval);
+  L.modes.assign(mode_slots, mode_slots + n_eval);
+  L.names = L.modes;
+  L.what = "mode slot";
+  return laplace_objective(c, Objective::kLaplaceAnySize, L, whole_upload(c), c->ex_fm, n_mode_slots, c->ex.n, tol,
+                           neg_log_z_out, grad_out);
 }
 
 namespace {
@@ -1613,24 +1637,6 @@ long long fold_rows_max(const Ctx* c) {
   long long m = 0;
   for (size_t k = 0; k + 1 < c->fold_row0.size(); ++k) m = std::max(m, c->fold_row0[k + 1] - c->fold_row0[k]);
   return m;
-}
-
-// The stored modes of mode slot `mode_slot` on fold set `set` (from the set's first row), after the fold-slot getters'
-// refusals; n_k and E_k: the set's rows and experts.
-int fold_slot_modes(Ctx* c, int32_t set, int32_t mode_slot, const void* out, const char* fn, const double** f,
-                    long long* n_k, long long* E_k) {
-  if (c->ex.E == 0 || c->fold_first.empty() || !out)
-    return fail(c, SGP_E_STATE, "sgp_experts_upload_folds should have been called first");
-  if (c->ex_fold_mode_slots == 0)
-    return fail(c, SGP_E_STATE, "no fold slot modes: sgp_laplace_nll_fold_slots_any_size has not run since the upload");
-  const int n_sets = static_cast<int>(c->fold_first.size()) - 1;
-  if (set < 0 || set >= n_sets) return fail(c, SGP_E_BADARG, std::string(fn) + ": set index outside [0, n_folds)");
-  if (mode_slot < 0 || mode_slot >= c->ex_fold_mode_slots)
-    return fail(c, SGP_E_BADARG, std::string(fn) + ": mode slot outside [0, n_mode_slots)");
-  *f = c->ex_ffm.as<double>() + static_cast<size_t>(mode_slot) * fold_rows_max(c);
-  *n_k = c->fold_row0[set + 1] - c->fold_row0[set];
-  *E_k = c->fold_first[set + 1] - c->fold_first[set];
-  return SGP_OK;
 }
 }  // namespace
 
@@ -1662,192 +1668,123 @@ int sgp_laplace_nll_fold_slots_any_size(sgp_ctx* h, int32_t n_mode_slots, const 
                                      " points (32-bit indexing of the per-expert kernel build)");
   if (tol >= 1.0) return fail(c, SGP_E_SINGULAR, kLaplaceNoIteration);
   if (!kernels || nh < 0 || (nh > 0 && !hypers)) return fail(c, SGP_E_BADARG, fn + ": null argument");
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  // Each slot runs the kernel its own set plans (sgp_laplace_nll_any_size's rule on the set's largest expert): the slots
-  // are set up in the order [on chip | global memory], each family a contiguous range launched on its own; pos[j] is
-  // the list position of set-up slot j.
-  ExpertSet probe = c->ex;
-  std::vector<char> on_chip(n_eval);
-  for (int s = 0; s < n_eval; ++s) {
-    probe.n_max = c->fold_nmax[sets[s]];
-    on_chip[s] = plan_objective(Objective::kLaplaceAnySize, probe, 1).variant == ObjectiveVariant::kLaplace;
-  }
-  std::vector<int> pos;
-  for (int s = 0; s < n_eval; ++s) if (on_chip[s]) pos.push_back(s);
-  const int n_chip = static_cast<int>(pos.size());
-  for (int s = 0; s < n_eval; ++s) if (!on_chip[s]) pos.push_back(s);
-  std::vector<sgp_kernel_desc> kp(n_eval);
-  std::vector<sgp_hyper> hp(static_cast<size_t>(n_eval) * nh);
-  std::vector<int> mp(n_eval), sp(n_eval), cp(n_eval);
-  long long E_max = 0;
-  for (int j = 0; j < n_eval; ++j) {
-    const int s = pos[j];
-    kp[j] = kernels[s];
-    std::copy(hypers + static_cast<size_t>(s) * nh, hypers + static_cast<size_t>(s + 1) * nh,
-              hp.begin() + static_cast<size_t>(j) * nh);
-    mp[j] = mode_slots[s]; sp[j] = sets[s]; cp[j] = classes[s];
-    E_max = std::max(E_max, c->fold_first[sets[s] + 1] - c->fold_first[sets[s]]);
-  }
-  ObjectiveSetup o;
-  int rc = objective_setup(c, n_eval, kp.data(), hp.data(), nh, cp.data(), o, E_max, mp.data(), sp.data());
-  if (rc != SGP_OK) return rc;
-  const long long stride = fold_rows_max(c);
-  rc = mode_store(c, c->ex_ffm, &c->ex_fold_mode_slots, n_mode_slots, stride);
-  if (rc != SGP_OK) return rc;
-  // one view and plan per family: the largest expert and expert count over the family's sets
-  struct Family { int s0, s1; ExpertSet view; long long E; ObjectivePlan plan; };
-  std::vector<Family> fams;
-  for (int f = 0; f < 2; ++f) {
-    Family fam{f == 0 ? 0 : n_chip, f == 0 ? n_chip : n_eval, c->ex, 0, ObjectivePlan{}};
-    if (fam.s0 == fam.s1) continue;
-    fam.view.n_max = 0;
-    for (int j = fam.s0; j < fam.s1; ++j) {
-      fam.view.n_max = std::max(fam.view.n_max, c->fold_nmax[sp[j]]);
-      fam.E = std::max(fam.E, c->fold_first[sp[j] + 1] - c->fold_first[sp[j]]);
-    }
-    fam.plan = plan_objective(Objective::kLaplaceAnySize, fam.view, o.hv.kf.n_terms);
-    fams.push_back(fam);
-  }
-  // the global-memory family's workspace, before anything launches (as laplace_run sizes it)
-  long long grid = 0;
-  for (const Family& fam : fams) {
-    if (fam.plan.variant != ObjectiveVariant::kLaplaceGlobal) continue;
-    size_t free_b = 0, total_b = 0;
-    SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
-    const size_t avail = free_b + c->laplace_ws.cap;
-    if (fam.plan.cta_ws > avail)
-      return fail(c, SGP_E_NOMEM, "the global-memory Laplace kernel needs " + std::to_string(fam.plan.cta_ws >> 20) +
-                                      " MiB of device memory for one expert of " + std::to_string(fam.view.n_max) +
-                                      " points, " + std::to_string(avail >> 20) + " MiB available");
-    const long long resident = static_cast<long long>(laplace_global_ctas_per_sm()) * c->num_sms;
-    grid = laplace_global_grid(fam.E * (fam.s1 - fam.s0), resident, fam.plan.cta_ws,
-                               std::min(kLaplaceGlobalCapBytes, avail));
-    rc = ctx_scratch(c, c->laplace_ws, static_cast<size_t>(grid) * fam.plan.cta_ws);
-    if (rc != SGP_OK) return rc;
-  }
-  const int W = 1 + nh;
-  c->laplace_path = 0;
-  for (const Family& fam : fams) {
-    const int s0 = fam.s0;
-    LaplaceClasses lc;
-    lc.n_slots = fam.s1 - s0; lc.cls = o.cls + s0; lc.mode = o.mode + s0; lc.kf = o.kf + s0;
-    lc.slot_stride = o.slot_stride; lc.f = c->ex_ffm.as<double>(); lc.f_stride = stride;
-    lc.sets = o.sets + s0; lc.first = c->ex_set_first.as<long long>(); lc.E_max = fam.E;
-    HyperView hv = o.hv;
-    hv.kf = o.kf_host[s0];
-    hv.beta += s0 * o.slot_stride; hv.h_coef += s0 * o.slot_stride; hv.h_value += s0 * o.slot_stride;
-    double* rows = c->nll_per_ws.as<double>() + static_cast<size_t>(s0) * E_max * W;
-    double* total = o.total + static_cast<size_t>(s0) * W;
-    if (fam.plan.variant == ObjectiveVariant::kLaplace) {
-      SGP_CUDA(c, launch_laplace(fam.plan, fam.view, hv, tol, rows, total, o.flags + s0, c->stream, &lc));
-    } else {
-      SGP_CUDA(c, launch_laplace_global(fam.view, hv, tol, c->laplace_ws.as<double>(), grid, rows, total, o.flags + s0,
-                                        c->stream, &lc));
-      c->laplace_path = 1;
-    }
-    c->launches += 2;
-  }
-  return objective_finish(c, o, nh, neg_log_z_out, grad_out, 1, SGP_E_NOT_PD, kLaplaceNotPd, mp.data(), "mode slot",
-                          pos.data());
+  SlotList L(kernels, hypers, nh, n_eval);
+  L.sets.assign(sets, sets + n_eval);
+  L.cls.assign(classes, classes + n_eval);
+  L.modes.assign(mode_slots, mode_slots + n_eval);
+  L.names = L.modes;
+  L.what = "mode slot";
+  return laplace_objective(c, Objective::kLaplaceAnySize, L, fold_sets(c), c->ex_ffm, n_mode_slots, fold_rows_max(c),
+                           tol, neg_log_z_out, grad_out);
 }
+
+namespace {
+constexpr int kModesFold = -1;   // the fold-slot store (sgp_experts_get_f_fold_*), next to sgp.h's SGP_MODES_*
+
+// The modes a getter reads: rows modes of `experts` experts from f.
+struct Modes {
+  const double* f;
+  long long rows, experts;
+};
+
+// The modes of store SGP_MODES_BINARY (index ignored), _CLASS or _SLOT (class or mode slot `index`), or kModesFold (mode
+// slot `index` on fold set `set`), after the getters' refusals in their order; fn names the getter.
+int find_modes(Ctx* c, int store, int index, int set, const void* out, const char* fn, Modes& m) {
+  const bool fold = store == kModesFold;
+  if (c->ex.E == 0 || (fold && c->fold_first.empty()) || !out)
+    return fail(c, SGP_E_STATE, fold ? "sgp_experts_upload_folds should have been called first"
+                                     : "sgp_experts_upload should have been called first");
+  m = {c->ex.f, c->ex.n, c->ex.E};
+  if (store == SGP_MODES_BINARY) return SGP_OK;
+  const ModeStore& s = fold ? c->ex_ffm : store == SGP_MODES_CLASS ? c->ex_fc : c->ex_fm;
+  if (s.slots == 0)
+    return fail(c, SGP_E_STATE, fold ? "no fold slot modes: sgp_laplace_nll_fold_slots_any_size has not run since the upload"
+                                : store == SGP_MODES_CLASS ? "no class modes: sgp_laplace_nll_classes has not run since the upload"
+                                : "no slot modes: sgp_laplace_nll_slots_any_size has not run since the upload");
+  long long stride = c->ex.n;
+  if (fold) {
+    if (set < 0 || set >= static_cast<int>(c->fold_first.size()) - 1)
+      return fail(c, SGP_E_BADARG, std::string(fn) + ": set index outside [0, n_folds)");
+    stride = fold_rows_max(c);
+    m.rows = c->fold_row0[set + 1] - c->fold_row0[set];
+    m.experts = c->fold_first[set + 1] - c->fold_first[set];
+  }
+  if (index < 0 || index >= s.slots)
+    return fail(c, SGP_E_BADARG, std::string(fn) + (store == SGP_MODES_CLASS ? ": class index out of range"
+                                                                           : ": mode slot outside [0, n_mode_slots)"));
+  m.f = s.buf.as<double>() + static_cast<size_t>(index) * stride;
+  return SGP_OK;
+}
+
+// the host getters: the modes in the experts' packed order
+int copy_modes(Ctx* c, int store, int index, int set, double* f_out, const char* fn) {
+  Modes m;
+  const int rc = find_modes(c, store, index, set, f_out, fn, m);
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  SGP_CUDA(c, cudaMemcpyAsync(f_out, m.f, static_cast<size_t>(m.rows) * 8, cudaMemcpyDeviceToHost, c->stream));
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  return SGP_OK;
+}
+
+// the _rows_device getters: the modes ungrouped into row order (a grouped upload, or a fold set, which is grouped as one)
+int ungroup_modes(Ctx* c, const Modes& m, double* dF_out, const char* fn) {
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  const int rc = device_ptr_ok(c, dF_out, fn, "f_out");
+  if (rc != SGP_OK) return rc;
+  SGP_CUDA(c, launch_ungroup_experts(dF_out, m.f, m.rows, m.experts, c->stream));
+  c->launches += 1;
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  return SGP_OK;
+}
+}  // namespace
 
 int sgp_experts_get_f_fold_slot(sgp_ctx* h, int32_t set, int32_t mode_slot, double* f_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
-  const double* f = nullptr;
-  long long n_k = 0, E_k = 0;
-  const int rc = fold_slot_modes(c, set, mode_slot, f_out, "sgp_experts_get_f_fold_slot", &f, &n_k, &E_k);
-  if (rc != SGP_OK) return rc;
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  SGP_CUDA(c, cudaMemcpyAsync(f_out, f, static_cast<size_t>(n_k) * 8, cudaMemcpyDeviceToHost, c->stream));
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  return SGP_OK;
+  return copy_modes(c, kModesFold, mode_slot, set, f_out, "sgp_experts_get_f_fold_slot");
 }
 
 int sgp_experts_get_f_fold_rows_device(sgp_ctx* h, int32_t set, int32_t mode_slot, double* dF_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
-  const double* f = nullptr;
-  long long n_k = 0, E_k = 0;
-  int rc = fold_slot_modes(c, set, mode_slot, dF_out, "sgp_experts_get_f_fold_rows_device", &f, &n_k, &E_k);
-  if (rc != SGP_OK) return rc;
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  rc = device_ptr_ok(c, dF_out, "sgp_experts_get_f_fold_rows_device", "f_out");
-  if (rc != SGP_OK) return rc;
-  SGP_CUDA(c, launch_ungroup_experts(dF_out, f, n_k, E_k, c->stream));   // the set is grouped as a grouped upload
-  c->launches += 1;
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  return SGP_OK;
+  const char* fn = "sgp_experts_get_f_fold_rows_device";
+  Modes m;
+  const int rc = find_modes(c, kModesFold, mode_slot, set, dF_out, fn, m);
+  return rc != SGP_OK ? rc : ungroup_modes(c, m, dF_out, fn);
 }
 
 int sgp_experts_get_f_slot(sgp_ctx* h, int32_t mode_slot, double* f_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
-  if (c->ex.E == 0 || !f_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
-  if (c->ex_mode_slots == 0)
-    return fail(c, SGP_E_STATE, "no slot modes: sgp_laplace_nll_slots_any_size has not run since the upload");
-  if (mode_slot < 0 || mode_slot >= c->ex_mode_slots)
-    return fail(c, SGP_E_BADARG, "sgp_experts_get_f_slot: mode slot outside [0, n_mode_slots)");
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  SGP_CUDA(c, cudaMemcpyAsync(f_out, c->ex_fm.as<double>() + static_cast<size_t>(mode_slot) * c->ex.n,
-                              static_cast<size_t>(c->ex.n) * 8, cudaMemcpyDeviceToHost, c->stream));
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  return SGP_OK;
+  return copy_modes(c, SGP_MODES_SLOT, mode_slot, 0, f_out, "sgp_experts_get_f_slot");
 }
 
 int sgp_experts_get_f_class(sgp_ctx* h, int32_t cls, double* f_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
-  if (c->ex.E == 0 || !f_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
-  if (c->ex_classes == 0) return fail(c, SGP_E_STATE, "no class modes: sgp_laplace_nll_classes has not run since the upload");
-  if (cls < 0 || cls >= c->ex_classes) return fail(c, SGP_E_BADARG, "sgp_experts_get_f_class: class index out of range");
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  SGP_CUDA(c, cudaMemcpyAsync(f_out, c->ex_fc.as<double>() + static_cast<size_t>(cls) * c->ex.n,
-                              static_cast<size_t>(c->ex.n) * 8, cudaMemcpyDeviceToHost, c->stream));
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  return SGP_OK;
+  return copy_modes(c, SGP_MODES_CLASS, cls, 0, f_out, "sgp_experts_get_f_class");
 }
 
 int sgp_experts_get_f(sgp_ctx* h, double* f_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
-  if (c->ex.E == 0 || !f_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  SGP_CUDA(c, cudaMemcpyAsync(f_out, c->ex.f, static_cast<size_t>(c->ex.n) * 8, cudaMemcpyDeviceToHost, c->stream));
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  return SGP_OK;
+  return copy_modes(c, SGP_MODES_BINARY, 0, 0, f_out, "sgp_experts_get_f");
 }
 
 int sgp_experts_get_f_rows_device(sgp_ctx* h, int32_t store, int32_t index, double* dF_out) {
   Ctx* c = reinterpret_cast<Ctx*>(h);
   if (!c) return SGP_E_BADARG;
+  const char* fn = "sgp_experts_get_f_rows_device";
   if (store != SGP_MODES_BINARY && store != SGP_MODES_CLASS && store != SGP_MODES_SLOT)
-    return fail(c, SGP_E_BADARG, "sgp_experts_get_f_rows_device: unknown mode store");
-  // the host getters' refusals, in their order and with their codes
-  if (c->ex.E == 0 || !dF_out) return fail(c, SGP_E_STATE, "sgp_experts_upload should have been called first");
-  const double* f = c->ex.f;
-  if (store == SGP_MODES_CLASS) {
-    if (c->ex_classes == 0) return fail(c, SGP_E_STATE, "no class modes: sgp_laplace_nll_classes has not run since the upload");
-    if (index < 0 || index >= c->ex_classes)
-      return fail(c, SGP_E_BADARG, "sgp_experts_get_f_rows_device: class index out of range");
-    f = c->ex_fc.as<double>() + static_cast<size_t>(index) * c->ex.n;
-  } else if (store == SGP_MODES_SLOT) {
-    if (c->ex_mode_slots == 0)
-      return fail(c, SGP_E_STATE, "no slot modes: sgp_laplace_nll_slots_any_size has not run since the upload");
-    if (index < 0 || index >= c->ex_mode_slots)
-      return fail(c, SGP_E_BADARG, "sgp_experts_get_f_rows_device: mode slot outside [0, n_mode_slots)");
-    f = c->ex_fm.as<double>() + static_cast<size_t>(index) * c->ex.n;
-  }
+    return fail(c, SGP_E_BADARG, std::string(fn) + ": unknown mode store");
+  Modes m;
+  const int rc = find_modes(c, store, index, 0, dF_out, fn, m);
+  if (rc != SGP_OK) return rc;
   if (!c->ex_grouped)
     return fail(c, SGP_E_STATE, "sgp_experts_get_f_rows_device: the experts were not uploaded by sgp_experts_upload_grouped "
                                 "or its _device form, so their rows have no row order");
-  SGP_CUDA(c, cudaSetDevice(c->device));
-  const int rc = device_ptr_ok(c, dF_out, "sgp_experts_get_f_rows_device", "f_out");
-  if (rc != SGP_OK) return rc;
-  SGP_CUDA(c, launch_ungroup_experts(dF_out, f, c->ex.n, c->ex.E, c->stream));
-  c->launches += 1;
-  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
-  return SGP_OK;
+  return ungroup_modes(c, m, dF_out, fn);
 }
 
 int sgp_last_path(const sgp_ctx* h) {

@@ -15,9 +15,9 @@
 // GPC:18), so Cholesky gives the same log-determinant and inverse (up to rounding) at a third of the work.  A
 // non-positive pivot is reported (the reference would return a negative-determinant "logdet" of |det| instead).
 //
-// Cross-validation (sgp_bcm_nll_folds): a second grid dimension runs several fold training sets of one fold upload in one
-// launch.  Block (x, s) evaluates expert x of the set listed in slot s with slot s's flattened kernel and hyper-parameter
-// block, output row [s][x]; the arithmetic is the single-set body's.
+// Slots (ObjectiveSlots): a second grid dimension runs several expert sets of the upload in one launch (sgp_bcm_nll is
+// one slot on the whole upload).  Block (x, s) evaluates expert x of the set listed in slot s with slot s's flattened
+// kernel and hyper-parameter block, output row [s][x]; the arithmetic does not depend on the slot.
 #include <cstdlib>
 #include <string>
 
@@ -505,18 +505,14 @@ cudaError_t launch_rows_reduce(double* dTotal, const double* dPerExpert, long lo
   return cudaGetLastError();
 }
 
-cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double* rows, double* total,
-                           int* flags, cudaStream_t s, const BcmFolds* folds) {
+cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, const ObjectiveSlots& sl,
+                           double* rows, double* total, int* flags, cudaStream_t s) {
   NllParams p{};
   p.X = ex.X; p.y = ex.y; p.off = ex.off; p.n_max = ex.n_max; p.x_in_smem = plan.x_in_smem;
-  p.hv = hv; p.out = rows; p.flags = flags;
-  long long E = ex.E;
-  int n_slots = 1;
-  if (folds) {
-    p.sets = folds->sets; p.first = folds->first; p.kf = folds->kf; p.slot_stride = folds->slot_stride;
-    E = folds->E_max;
-    n_slots = folds->n_slots;
-  }
+  p.hv = hv; p.sets = sl.sets; p.first = sl.first; p.kf = sl.kf; p.slot_stride = sl.slot_stride;
+  p.out = rows; p.flags = flags;
+  const long long E = sl.E_max;
+  const int n_slots = sl.n_slots;
   const bool reg = plan.variant < ObjectiveVariant::kSmem;
   void (*kernel)(NllParams) = reg ? kRegShapes[static_cast<int>(plan.variant)].kernel : bcm_nll_kernel;
   cudaError_t e = allow_dynamic_smem(reinterpret_cast<const void*>(kernel));

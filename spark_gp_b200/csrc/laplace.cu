@@ -8,16 +8,13 @@
 // before that iteration's update, while d3logP (GPCls:118, sign as in the reference) uses exp(-f) of the final f.
 // Summed over experts like commons/GaussianProcessCommons.scala:73-78.
 //
-// One-vs-rest (sgp_laplace_nll_classes) and param-map slots (sgp_laplace_nll_slots_any_size): a second grid dimension
-// runs several binary problems over the same experts in one launch.  Block (e, s) evaluates expert e for the s-th listed
-// slot, of class c and mode slot m: labels (y == c), modes f + m * n, its own flattened kernel and hyper-parameter
-// block, output row [s][e].  The classes entry passes m = c.  The arithmetic is the single-class body's, so a slot's
-// rows equal, bit for bit, those of a single-class launch on an upload of the labels (y == c) with the same modes.
-//
-// Fold slots (sgp_laplace_nll_fold_slots_any_size): slot s also names a training set of a fold upload.  Block (x, s) is
-// expert first[sets[s]] + x (a block past the set's expert count returns before its first barrier), its modes are indexed
-// from the set's first row, and its output row is [s][x].  n_max and x_in_smem only move addresses: every loop runs over
-// the expert's own n, so a slot's rows equal those of a launch on an upload of that set alone.
+// Slots (ObjectiveSlots): a second grid dimension runs several binary problems in one launch (sgp_laplace_nll is one
+// slot on the whole upload, its labels as uploaded).  Block (x, s) evaluates expert first[sets[s]] + x for the s-th
+// listed slot, of class c and mode slot m: labels (y == c) (c < 0: as uploaded), modes f + m * f_stride indexed from the
+// set's first row, its own flattened kernel and hyper-parameter block, output row [s][x]; a block past the set's expert
+// count returns before its first barrier.  The one-vs-rest entries pass m = c.  The arithmetic does not depend on the
+// slot, and n_max and x_in_smem only move addresses: every loop runs over the expert's own n.  So a slot's rows equal,
+// bit for bit, those of a one-slot launch on an upload of the labels (y == c) of that set alone with the same modes.
 #include "expert_common.cuh"
 
 namespace sgp {
@@ -29,13 +26,13 @@ struct LapParams {
   const double* X; const double* y; double* f; const long long* off;
   int n_max, x_in_smem;
   HyperView hv;              // slot 0's view; slot s reads kf[s] and the descriptor values s * slot_stride doubles on
-  const int* cls;            // [n_slots] class of each slot (one-vs-rest), or nullptr: one slot, labels as uploaded
-  const int* mode;           // [n_slots] mode slot of each slot: its modes are f + mode[s] * n (with cls)
-  const KernelFlat* kf;      // [n_slots] flattened kernel of each slot (with cls)
-  long long slot_stride;     // doubles between two slots' [beta | coef | value] blocks (with cls)
-  long long n;               // the stride of the per-slot modes f (with cls)
-  const int* sets;           // [n_slots] fold set of each slot (with cls), or nullptr: every slot over every expert
-  const long long* first;    // [n_sets + 1] first expert of each fold set (with sets)
+  const int* cls;            // [n_slots] class of each slot (one-vs-rest); < 0: labels as uploaded
+  const int* mode;           // [n_slots] mode slot of each slot: its modes are f + mode[s] * n
+  const KernelFlat* kf;      // [n_slots] flattened kernel of each slot
+  long long slot_stride;     // doubles between two slots' [beta | coef | value] blocks
+  long long n;               // the stride of the per-slot modes f
+  const int* sets;           // [n_slots] expert set of each slot
+  const long long* first;    // [n_sets + 1] first expert of each set
   double tol;
   double* out;               // [n_slots][E][1 + n_hypers]  (-logZ, -gradLogZ)
   int* flags;                // [n_slots]  bit 0: Cholesky pivot not positive
@@ -70,25 +67,18 @@ __global__ void __launch_bounds__(LT, 1) laplace_kernel(const LapParams p) {
   extern __shared__ double sm[];
   long long e = blockIdx.x;
   const int slot = blockIdx.y;
-  long long fr = 0;                                      // row of the modes that belong to the set's first row
-  if (p.sets) {
-    const long long first = p.first[p.sets[slot]];
-    if (e >= p.first[p.sets[slot] + 1] - first) return;
-    e += first;
-    fr = p.off[first];
-  }
+  const long long first = p.first[p.sets[slot]];
+  if (e >= p.first[p.sets[slot] + 1] - first) return;
+  e += first;
+  const long long fr = p.off[first];                    // row of the modes that belong to the set's first row
   const long long r0 = p.off[e];
   const int n = static_cast<int>(p.off[e + 1] - r0);
   const int ld = p.n_max + 1;
   HyperView hv = p.hv;
-  double* fg = p.f;
-  double cls = -1.0;                                     // < 0: labels as uploaded
-  if (p.cls) {
-    cls = p.cls[slot];
-    fg += static_cast<size_t>(p.mode[slot]) * p.n;
-    hv.kf = p.kf[slot];
-    hv.beta += slot * p.slot_stride; hv.h_coef += slot * p.slot_stride; hv.h_value += slot * p.slot_stride;
-  }
+  const double cls = p.cls[slot];                        // < 0: labels as uploaded
+  double* fg = p.f + static_cast<size_t>(p.mode[slot]) * p.n;
+  hv.kf = p.kf[slot];
+  hv.beta += slot * p.slot_stride; hv.h_coef += slot * p.slot_stride; hv.h_value += slot * p.slot_stride;
   fg += r0 - fr;                                         // the expert's modes
   double* K = sm;                                        // full symmetric
   double* M = K + static_cast<size_t>(p.n_max) * ld;     // B -> L -> L^-1 -> B^-1 (lower)
@@ -213,19 +203,14 @@ size_t laplace_smem_bytes(int n_max) {
   return sizeof(double) * (2 * static_cast<size_t>(n_max) * (n_max + 1) + 12 * static_cast<size_t>(n_max) + 8 + EX_SUMS);
 }
 
-cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol, double* rows,
-                           double* total, int* flags, cudaStream_t s, const LaplaceClasses* classes) {
+cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol,
+                           const ObjectiveSlots& sl, double* rows, double* total, int* flags, cudaStream_t s) {
   LapParams p{};
-  p.X = ex.X; p.y = ex.y; p.f = ex.f; p.off = ex.off; p.n_max = ex.n_max; p.x_in_smem = plan.x_in_smem;
-  p.hv = hv; p.n = ex.n; p.tol = tol; p.out = rows; p.flags = flags;
-  int n_slots = 1;
-  long long E = ex.E;
-  if (classes) {
-    p.f = classes->f; p.cls = classes->cls; p.mode = classes->mode; p.kf = classes->kf; p.slot_stride = classes->slot_stride;
-    p.n = classes->f_stride; p.sets = classes->sets; p.first = classes->first;
-    n_slots = classes->n_slots;
-    if (classes->sets) E = classes->E_max;
-  }
+  p.X = ex.X; p.y = ex.y; p.f = sl.f; p.off = ex.off; p.n_max = ex.n_max; p.x_in_smem = plan.x_in_smem;
+  p.hv = hv; p.cls = sl.cls; p.mode = sl.mode; p.kf = sl.kf; p.slot_stride = sl.slot_stride; p.n = sl.f_stride;
+  p.sets = sl.sets; p.first = sl.first; p.tol = tol; p.out = rows; p.flags = flags;
+  const int n_slots = sl.n_slots;
+  const long long E = sl.E_max;
   cudaError_t e = allow_dynamic_smem(reinterpret_cast<const void*>(laplace_kernel));
   if (e != cudaSuccess) return e;
   laplace_kernel<<<dim3(static_cast<unsigned>(E), static_cast<unsigned>(n_slots)), LT, plan.smem, s>>>(p);

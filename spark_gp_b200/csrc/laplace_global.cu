@@ -15,8 +15,8 @@
 //   - the level-2 steps (K b, the two triangular solves, K a, K s2, R t1) stay on the CUDA cores.
 // Every sum has a fixed order and the tiling depends on the expert's own n only, so a work item's bits do not depend on
 // the CTA that runs it, the grid size, n_max or the other experts and slots of the launch.
-// Fold slots (sgp_laplace_nll_fold_slots_any_size): item (s, x) is expert first[sets[s]] + x of slot s's training set
-// (items past the set's expert count are skipped), its modes are indexed from the set's first row, its row is [s][x].
+// Slots as laplace_kernel's: item (s, x) is expert first[sets[s]] + x of slot s's set (items past the set's expert count
+// are skipped), its modes are indexed from the set's first row, its row is [s][x].
 #include "expert_common.cuh"
 
 namespace sgp {
@@ -37,17 +37,17 @@ __host__ __device__ constexpr size_t lg_cta_doubles(int ld) {
 
 struct LapGlobalParams {
   const double* X; const double* y; double* f; const long long* off;
-  long long E;               // experts per slot (with sets: the largest expert count over the listed sets)
+  long long E;               // experts per slot: the largest expert count over the listed sets
   int n_slots;
   int ldw;                   // workspace row stride: n_max rounded up to NB
   HyperView hv;              // slot 0's view (as laplace_kernel's)
-  const int* cls;            // [n_slots] or nullptr
-  const int* mode;           // [n_slots] mode slot of each slot (with cls)
-  const KernelFlat* kf;      // [n_slots] (with cls)
-  long long slot_stride;     // (with cls)
-  long long n;               // stride of the per-slot modes (with cls)
-  const int* sets;           // [n_slots] fold set of each slot (with cls), or nullptr
-  const long long* first;    // [n_sets + 1] first expert of each fold set (with sets)
+  const int* cls;            // [n_slots] class of each slot; < 0: labels as uploaded
+  const int* mode;           // [n_slots] mode slot of each slot
+  const KernelFlat* kf;      // [n_slots]
+  long long slot_stride;
+  long long n;               // stride of the per-slot modes
+  const int* sets;           // [n_slots] expert set of each slot
+  const long long* first;    // [n_sets + 1] first expert of each set
   double tol;
   double* ws;                // [gridDim.x][lg_cta_doubles(ldw)]
   double* out;               // [n_slots][E][1 + n_hypers]
@@ -397,25 +397,19 @@ __global__ void __launch_bounds__(GT, 1) laplace_global_kernel(const LapGlobalPa
   const long long items = p.E * p.n_slots;
   for (long long w = blockIdx.x; w < items; w += gridDim.x) {
     const int slot = static_cast<int>(w / p.E);
-    long long e = w % p.E, fr = 0;                       // fr: row of the modes that belong to the set's first row
-    if (p.sets) {
-      const long long first = p.first[p.sets[slot]];
-      if (e >= p.first[p.sets[slot] + 1] - first) continue;   // the whole CTA skips the item
-      e += first;
-      fr = p.off[first];
-    }
+    long long e = w % p.E;
+    const long long first = p.first[p.sets[slot]];
+    if (e >= p.first[p.sets[slot] + 1] - first) continue;   // the whole CTA skips the item
+    e += first;
+    const long long fr = p.off[first];                   // row of the modes that belong to the set's first row
     const long long r0 = p.off[e];
     const int n = static_cast<int>(p.off[e + 1] - r0);
     const int np = (n + NB - 1) / NB * NB;
     HyperView hv = p.hv;
-    double* fg = p.f;
-    double cls = -1.0;                                   // < 0: labels as uploaded
-    if (p.cls) {
-      cls = p.cls[slot];
-      fg += static_cast<size_t>(p.mode[slot]) * p.n;
-      hv.kf = p.kf[slot];
-      hv.beta += slot * p.slot_stride; hv.h_coef += slot * p.slot_stride; hv.h_value += slot * p.slot_stride;
-    }
+    const double cls = p.cls[slot];                      // < 0: labels as uploaded
+    double* fg = p.f + static_cast<size_t>(p.mode[slot]) * p.n;
+    hv.kf = p.kf[slot];
+    hv.beta += slot * p.slot_stride; hv.h_coef += slot * p.slot_stride; hv.h_value += slot * p.slot_stride;
     const double* Xe = p.X + static_cast<size_t>(r0) * hv.d;
     __syncthreads();                                     // the previous item is done with the workspace
     for (int i = tid; i < np; i += GT) {
@@ -533,16 +527,11 @@ long long laplace_global_grid(long long items, long long resident, size_t cta_by
 }
 
 cudaError_t launch_laplace_global(const ExpertSet& ex, const HyperView& hv, double tol, double* ws, long long grid,
-                                  double* rows, double* total, int* flags, cudaStream_t s,
-                                  const LaplaceClasses* classes) {
+                                  const ObjectiveSlots& sl, double* rows, double* total, int* flags, cudaStream_t s) {
   LapGlobalParams p{};
-  p.X = ex.X; p.y = ex.y; p.f = ex.f; p.off = ex.off; p.E = ex.E; p.n_slots = 1; p.ldw = lg_ld(ex.n_max);
-  p.hv = hv; p.n = ex.n; p.tol = tol; p.ws = ws; p.out = rows; p.flags = flags;
-  if (classes) {
-    p.f = classes->f; p.cls = classes->cls; p.mode = classes->mode; p.kf = classes->kf; p.slot_stride = classes->slot_stride;
-    p.n_slots = classes->n_slots; p.n = classes->f_stride; p.sets = classes->sets; p.first = classes->first;
-    if (classes->sets) p.E = classes->E_max;
-  }
+  p.X = ex.X; p.y = ex.y; p.f = sl.f; p.off = ex.off; p.E = sl.E_max; p.n_slots = sl.n_slots; p.ldw = lg_ld(ex.n_max);
+  p.hv = hv; p.cls = sl.cls; p.mode = sl.mode; p.kf = sl.kf; p.slot_stride = sl.slot_stride; p.n = sl.f_stride;
+  p.sets = sl.sets; p.first = sl.first; p.tol = tol; p.ws = ws; p.out = rows; p.flags = flags;
   laplace_global_kernel<<<static_cast<unsigned>(grid), GT, 0, s>>>(p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;

@@ -116,6 +116,12 @@ struct ExpertSet {
   int d = 0, n_max = 0;       // n_max: largest expert
 };
 
+// Latent modes of the Laplace objective for `slots` mode slots (0: none since the last upload).
+struct ModeStore {
+  DevScratch buf;
+  int slots = 0;
+};
+
 struct Ctx {
   int device = 0;
   int precision = SGP_PREC_AUTO;
@@ -171,21 +177,18 @@ struct Ctx {
   long long i8_points = 0;       // points that went through the int8 kernel since begin
   // per-expert objective state
   ExpertSet ex;                  // view of ex_X, ex_y, ex_off, ex_f; E > 0 once an upload has completed
-  DevScratch ex_X, ex_y, ex_off, ex_f;
-  DevScratch ex_fc;              // one-vs-rest latent modes [ex_classes][n] (sgp_laplace_nll_classes)
-  int ex_classes = 0;            // classes ex_fc holds modes for; 0: none since the last upload
-  DevScratch ex_fm;              // param-map latent modes [ex_mode_slots][n] (sgp_laplace_nll_slots_any_size)
-  int ex_mode_slots = 0;         // mode slots ex_fm holds modes for; 0: none since the last upload
-  DevScratch ex_ffm;             // fold-slot latent modes [ex_fold_mode_slots][largest set's rows]
+  DevScratch ex_X, ex_y, ex_off;
+  ModeStore ex_f;                // the binary objectives' latent modes: one slot of n (ex.f), zeroed by every upload
+  ModeStore ex_fc;               // one-vs-rest latent modes [classes][n] (sgp_laplace_nll_classes)
+  ModeStore ex_fm;               // param-map latent modes [mode slots][n] (sgp_laplace_nll_slots_any_size)
+  ModeStore ex_ffm;              // fold-slot latent modes [mode slots][largest set's rows]
                                  // (sgp_laplace_nll_fold_slots_any_size), indexed from each set's first row
-  int ex_fold_mode_slots = 0;    // mode slots ex_ffm holds modes for; 0: none since the last upload
   bool ex_grouped = false;       // ex came from a grouped upload (point i -> expert i % E): its modes can be ungrouped
   // fold upload (sgp_experts_upload_folds): the training sets lie one after another in ex; set k owns the experts
   // fold_first[k] .. fold_first[k+1]-1.  Empty after any other upload.
   std::vector<long long> fold_first;   // [n_sets + 1]
   std::vector<int> fold_nmax;          // [n_sets] largest expert of each set
   std::vector<long long> fold_row0;    // [n_sets + 1] first row of each set
-  DevScratch ex_set_first;             // device copy of fold_first; {0, E} after a grouped upload (one set)
   DevScratch fold_pos_ws;              // upload scratch: the point indices grouped by fold, ascending in each fold
   DevScratch nll_per_ws;         // per-expert objective rows
   DevScratch hyper_ws;           // hyper-parameter descriptors + totals + flags of one evaluation
@@ -401,54 +404,39 @@ ObjectivePlan plan_objective(Objective kind, const ExpertSet& ex, int n_terms);
 size_t laplace_smem_bytes(int n_max);   // laplace_kernel without the staged rows (laplace.cu)
 size_t laplace_global_cta_bytes(int n_max);   // laplace_global_kernel's workspace per CTA (laplace_global.cu)
 
-// Fold slots of a BCM launch (sgp_bcm_nll_folds; sgp_bcm_nll_slots lists set 0 of a grouped upload's {0, E}): slot s evaluates the experts first[sets[s]] .. first[sets[s] + 1] - 1
-// of a fold upload with the flattened kernel kf[s] and the descriptor values slot_stride doubles per slot after hv's.
-// rows: [n_slots][E_max][1 + n_hypers], total: [n_slots][1 + n_hypers], flags: [n_slots].
-struct BcmFolds {
+// The slots of a per-expert objective launch (objective_setup in api.cu).  Every objective entry is a list of slots over
+// expert sets of the upload: slot s evaluates the experts first[sets[s]] .. first[sets[s] + 1] - 1 (the whole upload is
+// the one set {0, E}) with the flattened kernel kf[s] and the descriptor values slot_stride doubles per slot after hv's.
+// The Laplace objective adds the labels (y == cls[s]) (cls[s] < 0: the labels as uploaded) and the modes
+// f + mode[s] * f_stride, indexed from the set's first row.  rows: [n_slots][E_max][1 + n_hypers], total:
+// [n_slots][1 + n_hypers], flags: [n_slots].
+struct ObjectiveSlots {
   int n_slots = 0;
-  long long E_max = 0;                // the largest expert count over the listed sets
   const int* sets = nullptr;          // device, [n_slots]
   const long long* first = nullptr;   // device, [n_sets + 1]
+  long long E_max = 0;                // the largest expert count over the slots' sets
   const KernelFlat* kf = nullptr;     // device, [n_slots]
   long long slot_stride = 0;
+  const int* cls = nullptr;           // device, [n_slots] (Laplace)
+  const int* mode = nullptr;          // device, [n_slots], distinct (Laplace)
+  double* f = nullptr;                // device, [n_mode_slots][f_stride] (Laplace)
+  long long f_stride = 0;             // modes per mode slot: the uploaded points, or the largest fold set's rows
 };
-// Each launcher runs the planned kernel and sums the per-expert rows [E][1 + n_hypers] into total.
-// folds == nullptr: one slot over every uploaded expert (sgp_bcm_nll)
-cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double* rows, double* total,
-                           int* flags, cudaStream_t s, const BcmFolds* folds = nullptr);
-// ws: plan.lu_ws bytes.  cuBLAS failures are reported through *blas_status.
+// Each launcher runs the planned kernel over experts x slots and sums each slot's per-expert rows into total.
+cudaError_t launch_bcm_nll(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, const ObjectiveSlots& sl,
+                           double* rows, double* total, int* flags, cudaStream_t s);
+// The LU path on one set (ex: the set alone).  ws: plan.lu_ws bytes.  cuBLAS failures are reported through *blas_status.
 cudaError_t launch_bcm_nll_general(const ObjectivePlan& plan, cublasHandle_t blas, int* blas_status, void* ws,
                                    const ExpertSet& ex, const HyperView& hv, double* rows, double* total, int* flags,
                                    cudaStream_t s);
-// Slots of a Laplace launch (sgp_laplace_nll_classes*, sgp_laplace_nll_slots_any_size, sgp_laplace_nll_fold_slots_any_size):
-// slot s evaluates class cls[s]
-// with the labels (y == cls[s]), the modes f + mode[s] * n, the flattened kernel kf[s] and the descriptor values
-// slot_stride doubles per slot after hv's.  The classes entries pass mode = cls.  rows: [n_slots][E][1 + n_hypers],
-// total: [n_slots][1 + n_hypers], flags: [n_slots].
-struct LaplaceClasses {
-  int n_slots = 0;
-  const int* cls = nullptr;           // device, [n_slots]
-  const int* mode = nullptr;          // device, [n_slots], distinct
-  const KernelFlat* kf = nullptr;     // device, [n_slots]
-  long long slot_stride = 0;
-  double* f = nullptr;                // device, [n_mode_slots][f_stride]
-  long long f_stride = 0;             // modes per mode slot: the uploaded points, or the largest fold set's rows
-  // fold slots (sgp_laplace_nll_fold_slots_any_size): slot s evaluates the experts first[sets[s]] .. first[sets[s] + 1] - 1
-  // of a fold upload, its modes indexed from the set's first row; rows [n_slots][E_max][1 + n_hypers]
-  const int* sets = nullptr;          // device, [n_slots], or nullptr: every slot over every uploaded expert
-  const long long* first = nullptr;   // device, [n_sets + 1]
-  long long E_max = 0;                // the largest expert count over the slots' sets
-};
-// classes == nullptr: one slot on the labels and modes as uploaded (sgp_laplace_nll)
-cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol, double* rows,
-                           double* total, int* flags, cudaStream_t s, const LaplaceClasses* classes = nullptr);
+cudaError_t launch_laplace(const ObjectivePlan& plan, const ExpertSet& ex, const HyperView& hv, double tol,
+                           const ObjectiveSlots& sl, double* rows, double* total, int* flags, cudaStream_t s);
 // The global-memory kernel (plan kLaplaceGlobal) on `grid` CTAs, CTA b on the slice ws + b * plan.cta_ws.  The grid
-// is laplace_global_grid(E * n_slots, laplace_global_ctas_per_sm() * SMs, plan.cta_ws, workspace budget).
+// is laplace_global_grid(E_max * n_slots, laplace_global_ctas_per_sm() * SMs, plan.cta_ws, workspace budget).
 int laplace_global_ctas_per_sm();
 long long laplace_global_grid(long long items, long long resident, size_t cta_bytes, size_t budget);
 cudaError_t launch_laplace_global(const ExpertSet& ex, const HyperView& hv, double tol, double* ws, long long grid,
-                                  double* rows, double* total, int* flags, cudaStream_t s,
-                                  const LaplaceClasses* classes = nullptr);
+                                  const ObjectiveSlots& sl, double* rows, double* total, int* flags, cudaStream_t s);
 
 int ctx_scratch(Ctx* c, DevScratch& s, size_t bytes);
 // X and y below are host memory, or device memory on the context's device where x_on_device is set (the _device entries)
