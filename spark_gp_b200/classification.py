@@ -5,8 +5,8 @@ from __future__ import annotations
 import numpy as np
 
 from . import _native as N
-from .engine import ProjectedProcessEngine, device_fit_data, is_cuda_tensor
-from .hyperopt import group_for_experts, lbfgsb_bounds, optimise_slots
+from .engine import ProjectedProcessEngine, is_cuda_tensor
+from .hyperopt import each, expert_count, fit_data, fit_slots, own_context, produce, slot_modes, slot_objective
 from .regression import GaussianProcessParams, GaussianProjectedProcessRawPredictor
 
 
@@ -16,6 +16,12 @@ class GaussianProcessClassificationModel:
     def __init__(self, rawPredictor: GaussianProjectedProcessRawPredictor, hyperparameters):
         self.rawPredictor, self.hyperparameters = rawPredictor, hyperparameters
         self.numClasses = 2
+
+    @classmethod
+    def of(cls, fitted):
+        """The model of a fitted slot (`hyperopt.Fitted`), on the context that holds its active set and magic pair."""
+        return cls(GaussianProjectedProcessRawPredictor(fitted.engine, fitted.magic_vector, fitted.magic_matrix,
+                                                        fitted.kernel, fitted.active_set), fitted.theta)
 
     def predictRaw(self, features):
         """(-f, f) per row (GPCls:153-156).  A CUDA torch tensor stays on the device (CUDA float64 result)."""
@@ -55,11 +61,7 @@ class GaussianProcessClassificationModel:
         """ClassificationModel.predict = raw2prediction(predictRaw(x)); with no thresholds set (the reference sets none)
         Spark's ProbabilisticClassificationModel.raw2prediction is `rawPrediction.argmax`, i.e. class 1 iff f > 0 (first
         maximum on a tie) -- NOT the argmax of the (quirky) probability vector."""
-        raw = self.predictRaw(features)
-        if is_cuda_tensor(raw):
-            import torch
-            return torch.argmax(raw, dim=-1).to(torch.float64)
-        return np.argmax(raw, axis=-1).astype(np.float64)
+        return binary_prediction(self.predictRaw(features))
 
 
 class GaussianProcessClassifier(GaussianProcessParams):
@@ -81,33 +83,22 @@ class GaussianProcessClassifier(GaussianProcessParams):
         rows of this rank's experts, in global row order."""
         if self._process_group is not None:
             from . import distributed
-            eng, kernel, theta, active_set, mv, mm, self.last_stats, self.last_latent = distributed.fit(
-                self, X, y, hyperparameters, True)
-            return GaussianProcessClassificationModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, active_set),
-                                                      theta)
+            fitted = distributed.fit(self, X, y, hyperparameters, True)
+            self.last_stats, self.last_latent = fitted.stats, fitted.latent
+            return GaussianProcessClassificationModel.of(fitted)
         X, y = fit_data(X, y, self._device, "GaussianProcessClassifier.fit")
         assert_labels_are_01(y)
         eng = ProjectedProcessEngine.acquire(self._device)
         (theta,), (f,), fit = laplace_fit(
-            self, eng, X, y, binary_objective(self, eng), N.SGP_MODES_BINARY, lambda _: 0,
-            [self.getKernel().getHyperparameters()],
+            [self], eng, X, y, each(lambda k: eng.laplace_nll_any_size(k, self._tol)), N.SGP_MODES_BINARY, lambda _: 0,
             None if hyperparameters is None else [np.asarray(hyperparameters, dtype=np.float64)])
         if fit["slots"] is not None:
             self.last_objective = dict(fit["slots"][0], launches=fit["launches"])
         self.last_latent = f
         # GPCls:62-65 -> produceModel with (f, kernel): the same projected-process path as regression
-        kernel, active_set, mv, mm, self.last_stats = _produce_model(self, eng, X, f, theta)
-        return GaussianProcessClassificationModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, active_set), theta)
-
-
-def fit_data(X, y, device: int, what: str):
-    """The (X, y) of a classifier fit: X as float64 (the classifiers read float64 points) and y float64, on the host, or on
-    the device for a CUDA tensor X (`device_fit_data`)."""
-    if is_cuda_tensor(X):
-        import torch
-        X, y = device_fit_data(X, y, device, what)
-        return X.to(torch.float64), y
-    return np.asarray(X, dtype=np.float64), np.asarray(y, dtype=np.float64)
+        fitted = produce(self, eng, X, f, theta)
+        self.last_stats = fitted.stats
+        return GaussianProcessClassificationModel.of(fitted)
 
 
 def assert_labels_are_01(y):
@@ -116,71 +107,24 @@ def assert_labels_are_01(y):
         raise RuntimeError("Only 0 and 1 labels are supported.")
 
 
-def binary_objective(gp, eng):
-    """The binary classifier's objective for `laplace_optimise`: `laplace_nll_any_size` of each listed slot on eng."""
-    return lambda batch: [eng.laplace_nll_any_size(gp.getKernel().setHyperparameters(t), gp._tol) for _, t in batch]
-
-
-def classes_objective(gp, eng, n_classes: int):
-    """One-vs-rest's objective for `laplace_optimise` (slot c: class c): every listed class in one
-    `laplace_nll_classes_any_size` launch on eng."""
-    kernel_at = lambda t: gp.getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
-
-    def objective(batch):
-        vals, grads = eng.laplace_nll_classes_any_size(n_classes, [c for c, _ in batch], [kernel_at(t) for _, t in batch],
-                                                       gp._tol)
-        return [(float(v), g) for v, g in zip(vals, grads)]
-    return objective
-
-
-def laplace_fit(gp, eng, X, y, objective, store, index, x0s, thetas=None):
-    """The Laplace part of the binary fit (GPCls:53-60) for every slot of the caller, on one upload of (X, y) into eng,
-    grouped into experts by gp's datasetSizeForExpert (every slot's modes start at 0).
-      objective([(i, theta_i), ...]) -> [(value, gradient), ...]: slot i's Laplace objective at theta_i, warm-started from
-                                        and moving its device-resident modes;
-      store, index(i):                  where slot i's modes live (N.SGP_MODES_*, and the class or mode slot).
-    The slots are fitted by `laplace_optimise`.  Returns (thetas, modes [slot][row] in row order -- a CUDA float64 tensor,
-    ungrouped on the device, when X is a CUDA tensor --, the fit record of `laplace_optimise`)."""
-    order = np.concatenate(group_for_experts(len(X), gp._datasetSizeForExpert))
-    eng.experts_upload_grouped(X, y, gp._datasetSizeForExpert)
-    thetas, fit = laplace_optimise(gp, eng, objective, x0s, thetas)
+def laplace_fit(gps, eng, X, y, entry, store, index, thetas=None):
+    """The Laplace part of the binary fit (GPCls:53-60) for slot i of classifier gps[i], on one upload of (X, y) into eng
+    grouped by gps[0]'s datasetSizeForExpert (every slot's modes start at 0), fitted by `fit_slots` from each classifier's
+    kernel with gps[0]'s bounds, maxIter and tol.
+      entry(slots, kernels) -> (values, gradients): the listed slots' Laplace objective (`slot_objective`), warm-started
+                                                    from and moving their device-resident modes;
+      store, index(i):                              where slot i's modes live (N.SGP_MODES_*, and the class or mode slot).
+    Returns (thetas, modes [slot][row] in row order -- a CUDA float64 tensor, ungrouped on the device, when X is a CUDA
+    tensor --, the fit record of `fit_slots`)."""
+    n_experts = expert_count(len(X), gps[0]._datasetSizeForExpert)
+    eng.experts_upload_grouped(X, y, gps[0]._datasetSizeForExpert)
+    thetas, fit = fit_slots(eng, gps[0], slot_objective(gps, entry), [gp.getKernel().getHyperparameters() for gp in gps],
+                            thetas, laplace=True)
+    latent = [slot_modes(eng, is_cuda_tensor(X), len(X), n_experts, store, index(i)) for i in range(len(gps))]
     if is_cuda_tensor(X):
         import torch
-        return thetas, torch.stack([eng.experts_modes_rows(store, index(i), len(X)) for i in range(len(thetas))]), fit
-    latent = np.empty((len(thetas), len(X)))
-    for i in range(len(thetas)):
-        latent[i, order] = eng.experts_modes(store, index(i), len(X))
-    return thetas, latent, fit
-
-
-def laplace_optimise(gp, eng, objective, x0s, thetas=None):
-    """The slots' hyper-parameters on the experts already uploaded into eng (`objective` as for `laplace_fit`).  Unless
-    `thetas` are given, every slot is optimised from x0s (`optimise_slots`; skipped when there are no hyper-parameters).
-    Then the Laplace loop runs once more at every slot's theta (GPCls:60), so that its modes are the modes at theta.
-    Returns (thetas, dict(slots: each slot's optimisation record or None when nothing was optimised, rounds, launches:
-    the optimisation's, launches_total: with the call at theta))."""
-    launches0 = eng.launch_count()
-    records, rounds = None, 0
-    if thetas is None:
-        thetas = [np.asarray(x0, dtype=np.float64) for x0 in x0s]
-        if len(thetas[0]) > 0:
-            thetas, records, rounds = optimise_slots(objective, x0s, lbfgsb_bounds(gp.getKernel()), gp._maxIter, gp._tol)
-    launches = eng.launch_count() - launches0
-    objective(list(enumerate(thetas)))
-    return thetas, dict(slots=records, rounds=rounds, launches=launches, launches_total=eng.launch_count() - launches0)
-
-
-def _produce_model(gp, eng, X, f, theta):
-    """GPCls:62-65: the active set, the statistics with y := f and the tail, on eng.  Returns (kernel, active set, magic
-    vector, magic matrix, (G, b))."""
-    # every model starts from the default precision, as on a freshly acquired context: a fallback to F64 in one slot's
-    # statistics must not decide the next slot's path
-    eng.set_precision(N.SGP_PREC_AUTO)
-    active_set = gp._activeSetProvider(gp._activeSetSize, X, f, gp.getKernel, theta, gp._seed, gp=gp)
-    kernel = gp.getKernel().setHyperparameters(theta)
-    G, b = eng.statistics(kernel, active_set, X, f)                 # same helper as regression (fp64-kernel fallback)
-    mv, mm = eng.magic()
-    return kernel, active_set, mv, mm, (G, b)
+        return thetas, torch.stack(latent), fit
+    return thetas, np.stack(latent), fit
 
 
 # ---- one-vs-rest ------------------------------------------------------------------------------------------------------
@@ -212,6 +156,15 @@ def one_vs_rest_labels(y):
     if not bool((fin(y) & (y >= 0.0) & (y == floor(y))).all()):
         raise ValueError("OneVsRest: labels must be non-negative integers (class indices)")
     return y, int(y.max()) + 1
+
+
+def binary_prediction(raw):
+    """The binary classifier's prediction from its n x 2 raw matrix (-f, f): Spark's raw2prediction, `rawPrediction.argmax`
+    (class 1 iff f > 0, the first maximum on a tie), as float64 class indices."""
+    if is_cuda_tensor(raw):
+        import torch
+        return torch.argmax(raw, dim=-1).to(torch.float64)
+    return np.argmax(raw, axis=-1).astype(np.float64)
 
 
 def one_vs_rest_prediction(raw):
@@ -310,22 +263,17 @@ class OneVsRest:
             eng.release()
 
     def _fit(self, gp, eng, X, y, C, hyperparameters):
-        x0 = gp.getKernel().getHyperparameters()
-        given = None if hyperparameters is None else np.array(hyperparameters, dtype=np.float64).reshape(C, len(x0))
-        thetas, latent, fit = laplace_fit(gp, eng, X, y, classes_objective(gp, eng, C), N.SGP_MODES_CLASS, lambda c: c,
-                                          [x0] * C, given)
-        thetas = np.array(thetas).reshape(C, len(x0))
+        n_hypers = len(gp.getKernel().getHyperparameters())
+        given = None if hyperparameters is None else np.array(hyperparameters, dtype=np.float64).reshape(C, n_hypers)
+        thetas, latent, fit = laplace_fit(
+            [gp] * C, eng, X, y, lambda classes, kernels: eng.laplace_nll_classes_any_size(C, classes, kernels, gp._tol),
+            N.SGP_MODES_CLASS, lambda c: c, given)
+        thetas = np.array(thetas).reshape(C, n_hypers)
         self._record(fit)
         models = []
         for c in range(C):
-            # produceModel in the fit's context
-            kernel, active_set, mv, mm, _ = _produce_model(gp, eng, X, latent[c], thetas[c])
-            # the model's own small context: never runs statistics, so it holds no statistics workspace
-            model_eng = ProjectedProcessEngine(gp._device)
-            model_eng.begin(kernel, active_set)
-            model_eng.set_magic(mv, mm)
-            models.append(GaussianProcessClassificationModel(
-                GaussianProjectedProcessRawPredictor(model_eng, mv, mm, kernel, active_set), thetas[c]))
+            fitted = produce(gp, eng, X, latent[c], thetas[c])                  # produceModel in the fit's context
+            models.append(GaussianProcessClassificationModel.of(own_context(fitted, gp._device)))
         self.last_latent = latent
         return OneVsRestModel(models, thetas)
 
@@ -333,15 +281,14 @@ class OneVsRest:
         from . import distributed
         slots, fit = distributed.group_fit(gp, X, y, hyperparameters, "classes")
         self._record(fit)
-        thetas = np.array([s[2] for s in slots]).reshape(len(slots), -1)
-        latent = [s[7] for s in slots]
+        thetas = np.array([fitted.theta for fitted in slots]).reshape(len(slots), -1)
+        latent = [fitted.latent for fitted in slots]
         if is_cuda_tensor(latent[0]):
             import torch
             self.last_latent = torch.stack(latent)
         else:
             self.last_latent = np.stack(latent)
-        models = [GaussianProcessClassificationModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, Z), theta)
-                  for (eng, kernel, _, Z, mv, mm, _, _), theta in zip(slots, thetas)]
+        models = [GaussianProcessClassificationModel.of(fitted) for fitted in slots]
         return OneVsRestModel(models, thetas)
 
     def _record(self, fit):

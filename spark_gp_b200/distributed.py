@@ -25,7 +25,8 @@ from __future__ import annotations
 import numpy as np
 
 from . import _native as N
-from .engine import ProjectedProcessEngine, device_fit_data, is_cuda_tensor, rows_to_host
+from .engine import ProjectedProcessEngine, is_cuda_tensor, rows_to_host
+from .hyperopt import each, fit_data, fit_slots, optimize_hypers, own_context, produce, slot_modes, slot_objective
 
 # per-expert point limits of the library: the BCM LU path (sgp_bcm_nll) and the global-memory Laplace kernel
 BCM_MAX_EXPERT_POINTS = 46340
@@ -237,21 +238,9 @@ def attach_communicator(eng, group, device):
 
 
 def _local_data(X, y, device: int, kind: str, what: str):
-    """The shard as the single-GPU fit reads it (regression: float32 X kept, others float64; classifiers: float64), with
-    the labels checked for the classifiers.  Returns (X, y, the largest label: one-vs-rest's, -1 for an empty shard and
-    for the other fits)."""
-    if kind != "regression":
-        from .classification import fit_data
-        X, y = fit_data(X, y, device, what)
-    elif is_cuda_tensor(X):
-        X, y = device_fit_data(X, y, device, what)
-        import torch
-        if X.dtype not in (torch.float32, torch.float64):
-            X = X.to(torch.float64)
-    else:
-        X = np.asarray(X)
-        X = X if X.dtype == np.float32 else np.asarray(X, dtype=np.float64)
-        y = np.asarray(y, dtype=np.float64)
+    """The shard as the single-GPU fit reads it (`fit_data`), with the labels checked for the classifiers.  Returns (X, y,
+    the largest label: one-vs-rest's, -1 for an empty shard and for the other fits)."""
+    X, y = fit_data(X, y, device, what, keep_float32=kind == "regression")
     if X.ndim != 2 or y.ndim != 1 or len(y) != len(X):
         raise ValueError("%s: X must be n x d and y n entries" % what)
     top = -1
@@ -274,8 +263,7 @@ def _tensor(a, device, dtype=None):
 
 def fit(gp, X, y, hyperparameters, classifier: bool, engine_factory=ProjectedProcessEngine):
     """The data-parallel fit of gp (a GaussianProcessRegression or binary GaussianProcessClassifier with a process
-    group) on this rank's shard (`group_fit`).  Returns (model's engine, kernel, theta, active set, magic vector, magic
-    matrix, (G, b), latent modes of this rank's expert rows or None)."""
+    group) on this rank's shard (`group_fit`).  Returns the model's `Fitted` slot."""
     models, record = group_fit(gp, X, y, hyperparameters, "binary" if classifier else "regression", engine_factory)
     if record is not None and record["slots"] is not None:
         gp.last_objective = dict(record["slots"][0], launches=record["launches"])
@@ -286,10 +274,10 @@ def group_fit(gp, X, y, hyperparameters, kind: str, engine_factory=ProjectedProc
     """The data-parallel fit over gp's process group on this rank's shard.  kind: "regression", "binary" (gp a binary
     GaussianProcessClassifier) or "classes" (one-vs-rest over gp: y holds class indices, numClasses agreed by the ranks,
     and hyperparameters, if given, numClasses x n_hypers).  The fit runs on the group's context with a communicator
-    (`comm_engine`); each model gets a context of its own holding its active set and magic pair.  Returns (per slot --
-    the one model, or one per class -- (model's engine, kernel, theta, active set, magic vector, magic matrix, (G, b),
-    latent modes of this rank's expert rows or None), the Laplace fit record of `laplace_optimise` or None for the
-    regression).  Fits over one group must not run concurrently."""
+    (`comm_engine`); each model gets a context of its own holding its active set and magic pair (`own_context`).
+    Returns (per slot -- the one model, or one per class -- its `Fitted` value, with the latent modes of this rank's
+    expert rows for the classifiers, the Laplace fit record of `fit_slots` or None for the regression).  Fits over one group must
+    not run concurrently."""
     import contextlib
 
     import torch
@@ -320,69 +308,45 @@ def group_fit(gp, X, y, hyperparameters, kind: str, engine_factory=ProjectedProc
             _COMM_ENGINES.pop(key, None)
             eng.close()
             raise
-        models = []
-        for kernel, theta, Z, mv, mm, stats, f in slots:
-            model_eng = engine_factory(gp._device)
-            model_eng.begin(kernel, Z)
-            model_eng.set_magic(mv, mm)
-            models.append((model_eng, kernel, theta, Z, mv, mm, stats, f))
-        return models, record
+        return [own_context(fitted, gp._device, engine_factory) for fitted in slots], record
 
 
 def _fit(gp, plan, eng, X, y, hyperparameters, kind, n_classes, dtype, group, device):
+    """The fit on the group's context: each slot's `Fitted` value and the Laplace fit record.  Each slot's
+    model has the active set of the concatenation and the statistics all-reduced over the group: of this rank's shard
+    for the regression, of its expert rows with the slot's modes as labels for the classifiers."""
     import torch
-    from .hyperopt import lbfgsb_bounds, optimise_slots
     eng.set_precision(N.SGP_PREC_AUTO)                      # as on a freshly acquired context
-    k0 = gp.getKernel()
+    exchanged = lambda: exchange(plan, _tensor(X, device, getattr(torch, dtype)), _tensor(y, device, torch.float64), group)
+    x0 = gp.getKernel().getHyperparameters()
     if kind == "regression":
         if hyperparameters is not None:
-            theta = np.asarray(hyperparameters, dtype=np.float64)
+            theta = hyperparameters
         elif gp._maxIter > 0:
-            Xe, ye = exchange(plan, _tensor(X, device, getattr(torch, dtype)), _tensor(y, device, torch.float64), group)
+            Xe, ye = exchanged()
             eng.experts_upload_strided(Xe, ye, plan.local_experts)
-            launches0 = eng.launch_count()
-            evaluate = lambda batch: [eng.bcm_nll(gp.getKernel().setHyperparameters(t)) for _, t in batch]
-            (theta,), records, _ = optimise_slots(evaluate, [k0.getHyperparameters()], lbfgsb_bounds(k0), gp._maxIter,
-                                                  gp._tol)
-            if records is not None:
-                gp.last_objective = dict(records[0], n_experts=plan.E, launches=eng.launch_count() - launches0)
+            theta = optimize_hypers(gp, eng, plan.E)
         else:
-            theta = k0.getHyperparameters()
-        return [_model(gp, plan, eng, X, np.asarray(theta, dtype=np.float64), X, y, None, group, device)], None
+            theta = x0
+        theta = np.asarray(theta, dtype=np.float64)
+        return [produce(gp, eng, X, y, theta, active_set(gp, plan, eng, X, theta, group, device))], None
     # the Laplace fit of one slot (the binary classifier) or of every class (one-vs-rest), as `laplace_fit` on one GPU
-    from .classification import binary_objective, classes_objective, laplace_optimise
-    x0 = k0.getHyperparameters()
     if kind == "binary":
-        store, objective, x0s = N.SGP_MODES_BINARY, binary_objective(gp, eng), [x0]
+        store, n_slots, entry = N.SGP_MODES_BINARY, 1, each(lambda k: eng.laplace_nll_any_size(k, gp._tol))
         given = None if hyperparameters is None else [np.asarray(hyperparameters, dtype=np.float64)]
     else:
-        store, objective, x0s = N.SGP_MODES_CLASS, classes_objective(gp, eng, n_classes), [x0] * n_classes
+        store, n_slots = N.SGP_MODES_CLASS, n_classes
+        entry = lambda classes, kernels: eng.laplace_nll_classes_any_size(n_classes, classes, kernels, gp._tol)
         given = None if hyperparameters is None else \
             np.array(hyperparameters, dtype=np.float64).reshape(n_classes, len(x0))
-    Xe, ye = exchange(plan, _tensor(X, device, getattr(torch, dtype)), _tensor(y, device, torch.float64), group)
+    Xe, ye = exchanged()
     eng.experts_upload_strided(Xe, ye, plan.local_experts)
-    thetas, record = laplace_optimise(gp, eng, objective, x0s, given)
+    thetas, record = fit_slots(eng, gp, slot_objective([gp] * n_slots, entry), [x0] * n_slots, given, laplace=True)
     n_e = len(Xe)
     if not is_cuda_tensor(X):
         Xe = Xe.cpu().numpy()
     slots = []
     for i, theta in enumerate(thetas):
-        # every model starts from the default precision, as `_produce_model`
-        eng.set_precision(N.SGP_PREC_AUTO)
-        if is_cuda_tensor(X):                               # the modes stay on the device, ungrouped into row order
-            f = eng.experts_modes_rows(store, i, n_e)
-        else:
-            f = np.empty(n_e)
-            f[plan.local_order()] = eng.experts_modes(store, i, n_e)
-        slots.append(_model(gp, plan, eng, X, theta, Xe, f, f, group, device))
+        f = slot_modes(eng, is_cuda_tensor(X), n_e, plan.local_experts, store, i)
+        slots.append(produce(gp, eng, Xe, f, theta, active_set(gp, plan, eng, X, theta, group, device))._replace(latent=f))
     return slots, record
-
-
-def _model(gp, plan, eng, X, theta, stats_X, stats_y, f, group, device):
-    """One slot's model at theta: the active set of the concatenation, the statistics of (stats_X, stats_y) all-reduced
-    over the group, and the tail.  Returns (kernel, theta, active set, magic vector, magic matrix, (G, b), f)."""
-    Z = active_set(gp, plan, eng, X, theta, group, device)
-    kernel = gp.getKernel().setHyperparameters(theta)
-    G, b = eng.statistics(kernel, Z, stats_X, stats_y, getattr(gp, "_shard_points", 1 << 22))
-    mv, mm = eng.magic()
-    return kernel, theta, Z, mv, mm, (G, b), f

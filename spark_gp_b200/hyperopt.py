@@ -5,15 +5,21 @@ Expert grouping as the reference (GPC:26-31: E = Math.round(N / n_e), point i ->
 the bound-constrained quasi-Newton loop is SciPy's L-BFGS-B in place of Breeze's `LBFGSB(lower, upper, maxIter,
 tolerance = tol)` -- the reference pins no test on the iterate trajectory, so results are compared on the objective
 value and on predictive metrics, not on theta.  `optimise_slots` runs that loop for every estimator and model selector
-here, over one slot or several in lock-step."""
+here, over one slot or several in lock-step.
+
+The steps every estimator and model selector shares are written here once: the input rule (`fit_data`), the slot fit
+(`fit_slots` over a `slot_objective`), the read-back of a slot's latent modes (`slot_modes`) and the model step
+(`produce`, giving a `Fitted` slot, and `own_context`)."""
 from __future__ import annotations
 
 import threading
+from collections import namedtuple
 
 import numpy as np
 from scipy.optimize import minimize
 
-from .engine import ProjectedProcessEngine
+from . import _native as N
+from .engine import ProjectedProcessEngine, device_fit_data, is_cuda_tensor
 
 
 def lbfgsb_bounds(kernel):
@@ -132,12 +138,79 @@ def optimise_slots(evaluate, x0s, bounds, max_iter: int, tol: float):
             [dict(value=float(res.fun), evaluations=ev, iterations=int(res.nit)) for res, ev in results], rounds)
 
 
-def group_for_experts(n_points: int, dataset_size_for_expert: int):
-    """GPC:26-31."""
+def fit_slots(eng, gp, objective, x0s, thetas=None, laplace: bool = False):
+    """The hyper-parameters of every slot of `objective` (a `slot_objective`) on the experts uploaded into eng: unless
+    `thetas` are given, `optimise_slots` from x0s with gp's bounds, maxIter and tol.  laplace: the Laplace fit
+    (GPCls:53-60), which has nothing to optimise without hyper-parameters and runs the Laplace loop once more at every
+    slot's theta (GPCls:60), so that the modes are the modes at theta.  Returns (thetas, dict(slots: each slot's
+    `optimise_slots` record, or None when nothing was optimised, rounds, launches: the optimisation's, and with laplace
+    launches_total: with the call at theta))."""
+    launches0 = eng.launch_count()
+    records, rounds = None, 0
+    if thetas is None:
+        thetas = [np.asarray(x0, dtype=np.float64) for x0 in x0s]
+        if len(thetas[0]) > 0 or not laplace:
+            thetas, records, rounds = optimise_slots(objective, x0s, lbfgsb_bounds(gp.getKernel()), gp._maxIter, gp._tol)
+    fit = dict(slots=records, rounds=rounds, launches=eng.launch_count() - launches0)
+    if laplace:
+        objective(list(enumerate(thetas)))
+        fit["launches_total"] = eng.launch_count() - launches0
+    return thetas, fit
+
+
+def slot_objective(gps, entry):
+    """The objective of `fit_slots` over slots whose kernels are those of gps[i] (one estimator per slot): entry(slots,
+    kernels) -> (values, gradients) evaluates the listed slots at their kernels, in one batched call of the engine."""
+    def objective(batch):
+        vals, grads = entry([i for i, _ in batch],
+                            [gps[i].getKernel().setHyperparameters(np.asarray(t, dtype=np.float64)) for i, t in batch])
+        return [(float(v), g) for v, g in zip(vals, grads)]
+    return objective
+
+
+def each(fn):
+    """A `slot_objective` entry from a one-kernel entry fn(kernel) -> (value, gradient), called once per listed slot."""
+    return lambda slots, kernels: zip(*[fn(k) for k in kernels])
+
+
+def fit_data(X, y, device: int, what: str, keep_float32: bool = False):
+    """The (X, y) of a fit: host arrays, or CUDA tensors for a CUDA tensor X (`device_fit_data`, its messages naming
+    `what`).  y is float64; X float64, or float32 as given when keep_float32 (the regression reads float32 points as they
+    are; the classifiers read float64)."""
+    if is_cuda_tensor(X):
+        import torch
+        X, y = device_fit_data(X, y, device, what)
+        return (X if keep_float32 and X.dtype == torch.float32 else X.to(torch.float64)), y
+    X = np.asarray(X)
+    return (X if keep_float32 and X.dtype == np.float32 else np.asarray(X, dtype=np.float64)), \
+        np.asarray(y, dtype=np.float64)
+
+
+def expert_count(n_points: int, dataset_size_for_expert: int) -> int:
+    """numberOfExperts = Math.round(N / datasetSizeForExpert) (GPC:27); ZeroDivisionError when it is 0."""
     n_experts = int(np.floor(n_points / dataset_size_for_expert + 0.5))
     if n_experts <= 0:
         raise ZeroDivisionError("numberOfExperts == 0 (N < datasetSizeForExpert / 2)")
+    return n_experts
+
+
+def group_for_experts(n_points: int, dataset_size_for_expert: int):
+    """GPC:26-31."""
+    n_experts = expert_count(n_points, dataset_size_for_expert)
     return [np.arange(e, n_points, n_experts) for e in range(n_experts)]
+
+
+def slot_modes(eng, on_device: bool, n: int, n_experts: int, store: int, index: int, fold=None):
+    """The latent modes of one slot of an upload of n rows grouped into n_experts experts (row i -> expert
+    i % n_experts, as every upload groups them), in row order: of `store` (N.SGP_MODES_*, index: the class or mode
+    slot), or with fold=k of mode slot index on fold set k of a fold upload.  on_device: a CUDA float64 tensor ungrouped
+    on the device; else a host array, read packed expert-major and scattered into row order."""
+    if on_device:
+        return eng.experts_modes_rows(store, index, n) if fold is None else eng.experts_f_fold_slot_rows(fold, index, n)
+    f = np.empty(n)
+    f[np.concatenate([np.arange(e, n, n_experts) for e in range(n_experts)])] = \
+        eng.experts_modes(store, index, n) if fold is None else eng.experts_f_fold_slot(fold, index, n)
+    return f
 
 
 def pack_experts(X, y, dataset_size_for_expert: int):
@@ -147,9 +220,7 @@ def pack_experts(X, y, dataset_size_for_expert: int):
     X = np.asarray(X, dtype=np.float64)
     y = np.asarray(y, dtype=np.float64)
     n, d = X.shape
-    n_experts = int(np.floor(n / dataset_size_for_expert + 0.5))           # Math.round(N / n_e), GPC:27
-    if n_experts <= 0:
-        raise ZeroDivisionError("numberOfExperts == 0 (N < datasetSizeForExpert / 2)")
+    n_experts = expert_count(n, dataset_size_for_expert)
     k, r = divmod(n, n_experts)                       # every expert has k points, the first r experts k + 1
     sizes = np.full(n_experts, k, dtype=np.int64)
     sizes[:r] += 1
@@ -173,22 +244,45 @@ def pack_experts(X, y, dataset_size_for_expert: int):
     return Xp, yp, offsets
 
 
-def optimize_hypers(gp, X, y, engine: ProjectedProcessEngine | None = None):
-    """Returns the optimal hyper-parameter vector (layout of Kernel.getHyperparameters)."""
-    own = engine is None
-    engine = engine or ProjectedProcessEngine.acquire(gp._device)
-    try:
-        # expert grouping (GPC:26-31) as a strided gather on the device while the points stream in (the host-side
-        # pack_experts above is the same permutation, kept for callers that hold expert-major data and for the tests)
-        n_experts = engine.experts_upload_grouped(X, y, gp._datasetSizeForExpert)
-        launches0 = engine.launch_count()
-        k0 = gp.getKernel()
-        evaluate = lambda batch: [engine.bcm_nll(gp.getKernel().setHyperparameters(t)) for _, t in batch]
-        (theta,), records, _ = optimise_slots(evaluate, [k0.getHyperparameters()], lbfgsb_bounds(k0), gp._maxIter,
-                                              gp._tol)
-        if records is not None:
-            gp.last_objective = dict(records[0], n_experts=n_experts, launches=engine.launch_count() - launches0)
-        return theta
-    finally:
-        if own:
-            engine.release()
+def optimize_hypers(gp, eng, n_experts: int):
+    """The optimal hyper-parameter vector (layout of Kernel.getHyperparameters) of gp's BCM objective over the n_experts
+    experts uploaded into eng; records the optimisation in gp.last_objective."""
+    (theta,), fit = fit_slots(eng, gp, slot_objective([gp], each(eng.bcm_nll)), [gp.getKernel().getHyperparameters()])
+    if fit["slots"] is not None:
+        gp.last_objective = dict(fit["slots"][0], n_experts=n_experts, launches=fit["launches"])
+    return theta
+
+
+# A fitted slot: the context holding its active set and magic pair (the model's), the kernel at theta, theta, the active
+# set, the magic pair, the statistics (G, b), and the latent modes its labels were (the classifiers; None for the
+# regression).  The group fit has returned these eight, in this order, since before they had names.
+Fitted = namedtuple("Fitted", "engine kernel theta active_set magic_vector magic_matrix stats latent")
+
+
+def draw_active_set(gp, X, y, theta):
+    """gp's active-set provider on (X, y) at theta (GPC:40-47)."""
+    return gp._activeSetProvider(gp._activeSetSize, X, y, gp.getKernel, theta, gp._seed, gp=gp)
+
+
+def produce(gp, eng, X, y, theta, active_set=None) -> Fitted:
+    """produceModel -> projectedProcess (GPC:40-59, 102-110) on eng: the active set (drawn by gp's provider unless
+    given), the statistics of (X, y) in gp's shards (PGPH:20-36, with the fp64-kernel fallback) and the tail (PGPH:49-60).
+    The slot is eng's, with no latent modes.
+    Every model starts from the default precision, as on a freshly acquired context: a fall-back to F64 in one slot's
+    statistics must not decide the next slot's path."""
+    eng.set_precision(N.SGP_PREC_AUTO)
+    if active_set is None:
+        active_set = draw_active_set(gp, X, y, theta)
+    kernel = gp.getKernel().setHyperparameters(theta)
+    stats = eng.statistics(kernel, active_set, X, y, getattr(gp, "_shard_points", 1 << 22))
+    mv, mm = eng.magic()
+    return Fitted(eng, kernel, theta, active_set, mv, mm, stats, None)
+
+
+def own_context(fitted: Fitted, device: int, engine_factory=ProjectedProcessEngine) -> Fitted:
+    """The fitted slot on a small context of its own, which holds its active set and magic pair: it never runs
+    statistics, so it holds no statistics workspace."""
+    eng = engine_factory(device)
+    eng.begin(fitted.kernel, fitted.active_set)
+    eng.set_magic(fitted.magic_vector, fitted.magic_matrix)
+    return fitted._replace(engine=eng)

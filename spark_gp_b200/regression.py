@@ -12,8 +12,9 @@ import copy
 import numpy as np
 
 from . import _native as N
-from .engine import ProjectedProcessEngine, OperandRangeError, NotPositiveDefiniteException, device_fit_data, host_copy, \
-    is_cuda_tensor, rows_to_host
+from .engine import ProjectedProcessEngine, OperandRangeError, NotPositiveDefiniteException, host_copy, is_cuda_tensor, \
+    rows_to_host
+from .hyperopt import draw_active_set, fit_data, optimize_hypers, produce
 from .kernels import Kernel, RBFKernel, EyeKernel, const
 
 
@@ -255,6 +256,12 @@ class GaussianProcessRegressionModel:
         self.rawPredictor = rawPredictor
         self.hyperparameters = hyperparameters
 
+    @classmethod
+    def of(cls, fitted):
+        """The model of a fitted slot (`hyperopt.Fitted`), on the context that holds its active set and magic pair."""
+        return cls(GaussianProjectedProcessRawPredictor(fitted.engine, fitted.magic_vector, fitted.magic_matrix,
+                                                        fitted.kernel, fitted.active_set), fitted.theta)
+
     def predict(self, features):
         if is_cuda_tensor(features):                 # CUDA torch tensor in, CUDA float64 tensor out
             mean, _ = self.rawPredictor._engine.predict_tensor(features, with_variance=False)
@@ -287,31 +294,28 @@ class GaussianProcessRegression(GaussianProcessParams):
         concatenation of the shards in rank order, the same bits on every rank."""
         if self._process_group is not None:
             from . import distributed
-            eng, kernel, theta, active_set, mv, mm, self.last_stats, _ = distributed.fit(self, X, y, hyperparameters, False)
-            return GaussianProcessRegressionModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, active_set),
-                                                  theta)
-        if is_cuda_tensor(X):
-            X, y = device_fit_data(X, y, self._device, "GaussianProcessRegression.fit")
-        else:
-            X = np.asarray(X)
-            y = np.asarray(y, dtype=np.float64)
+            fitted = distributed.fit(self, X, y, hyperparameters, False)
+            self.last_stats = fitted.stats
+            return GaussianProcessRegressionModel.of(fitted)
+        X, y = fit_data(X, y, self._device, "GaussianProcessRegression.fit", keep_float32=True)
         if hyperparameters is None:
-            if self._maxIter > 0:
-                from .hyperopt import optimize_hypers     # per-expert BCM NLL on the GPU + L-BFGS-B on the host
-                hyperparameters = optimize_hypers(self, X, y)
+            if self._maxIter > 0:                   # per-expert BCM NLL on the GPU + L-BFGS-B on the host
+                eng = ProjectedProcessEngine.acquire(self._device)
+                try:
+                    # expert grouping (GPC:26-31) as a strided gather on the device while the points stream in
+                    hyperparameters = optimize_hypers(self, eng, eng.experts_upload_grouped(X, y,
+                                                                                            self._datasetSizeForExpert))
+                finally:
+                    eng.release()
             else:
                 hyperparameters = self.getKernel().getHyperparameters()
-        theta = np.asarray(hyperparameters, dtype=np.float64)
-        return self._produce_model(X, y, theta)
+        return self._produce_model(X, y, np.asarray(hyperparameters, dtype=np.float64))
 
-    def _produce_model(self, X, y, theta):
-        """produceModel -> projectedProcess  (commons/GaussianProcessCommons.scala:40-59, 102-110)."""
-        active_set = self._activeSetProvider(self._activeSetSize, X, y, self.getKernel, theta, self._seed, gp=self)
-        kernel = self.getKernel().setHyperparameters(theta)
+    def _produce_model(self, X, y, theta) -> GaussianProcessRegressionModel:
+        """produceModel (commons/GaussianProcessCommons.scala:40-59, 102-110) on a context of the pool that the model
+        keeps.  The active set is drawn first, so that a provider that takes a context of its own reuses the pooled one."""
+        active_set = draw_active_set(self, X, y, theta)
         eng = ProjectedProcessEngine.acquire(self._device)
-
-        G, b = eng.statistics(kernel, active_set, X, y, self._shard_points)   # PGPH:20-36 (+ fp64-kernel fallback)
-        mv, mm = eng.magic()                                            # PGPH:49-60
-        self.last_stats = (G, b)
-        return GaussianProcessRegressionModel(GaussianProjectedProcessRawPredictor(eng, mv, mm, kernel, active_set),
-                                              theta)
+        fitted = produce(self, eng, X, y, theta, active_set)
+        self.last_stats = fitted.stats
+        return GaussianProcessRegressionModel.of(fitted)

@@ -58,10 +58,10 @@ from __future__ import annotations
 import numpy as np
 
 from . import _native as N
-from .classification import GaussianProcessClassifier, OneVsRest, _produce_model, assert_labels_are_01, laplace_fit, \
-    laplace_optimise, one_vs_rest_labels, one_vs_rest_prediction
-from .engine import ProjectedProcessEngine, device_fit_data, host_copy, is_cuda_tensor, take_rows
-from .hyperopt import group_for_experts, lbfgsb_bounds, optimise_slots
+from .classification import GaussianProcessClassifier, OneVsRest, assert_labels_are_01, binary_prediction, laplace_fit, \
+    one_vs_rest_labels, one_vs_rest_prediction
+from .engine import ProjectedProcessEngine, host_copy, is_cuda_tensor, take_rows
+from .hyperopt import fit_data, fit_slots, lbfgsb_bounds, produce, slot_modes, slot_objective
 from .regression import GaussianProcessRegression
 from .utils import kfold_assignment, train_validation_assignment
 
@@ -309,12 +309,11 @@ class _Validator:
         self._seed = int(value)
         return self
 
-    def _data(self, X, y, device: int):
-        if is_cuda_tensor(X):
-            return device_fit_data(X, y, device, self.NAME + ".fit")
-        X = np.asarray(X)
-        y = np.asarray(y, dtype=np.float64)
-        if X.ndim != 2 or len(y) != len(X):
+    def _data(self, X, y, device: int, classifier: bool):
+        """(X, y) as the estimator's fit reads them (`fit_data`)."""
+        on_device = is_cuda_tensor(X)
+        X, y = fit_data(X, y, device, self.NAME + ".fit", keep_float32=not classifier)
+        if not on_device and (X.ndim != 2 or len(y) != len(X)):
             raise ValueError("%s: X must be n x d and y n labels" % self.NAME)
         return X, y
 
@@ -327,6 +326,41 @@ def _rows(X, mask):
 def _host_predictions(p):
     """A model's predictions as the evaluator reads them (host float64)."""
     return np.asarray(host_copy(p), dtype=np.float64)
+
+
+def _latent_mean(eng, X):
+    """The latent mean of the model eng holds at the validation rows X, on X's side, as the evaluator reads it (host
+    float64)."""
+    if is_cuda_tensor(X):
+        return _host_predictions(eng.predict_tensor(X, with_variance=False)[0])
+    return eng.predict(X, with_variance=False)[0]
+
+
+def _validate(est, Xt, yt, Xv, theta):
+    """The validation predictions (host float64) and the magic vector of the regression estimator's model on the training
+    rows at theta.  The model's context goes back to the pool on return, before the next slot's."""
+    model = est._produce_model(Xt, yt, theta)
+    return _host_predictions(model.predict(Xv)), model.rawPredictor.magicVector
+
+
+def _bcm_groups(ests, n: int, upload, entry):
+    """The lock-step BCM optimisation of each group of (map p, j) slots, j in [0, n) (`group_slots`), on one context of
+    its own: upload(eng, datasetSizeForExpert) uploads the training rows, entry(eng, slots, kernels) evaluates the listed
+    slots in one launch.  A group with maxIter <= 0 is skipped: it takes its kernels' own hyper-parameters, as GPR.fit
+    does.  Yields (slots, thetas, the `fit_slots` record, upload's return) per optimised group."""
+    for slots in group_slots(ests, n).values():
+        e0 = ests[slots[0][0]]
+        if e0._maxIter <= 0:
+            continue
+        eng = ProjectedProcessEngine.acquire(e0._device)
+        try:
+            uploaded = upload(eng, e0._datasetSizeForExpert)
+            objective = slot_objective([ests[p] for p, _ in slots],
+                                       lambda listed, kernels: entry(eng, [slots[i] for i in listed], kernels))
+            thetas, fit = fit_slots(eng, e0, objective, [ests[p].getKernel().getHyperparameters() for p, _ in slots])
+        finally:
+            eng.release()
+        yield slots, thetas, fit, uploaded
 
 
 class CrossValidatorModel(_SelectedModel):
@@ -383,7 +417,7 @@ class CrossValidator(_Validator):
         ovr = isinstance(est, OneVsRest)
         if ovr and not isinstance(est.getClassifier(), GaussianProcessClassifier):
             raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
-        X, y = self._data(X, y, (est.getClassifier() if ovr else est)._device)
+        X, y = self._data(X, y, (est.getClassifier() if ovr else est)._device, ovr)
         K = self._num_folds
         if folds is None:
             fold_of = kfold_assignment(len(X), K, self._seed)
@@ -408,11 +442,9 @@ class CrossValidator(_Validator):
         for p, e in enumerate(ests):
             for k in range(K):
                 train, val = fold_of != k, fold_of == k
-                model = e._produce_model(_rows(X, train), _rows(y, train), thetas[p][k])
-                pred = _host_predictions(model.predict(_rows(X, val)))
-                folds_out[p, k] = dict(theta=thetas[p][k], magicVector=model.rawPredictor.magicVector, prediction=pred)
+                pred, mv = _validate(e, _rows(X, train), _rows(y, train), _rows(X, val), thetas[p][k])
+                folds_out[p, k] = dict(theta=thetas[p][k], magicVector=mv, prediction=pred)
                 metrics[p, k] = self._evaluator.evaluate(host_copy(_rows(y, val)), pred)
-                del model                         # its context goes back to the pool before the next slot
         return self._select(est, maps, X, y, K, metrics, folds_out, objective)
 
     def _select(self, est, maps, X, y, K, metrics, folds_out, objective):
@@ -430,11 +462,6 @@ class CrossValidator(_Validator):
         group of slots one fold upload, one lock-step L-BFGS-B over the (map, fold, class) slots with one
         `sgp_laplace_nll_fold_slots_any_size` call per round, and one more call at every slot's optimum (GPCls:60).
         Returns ({(p, k): theta (C_k x h), magicVector [C_k], prediction}, dict(groups=...))."""
-        if is_cuda_tensor(X):
-            import torch
-            X = X.to(torch.float64)
-        else:
-            X = np.asarray(X, dtype=np.float64)
         y = one_vs_rest_labels(y)[0]
         train = [fold_of != k for k in range(K)]
         n_k = [int(np.count_nonzero(t)) for t in train]
@@ -442,19 +469,14 @@ class CrossValidator(_Validator):
         thetas, latent, groups = {}, {}, []
         for slots in fold_class_slot_groups(gps, C).values():
             g0 = gps[slots[0][0]]
-            kernel_at = lambda p, t: gps[p].getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
             eng = ProjectedProcessEngine.acquire(g0._device)
             try:
-                eng.experts_upload_folds(X, y, fold_of, K, g0._datasetSizeForExpert)
-
-                def objective(batch):
-                    vals, grads = eng.laplace_nll_fold_slots_any_size(
-                        len(gps) * sum(C), [slots[i][3] for i, _ in batch], [slots[i][1] for i, _ in batch],
-                        [slots[i][2] for i, _ in batch], [kernel_at(slots[i][0], t) for i, t in batch], g0._tol)
-                    return [(float(v), g) for v, g in zip(vals, grads)]
-
-                fitted, fit = laplace_optimise(g0, eng, objective, [gps[p].getKernel().getHyperparameters()
-                                                                    for p, _, _, _ in slots])
+                n_experts = eng.experts_upload_folds(X, y, fold_of, K, g0._datasetSizeForExpert)
+                entry = lambda listed, kernels: eng.laplace_nll_fold_slots_any_size(
+                    len(gps) * sum(C), [slots[i][3] for i in listed], [slots[i][1] for i in listed],
+                    [slots[i][2] for i in listed], kernels, g0._tol)
+                fitted, fit = fit_slots(eng, g0, slot_objective([gps[p] for p, _, _, _ in slots], entry),
+                                        [gps[p].getKernel().getHyperparameters() for p, _, _, _ in slots], laplace=True)
                 # every objective call is one round, and one more runs at the slots' thetas
                 groups.append(dict(
                     slots=[dict(map=p, fold=k, cls=c, mode_slot=m, theta=theta, **r)
@@ -462,12 +484,7 @@ class CrossValidator(_Validator):
                     rounds=fit["rounds"], calls=fit["rounds"] + 1, launches=fit["launches_total"]))
                 for (p, k, c, m), theta in zip(slots, fitted):
                     thetas[p, k, c] = theta
-                    if is_cuda_tensor(X):
-                        latent[p, k, c] = eng.experts_f_fold_slot_rows(k, m, n_k[k])
-                    else:
-                        order = np.concatenate(group_for_experts(n_k[k], g0._datasetSizeForExpert))
-                        latent[p, k, c] = np.empty(n_k[k])
-                        latent[p, k, c][order] = eng.experts_f_fold_slot(k, m, n_k[k])
+                    latent[p, k, c] = slot_modes(eng, is_cuda_tensor(X), n_k[k], n_experts[k], None, m, fold=k)
             finally:
                 eng.release()
         folds_out = {}
@@ -478,12 +495,8 @@ class CrossValidator(_Validator):
                     Xt, Xv = _rows(X, train[k]), _rows(X, ~train[k])
                     raw, mvs = np.empty((len(Xv), C[k])), []
                     for c in range(C[k]):
-                        _, _, mv, _, _ = _produce_model(gp, eng, Xt, latent[p, k, c], thetas[p, k, c])
-                        mvs.append(mv)
-                        if is_cuda_tensor(Xv):
-                            raw[:, c] = _host_predictions(eng.predict_tensor(Xv, with_variance=False)[0])
-                        else:
-                            raw[:, c], _ = eng.predict(Xv, with_variance=False)
+                        mvs.append(produce(gp, eng, Xt, latent[p, k, c], thetas[p, k, c]).magic_vector)
+                        raw[:, c] = _latent_mean(eng, Xv)
                     folds_out[p, k] = dict(theta=np.array([thetas[p, k, c] for c in range(C[k])]), magicVector=mvs,
                                            prediction=one_vs_rest_prediction(raw))
         finally:
@@ -492,31 +505,15 @@ class CrossValidator(_Validator):
 
     @staticmethod
     def _optimise(ests, X, y, fold_of, K):
-        """Optimal hyper-parameters of every (map, fold) slot (thetas[p][k]), and what the optimisation took."""
-        x0s = [e.getKernel().getHyperparameters() for e in ests]
-        thetas = [[np.asarray(x0s[p], dtype=np.float64) for _ in range(K)] for p in range(len(ests))]
+        """Optimal hyper-parameters of every (map, fold) slot (thetas[p][k]), and what the optimisation took: per group
+        of slots one fold upload, each round one `sgp_bcm_nll_folds` launch (`_bcm_groups`)."""
+        thetas = [[np.asarray(e.getKernel().getHyperparameters(), dtype=np.float64)] * K for e in ests]
         groups = []
-        for key, slots in group_slots(ests, K).items():
-            e0 = ests[slots[0][0]]
-            if e0._maxIter <= 0:
-                continue                          # GPR.fit takes the kernel's own hyper-parameters
-            eng = ProjectedProcessEngine.acquire(e0._device)
-            try:
-                eng.experts_upload_folds(X, y, fold_of, K, e0._datasetSizeForExpert)
-                launches0 = eng.launch_count()
-                kernel_at = lambda p, t: ests[p].getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
-
-                def evaluate(batch):
-                    vals, grads = eng.bcm_nll_folds([slots[i][1] for i, _ in batch],
-                                                    [kernel_at(slots[i][0], t) for i, t in batch])
-                    return [(float(v), g) for v, g in zip(vals, grads)]
-
-                fitted, records, rounds = optimise_slots(evaluate, [x0s[p] for p, _ in slots],
-                                                         lbfgsb_bounds(e0.getKernel()), e0._maxIter, e0._tol)
-                groups.append(dict(slots=[dict(map=p, fold=k, **r) for (p, k), r in zip(slots, records)],
-                                   rounds=rounds, launches=eng.launch_count() - launches0))
-            finally:
-                eng.release()
+        for slots, fitted, fit, _ in _bcm_groups(
+                ests, K, lambda eng, n_e: eng.experts_upload_folds(X, y, fold_of, K, n_e),
+                lambda eng, slots, kernels: eng.bcm_nll_folds([k for _, k in slots], kernels)):
+            groups.append(dict(slots=[dict(map=p, fold=k, **r) for (p, k), r in zip(slots, fit["slots"])],
+                               rounds=fit["rounds"], launches=fit["launches"]))
             for (p, k), theta in zip(slots, fitted):
                 thetas[p][k] = theta
         return thetas, dict(groups=groups)
@@ -581,7 +578,8 @@ class TrainValidationSplit(_Validator):
             raise TypeError("TrainValidationSplit: a BinaryClassificationEvaluator scores the binary "
                             "GaussianProcessClassifier only, not a %s" % type(est).__name__)
         gp = est.getClassifier() if isinstance(est, OneVsRest) else est
-        X, y = self._data(X, y, getattr(gp, "_device", 0))           # a OneVsRest without a classifier fails below
+        X, y = self._data(X, y, getattr(gp, "_device", 0),          # a OneVsRest without a classifier fails below
+                          not isinstance(est, GaussianProcessRegression))
         if train is None:
             mask = train_validation_assignment(len(X), self._train_ratio, self._seed)
         else:
@@ -615,37 +613,20 @@ class TrainValidationSplit(_Validator):
         map's dict(theta, magicVector, evaluations, iterations; value and n_experts when optimised)],
         groups=[dict(maps, rounds, launches)]))."""
         Xt, yt, Xv = _rows(X, train), _rows(y, train), _rows(X, ~train)
-        x0s = [e.getKernel().getHyperparameters() for e in ests]
-        thetas = [np.asarray(x0, dtype=np.float64) for x0 in x0s]
+        thetas = [np.asarray(e.getKernel().getHyperparameters(), dtype=np.float64) for e in ests]
         records, groups = [dict(evaluations=0, iterations=0) for _ in ests], []
-        for slots in group_slots(ests, 1).values():
-            e0 = ests[slots[0][0]]
-            if e0._maxIter <= 0:
-                continue
-            eng = ProjectedProcessEngine.acquire(e0._device)
-            try:
-                n_experts = eng.experts_upload_grouped(Xt, yt, e0._datasetSizeForExpert)
-                launches0 = eng.launch_count()
-                kernel_at = lambda p, t: ests[p].getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
-
-                def evaluate(batch):
-                    vals, grads = eng.bcm_nll_slots([kernel_at(slots[i][0], t) for i, t in batch])
-                    return [(float(v), g) for v, g in zip(vals, grads)]
-
-                fitted, recs, rounds = optimise_slots(evaluate, [x0s[p] for p, _ in slots],
-                                                      lbfgsb_bounds(e0.getKernel()), e0._maxIter, e0._tol)
-                groups.append(dict(maps=[p for p, _ in slots], rounds=rounds, launches=eng.launch_count() - launches0))
-            finally:
-                eng.release()
-            for (p, _), theta, r in zip(slots, fitted, recs):
+        for slots, fitted, fit, n_experts in _bcm_groups(
+                ests, 1, lambda eng, n_e: eng.experts_upload_grouped(Xt, yt, n_e),
+                lambda eng, slots, kernels: eng.bcm_nll_slots(kernels)):
+            groups.append(dict(maps=[p for p, _ in slots], rounds=fit["rounds"], launches=fit["launches"]))
+            for (p, _), theta, r in zip(slots, fitted, fit["slots"]):
                 thetas[p] = theta
                 records[p] = dict(r, n_experts=n_experts)
         preds = []
         for e, theta, r in zip(ests, thetas, records):
-            model = e._produce_model(Xt, yt, theta)
-            preds.append(_host_predictions(model.predict(Xv)))
-            r.update(theta=theta, magicVector=model.rawPredictor.magicVector)
-            del model                             # its context goes back to the pool before the next map
+            pred, mv = _validate(e, Xt, yt, Xv, theta)
+            preds.append(pred)
+            r.update(theta=theta, magicVector=mv)
         return preds, dict(maps=records, groups=groups)
 
     @staticmethod
@@ -657,11 +638,6 @@ class TrainValidationSplit(_Validator):
         gps = [e.getClassifier() for e in ests] if ovr else ests
         if any(not isinstance(gp, GaussianProcessClassifier) for gp in gps):
             raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
-        if is_cuda_tensor(X):
-            import torch
-            X = X.to(torch.float64)
-        else:
-            X = np.asarray(X, dtype=np.float64)
         if ovr:
             one_vs_rest_labels(y)
             C = one_vs_rest_labels(_rows(y, train))[1]    # as an independent OneVsRest.fit(X[train], y[train])
@@ -676,32 +652,24 @@ class TrainValidationSplit(_Validator):
         for slots in tvs_slot_groups(gps, C).values():
             g0 = gps[slots[0][0]]
             modes = [m for _, _, m in slots]
-            kernel_at = lambda p, t: gps[p].getKernel().setHyperparameters(np.asarray(t, dtype=np.float64))
             eng = ProjectedProcessEngine.acquire(g0._device)
             try:
-                def objective(batch):
-                    vals, grads = eng.laplace_nll_slots_any_size(
-                        len(gps) * C, [modes[i] for i, _ in batch], [label(slots[i][1]) for i, _ in batch],
-                        [kernel_at(slots[i][0], t) for i, t in batch], g0._tol)
-                    return [(float(v), g) for v, g in zip(vals, grads)]
-
-                thetas, latent, fit = laplace_fit(g0, eng, Xt, yt, objective, N.SGP_MODES_SLOT, lambda i: modes[i],
-                                                  [gps[p].getKernel().getHyperparameters() for p, _, _ in slots])
+                entry = lambda listed, kernels: eng.laplace_nll_slots_any_size(
+                    len(gps) * C, [modes[i] for i in listed], [label(slots[i][1]) for i in listed], kernels, g0._tol)
+                thetas, latent, fit = laplace_fit([gps[p] for p, _, _ in slots], eng, Xt, yt, entry, N.SGP_MODES_SLOT,
+                                                  lambda i: modes[i])
                 # every objective call is one round, and one more runs at the slots' thetas
                 groups.append(dict(
                     slots=[dict(map=p, cls=c, mode_slot=m, theta=theta, **r)
                            for (p, c, m), r, theta in zip(slots, fit["slots"] or [], thetas)],
                     rounds=fit["rounds"], calls=fit["rounds"] + 1, launches=fit["launches_total"]))
                 for (p, c, _), f, theta in zip(slots, latent, thetas):
-                    _produce_model(gps[p], eng, Xt, f, theta)
-                    if is_cuda_tensor(Xv):
-                        raw[p][:, c] = _host_predictions(eng.predict_tensor(Xv, with_variance=False)[0])
-                    else:
-                        raw[p][:, c], _ = eng.predict(Xv, with_variance=False)
+                    produce(gps[p], eng, Xt, f, theta)
+                    raw[p][:, c] = _latent_mean(eng, Xv)
             finally:
                 eng.release()
         if ovr:
             preds = [one_vs_rest_prediction(r) for r in raw]
         else:                                               # GaussianProcessClassificationModel.predict
-            preds = [np.argmax(np.stack([-r[:, 0], r[:, 0]], axis=-1), axis=-1).astype(np.float64) for r in raw]
+            preds = [binary_prediction(np.stack([-r[:, 0], r[:, 0]], axis=-1)) for r in raw]
         return preds, raw, dict(groups=groups)
