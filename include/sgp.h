@@ -230,6 +230,21 @@ int sgp_experts_upload_folds(sgp_ctx* ctx, const void* X, int32_t x_is_f32, cons
  * allocation or launch. */
 int sgp_experts_upload_folds_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, const double* dy, int64_t n,
                                     int32_t d, const int32_t* fold_of, int32_t n_folds, int32_t dataset_size_for_expert);
+/* The training sets of a data-parallel model selection, stored as sgp_experts_upload_folds stores its sets.  dX / dy
+ * hold n_sets blocks one after another: block k has set_rows[k] rows, the rows of training set k that this rank's
+ * experts own, in the set's row order.  Row i of block k goes to local expert i % set_experts[k] of set k.
+ * Per set, one expert-offset launch and one gather of the block, by the fold upload's kernels and arithmetic.  It fills
+ * the state sgp_experts_upload_folds fills (the sets, their experts and largest experts, the reset latent and one-vs-rest
+ * modes), so sgp_bcm_nll_folds, sgp_laplace_nll_fold_slots_any_size, sgp_experts_get_f_fold_slot and
+ * sgp_experts_get_f_fold_rows_device read it unchanged; like the fold upload, its modes are read per set.
+ * Contract: with block k the plain fold set X[fold_of != k] and set_experts[k] = Math.round(N_k / dataset_size_for_expert),
+ * every fold-slot value, gradient and mode equals the one after sgp_experts_upload_folds_device, bit for bit.
+ * SGP_E_BADARG for null pointers, n_sets < 1, d < 1, set_rows[k] < 1, set_experts[k] < 1, set_experts[k] > set_rows[k]
+ * (an empty expert), and for pointers that are not device memory on the context's device; SGP_E_NOMEM under the fold
+ * upload's free-memory rule (the sets' rows, labels and modes, sum set_rows (d + 2) * 8 bytes).  Every refusal comes
+ * before any allocation or launch. */
+int sgp_experts_upload_fold_sets_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, const double* dy,
+                                        const int64_t* set_rows, const int64_t* set_experts, int32_t n_sets, int32_t d);
 
 /* The BCM objective of sgp_bcm_nll on several training sets of the last sgp_experts_upload_folds, in one launch over
  * experts x slots.  Slot s evaluates set sets[s] at its own kernels[s] and hypers[s * n_hypers ...] (the same kernel

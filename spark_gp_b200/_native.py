@@ -30,7 +30,8 @@ EXPORTS = ["sgp_ctx_create", "sgp_ctx_destroy", "sgp_last_error", "sgp_set_preci
            "sgp_greedy_active_set_device", "sgp_laplace_nll_fold_slots_any_size", "sgp_experts_get_f_fold_slot",
            "sgp_experts_get_f_fold_rows_device", "sgp_gauss_hermite_rule", "sgp_predict_probability",
            "sgp_predict_probability_device", "sgp_bcm_nll_slots", "sgp_kernel_eval", "sgp_kernel_eval_device",
-           "sgp_experts_upload_strided_device", "sgp_kmeans_sharded", "sgp_kmeans_sharded_device"]
+           "sgp_experts_upload_strided_device", "sgp_kmeans_sharded", "sgp_kmeans_sharded_device",
+           "sgp_experts_upload_fold_sets_device"]
 
 
 class KernelTerm(C.Structure):
@@ -123,6 +124,7 @@ def load() -> C.CDLL:
     lib.sgp_kernel_eval.argtypes = [vp, C.POINTER(KernelDesc), vp, i32, vp, i32, i64, vp, i32, i32, i32, vp, vp]
     lib.sgp_kernel_eval_device.argtypes = lib.sgp_kernel_eval.argtypes
     lib.sgp_experts_upload_strided_device.argtypes = [vp, vp, i32, vp, i64, i32, i64]
+    lib.sgp_experts_upload_fold_sets_device.argtypes = [vp, vp, i32, vp, vp, vp, i32, i32]
     lib.sgp_kmeans_sharded.argtypes = [vp, vp, i32, i64, i64, i64, i32, i32, i32, C.c_double, i64, vp, vp, vp, vp, vp, vp]
     lib.sgp_kmeans_sharded_device.argtypes = lib.sgp_kmeans_sharded.argtypes
     lib.sgp_event_elapsed_ms.argtypes = [vp, C.c_int, C.c_int, dp]

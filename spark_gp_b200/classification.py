@@ -107,20 +107,26 @@ def assert_labels_are_01(y):
         raise RuntimeError("Only 0 and 1 labels are supported.")
 
 
-def laplace_fit(gps, eng, X, y, entry, store, index, thetas=None):
+def laplace_fit(gps, eng, X, y, entry, store, index, thetas=None, upload=None):
     """The Laplace part of the binary fit (GPCls:53-60) for slot i of classifier gps[i], on one upload of (X, y) into eng
     grouped by gps[0]'s datasetSizeForExpert (every slot's modes start at 0), fitted by `fit_slots` from each classifier's
     kernel with gps[0]'s bounds, maxIter and tol.
       entry(slots, kernels) -> (values, gradients): the listed slots' Laplace objective (`slot_objective`), warm-started
                                                     from and moving their device-resident modes;
-      store, index(i):                              where slot i's modes live (N.SGP_MODES_*, and the class or mode slot).
+      store, index(i):                              where slot i's modes live (N.SGP_MODES_*, and the class or mode slot);
+      upload(eng) -> (rows, experts):               another grouped upload in place of (X, y)'s (a data-parallel model
+                                                    selection's rank uploads its experts' rows), X then only saying
+                                                    on which side the modes go.
     Returns (thetas, modes [slot][row] in row order -- a CUDA float64 tensor, ungrouped on the device, when X is a CUDA
     tensor --, the fit record of `fit_slots`)."""
-    n_experts = expert_count(len(X), gps[0]._datasetSizeForExpert)
-    eng.experts_upload_grouped(X, y, gps[0]._datasetSizeForExpert)
+    if upload is None:
+        n_rows, n_experts = len(X), expert_count(len(X), gps[0]._datasetSizeForExpert)
+        eng.experts_upload_grouped(X, y, gps[0]._datasetSizeForExpert)
+    else:
+        n_rows, n_experts = upload(eng)
     thetas, fit = fit_slots(eng, gps[0], slot_objective(gps, entry), [gp.getKernel().getHyperparameters() for gp in gps],
                             thetas, laplace=True)
-    latent = [slot_modes(eng, is_cuda_tensor(X), len(X), n_experts, store, index(i)) for i in range(len(gps))]
+    latent = [slot_modes(eng, is_cuda_tensor(X), n_rows, n_experts, store, index(i)) for i in range(len(gps))]
     if is_cuda_tensor(X):
         import torch
         return thetas, torch.stack(latent), fit

@@ -964,6 +964,19 @@ int upload_grouped(Ctx* c, bool on_device, const void* X, int x_is_f32, const do
   return upload_strided(c, on_device, X, x_is_f32, y, n, d, E);
 }
 
+// The free-memory rule of the fold uploads: the sets' rows, labels and modes, n_rows (d + 2) doubles, against what the
+// device has free plus what the context's expert buffers already hold.
+int fold_sets_fit(Ctx* c, long long n_rows, int d, const char* entry) {
+  size_t free_b = 0, total_b = 0;
+  SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+  const size_t held = c->ex_X.cap + c->ex_y.cap + c->ex_f.buf.cap;
+  const size_t need = static_cast<size_t>(n_rows) * (static_cast<size_t>(d) + 2) * 8;
+  if (need > free_b + held)
+    return fail(c, SGP_E_NOMEM, std::string(entry) + ": the training sets need " + std::to_string(need >> 20) +
+                                    " MiB of device memory, " + std::to_string((free_b + held) >> 20) + " MiB available");
+  return SGP_OK;
+}
+
 // sgp_experts_upload_folds and its _device form; fold_of is host memory in both
 int upload_folds(Ctx* c, bool on_device, const void* X, int x_is_f32, const double* y, long long n, int d,
                  const int32_t* fold_of, int n_folds, int dataset_size_for_expert, const char* entry) {
@@ -1001,16 +1014,9 @@ int upload_folds(Ctx* c, bool on_device, const void* X, int x_is_f32, const doub
   }
   const long long n_rows = row0[n_folds], E = first[n_folds];
   SGP_CUDA(c, cudaSetDevice(c->device));
-  {                                           // the sets' rows, labels and modes, (n_folds - 1) n (d + 2) doubles
-    size_t free_b = 0, total_b = 0;
-    SGP_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
-    const size_t held = c->ex_X.cap + c->ex_y.cap + c->ex_f.buf.cap;
-    const size_t need = static_cast<size_t>(n_rows) * (static_cast<size_t>(d) + 2) * 8;
-    if (need > free_b + held)
-      return fail(c, SGP_E_NOMEM, std::string(entry) + ": the training sets need " + std::to_string(need >> 20) +
-                                      " MiB of device memory, " + std::to_string((free_b + held) >> 20) + " MiB available");
-  }
-  int rc = experts_alloc(c, E, n_rows, d, *std::max_element(nmax.begin(), nmax.end()));
+  int rc = fold_sets_fit(c, n_rows, d, entry);              // (n_folds - 1) n (d + 2) doubles
+  if (rc != SGP_OK) return rc;
+  rc = experts_alloc(c, E, n_rows, d, *std::max_element(nmax.begin(), nmax.end()));
   if (rc == SGP_OK) rc = ctx_scratch(c, c->fold_pos_ws, static_cast<size_t>(n) * 8);
   if (rc != SGP_OK) return rc;
   const long long* dpos = c->fold_pos_ws.as<long long>();
@@ -1042,6 +1048,59 @@ int upload_folds(Ctx* c, bool on_device, const void* X, int x_is_f32, const doub
   return SGP_OK;
 }
 }  // namespace
+
+int sgp_experts_upload_fold_sets_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, const double* dy,
+                                        const int64_t* set_rows, const int64_t* set_experts, int32_t n_sets, int32_t d) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  const char* entry = "sgp_experts_upload_fold_sets_device";
+  if (!dX || !dy || !set_rows || !set_experts || n_sets < 1 || d < 1)
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": null or empty argument");
+  // set k: set_rows[k] rows in set_experts[k] experts, stored after set k-1, as upload_folds stores its sets
+  std::vector<long long> first(static_cast<size_t>(n_sets) + 1, 0), row0(static_cast<size_t>(n_sets) + 1, 0);
+  std::vector<int> nmax(n_sets);
+  for (int k = 0; k < n_sets; ++k) {
+    const long long Nk = set_rows[k], Ek = set_experts[k];
+    if (Nk < 1 || Ek < 1)
+      return fail(c, SGP_E_BADARG, std::string(entry) + ": set " + std::to_string(k) + " has no rows or no experts");
+    if (Ek > Nk)
+      return fail(c, SGP_E_BADARG, std::string(entry) + ": set " + std::to_string(k) +
+                                       ": more experts than rows (an empty expert)");
+    first[k + 1] = first[k] + Ek;
+    row0[k + 1] = row0[k] + Nk;
+    nmax[k] = static_cast<int>(Nk / Ek + ((Nk % Ek) ? 1 : 0));
+  }
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  int rc = device_ptr_ok(c, dX, entry, "X");
+  if (rc == SGP_OK) rc = device_ptr_ok(c, dy, entry, "y");
+  if (rc == SGP_OK) rc = fold_sets_fit(c, row0[n_sets], d, entry);
+  if (rc == SGP_OK) rc = experts_alloc(c, first[n_sets], row0[n_sets], d, *std::max_element(nmax.begin(), nmax.end()));
+  if (rc != SGP_OK) return rc;
+  for (int k = 0; k < n_sets; ++k) {
+    SGP_CUDA(c, launch_expert_offsets(c->ex.off + first[k], row0[k + 1] - row0[k], first[k + 1] - first[k], row0[k],
+                                      c->stream));
+    c->launches += 1;
+  }
+  // block k is set k's rows in order: the fold upload's gather with no left-out points, in chunks of the same size
+  const size_t row = static_cast<size_t>(d) * (x_is_f32 ? 4 : 8);
+  const char* X = static_cast<const char*>(dX);
+  for (int k = 0; k < n_sets; ++k) {
+    const long long Nk = row0[k + 1] - row0[k], chunk = group_chunk(Nk, row);
+    for (long long p0 = 0; p0 < Nk; p0 += chunk) {
+      const long long cn = std::min(chunk, Nk - p0), at = row0[k] + p0;
+      SGP_CUDA(c, launch_group_experts(c->ex.X + static_cast<size_t>(row0[k]) * d, c->ex.y + row0[k],
+                                       X + static_cast<size_t>(at) * row, x_is_f32, dy + at, Nk, d,
+                                       first[k + 1] - first[k], p0, cn, nullptr, 0, c->stream));
+      c->launches += 1;
+    }
+  }
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  c->fold_first = first;
+  c->fold_nmax = nmax;
+  c->fold_row0 = row0;
+  c->ex.E = first[n_sets];
+  return SGP_OK;
+}
 
 int sgp_experts_upload_grouped(sgp_ctx* h, const void* X, int32_t x_is_f32, const double* y, int64_t n, int32_t d,
                                int32_t dataset_size_for_expert) {

@@ -19,6 +19,10 @@ A rank that returns before a collective leaves its peers blocked in it.  So befo
 states the refusals it can compute (its data, the global sizes), the ranks exchange them, and if any rank would refuse,
 every rank raises the same exception.  The SGP_E_NOMEM checks depend on each rank's free memory and are not agreed.
 
+The model selectors over a group (`selection`, `Selection`) reuse these steps with several training sets: one
+`ShardPlan` per set, one all-to-all that moves each row once per set it belongs to (`exchange_sets`), and one gather of
+the ranks' validation labels and predictions, so that every rank scores the same arrays.
+
 `engine_factory` is the context class (a test passes a stand-in)."""
 from __future__ import annotations
 
@@ -105,6 +109,12 @@ def group_refusal(plan: ShardPlan, infos, classifier: bool, experts: bool):
         return "ValueError", "every rank's shard is empty"
     if not experts:
         return None
+    return expert_refusal(plan, classifier)
+
+
+def expert_refusal(plan: ShardPlan, classifier: bool):
+    """The expert grouping's limits over the plan's ranks, or None: no expert, fewer experts than ranks, or an expert above
+    the BCM / Laplace point limit.  Returns (exception class name, message)."""
     if plan.E <= 0:
         return "ZeroDivisionError", "numberOfExperts == 0 (N < datasetSizeForExpert / 2)"
     if plan.E < plan.R:
@@ -142,22 +152,44 @@ def agree(group, n: int, d: int, dtype: str, err, dataset_size_for_expert: int, 
 def exchange(plan: ShardPlan, X, y, group):
     """Moves every row of the shard (torch tensors X n x d, y n, on the group's device) to its expert's owner in one
     all-to-all of the rows' bytes with y appended.  Returns (X, y) of the rows this rank owns, in global row order."""
+    return exchange_sets([plan], [None], X, y, group)[:2]
+
+
+def exchange_sets(plans, members, X, y, group):
+    """`exchange` of several training sets in one all-to-all: set k holds this rank's rows where the host bool mask
+    members[k] is set (None: every row), in row order, and plans[k] is its `ShardPlan` over the ranks' rows of the set.
+    A row moves once per set it belongs to, to the owner of its expert in that set.  Each rank sends its rows ordered by
+    (destination, set, row) and orders what it receives by (set, source rank, row): global row order within each set.
+    Returns (X, y, rows): the rows this rank owns, set after set, and rows[k], the size of set k's block."""
     import torch
     dist = _dist()
     d, es = X.shape[1], X.element_size()
-    order = torch.as_tensor(np.argsort(plan.destinations(), kind="stable"), device=X.device)
+    R, S = plans[0].R, len(plans)
+    local = [np.arange(len(X)) if m is None else np.flatnonzero(m) for m in members]
+    dest = np.concatenate([p.destinations() for p in plans]).astype(np.int64)
+    setof = np.concatenate([np.full(len(i), k, dtype=np.int64) for k, i in enumerate(local)])
+    order = np.argsort(dest * S + setof, kind="stable")
+    src = torch.as_tensor(np.concatenate(local)[order], device=X.device)
     rows = torch.empty((0, d * es + 8), dtype=torch.uint8, device=X.device)
-    if len(X):
+    if len(src):
         rows = torch.cat([X.contiguous().view(torch.uint8).reshape(len(X), d * es),
-                          y.reshape(len(y), 1).to(torch.float64).view(torch.uint8)], dim=1)[order].contiguous()
-    send, recv = plan.send_counts(), plan.recv_counts()
+                          y.reshape(len(y), 1).to(torch.float64).view(torch.uint8)], dim=1)[src].contiguous()
+    send = np.bincount(dest, minlength=R).astype(np.int64)
+    # counts[s, k]: the rows of set k that rank s sends here
+    counts = np.array([[int((p.destinations(s) == p.rank).sum()) for p in plans] for s in range(R)], dtype=np.int64)
+    recv = counts.sum(axis=1)
     out = torch.empty((int(recv.sum()), d * es + 8), dtype=torch.uint8, device=X.device)
     dist.all_to_all_single(out, rows, recv.tolist(), send.tolist(), group=group)
+    if S > 1 and len(out):
+        at = np.concatenate([[0], np.cumsum(counts.ravel())]).reshape(-1)[:-1].reshape(R, S)
+        out = out[torch.as_tensor(np.concatenate([np.arange(at[s, k], at[s, k] + counts[s, k])
+                                                  for k in range(S) for s in range(R)]), device=X.device)]
+    set_rows = counts.sum(axis=0)
     if len(out) == 0:
-        return X.new_empty((0, d)), y.new_empty(0, dtype=torch.float64)
+        return X.new_empty((0, d)), y.new_empty(0, dtype=torch.float64), set_rows
     Xr = out[:, :d * es].contiguous().view(X.dtype).reshape(len(out), d)
     yr = out[:, d * es:].contiguous().view(torch.float64).reshape(len(out))
-    return Xr, yr
+    return Xr, yr, set_rows
 
 
 def gather_rows(plan: ShardPlan, X, idx, group, device):
@@ -350,3 +382,189 @@ def _fit(gp, plan, eng, X, y, hyperparameters, kind, n_classes, dtype, group, de
         f = slot_modes(eng, is_cuda_tensor(X), n_e, plan.local_experts, store, i)
         slots.append(produce(gp, eng, Xe, f, theta, active_set(gp, plan, eng, X, theta, group, device))._replace(latent=f))
     return slots, record
+
+
+# ---- model selection over the group (`tuning.CrossValidator` / `TrainValidationSplit` with a process group) ----------
+def set_refusal(N: int, sizes, n_es, classifier: bool, validation):
+    """The refusal of a selection's training sets over N rows from every rank's rows in every set (sizes, R x n_sets), or
+    None: validation(N, N_k per set) names an empty validation side (the plain selector's message, or None), then for
+    every datasetSizeForExpert in n_es (the maps whose fit groups experts) and every set, `expert_refusal` of the set's
+    plan, named by set.  Returns (exception class name, message)."""
+    sizes = np.asarray(sizes, dtype=np.int64)
+    message = validation(int(N), sizes.sum(axis=0))
+    if message is not None:
+        return "ValueError", message
+    for n_e in sorted(set(n_es)):
+        for k in range(sizes.shape[1]):
+            verdict = expert_refusal(ShardPlan(sizes[:, k], 0, n_e), classifier)
+            if verdict is not None:
+                return verdict[0], "training set %d: %s" % (k, verdict[1])
+    return None
+
+
+def selection_refusal(infos, classifier: bool, n_es, validation):
+    """The refusal of a model selection over the group from every rank's entry (n, d, dtype, refusal, largest label, rows
+    per set, largest label per set), or None: `group_refusal` without experts, then `set_refusal`."""
+    plan = ShardPlan([i[0] for i in infos], 0, 1)
+    verdict = group_refusal(plan, infos, classifier, False)
+    if verdict is None:
+        verdict = set_refusal(plan.N, [i[5] for i in infos], n_es, classifier, validation)
+    return verdict
+
+
+class Selection:
+    """A model selection's side of the group, for the selectors' drivers (`tuning`): the group's context with a
+    communicator, this rank's rows of every training set (members[k], a host bool mask of its shard) and every rank's
+    count of them (sizes, R x n_sets), the sets regrouped across ranks for the slot fits, the fold models over the set
+    plans, and the gathered validation arrays.  classes[k]: one-vs-rest's C_k of set k (the maximum label over ranks
+    plus one)."""
+
+    def __init__(self, group, device, eng, X, y, members, sizes, classes):
+        self.group, self.device, self.eng = group, device, eng
+        self.X, self.y, self.members = X, y, members
+        self.sizes, self.classes = np.asarray(sizes, dtype=np.int64), classes
+        self.rank = _dist().get_rank(group)
+        self.on_device = is_cuda_tensor(X)
+        self._blocks = {}
+
+    def plan(self, k: int, dataset_size_for_expert: int = 1) -> ShardPlan:
+        return ShardPlan(self.sizes[:, k], self.rank, dataset_size_for_expert)
+
+    def context(self, device):
+        import contextlib
+        return contextlib.nullcontext(self.eng)
+
+    def gather(self, v):
+        """Every rank's v (its validation rows' labels or predictions) as one host float64 array, in rank order: global
+        row order."""
+        dist = _dist()
+        parts = [None] * dist.get_world_size(self.group)
+        dist.all_gather_object(parts, np.asarray(v.cpu().numpy() if is_cuda_tensor(v) else v, dtype=np.float64),
+                               group=self.group)
+        return np.concatenate(parts)
+
+    def blocks(self, dataset_size_for_expert: int):
+        """(X, y, rows, local experts) of this rank's experts of every training set (`exchange_sets`), kept per
+        datasetSizeForExpert for the fold models."""
+        import torch
+        n_e = int(dataset_size_for_expert)
+        if n_e not in self._blocks:
+            plans = [self.plan(k, n_e) for k in range(len(self.members))]
+            X = _tensor(self.X, self.device, getattr(torch, str(self.X.dtype).replace("torch.", "")))
+            Xe, ye, rows = exchange_sets(plans, self.members, X, _tensor(self.y, self.device, torch.float64), self.group)
+            self._blocks[n_e] = (Xe, ye, rows, [p.local_experts for p in plans], [p.E for p in plans])
+        return self._blocks[n_e]
+
+    def upload_sets(self, eng, dataset_size_for_expert: int):
+        """Uploads this rank's experts of every training set (`experts_upload_fold_sets`).  Returns (rows, experts) per
+        set."""
+        Xe, ye, rows, experts, _ = self.blocks(dataset_size_for_expert)
+        eng.experts_upload_fold_sets(Xe, ye, rows, experts)
+        return rows, experts
+
+    def set_classes(self, ovr: bool):
+        """C_k of every training set: the agreed one-vs-rest counts, or 1 for the binary classifier (the labels were
+        checked before the agreement)."""
+        return list(self.classes) if ovr else [1] * len(self.members)
+
+    def upload_training(self, eng, dataset_size_for_expert: int, Xt=None, yt=None, laplace: bool = False):
+        """Uploads this rank's experts of the one training set (`experts_upload_strided`) in place of the training rows
+        (Xt, yt).  Returns (rows, local experts, the set's number of experts)."""
+        Xe, ye, rows, experts, E = self.blocks(dataset_size_for_expert)
+        eng.experts_upload_strided(Xe, ye, experts[0])
+        return int(rows[0]), experts[0], E[0]
+
+    def validate(self, est, k: int, Xt, yt, Xv, theta):
+        """The regression's fold model of set k at theta (its own set-k rows Xt, yt, the active set of the set) on the
+        group's context, and its gathered validation predictions.  Returns (predictions, magic vector)."""
+        fitted = produce(est, self.eng, Xt, yt, theta,
+                         active_set(est, self.plan(k), self.eng, Xt, theta, self.group, self.device))
+        return self.gather(self.latent_mean(self.eng, Xv)), fitted.magic_vector
+
+    def fold_model(self, gp, eng, k: int, Xt, f, theta):
+        """The classifier's model of set k at theta on the group's context: the statistics of this rank's set-k expert
+        rows with the slot's modes f as labels, the active set of the set over its own set-k rows Xt."""
+        Xe, _, rows, _, _ = self.blocks(gp._datasetSizeForExpert)
+        lo = int(np.sum(rows[:k]))
+        Xk = Xe[lo:lo + int(rows[k])]
+        if not self.on_device:
+            Xk = Xk.cpu().numpy()
+        return produce(gp, eng, Xk, f, theta, active_set(gp, self.plan(k), eng, Xt, theta, self.group, self.device))
+
+    @staticmethod
+    def latent_mean(eng, Xv):
+        """The latent mean of the model eng holds at this rank's validation rows (host float64; none on a rank without
+        any)."""
+        if len(Xv) == 0:
+            return np.empty(0)
+        if is_cuda_tensor(Xv):
+            return eng.predict_tensor(Xv, with_variance=False)[0].cpu().numpy().astype(np.float64)
+        return eng.predict(Xv, with_variance=False)[0]
+
+
+def selection(gp, estimators, kind: str, X, y, split, what: str, validation, engine_factory=ProjectedProcessEngine):
+    """The set-up of a model selection over gp's process group on this rank's shard, as a context manager yielding a
+    `Selection`.  gp: the estimator with the group (the wrapped classifier of one-vs-rest); estimators: one per param map
+    (their providers and datasetSizeForExpert are checked); kind as in `group_fit`.  split(n, offset) -> the host bool
+    masks of the rank's rows in each training set, the rank's rows being the global rows [offset, offset + n)
+    (ValueError for a bad given split).  validation(N, N_k) -> the plain selector's message for an empty validation
+    side, or None.
+    Two collectives come before any context: the shard sizes (the seeded splits number the rows globally), then the
+    agreement, after which every rank raises the same exception for any rank's refusal.  A failure after the agreement
+    drops the communicator context, as `group_fit` does."""
+    import contextlib
+
+    import torch
+    dist = _dist()
+    group = gp._process_group
+    classifier = kind != "regression"
+    nccl = dist.get_backend(group) == "nccl"
+    device = torch.device("cuda", gp._device) if nccl else torch.device("cpu")
+    R, rank = dist.get_world_size(group), dist.get_rank(group)
+    n_es = [e._datasetSizeForExpert for e in estimators if classifier or e._maxIter > 0]
+
+    @contextlib.contextmanager
+    def run():
+        with torch.cuda.device(gp._device) if nccl else contextlib.nullcontext():
+            err, n, d, dtype, top, Xl, yl = None, 0, -1, "", -1, X, y
+            try:
+                for e in estimators:
+                    check_provider(e._activeSetProvider)
+                Xl, yl, top = _local_data(X, y, gp._device, kind, what)
+                n, d, dtype = len(Xl), Xl.shape[1], str(Xl.dtype).replace("torch.", "")
+            except (ValueError, TypeError, RuntimeError) as e:
+                err = (type(e).__name__, str(e))
+            counts = [None] * R
+            dist.all_gather_object(counts, int(n), group=group)
+            members, rows, tops = [], [], []
+            if err is None:
+                try:
+                    members = split(n, int(sum(counts[:rank])))
+                    rows = [int(np.count_nonzero(m)) for m in members]
+                    yh = np.asarray(yl.cpu().numpy() if is_cuda_tensor(yl) else yl)
+                    tops = [int(yh[m].max()) if kind == "classes" and m.any() else -1 for m in members]
+                except ValueError as e:
+                    err = (type(e).__name__, str(e))
+            infos = [None] * R
+            dist.all_gather_object(infos, (int(n), int(d), str(dtype), err, int(top), rows, tops), group=group)
+            verdict = selection_refusal(infos, classifier, n_es, validation)
+            if verdict is not None:
+                raise _EXCEPTIONS.get(verdict[0], RuntimeError)(verdict[1])
+            first = next(i for i in infos if i[0] > 0)
+            if n == 0:                                      # an empty shard takes the agreed dtype and width
+                Xl = np.empty((0, first[1]), dtype=np.float32 if first[2] == "float32" else np.float64)
+                yl = np.empty(0)
+                members = [np.zeros(0, dtype=bool) for _ in first[5]]
+            sizes = np.array([i[5] if i[0] > 0 else [0] * len(first[5]) for i in infos], dtype=np.int64)
+            classes = [max(i[6][k] if i[0] > 0 else -1 for i in infos) + 1 for k in range(len(first[5]))]
+            key, eng = comm_engine(group, gp._device, device, engine_factory)
+            try:
+                yield Selection(group, device, eng, Xl, yl, members, sizes, classes)
+            except BaseException:
+                # a failure after a collective may leave the ranks out of step: the communicator is not reused
+                if _COMM_ENGINES.get(key) is eng:
+                    _COMM_ENGINES.pop(key)
+                    eng.close()
+                raise
+
+    return run()

@@ -380,6 +380,22 @@ class ProjectedProcessEngine:
         n_k = len(X) - np.bincount(folds, minlength=int(n_folds))
         return np.floor(n_k / dataset_size_for_expert + 0.5).astype(np.int64)
 
+    def experts_upload_fold_sets(self, X, y, set_rows, set_experts):
+        """Uploads training sets given as blocks of CUDA tensor rows (`sgp_experts_upload_fold_sets_device`): block k is
+        the next set_rows[k] rows, grouped row i -> expert i % set_experts[k], and becomes fold set k, as
+        `experts_upload_folds` stores its sets.  A data-parallel model selection's rank uploads its block of every training
+        set's experts with it.  Returns set_experts as an int64 array."""
+        X, y, px, py, f32 = self._device_xy(X, y, "experts_upload_fold_sets")
+        rows = np.ascontiguousarray(set_rows, dtype=np.int64)
+        experts = np.ascontiguousarray(set_experts, dtype=np.int64)
+        if X.ndim != 2 or y.shape != (len(X),) or rows.ndim != 1 or experts.shape != rows.shape \
+                or int(rows.sum()) != len(X):
+            raise ValueError("experts_upload_fold_sets: X must be n x d, y n entries, and set_rows sum to n")
+        self._check(self._lib.sgp_experts_upload_fold_sets_device(self._h, px, f32, py, N.ptr(rows), N.ptr(experts),
+                                                                  len(rows), X.shape[1]))
+        self._experts_d = X.shape[1]
+        return experts
+
     def _batched_objective(self, fn, head, kernels, tail=()):
         """Runs one batched per-expert objective of the library, `fn(ctx, *head, descs, hypers, n_hypers, *tail, values,
         gradients)`, with one evaluation per kernel.  Returns (values [n_eval], gradients [n_eval x n_hypers])."""

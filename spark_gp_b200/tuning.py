@@ -52,8 +52,21 @@ CrossValidator does not take it, as it does not take the binary classifier.
 Both selectors take X (and y) as CUDA tensors on the estimator's device as well: the fold upload reads them in place
 (`sgp_experts_upload_folds_device`), the training and validation rows are gathered on the device and predicted there, and
 only the validation labels and predictions go to the host, for the evaluator.  `folds=` and `train=` stay host arrays.
-The results are the host fit's, bit for bit."""
+The results are the host fit's, bit for bit.
+
+Over a process group (the estimator, or one-vs-rest's classifier, built with `process_group=`), every rank passes its
+own shard, host array or CUDA tensor, uneven or empty, and a given `folds=` / `train=` is its slice of the split.  The
+seeded splits draw at the global row index (`kfold_assignment(..., offset)`), so they are the plain splits of the
+concatenation.  The drivers below are the plain ones, handed a `distributed.Selection` in place of `_Local`: every
+training set's rows move to their experts' owners (`sgp_experts_upload_fold_sets_device`, or the strided upload for the
+one training set of a split), the slot groups run in lock step on the group's context over the all-reducing batched
+objectives, each fold or map model is produced there with the set's active set, each rank predicts its own validation
+rows and one gather gives every rank every rank's labels and predictions in rank order.  So the metrics, bestIndex and
+the refitted map (the group fit of the estimator) are the same on every rank, and at one rank they are the plain
+selector's bit for bit (DESIGN.md section 5)."""
 from __future__ import annotations
+
+import contextlib
 
 import numpy as np
 
@@ -61,7 +74,7 @@ from . import _native as N
 from .classification import GaussianProcessClassifier, OneVsRest, assert_labels_are_01, binary_prediction, laplace_fit, \
     one_vs_rest_labels, one_vs_rest_prediction
 from .engine import ProjectedProcessEngine, host_copy, is_cuda_tensor, take_rows
-from .hyperopt import fit_data, fit_slots, lbfgsb_bounds, produce, slot_modes, slot_objective
+from .hyperopt import expert_count, fit_data, fit_slots, lbfgsb_bounds, produce, slot_modes, slot_objective
 from .regression import GaussianProcessRegression
 from .utils import kfold_assignment, train_validation_assignment
 
@@ -343,23 +356,82 @@ def _validate(est, Xt, yt, Xv, theta):
     return _host_predictions(model.predict(Xv)), model.rawPredictor.magicVector
 
 
-def _bcm_groups(ests, n: int, upload, entry):
+@contextlib.contextmanager
+def _pooled(device: int):
+    """A context of the device's pool for the span of a `with`."""
+    eng = ProjectedProcessEngine.acquire(device)
+    try:
+        yield eng
+    finally:
+        eng.release()
+
+
+class _Local:
+    """The plain selectors' side of the drivers below, on this process's rows: members[k] is the host bool mask of
+    training set k (fold_of != k, or the training mask), the slot fits run on pooled contexts over the sets uploaded from
+    every row, each fold model is the independent fit's, and the validation arrays are this process's.  Over a process
+    group `distributed.Selection` takes its place, with the same methods."""
+
+    def __init__(self, X, y, members, fold_of=None):
+        self.X, self.y, self.members, self.fold_of = X, y, members, fold_of
+        self.on_device = is_cuda_tensor(X)
+
+    context = staticmethod(_pooled)
+
+    @staticmethod
+    def gather(v):
+        return np.asarray(host_copy(v), dtype=np.float64)
+
+    def set_classes(self, ovr: bool):
+        """C_k of every training set: one-vs-rest's max(y[train]) + 1, as an independent OneVsRest.fit(X[train],
+        y[train]) counts them (the labels checked first), or 1 for the binary classifier (its labels checked)."""
+        if not ovr:
+            assert_labels_are_01(self.y)
+            return [1] * len(self.members)
+        one_vs_rest_labels(self.y)
+        return [one_vs_rest_labels(_rows(self.y, t))[1] for t in self.members]
+
+    def upload_sets(self, eng, dataset_size_for_expert: int):
+        """The fold upload of every training set.  Returns (rows, experts) per set."""
+        rows = [int(np.count_nonzero(t)) for t in self.members]
+        return rows, eng.experts_upload_folds(self.X, self.y, self.fold_of, len(self.members), dataset_size_for_expert)
+
+    @staticmethod
+    def upload_training(eng, dataset_size_for_expert: int, Xt, yt, laplace: bool = False):
+        """The grouped upload of the one training set (Xt, yt).  Returns (rows, experts, experts)."""
+        if laplace:
+            expert_count(len(Xt), dataset_size_for_expert)
+        n_experts = eng.experts_upload_grouped(Xt, yt, dataset_size_for_expert)
+        return len(Xt), n_experts, n_experts
+
+    @staticmethod
+    def validate(est, k: int, Xt, yt, Xv, theta):
+        return _validate(est, Xt, yt, Xv, theta)
+
+    @staticmethod
+    def fold_model(gp, eng, k: int, Xt, f, theta):
+        return produce(gp, eng, Xt, f, theta)
+
+    @staticmethod
+    def latent_mean(eng, Xv):
+        return _latent_mean(eng, Xv)
+
+
+def _bcm_groups(ests, n: int, upload, entry, context=_pooled):
     """The lock-step BCM optimisation of each group of (map p, j) slots, j in [0, n) (`group_slots`), on one context of
-    its own: upload(eng, datasetSizeForExpert) uploads the training rows, entry(eng, slots, kernels) evaluates the listed
-    slots in one launch.  A group with maxIter <= 0 is skipped: it takes its kernels' own hyper-parameters, as GPR.fit
-    does.  Yields (slots, thetas, the `fit_slots` record, upload's return) per optimised group."""
+    its own (`context(device)`, a context manager; a pooled one by default): upload(eng, datasetSizeForExpert) uploads the
+    training rows, entry(eng, slots, kernels) evaluates the listed slots in one launch.  A group with maxIter <= 0 is
+    skipped: it takes its kernels' own hyper-parameters, as GPR.fit does.  Yields (slots, thetas, the `fit_slots` record,
+    upload's return) per optimised group."""
     for slots in group_slots(ests, n).values():
         e0 = ests[slots[0][0]]
         if e0._maxIter <= 0:
             continue
-        eng = ProjectedProcessEngine.acquire(e0._device)
-        try:
+        with context(e0._device) as eng:
             uploaded = upload(eng, e0._datasetSizeForExpert)
             objective = slot_objective([ests[p] for p, _ in slots],
                                        lambda listed, kernels: entry(eng, [slots[i] for i in listed], kernels))
             thetas, fit = fit_slots(eng, e0, objective, [ests[p].getKernel().getHyperparameters() for p, _ in slots])
-        finally:
-            eng.release()
         yield slots, thetas, fit, uploaded
 
 
@@ -410,68 +482,94 @@ class CrossValidator(_Validator):
         return self._num_folds
 
     def fit(self, X, y, folds=None) -> CrossValidatorModel:
-        """folds: the fold of every row (integers in [0, numFolds)); default: the seeded split of the module docstring."""
+        """folds: the fold of every row (integers in [0, numFolds)); default: the seeded split of the module docstring.
+        When the estimator (or the wrapped classifier) has a process group, (X, y) and folds are this rank's shard of
+        the rows (`distributed.selection`); every rank returns the same metrics, bestIndex and refitted model."""
         est = self._estimator
         if est is None:
             raise TypeError("CrossValidator: setEstimator(GaussianProcessRegression or OneVsRest) first")
         ovr = isinstance(est, OneVsRest)
         if ovr and not isinstance(est.getClassifier(), GaussianProcessClassifier):
             raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
-        X, y = self._data(X, y, (est.getClassifier() if ovr else est)._device, ovr)
+        gp = est.getClassifier() if ovr else est
         K = self._num_folds
+        if gp._process_group is not None:
+            from . import distributed
+            ests = [est.copy(m) for m in self._maps or [{}]]
+            split = lambda n, offset: [f != k for f in [self._folds(folds, n, offset)] for k in range(K)]
+            with distributed.selection(gp, [e.getClassifier() if ovr else e for e in ests],
+                                       "classes" if ovr else "regression", X, y, split, self.NAME + ".fit",
+                                       self._empty_fold) as site:
+                return self._cross_validate(site, est, ests, site.X, site.y, (X, y))
+        X, y = self._data(X, y, gp._device, ovr)
+        fold_of = self._folds(folds, len(X), 0)
+        train = [fold_of != k for k in range(K)]
+        message = self._empty_fold(len(X), [int(np.count_nonzero(t)) for t in train])
+        if message is not None:
+            raise ValueError(message)
+        ests = [est.copy(m) for m in self._maps or [{}]]
+        return self._cross_validate(_Local(X, y, train, fold_of), est, ests, X, y, (X, y))
+
+    def _folds(self, folds, n: int, offset: int):
+        """The fold of each of n rows, the rows [offset, offset + n) of the data: the seeded split, or the given one
+        checked."""
         if folds is None:
-            fold_of = kfold_assignment(len(X), K, self._seed)
-        else:
-            f = np.asarray(folds)
-            if f.shape != (len(X),) or not np.all((f == np.floor(f)) & (f >= 0) & (f < K)):
-                raise ValueError("CrossValidator: folds must hold one integer in [0, numFolds) per row")
-            fold_of = f.astype(np.int32)
-        sizes = np.bincount(fold_of, minlength=K)
-        if np.any(sizes == 0):
-            raise ValueError("CrossValidator: fold %d has no rows to validate on" % int(np.argmin(sizes)))
+            return kfold_assignment(n, self._num_folds, self._seed, offset)
+        f = np.asarray(folds)
+        if f.shape != (n,) or not np.all((f == np.floor(f)) & (f >= 0) & (f < self._num_folds)):
+            raise ValueError("CrossValidator: folds must hold one integer in [0, numFolds) per row")
+        return f.astype(np.int32)
+
+    @staticmethod
+    def _empty_fold(n: int, n_train):
+        """The refusal of a split of n rows whose training set k holds n_train[k] rows: the first empty fold."""
+        empty = [k for k, t in enumerate(n_train) if t == n]
+        return "CrossValidator: fold %d has no rows to validate on" % empty[0] if empty else None
+
+    def _cross_validate(self, site, est, ests, X, y, refit):
+        """Every (map, fold) of the split site.members (fold k's training mask) on the site's rows (X, y): the slot fits,
+        the fold models, their metrics on the gathered validation arrays, and the refit of the best map on refit."""
+        K = len(site.members)
         maps = self._maps or [{}]
-        ests = [est.copy(m) for m in maps]
-        if ovr:
-            folds_out, objective = self._fit_one_vs_rest([e.getClassifier() for e in ests], X, y, fold_of, K)
-            metrics = np.array([[self._evaluator.evaluate(host_copy(_rows(y, fold_of == k)), folds_out[p, k]["prediction"])
-                                 for k in range(K)] for p in range(len(maps))])
-            return self._select(est, maps, X, y, K, metrics, folds_out, objective)
-        thetas, objective = self._optimise(ests, X, y, fold_of, K)
+        y_val = [site.gather(_rows(y, ~t)) for t in site.members]
+        if isinstance(est, OneVsRest):
+            folds_out, objective = self._fit_one_vs_rest([e.getClassifier() for e in ests], X, y, site)
+            metrics = np.array([[self._evaluator.evaluate(y_val[k], folds_out[p, k]["prediction"]) for k in range(K)]
+                                for p in range(len(maps))])
+            return self._select(est, maps, refit, K, metrics, folds_out, objective)
+        thetas, objective = self._optimise(ests, site)
         metrics = np.empty((len(maps), K))
         folds_out = {}
         for p, e in enumerate(ests):
-            for k in range(K):
-                train, val = fold_of != k, fold_of == k
-                pred, mv = _validate(e, _rows(X, train), _rows(y, train), _rows(X, val), thetas[p][k])
+            for k, train in enumerate(site.members):
+                pred, mv = site.validate(e, k, _rows(X, train), _rows(y, train), _rows(X, ~train), thetas[p][k])
                 folds_out[p, k] = dict(theta=thetas[p][k], magicVector=mv, prediction=pred)
-                metrics[p, k] = self._evaluator.evaluate(host_copy(_rows(y, val)), pred)
-        return self._select(est, maps, X, y, K, metrics, folds_out, objective)
+                metrics[p, k] = self._evaluator.evaluate(y_val[k], pred)
+        return self._select(est, maps, refit, K, metrics, folds_out, objective)
 
-    def _select(self, est, maps, X, y, K, metrics, folds_out, objective):
-        """avgMetrics, the first best map refitted on every row, and the records of the fit."""
+    def _select(self, est, maps, refit, K, metrics, folds_out, objective):
+        """avgMetrics, the first best map refitted on the rows refit = (X, y), and the records of the fit."""
         avg = [sum(metrics[p, k] for k in range(K)) / K for p in range(len(maps))]
         best = best_index(avg, self._evaluator.isLargerBetter())
         self.last_folds = folds_out
         objective["fold_metrics"] = metrics
-        return CrossValidatorModel(est.copy(maps[best]).fit(X, y), avg, best, objective)
+        return CrossValidatorModel(est.copy(maps[best]).fit(*refit), avg, best, objective)
 
     @staticmethod
-    def _fit_one_vs_rest(gps, X, y, fold_of, K):
+    def _fit_one_vs_rest(gps, X, y, site):
         """Every (map p, fold k) of one-vs-rest over the classifiers gps (one per map): the fold's C_k class models, as
         `OneVsRest().setClassifier(gps[p]).fit(X[train], y[train])` fits them, and their validation prediction.  Per
-        group of slots one fold upload, one lock-step L-BFGS-B over the (map, fold, class) slots with one
-        `sgp_laplace_nll_fold_slots_any_size` call per round, and one more call at every slot's optimum (GPCls:60).
-        Returns ({(p, k): theta (C_k x h), magicVector [C_k], prediction}, dict(groups=...))."""
-        y = one_vs_rest_labels(y)[0]
-        train = [fold_of != k for k in range(K)]
-        n_k = [int(np.count_nonzero(t)) for t in train]
-        C = [one_vs_rest_labels(_rows(y, t))[1] for t in train]   # as an independent OneVsRest.fit(X[train], y[train])
+        group of slots one upload of the training sets (`site.upload_sets`), one lock-step L-BFGS-B over the (map, fold,
+        class) slots with one `sgp_laplace_nll_fold_slots_any_size` call per round, and one more call at every slot's
+        optimum (GPCls:60).  Returns ({(p, k): theta (C_k x h), magicVector [C_k], prediction}, dict(groups=...))."""
+        train = site.members
+        K = len(train)
+        C = site.set_classes(True)
         thetas, latent, groups = {}, {}, []
         for slots in fold_class_slot_groups(gps, C).values():
             g0 = gps[slots[0][0]]
-            eng = ProjectedProcessEngine.acquire(g0._device)
-            try:
-                n_experts = eng.experts_upload_folds(X, y, fold_of, K, g0._datasetSizeForExpert)
+            with site.context(g0._device) as eng:
+                n_k, n_experts = site.upload_sets(eng, g0._datasetSizeForExpert)
                 entry = lambda listed, kernels: eng.laplace_nll_fold_slots_any_size(
                     len(gps) * sum(C), [slots[i][3] for i in listed], [slots[i][1] for i in listed],
                     [slots[i][2] for i in listed], kernels, g0._tol)
@@ -484,34 +582,31 @@ class CrossValidator(_Validator):
                     rounds=fit["rounds"], calls=fit["rounds"] + 1, launches=fit["launches_total"]))
                 for (p, k, c, m), theta in zip(slots, fitted):
                     thetas[p, k, c] = theta
-                    latent[p, k, c] = slot_modes(eng, is_cuda_tensor(X), n_k[k], n_experts[k], None, m, fold=k)
-            finally:
-                eng.release()
+                    latent[p, k, c] = slot_modes(eng, site.on_device, n_k[k], n_experts[k], None, m, fold=k)
         folds_out = {}
-        eng = ProjectedProcessEngine.acquire(gps[0]._device)
-        try:
+        with site.context(gps[0]._device) as eng:
             for p, gp in enumerate(gps):
                 for k in range(K):
                     Xt, Xv = _rows(X, train[k]), _rows(X, ~train[k])
                     raw, mvs = np.empty((len(Xv), C[k])), []
                     for c in range(C[k]):
-                        mvs.append(produce(gp, eng, Xt, latent[p, k, c], thetas[p, k, c]).magic_vector)
-                        raw[:, c] = _latent_mean(eng, Xv)
+                        mvs.append(site.fold_model(gp, eng, k, Xt, latent[p, k, c], thetas[p, k, c]).magic_vector)
+                        raw[:, c] = site.latent_mean(eng, Xv)
                     folds_out[p, k] = dict(theta=np.array([thetas[p, k, c] for c in range(C[k])]), magicVector=mvs,
-                                           prediction=one_vs_rest_prediction(raw))
-        finally:
-            eng.release()
+                                           prediction=one_vs_rest_prediction(site.gather(raw)))
         return folds_out, dict(groups=groups)
 
     @staticmethod
-    def _optimise(ests, X, y, fold_of, K):
+    def _optimise(ests, site):
         """Optimal hyper-parameters of every (map, fold) slot (thetas[p][k]), and what the optimisation took: per group
-        of slots one fold upload, each round one `sgp_bcm_nll_folds` launch (`_bcm_groups`)."""
+        of slots one upload of the training sets (`site.upload_sets`), each round one `sgp_bcm_nll_folds` launch
+        (`_bcm_groups`)."""
+        K = len(site.members)
         thetas = [[np.asarray(e.getKernel().getHyperparameters(), dtype=np.float64)] * K for e in ests]
         groups = []
         for slots, fitted, fit, _ in _bcm_groups(
-                ests, K, lambda eng, n_e: eng.experts_upload_folds(X, y, fold_of, K, n_e),
-                lambda eng, slots, kernels: eng.bcm_nll_folds([k for _, k in slots], kernels)):
+                ests, K, site.upload_sets, lambda eng, slots, kernels: eng.bcm_nll_folds([k for _, k in slots], kernels),
+                site.context):
             groups.append(dict(slots=[dict(map=p, fold=k, **r) for (p, k), r in zip(slots, fit["slots"])],
                                rounds=fit["rounds"], launches=fit["launches"]))
             for (p, k), theta in zip(slots, fitted):
@@ -567,7 +662,9 @@ class TrainValidationSplit(_Validator):
         return self._train_ratio
 
     def fit(self, X, y, train=None) -> TrainValidationSplitModel:
-        """train: a bool mask of the training rows; default: the seeded split of the module docstring."""
+        """train: a bool mask of the training rows; default: the seeded split of the module docstring.  When the
+        estimator (or the wrapped classifier) has a process group, (X, y) and train are this rank's shard of the rows
+        (`distributed.selection`); every rank returns the same metrics, bestIndex and refitted model."""
         est = self._estimator
         if est is None:
             raise TypeError("TrainValidationSplit: setEstimator first")
@@ -578,96 +675,117 @@ class TrainValidationSplit(_Validator):
             raise TypeError("TrainValidationSplit: a BinaryClassificationEvaluator scores the binary "
                             "GaussianProcessClassifier only, not a %s" % type(est).__name__)
         gp = est.getClassifier() if isinstance(est, OneVsRest) else est
+        if getattr(gp, "_process_group", None) is not None:
+            from . import distributed
+            ests = [est.copy(m) for m in self._maps or [{}]]
+            kind = {GaussianProcessRegression: "regression", GaussianProcessClassifier: "binary"}.get(type(est), "classes")
+            with distributed.selection(gp, [e.getClassifier() if kind == "classes" else e for e in ests], kind, X, y,
+                                       lambda n, offset: [self._mask(train, n, offset)], self.NAME + ".fit",
+                                       self._empty_side) as site:
+                return self._validate_split(site, est, ests, scored, site.X, site.y, (X, y))
         X, y = self._data(X, y, getattr(gp, "_device", 0),          # a OneVsRest without a classifier fails below
                           not isinstance(est, GaussianProcessRegression))
+        mask = self._mask(train, len(X), 0)
+        message = self._empty_side(len(X), [int(np.count_nonzero(mask))])
+        if message is not None:
+            raise ValueError(message)
+        ests = [est.copy(m) for m in self._maps or [{}]]
+        return self._validate_split(_Local(X, y, [mask]), est, ests, scored, X, y, (X, y))
+
+    def _mask(self, train, n: int, offset: int):
+        """The training mask of n rows, the rows [offset, offset + n) of the data: the seeded split, or the given one
+        checked."""
         if train is None:
-            mask = train_validation_assignment(len(X), self._train_ratio, self._seed)
-        else:
-            mask = np.asarray(train)
-            if mask.shape != (len(X),) or not np.all((mask == 0) | (mask == 1)):
-                raise ValueError("TrainValidationSplit: train must hold one bool per row")
-            mask = mask.astype(bool)
-        if not mask.any() or mask.all():
-            raise ValueError("TrainValidationSplit: the %s side of the split is empty"
-                             % ("training" if not mask.any() else "validation"))
+            return train_validation_assignment(n, self._train_ratio, self._seed, offset)
+        mask = np.asarray(train)
+        if mask.shape != (n,) or not np.all((mask == 0) | (mask == 1)):
+            raise ValueError("TrainValidationSplit: train must hold one bool per row")
+        return mask.astype(bool)
+
+    @staticmethod
+    def _empty_side(n: int, n_train):
+        """The refusal of a split of n rows with n_train[0] training rows: an empty side."""
+        if n_train[0] == 0 or n_train[0] == n:
+            return "TrainValidationSplit: the %s side of the split is empty" % ("training" if n_train[0] == 0
+                                                                                else "validation")
+        return None
+
+    def _validate_split(self, site, est, ests, scored, X, y, refit):
+        """Every map on the site's training rows (site.members[0]) of (X, y), its metric on the gathered validation
+        arrays, and the refit of the best map on refit."""
+        mask = site.members[0]
         maps = self._maps or [{}]
-        ests = [est.copy(m) for m in maps]
         if isinstance(est, GaussianProcessRegression):
-            preds, objective = self._fit_regression(ests, X, y, mask)
+            preds, objective = self._fit_regression(ests, X, y, mask, site)
             evaluated = preds
         else:
-            preds, raw, objective = self._fit_classifiers(ests, isinstance(est, OneVsRest), X, y, mask)
+            preds, raw, objective = self._fit_classifiers(ests, isinstance(est, OneVsRest), X, y, mask, site)
             evaluated = [r[:, 0] for r in raw] if scored else preds      # rawPrediction(1) = f
-        y_val = host_copy(_rows(y, ~mask))
+        y_val = site.gather(_rows(y, ~mask))
         metrics = [self._evaluator.evaluate(y_val, p) for p in evaluated]
         best = best_index(metrics, self._evaluator.isLargerBetter())
         self.last_predictions = preds
-        return TrainValidationSplitModel(est.copy(maps[best]).fit(X, y), metrics, best, objective)
+        return TrainValidationSplitModel(est.copy(maps[best]).fit(*refit), metrics, best, objective)
 
     @staticmethod
-    def _fit_regression(ests, X, y, train):
+    def _fit_regression(ests, X, y, train, site=None):
         """Validation predictions of every map of the regression estimator, and what the optimisation took: per group of
         maps (`group_slots`) one grouped upload of the training rows and one lock-step L-BFGS-B over the maps, each
         round one `sgp_bcm_nll_slots` launch.  A group with maxIter <= 0 takes its kernels' own hyper-parameters, as
-        GPR.fit does.  Each map's model is then produced on the training rows.  Returns (predictions, dict(maps=[each
-        map's dict(theta, magicVector, evaluations, iterations; value and n_experts when optimised)],
-        groups=[dict(maps, rounds, launches)]))."""
+        GPR.fit does.  Each map's model is then produced on the training rows.  site: the `_Local` of (X, y, train) by
+        default.  Returns (predictions, dict(maps=[each map's dict(theta, magicVector, evaluations, iterations; value and
+        n_experts when optimised)], groups=[dict(maps, rounds, launches)]))."""
+        site = site or _Local(X, y, [train])
         Xt, yt, Xv = _rows(X, train), _rows(y, train), _rows(X, ~train)
         thetas = [np.asarray(e.getKernel().getHyperparameters(), dtype=np.float64) for e in ests]
         records, groups = [dict(evaluations=0, iterations=0) for _ in ests], []
-        for slots, fitted, fit, n_experts in _bcm_groups(
-                ests, 1, lambda eng, n_e: eng.experts_upload_grouped(Xt, yt, n_e),
-                lambda eng, slots, kernels: eng.bcm_nll_slots(kernels)):
+        for slots, fitted, fit, uploaded in _bcm_groups(
+                ests, 1, lambda eng, n_e: site.upload_training(eng, n_e, Xt, yt),
+                lambda eng, slots, kernels: eng.bcm_nll_slots(kernels), site.context):
             groups.append(dict(maps=[p for p, _ in slots], rounds=fit["rounds"], launches=fit["launches"]))
             for (p, _), theta, r in zip(slots, fitted, fit["slots"]):
                 thetas[p] = theta
-                records[p] = dict(r, n_experts=n_experts)
+                records[p] = dict(r, n_experts=uploaded[2])
         preds = []
         for e, theta, r in zip(ests, thetas, records):
-            pred, mv = _validate(e, Xt, yt, Xv, theta)
+            pred, mv = site.validate(e, 0, Xt, yt, Xv, theta)
             preds.append(pred)
             r.update(theta=theta, magicVector=mv)
         return preds, dict(maps=records, groups=groups)
 
     @staticmethod
-    def _fit_classifiers(ests, ovr: bool, X, y, train):
+    def _fit_classifiers(ests, ovr: bool, X, y, train, site=None):
         """Validation predictions of every map of the binary classifier (ovr False) or of one-vs-rest, their raw
         columns (each class's latent mean f), and what the optimisation took: per group of maps one upload, one
         lock-step L-BFGS-B over the (map, class) slots, one `sgp_laplace_nll_slots_any_size` call per round and one at
-        every slot's optimum (GPCls:60)."""
+        every slot's optimum (GPCls:60).  site: the `_Local` of (X, y, train) by default."""
+        site = site or _Local(X, y, [train])
         gps = [e.getClassifier() for e in ests] if ovr else ests
         if any(not isinstance(gp, GaussianProcessClassifier) for gp in gps):
             raise TypeError("OneVsRest: setClassifier(GaussianProcessClassifier) first")
-        if ovr:
-            one_vs_rest_labels(y)
-            C = one_vs_rest_labels(_rows(y, train))[1]    # as an independent OneVsRest.fit(X[train], y[train])
-            label = lambda c: c
-        else:
-            assert_labels_are_01(y)
-            C = 1
-            label = lambda c: 1                             # y == 1 is y itself
+        C = site.set_classes(ovr)[0]                        # as an independent OneVsRest.fit(X[train], y[train])
+        label = (lambda c: c) if ovr else (lambda c: 1)     # binary: y == 1 is y itself
         Xt, yt, Xv = _rows(X, train), _rows(y, train), _rows(X, ~train)
         raw = [np.empty((len(Xv), C)) for _ in gps]
         groups = []
         for slots in tvs_slot_groups(gps, C).values():
             g0 = gps[slots[0][0]]
             modes = [m for _, _, m in slots]
-            eng = ProjectedProcessEngine.acquire(g0._device)
-            try:
+            with site.context(g0._device) as eng:
                 entry = lambda listed, kernels: eng.laplace_nll_slots_any_size(
                     len(gps) * C, [modes[i] for i in listed], [label(slots[i][1]) for i in listed], kernels, g0._tol)
+                upload = lambda eng: site.upload_training(eng, g0._datasetSizeForExpert, Xt, yt, laplace=True)[:2]
                 thetas, latent, fit = laplace_fit([gps[p] for p, _, _ in slots], eng, Xt, yt, entry, N.SGP_MODES_SLOT,
-                                                  lambda i: modes[i])
+                                                  lambda i: modes[i], upload=upload)
                 # every objective call is one round, and one more runs at the slots' thetas
                 groups.append(dict(
                     slots=[dict(map=p, cls=c, mode_slot=m, theta=theta, **r)
                            for (p, c, m), r, theta in zip(slots, fit["slots"] or [], thetas)],
                     rounds=fit["rounds"], calls=fit["rounds"] + 1, launches=fit["launches_total"]))
                 for (p, c, _), f, theta in zip(slots, latent, thetas):
-                    produce(gps[p], eng, Xt, f, theta)
-                    raw[p][:, c] = _latent_mean(eng, Xv)
-            finally:
-                eng.release()
+                    site.fold_model(gps[p], eng, 0, Xt, f, theta)
+                    raw[p][:, c] = site.latent_mean(eng, Xv)
+        raw = [site.gather(r) for r in raw]
         if ovr:
             preds = [one_vs_rest_prediction(r) for r in raw]
         else:                                               # GaussianProcessClassificationModel.predict

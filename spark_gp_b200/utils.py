@@ -41,11 +41,14 @@ def uniform(seed: int, stream: int, i) -> np.ndarray:
     return (z >> np.uint64(11)).astype(np.float64) * 2.0 ** -53
 
 
-def kfold_assignment(n: int, num_folds: int, seed: int) -> np.ndarray:
-    """CrossValidator's default split: point i goes to fold floor(u(seed, 200, i) * numFolds) (int32)."""
-    return np.floor(uniform(seed, 200, np.arange(int(n))) * int(num_folds)).astype(np.int32)
+def kfold_assignment(n: int, num_folds: int, seed: int, offset: int = 0) -> np.ndarray:
+    """CrossValidator's default split: point i goes to fold floor(u(seed, 200, i) * numFolds) (int32), for the n points
+    i in [offset, offset + n) (a rank's shard of a data-parallel selection numbers its rows globally)."""
+    i = np.arange(int(offset), int(offset) + int(n))
+    return np.floor(uniform(seed, 200, i) * int(num_folds)).astype(np.int32)
 
 
-def train_validation_assignment(n: int, train_ratio: float, seed: int) -> np.ndarray:
-    """TrainValidationSplit's default split: row i trains iff u(seed, 201, i) < trainRatio (bool mask)."""
-    return uniform(seed, 201, np.arange(int(n))) < float(train_ratio)
+def train_validation_assignment(n: int, train_ratio: float, seed: int, offset: int = 0) -> np.ndarray:
+    """TrainValidationSplit's default split: row i trains iff u(seed, 201, i) < trainRatio (bool mask), for the n rows
+    i in [offset, offset + n)."""
+    return uniform(seed, 201, np.arange(int(offset), int(offset) + int(n))) < float(train_ratio)

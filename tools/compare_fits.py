@@ -24,7 +24,8 @@ rows, `last_stats`, `last_objective` (values, evaluations, iterations, rounds, c
   regression_kmeans / regression_explicit   the same with KMeansActiveSetProvider(on_gpu=True) / an explicit active set
 Every case runs from host arrays (`host.*`) and from CUDA tensors on cuda:0 (`cuda.*`).  With --group, the data-parallel
 fit of the regression, the binary classifier and one-vs-rest over a one-rank NCCL group on cuda:0 (the store on the
-loopback address only), from host and CUDA input, is added as `group.*`."""
+loopback address only), from host and CUDA input, is added as `group.*`, with the model selectors over that group:
+`tvs_regression`, `cv`, `tvs_binary_auc` and `cv_ovr` as above."""
 from __future__ import annotations
 
 import argparse
@@ -214,9 +215,36 @@ def run_group(sg, put):
         res["ovr_iris"] = dict(model=ovr_outputs(model, put(c["X"][te])), last_objective=ovr.last_objective,
                                last_latent=ovr.last_latent)
         del model
+        # the model selectors over the group, as `run` configures them
+        maps = sg.ParamGridBuilder().addGrid("sigma2", [1e-3, 1e-1]).build()
+        reg = (sg.GaussianProcessRegression(process_group=group).setKernel(lambda: 1 * sg.RBFKernel(0.1, 1e-6, 10))
+               .setDatasetSizeForExpert(100).setActiveSetSize(60).setSeed(13).setMaxIter(20))
+        tvs = (sg.TrainValidationSplit().setEstimator(reg).setEvaluator(sg.RegressionEvaluator())
+               .setEstimatorParamMaps(maps).setSeed(4))
+        res["tvs_regression"] = selection_outputs(tvs, tvs.fit(put(Xr), put(yr)), Xrt)
+        cv = sg.CrossValidator().setEstimator(reg).setEstimatorParamMaps(maps).setNumFolds(3).setSeed(6)
+        res["cv"] = selection_outputs(cv, cv.fit(put(Xr), put(yr)), Xrt)
+        tvs = (sg.TrainValidationSplit().setEstimator(gp).setEvaluator(sg.BinaryClassificationEvaluator())
+               .setEstimatorParamMaps(maps).setSeed(5))
+        res["tvs_binary_auc"] = selection_outputs(tvs, tvs.fit(put(X), put(y)), put(Xte))
+        cv = (sg.CrossValidator().setEstimator(ovr).setEvaluator(sg.MulticlassClassificationEvaluator())
+              .setEstimatorParamMaps(maps).setNumFolds(3).setSeed(6))
+        res["cv_ovr"] = selection_outputs(cv, cv.fit(put(c["X"]), put(c["y"])), put(c["X"][te]))
         return res
     finally:
         dist.destroy_process_group()
+
+
+def selection_outputs(selector, model, Xte):
+    """A model selector's metrics, bestIndex, records and best model."""
+    best = model.bestModel
+    out = dict(bestIndex=model.bestIndex, last_objective=model.last_objective,
+               best=ovr_outputs(best, Xte) if hasattr(best, "models") else model_outputs(best, Xte))
+    if hasattr(model, "avgMetrics"):
+        out.update(avgMetrics=model.avgMetrics, last_folds={"%d_%d" % pk: v for pk, v in selector.last_folds.items()})
+    else:
+        out.update(metrics=model.validationMetrics, last_predictions=selector.last_predictions)
+    return out
 
 
 def compare(a_path, b_path):
