@@ -366,19 +366,30 @@ __global__ void __launch_bounds__(GTHREADS, 1) gram_i8_kernel(const GramI8Params
       // ---- fold the exact int32 accumulators into the fp64 partial tile -----------------------------------------
       until_flush = FLUSH_UNITS;
       wg_wait<0>();
-      // the row stride, read through an opaque move: the 32 column addresses are formed here, not hoisted out of the
+      // the row stride, read through an opaque move: the column addresses are formed here, not hoisted out of the
       // unit loop into registers the accumulators need
       uint32_t ld;
       asm volatile("mov.b32 %0, %1;" : "=r"(ld) : "r"(static_cast<uint32_t>(p.m_pad)));
       double* const trow = gtile + R;
+      const auto at = [&](int e) {
+        return trow + static_cast<size_t>(8 * (e >> 2) + c0 + (e & 1)) * ld + ((e & 2) ? 8 : 0);
+      };
+      // the compiler cannot tell the elements' addresses apart, so a load after a store waits for it: each batch reads
+      // all its old values before it writes any, FB loads in flight instead of one (in the registers of the accumulators
+      // already folded; a batch of 16 spills under MMA_REGS)
+      constexpr int FB = 8;
 #pragma unroll
-      for (int e = 0; e < 64; ++e) {
-        const int c = 8 * (e >> 2) + c0 + (e & 1);
-        const double v = p.gscale * (4294967296.0 * static_cast<double>(acc4[e]) + 16777216.0 * static_cast<double>(acc3[e]) +
-                                     65536.0 * static_cast<double>(acc2[e]));
-        double* dst = trow + static_cast<size_t>(c) * ld + ((e & 2) ? 8 : 0);
-        if (first_flush) *dst = v;
-        else *dst += v;
+      for (int e0 = 0; e0 < 64; e0 += FB) {
+        double old[FB];
+#pragma unroll
+        for (int k = 0; k < FB; ++k) old[k] = first_flush ? 0.0 : *at(e0 + k);
+#pragma unroll
+        for (int k = 0; k < FB; ++k) {
+          const int e = e0 + k;
+          const double v = p.gscale * (4294967296.0 * static_cast<double>(acc4[e]) + 16777216.0 * static_cast<double>(acc3[e]) +
+                                       65536.0 * static_cast<double>(acc2[e]));
+          *at(e) = first_flush ? v : old[k] + v;
+        }
       }
       first_flush = false;
       fresh = true;
