@@ -602,6 +602,27 @@ int sgp_kernel_eval_device(sgp_ctx* ctx, const sgp_kernel_desc* kernel, const sg
                            const void* dA, int32_t a_is_f32, int64_t n, const double* dB, int32_t m, int32_t d,
                            int32_t mode, double* dK_out /* n x m */, double* ddK_out /* n_hypers x n x m, or NULL */);
 
+/* ---- Feature standardisation: commons/util/Scaling.scala:10-25 on device-resident rows -----------------------------
+ * dX is n x d row-major in device memory on the context's device, fp64 (x_is_f32 = 0) or fp32 (x_is_f32 = 1), read in
+ * place on the context's stream.  Refused with SGP_E_BADARG before any allocation or launch: x_is_f32 other than 0 or 1,
+ * n < 0, d < 1, and where n > 0 a null dX or a dX that is not device (or managed) memory on the context's device.  n = 0
+ * launches nothing.  Work outside any begin..finish window and leave its statistics untouched; rank-local.
+ *
+ * sgp_column_sums_device: out[k] (host, d values) = sum_i x_ik, or with center (host, d values, or NULL)
+ * sum_i (x_ik - center_k)^2, every x converted exactly to fp64 and every subtraction and square rounded once.  The sum
+ * order is fixed: rows go in blocks of 2048, each block gets one fp64 partial per column, and the partials are added in
+ * block order, so the same inputs give the same bits on any H100 whatever the grid or the other work on the GPU.  n = 0
+ * writes d zeros.  Returns when out is written (SGP_E_BADARG also for a null out). */
+int sgp_column_sums_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n, int32_t d, const double* center,
+                           double* out);
+/* sgp_scale_apply_device: dY[i][k] = (x_ik - mean_k) / sd_k (n x d row-major fp64, device memory on the context's
+ * device) with mean and sd host arrays of d values: a correctly rounded fp64 subtraction, then a correctly rounded
+ * division (the reference's operation order; no reciprocal), so every element equals the host formula's on the same mean
+ * and sd.  Refuses, besides the above, a null mean, sd or dY and a dY that is not device memory on the context's device,
+ * where n > 0.  Asynchronous on the context's stream: synchronise with sgp_sync before reading dY. */
+int sgp_scale_apply_device(sgp_ctx* ctx, const void* dX, int32_t x_is_f32, int64_t n, int32_t d, const double* mean,
+                           const double* sd, double* dY);
+
 #ifdef __cplusplus
 }
 #endif

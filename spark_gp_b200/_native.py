@@ -31,7 +31,7 @@ EXPORTS = ["sgp_ctx_create", "sgp_ctx_destroy", "sgp_last_error", "sgp_set_preci
            "sgp_experts_get_f_fold_rows_device", "sgp_gauss_hermite_rule", "sgp_predict_probability",
            "sgp_predict_probability_device", "sgp_bcm_nll_slots", "sgp_kernel_eval", "sgp_kernel_eval_device",
            "sgp_experts_upload_strided_device", "sgp_kmeans_sharded", "sgp_kmeans_sharded_device",
-           "sgp_experts_upload_fold_sets_device"]
+           "sgp_experts_upload_fold_sets_device", "sgp_column_sums_device", "sgp_scale_apply_device"]
 
 
 class KernelTerm(C.Structure):
@@ -128,6 +128,8 @@ def load() -> C.CDLL:
     lib.sgp_kmeans_sharded.argtypes = [vp, vp, i32, i64, i64, i64, i32, i32, i32, C.c_double, i64, vp, vp, vp, vp, vp, vp]
     lib.sgp_kmeans_sharded_device.argtypes = lib.sgp_kmeans_sharded.argtypes
     lib.sgp_event_elapsed_ms.argtypes = [vp, C.c_int, C.c_int, dp]
+    lib.sgp_column_sums_device.argtypes = [vp, vp, i32, i64, i32, vp, vp]
+    lib.sgp_scale_apply_device.argtypes = [vp, vp, i32, i64, i32, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("sgp_last_error", "sgp_launch_count"):
             getattr(lib, name).restype = C.c_int

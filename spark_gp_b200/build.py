@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsgp.so")
-SOURCES = ["api.cu", "bcm_nll.cu", "gram_f64.cu", "gram_i8.cu", "gram_i8_wgmma.cu", "greedy.cu", "kernel_eval.cu", "kmeans.cu", "kmn_sweep.cu", "laplace.cu", "laplace_global.cu", "misc_kernels.cu", "predict.cu", "tail.cu"]
+SOURCES = ["api.cu", "bcm_nll.cu", "gram_f64.cu", "gram_i8.cu", "gram_i8_wgmma.cu", "greedy.cu", "kernel_eval.cu", "kmeans.cu", "kmn_sweep.cu", "laplace.cu", "laplace_global.cu", "misc_kernels.cu", "predict.cu", "scale.cu", "tail.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-Xptxas", "-v"]
 LINK = ["-lcusolver", "-lcublas", "-ldl", "-Xlinker", "-rpath=/usr/local/cuda/lib64"]

@@ -2378,4 +2378,63 @@ int sgp_kernel_eval_device(sgp_ctx* h, const sgp_kernel_desc* kernel, const sgp_
   return SGP_OK;
 }
 
+namespace {
+// The refusals both scale entries share, taken before any allocation or launch: the dtype flag, the shape, and X on
+// the context's device wherever rows exist.
+int scale_args(Ctx* c, const char* entry, const void* dX, int32_t x_is_f32, int64_t n, int32_t d) {
+  if (x_is_f32 != 0 && x_is_f32 != 1)
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": x_is_f32 must be 0 (fp64) or 1 (fp32), not " +
+                                     std::to_string(x_is_f32));
+  if (n < 0 || d < 1) return fail(c, SGP_E_BADARG, std::string(entry) + ": no features or a negative row count");
+  if (n > 0 && (n > INT64_MAX / d || scale_row_blocks(n) > 2147483647LL))
+    return fail(c, SGP_E_BADARG, std::string(entry) + ": too many rows");
+  if (n > 0 && !dX) return fail(c, SGP_E_BADARG, std::string(entry) + ": null X");
+  SGP_CUDA(c, cudaSetDevice(c->device));
+  return n > 0 ? device_ptr_ok(c, dX, entry, "X") : SGP_OK;
+}
+}  // namespace
+
+int sgp_column_sums_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, int64_t n, int32_t d, const double* center,
+                           double* out) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  const char* entry = "sgp_column_sums_device";
+  int rc = scale_args(c, entry, dX, x_is_f32, n, d);
+  if (rc != SGP_OK) return rc;
+  if (!out) return fail(c, SGP_E_BADARG, std::string(entry) + ": null out");
+  if (n == 0) {
+    std::fill(out, out + d, 0.0);
+    return SGP_OK;
+  }
+  const size_t cols = static_cast<size_t>(d);
+  rc = ctx_scratch(c, c->scale_ws, (2 + static_cast<size_t>(scale_row_blocks(n))) * cols * sizeof(double));
+  if (rc != SGP_OK) return rc;
+  double* ws = c->scale_ws.as<double>();
+  if (center) SGP_CUDA(c, cudaMemcpyAsync(ws, center, cols * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, launch_column_sums(dX, x_is_f32, n, d, center ? ws : nullptr, ws + 2 * cols, ws + cols, c->stream));
+  c->launches += 2;
+  SGP_CUDA(c, cudaMemcpyAsync(out, ws + cols, cols * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  SGP_CUDA(c, cudaStreamSynchronize(c->stream));
+  return SGP_OK;
+}
+
+int sgp_scale_apply_device(sgp_ctx* h, const void* dX, int32_t x_is_f32, int64_t n, int32_t d, const double* mean,
+                           const double* sd, double* dY) {
+  Ctx* c = reinterpret_cast<Ctx*>(h);
+  if (!c) return SGP_E_BADARG;
+  const char* entry = "sgp_scale_apply_device";
+  int rc = scale_args(c, entry, dX, x_is_f32, n, d);
+  if (rc != SGP_OK || n == 0) return rc;
+  if (!mean || !sd || !dY) return fail(c, SGP_E_BADARG, std::string(entry) + ": null mean, sd or Y");
+  rc = device_ptr_ok(c, dY, entry, "Y");
+  if (rc == SGP_OK) rc = ctx_scratch(c, c->scale_ws, 2 * static_cast<size_t>(d) * sizeof(double));
+  if (rc != SGP_OK) return rc;
+  double* ws = c->scale_ws.as<double>();
+  SGP_CUDA(c, cudaMemcpyAsync(ws, mean, static_cast<size_t>(d) * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, cudaMemcpyAsync(ws + d, sd, static_cast<size_t>(d) * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  SGP_CUDA(c, launch_scale_apply(dX, x_is_f32, n, d, ws, ws + d, dY, c->stream));
+  c->launches += 1;
+  return SGP_OK;
+}
+
 }  // extern "C"

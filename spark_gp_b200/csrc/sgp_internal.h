@@ -47,6 +47,9 @@ constexpr int kBcmLuMaxPoints = 46340;
 // 32768 points per window)
 constexpr size_t kPredictKBytes = size_t(256) << 20;
 
+// feature standardisation (scale.cu): rows per row block of the column sums, whose partials are added in block order
+constexpr long long kScaleRows = 2048;
+
 // sqrt(log2 e): coordinates scaled by it turn exp(-q) into 2^(-q'), one ex2 (int8 modes, fp32 element of the fp64 Gram)
 constexpr double kSqrtLog2e = 0x1.337cc2183b050p+0;
 
@@ -138,6 +141,8 @@ struct Ctx {
   DevScratch kmeans_pts_ws, kmeans_cen_ws, kmeans_new_ws, kmeans_cand_ws;   // sgp_kmeans: point-, centre-, candidate-sized
   DevScratch kmeans_rows_ws;           // sgp_kmeans_device: indices and fp64 copies of the rows the host reads
   DevScratch kmeans_comm_ws;           // sgp_kmeans_sharded: the buffers its collectives sum over the ranks
+  DevScratch scale_ws;                 // sgp_column_sums_device, sgp_scale_apply_device: [2][d] column values, then
+                                       // the [row blocks][d] partial sums
   bool has_magic_run = false;
   bool tail_fast = false;              // last sgp_magic took the Cholesky path for both matrices
   ncclComm_t comm = nullptr;
@@ -278,6 +283,15 @@ cudaError_t launch_status_to_double(double* dst, const int* flags, int mask, con
                                     cudaStream_t s);
 // dst[i] = (flags[i] & mask) ? 1 : 0 for i < n: the per-slot status words of an objective evaluation
 cudaError_t launch_flags_to_double(double* dst, const int* flags, int mask, int n, cudaStream_t s);
+
+// Feature standardisation (scale.cu) of n x d device rows (fp32 or fp64), on stream s.  launch_column_sums: out[k] =
+// sum_i x_ik, or with centre sum_i (x_ik - centre_k)^2; part holds scale_row_blocks(n) x d partials.  launch_scale_apply:
+// Y[i][k] = (x_ik - mean_k) / sd_k.  n >= 1; centre, mean, sd, part, out and Y are device memory.
+long long scale_row_blocks(long long n);
+cudaError_t launch_column_sums(const void* X, int x_is_f32, long long n, int d, const double* centre, double* part,
+                               double* out, cudaStream_t s);
+cudaError_t launch_scale_apply(const void* X, int x_is_f32, long long n, int d, const double* mean, const double* sd,
+                               double* Y, cudaStream_t s);
 
 // Prediction (predict.cu) over one window of device-resident points.
 struct PredictArgs {

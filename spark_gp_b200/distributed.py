@@ -23,6 +23,9 @@ The model selectors over a group (`selection`, `Selection`) reuse these steps wi
 `ShardPlan` per set, one all-to-all that moves each row once per set it belongs to (`exchange_sets`), and one gather of
 the ranks' validation labels and predictions, so that every rank scores the same arrays.
 
+`scale` standardises every rank's shard with the mean and standard deviation of the concatenation: two all-reduces of
+d + 1 and d values after the agreement, no rows moved.
+
 `engine_factory` is the context class (a test passes a stand-in)."""
 from __future__ import annotations
 
@@ -382,6 +385,55 @@ def _fit(gp, plan, eng, X, y, hyperparameters, kind, n_classes, dtype, group, de
         f = slot_modes(eng, is_cuda_tensor(X), n_e, plan.local_experts, store, i)
         slots.append(produce(gp, eng, Xe, f, theta, active_set(gp, plan, eng, X, theta, group, device))._replace(latent=f))
     return slots, record
+
+
+# ---- feature scaling over the group (`utils.scale` with a process group) --------------------------------------------
+def scale(X, group, engine_factory=ProjectedProcessEngine.acquire):
+    """`utils.scale` of this rank's shard X (a host array or a CUDA tensor, n x d, possibly empty) with the mean and
+    standard deviation of the concatenation of every rank's shard, as the reference's `reduce`s over the whole RDD give
+    them.  The agreement step comes first (as `agree`: the number of features, the dtype and every rank's own refusal;
+    every rank raises the same exception, before any context exists, also when every shard is empty).  Then every rank
+    sums its column-sum partials [S; n] over the group in one all-reduce, computes the same mean, and sums its centred
+    squares Q in a second one (`utils.moments`).  No rows move.  Each rank returns its own rows scaled: a CUDA float64
+    tensor for a CUDA shard, a host float64 array for a host shard (staged through the rank's current CUDA device)."""
+    import contextlib
+
+    import torch
+
+    from .utils import moments
+    dist = _dist()
+    on_device = is_cuda_tensor(X)
+    index = X.device.index if on_device else (torch.cuda.current_device() if torch.cuda.is_available() else 0)
+    nccl = dist.get_backend(group) == "nccl"
+    device = torch.device("cuda", index) if nccl else torch.device("cpu")
+    with torch.cuda.device(index) if nccl else contextlib.nullcontext():
+        err, n, d, dtype = None, 0, -1, ""
+        try:
+            if not on_device:
+                X = np.asarray(X)
+                X = np.ascontiguousarray(X if X.dtype == np.float32 else X.astype(np.float64))
+            if X.ndim != 2:
+                raise ValueError("scale: X must be n x d")
+            n, d, dtype = len(X), X.shape[1], str(X.dtype).replace("torch.", "")
+        except (ValueError, TypeError, RuntimeError) as e:
+            err = (type(e).__name__, str(e))
+        d = agree(group, n, d, dtype, err, 1, False, False)[2]
+        if len(X) == 0:                                     # an empty shard takes the agreed width
+            X = torch.empty((0, d), dtype=torch.float64, device=X.device) if on_device else np.empty((0, d))
+        Xd = X if on_device else _tensor(X, torch.device("cuda", index) if torch.cuda.is_available() else "cpu")
+
+        def total(v):
+            t = torch.as_tensor(v, dtype=torch.float64, device=device)
+            dist.all_reduce(t, group=group)
+            return t.cpu().numpy()
+
+        eng = engine_factory(index)
+        try:
+            mean, sd = moments(eng, Xd, total)
+            Y = eng.scale_apply(Xd, mean, sd)
+        finally:
+            eng.release()
+        return Y if on_device else Y.cpu().numpy()
 
 
 # ---- model selection over the group (`tuning.CrossValidator` / `TrainValidationSplit` with a process group) ----------

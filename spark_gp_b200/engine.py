@@ -763,6 +763,42 @@ class ProjectedProcessEngine:
                        C.byref(iters), C.byref(cost)))
         return np.ascontiguousarray(centres[:k_out.value]), labels[:n], iters.value, cost.value
 
+    def column_sums(self, X, center=None):
+        """fp64 sums over the rows of a CUDA tensor X (n x d, on this context's device, read in place; float32 as it is,
+        other dtypes as float64) in the library's fixed order (`sgp_column_sums_device`): sum_i x_ik per column, or with
+        `center` (d values) sum_i (x_ik - center_k)^2.  Returns a host array of d values."""
+        import torch
+        X = device_tensor(X, self._device, "column_sums")
+        if X.ndim != 2:
+            raise ValueError("column_sums: X must be n x d")
+        n, d = X.shape
+        c = None if center is None else np.ascontiguousarray(center, dtype=np.float64)
+        if c is not None and c.shape != (d,):
+            raise ValueError("column_sums: center must hold %d values" % d)
+        out = np.empty(d)
+        self._check(self._lib.sgp_column_sums_device(self._h, C.c_void_p(X.data_ptr() if n else None),
+                                                     int(X.dtype == torch.float32), n, d,
+                                                     N.ptr(c) if c is not None else None, N.ptr(out)))
+        return out
+
+    def scale_apply(self, X, mean, sd):
+        """(x_ik - mean_k) / sd_k for a CUDA tensor X (n x d, on this context's device) as a CUDA float64 n x d tensor on
+        X's device (`sgp_scale_apply_device`): every element is the host formula's on the same mean and sd."""
+        import torch
+        X = device_tensor(X, self._device, "scale_apply")
+        if X.ndim != 2:
+            raise ValueError("scale_apply: X must be n x d")
+        n, d = X.shape
+        mean, sd = (np.ascontiguousarray(v, dtype=np.float64) for v in (mean, sd))
+        if mean.shape != (d,) or sd.shape != (d,):
+            raise ValueError("scale_apply: mean and sd must hold %d values each" % d)
+        Y = torch.empty((n, d), dtype=torch.float64, device=X.device)
+        self._check(self._lib.sgp_scale_apply_device(self._h, C.c_void_p(X.data_ptr() if n else None),
+                                                     int(X.dtype == torch.float32), n, d, N.ptr(mean), N.ptr(sd),
+                                                     C.c_void_p(Y.data_ptr() if n else None)))
+        self.sync()
+        return Y
+
     def kmn_sweep(self, X):
         """fp32 K[i][j] = k(x_i, z_j) (n x m) through the tensor-core sweep kernel (one non-Eye term, d <= 32)."""
         X = _rows(X)
